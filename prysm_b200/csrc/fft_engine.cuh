@@ -189,6 +189,13 @@ __device__ __forceinline__ uint64_t l2_policy(int kind) {   // 0 evict_normal, 1
     else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
     return pol;
 }
+__device__ __forceinline__ uint64_t l2_policy_last_first(float fraction) {   // that fraction of the lines evict_last, the rest evict_first
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_last.L2::evict_first.b64 %0, %1;" : "=l"(pol) : "f"(fraction));
+    return pol;
+}
+// invalidate the 128-byte L2 line at p (128-byte aligned) without writing it back: its contents become undefined
+__device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar, uint64_t pol) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4}], [%5], %6;"
@@ -306,7 +313,9 @@ struct FocusParams {
     long long in_bs, amp_bs, out_bs;
     // v2 pipeline
     int ntiles;             // column kernel: batch * N / T tiles, walked by a persistent grid
-    int hints;              // 1: L2 eviction hints (intermediate evict_last when written / evict_first when read, streams evict_first)
+    // 1: L2 eviction hints (streams evict_first); 2: L2 prefetch of the tile after next; 4 (v2 with focus_row4_kernel):
+    // plane 0 of the intermediate is written evict_last, and the row kernel discards its lines once they are read
+    int hints;
 };
 
 template <int L> struct Geo2 {
@@ -399,7 +408,11 @@ template <int L> struct GeoR4 {
     static constexpr size_t GROUP = (size_t)G::SBUF * 16 + (size_t)L * 8;       // exchange + row buffer, bytes (multiple of 128)
     static constexpr size_t PLAN_OFF = 4 * GROUP;
     static constexpr size_t BAR_OFF = PLAN_OFF + (size_t)((Geo4<L>::PLANLEN * 8 + 15) / 16) * 16;
-    static constexpr size_t SMEM = BAR_OFF + 8 * sizeof(uint64_t);
+    // arrivals of the four groups at each plane-0 line group (indexed by iteration; a CTA has at most L/4 of them), then one
+    // "this group arrived last" flag per group
+    static constexpr size_t CNT_OFF = BAR_OFF + 8 * sizeof(uint64_t);
+    static constexpr int NCNT = L / 4 + 4;
+    static constexpr size_t SMEM = CNT_OFF + NCNT * sizeof(unsigned int);
 };
 
 static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }

@@ -23,8 +23,9 @@
 //   focus_row_kernel : persistent; per intermediate row both half-transforms; thread owns outputs
 //                      (2j, 2j+1) and stores them as one float4.  Rows arrive by bulk async copy
 //                      (cp.async.bulk + mbarrier), one row ahead.
-//   HBM traffic: pupil 8N^2 once, output 8K^2 once; the 16N^2-byte intermediate (64 MiB at N = 2048)
-//   is written and re-read through L2 where it fits (one field's at N <= 1024 on the H100's 50 MB), HBM otherwise.
+//   HBM traffic: pupil 8N^2 once, output 8K^2 once; the 16N^2-byte intermediate (64 MiB at N = 2048) is written and
+//   re-read through L2 where it fits (N <= 1024 on the H100's 50 MB).  At N = 2048 the v2 pair below keeps its plane 0
+//   in L2 and discards it after the read: only plane 1 (32 MiB) makes the trip through HBM.
 //
 // FFT_N engine: N/16 threads per line, 16 points x 2 lanes per thread in registers, radix
 // 16 x 16 x N/256, two shared-memory exchanges of float4 (1-in-16 padded, conflict free).
@@ -185,13 +186,20 @@ __global__ void __launch_bounds__(L / 16) focus_row_kernel(const FocusParams p) 
 //     4 x 4 block (4 output rows of one plane, 4 adjacent columns) is one 128-byte line.  A warp of the column kernel
 //     (8 consecutive j x 4 columns) stores two full lines per instruction instead of eight 32-byte sectors in eight
 //     lines -- the LSU pressure (`lg_throttle`) of the row-major layout is gone.
-//   * The column kernel is persistent (one 512-thread CTA per SM walks the tiles of all fields of the launch) and takes
+//   * The column kernel is persistent (one 512-thread CTA per SM walks the tiles of the field) and takes
 //     its 4-column input tile by tensor TMA (box = 4 columns x 256 rows, 32-byte runs gathered into a contiguous
 //     [row][4] image that aliases the exchange buffers); the tile after next is requested as soon as the exchange
 //     buffers are free, so it lands while the last butterflies and the stores of the current tile run.
 //   * The row kernel gathers one intermediate row (512 runs of 32 bytes, 128 bytes apart) with two tensor-TMA boxes into
 //     the same contiguous row buffer the v1 kernel fills by a bulk copy; everything after that is the v1 code.
+//   * One field per launch pair, and plane 0 of its intermediate (the even output rows, 8 N^2 bytes = 32 MiB at N = 2048)
+//     stays in L2: the column kernel writes it evict_last, the row kernel reads it first and then discards each line
+//     (discard.global.L2), so it never reaches HBM in either direction.  Plane 1 is written evict_first and makes the trip.
 // =====================================================================================================
+
+// share of plane 0's lines written evict_last (the rest evict_first): what the H100's 50 MB L2 keeps next to the
+// streaming input and plane 1
+constexpr float kPlane0Keep = 1.0f;
 
 
 template <int L, bool INV, int HALF>
@@ -206,7 +214,9 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
     const float2* __restrict__ plan = reinterpret_cast<const float2*>(smem4 + G4::PLAN2);
     float4* S = smem4 + (HALF * 2 + cp) * G4::XBUF;
     const SyncGroup gsync{1 + HALF, 2 * NT};
-    const uint64_t pol_tmp = l2_policy((p.hints & 1) ? 2 : 0), pol_in = l2_policy((p.hints & 1) ? 1 : 0);
+    // plane 0 is read back first by the row kernel that follows: it stays in L2 (and is discarded there); plane 1 streams
+    const uint64_t pol_tmp = (HALF == 0 && (p.hints & 4)) ? l2_policy_last_first(kPlane0Keep) : l2_policy((p.hints & 1) ? 1 : 0);
+    const uint64_t pol_in = l2_policy((p.hints & 1) ? 1 : 0);
     auto request_tile = [&](int ww) {   // one thread: gather tile ww = (field, column tile) into the staging area
         const int fb = ww / G2::TILES, tile = ww - fb * G2::TILES;
         mbar_expect_tx(bar + 1, (uint32_t)(L * 4 * sizeof(float2)));
@@ -406,16 +416,26 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
     uint64_t* bars = reinterpret_cast<uint64_t*>(smraw + R4::BAR_OFF);   // [0] plan, [1 + grp] row of group grp
     uint64_t* bar = bars + 1 + grp;
     const uint64_t pol_tmp = l2_policy((p.hints & 1) ? 1 : 0), pol_out = l2_policy((p.hints & 1) ? 1 : 0);
+    // plane 0 (p.hints & 4): read evict_last so that no line leaves L2 -- written back -- before all four of its rows are
+    // read; then discarded
+    const uint64_t pol_keep = l2_policy((p.hints & 4) ? 2 : 0);
     auto request_row = [&](int R) {   // one thread: gather intermediate row R = (field, plane, j) into `inb`
         const int fb = R / (2 * L), rf = R - fb * (2 * L);
         const int ph = rf / L, j = rf - ph * L;
         const int grow = (fb * 2 + ph) * (L / 4) + (j >> 2);
+        const uint64_t pol = ph == 0 && (p.hints & 4) ? pol_keep : pol_tmp;
         mbar_expect_tx(bar, ROW_BYTES);
 #pragma unroll
-        for (int b = 0; b < G2::NBOX_ROW; ++b) tma_load_4d(inb + b * G2::BOXT * 4, &tmp_map, 0, j & 3, b * G2::BOXT, grow, bar, pol_tmp);
+        for (int b = 0; b < G2::NBOX_ROW; ++b) tma_load_4d(inb + b * G2::BOXT * 4, &tmp_map, 0, j & 3, b * G2::BOXT, grow, bar, pol);
     };
     int r = blockIdx.x * 4 + grp;
     const int rstep = gridDim.x * 4;
+    // Discard of plane 0 (one field per launch: rows R < L, R / 4 = line group).  The four groups of the CTA read the four
+    // rows j % 4 = 0..3 of the same line group at the same iteration, and no other CTA reads those lines.  Each group counts
+    // itself in arrived[it] once its row is in shared memory; the last of the four drops the group's 512 lines from L2.
+    unsigned int* arrived = reinterpret_cast<unsigned int*>(smraw + R4::CNT_OFF);
+    unsigned int* last = arrived + L / 4;   // [grp]: this group arrived last at its current line group
+    for (int i = threadIdx.x; i < R4::NCNT; i += blockDim.x) arrived[i] = 0u;
     if (threadIdx.x == 0) {
         for (int i = 0; i < 5; ++i) mbar_init(bars + i, 1);
         mbar_fence_init();
@@ -432,6 +452,11 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
     for (int it = 0; r < p.nrows; ++it, r += rstep) {
         P2 v[16];
         mbar_wait(bar, it & 1);
+        const bool drop = (p.hints & 4) && r < L;
+        if (drop && t == 0) {
+            __threadfence_block();
+            last[grp] = atomicAdd(arrived + it, 1u) == 3u;
+        }
         {
             const float2* __restrict__ row = inb + t;
 #define PB_X(n) row[(n) * NT]
@@ -457,6 +482,11 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
         if (t == 0 && rn < p.nrows) {
             fence_proxy_async();
             request_row(rn);
+        }
+        if (drop && last[grp]) {   // all four rows of line group r / 4 are in shared memory: its lines are dead
+            const char* lines = reinterpret_cast<const char*>(p.tmp) + (size_t)(r >> 2) * (G2::TILES * 128);
+#pragma unroll
+            for (int i = 0; i < G2::TILES / NT; ++i) l2_discard(lines + (size_t)(t + i * NT) * 128);
         }
         {
             const float4* __restrict__ s4 = S + pad16(t);
@@ -605,8 +635,10 @@ int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, 
 namespace {
 
 
+// one field: `p.tmp` holds its [2][L][L] intermediate
 template <int L, bool INV>
-int launch_focus2(Handle* h, FocusParams p, int batch, cudaStream_t st) {
+int launch_focus2(Handle* h, FocusParams p, cudaStream_t st) {
+    constexpr int batch = 1;
     using G = Geo<L>;
     using G2 = Geo2<L>;
     using G4 = Geo4<L>;
@@ -627,8 +659,10 @@ int launch_focus2(Handle* h, FocusParams p, int batch, cudaStream_t st) {
     PB_TRY(get_col4_plan<L>(h, &plan_col));
     p.nrows = batch * 2 * L;
     p.ntiles = batch * G2::TILES;
-    static const int hints = env_int("PB_FOCUS_L2_HINTS", 1);   // bit 0: eviction hints, bit 1: L2 prefetch of the tile after next
-    p.hints = hints;
+    static const int hints = env_int("PB_FOCUS_L2_HINTS", 1) & 3;   // bit 0: eviction hints, bit 1: L2 prefetch of the tile after next
+    static const int row_version = env_int("PB_ROW_V", 4);
+    // plane 0 kept in L2 needs the row kernel that discards it
+    p.hints = hints | ((hints & 1) && row_version == 4 ? 4 : 0);
     // (descriptors are copied out at once: the handle's cache may be flushed by the next lookup)
     const CUtensorMap* map = nullptr;
     CUtensorMap in_m, tmp_m;
@@ -646,11 +680,10 @@ int launch_focus2(Handle* h, FocusParams p, int batch, cudaStream_t st) {
         PB_TRY(get_map_c64(h, MapKey{p.in, 2, L, batch, p.in_ld, batch > 1 ? p.in_bs : 0}, 3, dims, str, box, &map));
         in_m = *map;
     }
-    // column pass: one CTA per SM walks the tiles of all fields of the launch
+    // column pass: one CTA per SM walks the tiles of the field
     p.plan = reinterpret_cast<const float4*>(plan_col);
     colk<<<std::min(h->sm_count, p.ntiles), G4::THREADS, smem_col, st>>>(in_m, p);
     PB_LAUNCH_CHECK(h);
-    static const int row_version = env_int("PB_ROW_V", 4);
     if (row_version == 4) {   // four line groups per CTA, plan in shared memory
         PB_TRY(set_smem_attrs(h, focus_row4_kernel<L, INV>, GeoR4<L>::SMEM, 1));
         focus_row4_kernel<L, INV><<<std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, GeoR4<L>::SMEM, st>>>(tmp_m, p);
@@ -1041,13 +1074,6 @@ int try_tuned_axis_pass(Handle* h, const AxisPass& p, cudaStream_t st) {
     }
 }
 
-// fields per launch pair: more than one evens out the tails of the column and row grids (512 column tiles at N = 2048 are
-// 3.9 waves on 132 SMs).  The intermediates of a group (64 MiB each at N = 2048) do not fit L2 and round-trip through HBM.
-static int focus_fields_per_launch() {
-    static const int n = [] { const char* e = getenv("PB_FOCUS_BATCH"); return e ? std::max(1, atoi(e)) : 8; }();
-    return n;
-}
-
 int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, const void* amp, int amp_kind, double kturns,
                          int batch, long long in_bs, long long amp_bs, int ny, int nx, long long in_ld, int ky, int kx, int dir,
                          double scale, int shift_in, int shift_out, void* out, int out_kind, double weight, int oy, int ox,
@@ -1071,7 +1097,10 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
         const int rc = try_focus_fused(h, N, dir, in, in_ld, in_bs, batch, out, out_kind, out_ld, out_bs, scale, weight, st);
         if (rc != PB_ERR_UNSUPPORTED) return rc;
     }
-    const int per = std::min(batch, focus_fields_per_launch());
+    const bool v2 = version >= 2 && tma_ok;
+    // v2: one field per launch pair, so that the plane 0 its column pass leaves in L2 is what its row pass reads first.
+    // v1: up to 8 fields per launch pair, which evens out the tails of the two grids.
+    const int per = v2 ? 1 : std::min(batch, 8);
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 0, (size_t)per * 2 * N * N * sizeof(float2), &tmp));
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
@@ -1091,10 +1120,9 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
         p.nrows = 0; p.ntiles = 0; p.hints = 0;
         p.in_bs = in_bs; p.amp_bs = amp_bs; p.out_bs = out_bs;
         int rc;
-        const bool v2_ok = tma_ok && !((uintptr_t)p.in & 15);
-        if (version >= 2 && v2_ok) {
-            if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, nb, st) : N == 1024 ? launch_focus2<1024, false>(h, p, nb, st) : launch_focus2<2048, false>(h, p, nb, st);
-            else rc = N == 512 ? launch_focus2<512, true>(h, p, nb, st) : N == 1024 ? launch_focus2<1024, true>(h, p, nb, st) : launch_focus2<2048, true>(h, p, nb, st);
+        if (v2) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)
+            if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, st) : N == 1024 ? launch_focus2<1024, false>(h, p, st) : launch_focus2<2048, false>(h, p, st);
+            else rc = N == 512 ? launch_focus2<512, true>(h, p, st) : N == 1024 ? launch_focus2<1024, true>(h, p, st) : launch_focus2<2048, true>(h, p, st);
         } else if (dir < 0) rc = N == 512 ? launch_focus<512, false>(h, p, nb, st) : N == 1024 ? launch_focus<1024, false>(h, p, nb, st) : launch_focus<2048, false>(h, p, nb, st);
         else rc = N == 512 ? launch_focus<512, true>(h, p, nb, st) : N == 1024 ? launch_focus<1024, true>(h, p, nb, st) : launch_focus<2048, true>(h, p, nb, st);
         if (rc != PB_OK) return rc;
