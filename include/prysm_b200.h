@@ -361,6 +361,28 @@ int pb_tile(pb_handle_t h, int dtype, const void* in, int ny, int nx, int fy, in
 int pb_separable_tf(pb_handle_t h, int dtype, int kind, const void* fx, const void* fy, int ny, int nx,
                     double wx, double wy, void* out, void* stream);
 
+
+/* ---- deformable mirror and the cubic-spline warp (prysm/x/dm.py, prysm/coordinates.py:644-672) -------------------
+ * pb_spline_prefilter: coef (ny, nx, always float64) = the order-3 B-spline coefficients of the real array `in` (or the
+ *   real part of a complex one, in_complex != 0), both axes, mirror boundary: scipy.ndimage.spline_filter(in, 3,
+ *   output=float64, mode='mirror'), which is also what map_coordinates(mode='constant') prefilters with.
+ * pb_warp: out (oy, ox, real) = scale * map_coordinates(in, (y, x), order=3, mode='constant', cval=0) with
+ *   x, y either the arrays xc, yc (oy*ox values, float when coord_dtype is PB_C64, double for PB_C128) or, when both
+ *   are NULL, (x', y', w) = M (x, y, 1) / w at every output pixel (x = column, y = row) for the HOST row-major
+ *   3 x 3 matrix matrix_host, evaluated in fp64 on the device.  The coefficients live in handle scratch.
+ * pb_dm_scatter: poke (ny, nx, real) = act[(y - y0)/sy, (x - x0)/sx] at the lattice points y0 + k*sy, x0 + l*sx and 0
+ *   elsewhere (every sample is written): poke_arr[iyy, ixx] = actuators (prysm/x/dm.py:251).
+ * pb_dm_gather: act (nay, nax, real) = real(in)[y0 + k*sy, x0 + l*sx] (in real, or complex when in_complex != 0):
+ *   in_actuator_space[iyy, ixx] (prysm/x/dm.py:331). */
+int pb_spline_prefilter(pb_handle_t h, int dtype, const void* in, int in_complex, int ny, int nx, double* coef,
+                        void* stream);
+int pb_warp(pb_handle_t h, int dtype, const void* in, int in_complex, int ny, int nx, const void* xc, const void* yc,
+            int coord_dtype, const double* matrix_host, int oy, int ox, double scale, void* out, void* stream);
+int pb_dm_scatter(pb_handle_t h, int dtype, const void* act, int nay, int nax, int ny, int nx, int y0, int sy, int x0,
+                  int sx, void* poke, void* stream);
+int pb_dm_gather(pb_handle_t h, int dtype, const void* in, int in_complex, int ny, int nx, int nay, int nax, int y0,
+                 int sy, int x0, int sx, void* act, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

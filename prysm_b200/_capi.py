@@ -78,6 +78,10 @@ SIGNATURES = {
     'pb_tile': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _d, _vp, _vp]),
     'pb_separable_tf': (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _d, _d, _vp, _vp]),
     'pb_radial_window': (_i, [_vp, _i, _i, _i, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp, _vp]),
+    'pb_spline_prefilter': (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp]),
+    'pb_warp': (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(_d), _i, _i, _d, _vp, _vp]),
+    'pb_dm_scatter': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    'pb_dm_gather': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
 }
 
 

@@ -817,6 +817,83 @@ def separable_tf(kind, fx, fy, wx, wy):
     return out
 
 
+def _real_or_complex2d(a):
+    """2-D real (float32 / float64) or complex tensor, contiguous; returns (tensor, is_complex)."""
+    a = asdevice(a)
+    if a.ndim != 2:
+        raise ValueError(f'a 2-D array is required, got shape {tuple(a.shape)}')
+    if a.is_complex():
+        return a.contiguous(), True
+    return _real2d(a), False
+
+
+def spline_prefilter(a):
+    """float64 cubic B-spline coefficients of a real 2-D array (of the real part of a complex one), mirror boundary
+    (pb_spline_prefilter; scipy.ndimage.spline_filter(a, 3, output=float64, mode='mirror'))."""
+    a, cplx_in = _real_or_complex2d(a)
+    ny, nx = a.shape
+    out = torch.empty((ny, nx), dtype=torch.float64, device=a.device)
+    h, st = _ctx(a)
+    h.check(lib.pb_spline_prefilter(h.ptr, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, _p(out), st))
+    return out
+
+
+def warp(img, xc=None, yc=None, matrix=None, shape=None, scale=1.0, out=None):
+    """scale * map_coordinates(real(img), (yc, xc), order=3, mode='constant', cval=0) (pb_warp).  Either the
+    coordinate arrays (same shape; float32 or float64) or a host 3 x 3 `matrix` mapping each output pixel (x, y, 1)
+    of an output of `shape` (default: the input's) to input coordinates.  The result has img's real dtype."""
+    img, cplx_in = _real_or_complex2d(img)
+    ny, nx = img.shape
+    rd = _REAL_OF.get(img.dtype, img.dtype)
+    mp = None
+    if matrix is not None:
+        m, mp = _darr(np.asarray(matrix, dtype=np.float64).reshape(9))
+        oshape = (ny, nx) if shape is None else tuple(shape)
+        cdt, xc_t, yc_t = capi.PB_C128, None, None
+    else:
+        xc_t, yc_t = asdevice(xc), asdevice(yc)
+        if tuple(xc_t.shape) != tuple(yc_t.shape):
+            raise ValueError(f'coordinate arrays differ in shape: {tuple(xc_t.shape)} vs {tuple(yc_t.shape)}')
+        cd = torch.float64 if torch.float64 in (xc_t.dtype, yc_t.dtype) else torch.float32
+        xc_t, yc_t = xc_t.to(cd).contiguous(), yc_t.to(cd).contiguous()
+        oshape, cdt = tuple(xc_t.shape), _CODE[cd]
+    if out is None:
+        out = torch.empty(oshape, dtype=rd, device=img.device)
+    else:
+        _check_out(out, oshape, rd, img.device)
+        if not out.is_contiguous():
+            raise ValueError('`out` must be contiguous')
+    oy, ox = (oshape[0], int(np.prod(oshape[1:]))) if len(oshape) else (1, 1)
+    h, st = _ctx(img)
+    h.check(lib.pb_warp(h.ptr, _CODE[img.dtype], _p(img), int(cplx_in), ny, nx, _p(xc_t), _p(yc_t), cdt, mp, oy, ox,
+                        float(scale), _p(out), st))
+    return out
+
+
+def dm_scatter(act, shape, lattice):
+    """poke grid of `shape`: actuators on the lattice (y0, sy, x0, sx), zero elsewhere (pb_dm_scatter)."""
+    act = act.contiguous()
+    nay, nax = act.shape
+    ny, nx = shape
+    y0, sy, x0, sx = lattice
+    out = torch.empty((ny, nx), dtype=act.dtype, device=act.device)
+    h, st = _ctx(act)
+    h.check(lib.pb_dm_scatter(h.ptr, _CODE[act.dtype], _p(act), nay, nax, ny, nx, y0, sy, x0, sx, _p(out), st))
+    return out
+
+
+def dm_gather(a, nact, lattice):
+    """real(a) at the lattice points (y0 + k sy, x0 + l sx) -> (nact_y, nact_x) (pb_dm_gather)."""
+    a, cplx_in = _real_or_complex2d(a)
+    ny, nx = a.shape
+    nay, nax = nact
+    y0, sy, x0, sx = lattice
+    out = torch.empty((nay, nax), dtype=_REAL_OF.get(a.dtype, a.dtype), device=a.device)
+    h, st = _ctx(a)
+    h.check(lib.pb_dm_gather(h.ptr, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, nay, nax, y0, sy, x0, sx, _p(out), st))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

@@ -29,6 +29,13 @@ def make_polar_grid(shape, *, dx=0, diameter=0):
     return g['r'], g['t']
 
 
+def warp(img, xnew, ynew):
+    """Pull-warp a real image: out[i, j] = img at (row ynew[i, j], column xnew[i, j]) by cubic-spline interpolation,
+    0 outside the image (prysm/coordinates.py:644-672: map_coordinates(img, (ynew, xnew)) at order 3,
+    mode='constant', prefilter=True).  One prefilter and one interpolation kernel; the output has img's dtype."""
+    return _ops.warp(img, xc=xnew, yc=ynew)
+
+
 def cart_to_polar(x, y, vec_to_grid=True):
     """rho = hypot(x, y), phi = arctan2(y, x) (prysm/coordinates.py:73-102); 1-D vectors broadcast to a grid."""
     x, y = _ops.asdevice(x), _ops.asdevice(y)

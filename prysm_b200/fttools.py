@@ -361,24 +361,44 @@ class FFTDFT:
         return sum(v.numel() * v.element_size() for v in (self._pre_x, self._pre_y, self._post_x, self._post_y))
 
 
-def fourier_resample(f, zoom):
-    """Resample f by Fourier methods: centred FFT, then a sign=+1 matrix DFT onto int(m*zoom) x int(n*zoom)
-    samples spaced 1/zoom, scaled by 1/(m n) (prysm/fttools.py:538-593).  Real in -> real out."""
-    if zoom == 1:
-        return f
+def _resample_geometry(shape, zoom):
+    """(zoom pair, output shape) of fourier_resample, with the reference's checks (prysm/fttools.py:562-576)."""
     if isinstance(zoom, (float, int)):
         zoom = (zoom, zoom)
     elif not isinstance(zoom, tuple):
         zoom = tuple(float(z) for z in zoom)
     if len(zoom) != 2 or any(z <= 0 for z in zoom):
         raise ValueError('zoom must contain two positive values')
-    f = _ops.asdevice(f)
-    m, n = f.shape
+    m, n = shape
     M, N = int(m * zoom[0]), int(n * zoom[1])
     if M < 1 or N < 1:
         raise ValueError('zoom produces an empty output')
-    F = _ops.fft2(f, (m, n), dir=-1, shift_in=True, shift_out=True)
-    rng = lambda k: np.arange(-(k // 2), -(k // 2) + k, dtype=np.float64)      # noqa: E731  (fftrange on the host)
-    op = MDFT(rng(n), rng(m), rng(N) * (1.0 / zoom[1] / n), rng(M) * (1.0 / zoom[0] / m), sign=+1, norm=1.0 / (m * n))
-    out = op(F)
+    return zoom, (M, N)
+
+
+class FourierResampler:
+    """The fixed part of fourier_resample for one input shape and zoom, built once: calling it on an (m, n) array runs
+    the centred FFT and the matrix DFT and returns the COMPLEX (int(m*zoom), int(n*zoom)) result."""
+
+    def __init__(self, shape, zoom):
+        zoom, (M, N) = _resample_geometry(shape, zoom)
+        m, n = shape
+        rng = lambda k: np.arange(-(k // 2), -(k // 2) + k, dtype=np.float64)      # noqa: E731  (fftrange on the host)
+        self.shape, self.out_shape = (m, n), (M, N)
+        self._op = MDFT(rng(n), rng(m), rng(N) * (1.0 / zoom[1] / n), rng(M) * (1.0 / zoom[0] / m), sign=+1,
+                        norm=1.0 / (m * n))
+
+    def __call__(self, f):
+        F = _ops.fft2(f, self.shape, dir=-1, shift_in=True, shift_out=True)
+        return self._op(F)
+
+
+def fourier_resample(f, zoom):
+    """Resample f by Fourier methods: centred FFT, then a sign=+1 matrix DFT onto int(m*zoom) x int(n*zoom)
+    samples spaced 1/zoom, scaled by 1/(m n) (prysm/fttools.py:538-593).  Real in -> real out."""
+    if zoom == 1:
+        return f
+    _resample_geometry(tuple(f.shape), zoom)
+    f = _ops.asdevice(f)
+    out = FourierResampler(tuple(f.shape), zoom)(f)
     return out if f.is_complex() else out.real

@@ -20,6 +20,8 @@ touches numpy `exp` or eager tensor arithmetic.
 import importlib
 
 from . import convolution as _conv
+from . import coordinates as _coords
+from . import dm as _dm
 from . import fttools as _ft
 from . import otf as _otf
 from . import polynomials as _poly
@@ -62,6 +64,8 @@ _TARGETS = {
     'prysm.polynomials': {'sum_of_2d_modes': _poly.sum_of_2d_modes, 'sum_of_2d_modes_adjoint': _poly.sum_of_2d_modes_adjoint},
     'prysm.polynomials.fitting': {'sum_of_2d_modes': _poly.sum_of_2d_modes,
                                   'sum_of_2d_modes_adjoint': _poly.sum_of_2d_modes_adjoint},
+    'prysm.coordinates': {'warp': _coords.warp},
+    'prysm.x.dm': {'DM': _dm.DM},
 }
 
 _saved = {}  # (module name, attribute) -> original
@@ -171,11 +175,16 @@ def set_backend_to_b200(device=None):
         raise ImportError('set_backend_to_b200() plugs into an installed prysm; it is not importable here') from exc
     from .conf import config
     config.precision = pconf.config.precision  # follow prysm's precision setting
-    for modname, repl in _TARGETS.items():
+    # import every target before re-binding any: a module imported mid-way (prysm.x.dm binds fourier_resample,
+    # apply_transfer_functions and warp at import time) would otherwise capture engine functions as its defaults
+    mods = {}
+    for modname in _TARGETS:
         try:
-            mod = importlib.import_module(modname)
+            mods[modname] = importlib.import_module(modname)
         except ImportError:
             continue
+    for modname, mod in mods.items():
+        repl = _TARGETS[modname]
         if modname == 'prysm.otf':   # these return RichData: hand back the reference's own container
             repl = {k: _returning_reference_richdata(v) for k, v in repl.items()}
         for attr, new in repl.items():
