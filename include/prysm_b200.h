@@ -383,6 +383,58 @@ int pb_dm_scatter(pb_handle_t h, int dtype, const void* act, int nay, int nax, i
 int pb_dm_gather(pb_handle_t h, int dtype, const void* in, int in_complex, int ny, int nx, int nay, int nax, int y0,
                  int sy, int x0, int sx, void* act, void* stream);
 
+
+/* ---- signed-distance geometry and segmented apertures (prysm/geometry.py, prysm/segmented.py:133-368) -------------
+ * pb_sdf: out (ny, nx) = the signed distance (negative inside) of one shape at (x, y), computed in fp64 and rounded
+ *   once to dtype's real type, or with mask != 0 the uint8 mask sdf <= 0.  separable != 0: x is a row of nx values and
+ *   y a column of ny values (optimize_xy_separable's form); otherwise both are (ny, nx).  Parameters, HOST:
+ *     PB_SDF_POLYGON          verts = nverts (x, y) vertices, any winding, even-odd parity   (geometry.py:419-463)
+ *     PB_SDF_SPIDER           params = half width, cx, cy; verts = (cos, sin) of each vane's angle (geometry.py:550-594)
+ *     PB_SDF_RECTANGLE        params = half width, half height, mode (0 none, 1 swap x/y, 2 rotate), cos, sin
+ *                             (geometry.py:182-222)
+ *     PB_SDF_FILLET_RECTANGLE params = half width, half height, fillet radius, cx, cy, rotate (0/1), cos, sin
+ *                             (geometry.py:656-696)
+ *     PB_SDF_ANNULUS          x = r (y unused); params = inner radius, outer radius        (geometry.py:375-395)
+ *     PB_SDF_OFFSET_CIRCLE    params = radius, cx, cy                                       (geometry.py:627-653)
+ *   At most 8 params and 128 vertices / vanes.
+ * pb_sdf_combine: out = min(a, b) (PB_SDF_UNION), max(a, b) (PB_SDF_INTERSECT) or max(a, -b) (PB_SDF_SUBTRACT)
+ *   (geometry.py:37-93).
+ * Segments: the DEVICE table `seg` has PB_SEGMENT_FIELDS int64 per segment: window row y0, column x0, height, width, the
+ *   offset of its h*w samples in the packed per-segment buffers, and the offset of its (nmodes, h, w) basis in `bases`.
+ *   tile_ptr (tiles_y*tiles_x + 1) / tile_seg (int32, DEVICE) list, per output tile of PB_SEGMENT_TILE_Y x
+ *   PB_SEGMENT_TILE_X samples (row-major tiles), the segments whose windows meet it, in ascending segment order.
+ * pb_hex_segments: for every listed segment, cover = clip(0.5 - polygon_sdf/dx, 0, 1) over its window, local_x = x - cx,
+ *   local_y = y - cy (packed like cover); amp (ny, nx) = max of cover over the covering segments, 0 elsewhere.  geo
+ *   (DEVICE fp64) holds per segment nverts (x, y) vertices, then (cx, cy); 3 <= nverts <= 8.
+ * pb_segment_compose: out (ny, nx) += sum over segments s < ncoef of mask_s * sum_k coefs[s*coef_stride + k] *
+ *   base_{s,k} over its window (compose_opd), accumulated per sample in fp64 in segment order and rounded once; coefs
+ *   is a DEVICE fp64 array.  No atomics.
+ * pb_segment_compose_adjoint: out (nseg, nmodes) = sum over segment s's window of opdbar * mask_s * base_{s,k},
+ *   through `partial` (DEVICE fp64, nseg * nchunk * nmodes) with nchunk * PB_SEGMENT_CHUNK >= every window's h*w:
+ *   a fixed-order two-level reduction. */
+typedef enum {
+    PB_SDF_POLYGON = 0, PB_SDF_SPIDER = 1, PB_SDF_RECTANGLE = 2, PB_SDF_FILLET_RECTANGLE = 3, PB_SDF_ANNULUS = 4,
+    PB_SDF_OFFSET_CIRCLE = 5
+} pb_sdf_kind;
+typedef enum { PB_SDF_UNION = 0, PB_SDF_INTERSECT = 1, PB_SDF_SUBTRACT = 2 } pb_sdf_op;
+typedef enum {
+    PB_SEGMENT_FIELDS = 6, PB_SEGMENT_TILE_Y = 32, PB_SEGMENT_TILE_X = 64, PB_SEGMENT_CHUNK = 2048
+} pb_segment_layout;
+int pb_sdf(pb_handle_t h, int dtype, int kind, const void* x, const void* y, int separable, int ny, int nx,
+           const double* params_host, int nparams, const double* verts_host, int nverts, int mask, void* out,
+           void* stream);
+int pb_sdf_combine(pb_handle_t h, int dtype, int op, const void* a, const void* b, long long count, void* out,
+                   void* stream);
+int pb_hex_segments(pb_handle_t h, int dtype, const void* x, const void* y, int ny, int nx, int tiles_y, int tiles_x,
+                    const int* tile_ptr, const int* tile_seg, const long long* seg, const double* geo, int nverts,
+                    double dx, void* cover, void* local_x, void* local_y, void* amp, void* stream);
+int pb_segment_compose(pb_handle_t h, int dtype, int ny, int nx, int tiles_y, int tiles_x, const int* tile_ptr,
+                       const int* tile_seg, const long long* seg, const void* masks, const void* bases, int nmodes,
+                       const double* coefs, long long coef_stride, int ncoef, void* out, void* stream);
+int pb_segment_compose_adjoint(pb_handle_t h, int dtype, int ny, int nx, int nseg, const long long* seg,
+                               const void* masks, const void* bases, int nmodes, const void* opdbar, int nchunk,
+                               double* partial, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

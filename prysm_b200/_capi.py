@@ -82,7 +82,16 @@ SIGNATURES = {
     'pb_warp': (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(_d), _i, _i, _d, _vp, _vp]),
     'pb_dm_scatter': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     'pb_dm_gather': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    'pb_sdf': (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, C.POINTER(_d), _i, C.POINTER(_d), _i, _i, _vp, _vp]),
+    'pb_sdf_combine': (_i, [_vp, _i, _i, _vp, _vp, _ll, _vp, _vp]),
+    'pb_hex_segments': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _d, _vp, _vp, _vp, _vp, _vp]),
+    'pb_segment_compose': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _ll, _i, _vp, _vp]),
+    'pb_segment_compose_adjoint': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
 }
+
+SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
+SDF_UNION, SDF_INTERSECT, SDF_SUBTRACT = range(3)
+SEGMENT_FIELDS, SEGMENT_TILE_Y, SEGMENT_TILE_X, SEGMENT_CHUNK = 6, 32, 64, 2048
 
 
 def load_library(path=LIB_PATH):

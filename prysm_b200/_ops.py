@@ -894,6 +894,90 @@ def dm_gather(a, nact, lattice):
     return out
 
 
+def _real_pair(x, y):
+    x = asdevice(x)
+    y = None if y is None else asdevice(y)
+    rd = torch.float64 if torch.float64 in (x.dtype, getattr(y, 'dtype', None)) else torch.float32
+    return x.to(rd).contiguous(), (None if y is None else y.to(rd).contiguous())
+
+
+SDF_MAX_VERTICES = 128      # the shape travels in kernel-parameter space (csrc/geometry.cu)
+
+
+def sdf(kind, x, y, params=(), verts=None, mask=False):
+    """One signed-distance shape (pb_sdf) on a pair of (ny, nx) grids, or on the separable row (nx values) and
+    column (ny values) that optimize_xy_separable reduces them to; y is None for the annulus (x is then r, any
+    shape).  Returns the real distance in the coordinates' dtype, or the bool mask sdf <= 0."""
+    x, y = _real_pair(x, y)
+    if y is None or tuple(x.shape) == tuple(y.shape):
+        oshape = tuple(x.shape)
+        separable, ny = 0, (oshape[0] if len(oshape) > 1 else 1)
+        nx = x.numel() // ny if ny else 0
+    else:
+        if x.ndim > 2 or y.ndim > 2 or (x.ndim == 2 and x.shape[0] != 1) or (y.ndim == 2 and y.shape[1] != 1):
+            raise ValueError(f'x {tuple(x.shape)} and y {tuple(y.shape)} are neither one grid shape nor a row and a column')
+        ny, nx = y.numel(), x.numel()
+        oshape, separable = (ny, nx), 1
+    out = torch.empty(oshape, dtype=torch.bool if mask else x.dtype, device=x.device)
+    p, pp = _darr(np.asarray(params, dtype=np.float64).reshape(-1))
+    v = np.zeros(0) if verts is None else np.asarray(verts, dtype=np.float64).reshape(-1)
+    if len(v) // 2 > SDF_MAX_VERTICES:
+        raise ValueError(f'{len(v) // 2} polygon vertices or spider vanes: at most {SDF_MAX_VERTICES} are supported')
+    v, vp = _darr(v)
+    h, st = _ctx(x)
+    h.check(lib.pb_sdf(h.ptr, _CODE[x.dtype], int(kind), _p(x), _p(y), separable, int(ny), int(nx), pp, len(p), vp,
+                       len(v) // 2, int(bool(mask)), _p(out), st))
+    return out
+
+
+def sdf_combine(op, a, b):
+    """min(a, b) / max(a, b) / max(a, -b) of two signed distances (pb_sdf_combine); the two arrays broadcast
+    against each other as numpy's minimum / maximum do."""
+    a, b = _real_pair(a, b)
+    if a.shape != b.shape:
+        a, b = (t.contiguous() for t in torch.broadcast_tensors(a, b))
+    out = torch.empty_like(a)
+    h, st = _ctx(a)
+    h.check(lib.pb_sdf_combine(h.ptr, _CODE[a.dtype], int(op), _p(a), _p(b), a.numel(), _p(out), st))
+    return out
+
+
+def hex_segments(x, y, tiles, seg, geo, nverts, dx, total):
+    """Coverage, local x, local y of every segment window, packed (`total` samples each), and the amplitude
+    (pb_hex_segments).  tiles = (tiles_y, tiles_x, tile_ptr, tile_seg); seg / geo are the device tables."""
+    ny, nx = x.shape
+    ty, tx, ptr, lst = tiles
+    cover, lx, ly = (torch.empty(total, dtype=x.dtype, device=x.device) for _ in range(3))
+    amp = torch.empty((ny, nx), dtype=x.dtype, device=x.device)
+    h, st = _ctx(x)
+    h.check(lib.pb_hex_segments(h.ptr, _CODE[x.dtype], _p(x), _p(y), ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(geo),
+                                int(nverts), float(dx), _p(cover), _p(lx), _p(ly), _p(amp), st))
+    return cover, lx, ly, amp
+
+
+def segment_compose(tiles, seg, masks, bases, nmodes, coefs, ncoef, out):
+    """out += the masked per-segment modal sums of the first `ncoef` segments (pb_segment_compose); coefs is a
+    contiguous (n, nmodes) float64 device tensor."""
+    ny, nx = out.shape
+    ty, tx, ptr, lst = tiles
+    h, st = _ctx(out)
+    h.check(lib.pb_segment_compose(h.ptr, _CODE[out.dtype], ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(masks), _p(bases),
+                                   int(nmodes), _p(coefs), int(nmodes), int(ncoef), _p(out), st))
+    return out
+
+
+def segment_compose_adjoint(seg, nseg, masks, bases, nmodes, opdbar, max_window):
+    """(nseg, nmodes) = per-segment windowed projections of opdbar * mask onto the basis (pb_segment_compose_adjoint)."""
+    ny, nx = opdbar.shape
+    nchunk = max(1, -(-int(max_window) // capi.SEGMENT_CHUNK))
+    partial = torch.empty(max(1, nseg * nchunk * nmodes), dtype=torch.float64, device=opdbar.device)
+    out = torch.empty((nseg, nmodes), dtype=opdbar.dtype, device=opdbar.device)
+    h, st = _ctx(opdbar)
+    h.check(lib.pb_segment_compose_adjoint(h.ptr, _CODE[opdbar.dtype], ny, nx, int(nseg), _p(seg), _p(masks), _p(bases),
+                                           int(nmodes), _p(opdbar), nchunk, _p(partial), _p(out), st))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)
