@@ -210,6 +210,11 @@ __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, 
     asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global [%0, {%1, %2, %3}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// programmatic dependent launch: let the next kernel of the stream (launched with the programmatic-serialization
+// attribute) be scheduled on the SMs this grid frees; wait until the previous kernel has completed and its memory is
+// visible (no-op for a kernel launched without the attribute)
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void st_hint(float4* p, float4 v, uint64_t pol) {
     asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
 }
@@ -316,6 +321,9 @@ struct FocusParams {
     // 1: L2 eviction hints (streams evict_first); 2: L2 prefetch of the tile after next; 4 (v2 with focus_row4_kernel):
     // plane 0 of the intermediate is written evict_last, and the row kernel discards its lines once they are read
     int hints;
+    // v2 column kernel launched as a programmatic dependent of the previous field's row kernel: 1 = its input does not
+    // overlap what that kernel writes, so the first tile may be gathered (and transformed) before the wait; 0 = wait first
+    int early_input;
 };
 
 template <int L> struct Geo2 {

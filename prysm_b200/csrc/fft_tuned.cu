@@ -277,6 +277,9 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
         sync();   // this group's exchange buffers are free for its next tile
 #pragma unroll
         for (int g = 0; g < G::GI; ++g) dftR<G::R3, INV>(v + g * G::R3);
+        // the intermediate is the previous field's row kernel's input (and its plane 0 is being discarded there): the first
+        // store waits for that kernel to complete
+        if (it == 0 && p.early_input) pdl_wait();
         // tile-major store: element (plane, j, tile, c) at ((plane*L/4 + j/4) * TILES + tile) * 16 + (j%4)*4 + c ; c = 2 cp
         float4* __restrict__ dst = reinterpret_cast<float4*>(
             p.tmp + fb * (2LL * L * L) + (long long)HALF * L * L + ((long long)(t >> 2) * G2::TILES + tile) * 16 + (t & 3) * 4 + 2 * cp);
@@ -309,6 +312,10 @@ __global__ void __launch_bounds__(Geo4<L>::THREADS) focus_col4_kernel(const __gr
         *reinterpret_cast<unsigned int*>(bar + 2) = 0u;   // release counter of the staging area
         mbar_fence_init();
     }
+    // every CTA of the grid is resident (one per SM, grid <= SMs): the row kernel that follows may take each SM this
+    // kernel's last wave frees, and run its prologue there
+    pdl_launch_dependents();
+    if (!p.early_input) pdl_wait();
     __syncthreads();
     const int grp = threadIdx.x / (2 * G::NT);
     if (grp == 0) focus_col4_group<L, INV, 0>(in_map, p, smem4, bar);
@@ -442,6 +449,11 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
         mbar_expect_tx(bars, (uint32_t)(G4::PLANLEN * sizeof(float2)));
         bulk_g2s(smraw + R4::PLAN_OFF, p.plan, (uint32_t)(G4::PLANLEN * sizeof(float2)), bars);
     }
+    // all CTAs are resident (grid <= SMs): the next field's column kernel may take the SMs this grid's last wave frees.
+    // The intermediate comes from the column kernel before this one: wait for it to complete (the prologue above -- the
+    // static plan -- overlapped its tail)
+    pdl_launch_dependents();
+    pdl_wait();
     __syncthreads();
     if (t == 0 && r < p.nrows) request_row(r);
     const SyncGroup gsync{1 + grp, NT};
@@ -635,9 +647,11 @@ int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, 
 namespace {
 
 
-// one field: `p.tmp` holds its [2][L][L] intermediate
+// one field: `p.tmp` holds its [2][L][L] intermediate.  col_dep: how the column kernel follows what precedes it in the
+// stream -- 0: plain launch; 1: programmatic dependent of the previous field's row kernel; 2: the same, and its input does
+// not overlap that kernel's output (the first tile is gathered before the wait)
 template <int L, bool INV>
-int launch_focus2(Handle* h, FocusParams p, cudaStream_t st) {
+int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     constexpr int batch = 1;
     using G = Geo<L>;
     using G2 = Geo2<L>;
@@ -680,13 +694,35 @@ int launch_focus2(Handle* h, FocusParams p, cudaStream_t st) {
         PB_TRY(get_map_c64(h, MapKey{p.in, 2, L, batch, p.in_ld, batch > 1 ? p.in_bs : 0}, 3, dims, str, box, &map));
         in_m = *map;
     }
+    // Programmatic dependent launch (`pdl`): each kernel of the chain col(f), row(f), col(f + 1), ... is launched with
+    // programmatic stream serialization, so that its CTAs take the SMs the previous kernel's last wave frees and run their
+    // prologue (barriers, plan, for a column kernel with `early_input` its first gather and transform) while that wave
+    // finishes; griddepcontrol.wait orders everything that depends on the previous kernel.  The column kernel of the
+    // first field of a call is launched plainly: what precedes it is not known.
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    auto launch = [&](auto kern, int grid, int threads, size_t smem, bool dependent, const CUtensorMap& map) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(grid);
+        cfg.blockDim = dim3(threads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cfg.attrs = dependent ? &attr : nullptr;
+        cfg.numAttrs = dependent ? 1 : 0;
+        return cudaLaunchKernelEx(&cfg, kern, map, p);
+    };
     // column pass: one CTA per SM walks the tiles of the field
     p.plan = reinterpret_cast<const float4*>(plan_col);
-    colk<<<std::min(h->sm_count, p.ntiles), G4::THREADS, smem_col, st>>>(in_m, p);
-    PB_LAUNCH_CHECK(h);
+    static const bool pdl = env_int("PB_FOCUS_PDL", 1) != 0;
+    if (!pdl) col_dep = 0;
+    p.early_input = col_dep == 2;
+    PB_CUDA(h, launch(colk, std::min(h->sm_count, p.ntiles), G4::THREADS, smem_col, col_dep > 0, in_m));
+    h->launches++;
+    p.early_input = 0;
     if (row_version == 4) {   // four line groups per CTA, plan in shared memory
         PB_TRY(set_smem_attrs(h, focus_row4_kernel<L, INV>, GeoR4<L>::SMEM, 1));
-        focus_row4_kernel<L, INV><<<std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, GeoR4<L>::SMEM, st>>>(tmp_m, p);
+        PB_CUDA(h, launch(focus_row4_kernel<L, INV>, std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, GeoR4<L>::SMEM, pdl, tmp_m));
     } else {
         p.plan = plan_row;
         focus_row2_kernel<L, INV><<<std::min(h->sm_count * row_ctas, p.nrows), L / 16, smem_row, st>>>(tmp_m, p);
@@ -1087,13 +1123,20 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
     if (out_kind == PB_OUT_COMPLEX ? (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 15) : (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 7))
         return PB_ERR_UNSUPPORTED;  // vector stores need aligned rows
     const int N = nx;
-    // 2 = column kernel + row kernel per group of fields (default); 3 = the role-specialised single kernel of
-    // focus_fused.cu (opt-in, bit-identical, not faster than the kernel pair)
+    // 2 = column kernel + row kernel per field; 3 = the role-specialised single kernel of focus_fused.cu with a whole
+    // field as its unit of work (opt-in, bit-identical; its 64 MiB unit does not fit L2 at N = 2048); 4 = the same kernel
+    // skeleton with one plane of one field as the unit, so that the whole intermediate stays in L2 (opt-in,
+    // bit-identical; at N = 2048 it moves 192 instead of 224 MiB per propagation but is limited by its column side:
+    // 149 us against the pair's 128 us on a 400 W H100 without launch_focus2's programmatic dependent launch, DESIGN 4.1)
     static const int version = env_int("PB_FOCUS_V", 2);
-    // v2 / v3 take their input tiles by tensor TMA: complex input, 16-byte aligned base and even pitches; everything else
-    // (the fused phase-screen input, odd pitches) runs the v1 kernels
+    // v2 / v3 / v4 take their input tiles by tensor TMA: complex input, 16-byte aligned base and even pitches; everything
+    // else (the fused phase-screen input, odd pitches) runs the v1 kernels
     const bool tma_ok = in_kind == PB_IN_COMPLEX && !((uintptr_t)in & 15) && !(in_ld & 1) && !(in_bs & 1);
-    if (version >= 3 && tma_ok) {   // stacks: one role-specialised kernel, column and row passes overlapped (focus_fused.cu)
+    if (version == 4 && tma_ok) {   // stacks: one launch, one plane of one field per unit of work (focus_fused.cu)
+        const int rc = try_focus_plane(h, N, dir, in, in_ld, in_bs, batch, out, out_kind, out_ld, out_bs, scale, weight, st);
+        if (rc != PB_ERR_UNSUPPORTED) return rc;
+    }
+    if (version == 3 && tma_ok) {   // stacks: one role-specialised kernel, column and row passes overlapped (focus_fused.cu)
         const int rc = try_focus_fused(h, N, dir, in, in_ld, in_bs, batch, out, out_kind, out_ld, out_bs, scale, weight, st);
         if (rc != PB_ERR_UNSUPPORTED) return rc;
     }
@@ -1106,6 +1149,11 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
     const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : sizeof(float);
     const size_t out_elt = out_kind == PB_OUT_COMPLEX ? sizeof(float2) : sizeof(float);
+    // v2, fields after the first: the column kernel follows this call's previous row kernel (programmatic dependent
+    // launch, see launch_focus2); it may gather its input early unless the input stack overlaps the output stack
+    const uintptr_t in_lo = (uintptr_t)in, in_hi = in_lo + (size_t)((long long)(batch - 1) * in_bs + (long long)(ny - 1) * in_ld + nx) * in_elt;
+    const uintptr_t out_lo = (uintptr_t)out, out_hi = out_lo + (size_t)((long long)(batch - 1) * out_bs + (long long)(ky - 1) * out_ld + kx) * out_elt;
+    const int col_dep_next = (in_hi <= out_lo || out_hi <= in_lo) ? 2 : 1;
     for (int b0 = 0; b0 < batch; b0 += per) {
         const int nb = std::min(per, batch - b0);
         FocusParams p;
@@ -1117,12 +1165,13 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
         p.plan = nullptr;
         p.out = reinterpret_cast<char*>(out) + (size_t)b0 * out_bs * out_elt;
         p.out_ld = out_ld; p.out_kind = out_kind; p.scale = (float)scale; p.weight = (float)weight;
-        p.nrows = 0; p.ntiles = 0; p.hints = 0;
+        p.nrows = 0; p.ntiles = 0; p.hints = 0; p.early_input = 0;
         p.in_bs = in_bs; p.amp_bs = amp_bs; p.out_bs = out_bs;
         int rc;
         if (v2) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)
-            if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, st) : N == 1024 ? launch_focus2<1024, false>(h, p, st) : launch_focus2<2048, false>(h, p, st);
-            else rc = N == 512 ? launch_focus2<512, true>(h, p, st) : N == 1024 ? launch_focus2<1024, true>(h, p, st) : launch_focus2<2048, true>(h, p, st);
+            const int cd = b0 > 0 ? col_dep_next : 0;
+            if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
+            else rc = N == 512 ? launch_focus2<512, true>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, true>(h, p, cd, st) : launch_focus2<2048, true>(h, p, cd, st);
         } else if (dir < 0) rc = N == 512 ? launch_focus<512, false>(h, p, nb, st) : N == 1024 ? launch_focus<1024, false>(h, p, nb, st) : launch_focus<2048, false>(h, p, nb, st);
         else rc = N == 512 ? launch_focus<512, true>(h, p, nb, st) : N == 1024 ? launch_focus<1024, true>(h, p, nb, st) : launch_focus<2048, true>(h, p, nb, st);
         if (rc != PB_OK) return rc;

@@ -22,4 +22,8 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
 int try_focus_fused(Handle* h, int N, int dir, const void* in, long long in_ld, long long in_bs, int batch, void* out, int out_kind,
                     long long out_ld, long long out_bs, double scale, double weight, cudaStream_t st);
 
+// The same with one plane of one field as the unit of work, the whole stack in one launch (focus_fused.cu)
+int try_focus_plane(Handle* h, int N, int dir, const void* in, long long in_ld, long long in_bs, int batch, void* out, int out_kind,
+                    long long out_ld, long long out_bs, double scale, double weight, cudaStream_t st);
+
 }  // namespace pb

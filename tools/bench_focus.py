@@ -1,0 +1,154 @@
+"""Kernel-level timing of the batched focus pipeline at the benchmark's shape, one variant per subprocess.
+
+    python tools/bench_focus.py [--variants SPEC ...] [--alternate N] [--intensity] [--profile DIR] [--out FILE.json]
+
+SPEC is `V` or `V:KEY=VAL,KEY=VAL`: PB_FOCUS_V=V plus extra environment switches, e.g. `4:PB_FOCUS_L2_SLACK_MIB=8`
+or `4:PB_FUSED_NCOL=60`.  The switches are read once per process, so every variant runs in a process of its own.
+Each run times `propagation.focus` (and, with --intensity, `propagation.focus_intensity`) on a (16, 2048, 2048)
+complex64 stack -> 4096^2 with CUDA events over a window of at least 0.5 s, and reports microseconds per
+propagation, the algorithmic bandwidth (pupil read + field written) and the HBM bytes the variant moves, counted from
+the shapes.  --alternate N runs the variant list N times in turn (A/B/A/B...), so that drifts of the card show as
+spread.  --profile DIR writes torch.profiler kernel times of one call per variant under DIR.  The card's name, power
+limit and SM clock are printed with the numbers (read-only nvidia-smi queries).
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+N, Q, BATCH = 2048, 2, 16
+K = N * Q
+MIB = 2 ** 20
+ALG = {'complex': 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 4 * K * K}
+# HBM bytes per propagation counted from the shapes: pupil reads, the part of the 16 N^2-byte intermediate that leaves
+# L2 (written and read back), output writes
+HBM = {
+    '1': {'complex': 8 * N * N + 2 * 16 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 16 * N * N + 4 * K * K},
+    '2': {'complex': 8 * N * N + 2 * 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 8 * N * N + 4 * K * K},
+    '3': {'complex': 8 * N * N + 2 * 16 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 16 * N * N + 4 * K * K},
+    '4': {'complex': 2 * 8 * N * N + 8 * K * K, 'intensity': 2 * 8 * N * N + 4 * K * K},
+}
+
+_CHILD = r'''
+import json, sys, time
+import torch
+sys.path.insert(0, %(root)r)
+import prysm_b200 as pb
+from prysm_b200 import propagation as P, _ops
+pb.config.precision = 32
+N, Q, B = %(n)d, %(q)d, %(b)d
+gen = torch.Generator(device='cuda').manual_seed(5)
+stack = torch.complex(torch.randn((B, N, N), generator=gen, device='cuda'), torch.randn((B, N, N), generator=gen, device='cuda'))
+res = {}
+kinds = ['complex'] + (['intensity'] if %(intensity)r else [])
+for kind in kinds:
+    fn = (lambda: P.focus(stack, Q)) if kind == 'complex' else (lambda: P.focus_intensity(stack, Q))
+    for _ in range(3):
+        out = fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(); out = fn(); e1.record(); torch.cuda.synchronize()
+    reps = max(4, int(0.6e3 / max(e0.elapsed_time(e1), 1e-3)) + 1)   # a window of >= 0.5 s
+    l0 = _ops.launch_count()
+    e0.record()
+    for _ in range(reps):
+        out = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1)
+    res[kind] = {'us_per_prop': ms * 1e3 / (reps * B), 'window_ms': ms, 'calls': reps,
+                 'launches_per_call': (_ops.launch_count() - l0) / reps}
+    del out
+    if %(profile)r:
+        from torch.profiler import profile, ProfilerActivity
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn(); torch.cuda.synchronize()
+        kt = {}
+        for ev in prof.events():
+            if ev.device_type == torch.autograd.DeviceType.CUDA:
+                kt.setdefault(ev.name, []).append(ev.device_time_total if hasattr(ev, 'device_time_total') else ev.cuda_time_total)
+        res[kind]['kernels_us'] = {k: {'count': len(v), 'total': sum(v), 'mean': sum(v) / len(v)} for k, v in kt.items()}
+print('RESULT', json.dumps(res))
+'''
+
+
+def card():
+    q = 'name,power.limit,clocks.sm,clocks.max.sm'
+    try:
+        r = subprocess.run(['nvidia-smi', f'--query-gpu={q}', '--format=csv,noheader', '-i', '0'],
+                           capture_output=True, text=True, timeout=30)
+        return r.stdout.strip().splitlines()[0]
+    except (OSError, subprocess.SubprocessError, IndexError):
+        return 'nvidia-smi unavailable'
+
+
+def parse_spec(spec):
+    v, _, rest = spec.partition(':')
+    env = {'PB_FOCUS_V': v}
+    for kv in filter(None, rest.split(',')):
+        k, _, val = kv.partition('=')
+        env[k] = val
+    return v, env
+
+
+def run_variant(spec, intensity, profile):
+    v, env = parse_spec(spec)
+    e = {k: val for k, val in os.environ.items() if not k.startswith('PB_')}
+    e.update(env)
+    src = _CHILD % {'root': ROOT, 'n': N, 'q': Q, 'b': BATCH, 'intensity': intensity, 'profile': bool(profile)}
+    r = subprocess.run([sys.executable, '-c', src], env=e, capture_output=True, text=True, timeout=900)
+    if r.returncode != 0:
+        raise RuntimeError(f'{spec}: exit {r.returncode}\n{r.stderr[-3000:]}')
+    res = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith('RESULT ')][-1][7:])
+    for kind, row in res.items():
+        us = row['us_per_prop']
+        row['alg_gbs'] = ALG[kind] / (us * 1e-6) / 1e9
+        hbm = HBM.get(v, {}).get(kind)
+        row['hbm_mib_counted'] = hbm / MIB if hbm else None
+        row['hbm_gbs_counted'] = hbm / (us * 1e-6) / 1e9 if hbm else None
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--variants', nargs='+', default=['2', '3', '4'])
+    ap.add_argument('--alternate', type=int, default=1, metavar='N', help='run the variant list N times in turn')
+    ap.add_argument('--intensity', action='store_true', help='time focus_intensity (the fused PSF variant) too')
+    ap.add_argument('--profile', default=None, metavar='DIR', help='write torch.profiler kernel times under DIR')
+    ap.add_argument('--out', default=None)
+    args = ap.parse_args()
+    print('card (name, power limit, SM clock, max SM clock):', card(), flush=True)
+    runs = []
+    for rnd in range(args.alternate):
+        for spec in args.variants:
+            res = run_variant(spec, args.intensity, args.profile)
+            runs.append({'round': rnd, 'variant': spec, **res})
+            line = f'[{rnd}] {spec:32s}'
+            for kind, row in res.items():
+                hbm = f'{row["hbm_mib_counted"]:.0f} MiB' if row['hbm_mib_counted'] else 'n/a'
+                line += (f'  {kind}: {row["us_per_prop"]:7.1f} us/prop  {row["alg_gbs"]:6.0f} GB/s alg  '
+                         f'HBM {hbm}  {row["launches_per_call"]:.0f} launches/call')
+            print(line, flush=True)
+            if args.profile:
+                os.makedirs(args.profile, exist_ok=True)
+                name = spec.replace(':', '_').replace(',', '_').replace('=', '-')
+                with open(os.path.join(args.profile, f'kernels_{name}_{rnd}.json'), 'w') as fh:
+                    json.dump(res, fh, indent=1)
+    print('card after:', card(), flush=True)
+    summary = {}
+    for spec in args.variants:
+        for kind in ('complex', 'intensity'):
+            xs = [r[kind]['us_per_prop'] for r in runs if r['variant'] == spec and kind in r]
+            if xs:
+                summary[f'{spec} {kind}'] = {'min': min(xs), 'max': max(xs), 'spread_pct': 100 * (max(xs) - min(xs)) / min(xs)}
+    for k, s in summary.items():
+        print(f'{k:44s} min {s["min"]:7.1f}  max {s["max"]:7.1f} us/prop  spread {s["spread_pct"]:.1f} %')
+    if args.out:
+        with open(args.out, 'w') as fh:
+            json.dump({'card': card(), 'runs': runs, 'summary': summary}, fh, indent=1)
+
+
+if __name__ == '__main__':
+    main()
