@@ -1,5 +1,5 @@
-// Register-resident packed-lane FFT engine shared by the tuned kernels (fft_tuned.cu, focus_fused.cu): radix-16 butterflies on
-// two packed fp32 lanes, the two-exchange FFT_L skeleton, async-copy / TMA plumbing, and the geometry of the focus pipeline.
+// Register-resident packed-lane FFT engine of the tuned kernels (fft_tuned.cu): radix-16 butterflies on two packed fp32
+// lanes, the two-exchange FFT_L skeleton, async-copy / TMA plumbing, and the geometry of the focus pipeline.
 // Everything device-side lives in an anonymous namespace (each translation unit gets its own copy).
 #pragma once
 #include <cstdlib>
@@ -7,10 +7,6 @@
 #include "fft_tuned.cuh"
 
 namespace pb {
-
-// TMA descriptor (complex64 elements as UINT64), cached in the handle by (base pointer, geometry); defined in fft_tuned.cu
-int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                const cuuint32_t* box, const CUtensorMap** out);
 
 namespace {
 
@@ -153,19 +149,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                  "l"(src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {   // non-blocking
-    uint32_t ok;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
@@ -316,10 +299,12 @@ struct FocusParams {
     // batch of independent fields in one launch pair (blockIdx.y in the column kernel; rows of all fields in the row
     // kernel's persistent loop): element strides of in / amp / out in units of their own scalar type
     long long in_bs, amp_bs, out_bs;
-    // v2 pipeline
-    int ntiles;             // column kernel: batch * N / T tiles, walked by a persistent grid
-    // 1: L2 eviction hints (streams evict_first); 2: L2 prefetch of the tile after next; 4 (v2 with focus_row4_kernel):
-    // plane 0 of the intermediate is written evict_last, and the row kernel discards its lines once they are read
+    // v2 pipeline (one field per launch pair)
+    int ntiles;             // column kernel: N / T tiles, walked by a persistent grid
+    // 1: L2 eviction hints (streams evict_first); 2: L2 prefetch of the tile after next (unused); 4: plane 0 of the
+    // intermediate is written evict_last, and the row kernel discards its lines once they are read.  launch_focus2
+    // always passes 1 | 4.  It stays a run-time value: folding it into constants changes the code ptxas makes for the
+    // two kernels, and that code measured 0.5-0.6 % slower at N = 2048 (H100 SXM, 700 W)
     int hints;
     // v2 column kernel launched as a programmatic dependent of the previous field's row kernel: 1 = its input does not
     // overlap what that kernel writes, so the first tile may be gathered (and transformed) before the wait; 0 = wait first
@@ -405,12 +390,12 @@ __device__ __forceinline__ void fft_two_stages_u(P2 (&v)[16], const int t, float
     sync();
 }
 
-// Row kernel, second form: ONE 512-thread CTA per SM = four independent 128-thread line groups (named barriers, own
+// Row kernel of the v2 pipeline: ONE 512-thread CTA per SM = four independent 128-thread line groups (named barriers, own
 // exchange buffer, own row buffer and mbarrier) that share the float2 twiddle plan of the column kernel in shared memory.
-// Against three 128-thread CTAs with the float4 plan in L1 (focus_row2_kernel): 16 instead of 12 warps per SM, stage-1
-// twiddles are 64-bit shared-memory loads (lane B's twiddle = lane A's times the per-thread constant w_2L^t, four scalar
-// FP32 operations) instead of 128-bit L1 loads whose latency shows up as the kernel's top stall, and the whole unified
-// array is shared memory (no L1 working set to protect).
+// Against three 128-thread CTAs with the float4 plan in L1: 16 instead of 12 warps per SM, stage-1 twiddles are 64-bit
+// shared-memory loads (lane B's twiddle = lane A's times the per-thread constant w_2L^t, four scalar FP32 operations)
+// instead of 128-bit L1 loads whose latency shows up as the kernel's top stall, and the whole unified array is shared
+// memory (no L1 working set to protect).
 template <int L> struct GeoR4 {
     using G = Geo<L>;
     static constexpr size_t GROUP = (size_t)G::SBUF * 16 + (size_t)L * 8;       // exchange + row buffer, bytes (multiple of 128)
@@ -423,13 +408,10 @@ template <int L> struct GeoR4 {
     static constexpr size_t SMEM = CNT_OFF + NCNT * sizeof(unsigned int);
 };
 
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
-
 template <class K> int set_smem_attrs(Handle* h, K kernel, size_t smem, int ctas_per_sm) {
     if (!attr_needed(h, reinterpret_cast<const void*>(kernel))) return PB_OK;
     PB_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int pct = (int)std::min<size_t>(100, ((size_t)ctas_per_sm * (smem + 1024) * 100 + h->max_smem_optin - 1) / h->max_smem_optin);
-    if (const char* e = getenv("PB_CARVEOUT_PCT")) pct = atoi(e);
+    const int pct = (int)std::min<size_t>(100, ((size_t)ctas_per_sm * (smem + 1024) * 100 + h->max_smem_optin - 1) / h->max_smem_optin);
     PB_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
     return PB_OK;
 }

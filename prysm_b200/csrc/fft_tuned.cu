@@ -190,8 +190,8 @@ __global__ void __launch_bounds__(L / 16) focus_row_kernel(const FocusParams p) 
 //     its 4-column input tile by tensor TMA (box = 4 columns x 256 rows, 32-byte runs gathered into a contiguous
 //     [row][4] image that aliases the exchange buffers); the tile after next is requested as soon as the exchange
 //     buffers are free, so it lands while the last butterflies and the stores of the current tile run.
-//   * The row kernel gathers one intermediate row (512 runs of 32 bytes, 128 bytes apart) with two tensor-TMA boxes into
-//     the same contiguous row buffer the v1 kernel fills by a bulk copy; everything after that is the v1 code.
+//   * The row kernel (four line groups per CTA, see GeoR4) gathers each intermediate row (512 runs of 32 bytes, 128 bytes
+//     apart) with two tensor-TMA boxes into a contiguous row buffer; the arithmetic after that is the v1 row kernel's.
 //   * One field per launch pair, and plane 0 of its intermediate (the even output rows, 8 N^2 bytes = 32 MiB at N = 2048)
 //     stays in L2: the column kernel writes it evict_last, the row kernel reads it first and then discards each line
 //     (discard.global.L2), so it never reaches HBM in either direction.  Plane 1 is written evict_first and makes the trip.
@@ -321,91 +321,6 @@ __global__ void __launch_bounds__(Geo4<L>::THREADS) focus_col4_kernel(const __gr
     if (grp == 0) focus_col4_group<L, INV, 0>(in_map, p, smem4, bar);
     else focus_col4_group<L, INV, 1>(in_map, p, smem4, bar);
 }
-
-template <int L, bool INV>
-__global__ void __launch_bounds__(L / 16) focus_row2_kernel(const __grid_constant__ CUtensorMap tmp_map, const FocusParams p) {
-    using G = Geo<L>;
-    using G2 = Geo2<L>;
-    constexpr int NT = G::NT, R3 = G::R3, GI = G::GI;
-    constexpr uint32_t ROW_BYTES = L * sizeof(float2);
-    extern __shared__ __align__(128) unsigned char smraw[];
-    float4* S = reinterpret_cast<float4*>(smraw);                // SBUF exchange
-    float2* inb = reinterpret_cast<float2*>(S + G::SBUF);        // L-element input row
-    uint64_t* bar = reinterpret_cast<uint64_t*>(inb + L);        // 1 mbarrier
-    const int t = threadIdx.x;
-    int r = blockIdx.x;
-    const uint64_t pol_tmp = l2_policy((p.hints & 1) ? 1 : 0), pol_out = l2_policy((p.hints & 1) ? 1 : 0);
-    auto request_row = [&](int R) {   // one thread: gather intermediate row R = (field, plane, j) into `inb`
-        const int fb = R / (2 * L), rf = R - fb * (2 * L);
-        const int ph = rf / L, j = rf - ph * L;
-        const int grp = (fb * 2 + ph) * (L / 4) + (j >> 2);
-        mbar_expect_tx(bar, ROW_BYTES);
-#pragma unroll
-        for (int b = 0; b < G2::NBOX_ROW; ++b) tma_load_4d(inb + b * G2::BOXT * 4, &tmp_map, 0, j & 3, b * G2::BOXT, grp, bar, pol_tmp);
-    };
-    if (t == 0) {
-        mbar_init(bar, 1);
-        mbar_fence_init();
-        if (r < p.nrows) request_row(r);
-    }
-    __syncthreads();
-    const float sgn = ((t & 1) ? -1.0f : 1.0f) * p.scale;
-    for (int it = 0; r < p.nrows; ++it, r += gridDim.x) {
-        P2 v[16];
-        mbar_wait(bar, it & 1);
-        {
-            const float2* __restrict__ row = inb + t;
-#define PB_X(n) row[(n) * NT]
-            PB_MAKE_LANES_16(v, INV, PB_X)
-#undef PB_X
-        }
-        const int rn = r + gridDim.x;
-        auto sync_and_prefetch = [&]() {
-            __syncthreads();  // every thread holds its inputs in registers: the row buffer is free
-            if (t == 0 && rn < p.nrows) {
-                fence_proxy_async();
-                request_row(rn);
-            }
-        };
-        fft_two_stages<L, INV, 0>(v, t, S, p.plan + G::TW1, p.plan + G::TW2, sync_and_prefetch, SyncCta());
-        fft_last_stage_load<L, INV>(v, t, S);
-        __syncthreads();  // exchange buffer is free for the next row
-#pragma unroll
-        for (int g = 0; g < GI; ++g) dftR<R3, INV>(v + g * R3);
-        const int fb = r / (2 * L), rf = r - fb * (2 * L);   // field of the batch, row within its [2][L] planes
-        const int phs = rf / L, rr = rf - phs * L;
-        const int orow = (2 * rr + phs + L) & (2 * L - 1);  // fftshift along y
-        if (p.out_kind == PB_OUT_COMPLEX) {
-            float4* __restrict__ dst = reinterpret_cast<float4*>(reinterpret_cast<float2*>(p.out) + fb * p.out_bs + (long long)orow * p.out_ld);
-#pragma unroll
-            for (int g = 0; g < GI; ++g)
-#pragma unroll
-                for (int kk = 0; kk < R3; ++kk) {
-                    const int j = t + g * NT + 256 * kk;
-                    const P2 y = v[g * R3 + kk];
-                    const float4 o = INV ? make_float4(sgn * y.re.x, sgn * y.im.x, sgn * y.im.y, -sgn * y.re.y)
-                                         : make_float4(sgn * y.re.x, sgn * y.im.x, -sgn * y.im.y, sgn * y.re.y);
-                    st_hint(dst + ((j + L / 2) & (L - 1)), o, pol_out);
-                }
-        } else {
-            float2* __restrict__ dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + fb * p.out_bs + (long long)orow * p.out_ld);
-            const float2 s2 = make_float2(p.scale * p.scale, p.scale * p.scale);
-            const float2 wgt = make_float2(p.weight, p.weight);
-#pragma unroll
-            for (int g = 0; g < GI; ++g)
-#pragma unroll
-                for (int kk = 0; kk < R3; ++kk) {
-                    const int j = t + g * NT + 256 * kk;
-                    const P2 y = v[g * R3 + kk];
-                    float2 I = mul2(s2, fma2(y.re, y.re, mul2(y.im, y.im)));
-                    float2* q = dst + ((j + L / 2) & (L - 1));
-                    if (p.out_kind == PB_OUT_ACCUMULATE) I = fma2(wgt, I, ld_stream(q));
-                    st_hint(q, I, pol_out);
-                }
-        }
-    }
-}
-
 
 template <int L, bool INV>
 __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_constant__ CUtensorMap tmp_map, const FocusParams p) {
@@ -601,8 +516,7 @@ int launch_focus(Handle* h, FocusParams p, int batch, cudaStream_t st) {
     // re-read by every line and must hit there.  (Left to itself the driver picks the 228 KB carve-out and the plan
     // streams from L2 at ~300 cycles a load.)
     const size_t unified = 256 * 1024, l1_keep = 64 * 1024;
-    int row_ctas = std::max(1, (int)((unified - l1_keep) / (smem_row + 1024)));
-    if (const char* e = getenv("PB_ROW_CTAS_PER_SM")) row_ctas = std::max(1, atoi(e));
+    const int row_ctas = std::max(1, (int)((unified - l1_keep) / (smem_row + 1024)));
     PB_TRY(set_smem_attrs(h, focus_col_kernel<L, INV, T>, smem_col, 1));
     PB_TRY(set_smem_attrs(h, focus_row_kernel<L, INV>, smem_row, row_ctas));
     PB_TRY(get_focus_plan<L>(h, &p.plan));
@@ -613,8 +527,6 @@ int launch_focus(Handle* h, FocusParams p, int batch, cudaStream_t st) {
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
-
-}  // namespace
 
 // ---- TMA descriptors, cached in the handle by (base pointer, geometry) -----------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -644,57 +556,43 @@ int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, 
     return PB_OK;
 }
 
-namespace {
-
-
 // one field: `p.tmp` holds its [2][L][L] intermediate.  col_dep: how the column kernel follows what precedes it in the
 // stream -- 0: plain launch; 1: programmatic dependent of the previous field's row kernel; 2: the same, and its input does
 // not overlap that kernel's output (the first tile is gathered before the wait)
 template <int L, bool INV>
 int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
-    constexpr int batch = 1;
     using G = Geo<L>;
     using G2 = Geo2<L>;
     using G4 = Geo4<L>;
-    const size_t smem_col = G4::SMEM;
-    const size_t smem_row = (size_t)G::SBUF * sizeof(float4) + (size_t)L * sizeof(float2) + 2 * sizeof(uint64_t);
-    auto colk = focus_col4_kernel<L, INV>;
-    // resident CTAs per SM: rows -- as many as leave >= 64 KB of the unified L1/shared array as L1 (the 34 KB twiddle plan
-    // is re-read by every line and must hit there; left alone the driver picks the 228 KB carve-out and the plan streams
-    // from L2 at ~300 cycles a load); columns -- two 256-thread CTAs (the register file holds no more)
-    static const int row_ctas_env = env_int("PB_ROW_CTAS_PER_SM", 0);
-    const size_t unified = 256 * 1024, l1_keep = 64 * 1024;
-    const int row_ctas = row_ctas_env > 0 ? row_ctas_env : std::max(1, (int)((unified - l1_keep) / (smem_row + 1024)));
-    PB_TRY(set_smem_attrs(h, colk, smem_col, 1));
-    PB_TRY(set_smem_attrs(h, focus_row2_kernel<L, INV>, smem_row, row_ctas));
-    PB_TRY(get_focus_plan<L>(h, &p.plan));
-    const float4* plan_row = p.plan;
-    const float2* plan_col = nullptr;
-    PB_TRY(get_col4_plan<L>(h, &plan_col));
-    p.nrows = batch * 2 * L;
-    p.ntiles = batch * G2::TILES;
-    static const int hints = env_int("PB_FOCUS_L2_HINTS", 1) & 3;   // bit 0: eviction hints, bit 1: L2 prefetch of the tile after next
-    static const int row_version = env_int("PB_ROW_V", 4);
-    // plane 0 kept in L2 needs the row kernel that discards it
-    p.hints = hints | ((hints & 1) && row_version == 4 ? 4 : 0);
+    using R4 = GeoR4<L>;
+    // one CTA per SM for both kernels: the column kernel's 512 threads fill the register file, and the row kernel keeps
+    // its plan in shared memory, so it has no L1 working set to protect
+    PB_TRY(set_smem_attrs(h, focus_col4_kernel<L, INV>, G4::SMEM, 1));
+    PB_TRY(set_smem_attrs(h, focus_row4_kernel<L, INV>, R4::SMEM, 1));
+    const float2* plan = nullptr;
+    PB_TRY(get_col4_plan<L>(h, &plan));
+    p.plan = reinterpret_cast<const float4*>(plan);
+    p.nrows = 2 * L;
+    p.ntiles = G2::TILES;
+    p.hints = 1 | 4;   // eviction hints, plane 0 kept in L2 (FocusParams::hints)
     // (descriptors are copied out at once: the handle's cache may be flushed by the next lookup)
     const CUtensorMap* map = nullptr;
     CUtensorMap in_m, tmp_m;
-    {   // intermediate: [group = (field, plane, j/4)][tile][j%4][c]
-        const cuuint64_t dims[4] = {4, 4, (cuuint64_t)G2::TILES, (cuuint64_t)batch * 2 * (L / 4)};
+    {   // intermediate: [group = (plane, j/4)][tile][j%4][c]
+        const cuuint64_t dims[4] = {4, 4, (cuuint64_t)G2::TILES, (cuuint64_t)2 * (L / 4)};
         const cuuint64_t str[3] = {32, 128, (cuuint64_t)G2::TILES * 128};
         const cuuint32_t box[4] = {4, 1, (cuuint32_t)G2::BOXT, 1};
-        PB_TRY(get_map_c64(h, MapKey{p.tmp, 1, L, batch, 0, 0}, 4, dims, str, box, &map));
+        PB_TRY(get_map_c64(h, MapKey{p.tmp, 1, L, 0, 0, 0}, 4, dims, str, box, &map));
         tmp_m = *map;
     }
-    {   // input: (field, row, column) complex64; box = one 4-column run of 256 rows
-        const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)L, (cuuint64_t)batch};
-        const cuuint64_t str[2] = {(cuuint64_t)p.in_ld * 8, (cuuint64_t)(batch > 1 ? p.in_bs : (long long)L * p.in_ld) * 8};
+    {   // input: (field, row, column) complex64, one field; box = one 4-column run of 256 rows
+        const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)L, 1};
+        const cuuint64_t str[2] = {(cuuint64_t)p.in_ld * 8, (cuuint64_t)L * p.in_ld * 8};
         const cuuint32_t box[3] = {4, (cuuint32_t)G2::BOXR, 1};
-        PB_TRY(get_map_c64(h, MapKey{p.in, 2, L, batch, p.in_ld, batch > 1 ? p.in_bs : 0}, 3, dims, str, box, &map));
+        PB_TRY(get_map_c64(h, MapKey{p.in, 2, L, p.in_ld, 0, 0}, 3, dims, str, box, &map));
         in_m = *map;
     }
-    // Programmatic dependent launch (`pdl`): each kernel of the chain col(f), row(f), col(f + 1), ... is launched with
+    // Programmatic dependent launch: each kernel of the chain col(f), row(f), col(f + 1), ... is launched with
     // programmatic stream serialization, so that its CTAs take the SMs the previous kernel's last wave frees and run their
     // prologue (barriers, plan, for a column kernel with `early_input` its first gather and transform) while that wave
     // finishes; griddepcontrol.wait orders everything that depends on the previous kernel.  The column kernel of the
@@ -713,20 +611,12 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
         return cudaLaunchKernelEx(&cfg, kern, map, p);
     };
     // column pass: one CTA per SM walks the tiles of the field
-    p.plan = reinterpret_cast<const float4*>(plan_col);
-    static const bool pdl = env_int("PB_FOCUS_PDL", 1) != 0;
-    if (!pdl) col_dep = 0;
     p.early_input = col_dep == 2;
-    PB_CUDA(h, launch(colk, std::min(h->sm_count, p.ntiles), G4::THREADS, smem_col, col_dep > 0, in_m));
+    PB_CUDA(h, launch(focus_col4_kernel<L, INV>, std::min(h->sm_count, p.ntiles), G4::THREADS, G4::SMEM, col_dep > 0, in_m));
     h->launches++;
+    // row pass: four line groups per CTA, plan in shared memory
     p.early_input = 0;
-    if (row_version == 4) {   // four line groups per CTA, plan in shared memory
-        PB_TRY(set_smem_attrs(h, focus_row4_kernel<L, INV>, GeoR4<L>::SMEM, 1));
-        PB_CUDA(h, launch(focus_row4_kernel<L, INV>, std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, GeoR4<L>::SMEM, pdl, tmp_m));
-    } else {
-        p.plan = plan_row;
-        focus_row2_kernel<L, INV><<<std::min(h->sm_count * row_ctas, p.nrows), L / 16, smem_row, st>>>(tmp_m, p);
-    }
+    PB_CUDA(h, launch(focus_row4_kernel<L, INV>, std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, R4::SMEM, true, tmp_m));
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -760,8 +650,9 @@ __global__ void __launch_bounds__((COLS ? TP : 1) * L / 16, (RT && (!COLS || TP 
     const bool vin = COLS && (DENSE || ((p.batch_contiguous & 2) && hasB));
     const bool vout = COLS && (DENSE || ((p.batch_contiguous & 4) && hasB));
     if (DENSE) {
-        // L2 prefetch of the lines of the CTA that will run `pf` CTAs later (= the number of resident CTAs): its input loads
-        // then hit L2 instead of paying the DRAM latency at the head of a CTA that cannot overlap loading with computing
+        // L2 prefetch of the lines of the CTA that will run `pf` CTAs later: measured, no gain, and no launch sets pf
+        // (bits 8 and up of batch_contiguous) any more.  The block stays because without it ptxas makes different code
+        // for the DENSE kernels, and that code measured 3.7 % slower on the screened free-space chain (H100 SXM, 700 W)
         const int pf = p.batch_contiguous >> 8;
         if (pf) {
             const int nb0 = ((int)blockIdx.x + pf) * (COLS ? TP : 1) * 2;
@@ -1037,20 +928,6 @@ int launch_axis_reg(Handle* h, const AxisPass& p, cudaStream_t st) {
     PB_TRY(get_plain_plan<L>(h, &tw1, &tw2));
     const int lines_per_cta = 2 * TP;
     const int grid = (p.nb + lines_per_cta - 1) / lines_per_cta;
-    if (DENSE) {   // L2 prefetch distance = resident CTAs (PB_AXIS_PREFETCH: bit 0 row passes, bit 1 column passes)
-        static const int pf_mode = env_int("PB_AXIS_PREFETCH", 0);
-        const size_t unified = 256 * 1024, l1_keep = 64 * 1024;
-        const int regs_ctas = COLS ? 1 : 2;
-        const int ctas = std::min<int>(regs_ctas, std::max<int>(1, (int)((unified - l1_keep) / (smem + 1024))));
-        const bool on = COLS ? (pf_mode & 2) != 0 : ((pf_mode & 1) != 0 && p.ies == 1 && (!PM || p.pmi_es == 1));
-        if (on) {
-            AxisPass q = p;
-            q.batch_contiguous = (p.batch_contiguous & 255) | ((ctas * h->sm_count) << 8);
-            axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE><<<grid, TP * G::NT, smem, st>>>(q, tw1, tw2);
-            PB_LAUNCH_CHECK(h);
-            return PB_OK;
-        }
-    }
     axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE><<<grid, TP * G::NT, smem, st>>>(p, tw1, tw2);
     PB_LAUNCH_CHECK(h);
     return PB_OK;
@@ -1123,27 +1000,12 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
     if (out_kind == PB_OUT_COMPLEX ? (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 15) : (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 7))
         return PB_ERR_UNSUPPORTED;  // vector stores need aligned rows
     const int N = nx;
-    // 2 = column kernel + row kernel per field; 3 = the role-specialised single kernel of focus_fused.cu with a whole
-    // field as its unit of work (opt-in, bit-identical; its 64 MiB unit does not fit L2 at N = 2048); 4 = the same kernel
-    // skeleton with one plane of one field as the unit, so that the whole intermediate stays in L2 (opt-in,
-    // bit-identical; at N = 2048 it moves 192 instead of 224 MiB per propagation but is limited by its column side:
-    // 149 us against the pair's 128 us on a 400 W H100 without launch_focus2's programmatic dependent launch, DESIGN 4.1)
-    static const int version = env_int("PB_FOCUS_V", 2);
-    // v2 / v3 / v4 take their input tiles by tensor TMA: complex input, 16-byte aligned base and even pitches; everything
-    // else (the fused phase-screen input, odd pitches) runs the v1 kernels
+    // Inputs tensor TMA can gather (complex, 16-byte aligned base, even pitches) run the tile-major pair (v2), one field
+    // per launch pair, so that the plane 0 its column pass leaves in L2 is what its row pass reads first.  Everything else
+    // (the fused phase-screen input, odd pitches, misaligned bases) runs the v1 pair, up to 8 fields per launch pair,
+    // which evens out the tails of the two grids.
     const bool tma_ok = in_kind == PB_IN_COMPLEX && !((uintptr_t)in & 15) && !(in_ld & 1) && !(in_bs & 1);
-    if (version == 4 && tma_ok) {   // stacks: one launch, one plane of one field per unit of work (focus_fused.cu)
-        const int rc = try_focus_plane(h, N, dir, in, in_ld, in_bs, batch, out, out_kind, out_ld, out_bs, scale, weight, st);
-        if (rc != PB_ERR_UNSUPPORTED) return rc;
-    }
-    if (version == 3 && tma_ok) {   // stacks: one role-specialised kernel, column and row passes overlapped (focus_fused.cu)
-        const int rc = try_focus_fused(h, N, dir, in, in_ld, in_bs, batch, out, out_kind, out_ld, out_bs, scale, weight, st);
-        if (rc != PB_ERR_UNSUPPORTED) return rc;
-    }
-    const bool v2 = version >= 2 && tma_ok;
-    // v2: one field per launch pair, so that the plane 0 its column pass leaves in L2 is what its row pass reads first.
-    // v1: up to 8 fields per launch pair, which evens out the tails of the two grids.
-    const int per = v2 ? 1 : std::min(batch, 8);
+    const int per = tma_ok ? 1 : std::min(batch, 8);
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 0, (size_t)per * 2 * N * N * sizeof(float2), &tmp));
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
@@ -1168,7 +1030,7 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
         p.nrows = 0; p.ntiles = 0; p.hints = 0; p.early_input = 0;
         p.in_bs = in_bs; p.amp_bs = amp_bs; p.out_bs = out_bs;
         int rc;
-        if (v2) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)
+        if (tma_ok) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)
             const int cd = b0 > 0 ? col_dep_next : 0;
             if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
             else rc = N == 512 ? launch_focus2<512, true>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, true>(h, p, cd, st) : launch_focus2<2048, true>(h, p, cd, st);

@@ -1,84 +1,111 @@
-"""GPU: the plane-unit focus kernel (PB_FOCUS_V=4, csrc/focus_fused.cu) gives the same bits as the column + row kernel
-pair (PB_FOCUS_V=2).
+"""GPU: the focus pipeline at N = 2048 (column + row kernel pair of csrc/fft_tuned.cu, one pair per field) gives the same
+bits however a field reaches it.
 
-Both do the same per-column and per-row arithmetic in the same order, so the SHA-1 of every output must agree:
-N = 2048 stacks of 2, 3 and 16 fields and one of 66 (two launches: the counter arrays take 64 fields), both directions,
-complex, intensity and accumulated-intensity outputs, and an output with padded row and field strides.  In the v4
-process two repeated calls and a CUDA-graph replay (prysm_b200.graphs) give the same bits too.  The switches are read
-once per process, so each variant runs in a subprocess, under a timeout: the kernel's workers spin on each other's
-counters.
+In a call on a stack the column kernel of field 0 is a plain launch; those of fields 1, 2, ... are programmatic dependents
+of the previous field's row kernel.  They gather their first tile before the wait when the host sees that the input stack
+does not overlap the output stack (early input), and wait first when it does.  Every field of a stack must have the
+bits of the single-field call, in both directions and for complex, intensity and accumulated-intensity outputs; so must
+an output with padded strides, repeated calls, a CUDA-graph replay, and an input stack placed inside the output stack's
+allocation.
 """
-import os
-import subprocess
-import sys
+import ctypes as C
 
 import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-_SCRIPT = r'''
-import hashlib, sys
 import torch
-sys.path.insert(0, %(root)r)
-import prysm_b200 as pb
-from prysm_b200 import _ops, _capi, graphs
-pb.config.precision = 32
-n = 2048
 
-def digest(t):
-    h = hashlib.sha1()
-    flat = t.reshape(t.shape[0], -1)
-    for i in range(flat.shape[0]):      # field by field: the large case does not need a host copy of the whole stack
-        h.update(flat[i].cpu().numpy().tobytes())
-    return h.hexdigest()
+pytestmark = pytest.mark.gpu
 
-def stack(b, seed):
-    gen = torch.Generator(device='cuda').manual_seed(seed)
-    return torch.complex(torch.randn((b, n, n), generator=gen, device='cuda'), torch.randn((b, n, n), generator=gen, device='cuda'))
-
-def run(x, d, kind=_capi.OUT_COMPLEX, out=None):
-    return _ops.fft2_batch(x, (2 * n, 2 * n), dir=d, scale=1.0 / (2 * n), shift_in=True, shift_out=True, out_kind=kind, out=out)
-
-for b in (2, 3, 16):
-    x = stack(b, 100 + b)
-    for d in (-1, 1):
-        print('complex', b, d, digest(run(x, d)))
-        torch.cuda.empty_cache()
-x = stack(3, 7)
-print('intensity', digest(run(x, -1, _capi.OUT_INTENSITY)))
-gen = torch.Generator(device='cuda').manual_seed(8)
-acc = torch.rand((3, 2 * n, 2 * n), generator=gen, device='cuda')
-print('accumulate', digest(run(x, 1, _capi.OUT_ACCUMULATE, out=acc)))
-big = torch.zeros((3, 2 * n + 3, 2 * n + 6), dtype=torch.complex64, device='cuda')   # padded field and row strides
-view = big[:, 1:2 * n + 1, 2:2 * n + 2]
-run(x, -1, out=view)
-print('padded', digest(big))
-del big, view, acc
-first = digest(run(x, -1))
-print('repeat', first == digest(run(x, -1)))
-step = graphs.capture(lambda w: run(w, -1), x)
-print('graph', digest(step(x)) == first)
-step.close()
-del x, step
-torch.cuda.empty_cache()
-x = stack(66, 9)
-print('two_launches', digest(run(x, -1, _capi.OUT_INTENSITY)))
-'''
+N, B = 2048, 3
 
 
-def _run(version):
-    e = {k: v for k, v in os.environ.items() if not k.startswith('PB_')}
-    e['PB_FOCUS_V'] = version
-    r = subprocess.run([sys.executable, '-c', _SCRIPT % {'root': ROOT}], env=e, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return [line for line in r.stdout.strip().splitlines() if line.split()[0] in
-            ('complex', 'intensity', 'accumulate', 'padded', 'repeat', 'graph', 'two_launches')]
+@pytest.fixture(scope='module')
+def ops():
+    if not torch.cuda.is_available():
+        pytest.skip('needs a CUDA device')
+    from prysm_b200 import _ops
+    return _ops
 
 
-@pytest.mark.gpu
-def test_plane_kernel_is_bit_identical_to_the_kernel_pair():
-    base = _run('2')
-    plane = _run('4')
-    assert 'repeat True' in plane and 'graph True' in plane
-    assert [ln for ln in plane if ln.split()[0] not in ('repeat', 'graph')] == \
-           [ln for ln in base if ln.split()[0] not in ('repeat', 'graph')]
+@pytest.fixture(scope='module')
+def stack(ops):
+    gen = torch.Generator(device='cuda').manual_seed(7)
+    return torch.complex(torch.randn((B, N, N), generator=gen, device='cuda'), torch.randn((B, N, N), generator=gen, device='cuda'))
+
+
+def run(ops, x, d=-1, kind=None, out=None):
+    kind = ops.capi.OUT_COMPLEX if kind is None else kind
+    return ops.fft2_batch(x, (2 * N, 2 * N), dir=d, scale=1.0 / (2 * N), shift_in=True, shift_out=True, out_kind=kind, out=out)
+
+
+def launches(ops, x, fn):
+    """fn() and the number of kernels it launched on x's stream"""
+    h = ops._ctx(x)[0]
+    n0 = h.launch_count()
+    res = fn()
+    return res, h.launch_count() - n0
+
+
+@pytest.mark.parametrize('d', [-1, 1])
+def test_each_field_of_a_stack_has_the_bits_of_the_single_field_call(ops, stack, d):
+    got, n = launches(ops, stack, lambda: run(ops, stack, d))
+    assert n == 2 * B                 # one column + row kernel pair per field
+    for b in range(B):
+        assert torch.equal(got[b], run(ops, stack[b:b + 1], d)[0]), b
+
+
+def test_intensity_and_accumulate_per_field(ops, stack):
+    capi = ops.capi
+    got = run(ops, stack, -1, capi.OUT_INTENSITY)
+    for b in range(B):
+        assert torch.equal(got[b], run(ops, stack[b:b + 1], -1, capi.OUT_INTENSITY)[0]), b
+    gen = torch.Generator(device='cuda').manual_seed(8)
+    acc = torch.rand((B, 2 * N, 2 * N), generator=gen, device='cuda')
+    one = acc.clone()
+    run(ops, stack, 1, capi.OUT_ACCUMULATE, out=acc)
+    for b in range(B):
+        run(ops, stack[b:b + 1], 1, capi.OUT_ACCUMULATE, out=one[b:b + 1])
+        assert torch.equal(acc[b], one[b]), b
+
+
+def test_padded_output_strides(ops, stack):
+    big = torch.zeros((B, 2 * N + 3, 2 * N + 6), dtype=torch.complex64, device='cuda')   # padded field and row strides
+    view = big[:, 1:2 * N + 1, 2:2 * N + 2]
+    run(ops, stack, -1, out=view)
+    assert torch.equal(view, run(ops, stack, -1))
+    assert not big[:, 0].any() and not big[:, 2 * N + 1:].any() and not big[:, :, :2].any() and not big[:, :, 2 * N + 2:].any()
+
+
+def test_repeated_calls_and_graph_replay(ops, stack):
+    from prysm_b200 import graphs
+    first = run(ops, stack, -1)
+    assert torch.equal(first, run(ops, stack, -1))
+    step = graphs.capture(lambda w: run(ops, w, -1), stack)
+    try:
+        assert torch.equal(step(stack), first)
+        assert torch.equal(step(stack), first)
+    finally:
+        step.close()
+
+
+@pytest.mark.parametrize('d', [-1, 1])
+def test_input_inside_the_output_allocation(ops, stack, d):
+    """The input stack lies in the never-written padding columns of the output stack's allocation, so the host sees
+    overlapping ranges and the column kernels of fields 1, 2 wait before their first gather.  (_ops.fft2_batch copies
+    strided inputs, hence the direct C-ABI call.)"""
+    capi = ops.capi
+    buf = torch.zeros((B, 2 * N, 3 * N), dtype=torch.complex64, device='cuda')
+    out = buf[:, :, :2 * N]
+    src = buf[:, :N, 2 * N:]          # row pitch 3N (even), 16-byte-aligned base
+    src.copy_(stack)
+    h, st = ops._ctx(buf)
+
+    def call():
+        h.check(capi.lib.pb_fft2_batch(h.ptr, capi.PB_C64, C.c_void_p(src.data_ptr()), capi.IN_COMPLEX, C.c_void_p(0),
+                                       capi.AMP_NONE, 0.0, B, src.stride(0), 0, N, N, src.stride(1), 2 * N, 2 * N, d,
+                                       1.0 / (2 * N), 1, 1, C.c_void_p(out.data_ptr()), capi.OUT_COMPLEX, 1.0, 2 * N,
+                                       2 * N, out.stride(1), out.stride(0), st))
+
+    _, n = launches(ops, buf, call)
+    assert n == 2 * B
+    assert torch.equal(src, stack)    # the input was not written over
+    assert torch.equal(out, run(ops, stack, d))

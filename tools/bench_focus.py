@@ -1,15 +1,15 @@
-"""Kernel-level timing of the batched focus pipeline at the benchmark's shape, one variant per subprocess.
+"""Kernel-level timing of the batched focus pipeline at the benchmark's shape, one package tree per subprocess.
 
-    python tools/bench_focus.py [--variants SPEC ...] [--alternate N] [--intensity] [--profile DIR] [--out FILE.json]
+    python tools/bench_focus.py [--trees DIR ...] [--alternate N] [--intensity] [--profile DIR] [--out FILE.json]
 
-SPEC is `V` or `V:KEY=VAL,KEY=VAL`: PB_FOCUS_V=V plus extra environment switches, e.g. `4:PB_FOCUS_L2_SLACK_MIB=8`
-or `4:PB_FUSED_NCOL=60`.  The switches are read once per process, so every variant runs in a process of its own.
-Each run times `propagation.focus` (and, with --intensity, `propagation.focus_intensity`) on a (16, 2048, 2048)
-complex64 stack -> 4096^2 with CUDA events over a window of at least 0.5 s, and reports microseconds per
-propagation, the algorithmic bandwidth (pupil read + field written) and the HBM bytes the variant moves, counted from
-the shapes.  --alternate N runs the variant list N times in turn (A/B/A/B...), so that drifts of the card show as
-spread.  --profile DIR writes torch.profiler kernel times of one call per variant under DIR.  The card's name, power
-limit and SM clock are printed with the numbers (read-only nvidia-smi queries).
+Each DIR is the root of a built checkout (default: this one); its `prysm_b200` is imported in a process of its own, so
+that two builds, e.g. a change and its parent, can be compared in one session.  Each run times `propagation.focus`
+(and, with --intensity, `propagation.focus_intensity`) on a (16, 2048, 2048) complex64 stack -> 4096^2 with CUDA
+events over a window of at least 0.5 s, and reports microseconds per propagation, the algorithmic bandwidth (pupil read
++ field written) and the HBM bytes the pipeline moves, counted from the shapes.  --alternate N runs the tree list N
+times in turn (A/B/A/B...), so that drifts of the card show as spread.  --profile DIR writes torch.profiler kernel
+times of one call per tree under DIR.  The card's name, power limit and SM clock are printed with the numbers
+(read-only nvidia-smi queries).
 """
 import argparse
 import json
@@ -22,14 +22,9 @@ N, Q, BATCH = 2048, 2, 16
 K = N * Q
 MIB = 2 ** 20
 ALG = {'complex': 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 4 * K * K}
-# HBM bytes per propagation counted from the shapes: pupil reads, the part of the 16 N^2-byte intermediate that leaves
-# L2 (written and read back), output writes
-HBM = {
-    '1': {'complex': 8 * N * N + 2 * 16 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 16 * N * N + 4 * K * K},
-    '2': {'complex': 8 * N * N + 2 * 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 8 * N * N + 4 * K * K},
-    '3': {'complex': 8 * N * N + 2 * 16 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 16 * N * N + 4 * K * K},
-    '4': {'complex': 2 * 8 * N * N + 8 * K * K, 'intensity': 2 * 8 * N * N + 4 * K * K},
-}
+# HBM bytes per propagation counted from the shapes: pupil reads, plane 1 of the 16 N^2-byte intermediate (written and
+# read back; plane 0 stays in L2), output writes
+HBM = {'complex': 8 * N * N + 2 * 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 8 * N * N + 4 * K * K}
 
 _CHILD = r'''
 import json, sys, time
@@ -84,65 +79,51 @@ def card():
         return 'nvidia-smi unavailable'
 
 
-def parse_spec(spec):
-    v, _, rest = spec.partition(':')
-    env = {'PB_FOCUS_V': v}
-    for kv in filter(None, rest.split(',')):
-        k, _, val = kv.partition('=')
-        env[k] = val
-    return v, env
-
-
-def run_variant(spec, intensity, profile):
-    v, env = parse_spec(spec)
-    e = {k: val for k, val in os.environ.items() if not k.startswith('PB_')}
-    e.update(env)
-    src = _CHILD % {'root': ROOT, 'n': N, 'q': Q, 'b': BATCH, 'intensity': intensity, 'profile': bool(profile)}
-    r = subprocess.run([sys.executable, '-c', src], env=e, capture_output=True, text=True, timeout=900)
+def run_tree(root, intensity, profile):
+    src = _CHILD % {'root': root, 'n': N, 'q': Q, 'b': BATCH, 'intensity': intensity, 'profile': bool(profile)}
+    r = subprocess.run([sys.executable, '-c', src], capture_output=True, text=True, timeout=900)
     if r.returncode != 0:
-        raise RuntimeError(f'{spec}: exit {r.returncode}\n{r.stderr[-3000:]}')
+        raise RuntimeError(f'{root}: exit {r.returncode}\n{r.stderr[-3000:]}')
     res = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith('RESULT ')][-1][7:])
     for kind, row in res.items():
         us = row['us_per_prop']
         row['alg_gbs'] = ALG[kind] / (us * 1e-6) / 1e9
-        hbm = HBM.get(v, {}).get(kind)
-        row['hbm_mib_counted'] = hbm / MIB if hbm else None
-        row['hbm_gbs_counted'] = hbm / (us * 1e-6) / 1e9 if hbm else None
+        row['hbm_mib_counted'] = HBM[kind] / MIB
+        row['hbm_gbs_counted'] = HBM[kind] / (us * 1e-6) / 1e9
     return res
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--variants', nargs='+', default=['2', '3', '4'])
-    ap.add_argument('--alternate', type=int, default=1, metavar='N', help='run the variant list N times in turn')
+    ap.add_argument('--trees', nargs='+', default=[ROOT], metavar='DIR', help='roots of built checkouts to time')
+    ap.add_argument('--alternate', type=int, default=1, metavar='N', help='run the tree list N times in turn')
     ap.add_argument('--intensity', action='store_true', help='time focus_intensity (the fused PSF variant) too')
     ap.add_argument('--profile', default=None, metavar='DIR', help='write torch.profiler kernel times under DIR')
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
+    trees = [os.path.abspath(t) for t in args.trees]
     print('card (name, power limit, SM clock, max SM clock):', card(), flush=True)
     runs = []
     for rnd in range(args.alternate):
-        for spec in args.variants:
-            res = run_variant(spec, args.intensity, args.profile)
-            runs.append({'round': rnd, 'variant': spec, **res})
-            line = f'[{rnd}] {spec:32s}'
+        for i, tree in enumerate(trees):
+            res = run_tree(tree, args.intensity, args.profile)
+            runs.append({'round': rnd, 'tree': tree, **res})
+            line = f'[{rnd}] {tree:32s}'
             for kind, row in res.items():
-                hbm = f'{row["hbm_mib_counted"]:.0f} MiB' if row['hbm_mib_counted'] else 'n/a'
                 line += (f'  {kind}: {row["us_per_prop"]:7.1f} us/prop  {row["alg_gbs"]:6.0f} GB/s alg  '
-                         f'HBM {hbm}  {row["launches_per_call"]:.0f} launches/call')
+                         f'HBM {row["hbm_mib_counted"]:.0f} MiB  {row["launches_per_call"]:.0f} launches/call')
             print(line, flush=True)
             if args.profile:
                 os.makedirs(args.profile, exist_ok=True)
-                name = spec.replace(':', '_').replace(',', '_').replace('=', '-')
-                with open(os.path.join(args.profile, f'kernels_{name}_{rnd}.json'), 'w') as fh:
-                    json.dump(res, fh, indent=1)
+                with open(os.path.join(args.profile, f'kernels_tree{i}_{rnd}.json'), 'w') as fh:
+                    json.dump({'tree': tree, **res}, fh, indent=1)
     print('card after:', card(), flush=True)
     summary = {}
-    for spec in args.variants:
+    for tree in trees:
         for kind in ('complex', 'intensity'):
-            xs = [r[kind]['us_per_prop'] for r in runs if r['variant'] == spec and kind in r]
+            xs = [r[kind]['us_per_prop'] for r in runs if r['tree'] == tree and kind in r]
             if xs:
-                summary[f'{spec} {kind}'] = {'min': min(xs), 'max': max(xs), 'spread_pct': 100 * (max(xs) - min(xs)) / min(xs)}
+                summary[f'{tree} {kind}'] = {'min': min(xs), 'max': max(xs), 'spread_pct': 100 * (max(xs) - min(xs)) / min(xs)}
     for k, s in summary.items():
         print(f'{k:44s} min {s["min"]:7.1f}  max {s["max"]:7.1f} us/prop  spread {s["spread_pct"]:.1f} %')
     if args.out:
