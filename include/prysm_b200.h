@@ -435,6 +435,40 @@ int pb_segment_compose_adjoint(pb_handle_t h, int dtype, int ny, int nx, int nse
                                const void* masks, const void* bases, int nmodes, const void* opdbar, int nchunk,
                                double* partial, void* out, void* stream);
 
+/* ---- Jones calculus (prysm/x/polarization.py) ----------------------------------------------------------------------
+ * Element-planar layout: a Jones array of n pixels is 4 contiguous planes of n complex samples at dtype, plane 2*i + j
+ * holding J[..., i, j]; Mueller and Kronecker arrays are 16 planes, plane 4*r + c (Mueller planes are real).
+ * pb_jones_planar: src is a (rows, cols, 2, 2) array of src_type with strides s_row, s_col, s_i, s_j counted in
+ *   elements of src_type (one complex value is one element); out = its 4 planes (n = rows*cols), converted to dtype.
+ * pb_jones_product: out = op_a(A) * op_b(B) per pixel, the 2x2 matrix product (PB_JONES_MATMUL) or the elementwise
+ *   product (PB_JONES_HADAMARD).  An operand is a constant 2x2 (PB_JONES_CONST: four complex values from consts_host,
+ *   A's at [0, 8), B's at [8, 16)), 4 planes (PB_JONES_PLANES) or one complex / real plane broadcast to all four
+ *   elements (PB_JONES_SCALAR / PB_JONES_SCALAR_REAL); op is PB_JONES_OP_N or PB_JONES_OP_H (conjugate transpose).
+ *   out may be one of the operands.
+ * pb_jones_elements: out = 4 planes of one constructor, phases evaluated in fp64.  params_host (host fp64):
+ *   PB_JONES_FILL: 4 complex values (8 doubles);  PB_JONES_ROTATION: theta, scale (with a plane, theta = plane*scale);
+ *   PB_JONES_RETARDER / PB_JONES_DIATTENUATOR: theta, retardance / alpha (a plane replaces the second);
+ *   PB_JONES_VVR: charge, retardance, rotate, with the azimuth plane (required; it is not modified).
+ *   plane: optional, n real values of plane_type PB_JONES_SRC_F32 or PB_JONES_SRC_F64.
+ * pb_jones_reduce: PB_JONES_MUELLER: out = 16 real planes of real(U kron(conj a, a) U^-1);  PB_JONES_KRON: out = 16
+ *   complex planes of kron(a, b);  PB_JONES_PAULI: out = 4 complex planes c0..c3. */
+typedef enum { PB_JONES_SRC_F32 = 0, PB_JONES_SRC_F64 = 1, PB_JONES_SRC_C64 = 2, PB_JONES_SRC_C128 = 3 } pb_jones_src;
+typedef enum { PB_JONES_CONST = 0, PB_JONES_PLANES = 1, PB_JONES_SCALAR = 2, PB_JONES_SCALAR_REAL = 3 } pb_jones_operand;
+typedef enum { PB_JONES_MATMUL = 0, PB_JONES_HADAMARD = 1 } pb_jones_mode;
+typedef enum { PB_JONES_OP_N = 0, PB_JONES_OP_H = 1 } pb_jones_op;
+typedef enum {
+    PB_JONES_FILL = 0, PB_JONES_ROTATION = 1, PB_JONES_RETARDER = 2, PB_JONES_DIATTENUATOR = 3, PB_JONES_VVR = 4
+} pb_jones_element;
+typedef enum { PB_JONES_MUELLER = 0, PB_JONES_KRON = 1, PB_JONES_PAULI = 2 } pb_jones_reduction;
+int pb_jones_planar(pb_handle_t h, int dtype, const void* src, int src_type, long long rows, long long cols,
+                    long long s_row, long long s_col, long long s_i, long long s_j, void* out, void* stream);
+int pb_jones_product(pb_handle_t h, int dtype, int mode, long long n, int a_kind, const void* a, int a_op, int b_kind,
+                     const void* b, int b_op, const double* consts_host, void* out, void* stream);
+int pb_jones_elements(pb_handle_t h, int dtype, int kind, long long n, const void* plane, int plane_type,
+                      const double* params_host, int nparams, void* out, void* stream);
+int pb_jones_reduce(pb_handle_t h, int dtype, int kind, long long n, const void* a, const void* b, void* out,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

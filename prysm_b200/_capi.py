@@ -87,11 +87,21 @@ SIGNATURES = {
     'pb_hex_segments': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _d, _vp, _vp, _vp, _vp, _vp]),
     'pb_segment_compose': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _ll, _i, _vp, _vp]),
     'pb_segment_compose_adjoint': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    'pb_jones_planar': (_i, [_vp, _i, _vp, _i, _ll, _ll, _ll, _ll, _ll, _ll, _vp, _vp]),
+    'pb_jones_product': (_i, [_vp, _i, _i, _ll, _i, _vp, _i, _i, _vp, _i, C.POINTER(_d), _vp, _vp]),
+    'pb_jones_elements': (_i, [_vp, _i, _i, _ll, _vp, _i, C.POINTER(_d), _i, _vp, _vp]),
+    'pb_jones_reduce': (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
 SDF_UNION, SDF_INTERSECT, SDF_SUBTRACT = range(3)
 SEGMENT_FIELDS, SEGMENT_TILE_Y, SEGMENT_TILE_X, SEGMENT_CHUNK = 6, 32, 64, 2048
+JONES_SRC_F32, JONES_SRC_F64, JONES_SRC_C64, JONES_SRC_C128 = range(4)
+JONES_CONST, JONES_PLANES, JONES_SCALAR, JONES_SCALAR_REAL = range(4)
+JONES_MATMUL, JONES_HADAMARD = range(2)
+JONES_OP_N, JONES_OP_H = range(2)
+JONES_FILL, JONES_ROTATION, JONES_RETARDER, JONES_DIATTENUATOR, JONES_VVR = range(5)
+JONES_MUELLER, JONES_KRON, JONES_PAULI = range(3)
 
 
 def load_library(path=LIB_PATH):

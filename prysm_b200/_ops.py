@@ -92,6 +92,17 @@ def _check_out(out, shape, dtype, device, name='out'):
     return out
 
 
+def _contiguous_out(out, shape, like):
+    """A new (shape) array of like's dtype, or the caller's `out` checked to be exactly that and contiguous (the
+    kernels that take it write a dense array)."""
+    if out is None:
+        return torch.empty(shape, dtype=like.dtype, device=like.device)
+    _check_out(out, shape, like.dtype, like.device)
+    if not out.is_contiguous():
+        raise ValueError('`out` must be contiguous')
+    return out
+
+
 def _darr(v):
     v = np.ascontiguousarray(v, dtype=np.float64)
     return v, v.ctypes.data_as(C.POINTER(C.c_double))
@@ -139,9 +150,10 @@ def fft2(field, k=None, *, dir=-1, scale=1.0, shift_in=False, shift_out=False, c
 
 
 def fft2_batch(fields, k=None, *, dir=-1, scale=1.0, shift_in=False, shift_out=False, out_kind=capi.OUT_COMPLEX, out=None,
-               amp=None, opd=None, kscale=0.0):
+               amp=None, opd=None, kscale=0.0, crop=None):
     """pb_fft2_batch over a (B, ny, nx) stack -> (B, ky, kx): either `fields` (complex or real) or `opd` (B, ny, nx)
-    with an optional amplitude that is (ny, nx) (shared) or (B, ny, nx)."""
+    with an optional amplitude that is (ny, nx) (shared) or (B, ny, nx).  `crop` = (oy, ox) keeps the centred
+    window of each transform, as fft2's does (the adjoints of focus / unfocus)."""
     amp_kind, amp_t, amp_bs = capi.AMP_NONE, None, 0
     if opd is not None:
         src = opd if opd.dtype in _CPLX_OF else opd.to(torch.float32)
@@ -163,17 +175,18 @@ def fft2_batch(fields, k=None, *, dir=-1, scale=1.0, shift_in=False, shift_out=F
     src = src.contiguous()
     nb, ny, nx = src.shape
     ky, kx = (ny, nx) if k is None else k
+    oy, ox = (ky, kx) if crop is None else crop
     odt = cdtype if out_kind == capi.OUT_COMPLEX else _REAL_OF[cdtype]
     if out is None:
-        out = torch.empty((nb, ky, kx), dtype=odt, device=src.device)
+        out = torch.empty((nb, oy, ox), dtype=odt, device=src.device)
     else:
-        _check_out(out, (nb, ky, kx), odt, src.device)
-        if out.stride(1) < kx or (nb > 1 and out.stride(0) < (ky - 1) * out.stride(1) + kx):
+        _check_out(out, (nb, oy, ox), odt, src.device)
+        if out.stride(1) < ox or (nb > 1 and out.stride(0) < (oy - 1) * out.stride(1) + ox):
             raise ValueError('`out` rows / fields overlap')
     h, st = _ctx(src)
     h.check(lib.pb_fft2_batch(h.ptr, _CODE[cdtype], _p(src), in_kind, _p(amp_t), amp_kind, float(kscale), nb,
                               src.stride(0), amp_bs, ny, nx, src.stride(1), ky, kx, int(dir), float(scale), int(shift_in),
-                              int(shift_out), _p(out), out_kind, 1.0, ky, kx, out.stride(1), out.stride(0), st))
+                              int(shift_out), _p(out), out_kind, 1.0, oy, ox, out.stride(1), out.stride(0), st))
     return out
 
 
@@ -193,15 +206,15 @@ def fft1(a, n=None, axis=-1, dir=-1, scale=1.0):
 
 
 def axis_dft(a, n, axis, dir=-1, scale=1.0, pre_e=None, pre_e_conj=False, pre_b=None, pre_b_conj=False,
-             post_e=None, post_e_conj=False, post_b=None, post_b_conj=False, out_off=0, n_out=None):
-    """pb_axis_dft: one DFT pass with fused multipliers and an output window."""
+             post_e=None, post_e_conj=False, post_b=None, post_b_conj=False, out_off=0, n_out=None, out=None):
+    """pb_axis_dft: one DFT pass with fused multipliers and an output window; `out`: a contiguous array to write."""
     a = ascomplex(a).contiguous()
     ny, nx = a.shape
     axis = axis % 2
     if n_out is None:
         n_out = n - out_off
     oshape = (n_out, nx) if axis == 0 else (ny, n_out)
-    out = torch.empty(oshape, dtype=a.dtype, device=a.device)
+    out = _contiguous_out(out, oshape, a)
     h, st = _ctx(a)
     h.check(lib.pb_axis_dft(h.ptr, _CODE[a.dtype], _p(a), ny, nx, nx, axis, int(n), int(dir), float(scale),
                             _p(pre_e), int(pre_e_conj), _p(pre_b), int(pre_b_conj),
@@ -281,20 +294,21 @@ def czt_axis(a, K, axis, pre_e, H, post_e, out_off, n_out, scale=1.0, pre_conj=F
                                           int(pre_conj), _p(H), _p(post_e), int(post_conj), int(out_off), int(n_out),
                                           float(scale), int(out_kind), float(weight), _p(out), out.stride(0), st))
         return out
-    out = torch.empty(oshape, dtype=a.dtype, device=a.device)
+    out = _contiguous_out(out, oshape, a)
     h.check(lib.pb_czt_axis(h.ptr, _CODE[a.dtype], _p(a), ny, nx, a.stride(0), axis, int(K), _p(pre_e), int(pre_conj), _p(H),
                             _p(post_e), int(post_conj), int(out_off), int(n_out), float(scale), _p(out), oshape[1], st))
     return out
 
 
-def angular_spectrum(field, k, ty=None, tx=None, tf=None, conj_tf=False, crop=None, screen=None, conj_screen=False):
+def angular_spectrum(field, k, ty=None, tx=None, tf=None, conj_tf=False, crop=None, screen=None, conj_screen=False,
+                     out=None):
     """pb_angular_spectrum; with `screen` (complex, same shape as the field) pb_angular_spectrum_screen: the field is
-    multiplied by the screen inside the first transform pass."""
+    multiplied by the screen inside the first transform pass.  `out`: a contiguous array to write."""
     field = ascomplex(field).contiguous()
     ny, nx = field.shape
     ky, kx = k
     oy, ox = (ky, kx) if crop is None else crop
-    out = torch.empty((oy, ox), dtype=field.dtype, device=field.device)
+    out = _contiguous_out(out, (oy, ox), field)
     if tf is not None:
         tf = tf.to(field.dtype).contiguous()
     h, st = _ctx(field)
@@ -366,7 +380,7 @@ def cgemm(A, B, opA=capi.OP_N, opB=capi.OP_N, alpha=1.0):
     return out
 
 
-def mdft_apply(Ey, Ex, a, norm, adjoint, left_first):
+def mdft_apply(Ey, Ex, a, norm, adjoint, left_first, out=None):
     my, ny = Ey.shape
     mx, nx = Ex.shape
     a = a.contiguous()
@@ -374,7 +388,7 @@ def mdft_apply(Ey, Ex, a, norm, adjoint, left_first):
     if tuple(a.shape) != want:
         raise ValueError(f'array of shape {tuple(a.shape)} does not match the executor ({want})')
     oshape = (ny, nx) if adjoint else (my, mx)
-    out = torch.empty(oshape, dtype=a.dtype, device=a.device)
+    out = _contiguous_out(out, oshape, a)
     nwork = lib.pb_mdft_work_elems(my, ny, mx, nx, int(adjoint), int(left_first))
     work = torch.empty(nwork, dtype=a.dtype, device=a.device)
     h, st = _ctx(a)
@@ -397,13 +411,13 @@ def mdft_tc_expand(E):
     return hi, lo
 
 
-def mdft_tc_apply(ex_hi, ex_lo, ey_hi, ey_lo, a, norm):
+def mdft_tc_apply(ex_hi, ex_lo, ey_hi, ey_lo, a, norm, out=None):
     my, ny = ey_hi.shape[0] // 2, ey_hi.shape[1] // 2
     mx, nx = ex_hi.shape[0] // 2, ex_hi.shape[1] // 2
     a = a.contiguous()
     if tuple(a.shape) != (ny, nx):
         raise ValueError(f'array of shape {tuple(a.shape)} does not match the executor ({(ny, nx)})')
-    out = torch.empty((my, mx), dtype=torch.complex64, device=a.device)
+    out = _contiguous_out(out, (my, mx), a)
     work = torch.empty(lib.pb_mdft_tc_work_bytes(my, ny, mx, nx), dtype=torch.uint8, device=a.device)
     h, st = _ctx(a)
     h.check(lib.pb_mdft_tc_apply(h.ptr, _p(ex_hi), _p(ex_lo), _p(ey_hi), _p(ey_lo), my, ny, mx, nx, _p(a), _p(out),
@@ -975,6 +989,49 @@ def segment_compose_adjoint(seg, nseg, masks, bases, nmodes, opdbar, max_window)
     h, st = _ctx(opdbar)
     h.check(lib.pb_segment_compose_adjoint(h.ptr, _CODE[opdbar.dtype], ny, nx, int(nseg), _p(seg), _p(masks), _p(bases),
                                            int(nmodes), _p(opdbar), nchunk, _p(partial), _p(out), st))
+    return out
+
+
+_JONES_SRC = {torch.float32: capi.JONES_SRC_F32, torch.float64: capi.JONES_SRC_F64,
+              torch.complex64: capi.JONES_SRC_C64, torch.complex128: capi.JONES_SRC_C128}
+
+
+def jones_planar(src, cdtype, out=None):
+    """A (rows, cols, 2, 2) device tensor of any strides, real or complex -> its 4 element planes (4, rows, cols) at
+    `cdtype` (pb_jones_planar)."""
+    rows, cols = src.shape[:2]
+    if out is None:
+        out = torch.empty((4, rows, cols), dtype=cdtype, device=src.device)
+    h, st = _ctx(src)
+    h.check(lib.pb_jones_planar(h.ptr, _CODE[cdtype], _p(src), _JONES_SRC[src.dtype], rows, cols, *src.stride(), _p(out), st))
+    return out
+
+
+def jones_product(mode, n, a, b, out, consts=None):
+    """out = op(A) (x) op(B) over n pixels (pb_jones_product); a / b = (kind, tensor or None, op), consts = 4 + 4
+    complex values of the constant operands."""
+    (ak, at, ao), (bk, bt, bo) = a, b
+    c = np.zeros(16) if consts is None else np.asarray(consts, dtype=np.complex128).view(np.float64)
+    c, cp = _darr(c)
+    h, st = _ctx(out)
+    h.check(lib.pb_jones_product(h.ptr, _CODE[out.dtype], int(mode), int(n), int(ak), _p(at), int(ao), int(bk), _p(bt),
+                                 int(bo), cp, _p(out), st))
+    return out
+
+
+def jones_elements(kind, n, params, out, plane=None):
+    """4 planes of one Jones constructor over n pixels (pb_jones_elements); plane: optional real device tensor."""
+    p, pp = _darr(np.asarray(params, dtype=np.float64).reshape(-1))
+    ptype = _JONES_SRC[plane.dtype] if plane is not None else 0
+    h, st = _ctx(out)
+    h.check(lib.pb_jones_elements(h.ptr, _CODE[out.dtype], int(kind), int(n), _p(plane), ptype, pp, len(p), _p(out), st))
+    return out
+
+
+def jones_reduce(kind, n, a, out, b=None):
+    """Mueller (16 real planes), Kronecker (16 complex planes) or Pauli (4 planes) of 4-plane operands (pb_jones_reduce)."""
+    h, st = _ctx(a)
+    h.check(lib.pb_jones_reduce(h.ptr, _CODE[a.dtype], int(kind), int(n), _p(a), _p(b), _p(out), st))
     return out
 
 

@@ -116,16 +116,30 @@ class MDFT:
                             + _ops.mdft_tc_expand(_ops.mdft_basis(y, fy, -sign, cd, dev)))
 
     def __call__(self, ary):
-        ary = _prep(ary, self.Ey.dtype)
-        if self._tc is not None:
-            return _ops.mdft_tc_apply(*self._tc, ary, self.norm)
-        return _ops.mdft_apply(self.Ey, self.Ex, ary, self.norm, False, self._forward_left_first)
+        return self._forward(ary)
 
     def adjoint(self, grad):
+        return self._adjoint(grad)
+
+    # _forward / _adjoint write into a given contiguous `out` (one plane of a stack, prysm_b200.polarization)
+    def _forward(self, ary, out=None):
+        ary = _prep(ary, self.Ey.dtype)
+        if self._tc is not None:
+            return _ops.mdft_tc_apply(*self._tc, ary, self.norm, out=out)
+        return _ops.mdft_apply(self.Ey, self.Ex, ary, self.norm, False, self._forward_left_first, out=out)
+
+    def _adjoint(self, grad, out=None):
         grad = _prep(grad, self.Ey.dtype)
         if self._tc_adj is not None:
-            return _ops.mdft_tc_apply(*self._tc_adj, grad, self.norm)
-        return _ops.mdft_apply(self.Ey, self.Ex, grad, self.norm, True, self._adjoint_left_first)
+            return _ops.mdft_tc_apply(*self._tc_adj, grad, self.norm, out=out)
+        return _ops.mdft_apply(self.Ey, self.Ex, grad, self.norm, True, self._adjoint_left_first, out=out)
+
+    def _out_shape(self, adjoint):
+        return (self.Ey.shape[1], self.Ex.shape[1]) if adjoint else (self.Ey.shape[0], self.Ex.shape[0])
+
+    @property
+    def _dtype(self):
+        return self.Ey.dtype
 
     def nbytes(self):
         return self.Ex.numel() * self.Ex.element_size() + self.Ey.numel() * self.Ey.element_size()
@@ -220,29 +234,46 @@ class CZT:
         y_first_cost = Nx * Ky * math.log2(Ky) * len(self._ay) + My * Kx * math.log2(Kx) * len(self._ax)
         self._x_first = x_first_cost <= y_first_cost
 
-    def _forward_axis(self, o, axis, parts, M, scale):
+    def _forward_axis(self, o, axis, parts, M, scale, out=None):
         # ONE fused call per part: chirp -> FFT_K -> kernel spectrum -> IFFT_K -> slice -> chirp*phase.
         # (the row chirp by[y] of the reference's `out *= brow` commutes with the x pass: it is the y pass's pre_e)
         acc = None
         for start, n, K, b, post, H, _ in parts:
             piece = o[:, start:start + n] if axis == 1 else o[start:start + n]
-            r = _ops.czt_axis(piece, K, axis, b, H, post, n - 1, M, scale)
+            r = _ops.czt_axis(piece, K, axis, b, H, post, n - 1, M, scale, out=out if len(parts) == 1 else None)
             acc = r if acc is None else _ops.binary('add', acc, r)
-        return acc
+        if out is not None and acc is not out:     # a split axis adds its halves into a new array
+            out.copy_(acc)
+        return acc if out is None else out
 
-    def _adjoint_axis(self, o, axis, parts, scale):
+    def _adjoint_axis(self, o, axis, parts, scale, out=None):
         # conj(post) -> FFT_K -> conj(H) with the embedding offset folded in -> IFFT_K -> [:n] -> conj(chirp), per part
+        if out is not None and len(parts) == 1:
+            _, n, K, b, post, _, Hadj = parts[0]
+            return _ops.czt_axis(o, K, axis, post, Hadj, b, 0, n, scale, pre_conj=True, post_conj=True, out=out)
         outs = [_ops.czt_axis(o, K, axis, post, Hadj, b, 0, n, scale, pre_conj=True, post_conj=True)
                 for _, n, K, b, post, _, Hadj in parts]
+        if out is not None:
+            return torch.cat(outs, dim=axis, out=out)
         return outs[0] if len(outs) == 1 else torch.cat(outs, dim=axis)
 
     def __call__(self, ary):
+        return self._forward(ary)
+
+    def _forward(self, ary, out=None):
         o = _prep(ary, self._bx.dtype)
         if tuple(o.shape) != (self._Ny, self._Nx):
             raise ValueError(f'array of shape {tuple(o.shape)} does not match the executor')
         if self._x_first:
-            return self._forward_axis(self._forward_axis(o, 1, self._ax, self._Mx, 1.0), 0, self._ay, self._My, self.norm)
-        return self._forward_axis(self._forward_axis(o, 0, self._ay, self._My, 1.0), 1, self._ax, self._Mx, self.norm)
+            return self._forward_axis(self._forward_axis(o, 1, self._ax, self._Mx, 1.0), 0, self._ay, self._My, self.norm, out)
+        return self._forward_axis(self._forward_axis(o, 0, self._ay, self._My, 1.0), 1, self._ax, self._Mx, self.norm, out)
+
+    def _out_shape(self, adjoint):
+        return (self._Ny, self._Nx) if adjoint else (self._My, self._Mx)
+
+    @property
+    def _dtype(self):
+        return self._bx.dtype
 
     def intensity(self, ary, weight=1.0, out=None):
         """|self(ary)|^2, written to a new real array or, with `out`, accumulated as out += weight * |.|^2: the modulus
@@ -261,12 +292,15 @@ class CZT:
         return _ops.czt_axis(mid, K, last[0], b, H, post, n - 1, last[2], self.norm, out_kind=kind, weight=weight, out=out)
 
     def adjoint(self, grad):
+        return self._adjoint(grad)
+
+    def _adjoint(self, grad, out=None):
         o = _prep(grad, self._bx.dtype)
         if tuple(o.shape) != (self._My, self._Mx):
             raise ValueError(f'array of shape {tuple(o.shape)} does not match the executor')
         if self._x_first:  # undo y then x
-            return self._adjoint_axis(self._adjoint_axis(o, 0, self._ay, 1.0), 1, self._ax, self.norm)
-        return self._adjoint_axis(self._adjoint_axis(o, 1, self._ax, 1.0), 0, self._ay, self.norm)
+            return self._adjoint_axis(self._adjoint_axis(o, 0, self._ay, 1.0), 1, self._ax, self.norm, out)
+        return self._adjoint_axis(self._adjoint_axis(o, 1, self._ax, 1.0), 0, self._ay, self.norm, out)
 
     def nbytes(self):
         vs = {id(v): v for part in self._ax + self._ay for v in part[3:]}
@@ -328,20 +362,35 @@ class FFTDFT:
         self._x_first = x_first_cost <= y_first_cost
 
     def __call__(self, ary):
+        return self._forward(ary)
+
+    def adjoint(self, grad):
+        return self._adjoint(grad)
+
+    def _out_shape(self, adjoint):
+        return (self._Ny, self._Nx) if adjoint else (self._My, self._Mx)
+
+    @property
+    def _dtype(self):
+        return self._pre_x.dtype
+
+    def _forward(self, ary, out=None):
         o = _prep(ary, self._pre_x.dtype)
         if tuple(o.shape) != (self._Ny, self._Nx):
             raise ValueError(f'array of shape {tuple(o.shape)} does not match the executor')
         if self._x_first:
             o = _ops.axis_dft(o, self._Kx, 1, self._x_direction, pre_e=self._pre_x, pre_b=self._pre_y,
                               n_out=self._Mx, post_e=self._post_x)
-            o = _ops.axis_dft(o, self._Ky, 0, self._y_direction, n_out=self._My, post_e=self._post_y, scale=self.norm)
+            o = _ops.axis_dft(o, self._Ky, 0, self._y_direction, n_out=self._My, post_e=self._post_y, scale=self.norm,
+                              out=out)
         else:
             o = _ops.axis_dft(o, self._Ky, 0, self._y_direction, pre_e=self._pre_y, pre_b=self._pre_x,
                               n_out=self._My, post_e=self._post_y)
-            o = _ops.axis_dft(o, self._Kx, 1, self._x_direction, n_out=self._Mx, post_e=self._post_x, scale=self.norm)
+            o = _ops.axis_dft(o, self._Kx, 1, self._x_direction, n_out=self._Mx, post_e=self._post_x, scale=self.norm,
+                              out=out)
         return o
 
-    def adjoint(self, grad):
+    def _adjoint(self, grad, out=None):
         o = _prep(grad, self._pre_x.dtype)
         if tuple(o.shape) != (self._My, self._Mx):
             raise ValueError(f'array of shape {tuple(o.shape)} does not match the executor')
@@ -349,12 +398,12 @@ class FFTDFT:
             o = _ops.axis_dft(o, self._Ky, 0, -self._y_direction, pre_e=self._post_y, pre_e_conj=True,
                               pre_b=self._post_x, pre_b_conj=True, n_out=self._Ny, post_e=self._pre_y, post_e_conj=True)
             o = _ops.axis_dft(o, self._Kx, 1, -self._x_direction, n_out=self._Nx, post_e=self._pre_x, post_e_conj=True,
-                              scale=self.norm)
+                              scale=self.norm, out=out)
         else:
             o = _ops.axis_dft(o, self._Kx, 1, -self._x_direction, pre_e=self._post_x, pre_e_conj=True,
                               pre_b=self._post_y, pre_b_conj=True, n_out=self._Nx, post_e=self._pre_x, post_e_conj=True)
             o = _ops.axis_dft(o, self._Ky, 0, -self._y_direction, n_out=self._Ny, post_e=self._pre_y, post_e_conj=True,
-                              scale=self.norm)
+                              scale=self.norm, out=out)
         return o
 
     def nbytes(self):

@@ -24,6 +24,7 @@ from . import coordinates as _coords
 from . import dm as _dm
 from . import fttools as _ft
 from . import otf as _otf
+from . import polarization as _pol
 from . import polynomials as _poly
 from . import propagation as _prop
 from . import psf as _psf
@@ -66,6 +67,11 @@ _TARGETS = {
                                   'sum_of_2d_modes_adjoint': _poly.sum_of_2d_modes_adjoint},
     'prysm.coordinates': {'warp': _coords.warp},
     'prysm.x.dm': {'DM': _dm.DM},
+    # the reference's own add_jones_propagation() then wraps the engine's functions with the engine's adapter; the
+    # small 2x2 constructors stay the reference's
+    'prysm.x.polarization': {n: getattr(_pol, n) for n in (
+        'jones_adapter', 'apply_polarization_optic', 'vector_vortex_retarder', 'jones_to_mueller', 'broadcast_kron',
+        'pauli_coefficients')},
 }
 
 _saved = {}  # (module name, attribute) -> original
