@@ -469,6 +469,47 @@ int pb_jones_elements(pb_handle_t h, int dtype, int kind, long long n, const voi
 int pb_jones_reduce(pb_handle_t h, int dtype, int kind, long long n, const void* a, const void* b, void* out,
                     void* stream);
 
+/* ---- wavefront sensing (prysm/x/fibers.py, sri.py, pdi.py, psi.py) ---------------------------------------------------
+ * pb_lp_modes: out = nmodes packed real fields (nmodes, n) of dtype's real type from the radius r and angle t grids
+ *   (n values each; t may be NULL when no mode has an azimuth factor).  plan_host holds 6 doubles per mode:
+ *   l, ld, U, W, rule, az.  rho = r / a and the core is r <= a (PB_LP_RULE_LP, compute_LP_modes) or rho = r * (1/a)
+ *   and the core is rho < 1 (PB_LP_RULE_SMF, smf_mode_field).  Core: J_l(U rho) / J_ld(U); cladding:
+ *   K_l(W rho) / K_ld(W), evaluated exponentially scaled; times cos(l t) (PB_LP_COS) or sin(l t) (PB_LP_SIN).
+ * pb_overlap: for each of nmodes modes M_p (real or complex at dtype; packed (nmodes, n) in `modes`, or the host
+ *   array mode_ptrs_host of nmodes device pointers when `modes` is NULL) and the complex field E (n values):
+ *   eta[p] = |sum conj(M_p) E|^2 / (I_p I_E), I_p = sum |M_p|^2 (or ip_dev[p], fp64 on the device), I_E = sum |E|^2
+ *   (or ie_dev[0]).  partial: fp64 device workspace of nchunk * (3 nmodes + 1) values, nchunk =
+ *   ceil(n / PB_OVERLAP_CHUNK).  c_out (optional): sqrt(I_E eta[0]).  eta and c_out are dtype's real type.
+ *   Deterministic: per-chunk partials summed in a fixed order.
+ * pb_wfs_combine: out = alpha a + beta b (complex) or |alpha a + beta b|^2 (real_out: real).  coefs_host = re, im of
+ *   alpha then of beta; each is multiplied by the device real scalar alpha_scale / beta_scale when given.  b may be
+ *   NULL.
+ * pb_grating: g = the grating of kind at x + shift (x real at dtype, the arithmetic in fp64); out = E g (complex), or
+ *   g itself (real) when E is NULL.  PB_GRATING_SIN_AMP params: prefix (g = 1 - (sin(prefix x) + 1) / 2 * 0.1);
+ *   PB_GRATING_RECTANGLE params: period, edge, hi, lo, mid, eps (numpy's mod by period, hi below edge else lo, mid
+ *   where |x mod period| < eps).
+ * pb_psi: num = sum s_k g_k, den = sum c_k g_k over nframes <= 64 frames of frame_type (the host pointer array
+ *   frames_host, or `stack` with frame_stride elements between frames) and phase = atan2(num, den).  Any of num,
+ *   den and phase may be NULL.  Float frames: num_type = phase_type = frame_type.  Integer frames: phase_type =
+ *   PB_PSI_F64 and num_type PB_PSI_I64 (integer weights, exact) or PB_PSI_F64. */
+enum { PB_OVERLAP_CHUNK = 4096 };
+typedef enum { PB_LP_RULE_LP = 0, PB_LP_RULE_SMF = 1 } pb_lp_rule;
+typedef enum { PB_LP_NONE = 0, PB_LP_COS = 1, PB_LP_SIN = 2 } pb_lp_azimuth;
+typedef enum { PB_GRATING_SIN_AMP = 0, PB_GRATING_RECTANGLE = 1 } pb_grating_kind;
+typedef enum { PB_PSI_F32 = 0, PB_PSI_F64 = 1, PB_PSI_U16 = 2, PB_PSI_I32 = 3, PB_PSI_I64 = 4 } pb_psi_type;
+int pb_lp_modes(pb_handle_t h, int dtype, const void* r, const void* t, long long n, double a, int nmodes,
+                const double* plan_host, void* out, void* stream);
+int pb_overlap(pb_handle_t h, int dtype, const void* E, long long n, int nmodes, const void* modes,
+               const void* const* mode_ptrs_host, int modes_complex, const double* ip_dev, const double* ie_dev,
+               void* partial, void* eta, void* c_out, void* stream);
+int pb_wfs_combine(pb_handle_t h, int dtype, long long n, const void* a, const void* b, const double* coefs_host,
+                   const void* alpha_scale, const void* beta_scale, int real_out, void* out, void* stream);
+int pb_grating(pb_handle_t h, int dtype, int kind, long long n, const void* x, double shift, const double* params_host,
+               int nparams, const void* E, void* out, void* stream);
+int pb_psi(pb_handle_t h, int frame_type, int nframes, const void* const* frames_host, const void* stack,
+           long long frame_stride, long long n, const double* s_host, const double* c_host, int num_type, void* num,
+           void* den, int phase_type, void* phase, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,8 @@ Mirrors the reference's module layout for the path only:
     prysm_b200.dm           <-> prysm.x.dm (DM: render / render_adjoint; coordinates.warp is its spline warp)
     prysm_b200.segmented    <-> prysm.segmented (CompositeHexagonalAperture: rasterise, compose_opd and its adjoint)
     prysm_b200.polarization <-> prysm.x.polarization (Jones constructors, products, Mueller / Pauli, jones_adapter)
+    prysm_b200.fibers / .sri / .pdi / .psi  <-> prysm.x.fibers / sri / pdi / psi (LP modes and coupling, the SRI and
+                            PS/PDI forward models, PSI phase reconstruction)
     prysm_b200.graphs       CUDA-graph capture of launch-bound compositions (no reference counterpart)
 Every array operation is a call into libprysm_b200.so (hand-written sm_90a CUDA behind the C ABI
 of include/prysm_b200.h).  Importing this package without the built library raises ImportError.
@@ -22,6 +24,7 @@ from . import _capi  # noqa: F401  (fails loudly if the CUDA library is missing)
 from .conf import config  # noqa: F401
 from . import fttools, propagation, coronagraph, otf, psf, polynomials, polychromatic, mathops, graphs  # noqa: F401
 from . import coordinates, geometry, convolution, detector, dm, segmented, polarization  # noqa: F401
+from . import fibers, sri, pdi, psi  # noqa: F401
 from ._capi import B200Error  # noqa: F401
 from .propagation import Wavefront  # noqa: F401
 from ._ops import asdevice, asnumpy, set_device  # noqa: F401

@@ -91,6 +91,12 @@ SIGNATURES = {
     'pb_jones_product': (_i, [_vp, _i, _i, _ll, _i, _vp, _i, _i, _vp, _i, C.POINTER(_d), _vp, _vp]),
     'pb_jones_elements': (_i, [_vp, _i, _i, _ll, _vp, _i, C.POINTER(_d), _i, _vp, _vp]),
     'pb_jones_reduce': (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _vp]),
+    'pb_lp_modes': (_i, [_vp, _i, _vp, _vp, _ll, _d, _i, C.POINTER(_d), _vp, _vp]),
+    'pb_overlap': (_i, [_vp, _i, _vp, _ll, _i, _vp, C.POINTER(_vp), _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'pb_wfs_combine': (_i, [_vp, _i, _ll, _vp, _vp, C.POINTER(_d), _vp, _vp, _i, _vp, _vp]),
+    'pb_grating': (_i, [_vp, _i, _i, _ll, _vp, _d, C.POINTER(_d), _i, _vp, _vp, _vp]),
+    'pb_psi': (_i, [_vp, _i, _i, C.POINTER(_vp), _vp, _ll, _ll, C.POINTER(_d), C.POINTER(_d), _i, _vp, _vp, _i, _vp,
+                    _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -102,6 +108,11 @@ JONES_MATMUL, JONES_HADAMARD = range(2)
 JONES_OP_N, JONES_OP_H = range(2)
 JONES_FILL, JONES_ROTATION, JONES_RETARDER, JONES_DIATTENUATOR, JONES_VVR = range(5)
 JONES_MUELLER, JONES_KRON, JONES_PAULI = range(3)
+OVERLAP_CHUNK = 4096
+LP_RULE_LP, LP_RULE_SMF = range(2)
+LP_NONE, LP_COS, LP_SIN = range(3)
+GRATING_SIN_AMP, GRATING_RECTANGLE = range(2)
+PSI_F32, PSI_F64, PSI_U16, PSI_I32, PSI_I64 = range(5)
 
 
 def load_library(path=LIB_PATH):

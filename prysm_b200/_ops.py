@@ -1035,6 +1035,127 @@ def jones_reduce(kind, n, a, out, b=None):
     return out
 
 
+def lp_modes(r, t, a, plan, out=None):
+    """(P, *r.shape) LP / single-mode fiber fields of the real radius (and angle) grids (pb_lp_modes); plan is a
+    (P, 6) host array of l, ld, U, W, rule, az rows."""
+    r = r.contiguous()
+    t = None if t is None else t.to(r.dtype).contiguous()
+    plan = np.ascontiguousarray(plan, dtype=np.float64).reshape(-1, 6)
+    P = plan.shape[0]
+    if out is None:
+        out = torch.empty((P, *r.shape), dtype=r.dtype, device=r.device)
+    else:
+        _check_out(out, (P, *r.shape), r.dtype, r.device)
+    pp = plan.ctypes.data_as(C.POINTER(C.c_double))
+    h, st = _ctx(r)
+    h.check(lib.pb_lp_modes(h.ptr, _CODE[r.dtype], _p(r), _p(t), r.numel(), float(a), P, pp, _p(out), st))
+    return out
+
+
+def overlap(E, modes, ip=None, ie=None, want_c=False):
+    """eta_p = |sum conj(M_p) E|^2 / (I_p I_E) for every mode (pb_overlap), as one (P,) device tensor of E's real
+    type, and sqrt(I_E eta_0) as a 0-d device tensor when want_c.  `modes` is one packed (P, *E.shape) tensor or a
+    sequence of P tensors of E's shape (passed as pointers, never gathered); ip (P,) / ie (1,) are optional fp64 device
+    tensors of the intensity sums."""
+    E = E.contiguous()
+    rd = _REAL_OF[E.dtype]
+    n = E.numel()
+    if isinstance(modes, torch.Tensor):
+        packed, ptrs, P, first = modes.contiguous(), None, modes.shape[0], modes
+        if tuple(packed.shape[1:]) != tuple(E.shape):
+            raise ValueError(f'modes {tuple(packed.shape)} do not match the field {tuple(E.shape)}')
+        keep = (packed,)
+    else:
+        keep = tuple(m.contiguous() for m in modes)
+        P, first = len(keep), keep[0]
+        packed = None
+        for m in keep:
+            if tuple(m.shape) != tuple(E.shape) or m.dtype != first.dtype or m.device != E.device:
+                raise ValueError('every mode must be a device tensor of the field\'s shape, all of one dtype')
+        ptrs = (C.c_void_p * P)(*[m.data_ptr() for m in keep])
+    mc = first.is_complex()
+    if (_REAL_OF[first.dtype] if mc else first.dtype) != rd:
+        raise ValueError(f'modes of {first.dtype} with a field of {E.dtype}')
+    nchunk = -(-n // capi.OVERLAP_CHUNK)
+    work = torch.empty(nchunk * (3 * P + 1), dtype=torch.float64, device=E.device)
+    eta = torch.empty(P, dtype=rd, device=E.device)
+    c = torch.empty((), dtype=rd, device=E.device) if want_c else None
+    h, st = _ctx(E)
+    h.check(lib.pb_overlap(h.ptr, _CODE[E.dtype], _p(E), n, P, _p(packed), ptrs, int(mc), _p(ip), _p(ie), _p(work),
+                           _p(eta), _p(c), st))
+    del keep
+    return eta, c
+
+
+def wfs_combine(a, alpha=1.0, b=None, beta=1.0, alpha_scale=None, beta_scale=None, real_out=False):
+    """alpha a + beta b, or |alpha a + beta b|^2 with real_out (pb_wfs_combine); alpha / beta are host complex numbers,
+    each optionally times a 0-d real device tensor."""
+    a = a.contiguous()
+    if b is not None:
+        if tuple(b.shape) != tuple(a.shape):
+            raise ValueError(f'shape mismatch {tuple(a.shape)} vs {tuple(b.shape)}')
+        b = b.to(a.dtype).contiguous()
+    rd = _REAL_OF[a.dtype]
+    al, be = complex(alpha), complex(beta)
+    k, kp = _darr([al.real, al.imag, be.real, be.imag])
+    sa = None if alpha_scale is None else alpha_scale.to(rd).contiguous()
+    sb = None if beta_scale is None else beta_scale.to(rd).contiguous()
+    out = torch.empty(a.shape, dtype=rd if real_out else a.dtype, device=a.device)
+    h, st = _ctx(a)
+    h.check(lib.pb_wfs_combine(h.ptr, _CODE[a.dtype], a.numel(), _p(a), _p(b), kp, _p(sa), _p(sb), int(real_out),
+                               _p(out), st))
+    return out
+
+
+def grating(kind, x, params, shift=0.0, E=None):
+    """E * g(x + shift), or g itself when E is None (pb_grating); x real, the arithmetic in fp64."""
+    x = x.contiguous()
+    if E is not None:
+        E = E.to(_CPLX_OF[x.dtype]).contiguous()
+        if tuple(E.shape) != tuple(x.shape):
+            raise ValueError(f'shape mismatch {tuple(E.shape)} vs grid {tuple(x.shape)}')
+    p, pp = _darr(params)
+    out = torch.empty(x.shape, dtype=x.dtype if E is None else E.dtype, device=x.device)
+    h, st = _ctx(x)
+    h.check(lib.pb_grating(h.ptr, _CODE[x.dtype], int(kind), x.numel(), _p(x), float(shift), pp, len(p), _p(E),
+                           _p(out), st))
+    return out
+
+
+_PSI_TYPE = {torch.float32: capi.PSI_F32, torch.float64: capi.PSI_F64, torch.uint16: capi.PSI_U16,
+             torch.int32: capi.PSI_I32, torch.int64: capi.PSI_I64}
+
+
+def psi(frames, s, c, num_dtype, phase_dtype, want_num=True, want_phase=True):
+    """num = sum s_k g_k, den = sum c_k g_k and phase = atan2(num, den) in one pass over the frames (pb_psi): a (N, ...)
+    tensor or a sequence of N tensors of one shape and dtype (passed as pointers, never stacked)."""
+    if isinstance(frames, torch.Tensor):
+        stack, ptrs, N, f0 = frames.contiguous(), None, frames.shape[0], frames[0]
+        keep = (stack,)
+    else:
+        keep = tuple(f.contiguous() for f in frames)
+        N, f0, stack = len(keep), keep[0], None
+        for f in keep:
+            if f.shape != f0.shape or f.dtype != f0.dtype or f.device != f0.device:
+                raise ValueError('every frame must have one shape, dtype and device')
+        ptrs = (C.c_void_p * N)(*[f.data_ptr() for f in keep])
+    if f0.dtype not in _PSI_TYPE or f0.dtype == torch.int64:
+        raise ValueError(f'frames of {f0.dtype} are not supported (float32, float64, uint16, int32)')
+    shape, n = tuple(f0.shape), f0.numel()
+    s, sp = _darr(s)
+    c, cp = _darr(c)
+    if len(s) != N or len(c) != N:
+        raise ValueError(f'{N} frames but {len(s)} / {len(c)} weights')
+    num = torch.empty(shape, dtype=num_dtype, device=f0.device) if want_num else None
+    den = torch.empty(shape, dtype=num_dtype, device=f0.device) if want_num else None
+    phase = torch.empty(shape, dtype=phase_dtype, device=f0.device) if want_phase else None
+    h, st = _ctx(f0)
+    h.check(lib.pb_psi(h.ptr, _PSI_TYPE[f0.dtype], N, ptrs, _p(stack), n, n, sp, cp, _PSI_TYPE[num_dtype], _p(num),
+                       _p(den), _PSI_TYPE[phase_dtype], _p(phase), st))
+    del keep
+    return num, den, phase
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

@@ -22,12 +22,16 @@ import importlib
 from . import convolution as _conv
 from . import coordinates as _coords
 from . import dm as _dm
+from . import fibers as _fib
 from . import fttools as _ft
 from . import otf as _otf
+from . import pdi as _pdi
 from . import polarization as _pol
 from . import polynomials as _poly
 from . import propagation as _prop
 from . import psf as _psf
+from . import psi as _psi
+from . import sri as _sri
 
 # prysm module -> {attribute: replacement}
 _PROPAGATION_FUNCS = (
@@ -72,6 +76,14 @@ _TARGETS = {
     'prysm.x.polarization': {n: getattr(_pol, n) for n in (
         'jones_adapter', 'apply_polarization_optic', 'vector_vortex_retarder', 'jones_to_mueller', 'broadcast_kron',
         'pauli_coefficients')},
+    # wavefront sensing: prysm.x.sri binds smf_mode_field, prepare_executor and unfocus_dft at import time, so its
+    # classes and functions themselves are re-bound (as prysm.x.dm's DM is)
+    'prysm.x.fibers': {n: getattr(_fib, n) for n in (
+        'compute_LP_modes', 'smf_mode_field', 'mode_overlap_integral', 'multimode_coupling')},
+    'prysm.x.sri': {n: getattr(_sri, n) for n in (
+        'overlap_integral', 'to_photonic_fiber_and_back', 'SelfReferencedInterferometer')},
+    'prysm.x.pdi': {n: getattr(_pdi, n) for n in ('rectangle_pulse', 'PSPDI', 'evaluate_test_ref_arm_matching')},
+    'prysm.x.psi': {n: getattr(_psi, n) for n in ('psi_accumulate', 'degroot_formalism_psi')},
 }
 
 _saved = {}  # (module name, attribute) -> original
@@ -191,7 +203,7 @@ def set_backend_to_b200(device=None):
             continue
     for modname, mod in mods.items():
         repl = _TARGETS[modname]
-        if modname == 'prysm.otf':   # these return RichData: hand back the reference's own container
+        if modname in ('prysm.otf', 'prysm.x.psi'):   # these return RichData: hand back the reference's own container
             repl = {k: _returning_reference_richdata(v) for k, v in repl.items()}
         for attr, new in repl.items():
             if hasattr(mod, attr) and (modname, attr) not in _saved:
