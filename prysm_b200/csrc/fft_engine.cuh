@@ -145,6 +145,9 @@ __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {   // one arrival, no transaction bytes (release)
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                  "l"(src), "r"(bytes), "r"(smem_u32(bar))
@@ -301,13 +304,17 @@ struct FocusParams {
     long long in_bs, amp_bs, out_bs;
     // v2 pipeline (one field per launch pair)
     int ntiles;             // column kernel: N / T tiles, walked by a persistent grid
-    // 1: L2 eviction hints (streams evict_first); 2: L2 prefetch of the tile after next (unused); 4: plane 0 of the
-    // intermediate is written evict_last, and the row kernel discards its lines once they are read.  launch_focus2
+    // tiles claimed beyond the first wave (column kernel, atomicAdd); zero when the kernel starts, set back to zero by the
+    // row kernel of the same field
+    unsigned int* tile_ctr;
+    // 1: L2 eviction hints (streams evict_first); 2: unused; 4: plane 0 of the
+    // intermediate and the leading line groups of plane 1 are written evict_last, and the row kernel discards their
+    // lines once they are read.  launch_focus2
     // always passes 1 | 4.  It stays a run-time value: folding it into constants changes the code ptxas makes for the
     // two kernels, and that code measured 0.5-0.6 % slower at N = 2048 (H100 SXM, 700 W)
     int hints;
     // v2 column kernel launched as a programmatic dependent of the previous field's row kernel: 1 = its input does not
-    // overlap what that kernel writes, so the first tile may be gathered (and transformed) before the wait; 0 = wait first
+    // overlap what that kernel writes, so the kernel waits for it at its end; 0 = wait first
     int early_input;
 };
 
@@ -395,16 +402,18 @@ __device__ __forceinline__ void fft_two_stages_u(P2 (&v)[16], const int t, float
 // Against three 128-thread CTAs with the float4 plan in L1: 16 instead of 12 warps per SM, stage-1 twiddles are 64-bit
 // shared-memory loads (lane B's twiddle = lane A's times the per-thread constant w_2L^t, four scalar FP32 operations)
 // instead of 128-bit L1 loads whose latency shows up as the kernel's top stall, and the whole unified array is shared
-// memory (no L1 working set to protect).
-template <int L> struct GeoR4 {
+// memory (no L1 working set to protect).  KEEP1: line groups of plane 1 kept in L2 after plane 0's L/4.
+template <int L, int KEEP1> struct GeoR4 {
     using G = Geo<L>;
     static constexpr size_t GROUP = (size_t)G::SBUF * 16 + (size_t)L * 8;       // exchange + row buffer, bytes (multiple of 128)
     static constexpr size_t PLAN_OFF = 4 * GROUP;
     static constexpr size_t BAR_OFF = PLAN_OFF + (size_t)((Geo4<L>::PLANLEN * 8 + 15) / 16) * 16;
-    // arrivals of the four groups at each plane-0 line group (indexed by iteration; a CTA has at most L/4 of them), then one
-    // "this group arrived last" flag per group
+    // arrivals of the four groups at each kept line group, indexed by iteration: CTA b reads line group b + it * gridDim.x
+    // at iteration it, so the kept ones (< L/4 + KEEP1) come at it < (L/4 + KEEP1) / gridDim.x, at most L/4 + KEEP1
+    // counters for any grid.  Then one "this group arrived last" flag per group.
     static constexpr size_t CNT_OFF = BAR_OFF + 8 * sizeof(uint64_t);
-    static constexpr int NCNT = L / 4 + 4;
+    static constexpr int NKEEP = L / 4 + KEEP1;
+    static constexpr int NCNT = NKEEP + 4;
     static constexpr size_t SMEM = CNT_OFF + NCNT * sizeof(unsigned int);
 };
 

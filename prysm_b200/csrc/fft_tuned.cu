@@ -25,7 +25,8 @@
 //                      (cp.async.bulk + mbarrier), one row ahead.
 //   HBM traffic: pupil 8N^2 once, output 8K^2 once; the 16N^2-byte intermediate (64 MiB at N = 2048) is written and
 //   re-read through L2 where it fits (N <= 1024 on the H100's 50 MB).  At N = 2048 the v2 pair below keeps its plane 0
-//   in L2 and discards it after the read: only plane 1 (32 MiB) makes the trip through HBM.
+//   and the first 2 MiB of plane 1 in L2 and discards them after the read: only the rest of plane 1 (30 MiB) makes the
+//   trip through HBM.
 //
 // FFT_N engine: N/16 threads per line, 16 points x 2 lanes per thread in registers, radix
 // 16 x 16 x N/256, two shared-memory exchanges of float4 (1-in-16 padded, conflict free).
@@ -194,12 +195,24 @@ __global__ void __launch_bounds__(L / 16) focus_row_kernel(const FocusParams p) 
 //     apart) with two tensor-TMA boxes into a contiguous row buffer; the arithmetic after that is the v1 row kernel's.
 //   * One field per launch pair, and plane 0 of its intermediate (the even output rows, 8 N^2 bytes = 32 MiB at N = 2048)
 //     stays in L2: the column kernel writes it evict_last, the row kernel reads it first and then discards each line
-//     (discard.global.L2), so it never reaches HBM in either direction.  Plane 1 is written evict_first and makes the trip.
+//     (discard.global.L2), so it never reaches HBM in either direction.  So do the first kPlane1KeepBytes of plane 1,
+//     which the row kernel reads next; the rest of plane 1 is written evict_first and makes the trip.
+//   * The fields of a stack alternate between two intermediates, so that the column kernel of field f + 1 runs under the
+//     tail of field f's row kernel instead of waiting for it (focus_col4_kernel).
 // =====================================================================================================
 
 // share of plane 0's lines written evict_last (the rest evict_first): what the H100's 50 MB L2 keeps next to the
 // streaming input and plane 1
 constexpr float kPlane0Keep = 1.0f;
+// bytes of plane 1 kept in L2 as well, from its first line group on: the row kernel reads them right after plane 0 and
+// discards them in the same way.  Chosen by a sweep at N = 2048 (DESIGN §4.1)
+constexpr long long kPlane1KeepBytes = 2LL << 20;
+// ... in line groups of an L-point field (L/4 lines of 128 bytes each): at most all of plane 1, and a multiple of L/64
+// (whole thread ranges of the column kernel's stores, so that its choice of policy is a compile-time one)
+template <int L> constexpr int plane1_keep() {
+    const long long g = kPlane1KeepBytes / (32LL * L);
+    return (int)((g < L / 4 ? g : L / 4) / (L / 64) * (L / 64));
+}
 
 
 template <int L, bool INV, int HALF>
@@ -214,8 +227,11 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
     const float2* __restrict__ plan = reinterpret_cast<const float2*>(smem4 + G4::PLAN2);
     float4* S = smem4 + (HALF * 2 + cp) * G4::XBUF;
     const SyncGroup gsync{1 + HALF, 2 * NT};
-    // plane 0 is read back first by the row kernel that follows: it stays in L2 (and is discarded there); plane 1 streams
+    // plane 0 is read back first by the row kernel that follows: it stays in L2 (and is discarded there); plane 1 streams,
+    // but for its first KEEP1 line groups (rows j < 4 KEEP1), which the row kernel reads next and which stay as well
+    constexpr int KEEP1 = plane1_keep<L>();
     const uint64_t pol_tmp = (HALF == 0 && (p.hints & 4)) ? l2_policy_last_first(kPlane0Keep) : l2_policy((p.hints & 1) ? 1 : 0);
+    const uint64_t pol_tmp1 = (HALF == 1 && KEEP1 > 0 && (p.hints & 4)) ? l2_policy_last_first(kPlane0Keep) : pol_tmp;
     const uint64_t pol_in = l2_policy((p.hints & 1) ? 1 : 0);
     auto request_tile = [&](int ww) {   // one thread: gather tile ww = (field, column tile) into the staging area
         const int fb = ww / G2::TILES, tile = ww - fb * G2::TILES;
@@ -223,31 +239,38 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
 #pragma unroll
         for (int b = 0; b < G2::NBOX_IN; ++b)
             tma_load_3d(smem4 + G4::STAGE + b * G2::BOXR * 2, &in_map, tile * 4, b * G2::BOXR, fb, bar + 1, pol_in);
-        const int nn = ww + gridDim.x;   // the tile after: pull it from HBM into L2 now, so that its gather is an L2 hit
-        if ((p.hints & 2) && nn < p.ntiles) {
-            const int fb2 = nn / G2::TILES, tile2 = nn - fb2 * G2::TILES;
-#pragma unroll
-            for (int b = 0; b < G2::NBOX_IN; ++b) tma_prefetch_3d(&in_map, tile2 * 4, b * G2::BOXR, fb2);
-        }
+    };
+    // Tiles are handed out at run time: the first wave statically (CTA b: tile b), every later one by an atomic counter,
+    // so that the CTAs that start early -- on the SMs the previous row kernel's last wave leaves idle -- take more tiles.
+    // The tile of iteration it goes to slot[it & 1] before the arrival on bar[1] that the gather completes, so a thread
+    // reads it after its wait; p.ntiles there means "no more": the arrival is then a plain one.
+    int* slot = reinterpret_cast<int*>(bar + 3);
+    auto claim = [&](int it_next) {   // one thread, the staging area free: the CTA's tile of iteration it_next
+        const int ww = it_next == 0 ? (int)blockIdx.x : (int)gridDim.x + (int)atomicAdd(p.tile_ctr, 1u);
+        const int wc = ww < p.ntiles ? ww : p.ntiles;
+        slot[it_next & 1] = wc;
+        if (wc < p.ntiles) request_tile(wc);
+        else mbar_arrive(bar + 1);
     };
     unsigned int* released = reinterpret_cast<unsigned int*>(bar + 2);   // warps that hold the inputs of the current tile, summed over tiles
     if (HALF == 0 && lt == 0) {
         mbar_expect_tx(bar, (uint32_t)(G4::PLANLEN * sizeof(float2)));
         bulk_g2s(smem4 + G4::PLAN2, p.plan, (uint32_t)(G4::PLANLEN * sizeof(float2)), bar);
-        if ((int)blockIdx.x < p.ntiles) request_tile(blockIdx.x);
+        claim(0);
     }
     const float sgn = (t & 1) ? -1.0f : 1.0f;
     float2 u = make_float2(1.f, 0.f);
     if (HALF) { float sn, cs; sincospif(-(float)t / (float)L, &sn, &cs); u = make_float2(cs, sn); }   // w_2L^t = exp(-i pi t / L)
     mbar_wait(bar, 0);   // plan
-    int it = 0;
-    for (int w = blockIdx.x; w < p.ntiles; w += gridDim.x, ++it) {
+    for (int it = 0;; ++it) {
+        mbar_wait(bar + 1, it & 1);
+        const int w = slot[it & 1];
+        if (w >= p.ntiles) break;
         const int fb = w / G2::TILES, tile = w - fb * G2::TILES;
         auto sync = [&]() { gsync(); };
         P2 v[16];
         {
             float4 x[16];   // (col, col + 1) x (re, im)
-            mbar_wait(bar + 1, it & 1);
             const float4* __restrict__ sg = stage + lt;   // ((n*NT + t)*2 + cp)
 #pragma unroll
             for (int n = 0; n < 16; ++n) x[n] = sg[n * NT * 2];
@@ -266,9 +289,9 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
                 __threadfence_block();       // the LAST warp to release it requests the next tile on the spot
                 const unsigned int n = atomicAdd(released, 1u) + 1u;
                 __threadfence_block();
-                if (n == (unsigned int)(it + 1) * (4 * NT / 32) && w + (int)gridDim.x < p.ntiles) {
+                if (n == (unsigned int)(it + 1) * (4 * NT / 32)) {
                     fence_proxy_async();
-                    request_tile(w + gridDim.x);
+                    claim(it + 1);
                 }
             }
         }
@@ -277,9 +300,6 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
         sync();   // this group's exchange buffers are free for its next tile
 #pragma unroll
         for (int g = 0; g < G::GI; ++g) dftR<G::R3, INV>(v + g * G::R3);
-        // the intermediate is the previous field's row kernel's input (and its plane 0 is being discarded there): the first
-        // store waits for that kernel to complete
-        if (it == 0 && p.early_input) pdl_wait();
         // tile-major store: element (plane, j, tile, c) at ((plane*L/4 + j/4) * TILES + tile) * 16 + (j%4)*4 + c ; c = 2 cp
         float4* __restrict__ dst = reinterpret_cast<float4*>(
             p.tmp + fb * (2LL * L * L) + (long long)HALF * L * L + ((long long)(t >> 2) * G2::TILES + tile) * 16 + (t & 3) * 4 + 2 * cp);
@@ -294,7 +314,8 @@ __device__ __forceinline__ void focus_col4_group(const CUtensorMap& in_map, cons
                 if (HALF == 0) q = make_float4(sgn * y.re.x, sgn * y.im.x, sgn * y.re.y, sgn * y.im.y);
                 else q = INV ? make_float4(sgn * y.im.x, -sgn * y.re.x, sgn * y.im.y, -sgn * y.re.y)
                              : make_float4(-sgn * y.im.x, sgn * y.re.x, -sgn * y.im.y, sgn * y.re.y);
-                st_hint(dst + o, q, pol_tmp);
+                // rows g NT + 256 kk + t, t < NT: all below 4 KEEP1 (a multiple of NT) or none
+                st_hint(dst + o, q, (HALF == 1 && g * NT + 256 * kk < 4 * KEEP1) ? pol_tmp1 : pol_tmp);
             }
     }
 }
@@ -320,6 +341,18 @@ __global__ void __launch_bounds__(Geo4<L>::THREADS) focus_col4_kernel(const __gr
     const int grp = threadIdx.x / (2 * G::NT);
     if (grp == 0) focus_col4_group<L, INV, 0>(in_map, p, smem4, bar);
     else focus_col4_group<L, INV, 1>(in_map, p, smem4, bar);
+    // Field f of a call writes intermediate buffer f mod 2, so col(f + 1) writes the buffer row(f - 1) read and discarded,
+    // never the one row(f), its predecessor in the stream, is reading: it does not wait before its stores.  That they
+    // follow all of row(f - 1)'s reads and discards rests on griddepcontrol alone:
+    //   * griddepcontrol.wait returns once the prerequisite grid has completed and its memory operations are performed
+    //     and visible.  Every dependent column kernel executes it (here, or before its first gather when its input may
+    //     overlap the output), so col(f) completes only after row(f - 1) has completed;
+    //   * row(f) executes griddepcontrol.launch_dependents only after its own griddepcontrol.wait, i.e. after col(f) has
+    //     completed, and col(f + 1) is launched only once every CTA of row(f) has done so (or exited).
+    // So no CTA of col(f + 1) exists before row(f - 1) has completed.  The same chain orders row(f) after row(f - 1) --
+    // their outputs may be the same plane (accumulated intensity) -- and the plain launch of a call's first column kernel
+    // orders it after everything before it in the stream.
+    if (p.early_input) pdl_wait();
 }
 
 template <int L, bool INV>
@@ -327,7 +360,7 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
     using G = Geo<L>;
     using G2 = Geo2<L>;
     using G4 = Geo4<L>;
-    using R4 = GeoR4<L>;
+    using R4 = GeoR4<L, plane1_keep<L>()>;
     constexpr int NT = G::NT, R3 = G::R3, GI = G::GI;
     constexpr uint32_t ROW_BYTES = L * sizeof(float2);
     extern __shared__ __align__(128) unsigned char smraw[];
@@ -338,25 +371,26 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
     uint64_t* bars = reinterpret_cast<uint64_t*>(smraw + R4::BAR_OFF);   // [0] plan, [1 + grp] row of group grp
     uint64_t* bar = bars + 1 + grp;
     const uint64_t pol_tmp = l2_policy((p.hints & 1) ? 1 : 0), pol_out = l2_policy((p.hints & 1) ? 1 : 0);
-    // plane 0 (p.hints & 4): read evict_last so that no line leaves L2 -- written back -- before all four of its rows are
-    // read; then discarded
+    // the kept rows, plane 0 and the first KEEP1 line groups of plane 1 (p.hints & 4): read evict_last so that no line
+    // leaves L2 -- written back -- before all four of its rows are read; then discarded
     const uint64_t pol_keep = l2_policy((p.hints & 4) ? 2 : 0);
     auto request_row = [&](int R) {   // one thread: gather intermediate row R = (field, plane, j) into `inb`
         const int fb = R / (2 * L), rf = R - fb * (2 * L);
         const int ph = rf / L, j = rf - ph * L;
         const int grow = (fb * 2 + ph) * (L / 4) + (j >> 2);
-        const uint64_t pol = ph == 0 && (p.hints & 4) ? pol_keep : pol_tmp;
+        const uint64_t pol = rf < 4 * R4::NKEEP && (p.hints & 4) ? pol_keep : pol_tmp;
         mbar_expect_tx(bar, ROW_BYTES);
 #pragma unroll
         for (int b = 0; b < G2::NBOX_ROW; ++b) tma_load_4d(inb + b * G2::BOXT * 4, &tmp_map, 0, j & 3, b * G2::BOXT, grow, bar, pol);
     };
     int r = blockIdx.x * 4 + grp;
     const int rstep = gridDim.x * 4;
-    // Discard of plane 0 (one field per launch: rows R < L, R / 4 = line group).  The four groups of the CTA read the four
-    // rows j % 4 = 0..3 of the same line group at the same iteration, and no other CTA reads those lines.  Each group counts
-    // itself in arrived[it] once its row is in shared memory; the last of the four drops the group's 512 lines from L2.
+    // Discard of the kept line groups (one field per launch: rows R < 4 NKEEP, R / 4 = line group; plane 1's follow plane
+    // 0's).  The four groups of the CTA read the four rows j % 4 = 0..3 of the same line group at the same iteration, and
+    // no other CTA reads those lines.  Each group counts itself in arrived[it] once its row is in shared memory; the last
+    // of the four drops the group's lines from L2.
     unsigned int* arrived = reinterpret_cast<unsigned int*>(smraw + R4::CNT_OFF);
-    unsigned int* last = arrived + L / 4;   // [grp]: this group arrived last at its current line group
+    unsigned int* last = arrived + R4::NKEEP;   // [grp]: this group arrived last at its current line group
     for (int i = threadIdx.x; i < R4::NCNT; i += blockDim.x) arrived[i] = 0u;
     if (threadIdx.x == 0) {
         for (int i = 0; i < 5; ++i) mbar_init(bars + i, 1);
@@ -364,11 +398,14 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
         mbar_expect_tx(bars, (uint32_t)(G4::PLANLEN * sizeof(float2)));
         bulk_g2s(smraw + R4::PLAN_OFF, p.plan, (uint32_t)(G4::PLANLEN * sizeof(float2)), bars);
     }
-    // all CTAs are resident (grid <= SMs): the next field's column kernel may take the SMs this grid's last wave frees.
     // The intermediate comes from the column kernel before this one: wait for it to complete (the prologue above -- the
-    // static plan -- overlapped its tail)
-    pdl_launch_dependents();
+    // static plan -- overlapped its tail).  Only then let the next field's column kernel be launched, to take the SMs
+    // this grid's last wave frees: it writes the buffer the row kernel before this one read (see focus_col4_kernel)
     pdl_wait();
+    pdl_launch_dependents();
+    // the column kernel is complete: its tile counter is free for the column kernel two fields on, which starts only after
+    // this kernel has completed (the chain in focus_col4_kernel)
+    if (blockIdx.x == 0 && threadIdx.x == 0) *p.tile_ctr = 0u;
     __syncthreads();
     if (t == 0 && r < p.nrows) request_row(r);
     const SyncGroup gsync{1 + grp, NT};
@@ -379,7 +416,7 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
     for (int it = 0; r < p.nrows; ++it, r += rstep) {
         P2 v[16];
         mbar_wait(bar, it & 1);
-        const bool drop = (p.hints & 4) && r < L;
+        const bool drop = (p.hints & 4) && r < 4 * R4::NKEEP;
         if (drop && t == 0) {
             __threadfence_block();
             last[grp] = atomicAdd(arrived + it, 1u) == 3u;
@@ -558,13 +595,13 @@ int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, 
 
 // one field: `p.tmp` holds its [2][L][L] intermediate.  col_dep: how the column kernel follows what precedes it in the
 // stream -- 0: plain launch; 1: programmatic dependent of the previous field's row kernel; 2: the same, and its input does
-// not overlap that kernel's output (the first tile is gathered before the wait)
+// not overlap that kernel's output (the kernel waits for it at its end instead of its start)
 template <int L, bool INV>
 int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     using G = Geo<L>;
     using G2 = Geo2<L>;
     using G4 = Geo4<L>;
-    using R4 = GeoR4<L>;
+    using R4 = GeoR4<L, plane1_keep<L>()>;
     // one CTA per SM for both kernels: the column kernel's 512 threads fill the register file, and the row kernel keeps
     // its plan in shared memory, so it has no L1 working set to protect
     PB_TRY(set_smem_attrs(h, focus_col4_kernel<L, INV>, G4::SMEM, 1));
@@ -574,7 +611,7 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     p.plan = reinterpret_cast<const float4*>(plan);
     p.nrows = 2 * L;
     p.ntiles = G2::TILES;
-    p.hints = 1 | 4;   // eviction hints, plane 0 kept in L2 (FocusParams::hints)
+    p.hints = 1 | 4;   // eviction hints, plane 0 and the head of plane 1 kept in L2 (FocusParams::hints)
     // (descriptors are copied out at once: the handle's cache may be flushed by the next lookup)
     const CUtensorMap* map = nullptr;
     CUtensorMap in_m, tmp_m;
@@ -594,9 +631,10 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     }
     // Programmatic dependent launch: each kernel of the chain col(f), row(f), col(f + 1), ... is launched with
     // programmatic stream serialization, so that its CTAs take the SMs the previous kernel's last wave frees and run their
-    // prologue (barriers, plan, for a column kernel with `early_input` its first gather and transform) while that wave
-    // finishes; griddepcontrol.wait orders everything that depends on the previous kernel.  The column kernel of the
-    // first field of a call is launched plainly: what precedes it is not known.
+    // prologue (barriers, plan) while that wave finishes; griddepcontrol.wait orders everything that depends on the
+    // previous kernel.  A column kernel with `early_input` writes the other intermediate buffer than the row kernel it
+    // follows and runs its whole pass under that kernel's tail, waiting only at its end (focus_col4_kernel).  The column
+    // kernel of the first field of a call is launched plainly: what precedes it is not known.
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr.val.programmaticStreamSerializationAllowed = 1;
@@ -1005,9 +1043,22 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
     // (the fused phase-screen input, odd pitches, misaligned bases) runs the v1 pair, up to 8 fields per launch pair,
     // which evens out the tails of the two grids.
     const bool tma_ok = in_kind == PB_IN_COMPLEX && !((uintptr_t)in & 15) && !(in_ld & 1) && !(in_bs & 1);
+    // v2 stacks alternate between two intermediates (field f: buffer f mod 2), so that a column kernel never writes what
+    // the row kernel before it reads (focus_col4_kernel)
     const int per = tma_ok ? 1 : std::min(batch, 8);
+    const int nbuf = tma_ok && batch > 1 ? 2 : 1;
+    const size_t buf_bytes = (size_t)per * 2 * N * N * sizeof(float2);
     void* tmp = nullptr;
-    PB_TRY(ensure_scratch(h, 0, (size_t)per * 2 * N * N * sizeof(float2), &tmp));
+    PB_TRY(ensure_scratch(h, 0, nbuf * buf_bytes, &tmp));
+    // the column kernels' tile counters, one per buffer: zeroed once here, then by each field's row kernel
+    unsigned int* ctr = nullptr;
+    if (tma_ok) {
+        const TwKey key{2, PB_C64, 14};
+        auto it = h->tables.find(key);
+        const void* d = it != h->tables.end() ? it->second : nullptr;
+        if (!d) PB_TRY(upload_table(h, key, std::vector<std::complex<double>>(1), &d));   // one complex64 zero = two counters
+        ctr = reinterpret_cast<unsigned int*>(const_cast<void*>(d));
+    }
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
     const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : sizeof(float);
     const size_t out_elt = out_kind == PB_OUT_COMPLEX ? sizeof(float2) : sizeof(float);
@@ -1023,11 +1074,12 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
         p.in_kind = in_kind;
         p.amp = amp ? reinterpret_cast<const char*>(amp) + (size_t)b0 * amp_bs * amp_elt : nullptr;
         p.amp_kind = amp_kind; p.kturns = kturns; p.in_ld = in_ld;
-        p.tmp = reinterpret_cast<float2*>(tmp);
+        p.tmp = reinterpret_cast<float2*>(reinterpret_cast<char*>(tmp) + (size_t)(b0 % nbuf) * buf_bytes);
         p.plan = nullptr;
         p.out = reinterpret_cast<char*>(out) + (size_t)b0 * out_bs * out_elt;
         p.out_ld = out_ld; p.out_kind = out_kind; p.scale = (float)scale; p.weight = (float)weight;
         p.nrows = 0; p.ntiles = 0; p.hints = 0; p.early_input = 0;
+        p.tile_ctr = ctr ? ctr + (b0 % nbuf) : nullptr;
         p.in_bs = in_bs; p.amp_bs = amp_bs; p.out_bs = out_bs;
         int rc;
         if (tma_ok) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)

@@ -22,9 +22,11 @@ N, Q, BATCH = 2048, 2, 16
 K = N * Q
 MIB = 2 ** 20
 ALG = {'complex': 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 4 * K * K}
-# HBM bytes per propagation counted from the shapes: pupil reads, plane 1 of the 16 N^2-byte intermediate (written and
-# read back; plane 0 stays in L2), output writes
-HBM = {'complex': 8 * N * N + 2 * 8 * N * N + 8 * K * K, 'intensity': 8 * N * N + 2 * 8 * N * N + 4 * K * K}
+# HBM bytes per propagation counted from the shapes: pupil reads, plane 1 of the 16 N^2-byte intermediate but for its
+# first KEEP1 bytes (written and read back; plane 0 and those bytes stay in L2, kPlane1KeepBytes in csrc/fft_tuned.cu),
+# output writes
+KEEP1 = 2 * MIB
+HBM = {'complex': 8 * N * N + 2 * (8 * N * N - KEEP1) + 8 * K * K, 'intensity': 8 * N * N + 2 * (8 * N * N - KEEP1) + 4 * K * K}
 
 _CHILD = r'''
 import json, sys, time
