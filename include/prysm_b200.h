@@ -63,6 +63,21 @@ const char* pb_last_error(pb_handle_t h);
 const char* pb_version(void);
 /* number of kernels this handle has launched since creation (bench.py's gpu_launches) */
 long long pb_launch_count(pb_handle_t h);
+/* number of kernels this handle has launched on one route of the transform kernels, so that a caller (the test suite)
+ * can tell which specialisation a call ran.  route = kind << 28 | L << 8 | flags:
+ *   PB_ROUTE_AXIS_REG     axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>; flags INV | COLS << 1 | RT << 2 | PM << 3 |
+ *                         DENSE << 4
+ *   PB_ROUTE_AXIS_GENERIC the generic shared-memory axis pass, any length (L = 0, flags = 0)
+ *   PB_ROUTE_FOCUS_V1     focus_col_kernel / focus_row_kernel of N = L; flags INV (two kernels per chunk of fields)
+ *   PB_ROUTE_FOCUS_V2     focus_col4_kernel / focus_row4_kernel of N = L; flags INV (two kernels per field)
+ * Returns -1 for a NULL handle. */
+typedef enum {
+    PB_ROUTE_AXIS_REG = 1,
+    PB_ROUTE_AXIS_GENERIC = 2,
+    PB_ROUTE_FOCUS_V1 = 3,
+    PB_ROUTE_FOCUS_V2 = 4
+} pb_route_kind;
+long long pb_route_launch_count(pb_handle_t h, int route);
 
 /* ---- centred / plain 2-D FFT with fused pad, shifts, synthesis and |.|^2 ---------------
  * out = crop( S_out( FFT2_{dir}( S_in( pad( field ) ) ) ) ) * scale

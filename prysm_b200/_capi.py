@@ -16,6 +16,12 @@ OUT_COMPLEX, OUT_INTENSITY, OUT_ACCUMULATE = 0, 1, 2
 OP_N, OP_T, OP_H, OP_C = 0, 1, 2, 3
 MASK_REAL, MASK_COMPLEX = 0, 1
 MASK_CONJ, MASK_ONE_MINUS, MASK_REAL_OUT, MASK_ACCUMULATE = 1, 2, 4, 8
+ROUTE_AXIS_REG, ROUTE_AXIS_GENERIC, ROUTE_FOCUS_V1, ROUTE_FOCUS_V2 = 1, 2, 3, 4
+
+
+def route_code(kind, L=0, flags=0):
+    """the `route` argument of pb_route_launch_count"""
+    return kind << 28 | L << 8 | flags
 
 _vp, _i, _ll, _d = C.c_void_p, C.c_int, C.c_longlong, C.c_double
 
@@ -26,6 +32,7 @@ SIGNATURES = {
     'pb_last_error': (C.c_char_p, [_vp]),
     'pb_version': (C.c_char_p, []),
     'pb_launch_count': (_ll, [_vp]),
+    'pb_route_launch_count': (_ll, [_vp, _i]),
     'pb_fft2': (_i, [_vp, _i, _vp, _i, _vp, _i, _d, _i, _i, _ll, _i, _i, _i, _d, _i, _i,
                      _vp, _i, _d, _i, _i, _ll, _vp]),
     'pb_fft2_batch': (_i, [_vp, _i, _vp, _i, _vp, _i, _d, _i, _ll, _ll, _i, _i, _ll, _i, _i, _i, _d, _i, _i,
@@ -158,6 +165,10 @@ class Handle:
 
     def launch_count(self):
         return int(lib.pb_launch_count(self._h))
+
+    def route_launch_count(self, route):
+        """kernels launched on one route of the transform kernels (pb_route_launch_count)"""
+        return int(lib.pb_route_launch_count(self._h, int(route)))
 
     def close(self):
         if self._h:

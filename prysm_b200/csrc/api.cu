@@ -68,3 +68,10 @@ extern "C" long long pb_launch_count(pb_handle_t hh) {
     Handle* h = reinterpret_cast<Handle*>(hh);
     return h ? h->launches : 0;
 }
+
+extern "C" long long pb_route_launch_count(pb_handle_t hh, int route) {
+    Handle* h = reinterpret_cast<Handle*>(hh);
+    if (!h) return PB_ERR_INVALID;
+    auto it = h->route_launches.find(route);
+    return it == h->route_launches.end() ? 0 : it->second;
+}

@@ -172,6 +172,7 @@ static int launch_generic(Handle* h, const AxisPass& p, cudaStream_t st) {
     const int grid = (p.nb + T - 1) / T;
     axis_pass_kernel<R><<<grid, threads, smem, st>>>(p, T, ilog2(L), reinterpret_cast<const cplx<R>*>(tw));
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_AXIS_GENERIC, 0, 0)]++;
     return PB_OK;
 }
 

@@ -71,6 +71,8 @@ struct Handle {
     int device = 0;
     std::string err;
     long long launches = 0;
+    // kernel launches per route of the transform kernels (pb_route_launch_count; the codes are in prysm_b200.h)
+    std::map<int, long long> route_launches;
     std::map<TwKey, void*> tables;
     // scratch arenas, grown on demand (never on a warmed-up hot call)
     void* scratch[3] = {nullptr, nullptr, nullptr};
@@ -137,6 +139,9 @@ inline int fail(Handle* h, int code, const std::string& msg) {
             return pb::fail(h, PB_ERR_CUDA, std::string("kernel launch: ") + cudaGetErrorString(e_)); \
         (h)->launches++;                                                                      \
     } while (0)
+
+// key of Handle::route_launches (pb_route_launch_count)
+constexpr int route_code(int kind, int L, int flags) { return kind << 28 | L << 8 | flags; }
 
 #define PB_TRY(expr)               \
     do {                           \

@@ -562,6 +562,7 @@ int launch_focus(Handle* h, FocusParams p, int batch, cudaStream_t st) {
     PB_LAUNCH_CHECK(h);
     focus_row_kernel<L, INV><<<std::min(h->sm_count * row_ctas, p.nrows), L / 16, smem_row, st>>>(p);
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_FOCUS_V1, L, INV)] += 2;
     return PB_OK;
 }
 
@@ -656,6 +657,7 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     p.early_input = 0;
     PB_CUDA(h, launch(focus_row4_kernel<L, INV>, std::min(h->sm_count, (p.nrows + 3) / 4), 4 * G::NT, R4::SMEM, true, tmp_m));
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_FOCUS_V2, L, INV)] += 2;
     return PB_OK;
 }
 
@@ -968,6 +970,7 @@ int launch_axis_reg(Handle* h, const AxisPass& p, cudaStream_t st) {
     const int grid = (p.nb + lines_per_cta - 1) / lines_per_cta;
     axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE><<<grid, TP * G::NT, smem, st>>>(p, tw1, tw2);
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_AXIS_REG, L, INV | COLS << 1 | RT << 2 | PM << 3 | DENSE << 4)]++;
     return PB_OK;
 }
 
