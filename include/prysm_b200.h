@@ -70,12 +70,20 @@ long long pb_launch_count(pb_handle_t h);
  *   PB_ROUTE_AXIS_GENERIC the generic shared-memory axis pass, any length (L = 0, flags = 0)
  *   PB_ROUTE_FOCUS_V1     focus_col_kernel / focus_row_kernel of N = L; flags INV (two kernels per chunk of fields)
  *   PB_ROUTE_FOCUS_V2     focus_col4_kernel / focus_row4_kernel of N = L; flags INV (two kernels per field)
+ *   PB_ROUTE_MDFT_TC      wgmma_gemm_kernel of the tensor-core matrix DFT; L = split-K pieces (1 when not split);
+ *                         flags STREAMK | STAGE2 << 1 | PARTIALS << 2 (PARTIALS: writes split-K partial planes)
+ *   PB_ROUTE_MDFT_REDUCE  reduce_splits_kernel, the sum of the split-K partial planes; L = pieces, flags = 0
+ *   PB_ROUTE_CGEMM        cgemm_kernel<R, OPA, OPB> of the CUDA-core GEMM (pb_cgemm, pb_mdft_apply); L = 0,
+ *                         flags DTYPE | OPA << 1 | OPB << 3 (DTYPE: PB_C64 / PB_C128; OP as in pb_cgemm)
  * Returns -1 for a NULL handle. */
 typedef enum {
     PB_ROUTE_AXIS_REG = 1,
     PB_ROUTE_AXIS_GENERIC = 2,
     PB_ROUTE_FOCUS_V1 = 3,
-    PB_ROUTE_FOCUS_V2 = 4
+    PB_ROUTE_FOCUS_V2 = 4,
+    PB_ROUTE_MDFT_TC = 5,
+    PB_ROUTE_MDFT_REDUCE = 6,
+    PB_ROUTE_CGEMM = 7
 } pb_route_kind;
 long long pb_route_launch_count(pb_handle_t h, int route);
 

@@ -17,6 +17,7 @@ OP_N, OP_T, OP_H, OP_C = 0, 1, 2, 3
 MASK_REAL, MASK_COMPLEX = 0, 1
 MASK_CONJ, MASK_ONE_MINUS, MASK_REAL_OUT, MASK_ACCUMULATE = 1, 2, 4, 8
 ROUTE_AXIS_REG, ROUTE_AXIS_GENERIC, ROUTE_FOCUS_V1, ROUTE_FOCUS_V2 = 1, 2, 3, 4
+ROUTE_MDFT_TC, ROUTE_MDFT_REDUCE, ROUTE_CGEMM = 5, 6, 7
 
 
 def route_code(kind, L=0, flags=0):

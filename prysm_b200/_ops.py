@@ -411,10 +411,17 @@ def mdft_tc_expand(E):
     return hi, lo
 
 
+def _tc_aligned(a):
+    """a contiguous, with a 16-byte aligned base: the tensor-core GEMM reads its input through TMA, which needs that.
+    A contiguous view at an odd element offset (flat[1:].view(N, N)) is copied; anything else is passed as is."""
+    a = a.contiguous()
+    return a if a.data_ptr() % 16 == 0 else a.clone()
+
+
 def mdft_tc_apply(ex_hi, ex_lo, ey_hi, ey_lo, a, norm, out=None):
     my, ny = ey_hi.shape[0] // 2, ey_hi.shape[1] // 2
     mx, nx = ex_hi.shape[0] // 2, ex_hi.shape[1] // 2
-    a = a.contiguous()
+    a = _tc_aligned(a)
     if tuple(a.shape) != (ny, nx):
         raise ValueError(f'array of shape {tuple(a.shape)} does not match the executor ({(ny, nx)})')
     out = _contiguous_out(out, (my, mx), a)

@@ -117,6 +117,7 @@ int cgemm_simt(Handle* h, int dtype, int opA, int opB, int m, int n, int k, doub
     else
         launch_ab<double>(opA, opB, g, st, m, n, k, alpha, (const double2*)A, lda, (const double2*)B, ldb, (double2*)C, ldc);
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_CGEMM, 0, dtype | opA << 1 | opB << 3)]++;
     return PB_OK;
 }
 

@@ -393,12 +393,12 @@ int make_map(Handle* h, CUtensorMap* map, const void* base, long long rows, long
 
 // C'(M x N) = A'(M x K) @ B'(N x K)^T on the tensor cores; see GemmParams for the output modes.  Split-K: `splits`
 // pieces of gp.kblocks K-blocks along grid z.  Stream-K (mode 0 only): one CTA per SM over all tiles, `work` =
-// SK_WORK_BYTES of scratch.
+// SK_WORK_BYTES of scratch.  `stage` (1 or 2) only keys the launch's route counter.
 constexpr int SK_MAX_CTAS = 160;
 constexpr long long SK_WORK_BYTES = (long long)SK_MAX_CTAS * BM * BN * 4 + 4096;   // partial tiles + flags
 
 template <bool SK>
-int launch_gemm(Handle* h, const float* A, const float* Bhi, const float* Blo, int M, int N, long long K,
+int launch_gemm(Handle* h, int stage, const float* A, const float* Bhi, const float* Blo, int M, int N, long long K,
                 int splits, GemmParams gp, void* work, cudaStream_t st) {
     CUtensorMap mA, mBhi, mBlo;
     PB_TRY(make_map(h, &mA, A, M, K, BM));
@@ -417,6 +417,7 @@ int launch_gemm(Handle* h, const float* A, const float* Bhi, const float* Blo, i
     }
     wgmma_gemm_kernel<SK><<<grid, NTHREADS, SMEM_BYTES, st>>>(mA, mBhi, mBlo, gp);
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_MDFT_TC, splits, int(SK) | (stage == 2) << 1 | gp.mode << 2)]++;
     return PB_OK;
 }
 
@@ -489,8 +490,8 @@ extern "C" int pb_mdft_tc_apply(pb_handle_t hh, const void* ExB_hi, const void* 
         GemmParams gp{};
         gp.kblocks = (int)(2LL * nx / BK); gp.chunk = chunk; gp.mode = 0; gp.out = t1; gp.ldo = ny; gp.scale = 1.0f;
         if (use_streamk(h, (ny / BM) * (2 * mx / BN), gp.kblocks, chunk))
-            PB_TRY(launch_gemm<true>(h, (const float*)a, (const float*)ExB_hi, (const float*)ExB_lo, ny, 2 * mx, 2LL * nx, 1, gp, skw, st));
-        else PB_TRY(launch_gemm<false>(h, (const float*)a, (const float*)ExB_hi, (const float*)ExB_lo, ny, 2 * mx, 2LL * nx, 1, gp, nullptr, st));
+            PB_TRY(launch_gemm<true>(h, 1, (const float*)a, (const float*)ExB_hi, (const float*)ExB_lo, ny, 2 * mx, 2LL * nx, 1, gp, skw, st));
+        else PB_TRY(launch_gemm<false>(h, 1, (const float*)a, (const float*)ExB_hi, (const float*)ExB_lo, ny, 2 * mx, 2LL * nx, 1, gp, nullptr, st));
     }
     // stage 2: out^T' = T1^T' @ Ey'^T : M = mx, N = 2*my, K = 2*ny.  Few tiles and a long contraction: stream-K over all SMs
     // with the owner's store landing the result, scaled by `norm`, directly in (My, Mx) complex orientation (same index
@@ -501,19 +502,20 @@ extern "C" int pb_mdft_tc_apply(pb_handle_t hh, const void* ExB_hi, const void* 
         gp.kblocks = (int)(2LL * ny / BK); gp.chunk = chunk; gp.mode = 0; gp.out = reinterpret_cast<float*>(out); gp.ldo = mx;
         gp.scale = (float)norm;
         if (use_streamk(h, (mx / BM) * (2 * my / BN), gp.kblocks, chunk))
-            return launch_gemm<true>(h, t1, (const float*)EyB_hi, (const float*)EyB_lo, mx, 2 * my, 2LL * ny, 1, gp, skw, st);
+            return launch_gemm<true>(h, 2, t1, (const float*)EyB_hi, (const float*)EyB_lo, mx, 2 * my, 2LL * ny, 1, gp, skw, st);
     }
     {   // split-K partials transposed into ws[s][2my][mx]
         GemmParams gp{};
         gp.kblocks = (int)(2LL * ny / BK / splits); gp.chunk = chunk; gp.mode = 1; gp.out = ws; gp.ldo = mx;
         gp.split_stride = 2LL * my * mx; gp.scale = 1.0f;
-        PB_TRY(launch_gemm<false>(h, t1, (const float*)EyB_hi, (const float*)EyB_lo, mx, 2 * my, 2LL * ny, splits, gp, nullptr, st));
+        PB_TRY(launch_gemm<false>(h, 2, t1, (const float*)EyB_hi, (const float*)EyB_lo, mx, 2 * my, 2LL * ny, splits, gp, nullptr, st));
     }
     {
         const long long tot = (long long)my * mx;
         const int g = (int)std::min<long long>((tot + 255) / 256, (long long)h->sm_count * 8);
         reduce_splits_kernel<<<g, 256, 0, st>>>(ws, splits, my, mx, (float)norm, (float2*)out);
         PB_LAUNCH_CHECK(h);
+        h->route_launches[route_code(PB_ROUTE_MDFT_REDUCE, splits, 0)]++;
     }
     return PB_OK;
 }

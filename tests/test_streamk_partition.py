@@ -37,8 +37,17 @@ def gathered_by_owner(g, G, ntiles, upt, tile):
 # H100 grids (G = 132 SMs, 128 x 128 tiles, 2 K-blocks of 32 per unit): (64, 32) the first stage of a 1024^2 -> 512^2 MDFT,
 # (64, 16) of its adjoint, (32, 128) the second stage of C3 (4096^2 -> 512^2) and (128, 32) the first stage of a 1024^2 <->
 # 1024^2 coronagraph leg, the last two under PB_MDFT_STREAMK=2.  The rest are other grid sizes and edge cases.
-@pytest.mark.parametrize('ntiles,upt,G', [(64, 32, 132), (64, 16, 132), (32, 128, 132), (128, 32, 132), (33, 4, 132),
-                                          (128, 128, 148), (64, 32, 148), (16, 128, 148), (5, 7, 3), (128, 128, 160), (8, 128, 148)])
+GRIDS = [(64, 32, 132), (64, 16, 132), (32, 128, 132), (128, 32, 132), (33, 4, 132),
+         (128, 128, 148), (64, 32, 148), (16, 128, 148), (5, 7, 3), (128, 128, 160), (8, 128, 148)]
+# the other grids the tensor-core cases of tests/test_gpu_mdft_vs_fp64.py reach on 132 SMs, by default or under
+# PB_MDFT_STREAMK=2 (tests/test_host_mdft_routes.py lists them): rectangular shapes, one K-block pair per unit (nx = 256),
+# a 16384-long contraction over 4 tiles, and the 2048 tiles of the C3 adjoint
+GRIDS += [(4, 256, 132), (20, 32, 132), (32, 20, 132), (32, 32, 132), (48, 64, 132), (80, 32, 132), (128, 8, 132),
+          (128, 16, 132), (128, 24, 132), (192, 64, 132), (256, 8, 132), (256, 16, 132), (256, 128, 132),
+          (512, 16, 132), (2048, 16, 132)]
+
+
+@pytest.mark.parametrize('ntiles,upt,G', GRIDS)
 def test_partition_invariants(ntiles, upt, G):
     cover = {}
     first_piece_owner = {}
