@@ -68,7 +68,6 @@ long long pb_launch_count(pb_handle_t h);
  *   PB_ROUTE_AXIS_REG     axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>; flags INV | COLS << 1 | RT << 2 | PM << 3 |
  *                         DENSE << 4
  *   PB_ROUTE_AXIS_GENERIC the generic shared-memory axis pass, any length (L = 0, flags = 0)
- *   PB_ROUTE_FOCUS_V1     focus_col_kernel / focus_row_kernel of N = L; flags INV (two kernels per chunk of fields)
  *   PB_ROUTE_FOCUS_V2     focus_col4_kernel / focus_row4_kernel of N = L; flags INV (two kernels per field)
  *   PB_ROUTE_MDFT_TC      wgmma_gemm_kernel of the tensor-core matrix DFT; L = split-K pieces (1 when not split);
  *                         flags STREAMK | STAGE2 << 1 | PARTIALS << 2 (PARTIALS: writes split-K partial planes)
@@ -79,7 +78,7 @@ long long pb_launch_count(pb_handle_t h);
 typedef enum {
     PB_ROUTE_AXIS_REG = 1,
     PB_ROUTE_AXIS_GENERIC = 2,
-    PB_ROUTE_FOCUS_V1 = 3,
+    /* 3 is retired: it counted a second focus pair, since removed */
     PB_ROUTE_FOCUS_V2 = 4,
     PB_ROUTE_MDFT_TC = 5,
     PB_ROUTE_MDFT_REDUCE = 6,

@@ -45,8 +45,18 @@ __device__ inline double2 expi_turns(double turns, double) {
     return make_double2(c, s);
 }
 
+// what a table of Handle::tables holds (TwKey::kind)
+enum TwKind {
+    TW_ROOTS = 0,                    // w_n^k, k < n (get_twiddles)
+    TW_CHIRP_FWD, TW_CHIRP_INV,      // Bluestein chirp of length n, dir -1 / +1
+    TW_FILTER_FWD, TW_FILTER_INV,    // spectrum of the Bluestein filter, dir -1 / +1
+    TW_PLAIN_PLAN,                   // stage twiddles of the register FFT engine, FFT_n (get_plain_plan)
+    TW_FOCUS_PLAN,                   // plan of the focus pair, FFT_n (get_col4_plan)
+    TW_TILE_COUNTERS,                // the focus column kernels' two tile counters (n = 2, one complex64 zero)
+};
+
 struct TwKey {
-    int n; int dtype; int kind;  // kind 0: w_n^k table; 1/2: bluestein chirp (dir -1/+1); 3/4: bluestein filter spectrum
+    int n; int dtype; int kind;  // kind: TwKind
     bool operator<(const TwKey& o) const {
         if (n != o.n) return n < o.n;
         if (dtype != o.dtype) return dtype < o.dtype;
@@ -150,6 +160,10 @@ constexpr int route_code(int kind, int L, int flags) { return kind << 28 | L << 
     } while (0)
 
 int ensure_scratch(Handle* h, int slot, size_t bytes, void** out);
+// amp * exp(2 pi i kturns opd) into the dense complex array out (count elements in rows of nx); opd and amp (pb_amp_kind)
+// have row pitch ld (elements)
+int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, const void* opd, double kturns, long long count,
+                        long long nx, long long ld, void* out, cudaStream_t st);
 // device table of w_n^k = exp(-2*pi*i*k/n), k in [0,n)
 int get_twiddles(Handle* h, int n, int dtype, const void** out);
 // upload a host fp64 complex table in the precision of key.dtype and cache it in the handle

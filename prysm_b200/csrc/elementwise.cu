@@ -12,20 +12,32 @@ static inline int grid_for(long long n, int threads, int sm_count) {
     return (int)std::max<long long>(1, std::min(g, cap));
 }
 
+// out[i] = amp * exp(2 pi i kturns opd) over the n elements of a dense array of rows of nx; opd and amp are read with
+// row pitch ld (elements)
 template <typename R>
 __global__ void phase_screen_kernel(const void* amp, int amp_kind, const R* __restrict__ opd, double kturns,
-                                    long long n, cplx<R>* __restrict__ out) {
+                                    long long n, long long nx, long long ld, cplx<R>* __restrict__ out) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long s = ld == nx ? i : i / nx * ld + i % nx;
         R a = R(1);
-        if (amp_kind == PB_AMP_REAL) a = reinterpret_cast<const R*>(amp)[i];
-        else if (amp_kind == PB_AMP_U8) a = reinterpret_cast<const unsigned char*>(amp)[i] ? R(1) : R(0);
+        if (amp_kind == PB_AMP_REAL) a = reinterpret_cast<const R*>(amp)[s];
+        else if (amp_kind == PB_AMP_U8) a = reinterpret_cast<const unsigned char*>(amp)[s] ? R(1) : R(0);
         cplx<R> e = mk<R>(R(0), R(0));
         if (a != R(0)) {
-            e = expi_turns(kturns * (double)opd[i], R(0));
+            e = expi_turns(kturns * (double)opd[s], R(0));
             e.x *= a; e.y *= a;
         }
         out[i] = e;
     }
+}
+
+int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, const void* opd, double kturns, long long count,
+                        long long nx, long long ld, void* out, cudaStream_t st) {
+    const int g = grid_for(count, 256, h->sm_count);
+    if (dtype == PB_C64) phase_screen_kernel<float><<<g, 256, 0, st>>>(amp, amp_kind, (const float*)opd, kturns, count, nx, ld, (float2*)out);
+    else phase_screen_kernel<double><<<g, 256, 0, st>>>(amp, amp_kind, (const double*)opd, kturns, count, nx, ld, (double2*)out);
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
 }
 
 template <typename R>
@@ -228,12 +240,7 @@ extern "C" int pb_phase_screen(pb_handle_t hh, int dtype, const void* amp, int a
                                double kscale, long long count, void* out, void* stream) {
     PB_HANDLE(hh);
     if (count <= 0) return PB_OK;
-    const int g = grid_for(count, 256, h->sm_count);
-    const double kt = kscale / (2.0 * M_PI);
-    if (dtype == PB_C64) phase_screen_kernel<float><<<g, 256, 0, st>>>(amp, amp_kind, (const float*)opd, kt, count, (float2*)out);
-    else phase_screen_kernel<double><<<g, 256, 0, st>>>(amp, amp_kind, (const double*)opd, kt, count, (double2*)out);
-    PB_LAUNCH_CHECK(h);
-    return PB_OK;
+    return launch_phase_screen(h, dtype, amp, amp_kind, opd, kscale / (2.0 * M_PI), count, count, count, out, st);
 }
 
 extern "C" int pb_intensity(pb_handle_t hh, int dtype, const void* in, long long count, double weight, int accumulate,

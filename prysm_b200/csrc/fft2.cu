@@ -52,7 +52,7 @@ int upload_table(Handle* h, const TwKey& key, const std::vector<std::complex<dou
 }
 
 int get_twiddles(Handle* h, int n, int dtype, const void** out) {
-    TwKey key{n, dtype, 0};
+    TwKey key{n, dtype, TW_ROOTS};
     auto it = h->tables.find(key);
     if (it != h->tables.end()) { *out = it->second; return PB_OK; }
     std::vector<std::complex<double>> t(n);
@@ -68,7 +68,7 @@ static int bluestein_len(int n) { int m = 1; while (m < 2 * n - 1) m <<= 1; retu
 
 // chirp c[j] = exp(dir*pi*i*j^2/n), j^2 reduced mod 2n exactly
 static int get_chirp(Handle* h, int n, int dtype, int dir, const void** out) {
-    TwKey key{n, dtype, dir < 0 ? 1 : 2};
+    TwKey key{n, dtype, dir < 0 ? TW_CHIRP_FWD : TW_CHIRP_INV};
     auto it = h->tables.find(key);
     if (it != h->tables.end()) { *out = it->second; return PB_OK; }
     std::vector<std::complex<double>> t(n);
@@ -82,7 +82,7 @@ static int get_chirp(Handle* h, int n, int dtype, int dir, const void** out) {
 
 // spectrum of the Bluestein filter g[d mod M] = conj(c[|d|]), |d| < n
 static int get_chirp_filter(Handle* h, int n, int dtype, int dir, const void** out) {
-    TwKey key{n, dtype, dir < 0 ? 3 : 4};
+    TwKey key{n, dtype, dir < 0 ? TW_FILTER_FWD : TW_FILTER_INV};
     auto it = h->tables.find(key);
     if (it != h->tables.end()) { *out = it->second; return PB_OK; }
     const int M = bluestein_len(n);

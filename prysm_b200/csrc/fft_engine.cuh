@@ -112,13 +112,8 @@ template <bool INV, int n> __device__ __forceinline__ P2 make_lanes(float2 x) {
 __device__ __forceinline__ int pad16(int a) { return a + (a >> 4); }
 
 // ---- cache-policy loads / stores --------------------------------------------------------------------
-// The only data with reuse inside an SM is the twiddle plan: it is pinned in L1 (evict_last) and every
+// The only data with reuse inside an SM is the twiddle plan: it is pinned in L1 (evict_last, ld_tw) and every
 // streaming access bypasses L1 allocation so that it cannot displace the plan.
-__device__ __forceinline__ float4 ld_plan(const float4* p) {
-    float4 r;
-    asm("ld.global.nc.L1::evict_last.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
-    return r;
-}
 __device__ __forceinline__ float2 ld_stream(const float2* p) {
     float2 r;
     asm("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(r.x), "=f"(r.y) : "l"(p));
@@ -213,61 +208,49 @@ template <int L> struct Geo {
     static constexpr int R3 = L / 256;         // last radix
     static constexpr int GI = 16 / R3;         // last-stage items per thread
     static constexpr int SBUF = L + L / 16;    // padded exchange buffer, float4 elements
-    // plan table layout (float4 elements):
-    //   TW1[k][t], k < 16 : (w_L^(tk).re, (w_L^(tk) w_2L^t).re, w_L^(tk).im, (w_L^(tk) w_2L^t).im)
-    //   TW2[k-1][m], 1 <= k < 16, m < NT/16 : (wr, wr, wi, wi), w = w_L^(16 m k)
-    static constexpr int TW1 = 0, TW2 = 16 * NT, PLAN = 16 * NT + 15 * (NT / 16);
 };
 
-// First two radix-16 stages on both lanes.  In: v[n] = lanes of x[n*NT + t].  Out: stage-2 results in S
-// (float4, 1-in-16 padded, position-major): final-stage item i in [0, 256) reads S[pad16(n*256 + i)],
-// n < L/256, and after the radix-(L/256) dft holds X[i + 256*k].
-// Twiddle sources: 0 = float4 plan in global memory (L1 evict_last), 1 = float4 plan in shared memory,
-// 2 = "plain" float2 tables in global memory, the same twiddle for both lanes (k = 1..15 only).
-template <int KIND> __device__ __forceinline__ float4 load_tw(const void* base, int idx) {
-    if (KIND == 1) return reinterpret_cast<const float4*>(base)[idx];
-    if (KIND == 0) return ld_plan(reinterpret_cast<const float4*>(base) + idx);
+// one twiddle of the "plain" float2 tables, pinned in L1, as the same twiddle for both lanes
+__device__ __forceinline__ float4 ld_tw(const float2* p) {
     float2 w;
-    asm("ld.global.nc.L1::evict_last.v2.f32 {%0, %1}, [%2];" : "=f"(w.x), "=f"(w.y) : "l"(reinterpret_cast<const float2*>(base) + idx));
+    asm("ld.global.nc.L1::evict_last.v2.f32 {%0, %1}, [%2];" : "=f"(w.x), "=f"(w.y) : "l"(p));
     return make_float4(w.x, w.x, w.y, w.y);
 }
 
-template <int L, bool INV, int KIND, class Sync1, class Sync>
+// First two radix-16 stages on both lanes, the whole CTA on one line pair.  In: v[n] = lanes of x[n*NT + t].  Out:
+// stage-2 results in S (float4, 1-in-16 padded, position-major): final-stage item i in [0, 256) reads
+// S[pad16(n*256 + i)], n < L/256, and after the radix-(L/256) dft holds X[i + 256*k].
+// Twiddles: the plain tables in global memory (get_plain_plan), tw1[(k-1)*NT + t] and tw2[(k-1)*NT/16 + m], k = 1..15.
+template <int L, bool INV>
 __device__ __forceinline__ void fft_two_stages(P2 (&v)[16], const int t, float4* __restrict__ S,
-                                               const void* __restrict__ tw1, const void* __restrict__ tw2, Sync1 sync1,
-                                               Sync sync) {
+                                               const float2* __restrict__ tw1, const float2* __restrict__ tw2) {
     using G = Geo<L>;
     constexpr int NT = G::NT;
     dft16<INV>(v);
-    if (KIND == 2) {  // tw1[(k-1)*NT + t]
 #pragma unroll
-        for (int k = 1; k < 16; ++k) v[k] = mul_tw<INV>(v[k], load_tw<KIND>(tw1, (k - 1) * NT + t));
-    } else {          // tw1[k*NT + t], k = 0 carries lane B's w_2L^t
-#pragma unroll
-        for (int k = 0; k < 16; ++k) v[k] = mul_tw<INV>(v[k], load_tw<KIND>(tw1, k * NT + t));
-    }
+    for (int k = 1; k < 16; ++k) v[k] = mul_tw<INV>(v[k], ld_tw(tw1 + ((k - 1) * NT + t)));
     {
         float4* __restrict__ d = S + t * 17;
 #pragma unroll
         for (int k = 0; k < 16; ++k) d[k] = pack(v[k]);
     }
-    sync1();
+    __syncthreads();
     {
         const float4* __restrict__ s = S + pad16(t);
 #pragma unroll
         for (int n = 0; n < 16; ++n) v[n] = unpack(s[n * (NT + NT / 16)]);
     }
-    sync();
+    __syncthreads();
     dft16<INV>(v);
     const int m = t >> 4, a = t & 15;
 #pragma unroll
-    for (int k = 1; k < 16; ++k) v[k] = mul_tw<INV>(v[k], load_tw<KIND>(tw2, (k - 1) * (NT / 16) + m));
+    for (int k = 1; k < 16; ++k) v[k] = mul_tw<INV>(v[k], ld_tw(tw2 + ((k - 1) * (NT / 16) + m)));
     {
         float4* __restrict__ d = S + m * 272 + a;
 #pragma unroll
         for (int k = 0; k < 16; ++k) d[17 * k] = pack(v[k]);
     }
-    sync();
+    __syncthreads();
 }
 
 // final radix-(L/256) stage inputs: afterwards v[g*R3 + n] holds the n-th input of item t + g*NT
@@ -289,20 +272,17 @@ __device__ __forceinline__ void fft_last_stage_load(P2 (&v)[16], const int t, co
     v[12] = make_lanes<INV, 12>(X(12)); v[13] = make_lanes<INV, 13>(X(13)); v[14] = make_lanes<INV, 14>(X(14)); \
     v[15] = make_lanes<INV, 15>(X(15));
 
-struct SyncCta { __device__ __forceinline__ void operator()() const { __syncthreads(); } };
-
+// One field per launch pair (launch_focus2)
 struct FocusParams {
-    // column kernel input
-    const void* in; int in_kind; const void* amp; int amp_kind; double kturns; long long in_ld;
-    float2* tmp;            // [2][N][N] intermediate (plane 0: even output rows, plane 1: odd)
-    const float4* plan;     // Geo<N> plan table
+    // column kernel input: N x N complex64, 16-byte aligned base, even row pitch in_ld (elements)
+    const void* in; long long in_ld;
+    float2* tmp;            // [2][N][N] tile-major intermediate (plane 0: even output rows, plane 1: odd)
+    const float2* plan;     // get_col4_plan<N>
     // row kernel output
     void* out; long long out_ld; int out_kind; float scale; float weight;
-    int nrows;              // row kernel: batch * 2N
-    // batch of independent fields in one launch pair (blockIdx.y in the column kernel; rows of all fields in the row
-    // kernel's persistent loop): element strides of in / amp / out in units of their own scalar type
-    long long in_bs, amp_bs, out_bs;
-    // v2 pipeline (one field per launch pair)
+    int nrows;              // row kernel: 2N
+    // element stride between fields of out; the row kernel indexes the field of row r / 2N, which is always 0
+    long long out_bs;
     int ntiles;             // column kernel: N / T tiles, walked by a persistent grid
     // tiles claimed beyond the first wave (column kernel, atomicAdd); zero when the kernel starts, set back to zero by the
     // row kernel of the same field
@@ -313,9 +293,13 @@ struct FocusParams {
     // always passes 1 | 4.  It stays a run-time value: folding it into constants changes the code ptxas makes for the
     // two kernels, and that code measured 0.5-0.6 % slower at N = 2048 (H100 SXM, 700 W)
     int hints;
-    // v2 column kernel launched as a programmatic dependent of the previous field's row kernel: 1 = its input does not
+    // column kernel launched as a programmatic dependent of the previous field's row kernel: 1 = its input does not
     // overlap what that kernel writes, so the kernel waits for it at its end; 0 = wait first
     int early_input;
+    // Never read.  Without these 40 bytes (or with only 32 of them) ptxas schedules both kernels differently from the
+    // code they were tuned as -- other register counts, 24 fewer instructions in the row kernel at N = 2048 -- and their
+    // speed moves with changes of that kind (hints, above)
+    long long unused[5];
 };
 
 template <int L> struct Geo2 {
@@ -327,13 +311,13 @@ template <int L> struct Geo2 {
     static constexpr int NBOX_ROW = TILES / BOXT;
 };
 
-// Column kernel of the v2 pipeline.  One CTA per SM, 16 compute warps + 1 producer warp:
+// Column kernel of the focus pair.  One CTA per SM, 16 compute warps + 1 producer warp:
 //   * two independent 256-thread GROUPS (named barriers, own exchange buffers): group h computes half-transform h
 //     (h = 0: FFT_N(x) -> plane 0; h = 1: FFT_N(x w_K^n) (-dir i) -> plane 1) of the CTA's 4-column tiles.  A thread's
 //     two packed lanes are two ADJACENT COLUMNS, so both lanes use the same twiddle, the tile image is read with
 //     128-bit shared-memory loads and the tile-major stores are float4 (two columns): four full 128-byte lines per
 //     warp instruction.  The groups drift apart by up to one tile, so the exchange phases of one overlap the butterfly
-//     phases of the other (the v1 column kernel ran one 16-warp line group in lock step: FP32 pipe 25 %).
+//     phases of the other (one 16-warp line group in lock step kept the FP32 pipe at 25 %).
 //   * the 4-column x L-row input tile (64 KB) is gathered ONCE for both halves by tensor TMA (box = 4 columns x 256
 //     rows) into a staging area of its own; the last of the 16 warps to have the inputs of tile i in registers (a
 //     shared-memory counter) requests tile i+1 on the spot -- most of a tile time of lead (the gather of 2048 32-byte
@@ -397,7 +381,7 @@ __device__ __forceinline__ void fft_two_stages_u(P2 (&v)[16], const int t, float
     sync();
 }
 
-// Row kernel of the v2 pipeline: ONE 512-thread CTA per SM = four independent 128-thread line groups (named barriers, own
+// Row kernel of the focus pair: ONE 512-thread CTA per SM = four independent 128-thread line groups (named barriers, own
 // exchange buffer, own row buffer and mbarrier) that share the float2 twiddle plan of the column kernel in shared memory.
 // Against three 128-thread CTAs with the float4 plan in L1: 16 instead of 12 warps per SM, stage-1 twiddles are 64-bit
 // shared-memory loads (lane B's twiddle = lane A's times the per-thread constant w_2L^t, four scalar FP32 operations)
@@ -425,24 +409,26 @@ template <class K> int set_smem_attrs(Handle* h, K kernel, size_t smem, int ctas
     return PB_OK;
 }
 
-// column-kernel plan of the v2 pipeline: float2 entries, one twiddle for both lanes (see Geo4)
+// exp(-2 pi i num/den) in fp64, the argument reduced exactly: an entry of the host-built plans below
+inline std::complex<double> host_tw(long long num, long long den) {
+    num %= den;
+    const double a = -2.0 * 3.14159265358979323846 * (double)num / (double)den;
+    return std::complex<double>(cos(a), sin(a));
+}
+
+// column- and row-kernel plan of the focus pair: float2 entries, one twiddle for both lanes (see Geo4)
 template <int L>
 int get_col4_plan(Handle* h, const float2** out) {
     using G4 = Geo4<L>;
     using G = Geo<L>;
-    TwKey key{L, PB_C64, 13};
+    const TwKey key{L, PB_C64, TW_FOCUS_PLAN};
     auto it = h->tables.find(key);
     if (it != h->tables.end()) { *out = reinterpret_cast<const float2*>(it->second); return PB_OK; }
     std::vector<std::complex<double>> tab(G4::PLANLEN);
-    auto w = [&](long long num, long long den) {  // exp(-2 pi i num/den), argument reduced exactly
-        num %= den;
-        const double a = -2.0 * 3.14159265358979323846 * (double)num / (double)den;
-        return std::complex<double>(cos(a), sin(a));
-    };
     for (int k = 0; k < 16; ++k)
-        for (int t = 0; t < G::NT; ++t) tab[G4::TW1 + k * G::NT + t] = w((long long)t * k, L);
+        for (int t = 0; t < G::NT; ++t) tab[G4::TW1 + k * G::NT + t] = host_tw((long long)t * k, L);
     for (int k = 1; k < 16; ++k)
-        for (int m = 0; m < G::NT / 16; ++m) tab[G4::TW2 + (k - 1) * (G::NT / 16) + m] = w(16LL * m * k, L);
+        for (int m = 0; m < G::NT / 16; ++m) tab[G4::TW2 + (k - 1) * (G::NT / 16) + m] = host_tw(16LL * m * k, L);
     const void* d = nullptr;
     PB_TRY(upload_table(h, key, tab, &d));
     *out = reinterpret_cast<const float2*>(d);

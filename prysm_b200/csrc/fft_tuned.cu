@@ -10,23 +10,35 @@
 // data, the shifts are sign patterns / index rotations at the store, and no zero is ever read,
 // written or multiplied.
 //
-// Two-lane arithmetic.  Each thread carries BOTH half-transforms of its line in structure-of-arrays form --
-// re = (re_A, re_B), im = (im_A, im_B) -- and every butterfly, twiddle multiply and store acts on the pair (add2 /
-// mul2 / fma2 in fft_engine.cuh): one set of index arithmetic, shared-memory addressing and twiddle loads serves two
-// transforms.  The two lanes differ only in their inputs (lane B = x * w_32^n, immediates) and in the stage-1 twiddle
-// (w_K^t folded into lane B's table entry).
+// Two-lane arithmetic.  Each thread carries two transforms in structure-of-arrays form -- re = (re_A, re_B),
+// im = (im_A, im_B) -- and every butterfly, twiddle multiply and store acts on the pair (add2 / mul2 / fma2 in
+// fft_engine.cuh): one set of index arithmetic, shared-memory addressing and twiddle loads serves two transforms.
 //
-// Data flow (columns first so that the K x K output is written by the row kernel in full rows with
-// 128-bit stores):
-//   focus_col_kernel : FFT_N down T adjacent columns of the pupil, both halves ->
-//                      intermediate [2][N][N] (plane p, row j  <->  output row 2j+p, rotated by K/2)
-//   focus_row_kernel : persistent; per intermediate row both half-transforms; thread owns outputs
-//                      (2j, 2j+1) and stores them as one float4.  Rows arrive by bulk async copy
-//                      (cp.async.bulk + mbarrier), one row ahead.
-//   HBM traffic: pupil 8N^2 once, output 8K^2 once; the 16N^2-byte intermediate (64 MiB at N = 2048) is written and
-//   re-read through L2 where it fits (N <= 1024 on the H100's 50 MB).  At N = 2048 the v2 pair below keeps its plane 0
-//   and the first 2 MiB of plane 1 in L2 and discards them after the read: only the rest of plane 1 (30 MiB) makes the
-//   trip through HBM.
+// Data flow (columns first so that the K x K output is written by the row kernel in full rows with 128-bit stores),
+// one field per launch pair:
+//   focus_col4_kernel : persistent, one 512-thread CTA per SM walking the 4-column tiles of the field.  Each tile comes
+//                       in by tensor TMA (box = 4 columns x 256 rows, 32-byte runs gathered into a contiguous [row][4]
+//                       image); a thread's two lanes are two adjacent columns, and group h of the CTA computes half h
+//                       (h = 1 multiplies the input ramp w_K^n in: w_32^(n/NT) as immediates, w_2L^t per thread).
+//                       Output: the intermediate [2][N][N] (plane p, row j  <->  output row 2j+p, rotated by K/2),
+//                       TILE-MAJOR: [plane p][j / 4][column tile = col / 4][j % 4][col % 4] complex64, i.e. the 4 x 4
+//                       block (4 output rows of one plane, 4 adjacent columns) is one 128-byte line and a warp stores
+//                       two full lines per instruction.
+//   focus_row4_kernel : persistent, four line groups per CTA (GeoR4); each intermediate row (512 runs of 32 bytes, 128
+//                       bytes apart) is gathered by two tensor-TMA boxes, one row ahead; per row both half-transforms,
+//                       lanes A and B, whose stage-1 twiddles differ by the per-thread w_2L^t; a thread owns outputs
+//                       (2j, 2j+1) and stores them as one float4.
+// Inputs tensor TMA cannot gather -- the fused phase-screen input PB_IN_AMP_OPD, a complex input with an odd pitch or a
+// base off 16-byte alignment -- are first written, one field at a time, as a dense aligned N x N field in scratch slot 1
+// (the phase-screen kernel of elementwise.cu, or one cudaMemcpy2DAsync) and then take the same pair.
+//
+// HBM traffic at N = 2048: pupil 8N^2 once, output 8K^2 once.  Plane 0 of the 16N^2-byte intermediate (the even output
+// rows, 32 MiB) stays in L2: the column kernel writes it evict_last, the row kernel reads it first and then discards each
+// line (discard.global.L2), so it never reaches HBM in either direction.  So do the first kPlane1KeepBytes of plane 1,
+// which the row kernel reads next; the rest of plane 1 (30 MiB) is written evict_first and makes the trip.  A staged
+// input adds the staging pass: its source read once and 8N^2 written.  The fields of a stack alternate between two
+// intermediates, so that the column kernel of field f + 1 runs under the tail of field f's row kernel instead of
+// waiting for it (focus_col4_kernel).
 //
 // FFT_N engine: N/16 threads per line, 16 points x 2 lanes per thread in registers, radix
 // 16 x 16 x N/256, two shared-memory exchanges of float4 (1-in-16 padded, conflict free).
@@ -34,172 +46,6 @@
 
 namespace pb {
 namespace {
-
-
-// ---- column pass: both half-transforms down T adjacent columns -------------------------------------
-template <int L, bool INV, int T>
-__global__ void __launch_bounds__(T * L / 16) focus_col_kernel(const FocusParams p) {
-    using G = Geo<L>;
-    extern __shared__ __align__(128) float4 smem4[];
-    float4* plan_s = smem4 + T * (G::SBUF + 2);                       // the twiddle plan, bulk-copied once
-    uint64_t* bar = reinterpret_cast<uint64_t*>(plan_s + G::PLAN);
-    const int c = threadIdx.x % T, t = threadIdx.x / T;
-    const int col = blockIdx.x * T + c;
-    const long long fb = blockIdx.y;                                   // field of the batch
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        mbar_fence_init();
-        mbar_expect_tx(bar, G::PLAN * sizeof(float4));
-        bulk_g2s(plan_s, p.plan, G::PLAN * sizeof(float4), bar);
-    }
-    __syncthreads();
-    P2 v[16];
-    float2 x[16];
-    if (p.in_kind == PB_IN_COMPLEX) {
-        const float2* __restrict__ src = reinterpret_cast<const float2*>(p.in) + fb * p.in_bs + col + (long long)t * p.in_ld;
-        const long long step = (long long)G::NT * p.in_ld;
-#pragma unroll
-        for (int n = 0; n < 16; ++n) x[n] = ld_stream(src + n * step);
-    } else {
-        const float* __restrict__ opd = reinterpret_cast<const float*>(p.in) + fb * p.in_bs + col;
-        const long long ab = fb * p.amp_bs + col;
-#pragma unroll
-        for (int n = 0; n < 16; ++n) {
-            const long long off = (long long)(n * G::NT + t) * p.in_ld;
-            float a = 1.0f;
-            if (p.amp_kind == PB_AMP_REAL) a = __ldg(reinterpret_cast<const float*>(p.amp) + ab + off);
-            else if (p.amp_kind == PB_AMP_U8) a = __ldg(reinterpret_cast<const unsigned char*>(p.amp) + ab + off) ? 1.0f : 0.0f;
-            float2 e = make_float2(0.f, 0.f);
-            if (a != 0.0f) {
-                e = expi_turns(p.kturns * (double)__ldg(opd + off), 0.0f);
-                e.x *= a; e.y *= a;
-            }
-            x[n] = e;
-        }
-    }
-#define PB_X(n) x[n]
-    PB_MAKE_LANES_16(v, INV, PB_X)
-#undef PB_X
-    float4* S = smem4 + c * (G::SBUF + 2);  // +2: skews the T buffers across banks
-    mbar_wait(bar, 0);
-    fft_two_stages<L, INV, 1>(v, t, S, plan_s + G::TW1, plan_s + G::TW2, SyncCta(), SyncCta());
-    fft_last_stage_load<L, INV>(v, t, S);
-#pragma unroll
-    for (int g = 0; g < G::GI; ++g) dftR<G::R3, INV>(v + g * G::R3);
-    // (-dir*i)^k with k = 2j + lane; j = t + g*NT + 256*kk has the parity of t
-    const float sgn = (t & 1) ? -1.0f : 1.0f;
-    float2* __restrict__ dA = p.tmp + fb * (2LL * L * L) + col + (long long)t * L;
-    float2* __restrict__ dB = dA + (long long)L * L;
-#pragma unroll
-    for (int g = 0; g < G::GI; ++g)
-#pragma unroll
-        for (int kk = 0; kk < G::R3; ++kk) {
-            const P2 y = v[g * G::R3 + kk];
-            const long long o = (long long)(g * G::NT + 256 * kk) * L;
-            st_stream(dA + o, make_float2(sgn * y.re.x, sgn * y.im.x));
-            // lane B times (-dir*i): forward (+i): (-im, re); inverse (-i): (im, -re)
-            st_stream(dB + o, INV ? make_float2(sgn * y.im.y, -sgn * y.re.y) : make_float2(-sgn * y.im.y, sgn * y.re.y));
-        }
-}
-
-// ---- row pass: persistent, both half-transforms of one intermediate row per iteration ---------------
-template <int L, bool INV>
-__global__ void __launch_bounds__(L / 16) focus_row_kernel(const FocusParams p) {
-    using G = Geo<L>;
-    constexpr int NT = G::NT, R3 = G::R3, GI = G::GI;
-    constexpr uint32_t ROW_BYTES = L * sizeof(float2);
-    extern __shared__ __align__(128) unsigned char smraw[];
-    float4* S = reinterpret_cast<float4*>(smraw);                // SBUF exchange
-    float2* inb = reinterpret_cast<float2*>(S + G::SBUF);        // L-element input row
-    uint64_t* bar = reinterpret_cast<uint64_t*>(inb + L);        // 1 mbarrier
-    const int t = threadIdx.x;
-    int r = blockIdx.x;
-    if (t == 0) {
-        mbar_init(bar, 1);
-        mbar_fence_init();
-        if (r < p.nrows) {
-            mbar_expect_tx(bar, ROW_BYTES);
-            bulk_g2s(inb, p.tmp + (long long)r * L, ROW_BYTES, bar);
-        }
-    }
-    __syncthreads();
-    const float sgn = ((t & 1) ? -1.0f : 1.0f) * p.scale;
-    for (int it = 0; r < p.nrows; ++it, r += gridDim.x) {
-        P2 v[16];
-        mbar_wait(bar, it & 1);
-        {
-            const float2* __restrict__ row = inb + t;
-#define PB_X(n) row[(n) * NT]
-            PB_MAKE_LANES_16(v, INV, PB_X)
-#undef PB_X
-        }
-        const int rn = r + gridDim.x;
-        auto sync_and_prefetch = [&]() {
-            __syncthreads();  // every thread holds its inputs in registers: the row buffer is free
-            if (t == 0 && rn < p.nrows) {
-                mbar_expect_tx(bar, ROW_BYTES);
-                bulk_g2s(inb, p.tmp + (long long)rn * L, ROW_BYTES, bar);
-            }
-        };
-        fft_two_stages<L, INV, 0>(v, t, S, p.plan + G::TW1, p.plan + G::TW2, sync_and_prefetch, SyncCta());
-        fft_last_stage_load<L, INV>(v, t, S);
-        __syncthreads();  // exchange buffer is free for the next row
-#pragma unroll
-        for (int g = 0; g < GI; ++g) dftR<R3, INV>(v + g * R3);
-        const int fb = r / (2 * L), rf = r - fb * (2 * L);   // field of the batch, row within its [2][L] planes
-        const int phs = rf / L, rr = rf - phs * L;
-        const int orow = (2 * rr + phs + L) & (2 * L - 1);  // fftshift along y
-        if (p.out_kind == PB_OUT_COMPLEX) {
-            float4* __restrict__ dst = reinterpret_cast<float4*>(reinterpret_cast<float2*>(p.out) + fb * p.out_bs + (long long)orow * p.out_ld);
-#pragma unroll
-            for (int g = 0; g < GI; ++g)
-#pragma unroll
-                for (int kk = 0; kk < R3; ++kk) {
-                    const int j = t + g * NT + 256 * kk;
-                    const P2 y = v[g * R3 + kk];
-                    // U[2j] = (-1)^j A,  U[2j+1] = (-1)^j (-dir*i) B ; fftshift along x: pair index (j + L/2) mod L
-                    const float4 o = INV ? make_float4(sgn * y.re.x, sgn * y.im.x, sgn * y.im.y, -sgn * y.re.y)
-                                         : make_float4(sgn * y.re.x, sgn * y.im.x, -sgn * y.im.y, sgn * y.re.y);
-                    st_stream(dst + ((j + L / 2) & (L - 1)), o);
-                }
-        } else {
-            float2* __restrict__ dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + fb * p.out_bs + (long long)orow * p.out_ld);
-            const float2 s2 = make_float2(p.scale * p.scale, p.scale * p.scale);
-            const float2 wgt = make_float2(p.weight, p.weight);
-#pragma unroll
-            for (int g = 0; g < GI; ++g)
-#pragma unroll
-                for (int kk = 0; kk < R3; ++kk) {
-                    const int j = t + g * NT + 256 * kk;
-                    const P2 y = v[g * R3 + kk];
-                    float2 I = mul2(s2, fma2(y.re, y.re, mul2(y.im, y.im)));
-                    float2* q = dst + ((j + L / 2) & (L - 1));
-                    if (p.out_kind == PB_OUT_ACCUMULATE) I = fma2(wgt, I, *q);
-                    *q = I;
-                }
-        }
-    }
-}
-
-// =====================================================================================================
-// v2 pipeline: same arithmetic, different traffic.
-//   * The intermediate is TILE-MAJOR: [field][plane p][j / 4][column tile = col / 4][j % 4][col % 4] complex64, i.e. the
-//     4 x 4 block (4 output rows of one plane, 4 adjacent columns) is one 128-byte line.  A warp of the column kernel
-//     (8 consecutive j x 4 columns) stores two full lines per instruction instead of eight 32-byte sectors in eight
-//     lines -- the LSU pressure (`lg_throttle`) of the row-major layout is gone.
-//   * The column kernel is persistent (one 512-thread CTA per SM walks the tiles of the field) and takes
-//     its 4-column input tile by tensor TMA (box = 4 columns x 256 rows, 32-byte runs gathered into a contiguous
-//     [row][4] image that aliases the exchange buffers); the tile after next is requested as soon as the exchange
-//     buffers are free, so it lands while the last butterflies and the stores of the current tile run.
-//   * The row kernel (four line groups per CTA, see GeoR4) gathers each intermediate row (512 runs of 32 bytes, 128 bytes
-//     apart) with two tensor-TMA boxes into a contiguous row buffer; the arithmetic after that is the v1 row kernel's.
-//   * One field per launch pair, and plane 0 of its intermediate (the even output rows, 8 N^2 bytes = 32 MiB at N = 2048)
-//     stays in L2: the column kernel writes it evict_last, the row kernel reads it first and then discards each line
-//     (discard.global.L2), so it never reaches HBM in either direction.  So do the first kPlane1KeepBytes of plane 1,
-//     which the row kernel reads next; the rest of plane 1 is written evict_first and makes the trip.
-//   * The fields of a stack alternate between two intermediates, so that the column kernel of field f + 1 runs under the
-//     tail of field f's row kernel instead of waiting for it (focus_col4_kernel).
-// =====================================================================================================
 
 // share of plane 0's lines written evict_last (the rest evict_first): what the H100's 50 MB L2 keeps next to the
 // streaming input and plane 1
@@ -511,61 +357,6 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
 }
 
 
-// plan table, see Geo<L>
-template <int L>
-int get_focus_plan(Handle* h, const float4** out) {
-    using G = Geo<L>;
-    TwKey key{L, PB_C64, 11};
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) { *out = reinterpret_cast<const float4*>(it->second); return PB_OK; }
-    auto w = [&](long long num, long long den) {  // exp(-2 pi i num/den), argument reduced exactly
-        num %= den;
-        const double a = -2.0 * 3.14159265358979323846 * (double)num / (double)den;
-        return std::complex<double>(cos(a), sin(a));
-    };
-    std::vector<float4> tab(G::PLAN);
-    for (int k = 0; k < 16; ++k)
-        for (int t = 0; t < G::NT; ++t) {
-            const std::complex<double> a = w((long long)t * k, L), b = w((long long)t * (2 * k + 1), 2 * L);
-            tab[G::TW1 + k * G::NT + t] = make_float4((float)a.real(), (float)b.real(), (float)a.imag(), (float)b.imag());
-        }
-    for (int k = 1; k < 16; ++k)
-        for (int m = 0; m < G::NT / 16; ++m) {
-            const std::complex<double> a = w(16LL * m * k, L);
-            tab[G::TW2 + (k - 1) * (G::NT / 16) + m] = make_float4((float)a.real(), (float)a.real(), (float)a.imag(), (float)a.imag());
-        }
-    void* d = nullptr;
-    PB_CUDA(h, cudaMalloc(&d, tab.size() * sizeof(float4)));
-    PB_CUDA(h, cudaMemcpy(d, tab.data(), tab.size() * sizeof(float4), cudaMemcpyHostToDevice));
-    h->tables[key] = d;
-    *out = reinterpret_cast<const float4*>(d);
-    return PB_OK;
-}
-
-
-template <int L, bool INV>
-int launch_focus(Handle* h, FocusParams p, int batch, cudaStream_t st) {
-    using G = Geo<L>;
-    constexpr int T = 4;
-    const size_t smem_col = (size_t)(T * (G::SBUF + 2) + G::PLAN) * sizeof(float4) + 2 * sizeof(uint64_t);
-    const size_t smem_row = (size_t)G::SBUF * sizeof(float4) + (size_t)L * sizeof(float2) + 2 * sizeof(uint64_t);
-    // Resident row CTAs per SM: as many as leave >= 64 KB of the unified L1/shared array as L1 -- the 34 KB twiddle plan is
-    // re-read by every line and must hit there.  (Left to itself the driver picks the 228 KB carve-out and the plan
-    // streams from L2 at ~300 cycles a load.)
-    const size_t unified = 256 * 1024, l1_keep = 64 * 1024;
-    const int row_ctas = std::max(1, (int)((unified - l1_keep) / (smem_row + 1024)));
-    PB_TRY(set_smem_attrs(h, focus_col_kernel<L, INV, T>, smem_col, 1));
-    PB_TRY(set_smem_attrs(h, focus_row_kernel<L, INV>, smem_row, row_ctas));
-    PB_TRY(get_focus_plan<L>(h, &p.plan));
-    p.nrows = batch * 2 * L;
-    focus_col_kernel<L, INV, T><<<dim3(L / T, batch), T * G::NT, smem_col, st>>>(p);
-    PB_LAUNCH_CHECK(h);
-    focus_row_kernel<L, INV><<<std::min(h->sm_count * row_ctas, p.nrows), L / 16, smem_row, st>>>(p);
-    PB_LAUNCH_CHECK(h);
-    h->route_launches[route_code(PB_ROUTE_FOCUS_V1, L, INV)] += 2;
-    return PB_OK;
-}
-
 // ---- TMA descriptors, cached in the handle by (base pointer, geometry) -----------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -607,9 +398,7 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     // its plan in shared memory, so it has no L1 working set to protect
     PB_TRY(set_smem_attrs(h, focus_col4_kernel<L, INV>, G4::SMEM, 1));
     PB_TRY(set_smem_attrs(h, focus_row4_kernel<L, INV>, R4::SMEM, 1));
-    const float2* plan = nullptr;
-    PB_TRY(get_col4_plan<L>(h, &plan));
-    p.plan = reinterpret_cast<const float4*>(plan);
+    PB_TRY(get_col4_plan<L>(h, &p.plan));
     p.nrows = 2 * L;
     p.ntiles = G2::TILES;
     p.hints = 1 | 4;   // eviction hints, plane 0 and the head of plane 1 kept in L2 (FocusParams::hints)
@@ -635,7 +424,8 @@ int launch_focus2(Handle* h, FocusParams p, int col_dep, cudaStream_t st) {
     // prologue (barriers, plan) while that wave finishes; griddepcontrol.wait orders everything that depends on the
     // previous kernel.  A column kernel with `early_input` writes the other intermediate buffer than the row kernel it
     // follows and runs its whole pass under that kernel's tail, waiting only at its end (focus_col4_kernel).  The column
-    // kernel of the first field of a call is launched plainly: what precedes it is not known.
+    // kernel of the first field of a call is launched plainly: what precedes it is not known.  So is that of a staged field:
+    // it follows its staging launch.
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr.val.programmaticStreamSerializationAllowed = 1;
@@ -777,7 +567,7 @@ __global__ void __launch_bounds__((COLS ? TP : 1) * L / 16, (RT && (!COLS || TP 
     // TP interleaved lines per CTA: consecutive exchange buffers are offset by 32 / TP banks (8 / TP float4 of padding), so
     // that the 8 threads of a 128-bit wavefront (8 / TP consecutive t  x  TP lines) cover all 32 banks
     float4* S = smem4 + c * (G::SBUF + 8 / (COLS ? TP : 1) % 8);
-    fft_two_stages<L, INV, 2>(v, t, S, tw1, tw2, SyncCta(), SyncCta());
+    fft_two_stages<L, INV>(v, t, S, tw1, tw2);
     fft_last_stage_load<L, INV>(v, t, S);
 #pragma unroll
     for (int g = 0; g < G::GI; ++g) dftR<G::R3, INV>(v + g * G::R3);
@@ -805,7 +595,7 @@ __global__ void __launch_bounds__((COLS ? TP : 1) * L / 16, (RT && (!COLS || TP 
                 w[g + G::GI * kk] = {make_float2(ya.x, yb.x), make_float2(ya.y, yb.y)};
             }
         __syncthreads();   // all last-stage reads of S are done before the inverse pass overwrites it
-        fft_two_stages<L, !INV, 2>(w, t, S, tw1, tw2, SyncCta(), SyncCta());
+        fft_two_stages<L, !INV>(w, t, S, tw1, tw2);
         fft_last_stage_load<L, !INV>(w, t, S);
 #pragma unroll
         for (int g = 0; g < G::GI; ++g) dftR<G::R3, !INV>(w + g * G::R3);
@@ -927,21 +717,16 @@ __global__ void __launch_bounds__((COLS ? TP : 1) * L / 16, (RT && (!COLS || TP 
 template <int L>
 int get_plain_plan(Handle* h, const float2** tw1, const float2** tw2) {
     using G = Geo<L>;
-    TwKey key{L, PB_C64, 12};
+    const TwKey key{L, PB_C64, TW_PLAIN_PLAN};
     const float2* base = nullptr;
     auto it = h->tables.find(key);
     if (it != h->tables.end()) base = reinterpret_cast<const float2*>(it->second);
     else {
         std::vector<std::complex<double>> tab(15 * G::NT + 15 * (G::NT / 16));
-        auto w = [&](long long num, long long den) {
-            num %= den;
-            const double a = -2.0 * 3.14159265358979323846 * (double)num / (double)den;
-            return std::complex<double>(cos(a), sin(a));
-        };
         for (int k = 1; k < 16; ++k)
-            for (int t = 0; t < G::NT; ++t) tab[(k - 1) * G::NT + t] = w((long long)t * k, L);
+            for (int t = 0; t < G::NT; ++t) tab[(k - 1) * G::NT + t] = host_tw((long long)t * k, L);
         for (int k = 1; k < 16; ++k)
-            for (int m = 0; m < G::NT / 16; ++m) tab[15 * G::NT + (k - 1) * (G::NT / 16) + m] = w(16LL * m * k, L);
+            for (int m = 0; m < G::NT / 16; ++m) tab[15 * G::NT + (k - 1) * (G::NT / 16) + m] = host_tw(16LL * m * k, L);
         const void* d = nullptr;
         PB_TRY(upload_table(h, key, tab, &d));
         base = reinterpret_cast<const float2*>(d);
@@ -958,7 +743,9 @@ int launch_axis_reg(Handle* h, const AxisPass& p, cudaStream_t st) {
     const size_t smem = (size_t)TP * (G::SBUF + 8 / TP % 8) * sizeof(float4);
     if (attr_needed(h, reinterpret_cast<const void*>(axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>))) {
         PB_CUDA(h, cudaFuncSetAttribute(axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        // keep >= 64 KB of L1 for the twiddle tables (see launch_focus)
+        // Resident CTAs per SM: as many as leave >= 64 KB of the unified L1/shared array as L1 -- the twiddle tables are
+        // re-read by every line and must hit there.  (Left to itself the driver picks the 228 KB carve-out and the tables
+        // stream from L2 at ~300 cycles a load.)
         const size_t unified = 256 * 1024, l1_keep = 64 * 1024;
         const int ctas = std::max<int>(1, (int)((unified - l1_keep) / (smem + 1024)));
         const int pct = (int)std::min<size_t>(100, ((size_t)ctas * (smem + 1024) * 100 + h->max_smem_optin - 1) / h->max_smem_optin);
@@ -1041,56 +828,57 @@ int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, cons
     if (out_kind == PB_OUT_COMPLEX ? (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 15) : (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 7))
         return PB_ERR_UNSUPPORTED;  // vector stores need aligned rows
     const int N = nx;
-    // Inputs tensor TMA can gather (complex, 16-byte aligned base, even pitches) run the tile-major pair (v2), one field
-    // per launch pair, so that the plane 0 its column pass leaves in L2 is what its row pass reads first.  Everything else
-    // (the fused phase-screen input, odd pitches, misaligned bases) runs the v1 pair, up to 8 fields per launch pair,
-    // which evens out the tails of the two grids.
-    const bool tma_ok = in_kind == PB_IN_COMPLEX && !((uintptr_t)in & 15) && !(in_ld & 1) && !(in_bs & 1);
-    // v2 stacks alternate between two intermediates (field f: buffer f mod 2), so that a column kernel never writes what
-    // the row kernel before it reads (focus_col4_kernel)
-    const int per = tma_ok ? 1 : std::min(batch, 8);
-    const int nbuf = tma_ok && batch > 1 ? 2 : 1;
-    const size_t buf_bytes = (size_t)per * 2 * N * N * sizeof(float2);
+    // Inputs tensor TMA can gather (complex, 16-byte aligned base, even pitches) go to the pair as they are; every other
+    // one is first written as a dense aligned field in scratch slot 1, one field at a time
+    const bool staged = in_kind != PB_IN_COMPLEX || ((uintptr_t)in & 15) || (in_ld & 1) || (in_bs & 1);
+    // the fields of a stack alternate between two intermediates (field f: buffer f mod 2), so that a column kernel never
+    // writes what the row kernel before it reads (focus_col4_kernel)
+    const int nbuf = batch > 1 ? 2 : 1;
+    const size_t field_bytes = (size_t)N * N * sizeof(float2);
     void* tmp = nullptr;
-    PB_TRY(ensure_scratch(h, 0, nbuf * buf_bytes, &tmp));
+    PB_TRY(ensure_scratch(h, 0, nbuf * 2 * field_bytes, &tmp));
+    void* stage = nullptr;
+    if (staged) PB_TRY(ensure_scratch(h, 1, field_bytes, &stage));
     // the column kernels' tile counters, one per buffer: zeroed once here, then by each field's row kernel
-    unsigned int* ctr = nullptr;
-    if (tma_ok) {
-        const TwKey key{2, PB_C64, 14};
-        auto it = h->tables.find(key);
-        const void* d = it != h->tables.end() ? it->second : nullptr;
-        if (!d) PB_TRY(upload_table(h, key, std::vector<std::complex<double>>(1), &d));   // one complex64 zero = two counters
-        ctr = reinterpret_cast<unsigned int*>(const_cast<void*>(d));
-    }
+    const TwKey key{2, PB_C64, TW_TILE_COUNTERS};
+    auto it = h->tables.find(key);
+    const void* d = it != h->tables.end() ? it->second : nullptr;
+    if (!d) PB_TRY(upload_table(h, key, std::vector<std::complex<double>>(1), &d));   // one complex64 zero = two counters
+    unsigned int* ctr = reinterpret_cast<unsigned int*>(const_cast<void*>(d));
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
     const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : sizeof(float);
     const size_t out_elt = out_kind == PB_OUT_COMPLEX ? sizeof(float2) : sizeof(float);
-    // v2, fields after the first: the column kernel follows this call's previous row kernel (programmatic dependent
-    // launch, see launch_focus2); it may gather its input early unless the input stack overlaps the output stack
+    // fields after the first of an unstaged stack: the column kernel follows this call's previous row kernel
+    // (programmatic dependent launch, see launch_focus2); it may gather its input early unless the input stack overlaps
+    // the output stack.  A staged field's column kernel is launched plainly, after its staging launch, which is plain too
+    // and so follows the previous field's row kernel.
     const uintptr_t in_lo = (uintptr_t)in, in_hi = in_lo + (size_t)((long long)(batch - 1) * in_bs + (long long)(ny - 1) * in_ld + nx) * in_elt;
     const uintptr_t out_lo = (uintptr_t)out, out_hi = out_lo + (size_t)((long long)(batch - 1) * out_bs + (long long)(ky - 1) * out_ld + kx) * out_elt;
-    const int col_dep_next = (in_hi <= out_lo || out_hi <= in_lo) ? 2 : 1;
-    for (int b0 = 0; b0 < batch; b0 += per) {
-        const int nb = std::min(per, batch - b0);
-        FocusParams p;
-        p.in = reinterpret_cast<const char*>(in) + (size_t)b0 * in_bs * in_elt;
-        p.in_kind = in_kind;
-        p.amp = amp ? reinterpret_cast<const char*>(amp) + (size_t)b0 * amp_bs * amp_elt : nullptr;
-        p.amp_kind = amp_kind; p.kturns = kturns; p.in_ld = in_ld;
-        p.tmp = reinterpret_cast<float2*>(reinterpret_cast<char*>(tmp) + (size_t)(b0 % nbuf) * buf_bytes);
-        p.plan = nullptr;
-        p.out = reinterpret_cast<char*>(out) + (size_t)b0 * out_bs * out_elt;
+    const int col_dep_next = staged ? 0 : (in_hi <= out_lo || out_hi <= in_lo) ? 2 : 1;
+    for (int b = 0; b < batch; ++b) {
+        FocusParams p = {};
+        p.in = reinterpret_cast<const char*>(in) + (size_t)b * in_bs * in_elt;   // (16-byte aligned if not staged: in_bs is even)
+        p.in_ld = in_ld;
+        if (staged) {
+            if (in_kind == PB_IN_AMP_OPD) {
+                const void* a = amp ? reinterpret_cast<const char*>(amp) + (size_t)b * amp_bs * amp_elt : nullptr;
+                PB_TRY(launch_phase_screen(h, PB_C64, a, amp_kind, p.in, kturns, (long long)N * N, N, in_ld, stage, st));
+            } else {
+                PB_CUDA(h, cudaMemcpy2DAsync(stage, N * sizeof(float2), p.in, in_ld * sizeof(float2), N * sizeof(float2), N,
+                                             cudaMemcpyDeviceToDevice, st));
+            }
+            p.in = stage;
+            p.in_ld = N;
+        }
+        p.tmp = reinterpret_cast<float2*>(reinterpret_cast<char*>(tmp) + (size_t)(b % nbuf) * 2 * field_bytes);
+        p.out = reinterpret_cast<char*>(out) + (size_t)b * out_bs * out_elt;
         p.out_ld = out_ld; p.out_kind = out_kind; p.scale = (float)scale; p.weight = (float)weight;
-        p.nrows = 0; p.ntiles = 0; p.hints = 0; p.early_input = 0;
-        p.tile_ctr = ctr ? ctr + (b0 % nbuf) : nullptr;
-        p.in_bs = in_bs; p.amp_bs = amp_bs; p.out_bs = out_bs;
+        p.out_bs = out_bs;
+        p.tile_ctr = ctr + (b % nbuf);
+        const int cd = b > 0 ? col_dep_next : 0;
         int rc;
-        if (tma_ok) {   // (the field offset keeps p.in 16-byte aligned: in_bs is even)
-            const int cd = b0 > 0 ? col_dep_next : 0;
-            if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
-            else rc = N == 512 ? launch_focus2<512, true>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, true>(h, p, cd, st) : launch_focus2<2048, true>(h, p, cd, st);
-        } else if (dir < 0) rc = N == 512 ? launch_focus<512, false>(h, p, nb, st) : N == 1024 ? launch_focus<1024, false>(h, p, nb, st) : launch_focus<2048, false>(h, p, nb, st);
-        else rc = N == 512 ? launch_focus<512, true>(h, p, nb, st) : N == 1024 ? launch_focus<1024, true>(h, p, nb, st) : launch_focus<2048, true>(h, p, nb, st);
+        if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
+        else rc = N == 512 ? launch_focus2<512, true>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, true>(h, p, cd, st) : launch_focus2<2048, true>(h, p, cd, st);
         if (rc != PB_OK) return rc;
     }
     return PB_OK;

@@ -16,7 +16,7 @@ field of the stack.
 
 Bounds are 1.5x the figures measured on an H100 (`MEASURED`, recorded with PB_TEST_MEASUREMENTS; the arithmetic is
 deterministic, so the figures repeat bit for bit) and never above the north-star 1e-6.  Ranges of the measured figures,
-H100 80GB HBM3 at a 400 W power limit:
+H100 80GB HBM3 at a 400 W power limit (the staged_* cases at 700 W):
 
     axis angular_spectrum              linf 2.4e-07-3.3e-07, l2 2.6e-07-3.1e-07
     axis angular_spectrum_adjoint      linf 2.7e-07-3.7e-07, l2 2.7e-07-3.1e-07
@@ -33,19 +33,19 @@ H100 80GB HBM3 at a 400 W power limit:
     axis ifft2_rows                    linf 1.5e-07-2.3e-07, l2 1.2e-07-1.7e-07
     axis screened_free_space           linf 2.4e-07-3.5e-07, l2 2.7e-07-3.1e-07
     axis unfocus_adjoint               linf 2.0e-07-2.3e-07, l2 1.7e-07-1.9e-07
-    v1 pair, N = 1024                  linf 2.2e-07-4.3e-07, l2 9.1e-08-2.5e-07, rows 2.0e-07-4.3e-07
-    v1 pair, N = 2048                  linf 6.4e-08-3.2e-07, l2 9.4e-08-2.6e-07, rows 3.0e-08-3.2e-07
-    v1 pair, N = 512                   linf 8.6e-08-3.2e-07, l2 9.0e-08-2.5e-07, rows 6.4e-08-3.2e-07
-    v2 pair, N = 1024                  linf 1.7e-07-4.4e-07, l2 8.6e-08-2.6e-07, rows 1.7e-07-4.4e-07
-    v2 pair, N = 2048                  linf 1.9e-07-4.9e-07, l2 9.3e-08-2.7e-07, rows 1.8e-07-4.9e-07
-    v2 pair, N = 512                   linf 1.7e-07-4.9e-07, l2 8.8e-08-2.5e-07, rows 1.7e-07-4.9e-07
+    focus pair, N = 1024               linf 1.7e-07-4.4e-07, l2 8.6e-08-2.6e-07, rows 1.7e-07-4.4e-07
+    focus pair, N = 2048               linf 6.3e-08-4.9e-07, l2 9.3e-08-2.7e-07, rows 3.7e-08-4.9e-07
+    focus pair, N = 512                linf 8.6e-08-4.9e-07, l2 8.8e-08-2.5e-07, rows 4.2e-08-4.9e-07
     (rows: the per-row-class figures; a centred impulse focuses exactly, figure 0)
 
+Inputs tensor TMA cannot gather (a misaligned base, an odd row or field pitch, the fused phase-screen input) are staged
+field by field into a dense aligned buffer and take the same pair; those cases are named `staged_*`.
+
 Every case also shows that it ran the kernel it is about, from the library's per-route launch counters
-(pb_route_launch_count): a focus case launches exactly the kernels of its pair (v1 or v2, N, direction) -- two per field
-for v2, two per chunk of <= 8 fields for v1 -- and nothing else; an axis case runs the `axis_reg_kernel<L, INV, COLS, TP,
-RT, PM, DENSE>` instantiations it names, no other route, and nothing outside EXPECTED.  The last test asserts that every
-instantiation the Python API can reach was hit by a case here.
+(pb_route_launch_count): a focus case launches exactly the kernels of the pair of its N and direction -- two per field
+-- and nothing else but one phase-screen launch per staged phase-screen field (a staging copy is not a launch); an axis
+case runs the `axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>` instantiations it names, no other route, and nothing
+outside EXPECTED.  The last test asserts that every instantiation the Python API can reach was hit by a case here.
 """
 import ctypes as C
 import math
@@ -159,86 +159,86 @@ MEASURED = {
     'axis/unfocus_adjoint_q2/1024': dict(linf=2.00e-7, l2=1.67e-7),
     'axis/unfocus_adjoint_q2/2048': dict(linf=2.28e-7, l2=1.75e-7),
     'axis/unfocus_adjoint_q2/4096': dict(linf=2.33e-7, l2=1.91e-7),
-    'v1/1024/+1/accumulate/misaligned': dict(linf=3.31e-7, l2=9.11e-8, plane0=3.05e-7, plane1=3.31e-7),
-    'v1/1024/+1/complex/misaligned': dict(linf=2.17e-7, l2=1.80e-7, plane0=2.04e-7, plane1=2.17e-7),
-    'v1/1024/+1/intensity/misaligned': dict(linf=4.26e-7, l2=2.53e-7, plane0=3.53e-7, plane1=4.26e-7),
-    'v1/1024/-1/accumulate/misaligned': dict(linf=3.39e-7, l2=9.10e-8, plane0=2.79e-7, plane1=3.39e-7),
-    'v1/1024/-1/complex/misaligned': dict(linf=2.27e-7, l2=1.80e-7, plane0=2.12e-7, plane1=2.27e-7),
-    'v1/1024/-1/intensity/misaligned': dict(linf=4.26e-7, l2=2.52e-7, plane0=3.50e-7, plane1=4.26e-7),
-    'v1/2048/+1/accumulate/misaligned': dict(linf=2.55e-7, l2=9.41e-8, plane0=2.55e-7, plane1=2.45e-7),
-    'v1/2048/+1/complex/misaligned': dict(linf=2.16e-7, l2=1.88e-7, plane0=2.02e-7, plane1=2.16e-7),
-    'v1/2048/+1/complex/odd_in_bs_batch9': dict(linf=2.38e-7, l2=1.88e-7, plane0=2.38e-7, plane1=2.36e-7),
-    'v1/2048/+1/complex/odd_in_ld': dict(linf=2.16e-7, l2=1.88e-7, plane0=2.02e-7, plane1=2.16e-7),
-    'v1/2048/+1/complex/opd30_amp_none': dict(linf=6.37e-8, l2=1.60e-7, plane0=5.11e-8, plane1=6.37e-8),
-    'v1/2048/+1/intensity/misaligned': dict(linf=2.95e-7, l2=2.62e-7, plane0=2.75e-7, plane1=2.95e-7),
-    'v1/2048/-1/accumulate/misaligned': dict(linf=3.05e-7, l2=9.42e-8, plane0=2.41e-7, plane1=3.05e-7),
-    'v1/2048/-1/accumulate/opd30_amp_real_batch9': dict(linf=1.51e-7, l2=1.34e-7, plane0=1.51e-7, plane1=7.04e-8),
-    'v1/2048/-1/complex/misaligned': dict(linf=2.07e-7, l2=1.88e-7, plane0=1.93e-7, plane1=2.07e-7),
-    'v1/2048/-1/complex/odd_in_bs_batch9': dict(linf=2.38e-7, l2=1.88e-7, plane0=2.38e-7, plane1=2.36e-7),
-    'v1/2048/-1/complex/odd_in_ld': dict(linf=2.07e-7, l2=1.88e-7, plane0=1.93e-7, plane1=2.07e-7),
-    'v1/2048/-1/complex/opd1e4_amp_u8_shared_batch9': dict(linf=2.28e-7, l2=1.93e-7, plane0=2.28e-7, plane1=2.24e-7),
-    'v1/2048/-1/intensity/misaligned': dict(linf=3.19e-7, l2=2.62e-7, plane0=2.83e-7, plane1=3.19e-7),
-    'v1/512/+1/accumulate/misaligned': dict(linf=2.38e-7, l2=9.03e-8, plane0=2.03e-7, plane1=2.38e-7),
-    'v1/512/+1/complex/misaligned': dict(linf=2.21e-7, l2=1.74e-7, plane0=1.93e-7, plane1=2.21e-7),
-    'v1/512/+1/complex/odd_in_bs_batch9': dict(linf=2.34e-7, l2=1.75e-7, plane0=2.16e-7, plane1=2.34e-7),
-    'v1/512/+1/complex/odd_in_ld': dict(linf=2.21e-7, l2=1.74e-7, plane0=1.93e-7, plane1=2.21e-7),
-    'v1/512/+1/complex/opd30_amp_none': dict(linf=8.61e-8, l2=1.50e-7, plane0=8.61e-8, plane1=6.38e-8),
-    'v1/512/+1/intensity/misaligned': dict(linf=3.18e-7, l2=2.51e-7, plane0=2.70e-7, plane1=3.18e-7),
-    'v1/512/-1/accumulate/misaligned': dict(linf=3.23e-7, l2=9.06e-8, plane0=3.23e-7, plane1=2.99e-7),
-    'v1/512/-1/accumulate/opd30_amp_real_batch9': dict(linf=1.68e-7, l2=1.52e-7, plane0=1.68e-7, plane1=9.43e-8),
-    'v1/512/-1/complex/misaligned': dict(linf=2.14e-7, l2=1.75e-7, plane0=2.08e-7, plane1=2.14e-7),
-    'v1/512/-1/complex/odd_in_bs_batch9': dict(linf=2.40e-7, l2=1.75e-7, plane0=2.16e-7, plane1=2.40e-7),
-    'v1/512/-1/complex/odd_in_ld': dict(linf=2.14e-7, l2=1.75e-7, plane0=2.08e-7, plane1=2.14e-7),
-    'v1/512/-1/complex/opd1e4_amp_u8_shared_batch9': dict(linf=2.45e-7, l2=1.80e-7, plane0=2.45e-7, plane1=2.41e-7),
-    'v1/512/-1/intensity/misaligned': dict(linf=3.14e-7, l2=2.52e-7, plane0=3.14e-7, plane1=2.99e-7),
     'v2/1024/+1/accumulate/stack5': dict(linf=3.67e-7, l2=9.28e-8, plane0=2.62e-7, plane1_kept=3.22e-7, plane1_streamed=3.67e-7),
+    'v2/1024/+1/accumulate/staged_misaligned': dict(linf=3.86e-7, l2=9.28e-8, plane0=3.06e-7, plane1_kept=3.32e-7, plane1_streamed=3.86e-7),
     'v2/1024/+1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0, plane1_streamed=0.0),
     'v2/1024/+1/complex/impulse_corners': dict(linf=1.70e-7, l2=8.72e-8, plane0=1.70e-7, plane1_kept=1.70e-7, plane1_streamed=1.70e-7),
     'v2/1024/+1/complex/impulse_mix': dict(linf=2.74e-7, l2=1.13e-7, plane0=2.74e-7, plane1_kept=2.73e-7, plane1_streamed=2.73e-7),
     'v2/1024/+1/complex/stack5': dict(linf=2.55e-7, l2=1.84e-7, plane0=2.28e-7, plane1_kept=2.30e-7, plane1_streamed=2.55e-7),
+    'v2/1024/+1/complex/staged_misaligned': dict(linf=2.53e-7, l2=1.84e-7, plane0=2.05e-7, plane1_kept=2.30e-7, plane1_streamed=2.53e-7),
     'v2/1024/+1/intensity/stack5': dict(linf=4.41e-7, l2=2.58e-7, plane0=3.53e-7, plane1_kept=4.26e-7, plane1_streamed=4.41e-7),
+    'v2/1024/+1/intensity/staged_misaligned': dict(linf=4.41e-7, l2=2.58e-7, plane0=3.54e-7, plane1_kept=4.26e-7, plane1_streamed=4.41e-7),
     'v2/1024/-1/accumulate/stack5': dict(linf=3.46e-7, l2=9.27e-8, plane0=3.46e-7, plane1_kept=2.95e-7, plane1_streamed=3.26e-7),
+    'v2/1024/-1/accumulate/staged_misaligned': dict(linf=3.06e-7, l2=9.26e-8, plane0=2.69e-7, plane1_kept=3.06e-7, plane1_streamed=2.98e-7),
     'v2/1024/-1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0, plane1_streamed=0.0),
     'v2/1024/-1/complex/impulse_corners': dict(linf=1.77e-7, l2=8.56e-8, plane0=1.77e-7, plane1_kept=1.77e-7, plane1_streamed=1.77e-7),
     'v2/1024/-1/complex/impulse_mix': dict(linf=2.83e-7, l2=1.14e-7, plane0=2.75e-7, plane1_kept=2.77e-7, plane1_streamed=2.83e-7),
     'v2/1024/-1/complex/stack5': dict(linf=2.51e-7, l2=1.83e-7, plane0=2.32e-7, plane1_kept=2.19e-7, plane1_streamed=2.51e-7),
+    'v2/1024/-1/complex/staged_misaligned': dict(linf=2.51e-7, l2=1.84e-7, plane0=2.22e-7, plane1_kept=2.09e-7, plane1_streamed=2.51e-7),
     'v2/1024/-1/intensity/stack5': dict(linf=4.01e-7, l2=2.58e-7, plane0=3.84e-7, plane1_kept=3.93e-7, plane1_streamed=4.01e-7),
+    'v2/1024/-1/intensity/staged_misaligned': dict(linf=3.93e-7, l2=2.58e-7, plane0=3.70e-7, plane1_kept=3.42e-7, plane1_streamed=3.93e-7),
     'v2/2048/+1/accumulate/padded': dict(linf=3.47e-7, l2=9.54e-8, plane0=3.47e-7, plane1_kept=2.64e-7, plane1_streamed=3.47e-7),
     'v2/2048/+1/accumulate/stack5': dict(linf=3.60e-7, l2=9.54e-8, plane0=3.60e-7, plane1_kept=2.48e-7, plane1_streamed=3.44e-7),
+    'v2/2048/+1/accumulate/staged_misaligned': dict(linf=2.58e-7, l2=9.53e-8, plane0=2.55e-7, plane1_kept=1.92e-7, plane1_streamed=2.58e-7),
     'v2/2048/+1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0, plane1_streamed=0.0),
     'v2/2048/+1/complex/impulse_corners': dict(linf=2.16e-7, l2=1.01e-7, plane0=2.16e-7, plane1_kept=2.16e-7, plane1_streamed=2.16e-7),
     'v2/2048/+1/complex/impulse_mix': dict(linf=3.06e-7, l2=1.10e-7, plane0=3.06e-7, plane1_kept=2.67e-7, plane1_streamed=2.83e-7),
     'v2/2048/+1/complex/overlapping': dict(linf=2.65e-7, l2=1.91e-7, plane0=2.26e-7, plane1_kept=2.25e-7, plane1_streamed=2.65e-7),
     'v2/2048/+1/complex/single': dict(linf=2.18e-7, l2=1.91e-7, plane0=1.91e-7, plane1_kept=1.87e-7, plane1_streamed=2.18e-7),
     'v2/2048/+1/complex/stack5': dict(linf=2.65e-7, l2=1.91e-7, plane0=2.26e-7, plane1_kept=2.25e-7, plane1_streamed=2.65e-7),
+    'v2/2048/+1/complex/staged_misaligned': dict(linf=2.18e-7, l2=1.92e-7, plane0=1.92e-7, plane1_kept=1.88e-7, plane1_streamed=2.18e-7),
+    'v2/2048/+1/complex/staged_odd_in_bs_batch9': dict(linf=2.65e-7, l2=1.92e-7, plane0=2.26e-7, plane1_kept=2.25e-7, plane1_streamed=2.65e-7),
+    'v2/2048/+1/complex/staged_odd_in_ld': dict(linf=2.18e-7, l2=1.92e-7, plane0=1.92e-7, plane1_kept=1.88e-7, plane1_streamed=2.18e-7),
+    'v2/2048/+1/complex/staged_opd30_amp_none': dict(linf=6.31e-8, l2=1.63e-7, plane0=5.13e-8, plane1_kept=5.51e-8, plane1_streamed=6.31e-8),
     'v2/2048/+1/intensity/stack5': dict(linf=4.13e-7, l2=2.66e-7, plane0=4.08e-7, plane1_kept=3.25e-7, plane1_streamed=4.13e-7),
+    'v2/2048/+1/intensity/staged_misaligned': dict(linf=2.86e-7, l2=2.66e-7, plane0=2.75e-7, plane1_kept=2.15e-7, plane1_streamed=2.86e-7),
     'v2/2048/-1/accumulate/padded': dict(linf=3.80e-7, l2=9.54e-8, plane0=3.11e-7, plane1_kept=3.80e-7, plane1_streamed=3.66e-7),
     'v2/2048/-1/accumulate/stack5': dict(linf=4.06e-7, l2=9.54e-8, plane0=3.03e-7, plane1_kept=3.89e-7, plane1_streamed=4.06e-7),
+    'v2/2048/-1/accumulate/staged_misaligned': dict(linf=3.09e-7, l2=9.54e-8, plane0=2.42e-7, plane1_kept=2.13e-7, plane1_streamed=3.09e-7),
+    'v2/2048/-1/accumulate/staged_opd30_amp_real_batch9': dict(linf=1.51e-7, l2=1.34e-7, plane0=1.51e-7, plane1_kept=3.72e-8, plane1_streamed=7.05e-8),
     'v2/2048/-1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0, plane1_streamed=0.0),
     'v2/2048/-1/complex/impulse_corners': dict(linf=1.93e-7, l2=9.26e-8, plane0=1.93e-7, plane1_kept=1.93e-7, plane1_streamed=1.93e-7),
     'v2/2048/-1/complex/impulse_mix': dict(linf=3.07e-7, l2=1.12e-7, plane0=3.07e-7, plane1_kept=2.80e-7, plane1_streamed=3.06e-7),
     'v2/2048/-1/complex/overlapping': dict(linf=2.62e-7, l2=1.91e-7, plane0=2.29e-7, plane1_kept=2.54e-7, plane1_streamed=2.62e-7),
     'v2/2048/-1/complex/single': dict(linf=2.14e-7, l2=1.91e-7, plane0=1.91e-7, plane1_kept=1.78e-7, plane1_streamed=2.14e-7),
     'v2/2048/-1/complex/stack5': dict(linf=2.62e-7, l2=1.91e-7, plane0=2.29e-7, plane1_kept=2.54e-7, plane1_streamed=2.62e-7),
+    'v2/2048/-1/complex/staged_misaligned': dict(linf=2.14e-7, l2=1.92e-7, plane0=1.91e-7, plane1_kept=1.78e-7, plane1_streamed=2.14e-7),
+    'v2/2048/-1/complex/staged_odd_in_bs_batch9': dict(linf=2.62e-7, l2=1.92e-7, plane0=2.29e-7, plane1_kept=2.54e-7, plane1_streamed=2.62e-7),
+    'v2/2048/-1/complex/staged_odd_in_ld': dict(linf=2.14e-7, l2=1.92e-7, plane0=1.91e-7, plane1_kept=1.78e-7, plane1_streamed=2.14e-7),
+    'v2/2048/-1/complex/staged_opd1e4_amp_u8_shared_batch9': dict(linf=2.42e-7, l2=1.96e-7, plane0=2.42e-7, plane1_kept=2.10e-7, plane1_streamed=2.40e-7),
     'v2/2048/-1/intensity/stack5': dict(linf=4.94e-7, l2=2.66e-7, plane0=3.66e-7, plane1_kept=4.94e-7, plane1_streamed=4.75e-7),
+    'v2/2048/-1/intensity/staged_misaligned': dict(linf=3.57e-7, l2=2.66e-7, plane0=2.84e-7, plane1_kept=2.30e-7, plane1_streamed=3.57e-7),
     'v2/512/+1/accumulate/padded': dict(linf=3.30e-7, l2=9.12e-8, plane0=3.30e-7, plane1_kept=3.15e-7),
     'v2/512/+1/accumulate/stack5': dict(linf=3.38e-7, l2=9.13e-8, plane0=2.92e-7, plane1_kept=3.38e-7),
+    'v2/512/+1/accumulate/staged_misaligned': dict(linf=2.68e-7, l2=9.12e-8, plane0=2.04e-7, plane1_kept=2.68e-7),
     'v2/512/+1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0),
     'v2/512/+1/complex/impulse_corners': dict(linf=1.93e-7, l2=1.04e-7, plane0=1.93e-7, plane1_kept=1.93e-7),
     'v2/512/+1/complex/impulse_mix': dict(linf=2.96e-7, l2=1.17e-7, plane0=2.96e-7, plane1_kept=2.95e-7),
     'v2/512/+1/complex/overlapping': dict(linf=2.34e-7, l2=1.77e-7, plane0=2.19e-7, plane1_kept=2.34e-7),
     'v2/512/+1/complex/single': dict(linf=2.05e-7, l2=1.77e-7, plane0=1.93e-7, plane1_kept=2.05e-7),
     'v2/512/+1/complex/stack5': dict(linf=2.34e-7, l2=1.77e-7, plane0=2.19e-7, plane1_kept=2.34e-7),
+    'v2/512/+1/complex/staged_misaligned': dict(linf=2.05e-7, l2=1.78e-7, plane0=1.93e-7, plane1_kept=2.05e-7),
+    'v2/512/+1/complex/staged_odd_in_bs_batch9': dict(linf=2.35e-7, l2=1.78e-7, plane0=2.19e-7, plane1_kept=2.35e-7),
+    'v2/512/+1/complex/staged_odd_in_ld': dict(linf=2.05e-7, l2=1.78e-7, plane0=1.93e-7, plane1_kept=2.05e-7),
+    'v2/512/+1/complex/staged_opd30_amp_none': dict(linf=8.59e-8, l2=1.50e-7, plane0=8.59e-8, plane1_kept=4.16e-8),
     'v2/512/+1/intensity/stack5': dict(linf=3.93e-7, l2=2.54e-7, plane0=3.88e-7, plane1_kept=3.93e-7),
+    'v2/512/+1/intensity/staged_misaligned': dict(linf=3.56e-7, l2=2.54e-7, plane0=2.70e-7, plane1_kept=3.56e-7),
     'v2/512/-1/accumulate/padded': dict(linf=3.98e-7, l2=9.16e-8, plane0=3.26e-7, plane1_kept=3.98e-7),
     'v2/512/-1/accumulate/stack5': dict(linf=3.64e-7, l2=9.17e-8, plane0=3.11e-7, plane1_kept=3.64e-7),
+    'v2/512/-1/accumulate/staged_misaligned': dict(linf=3.57e-7, l2=9.12e-8, plane0=3.45e-7, plane1_kept=3.57e-7),
+    'v2/512/-1/accumulate/staged_opd30_amp_real_batch9': dict(linf=1.69e-7, l2=1.49e-7, plane0=1.69e-7, plane1_kept=9.19e-8),
     'v2/512/-1/complex/impulse_centre': dict(linf=0.0, l2=0.0, plane0=0.0, plane1_kept=0.0),
     'v2/512/-1/complex/impulse_corners': dict(linf=1.68e-7, l2=8.78e-8, plane0=1.68e-7, plane1_kept=1.68e-7),
     'v2/512/-1/complex/impulse_mix': dict(linf=3.08e-7, l2=1.16e-7, plane0=2.74e-7, plane1_kept=3.08e-7),
     'v2/512/-1/complex/overlapping': dict(linf=2.48e-7, l2=1.78e-7, plane0=2.16e-7, plane1_kept=2.48e-7),
     'v2/512/-1/complex/single': dict(linf=2.48e-7, l2=1.77e-7, plane0=2.03e-7, plane1_kept=2.48e-7),
     'v2/512/-1/complex/stack5': dict(linf=2.48e-7, l2=1.78e-7, plane0=2.16e-7, plane1_kept=2.48e-7),
+    'v2/512/-1/complex/staged_misaligned': dict(linf=2.48e-7, l2=1.78e-7, plane0=2.04e-7, plane1_kept=2.48e-7),
+    'v2/512/-1/complex/staged_odd_in_bs_batch9': dict(linf=2.48e-7, l2=1.78e-7, plane0=2.17e-7, plane1_kept=2.48e-7),
+    'v2/512/-1/complex/staged_odd_in_ld': dict(linf=2.48e-7, l2=1.78e-7, plane0=2.04e-7, plane1_kept=2.48e-7),
+    'v2/512/-1/complex/staged_opd1e4_amp_u8_shared_batch9': dict(linf=2.74e-7, l2=1.82e-7, plane0=2.46e-7, plane1_kept=2.74e-7),
     'v2/512/-1/intensity/stack5': dict(linf=4.94e-7, l2=2.54e-7, plane0=3.42e-7, plane1_kept=4.94e-7),
+    'v2/512/-1/intensity/staged_misaligned': dict(linf=3.88e-7, l2=2.54e-7, plane0=3.36e-7, plane1_kept=3.88e-7),
 }
 
 
@@ -267,13 +267,13 @@ class Checker:
         if not ok:
             self.routes.append(msg)
 
-    def add(self, case, got, ref, rows=None, field=0, names=CLASSES):
+    def add(self, case, got, ref, rows=None, field=0):
         got = got.detach().cpu().numpy() if torch.is_tensor(got) else np.asarray(got)
         figs = {'linf': rel_linf(got, ref), 'l2': rel_l2(got, ref)}
         if rows is not None:
             rowmax = np.abs(got - ref).max(axis=1)
             den = float(np.abs(ref).max())
-            for c, cname in enumerate(names):
+            for c, cname in enumerate(CLASSES):
                 sel = rowmax[rows == c]
                 if sel.size:
                     figs[cname] = float(sel.max()) / den
@@ -312,15 +312,14 @@ def axis_code(k):
 
 
 def route_counts():
-    """launches so far of every axis_reg_kernel instantiation, of the generic axis pass and of both focus pairs"""
+    """launches so far of every axis_reg_kernel instantiation, of the generic axis pass and of the focus pair"""
     from prysm_b200 import _capi
     h = _handle()
     out = {k: h.route_launch_count(axis_code(k)) for k in AXIS_ALL}
     out['generic'] = h.route_launch_count(_capi.route_code(_capi.ROUTE_AXIS_GENERIC))
-    for v, kind in ((1, _capi.ROUTE_FOCUS_V1), (2, _capi.ROUTE_FOCUS_V2)):
-        for N in NS:
-            for inv in (0, 1):
-                out[('focus', v, N, inv)] = h.route_launch_count(_capi.route_code(kind, N, inv))
+    for N in NS:
+        for inv in (0, 1):
+            out[('focus', N, inv)] = h.route_launch_count(_capi.route_code(_capi.ROUTE_FOCUS_V2, N, inv))
     out['all'] = h.launch_count()
     return out
 
@@ -453,19 +452,19 @@ def batch_call(ops, src, N, d, nb, in_bs, in_ld, out, kind, *, in_kind=None, amp
     return out
 
 
-def check_focus(chk, case, v, N, d, fn, refs, nlaunch):
-    """fn() -> (nb, 2N, 2N) output; refs: {field: reference}; nlaunch: the launches of the v1 / v2 pair of <N, INV> the
-    call takes, and it launches nothing else.  v2 outputs are bounded per row class of its tile-major intermediate; the
-    v1 intermediate is row-major and keeps nothing in L2, so for v1 the classes are plane 0 and plane 1."""
+def check_focus(chk, case, N, d, fn, refs, nlaunch, nscreen=0):
+    """fn() -> (nb, 2N, 2N) output; refs: {field: reference}; nlaunch: the launches of the focus pair of <N, INV> the
+    call takes, and it launches nothing else but `nscreen` phase-screen kernels.  Outputs are bounded per row class of the
+    tile-major intermediate."""
     got, used = routes_of(fn)
-    want = {('focus', v, N, int(d > 0)): nlaunch, 'all': nlaunch}
+    want = {('focus', N, int(d > 0)): nlaunch, 'all': nlaunch + nscreen}
     chk.route(used == want, f'{case}: launches per route {used}, the route takes {want}')
-    rows, names = (row_classes(N), CLASSES) if v == 2 else (np.minimum(row_classes(N), 1), ('plane0', 'plane1'))
+    rows = row_classes(N)
     for b, ref in refs.items():
-        chk.add(case, got[b], ref, rows, b, names)
+        chk.add(case, got[b], ref, rows, b)
 
 
-# ---- the fused focus pair, v2 (tensor-TMA input, one launch pair per field) ---------------------------------------
+# ---- the fused focus pair (tensor-TMA input, one launch pair per field) -------------------------------------------
 @pytest.mark.parametrize('kind', KINDS)
 @pytest.mark.parametrize('d', (-1, 1))
 @pytest.mark.parametrize('N', NS)
@@ -484,7 +483,7 @@ def test_v2_stack_every_field(pb, N, d, kind):
 
     chk = Checker()
     refs = {b: derive(gauss_ref(N, b, d), kind, None if acc0h is None else acc0h[b]) for b in range(NSTACK)}
-    check_focus(chk, f'v2/{N}/{d:+d}/{kind}/stack5', 2, N, d, fn, refs, 2 * NSTACK)
+    check_focus(chk, f'v2/{N}/{d:+d}/{kind}/stack5', N, d, fn, refs, 2 * NSTACK)
     chk.done()
 
 
@@ -501,7 +500,7 @@ def test_v2_single_overlapping_padded(pb, N, d):
     chk = Checker()
     one = x[0].clone()
     fn = (lambda: (P.focus if d < 0 else P.unfocus)(one, 2)[None])
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/single', 2, N, d, fn, {0: gauss_ref(N, 0, d)}, 2)
+    check_focus(chk, f'v2/{N}/{d:+d}/complex/single', N, d, fn, {0: gauss_ref(N, 0, d)}, 2)
 
     buf = torch.zeros((NSTACK, K, K + N), dtype=torch.complex64, device='cuda')
     src = buf[:, :N, K:]
@@ -511,7 +510,7 @@ def test_v2_single_overlapping_padded(pb, N, d):
         out = buf[:, :, :K]
         batch_call(_ops, src, N, d, NSTACK, src.stride(0), src.stride(1), out, 'complex')
         return out
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/overlapping', 2, N, d, inside,
+    check_focus(chk, f'v2/{N}/{d:+d}/complex/overlapping', N, d, inside,
                 {b: gauss_ref(N, b, d) for b in range(NSTACK)}, 2 * NSTACK)
     assert torch.equal(src, x)
 
@@ -526,7 +525,7 @@ def test_v2_single_overlapping_padded(pb, N, d):
         outside[:, 1:K + 1, 2:K + 2] = False
         assert torch.equal(big[outside], big0[outside])      # no store outside the window
         return out
-    check_focus(chk, f'v2/{N}/{d:+d}/accumulate/padded', 2, N, d, padded,
+    check_focus(chk, f'v2/{N}/{d:+d}/accumulate/padded', N, d, padded,
                 {b: derive(gauss_ref(N, b, d), 'accumulate', acc0h[b]) for b in range(NSTACK)}, 2 * NSTACK)
     chk.done()
 
@@ -545,14 +544,14 @@ def test_v2_impulses(pb, N, d):
         x = torch.from_numpy(a).cuda()
         ref = impulse_focus(N, 2, [px[p] for p, _ in terms], [v for _, v in terms], inverse=d > 0)
         fn = (lambda: _ops.fft2(x, (2 * N, 2 * N), dir=d, scale=0.5 / N, shift_in=True, shift_out=True)[None])
-        check_focus(chk, f'v2/{N}/{d:+d}/complex/impulse_{name}', 2, N, d, fn, {0: ref}, 2)
+        check_focus(chk, f'v2/{N}/{d:+d}/complex/impulse_{name}', N, d, fn, {0: ref}, 2)
     chk.done()
 
 
-# ---- the fused focus pair, v1 (inputs tensor TMA cannot gather; up to 8 fields per launch pair) -----------------------
+# ---- the fused focus pair, staged inputs (tensor TMA cannot gather them: staged field by field) ------------------------
 @pytest.mark.parametrize('d', (-1, 1))
 @pytest.mark.parametrize('N', NS)
-def test_v1_misaligned_base_every_output_kind(pb, N, d):
+def test_staged_misaligned_base_every_output_kind(pb, N, d):
     """a complex input whose base is 8 bytes off 16-byte alignment, through the public call (with weight)"""
     from prysm_b200 import _ops
     K = 2 * N
@@ -568,15 +567,15 @@ def test_v1_misaligned_base_every_output_kind(pb, N, d):
             return _ops.fft2(src, (K, K), dir=d, scale=1.0 / K, shift_in=True, shift_out=True,
                              out_kind=out_kind(_ops.capi, kind), weight=WEIGHT, out=out)[None]
         ref = derive(gauss_ref(N, 0, d), kind, acc0.cpu().numpy())
-        check_focus(chk, f'v1/{N}/{d:+d}/{kind}/misaligned', 1, N, d, fn, {0: ref}, 2)
+        check_focus(chk, f'v2/{N}/{d:+d}/{kind}/staged_misaligned', N, d, fn, {0: ref}, 2)
     chk.done()
 
 
 @pytest.mark.parametrize('d', (-1, 1))
 @pytest.mark.parametrize('N', (512, 2048))
-def test_v1_odd_pitches_and_chunks(pb, N, d):
-    """an odd row pitch (one field), and an odd field pitch on a stack of 9 = chunks of 8 + 1 whose fields repeat the
-    Gaussian stack in the order 0 1 2 3 4 4 3 2 1 (a chunk read from the wrong base gets the wrong field)"""
+def test_staged_odd_pitches(pb, N, d):
+    """an odd row pitch (one field), and an odd field pitch on a stack of 9 whose fields repeat the Gaussian stack in the
+    order 0 1 2 3 4 4 3 2 1 (a field staged from the wrong base gets the wrong field)"""
     from prysm_b200 import _ops
     K = 2 * N
     host = gauss_stack(N)
@@ -587,7 +586,7 @@ def test_v1_odd_pitches_and_chunks(pb, N, d):
     def odd_ld():
         out = torch.empty((1, K, K), dtype=torch.complex64, device='cuda')
         return batch_call(_ops, buf, N, d, 1, 0, N + 1, out, 'complex')
-    check_focus(chk, f'v1/{N}/{d:+d}/complex/odd_in_ld', 1, N, d, odd_ld, {0: gauss_ref(N, 0, d)}, 2)
+    check_focus(chk, f'v2/{N}/{d:+d}/complex/staged_odd_in_ld', N, d, odd_ld, {0: gauss_ref(N, 0, d)}, 2)
 
     order = (0, 1, 2, 3, 4, 4, 3, 2, 1)
     bs = N * N + 1
@@ -599,13 +598,13 @@ def test_v1_odd_pitches_and_chunks(pb, N, d):
         out = torch.empty((9, K, K), dtype=torch.complex64, device='cuda')
         return batch_call(_ops, src, N, d, 9, bs, N, out, 'complex')
     fields = range(9) if N < 2048 else (0, 4, 7, 8)
-    check_focus(chk, f'v1/{N}/{d:+d}/complex/odd_in_bs_batch9', 1, N, d, odd_bs,
-                {b: gauss_ref(N, order[b], d) for b in fields}, 4)
+    check_focus(chk, f'v2/{N}/{d:+d}/complex/staged_odd_in_bs_batch9', N, d, odd_bs,
+                {b: gauss_ref(N, order[b], d) for b in fields}, 18)
     chk.done()
 
 
 @pytest.mark.parametrize('N', (512, 2048))
-def test_v1_phase_screen_input(pb, N):
+def test_staged_phase_screen_input(pb, N):
     """PB_IN_AMP_OPD: no amplitude and an OPD of tens of nm (one field); a bool amplitude shared by a stack of 9 with an
     OPD of ~1e4 nm (many waves: the fp64 phase range reduction); per-field real amplitudes, |.|^2 accumulated"""
     from prysm_b200 import _ops
@@ -616,15 +615,15 @@ def test_v1_phase_screen_input(pb, N):
     opd = torch.from_numpy(opd_s).cuda()
     fn = (lambda: _ops.fft2(None, (K, K), dir=1, scale=1.0 / K, shift_in=True, shift_out=True, opd=opd[0],
                             kscale=KSCALE)[None])
-    check_focus(chk, f'v1/{N}/+1/complex/opd30_amp_none', 1, N, 1, fn, {0: opd_ref(N, 9, 30.0, 'none', 0, 1)}, 2)
+    check_focus(chk, f'v2/{N}/+1/complex/staged_opd30_amp_none', N, 1, fn, {0: opd_ref(N, 9, 30.0, 'none', 0, 1)}, 2, 1)
 
     opd_l, mask_l, _ = opd_stack(N, 9, 1e4)
     opdl = torch.from_numpy(opd_l).cuda()
     m = torch.from_numpy(mask_l).cuda()
     fn = (lambda: _ops.fft2_batch(None, (K, K), dir=-1, scale=1.0 / K, shift_in=True, shift_out=True, amp=m, opd=opdl,
                                   kscale=KSCALE))
-    check_focus(chk, f'v1/{N}/-1/complex/opd1e4_amp_u8_shared_batch9', 1, N, -1, fn,
-                {b: opd_ref(N, 9, 1e4, 'mask', b, -1) for b in fields}, 4)
+    check_focus(chk, f'v2/{N}/-1/complex/staged_opd1e4_amp_u8_shared_batch9', N, -1, fn,
+                {b: opd_ref(N, 9, 1e4, 'mask', b, -1) for b in fields}, 18, 9)
 
     _, _, amps_s = opd_stack(N, 9, 30.0)
     amps = torch.from_numpy(amps_s).cuda()
@@ -635,8 +634,8 @@ def test_v1_phase_screen_input(pb, N):
         out = acc0.clone()
         return batch_call(_ops, opd, N, -1, 9, N * N, N, out, 'accumulate', in_kind=_ops.capi.IN_AMP_OPD, amp=amps,
                           amp_kind=_ops.capi.AMP_REAL, amp_bs=N * N)
-    check_focus(chk, f'v1/{N}/-1/accumulate/opd30_amp_real_batch9', 1, N, -1, fn2,
-                {b: derive(opd_ref(N, 9, 30.0, 'real', b, -1), 'accumulate', acc0h[b]) for b in fields}, 4)
+    check_focus(chk, f'v2/{N}/-1/accumulate/staged_opd30_amp_real_batch9', N, -1, fn2,
+                {b: derive(opd_ref(N, 9, 30.0, 'real', b, -1), 'accumulate', acc0h[b]) for b in fields}, 18, 9)
     chk.done()
 
 
