@@ -532,6 +532,53 @@ int pb_psi(pb_handle_t h, int frame_type, int nframes, const void* const* frames
            long long frame_stride, long long n, const double* s_host, const double* c_host, int num_type, void* num,
            void* den, int phase_type, void* phase, void* stream);
 
+/* ---- image sensors (prysm/detector.py, prysm/bayer.py) ---------------------------------------------------------------
+ * pb_expose: frames exposures of the n-pixel aerial image (real at dtype; viewed as (n / nx, nx)) -> out, frame-major
+ *   (frames, n).  lam = aerial t [* prnu] + dark [* dcnu], each step rounded at dtype; prnu / dcnu (optional, at dtype)
+ *   are read at row * sr + col * sc, so a broadcast map is never materialised.  Per (pixel, frame): k ~ Poisson(lam)
+ *   (exact: inversion below 10, PTRS from 10), x = k + read_sigma * N(0, 1) + bias, min(x, fwc) * scaling clipped to
+ *   [0, cap] and truncated to an unsigned code of code_bytes (1, 2, 4); with a lut (lut_len entries of out_bytes), out =
+ *   lut[code], else out_bytes = code_bytes.  params_host: t, dark, read_sigma, bias, fwc, scaling, cap.  Random
+ *   numbers: Philox4x32-10 keyed by `key`, counter (pixel, frame, draw), independent of the launch shape.  flags: two
+ *   zeroed uint32 on the device; bit 0 of flags[0]: some lam < 0 or NaN, bit 1: some lam > 9.2234e18 (numpy's
+ *   POISSON_LAM_MAX), bit 2: some code >= lut_len, whose maximum is in flags[1].  Never synchronises.
+ * pb_apply_lut: out[i] = lut[codes[i]] for unsigned codes of code_bytes; with check, a code >= lut_len sets bit 2 of
+ *   flags[0] and raises flags[1] to it.
+ * pb_pixel: out[i] = (x <= wx) & (x >= -wx) & (y <= wy) & (y >= -wy) as uint8, over an (n / nx, nx) view with x and y
+ *   (real at dtype) read at row * sr + col * sc.
+ * pb_bayer_interleave: out (M, N) with row pitch out_ld, elements of elem_bytes; the value at CFA site s (0 top-left,
+ *   1 top-right, 2 bottom-left, 3 bottom-right of each 2x2 cell) comes from planes_host[s] (row pitch ld_host[s]) at
+ *   (y, x), or at (y / 2, x / 2) with half (recomposite).
+ * pb_demosaic_deinterlace: (m / 2, n / 2, 3) = (R, (G1 + G2) / 2, B) of an even-sided mosaic with row pitch ld; the
+ *   green sum is formed in in_type (wrapping for unsigned types), the halving in out_type (PB_SENSOR_F32 / F64).
+ * pb_white_balance: a *= gain in place (a contiguous, real at dtype): gains_host[site] for a mosaic (kind 0, rows of
+ *   nx) or gains_host[i % 3] for interleaved RGB (kind 1).  With sat_host, every gain is first divided by max(1,
+ *   max_p(max(plane p) gains_p / sat_p)), computed on the device in work (fp64, 4 PB_WB_MAX_BLOCKS + 1 values).
+ * pb_demosaic_malvar: (m, n, 3) RGB of out_type (PB_SENSOR_F32 from f32 / u8 / u16, or PB_SENSOR_F64) from an m x n
+ *   mosaic of in_type with row pitch ld, rggb or bggr: Malvar-He-Cutler's 5x5 filters, scipy.ndimage's reflect
+ *   boundary, accumulated in fp64.  One pass.
+ * pb_bayer_assemble: (n, 3) = (Re rp, (Re g2p + g1) / 2, Re bp) for complex rp, g2p, bp and real g1 at dtype. */
+typedef enum { PB_SENSOR_F32 = 0, PB_SENSOR_F64 = 1, PB_SENSOR_U8 = 2, PB_SENSOR_U16 = 3, PB_SENSOR_U32 = 4 } pb_sensor_type;
+enum { PB_WB_MAX_BLOCKS = 1024 };
+int pb_expose(pb_handle_t h, int dtype, const void* aerial, long long n, long long nx, const void* prnu, long long prnu_sr,
+              long long prnu_sc, const void* dcnu, long long dcnu_sr, long long dcnu_sc, const double* params_host,
+              int frames, long long key, int code_bytes, const void* lut, long long lut_len, int out_bytes,
+              void* out, void* flags, void* stream);
+int pb_apply_lut(pb_handle_t h, int code_bytes, const void* codes, long long n, const void* lut, long long lut_len,
+                 int out_bytes, int check, void* out, void* flags, void* stream);
+int pb_pixel(pb_handle_t h, int dtype, const void* x, long long xsr, long long xsc, const void* y, long long ysr,
+             long long ysc, long long n, long long nx, double wx, double wy, void* out, void* stream);
+int pb_bayer_interleave(pb_handle_t h, int elem_bytes, const void* const* planes_host, const long long* ld_host, int half,
+                        long long M, long long N, void* out, long long out_ld, void* stream);
+int pb_demosaic_deinterlace(pb_handle_t h, int in_type, const void* img, long long m, long long n, long long ld, int bggr,
+                            int out_type, void* out, void* stream);
+int pb_white_balance(pb_handle_t h, int dtype, void* a, long long n, long long nx, int kind, const double* gains_host,
+                     const double* sat_host, void* work, void* stream);
+int pb_demosaic_malvar(pb_handle_t h, int in_type, const void* img, long long m, long long n, long long ld, int bggr,
+                       int out_type, void* out, void* stream);
+int pb_bayer_assemble(pb_handle_t h, int dtype, const void* rp, const void* g2p, const void* bp, const void* g1,
+                      long long n, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,7 +10,10 @@ Mirrors the reference's module layout for the path only:
     prysm_b200.coronagraph  <-> prysm.propagation.coronagraph (re-exported by .propagation like the reference)
     prysm_b200.coordinates / .geometry  <-> prysm.coordinates.make_xy_grid / cart_to_polar, prysm.geometry.circle / antialias
     prysm_b200.convolution  <-> prysm.convolution (conv, apply_transfer_functions)
-    prysm_b200.detector     <-> prysm.detector (bindown, tile, pixel_ft, olpf_ft)
+    prysm_b200.detector     <-> prysm.detector (Detector.expose with shot and read noise, apply_lut, pixel, bindown, tile,
+                            pixel_ft, olpf_ft)
+    prysm_b200.bayer        <-> prysm.bayer (white balance, composite / decomposite, deinterlace and Malvar demosaicing,
+                            assemble_superresolved)
     prysm_b200.dm           <-> prysm.x.dm (DM: render / render_adjoint; coordinates.warp is its spline warp)
     prysm_b200.segmented    <-> prysm.segmented (CompositeHexagonalAperture: rasterise, compose_opd and its adjoint)
     prysm_b200.polarization <-> prysm.x.polarization (Jones constructors, products, Mueller / Pauli, jones_adapter)
@@ -24,7 +27,7 @@ from . import _capi  # noqa: F401  (fails loudly if the CUDA library is missing)
 from .conf import config  # noqa: F401
 from . import fttools, propagation, coronagraph, otf, psf, polynomials, polychromatic, mathops, graphs  # noqa: F401
 from . import coordinates, geometry, convolution, detector, dm, segmented, polarization  # noqa: F401
-from . import fibers, sri, pdi, psi  # noqa: F401
+from . import fibers, sri, pdi, psi, bayer  # noqa: F401
 from ._capi import B200Error  # noqa: F401
 from .propagation import Wavefront  # noqa: F401
 from ._ops import asdevice, asnumpy, set_device  # noqa: F401

@@ -108,6 +108,15 @@ SIGNATURES = {
     'pb_grating': (_i, [_vp, _i, _i, _ll, _vp, _d, C.POINTER(_d), _i, _vp, _vp, _vp]),
     'pb_psi': (_i, [_vp, _i, _i, C.POINTER(_vp), _vp, _ll, _ll, C.POINTER(_d), C.POINTER(_d), _i, _vp, _vp, _i, _vp,
                     _vp]),
+    'pb_expose': (_i, [_vp, _i, _vp, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _ll, C.POINTER(_d), _i, _ll, _i, _vp,
+                       _ll, _i, _vp, _vp, _vp]),
+    'pb_apply_lut': (_i, [_vp, _i, _vp, _ll, _vp, _ll, _i, _i, _vp, _vp, _vp]),
+    'pb_pixel': (_i, [_vp, _i, _vp, _ll, _ll, _vp, _ll, _ll, _ll, _ll, _d, _d, _vp, _vp]),
+    'pb_bayer_interleave': (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_ll), _i, _ll, _ll, _vp, _ll, _vp]),
+    'pb_demosaic_deinterlace': (_i, [_vp, _i, _vp, _ll, _ll, _ll, _i, _i, _vp, _vp]),
+    'pb_white_balance': (_i, [_vp, _i, _vp, _ll, _ll, _i, C.POINTER(_d), C.POINTER(_d), _vp, _vp]),
+    'pb_demosaic_malvar': (_i, [_vp, _i, _vp, _ll, _ll, _ll, _i, _i, _vp, _vp]),
+    'pb_bayer_assemble': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _ll, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -124,6 +133,8 @@ LP_RULE_LP, LP_RULE_SMF = range(2)
 LP_NONE, LP_COS, LP_SIN = range(3)
 GRATING_SIN_AMP, GRATING_RECTANGLE = range(2)
 PSI_F32, PSI_F64, PSI_U16, PSI_I32, PSI_I64 = range(5)
+SENSOR_F32, SENSOR_F64, SENSOR_U8, SENSOR_U16, SENSOR_U32 = range(5)
+WB_MAX_BLOCKS = 1024
 
 
 def load_library(path=LIB_PATH):

@@ -1163,6 +1163,133 @@ def psi(frames, s, c, num_dtype, phase_dtype, want_num=True, want_phase=True):
     return num, den, phase
 
 
+_SENSOR_TYPE = {torch.float32: capi.SENSOR_F32, torch.float64: capi.SENSOR_F64, torch.uint8: capi.SENSOR_U8,
+                torch.uint16: capi.SENSOR_U16, torch.uint32: capi.SENSOR_U32}
+_CODE_BYTES = {torch.uint8: 1, torch.uint16: 2, torch.uint32: 4}
+
+
+def rows_view(m, shape):
+    """(map, row stride, column stride) through which an operand broadcast against `shape` is read as the (rows, last
+    axis) view of that shape: a broadcast dimension is stride 0, never materialised.  An operand whose broadcast cannot
+    be read that way is made contiguous at `shape`."""
+    nx = shape[-1] if shape else 1
+    rows = math.prod(shape[:-1]) if shape else 1
+    e = m.expand(shape) if shape else m.reshape(())
+    try:
+        v = e.view(rows, nx) if shape else e.reshape(1, 1)
+    except RuntimeError:
+        v = e.contiguous().view(rows, nx)
+    return v, v.stride(0), v.stride(1)
+
+
+def _flags_read(flags, words):
+    """The call's one synchronisation: the first `words` uint32 of the device flag buffer, to the host."""
+    return [int(v) & 0xFFFFFFFF for v in flags[:words].cpu().tolist()]
+
+
+def expose(aerial, prnu, dcnu, params, frames, key, code_dtype, lut=None):
+    """(frames, *shape) detector frames of code_dtype (or of the LUT's dtype) in one launch (pb_expose); returns
+    (out, flags) where flags are the host copy of the kernel's error words."""
+    shape = tuple(aerial.shape)
+    n = math.prod(shape)
+    nx = shape[-1] if shape else 1
+    mp = [prnu, dcnu]
+    views = []
+    for m in mp:
+        views.append(None if m is None else rows_view(m, shape))
+    lut_t = None if lut is None else lut.contiguous()
+    odt = code_dtype if lut_t is None else lut_t.dtype
+    out = torch.empty((frames, *shape), dtype=odt, device=aerial.device)
+    flags = torch.zeros(2, dtype=torch.int32, device=aerial.device)
+    if n == 0:
+        return out, [0, 0]
+    pp, pr, pc = views[0] or (None, 0, 0)
+    dp, dr, dc = views[1] or (None, 0, 0)
+    prm, prmp = _darr(params)
+    h, st = _ctx(aerial)
+    h.check(lib.pb_expose(h.ptr, _CODE[aerial.dtype], _p(aerial), n, nx, _p(pp), pr, pc, _p(dp), dr, dc, prmp,
+                          int(frames), int(key), _CODE_BYTES[code_dtype], _p(lut_t),
+                          0 if lut_t is None else lut_t.numel(), odt.itemsize, _p(out), _p(flags), st))
+    return out, _flags_read(flags, 2 if lut_t is not None else 1)
+
+
+def apply_lut(codes, lut, check):
+    """np.take(lut, codes) for unsigned codes (pb_apply_lut); returns (out, largest out-of-range code or None)."""
+    codes = codes.contiguous()
+    lut = lut.contiguous()
+    out = torch.empty(codes.shape, dtype=lut.dtype, device=codes.device)
+    flags = torch.zeros(2, dtype=torch.int32, device=codes.device) if check else None
+    h, st = _ctx(codes)
+    h.check(lib.pb_apply_lut(h.ptr, _CODE_BYTES[codes.dtype], _p(codes), codes.numel(), _p(lut), lut.numel(),
+                             lut.dtype.itemsize, int(bool(check)), _p(out), _p(flags), st))
+    if check and codes.numel():
+        f = _flags_read(flags, 2)
+        if f[0] & 4:
+            return out, f[1]
+    return out, None
+
+
+def pixel(x, y, wx, wy):
+    """(x <= wx) & (x >= -wx) & (y <= wy) & (y >= -wy) as a bool tensor of the broadcast shape (pb_pixel)."""
+    shape = tuple(torch.broadcast_shapes(x.shape, y.shape))
+    xv, xr, xc = rows_view(x, shape)
+    yv, yr, yc = rows_view(y, shape)
+    out = torch.empty(shape, dtype=torch.uint8, device=x.device)
+    n = math.prod(shape)
+    if n:
+        h, st = _ctx(x)
+        h.check(lib.pb_pixel(h.ptr, _CODE[x.dtype], _p(xv), xr, xc, _p(yv), yr, yc, n, shape[-1] if shape else 1,
+                             float(wx), float(wy), _p(out), st))
+    return out.view(torch.bool)
+
+
+def bayer_interleave(planes, half, out):
+    """out[site s] = planes[s] at (y, x), or at (y / 2, x / 2) with half (pb_bayer_interleave); planes are 2-D tensors
+    of out's dtype with unit column stride (or None for a site the output does not have)."""
+    M, N = out.shape
+    ptrs = (C.c_void_p * 4)(*[None if p is None else p.data_ptr() for p in planes])
+    lds = (C.c_longlong * 4)(*[0 if p is None else p.stride(0) for p in planes])
+    h, st = _ctx(out)
+    h.check(lib.pb_bayer_interleave(h.ptr, out.element_size(), ptrs, lds, int(half), M, N, _p(out), out.stride(0), st))
+    return out
+
+
+def demosaic_deinterlace(img, bggr, out_dtype):
+    m, n = img.shape
+    out = torch.empty((m // 2, n // 2, 3), dtype=out_dtype, device=img.device)
+    h, st = _ctx(img)
+    h.check(lib.pb_demosaic_deinterlace(h.ptr, _SENSOR_TYPE[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
+                                        _SENSOR_TYPE[out_dtype], _p(out), st))
+    return out
+
+
+def white_balance(a, kind, gains, sat=None):
+    """a *= gain in place (pb_white_balance): per CFA site (kind 0, a 2-D mosaic) or per channel (kind 1, (..., 3));
+    with `sat` the gains are first descaled on the device so that no plane exceeds its saturation."""
+    g, gp = _darr(gains)
+    s, sp = (None, None) if sat is None else _darr(sat)
+    work = None if sat is None else torch.empty(4 * capi.WB_MAX_BLOCKS + 1, dtype=torch.float64, device=a.device)
+    h, st = _ctx(a)
+    h.check(lib.pb_white_balance(h.ptr, _CODE[a.dtype], _p(a), a.numel(), a.shape[-1] if kind == 0 else 3, int(kind),
+                                 gp, sp, _p(work), st))
+    return a
+
+
+def demosaic_malvar(img, bggr, out_dtype):
+    m, n = img.shape
+    out = torch.empty((m, n, 3), dtype=out_dtype, device=img.device)
+    h, st = _ctx(img)
+    h.check(lib.pb_demosaic_malvar(h.ptr, _SENSOR_TYPE[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
+                                   _SENSOR_TYPE[out_dtype], _p(out), st))
+    return out
+
+
+def bayer_assemble(rp, g2p, bp, g1, out):
+    h, st = _ctx(g1)
+    h.check(lib.pb_bayer_assemble(h.ptr, _CODE[g1.dtype], _p(rp), _p(g2p), _p(bp), _p(g1), g1.numel(), _p(out), st))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

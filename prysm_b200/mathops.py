@@ -19,8 +19,10 @@ touches numpy `exp` or eager tensor arithmetic.
 """
 import importlib
 
+from . import bayer as _bayer
 from . import convolution as _conv
 from . import coordinates as _coords
+from . import detector as _det
 from . import dm as _dm
 from . import fibers as _fib
 from . import fttools as _ft
@@ -84,6 +86,11 @@ _TARGETS = {
         'overlap_integral', 'to_photonic_fiber_and_back', 'SelfReferencedInterferometer')},
     'prysm.x.pdi': {n: getattr(_pdi, n) for n in ('rectangle_pulse', 'PSPDI', 'evaluate_test_ref_arm_matching')},
     'prysm.x.psi': {n: getattr(_psi, n) for n in ('psi_accumulate', 'degroot_formalism_psi')},
+    # image sensors: the Detector class itself is re-bound (as prysm.x.dm's DM is)
+    'prysm.detector': {'Detector': _det.Detector, 'apply_lut': _det.apply_lut, 'pixel': _det.pixel},
+    'prysm.bayer': {n: getattr(_bayer, n) for n in (
+        'wb_prescale', 'wb_postscale', 'composite_bayer', 'decomposite_bayer', 'recomposite_bayer',
+        'demosaic_deinterlace', 'assemble_superresolved', 'demosaic_malvar')},
 }
 
 _saved = {}  # (module name, attribute) -> original
