@@ -579,6 +579,37 @@ int pb_demosaic_malvar(pb_handle_t h, int in_type, const void* img, long long m,
 int pb_bayer_assemble(pb_handle_t h, int dtype, const void* rp, const void* g2p, const void* bp, const void* g1,
                       long long n, void* out, void* stream);
 
+/* ---- Shack-Hartmann sensing (prysm/x/shack_hartmann.py) -------------------------------------------------------------
+ * pb_lenslet_screen: the complex (H, W) screen exp(i kphase total) of dtype, one thread per sample.  total is the sum,
+ *   in the storage precision and in lenslet order (row j outer, column i inner), of rsq / two_efl over the lenslets
+ *   (j, i) whose window covers the sample and whose aperture admits it, with lx = x - xc[i], ly = y - yc[j],
+ *   rsq = lx^2 + ly^2 in fp64 without fused multiply-add.  x, y: (H, W) real at dtype.  centres: fp64 device array,
+ *   xc [ncols] then yc [nrows].  cand: int32 device array, per grid column (first, one past last) lenslet column whose
+ *   window covers it [2 W], then the same per grid row [2 H].  params_host: half-width, half-height, angle (radians),
+ *   lenslet r^2.  kind: PB_LENSLET_RECT (|lx| <= w and |ly| <= h), PB_LENSLET_RECT_SWAP (|ly| <= w and |lx| <= h),
+ *   PB_LENSLET_RECT_ROTATED (the same after rotating (lx, ly) by the angle in polar form), PB_LENSLET_CIRCLE
+ *   (rsq <= lenslet r^2).
+ * pb_subaperture_centroids: for nframes frames of frame_type ((H, W) each, frame_stride elements apart) and each
+ *   subaperture (j, i): w = max(I - t, 0) with t = threshold max(I over the subaperture); disp (nframes, 2, nrows,
+ *   ncols) = scale (sum w x / sum w - xc[i], sum w y / sum w - yc[j]), NaN where sum w = 0; flux (nframes, nrows, ncols) =
+ *   sum I.  out_type: PB_SH_F64 for PB_SH_F64 frames, PB_SH_F32 otherwise; the sums are fp64 in a fixed order.
+ *   dtab (fp64, device): x of each grid column [W], y of each grid row [H], xc [ncols], yc [nrows].  itab (int32,
+ *   device): owning lenslet column of each grid column or -1 [W], each lenslet column's owned grid columns as
+ *   [lo, hi): lo [ncols] then hi [ncols], each lenslet row's owned grid rows: lo [nrows] then hi [nrows].  One launch.
+ * pb_sh_reconstruct: out[f, k] = sum_m R[k, m] (slopes[f][idx[m]] - ref[m]) for nframes slope vectors frame_stride
+ *   elements apart, R (K, M) and ref (M, optional) fp64 on the device, idx int32; slopes and out of dtype
+ *   (PB_SH_F32 / PB_SH_F64), accumulated in fp64.  A NaN in a selected slope propagates. */
+typedef enum { PB_LENSLET_RECT = 0, PB_LENSLET_RECT_SWAP = 1, PB_LENSLET_RECT_ROTATED = 2, PB_LENSLET_CIRCLE = 3 } pb_lenslet_kind;
+typedef enum { PB_SH_F32 = 0, PB_SH_F64 = 1, PB_SH_U16 = 2, PB_SH_I32 = 3 } pb_sh_type;
+int pb_lenslet_screen(pb_handle_t h, int dtype, const void* x, const void* y, int H, int W, int ncols, int nrows,
+                      const double* centres, const int* cand, int kind, const double* params_host, double two_efl,
+                      double kphase, void* out, void* stream);
+int pb_subaperture_centroids(pb_handle_t h, int frame_type, const void* frames, int nframes, int H, int W,
+                             long long frame_stride, int ncols, int nrows, const double* dtab, const int* itab,
+                             double threshold, double scale, int out_type, void* disp, void* flux, void* stream);
+int pb_sh_reconstruct(pb_handle_t h, int dtype, const void* slopes, int nframes, long long frame_stride, const int* idx,
+                      const double* ref, const double* R, int K, int M, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -117,6 +117,9 @@ SIGNATURES = {
     'pb_white_balance': (_i, [_vp, _i, _vp, _ll, _ll, _i, C.POINTER(_d), C.POINTER(_d), _vp, _vp]),
     'pb_demosaic_malvar': (_i, [_vp, _i, _vp, _ll, _ll, _ll, _i, _i, _vp, _vp]),
     'pb_bayer_assemble': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _ll, _vp, _vp]),
+    'pb_lenslet_screen': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, C.POINTER(_d), _d, _d, _vp, _vp]),
+    'pb_subaperture_centroids': (_i, [_vp, _i, _vp, _i, _i, _i, _ll, _i, _i, _vp, _vp, _d, _d, _i, _vp, _vp, _vp]),
+    'pb_sh_reconstruct': (_i, [_vp, _i, _vp, _i, _ll, _vp, _vp, _vp, _i, _i, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -135,6 +138,8 @@ GRATING_SIN_AMP, GRATING_RECTANGLE = range(2)
 PSI_F32, PSI_F64, PSI_U16, PSI_I32, PSI_I64 = range(5)
 SENSOR_F32, SENSOR_F64, SENSOR_U8, SENSOR_U16, SENSOR_U32 = range(5)
 WB_MAX_BLOCKS = 1024
+LENSLET_RECT, LENSLET_RECT_SWAP, LENSLET_RECT_ROTATED, LENSLET_CIRCLE = range(4)
+SH_F32, SH_F64, SH_U16, SH_I32 = range(4)
 
 
 def load_library(path=LIB_PATH):

@@ -1290,6 +1290,57 @@ def bayer_assemble(rp, g2p, bp, g1, out):
     return out
 
 
+def lenslet_screen(x, y, centres, cand, kind, params, two_efl, kphase, ncols, nrows):
+    """The complex Shack-Hartmann screen of x's precision in one launch (pb_lenslet_screen); centres (fp64) and cand
+    (int32) are the device tables shack_hartmann builds."""
+    H, W = x.shape
+    out = torch.empty((H, W), dtype=_CPLX_OF[x.dtype], device=x.device)
+    prm, prmp = _darr(params)
+    h, st = _ctx(x)
+    h.check(lib.pb_lenslet_screen(h.ptr, _CODE[x.dtype], _p(x), _p(y), H, W, int(ncols), int(nrows), _p(centres),
+                                  _p(cand), int(kind), prmp, float(two_efl), float(kphase), _p(out), st))
+    return out
+
+
+_SH_TYPE = {torch.float32: capi.SH_F32, torch.float64: capi.SH_F64, torch.uint16: capi.SH_U16,
+            torch.int32: capi.SH_I32}
+
+
+def subaperture_centroids(frames, dtab, itab, ncols, nrows, threshold, scale=1.0):
+    """(disp (F, 2, nrows, ncols) times scale, flux (F, nrows, ncols)) of an (F, H, W) stack in one launch
+    (pb_subaperture_centroids); float64 for float64 frames, float32 otherwise."""
+    if frames.dtype not in _SH_TYPE:
+        raise ValueError(f'frames of {frames.dtype} are not supported (float32, float64, uint16, int32)')
+    frames = frames.contiguous()
+    F, H, W = frames.shape
+    odt = torch.float64 if frames.dtype == torch.float64 else torch.float32
+    disp = torch.empty((F, 2, nrows, ncols), dtype=odt, device=frames.device)
+    flux = torch.empty((F, nrows, ncols), dtype=odt, device=frames.device)
+    h, st = _ctx(frames)
+    h.check(lib.pb_subaperture_centroids(h.ptr, _SH_TYPE[frames.dtype], _p(frames), F, H, W, H * W, int(ncols),
+                                         int(nrows), _p(dtab), _p(itab), float(threshold), float(scale), _SH_TYPE[odt], _p(disp),
+                                         _p(flux), st))
+    return disp, flux
+
+
+def sh_reconstruct(slopes, idx, ref, R, frame_shape):
+    """out[f, k] = sum_m R[k, m] (slopes[f].flat[idx[m]] - ref[m]) for an (F, *frame_shape) slope stack
+    (pb_sh_reconstruct).  idx is a device gather table the kernel cannot bound-check, so the stack's shape is checked
+    here against the frame_shape the table was built for."""
+    if not isinstance(slopes, torch.Tensor) or slopes.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f'slopes must be a float32 or float64 tensor, got {getattr(slopes, "dtype", type(slopes))}')
+    if slopes.ndim != 1 + len(frame_shape) or tuple(slopes.shape[1:]) != tuple(frame_shape):
+        raise ValueError(f'slopes must be (F, {", ".join(map(str, frame_shape))}), got {tuple(slopes.shape)}')
+    slopes = slopes.contiguous()
+    F = slopes.shape[0]
+    K, M = R.shape
+    out = torch.empty((F, K), dtype=slopes.dtype, device=slopes.device)
+    h, st = _ctx(slopes)
+    h.check(lib.pb_sh_reconstruct(h.ptr, _SH_TYPE[slopes.dtype], _p(slopes), F, math.prod(frame_shape), _p(idx),
+                                  _p(ref), _p(R), K, M, _p(out), st))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

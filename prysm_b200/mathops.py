@@ -33,6 +33,7 @@ from . import polynomials as _poly
 from . import propagation as _prop
 from . import psf as _psf
 from . import psi as _psi
+from . import shack_hartmann as _sh
 from . import sri as _sri
 
 # prysm module -> {attribute: replacement}
@@ -86,6 +87,7 @@ _TARGETS = {
         'overlap_integral', 'to_photonic_fiber_and_back', 'SelfReferencedInterferometer')},
     'prysm.x.pdi': {n: getattr(_pdi, n) for n in ('rectangle_pulse', 'PSPDI', 'evaluate_test_ref_arm_matching')},
     'prysm.x.psi': {n: getattr(_psi, n) for n in ('psi_accumulate', 'degroot_formalism_psi')},
+    'prysm.x.shack_hartmann': {'shack_hartmann': _sh.shack_hartmann},
     # image sensors: the Detector class itself is re-bound (as prysm.x.dm's DM is)
     'prysm.detector': {'Detector': _det.Detector, 'apply_lut': _det.apply_lut, 'pixel': _det.pixel},
     'prysm.bayer': {n: getattr(_bayer, n) for n in (
