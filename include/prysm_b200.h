@@ -610,6 +610,34 @@ int pb_subaperture_centroids(pb_handle_t h, int frame_type, const void* frames, 
 int pb_sh_reconstruct(pb_handle_t h, int dtype, const void* slopes, int nframes, long long frame_stride, const int* idx,
                       const double* ref, const double* R, int K, int M, void* out, void* stream);
 
+/* ---- Forbes polynomials (prysm/polynomials/qpoly.py) ------------------------------------------------------------
+ * family: PB_QPOLY_BFS (Q-bfs, oe-18-19-19700), PB_QPOLY_CON (Q-con, oe-18-13-13851), PB_QPOLY_2D (2D-Q, oe-20-3-2483;
+ * m = 0 is Q-bfs, m < 0 a sine term).  Orders are limited to n <= 64 and |m| <= 64, a call to 256 recurrence steps
+ * (the sum over its recurrences -- one for Q-bfs / Q-con, one per |m| for 2D-Q -- of the highest n + 1) and a basis
+ * call to 1024 modes; outside these PB_ERR_UNSUPPORTED, n < 0 PB_ERR_INVALID, both before any launch.  Each call is
+ * one kernel, one thread per sample, every recurrence run once in fp64 registers.
+ * pb_qpoly_seq: k HOST (n, m) pairs (m_host may be NULL except for 2D-Q), in any order, repeats allowed; plane q of
+ *   out0 (and out1), each (k, count), is mode q.
+ *   kind PB_QPOLY_VALUE:  out0 = Q(a) (Q-bfs / Q-con: a = x) or Q(a = r, b = t) (2D-Q)       (Qbfs_seq, Qcon_seq, Q2d_seq)
+ *   kind PB_QPOLY_DER:    out0 = d/dx (Q-bfs / Q-con), or d/dr -> out0 and d/dt -> out1 (2D-Q)
+ *                         (Qbfs_der_seq, Qcon_der_seq, Q2d_der_seq)
+ *   kind PB_QPOLY_DER_XY: 2D-Q only, a = x, b = y: d/dx -> out0, d/dy -> out1 through Re / Im (x + iy)^|m|, finite at
+ *                         the origin (Q2d_der_xy_seq)
+ * pb_qpoly_sum: the sag z = sum_q coefs[q] Q_q(u, t) and optionally dz/du, dz/dt (2D-Q) without the basis; zero
+ *   coefficients are skipped, so trailing zeros trim.  z, dzdr, dzdt: (count) each, any may be NULL but not all.
+ *   (compute_z_Qbfs, compute_z_zprime_Qbfs, compute_z_zprime_Qcon, compute_z_Q2d, compute_z_zprime_Q2d.)
+ * pb_qpoly_tables (host, no handle): rows n = 0..nmax of 7 fp64 each of the recurrence tables the kernels use:
+ *   PB_QPOLY_BFS: f(n), g(n), h(n) (f_qbfs, g_qbfs, h_qbfs);  PB_QPOLY_CON: A, B, C of order n (_qcon_abc);
+ *   PB_QPOLY_2D (m >= 1): A, B, C (abc_q2d, NaN where its denominator is 0), G, F, g, f (G_q2d, F_q2d, g_q2d, f_q2d). */
+typedef enum { PB_QPOLY_BFS = 0, PB_QPOLY_CON = 1, PB_QPOLY_2D = 2 } pb_qpoly_family;
+typedef enum { PB_QPOLY_VALUE = 0, PB_QPOLY_DER = 1, PB_QPOLY_DER_XY = 2 } pb_qpoly_kind;
+int pb_qpoly_seq(pb_handle_t h, int dtype, int family, int kind, const void* a, const void* b, long long count, int k,
+                 const int* n_host, const int* m_host, void* out0, void* out1, void* stream);
+int pb_qpoly_sum(pb_handle_t h, int dtype, int family, const void* u, const void* t, long long count, int k,
+                 const int* n_host, const int* m_host, const double* coefs_host, void* z, void* dzdr, void* dzdt,
+                 void* stream);
+int pb_qpoly_tables(int family, int m, int nmax, double* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,7 +4,8 @@ Mirrors the reference's module layout for the path only:
     prysm_b200.propagation  <-> prysm.propagation   (focus/unfocus/angular_spectrum/executors/Wavefront)
     prysm_b200.fttools      <-> prysm.fttools       (pad2d/crop_center/MDFT/CZT/FFTDFT)
     prysm_b200.otf / .psf   <-> prysm.otf / prysm.psf (transform_psf, mtf/ptf/otf, centroid)
-    prysm_b200.polynomials  <-> prysm.polynomials.sum_of_2d_modes
+    prysm_b200.polynomials  <-> prysm.polynomials.sum_of_2d_modes, jacobi / zernike and the Forbes names of qpoly
+    prysm_b200.qpoly        <-> prysm.polynomials.qpoly (Q-bfs, Q-con, 2D-Q: bases, derivatives and sag / slope sums)
     prysm_b200.conf         <-> prysm.conf          (config.precision)
     prysm_b200.mathops      <-> prysm.mathops       (set_backend_to_b200 / set_backend_to_defaults)
     prysm_b200.coronagraph  <-> prysm.propagation.coronagraph (re-exported by .propagation like the reference)
@@ -29,7 +30,7 @@ from . import _capi  # noqa: F401  (fails loudly if the CUDA library is missing)
 from .conf import config  # noqa: F401
 from . import fttools, propagation, coronagraph, otf, psf, polynomials, polychromatic, mathops, graphs  # noqa: F401
 from . import coordinates, geometry, convolution, detector, dm, segmented, polarization  # noqa: F401
-from . import fibers, sri, pdi, psi, bayer, shack_hartmann  # noqa: F401
+from . import fibers, sri, pdi, psi, bayer, shack_hartmann, qpoly  # noqa: F401
 from ._capi import B200Error  # noqa: F401
 from .propagation import Wavefront  # noqa: F401
 from ._ops import asdevice, asnumpy, set_device  # noqa: F401

@@ -120,6 +120,10 @@ SIGNATURES = {
     'pb_lenslet_screen': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, C.POINTER(_d), _d, _d, _vp, _vp]),
     'pb_subaperture_centroids': (_i, [_vp, _i, _vp, _i, _i, _i, _ll, _i, _i, _vp, _vp, _d, _d, _i, _vp, _vp, _vp]),
     'pb_sh_reconstruct': (_i, [_vp, _i, _vp, _i, _ll, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    'pb_qpoly_seq': (_i, [_vp, _i, _i, _i, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
+    'pb_qpoly_sum': (_i, [_vp, _i, _i, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_d), _vp, _vp, _vp,
+                          _vp]),
+    'pb_qpoly_tables': (_i, [_i, _i, _i, C.POINTER(_d)]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -140,6 +144,9 @@ SENSOR_F32, SENSOR_F64, SENSOR_U8, SENSOR_U16, SENSOR_U32 = range(5)
 WB_MAX_BLOCKS = 1024
 LENSLET_RECT, LENSLET_RECT_SWAP, LENSLET_RECT_ROTATED, LENSLET_CIRCLE = range(4)
 SH_F32, SH_F64, SH_U16, SH_I32 = range(4)
+QPOLY_BFS, QPOLY_CON, QPOLY_2D = range(3)
+QPOLY_VALUE, QPOLY_DER, QPOLY_DER_XY = range(3)
+QPOLY_NMAX = 64
 
 
 def load_library(path=LIB_PATH):

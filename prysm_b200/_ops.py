@@ -1341,6 +1341,54 @@ def sh_reconstruct(slopes, idx, ref, R, frame_shape):
     return out
 
 
+def qpoly_seq(family, kind, ns, ms, a, b=None):
+    """Forbes basis planes (len(ns), *a.shape) of a's dtype in one launch (pb_qpoly_seq): values, or d/dx of Q-bfs /
+    Q-con, or (d/dr, d/dt) / (d/dx, d/dy) of 2D-Q as a pair.  ms is None for Q-bfs / Q-con."""
+    a = a.contiguous()
+    if b is not None:
+        b = b.to(a.dtype).contiguous()
+    k = len(ns)
+    pair = family == capi.QPOLY_2D and kind != capi.QPOLY_VALUE
+    out0 = torch.empty((k,) + tuple(a.shape), dtype=a.dtype, device=a.device)
+    out1 = torch.empty_like(out0) if pair else None
+    if k == 0:
+        return (out0, out1) if pair else out0
+    n, nptr = _iarr(ns)
+    m, mptr = _iarr(ms) if ms is not None else (None, C.POINTER(C.c_int)())
+    h, st = _ctx(a)
+    h.check(lib.pb_qpoly_seq(h.ptr, _CODE[a.dtype], int(family), int(kind), _p(a), _p(b), a.numel(), k, nptr, mptr,
+                             _p(out0), _p(out1), st))
+    return (out0, out1) if pair else out0
+
+
+def qpoly_sum(family, ns, ms, coefs, u, t=None, want_der=False):
+    """The Forbes sag z (and with want_der dz/du, plus dz/dt for 2D-Q) of coefficient list (ns, ms, coefs) in one
+    launch (pb_qpoly_sum)."""
+    u = u.contiguous()
+    if t is not None:
+        t = t.to(u.dtype).contiguous()
+    z = torch.empty_like(u)
+    dr = torch.empty_like(u) if want_der else None
+    dt = torch.empty_like(u) if want_der and family == capi.QPOLY_2D else None
+    k = len(ns)
+    n, nptr = _iarr(ns if k else [0])
+    m, mptr = _iarr(ms if ms is not None and k else [0])
+    c, cptr = _darr(coefs if k else [0.0])
+    h, st = _ctx(u)
+    h.check(lib.pb_qpoly_sum(h.ptr, _CODE[u.dtype], int(family), _p(u), _p(t), u.numel(), k, nptr, mptr, cptr, _p(z),
+                             _p(dr), _p(dt), st))
+    return z, dr, dt
+
+
+def qpoly_tables(family, m, nmax):
+    """(nmax + 1, 7) fp64 recurrence tables from the host C++ the kernels are planned with (pb_qpoly_tables)."""
+    out = np.zeros((nmax + 1, 7), dtype=np.float64)
+    rc = lib.pb_qpoly_tables(int(family), int(m), int(nmax), out.ctypes.data_as(C.POINTER(C.c_double)))
+    if rc != 0:
+        raise ValueError(f'pb_qpoly_tables(family={family}, m={m}, nmax={nmax}) failed with status {rc}')
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

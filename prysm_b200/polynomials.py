@@ -103,3 +103,22 @@ def fringe_to_nm(idx):
     n = m_n // 2 + (idx - g_s) // 2
     m = (m_n - n) * (1 - ((idx - g_s) % 2) * 2)
     return int(n), int(m)
+
+
+# Forbes Q polynomials (prysm/polynomials/__init__.py re-exports the same names from its qpoly module)
+from .qpoly import (  # noqa: E402,F401
+    Qbfs,
+    Qbfs_seq,
+    Qbfs_der,
+    Qbfs_der_seq,
+    Qcon,
+    Qcon_seq,
+    Qcon_der,
+    Qcon_der_seq,
+    Q2d,
+    Q2d_seq,
+    Q2d_der,
+    Q2d_der_seq,
+    Q2d_der_xy,
+    Q2d_der_xy_seq,
+)
