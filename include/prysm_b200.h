@@ -638,6 +638,57 @@ int pb_qpoly_sum(pb_handle_t h, int dtype, int family, const void* u, const void
                  void* stream);
 int pb_qpoly_tables(int family, int m, int nmax, double* out);
 
+/* ---- Orthogonal polynomials, Zernike derivatives and polynomial sums (prysm/polynomials) ---------------------------
+ * The 1-D families are one three-term recurrence P_k = (A_k x + B_k) P_{k-1} - C_k P_{k-2}, run once per sample in
+ * fp64 registers by one kernel; outputs are rounded once to dtype.  Orders are limited to 0 <= n <= 120: n < 0 is
+ * PB_ERR_INVALID, n > 120 PB_ERR_UNSUPPORTED, both before any launch.  Each call is one launch.
+ * pb_jacobi_seq (above) is served by the same kernel.
+ * pb_poly_seq: k HOST orders n_host in any order, repeats allowed; alpha is Jacobi's and Laguerre's alpha and Dickson's
+ *   alpha, beta Jacobi's beta (ignored otherwise).
+ *   kind PB_POLY_VALUE:     plane q of out (k, count) = P_{n_q}(x)
+ *   kind PB_POLY_DER:       plane q = dP_{n_q}/dx by the reference's route: Jacobi 0.5 (n + a + b + 1) P_{n-1}^(a+1,b+1),
+ *                           Hermite kind n P_{n-1}, Laguerre -L_{n-1}^(a+1), the others the differentiated recurrence
+ *   kind PB_POLY_VALUE_DER: planes 0..k-1 = P, k..2k-1 = dP/dx by the differentiated recurrence (jacobi_seq_with_der)
+ *   k (2k for PB_POLY_VALUE_DER) <= 1024.
+ * pb_jacobi_radial_sum: z = sum_q coefs[q] P_{n_q}^(alpha,beta)(u), u = 2 (x^2 + y^2) / radius^2 - 1, zero coefficients
+ *   skipped; with dzdx and dzdy (both or neither) also dz/du 4x / radius^2 and dz/du 4y / radius^2, dz/du by the
+ *   differentiated recurrence in the same pass.  (jacobi_radial_sum, jacobi_radial_sum_der_xy.)
+ * pb_jacobi_clenshaw: Clenshaw's backward recurrence over the len (<= 121) HOST coefficients s_host for the sum and its
+ *   first j (<= 8) derivatives, N = max(len, 2); table != 0: every alpha plane (jj, n) into out (j + 1, N, count), rows
+ *   jj > len - 1 zero; table = 0: the sum alone into out (count).  (jacobi_sum_clenshaw, jacobi_sum_clenshaw_der.)
+ * pb_zernike_der: the (n, m) pairs' derivatives into out (k, 2, count): cartesian = 0, (a, b) = (r, t): dZ/dr, dZ/dt;
+ *   cartesian = 1, (a, b) = (x, y): dZ/dx, dZ/dy through Re / Im (x + iy)^|m|, finite at the origin.  norm as
+ *   pb_zernike_seq.  One launch per Zernike plan.  (zernike_nm_der_seq, zernike_nm_der_xy_seq.)
+ * pb_zernike_sum_der_xy: W, dW/dx, dW/dy of W = sum_q coefs[q] Z_q(x, y) into out (3, count) without the basis;
+ *   duplicate (n, m) pairs add, zero coefficients are skipped.  One launch per Zernike plan.  (zernike_sum_der_xy.)
+ * pb_xy_seq: plane q of out (k, count) is d^a/dx^a d^b/dy^b x^m y^n, (a, b) = bits 0 and 1 of kind_host[q];
+ *   separable != 0: the grid is (count / nx, nx), x[column] and y[row]; otherwise x and y are elementwise.
+ * pb_tensor_sum: z = sum_q coefs[q] P_{m_q}(x) P_{n_q}(y), P the monomials (PB_TSUM_MONOMIAL) or Chebyshev-1
+ *   (PB_TSUM_CHEBY1), (max m + 1)(max n + 1) <= 1024; with dzdx and dzdy also dz/dx / x_norm and dz/dy / y_norm.  Grid
+ *   as pb_xy_seq.  (xy_sum, xy_sum_der_xy, cheby1_2d_sum, cheby1_2d_sum_der_xy.) */
+typedef enum {
+    PB_POLY_JACOBI = 0, PB_POLY_CHEBY1 = 1, PB_POLY_CHEBY2 = 2, PB_POLY_CHEBY3 = 3, PB_POLY_CHEBY4 = 4, PB_POLY_LEGENDRE = 5,
+    PB_POLY_HERMITE_HE = 6, PB_POLY_HERMITE_H = 7, PB_POLY_LAGUERRE = 8, PB_POLY_DICKSON1 = 9, PB_POLY_DICKSON2 = 10
+} pb_poly_family;
+typedef enum { PB_POLY_VALUE = 0, PB_POLY_DER = 1, PB_POLY_VALUE_DER = 2 } pb_poly_kind;
+typedef enum { PB_TSUM_MONOMIAL = 0, PB_TSUM_CHEBY1 = 1 } pb_tsum_basis;
+int pb_poly_seq(pb_handle_t h, int dtype, int family, int kind, double alpha, double beta, const void* x, long long count,
+                int k, const int* n_host, void* out, void* stream);
+int pb_jacobi_radial_sum(pb_handle_t h, int dtype, double alpha, double beta, const void* x, const void* y, long long count,
+                         int k, const int* n_host, const double* coefs_host, double radius, void* z, void* dzdx, void* dzdy,
+                         void* stream);
+int pb_jacobi_clenshaw(pb_handle_t h, int dtype, double alpha, double beta, const void* x, long long count, int len,
+                       const double* s_host, int j, int table, void* out, void* stream);
+int pb_zernike_der(pb_handle_t h, int dtype, int cartesian, const void* a, const void* b, long long count, int k,
+                   const int* n_host, const int* m_host, int norm, void* out, void* stream);
+int pb_zernike_sum_der_xy(pb_handle_t h, int dtype, const void* x, const void* y, long long count, int k, const int* n_host,
+                          const int* m_host, const double* coefs_host, int norm, void* out, void* stream);
+int pb_xy_seq(pb_handle_t h, int dtype, const void* x, const void* y, long long count, long long nx, int separable, int k,
+              const int* m_host, const int* n_host, const int* kind_host, void* out, void* stream);
+int pb_tensor_sum(pb_handle_t h, int dtype, int basis, const void* x, const void* y, long long count, long long nx,
+                  int separable, int k, const int* m_host, const int* n_host, const double* coefs_host, double x_norm,
+                  double y_norm, void* z, void* dzdx, void* dzdy, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

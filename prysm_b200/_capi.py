@@ -124,6 +124,16 @@ SIGNATURES = {
     'pb_qpoly_sum': (_i, [_vp, _i, _i, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_d), _vp, _vp, _vp,
                           _vp]),
     'pb_qpoly_tables': (_i, [_i, _i, _i, C.POINTER(_d)]),
+    'pb_poly_seq': (_i, [_vp, _i, _i, _i, _d, _d, _vp, _ll, _i, C.POINTER(_i), _vp, _vp]),
+    'pb_jacobi_radial_sum': (_i, [_vp, _i, _d, _d, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_d), _d, _vp, _vp, _vp,
+                                  _vp]),
+    'pb_jacobi_clenshaw': (_i, [_vp, _i, _d, _d, _vp, _ll, _i, C.POINTER(_d), _i, _i, _vp, _vp]),
+    'pb_zernike_der': (_i, [_vp, _i, _i, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_i), _i, _vp, _vp]),
+    'pb_zernike_sum_der_xy': (_i, [_vp, _i, _vp, _vp, _ll, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_d), _i, _vp,
+                                   _vp]),
+    'pb_xy_seq': (_i, [_vp, _i, _vp, _vp, _ll, _ll, _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), _vp, _vp]),
+    'pb_tensor_sum': (_i, [_vp, _i, _i, _vp, _vp, _ll, _ll, _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_d), _d, _d,
+                           _vp, _vp, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -147,6 +157,12 @@ SH_F32, SH_F64, SH_U16, SH_I32 = range(4)
 QPOLY_BFS, QPOLY_CON, QPOLY_2D = range(3)
 QPOLY_VALUE, QPOLY_DER, QPOLY_DER_XY = range(3)
 QPOLY_NMAX = 64
+(POLY_JACOBI, POLY_CHEBY1, POLY_CHEBY2, POLY_CHEBY3, POLY_CHEBY4, POLY_LEGENDRE, POLY_HERMITE_HE, POLY_HERMITE_H,
+ POLY_LAGUERRE, POLY_DICKSON1, POLY_DICKSON2) = range(11)
+POLY_VALUE, POLY_DER, POLY_VALUE_DER = range(3)
+POLY_NMAX = 120
+CLENSHAW_JMAX = 8
+TSUM_MONOMIAL, TSUM_CHEBY1 = range(2)
 
 
 def load_library(path=LIB_PATH):

@@ -1389,6 +1389,118 @@ def qpoly_tables(family, m, nmax):
     return out
 
 
+def poly_seq(family, kind, ns, x, alpha=0.0, beta=0.0):
+    """1-D family planes of x's dtype in one launch (pb_poly_seq): (len(ns), *x.shape) of values (POLY_VALUE) or
+    derivatives (POLY_DER), or with POLY_VALUE_DER the pair (values, derivatives).  An empty ns launches nothing."""
+    x = x.contiguous()
+    k = len(ns)
+    both = kind == capi.POLY_VALUE_DER
+    out = torch.empty(((2 if both else 1) * k,) + tuple(x.shape), dtype=x.dtype, device=x.device)
+    if k:
+        n, nptr = _iarr(ns)
+        h, st = _ctx(x)
+        h.check(lib.pb_poly_seq(h.ptr, _CODE[x.dtype], int(family), int(kind), float(alpha), float(beta), _p(x), x.numel(),
+                                k, nptr, _p(out), st))
+    return (out[:k], out[k:]) if both else out
+
+
+def jacobi_radial_sum(coefs, ns, alpha, beta, x, y, radius, want_der):
+    """z (and dz/dx, dz/dy) of sum_q coefs[q] P_{ns[q]}(2 (x^2 + y^2) / R^2 - 1) in one launch (pb_jacobi_radial_sum)."""
+    x = x.contiguous()
+    y = y.to(x.dtype).contiguous()
+    z = torch.empty_like(x)
+    dx = torch.empty_like(x) if want_der else None
+    dy = torch.empty_like(x) if want_der else None
+    k = len(ns)
+    n, nptr = _iarr(ns if k else [0])
+    c, cptr = _darr(coefs if k else [0.0])
+    h, st = _ctx(x)
+    h.check(lib.pb_jacobi_radial_sum(h.ptr, _CODE[x.dtype], float(alpha), float(beta), _p(x), _p(y), x.numel(), k, nptr,
+                                     cptr, float(radius), _p(z), _p(dx), _p(dy), st))
+    return z, dx, dy
+
+
+def jacobi_clenshaw(s, alpha, beta, x, j, table, out=None):
+    """Clenshaw's alphas for sum_n s[n] P_n^(alpha,beta)(x) in one launch (pb_jacobi_clenshaw): with table the whole
+    (j + 1, max(len(s), 2), *x.shape) table (into `out` when given), otherwise the sum alone."""
+    x = x.contiguous()
+    N = max(len(s), 2)
+    shape = ((j + 1, N) + tuple(x.shape)) if table else tuple(x.shape)
+    out = _contiguous_out(out, shape, x)
+    c, cptr = _darr(s if len(s) else [0.0])
+    h, st = _ctx(x)
+    h.check(lib.pb_jacobi_clenshaw(h.ptr, _CODE[x.dtype], float(alpha), float(beta), _p(x), x.numel(), len(s), cptr,
+                                   int(j), int(bool(table)), _p(out), st))
+    return out
+
+
+def zernike_der(nms, a, b, norm, cartesian):
+    """(k, 2, *a.shape): (dZ/dr, dZ/dt) of (r, t), or (dZ/dx, dZ/dy) of (x, y) (pb_zernike_der)."""
+    a = a.contiguous()
+    b = b.to(a.dtype).contiguous()
+    k = len(nms)
+    out = torch.empty((k, 2) + tuple(a.shape), dtype=a.dtype, device=a.device)
+    if k == 0:
+        return out
+    n, nptr = _iarr([nm[0] for nm in nms])
+    m, mptr = _iarr([nm[1] for nm in nms])
+    h, st = _ctx(a)
+    h.check(lib.pb_zernike_der(h.ptr, _CODE[a.dtype], int(bool(cartesian)), _p(a), _p(b), a.numel(), k, nptr, mptr,
+                               int(bool(norm)), _p(out), st))
+    return out
+
+
+def zernike_sum_der_xy(coefs, nms, x, y, norm):
+    """(3, *x.shape): W, dW/dx, dW/dy of sum coefs[q] Z_q(x, y) (pb_zernike_sum_der_xy)."""
+    x = x.contiguous()
+    y = y.to(x.dtype).contiguous()
+    k = len(nms)
+    out = torch.empty((3,) + tuple(x.shape), dtype=x.dtype, device=x.device)
+    n, nptr = _iarr([nm[0] for nm in nms] if k else [0])
+    m, mptr = _iarr([nm[1] for nm in nms] if k else [0])
+    c, cptr = _darr(coefs if k else [0.0])
+    h, st = _ctx(x)
+    h.check(lib.pb_zernike_sum_der_xy(h.ptr, _CODE[x.dtype], _p(x), _p(y), x.numel(), k, nptr, mptr, cptr,
+                                      int(bool(norm)), _p(out), st))
+    return out
+
+
+def xy_seq(ms, ns, kinds, x, y, shape, separable):
+    """XY-monomial planes (len(ms), *shape) (pb_xy_seq); separable: x is the row of nx = shape[-1] values and y the
+    column, otherwise x and y hold one value per sample."""
+    x = x.contiguous()
+    y = y.to(x.dtype).contiguous()
+    k = len(ms)
+    out = torch.empty((k,) + tuple(shape), dtype=x.dtype, device=x.device)
+    if k == 0:
+        return out
+    m, mptr = _iarr(ms)
+    n, nptr = _iarr(ns)
+    kd, kptr = _iarr(kinds)
+    h, st = _ctx(x)
+    h.check(lib.pb_xy_seq(h.ptr, _CODE[x.dtype], _p(x), _p(y), math.prod(shape), int(shape[-1]) if separable else 1,
+                          int(bool(separable)), k, mptr, nptr, kptr, _p(out), st))
+    return out
+
+
+def tensor_sum(basis, coefs, ms, ns, x, y, shape, separable, want_der, x_norm=1.0, y_norm=1.0):
+    """z (and dz/dx / x_norm, dz/dy / y_norm) of sum coefs[q] P_{ms[q]}(x) P_{ns[q]}(y) in one launch (pb_tensor_sum)."""
+    x = x.contiguous()
+    y = y.to(x.dtype).contiguous()
+    z = torch.empty(tuple(shape), dtype=x.dtype, device=x.device)
+    dx = torch.empty_like(z) if want_der else None
+    dy = torch.empty_like(z) if want_der else None
+    k = len(ms)
+    m, mptr = _iarr(ms if k else [0])
+    n, nptr = _iarr(ns if k else [0])
+    c, cptr = _darr(coefs if k else [0.0])
+    h, st = _ctx(x)
+    h.check(lib.pb_tensor_sum(h.ptr, _CODE[x.dtype], int(basis), _p(x), _p(y), math.prod(shape),
+                              int(shape[-1]) if separable else 1, int(bool(separable)), k, mptr, nptr, cptr,
+                              float(x_norm), float(y_norm), _p(z), _p(dx), _p(dy), st))
+    return z, dx, dy
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

@@ -160,6 +160,8 @@ constexpr int route_code(int kind, int L, int flags) { return kind << 28 | L << 
     } while (0)
 
 int ensure_scratch(Handle* h, int slot, size_t bytes, void** out);
+// (A, B, C) of P_{n+1}^(alpha,beta) = (A x + B) P_n - C P_{n-1}, DLMF 18.9 as the reference writes them (synthesis.cu)
+void jacobi_abc(int n, double alpha, double beta, double* abc);
 // amp * exp(2 pi i kturns opd) into the dense complex array out (count elements in rows of nx); opd and amp (pb_amp_kind)
 // have row pitch ld (elements)
 int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, const void* opd, double kturns, long long count,

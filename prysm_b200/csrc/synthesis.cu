@@ -1,6 +1,6 @@
 // Pupil synthesis on the device -- the step before the path (SURVEY.md 8(f) rank 3): coordinate grids, circular
-// masks (binary / one-sample grey edge), Jacobi polynomials by three-term recurrence, Zernike sequences and
-// coefficient-weighted Zernike sums.  All streaming, HBM-bound on their outputs; the recurrences run in fp64
+// masks (binary / one-sample grey edge), Zernike sequences, their polar and Cartesian derivatives and
+// coefficient-weighted Zernike sums with and without slopes (the Jacobi sequences are in orthopoly.cu).  All streaming, HBM-bound on their outputs; the recurrences run in fp64
 // registers whatever the storage precision (the reference runs them in config precision, prysm/polynomials/
 // jacobi.py:147-175, zernike.py:74-181) and are driven by a plan passed in kernel-parameter space, so a launch
 // reads no table from memory and is CUDA-graph capturable.
@@ -62,30 +62,6 @@ __global__ void circle_kernel(const R* __restrict__ r, long long n, R radius, R 
     }
 }
 
-#define PB_JAC_MAX 120
-struct JacobiPlan {
-    double alpha, beta;
-    int nmax;
-    short slot[PB_JAC_MAX + 1];       // output index of order j, or -1
-    double abc[3 * PB_JAC_MAX];       // (A, B, C) of order k-1 for the step that makes P_k, k = 2..nmax at [3*(k-2)]
-};
-
-template <typename R>
-__global__ void jacobi_seq_kernel(const R* __restrict__ x, long long n, const __grid_constant__ JacobiPlan pl, R* __restrict__ out) {
-    PB_GRID_STRIDE(i, n) {
-        const double xv = x[i];
-        double Pm2 = 1.0, Pm1 = pl.alpha + 1.0 + (pl.alpha + pl.beta + 2.0) * ((xv - 1.0) / 2.0);
-        if (pl.slot[0] >= 0) out[(long long)pl.slot[0] * n + i] = (R)Pm2;
-        if (pl.nmax >= 1 && pl.slot[1] >= 0) out[(long long)pl.slot[1] * n + i] = (R)Pm1;
-        for (int k = 2; k <= pl.nmax; ++k) {
-            const double A = pl.abc[3 * (k - 2)], B = pl.abc[3 * (k - 2) + 1], C = pl.abc[3 * (k - 2) + 2];
-            const double Pn = (A * xv + B) * Pm1 - C * Pm2;
-            Pm2 = Pm1; Pm1 = Pn;
-            if (pl.slot[k] >= 0) out[(long long)pl.slot[k] * n + i] = (R)Pn;
-        }
-    }
-}
-
 // Zernike plan: one group per |m| (ascending); per Jacobi order j of a group one step holding the recurrence
 // coefficients that make P_j and the weights of the (at most one) cosine and sine mode of that (|m|, j).
 // m = 0 modes are "cosine" modes of the |m| = 0 group (cos 0 = r^0 = 1).  Every index is warp-uniform, so the
@@ -102,13 +78,23 @@ struct ZernPlan {
 };
 
 // MODE 0: out[k][i] = w * Z_k   (zernike_nm_seq);  MODE 1: out[i] (+)= sum w * Z_k  (zernike_sum, w = c*norm)
-// POLAR: inputs are (r, t); otherwise Cartesian (x, y) with r = hypot, cos t = x/r, sin t = y/r
+// MODE 2 (POLAR): out[k][0|1][i] = w dZ_k/dr, w dZ_k/dt  (zernike_nm_der_seq)
+// MODE 3: out[k][0|1][i] = w dZ_k/dx, w dZ_k/dy  (zernike_nm_der_xy_seq)
+// MODE 4: out[0|1|2][i] (+)= W, dW/dx, dW/dy of W = sum w Z_k  (zernike_sum_der_xy)
+// POLAR: inputs are (r, t); otherwise Cartesian (x, y) with r = hypot, cos t = x/r, sin t = y/r.  The derivative modes
+// carry dP_j/dx2 beside P_j (seed (|m| + 2)/2, the differentiated recurrence); MODE 2 forms r^|m|, r^(|m|-1) and
+// cos / sin(|m| t) per group, MODES 3 and 4 C_k, S_k = Re, Im (x + iy)^k for k = |m| and |m| - 1, finite at the origin.
 template <typename R, int MODE, bool POLAR>
 __global__ void zernike_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, const __grid_constant__ ZernPlan pl,
                                int accumulate, R* __restrict__ out) {
+    constexpr bool DER = MODE >= 2, XY = MODE >= 3;
     PB_GRID_STRIDE(i, n) {
-        double r, c1, s1;
-        if (POLAR) {
+        double r = 0.0, c1 = 1.0, s1 = 0.0, xv = 0.0, yv = 0.0, tv = 0.0;
+        if constexpr (XY) {
+            xv = a[i]; yv = b[i];
+        } else if constexpr (MODE == 2) {
+            r = a[i]; tv = b[i];
+        } else if (POLAR) {
             r = a[i];
             sincos((double)b[i], &s1, &c1);
         } else {
@@ -117,41 +103,100 @@ __global__ void zernike_kernel(const R* __restrict__ a, const R* __restrict__ b,
             c1 = r > 0.0 ? xv / r : 1.0;
             s1 = r > 0.0 ? yv / r : 0.0;
         }
-        const double x2 = 2.0 * (r * r) - 1.0, hx = (x2 - 1.0) / 2.0;
+        const double x2 = XY ? 2.0 * (xv * xv + yv * yv) - 1.0 : 2.0 * (r * r) - 1.0, hx = (x2 - 1.0) / 2.0;
         double rc = 1.0, rs = 0.0;                // r^am cos(am t), r^am sin(am t), advanced group to group
         const double rc1 = r * c1, rs1 = r * s1;
+        double hc1 = 1.0, hs1 = 0.0;              // MODE 3, 4: (rc, rs) = Re, Im (x + iy)^am, (hc1, hs1) of ^(am - 1)
+        double rm = 1.0, rm1 = 1.0, cs = 1.0, sn = 0.0;   // MODE 2: r^am, r^(am - 1), cos(am t), sin(am t)
         int am_now = 0;
-        double acc = 0.0;
+        double acc = 0.0, accx = 0.0, accy = 0.0;
         for (int gi = 0; gi < pl.ngroups; ++gi) {
             const ZernGroup g = pl.g[gi];
             for (; am_now < g.am; ++am_now) {     // (r e^{it})^am by repeated complex multiplication
-                const double t0 = rc * rc1 - rs * rs1;
-                rs = rs * rc1 + rc * rs1;
-                rc = t0;
+                if constexpr (XY) {
+                    hc1 = rc; hs1 = rs;
+                    const double t0 = xv * rc - yv * rs;
+                    rs = xv * rs + yv * rc;
+                    rc = t0;
+                } else if constexpr (MODE == 2) {
+                    rm1 = rm; rm = rm * r;
+                } else {
+                    const double t0 = rc * rc1 - rs * rs1;
+                    rs = rs * rc1 + rc * rs1;
+                    rc = t0;
+                }
             }
+            if constexpr (MODE == 2) sincos((double)g.am * tv, &sn, &cs);
+            const double am = g.am;
             double Pm2 = 1.0, Pm1 = 1.0 + ((double)g.am + 2.0) * hx, P = 1.0;
+            double dPm2 = 0.0, dPm1 = ((double)g.am + 2.0) / 2.0, dP = 0.0;
+            double Sa = 0.0, Sb = 0.0, dSa = 0.0, dSb = 0.0;
             for (int j = 0; j <= g.njmax; ++j) {
                 const int si = g.first + j;
-                if (j == 1) P = Pm1;
+                if (j == 1) { P = Pm1; dP = dPm1; }
                 else if (j >= 2) {
-                    P = (pl.s[si].A * x2 + pl.s[si].B) * Pm1 - pl.s[si].C * Pm2;
+                    if constexpr (DER) {
+                        const double lin = pl.s[si].A * x2 + pl.s[si].B;
+                        P = lin * Pm1 - pl.s[si].C * Pm2;
+                        dP = pl.s[si].A * Pm1 + lin * dPm1 - pl.s[si].C * dPm2;
+                        dPm2 = dPm1; dPm1 = dP;
+                    } else {
+                        P = (pl.s[si].A * x2 + pl.s[si].B) * Pm1 - pl.s[si].C * Pm2;
+                    }
                     Pm2 = Pm1; Pm1 = P;
                 }
-                if (MODE == 1) {
+                if constexpr (MODE == 1) {
                     acc += P * (pl.s[si].wc * rc + pl.s[si].ws * rs);
+                } else if constexpr (MODE == 4) {
+                    Sa += pl.s[si].wc * P; Sb += pl.s[si].ws * P;
+                    dSa += pl.s[si].wc * dP; dSb += pl.s[si].ws * dP;
                 } else {
                     const int kc = pl.kc[si], ks = pl.ks[si];
-                    if (kc >= 0) out[(long long)kc * n + i] = (R)(pl.s[si].wc * P * rc);
-                    if (ks >= 0) out[(long long)ks * n + i] = (R)(pl.s[si].ws * P * rs);
+                    if constexpr (MODE == 0) {
+                        if (kc >= 0) out[(long long)kc * n + i] = (R)(pl.s[si].wc * P * rc);
+                        if (ks >= 0) out[(long long)ks * n + i] = (R)(pl.s[si].ws * P * rs);
+                    } else if constexpr (MODE == 2) {
+                        const double radial = g.am == 0 ? (4.0 * r) * dP : am * rm1 * P + rm * ((4.0 * r) * dP);
+                        if (kc >= 0) {
+                            out[(long long)(2 * kc) * n + i] = (R)(pl.s[si].wc * (radial * cs));
+                            out[(long long)(2 * kc + 1) * n + i] = (R)(g.am == 0 ? 0.0 : pl.s[si].wc * (-am * sn * rm * P));
+                        }
+                        if (ks >= 0) {
+                            out[(long long)(2 * ks) * n + i] = (R)(pl.s[si].ws * (radial * sn));
+                            out[(long long)(2 * ks + 1) * n + i] = (R)(pl.s[si].ws * (am * cs * rm * P));
+                        }
+                    } else {
+                        const double ddx = 4.0 * xv * dP, ddy = 4.0 * yv * dP;
+                        if (kc >= 0) {
+                            out[(long long)(2 * kc) * n + i] = (R)(pl.s[si].wc * (ddx * rc + am * P * hc1));
+                            out[(long long)(2 * kc + 1) * n + i] = (R)(pl.s[si].wc * (ddy * rc - am * P * hs1));
+                        }
+                        if (ks >= 0) {
+                            out[(long long)(2 * ks) * n + i] = (R)(pl.s[si].ws * (ddx * rs + am * P * hs1));
+                            out[(long long)(2 * ks + 1) * n + i] = (R)(pl.s[si].ws * (ddy * rs + am * P * hc1));
+                        }
+                    }
                 }
             }
+            if constexpr (MODE == 4) {
+                const double dH = dSa * rc + dSb * rs;
+                acc += Sa * rc + Sb * rs;
+                accx += 4.0 * xv * dH + am * (Sa * hc1 + Sb * hs1);
+                accy += 4.0 * yv * dH + am * (Sb * hc1 - Sa * hs1);
+            }
         }
-        if (MODE == 1) out[i] = accumulate ? (R)((double)out[i] + acc) : (R)acc;
+        if constexpr (MODE == 1) out[i] = accumulate ? (R)((double)out[i] + acc) : (R)acc;
+        if constexpr (MODE == 4) {
+            if (accumulate) {
+                acc += (double)out[i]; accx += (double)out[n + i]; accy += (double)out[2 * n + i];
+            }
+            out[i] = (R)acc; out[n + i] = (R)accx; out[2 * n + i] = (R)accy;
+        }
     }
 }
 
 // DLMF 18.9 coefficients as the reference writes them (prysm/polynomials/jacobi.py:13-39)
-static void recurrence_abc(int n, double alpha, double beta, double* abc) {
+void jacobi_abc(int n, double alpha, double beta, double* abc) {
     const double apb = alpha + beta;
     if (n == 0 && (apb == 0.0 || apb == -1.0)) {
         abc[0] = 0.5 * (alpha + beta) + 1.0; abc[1] = 0.5 * (alpha - beta); abc[2] = 1.0;
@@ -188,7 +233,7 @@ static int next_plan(std::vector<HostTerm>& terms, ZernPlan& pl) {
         for (int j = 0; j <= njmax; ++j) {
             ZernStep& st = pl.s[nsteps + j];
             double abc[3] = {0.0, 0.0, 0.0};
-            if (j >= 2) recurrence_abc(j - 1, 0.0, (double)g.am, abc);
+            if (j >= 2) jacobi_abc(j - 1, 0.0, (double)g.am, abc);
             st.A = abc[0]; st.B = abc[1]; st.C = abc[2]; st.wc = 0.0; st.ws = 0.0;
             pl.kc[nsteps + j] = -1; pl.ks[nsteps + j] = -1;
         }
@@ -267,30 +312,13 @@ extern "C" int pb_circle(pb_handle_t hh, int dtype, const void* r, long long cou
     return PB_OK;
 }
 
-extern "C" int pb_jacobi_seq(pb_handle_t hh, int dtype, const void* x, long long count, int nmax, double alpha, double beta,
-                             const int* slots_host, void* out, void* stream) {
-    PB_HANDLE(hh);
-    if (!x || !out || !slots_host || nmax < 0) return fail(h, PB_ERR_INVALID, "bad jacobi arguments");
-    if (nmax > PB_JAC_MAX) return fail(h, PB_ERR_UNSUPPORTED, "jacobi order above 120");
-    if (count <= 0) return PB_OK;
-    JacobiPlan pl;
-    pl.alpha = alpha; pl.beta = beta; pl.nmax = nmax;
-    for (int j = 0; j <= PB_JAC_MAX; ++j) pl.slot[j] = j <= nmax ? (short)slots_host[j] : (short)-1;
-    for (int k = 2; k <= nmax; ++k) recurrence_abc(k - 1, alpha, beta, pl.abc + 3 * (k - 2));
-    const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) jacobi_seq_kernel<float><<<g, 256, 0, st>>>((const float*)x, count, pl, (float*)out);
-    else jacobi_seq_kernel<double><<<g, 256, 0, st>>>((const double*)x, count, pl, (double*)out);
-    PB_LAUNCH_CHECK(h);
-    return PB_OK;
-}
-
 template <int MODE>
 static int run_zernike(Handle* h, int dtype, int polar, const void* a, const void* b, long long count,
                        std::vector<HostTerm>& terms, void* out, cudaStream_t st) {
     const int g = grid_for(count, 256, h->sm_count);
     int launches = 0;
-    if (MODE == 1 && terms.empty()) {      // all weights zero: the sum is zero
-        PB_CUDA(h, cudaMemsetAsync(out, 0, (size_t)count * (dtype == PB_C64 ? 4 : 8), st));
+    if ((MODE == 1 || MODE == 4) && terms.empty()) {      // all weights zero: the sum (and its slopes) is zero
+        PB_CUDA(h, cudaMemsetAsync(out, 0, (size_t)count * (dtype == PB_C64 ? 4 : 8) * (MODE == 4 ? 3 : 1), st));
         return PB_OK;
     }
     while (!terms.empty()) {
@@ -330,4 +358,43 @@ extern "C" int pb_zernike_sum(pb_handle_t hh, int dtype, int polar, const void* 
     std::vector<HostTerm> terms;
     PB_TRY(build_terms(h, k, n_host, m_host, coefs_host, norm, terms));
     return run_zernike<1>(h, dtype, polar, a, b, count, terms, out, st);
+}
+
+// a radial order no plan can hold is refused before the first of several launches
+static int zernike_fits(Handle* h, const std::vector<HostTerm>& terms) {
+    for (const HostTerm& t : terms)
+        if (t.nj + 1 > PB_ZERN_STEPS) return fail(h, PB_ERR_UNSUPPORTED, "zernike: (n - |m|)/2 above 71");
+    return PB_OK;
+}
+
+extern "C" int pb_zernike_der(pb_handle_t hh, int dtype, int cartesian, const void* a, const void* b, long long count, int k,
+                              const int* n_host, const int* m_host, int norm, void* out, void* stream) {
+    PB_HANDLE(hh);
+    if (!a || !b || !out || k < 1 || !n_host || !m_host) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
+    if (k > 16383) return fail(h, PB_ERR_UNSUPPORTED, "more than 16383 modes");
+    std::vector<HostTerm> terms;
+    PB_TRY(build_terms(h, k, n_host, m_host, nullptr, norm, terms));
+    PB_TRY(zernike_fits(h, terms));
+    if (count <= 0) return PB_OK;
+    if (cartesian) return run_zernike<3>(h, dtype, 0, a, b, count, terms, out, st);
+    return run_zernike<2>(h, dtype, 1, a, b, count, terms, out, st);
+}
+
+extern "C" int pb_zernike_sum_der_xy(pb_handle_t hh, int dtype, const void* x, const void* y, long long count, int k,
+                                     const int* n_host, const int* m_host, const double* coefs_host, int norm, void* out,
+                                     void* stream) {
+    PB_HANDLE(hh);
+    if (!x || !y || !out || k < 0 || (k > 0 && (!n_host || !m_host || !coefs_host))) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
+    std::vector<HostTerm> terms, merged;
+    PB_TRY(build_terms(h, k, n_host, m_host, coefs_host, norm, terms));
+    // duplicate (n, m) pairs add their weights, in input order, as zernike.py:574-584 does
+    for (const HostTerm& t : terms) {
+        auto same = [&](const HostTerm& u) { return u.am == t.am && u.nj == t.nj && u.trig == t.trig; };
+        auto it = std::find_if(merged.begin(), merged.end(), same);
+        if (it == merged.end()) merged.push_back({t.am, t.nj, t.trig, t.k, 0.0 + t.scale});
+        else it->scale += t.scale;
+    }
+    PB_TRY(zernike_fits(h, merged));
+    if (count <= 0) return PB_OK;
+    return run_zernike<4>(h, dtype, 0, x, y, count, merged, out, st);
 }
