@@ -11,15 +11,6 @@
 
 namespace pb {
 
-static inline int grid_for(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
-#define PB_GRID_STRIDE(i, n) \
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (n); i += (long long)gridDim.x * blockDim.x)
-
 template <typename R>
 __global__ void mask_multiply_kernel(const cplx<R>* __restrict__ a, const cplx<R>* __restrict__ b, const void* __restrict__ m,
                                      int m_kind, int flags, const R* __restrict__ w, R scale, long long n, void* out) {
@@ -265,48 +256,45 @@ __global__ void radial_window_kernel(int ny, int nx, double fdx, double shift, d
 
 using namespace pb;
 
-#define PB_HANDLE(hh)                                   \
-    PB_ENTER(hh);                      \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_mask_multiply(pb_handle_t hh, int dtype, const void* a, const void* b, const void* m, int m_kind, int flags,
                                 const void* w, double scale, long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !out || (m && m_kind != PB_MASK_REAL && m_kind != PB_MASK_COMPLEX) || (flags & ~15))
         return fail(h, PB_ERR_INVALID, "bad masked-multiply arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64)
-        mask_multiply_kernel<float><<<g, 256, 0, st>>>((const float2*)a, (const float2*)b, m, m_kind, flags, (const float*)w, (float)scale, count, out);
-    else
-        mask_multiply_kernel<double><<<g, 256, 0, st>>>((const double2*)a, (const double2*)b, m, m_kind, flags, (const double*)w, scale, count, out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        mask_multiply_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)a, (const cplx<R>*)b, m, m_kind, flags, (const R*)w, (R)scale, count, out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_field_adjoint(pb_handle_t hh, int dtype, int mode, const void* field, const void* bar, const void* opd,
                                 double kscale, long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (mode < 0 || mode > 2 || !bar || !out || (mode < 2 && !field) || (mode == 2 && !opd))
         return fail(h, PB_ERR_INVALID, "bad field-adjoint arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64)
-        field_adjoint_kernel<float><<<g, 256, 0, st>>>(mode, (const float2*)field, (const float2*)bar, (const float*)opd, kscale, count, out);
-    else
-        field_adjoint_kernel<double><<<g, 256, 0, st>>>(mode, (const double2*)field, (const double2*)bar, (const double*)opd, kscale, count, out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        field_adjoint_kernel<R><<<g, 256, 0, st>>>(mode, (const cplx<R>*)field, (const cplx<R>*)bar, (const R*)opd, kscale, count, out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_component(pb_handle_t hh, int dtype, int which, const void* in, long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (which < 0 || which > 3 || !in || !out) return fail(h, PB_ERR_INVALID, "bad component arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) component_kernel<float><<<g, 256, 0, st>>>(which, (const float2*)in, count, (float*)out);
-    else component_kernel<double><<<g, 256, 0, st>>>(which, (const double2*)in, count, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        component_kernel<R><<<g, 256, 0, st>>>(which, (const cplx<R>*)in, count, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -322,15 +310,17 @@ static int zeroed_sums(Handle* h, int nd, cudaStream_t st, double** out) {
 
 extern "C" int pb_dot(pb_handle_t hh, int dtype, const void* a, const void* b, const void* w, long long count,
                       double* out_host, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !b || !out_host || count < 0) return fail(h, PB_ERR_INVALID, "bad dot arguments");
     out_host[0] = out_host[1] = 0.0;
     if (count == 0) return PB_OK;
     double* sums = nullptr;
     PB_TRY(zeroed_sums(h, 2, st, &sums));
     const int g = (int)std::min<long long>((count + 255) / 256, (long long)h->sm_count * 4);
-    if (dtype == PB_C64) dot_kernel<float><<<g, 256, 0, st>>>((const float2*)a, (const float2*)b, (const float*)w, count, sums);
-    else dot_kernel<double><<<g, 256, 0, st>>>((const double2*)a, (const double2*)b, (const double*)w, count, sums);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        dot_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)a, (const cplx<R>*)b, (const R*)w, count, sums);
+    });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
     PB_CUDA(h, cudaStreamSynchronize(st));
@@ -339,14 +329,16 @@ extern "C" int pb_dot(pb_handle_t hh, int dtype, const void* a, const void* b, c
 
 extern "C" int pb_mode_projection(pb_handle_t hh, int dtype, const void* modes, int k, long long count, const void* bar,
                                   int bar_complex, double* out_host, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (k < 1 || count <= 0 || !modes || !bar || !out_host) return fail(h, PB_ERR_INVALID, "bad mode-projection arguments");
     double* sums = nullptr;
     PB_TRY(zeroed_sums(h, 2 * k, st, &sums));
     const int gx = (int)std::min<long long>((count + 255) / 256, std::max(1LL, (long long)h->sm_count * 4 / k));
     dim3 g(gx, k);
-    if (dtype == PB_C64) mode_projection_kernel<float><<<g, 256, 0, st>>>((const float*)modes, count, bar, bar_complex, sums);
-    else mode_projection_kernel<double><<<g, 256, 0, st>>>((const double*)modes, count, bar, bar_complex, sums);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        mode_projection_kernel<R><<<g, 256, 0, st>>>((const R*)modes, count, bar, bar_complex, sums);
+    });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, sums, (size_t)2 * k * sizeof(double), cudaMemcpyDeviceToHost, st));
     PB_CUDA(h, cudaStreamSynchronize(st));
@@ -355,7 +347,7 @@ extern "C" int pb_mode_projection(pb_handle_t hh, int dtype, const void* modes, 
 
 extern "C" int pb_otf_adjoint_seed(pb_handle_t hh, int dtype, int which, const void* bar, const void* D, int ny, int nx,
                                    void* data_bar, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if ((which != 1 && which != 2 && which != 4) || !bar || !D || !data_bar || ny < 1 || nx < 1)
         return fail(h, PB_ERR_INVALID, "bad otf-adjoint arguments");
     const long long n = (long long)ny * nx, centre = (long long)(ny / 2) * nx + nx / 2;
@@ -363,13 +355,11 @@ extern "C" int pb_otf_adjoint_seed(pb_handle_t hh, int dtype, int which, const v
     PB_TRY(zeroed_sums(h, 2, st, &sums));
     const int gr = (int)std::min<long long>((n + 255) / 256, (long long)h->sm_count * 4);
     const int g = grid_for(n, 256, h->sm_count);
-    if (dtype == PB_C64) {
-        otf_adjoint_reduce_kernel<float><<<gr, 256, 0, st>>>(which, bar, (const float2*)D, n, sums);
-        otf_adjoint_apply_kernel<float><<<g, 256, 0, st>>>(which, bar, (const float2*)D, n, centre, sums, (float2*)data_bar);
-    } else {
-        otf_adjoint_reduce_kernel<double><<<gr, 256, 0, st>>>(which, bar, (const double2*)D, n, sums);
-        otf_adjoint_apply_kernel<double><<<g, 256, 0, st>>>(which, bar, (const double2*)D, n, centre, sums, (double2*)data_bar);
-    }
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        otf_adjoint_reduce_kernel<R><<<gr, 256, 0, st>>>(which, bar, (const cplx<R>*)D, n, sums);
+        otf_adjoint_apply_kernel<R><<<g, 256, 0, st>>>(which, bar, (const cplx<R>*)D, n, centre, sums, (cplx<R>*)data_bar);
+    });
     PB_LAUNCH_CHECK(h);
     h->launches++;
     return PB_OK;
@@ -377,7 +367,7 @@ extern "C" int pb_otf_adjoint_seed(pb_handle_t hh, int dtype, int which, const v
 
 extern "C" int pb_encircled_energy_adjoint_seed(pb_handle_t hh, int dtype, int ny, int nx, double df, const double* radii_mm_host,
                                                 const double* ee_bar_host, int nr, void* mtf_bar, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nr < 1 || !radii_mm_host || !ee_bar_host || !mtf_bar) return fail(h, PB_ERR_INVALID, "bad encircled-energy adjoint arguments");
     void* d = nullptr;
     PB_TRY(ensure_scratch(h, 2, (size_t)2 * nr * sizeof(double), &d));
@@ -386,8 +376,10 @@ extern "C" int pb_encircled_energy_adjoint_seed(pb_handle_t hh, int dtype, int n
     PB_CUDA(h, cudaMemcpyAsync(dr, radii_mm_host, nr * sizeof(double), cudaMemcpyHostToDevice, st));
     PB_CUDA(h, cudaMemcpyAsync(db, ee_bar_host, nr * sizeof(double), cudaMemcpyHostToDevice, st));
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) ee_adjoint_seed_kernel<float><<<g, 256, 0, st>>>(ny, nx, df, dr, db, nr, (float*)mtf_bar);
-    else ee_adjoint_seed_kernel<double><<<g, 256, 0, st>>>(ny, nx, df, dr, db, nr, (double*)mtf_bar);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        ee_adjoint_seed_kernel<R><<<g, 256, 0, st>>>(ny, nx, df, dr, db, nr, (R*)mtf_bar);
+    });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaStreamSynchronize(st));   // the host arrays may go away after the call
     return PB_OK;
@@ -395,12 +387,14 @@ extern "C" int pb_encircled_energy_adjoint_seed(pb_handle_t hh, int dtype, int n
 
 extern "C" int pb_vortex_phase(pb_handle_t hh, int dtype, int charge, const void* xf, const void* yf, long long count, void* out,
                                void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!xf || !yf || !out) return fail(h, PB_ERR_INVALID, "bad vortex arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) vortex_kernel<float><<<g, 256, 0, st>>>(charge, (const float*)xf, (const float*)yf, count, (float2*)out);
-    else vortex_kernel<double><<<g, 256, 0, st>>>(charge, (const double*)xf, (const double*)yf, count, (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        vortex_kernel<R><<<g, 256, 0, st>>>(charge, (const R*)xf, (const R*)yf, count, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -408,27 +402,28 @@ extern "C" int pb_vortex_phase(pb_handle_t hh, int dtype, int charge, const void
 extern "C" int pb_resample_bilinear(pb_handle_t hh, int dtype, const void* map, int ny, int nx, const void* xf, const void* yf,
                                     long long count, double cx, double cy, double dx, const void* fill, double fill_re,
                                     double fill_im, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!map || !xf || !yf || !out || ny < 1 || nx < 1 || dx == 0.0) return fail(h, PB_ERR_INVALID, "bad resample arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64)
-        resample_bilinear_kernel<float><<<g, 256, 0, st>>>((const float2*)map, ny, nx, (const float*)xf, (const float*)yf, count, cx, cy, dx,
-                                                            (const float2*)fill, make_float2((float)fill_re, (float)fill_im), (float2*)out);
-    else
-        resample_bilinear_kernel<double><<<g, 256, 0, st>>>((const double2*)map, ny, nx, (const double*)xf, (const double*)yf, count, cx, cy,
-                                                             dx, (const double2*)fill, make_double2(fill_re, fill_im), (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        resample_bilinear_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)map, ny, nx, (const R*)xf, (const R*)yf, count, cx, cy, dx,
+                                                       (const cplx<R>*)fill, mk<R>((R)fill_re, (R)fill_im), (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_radial_window(pb_handle_t hh, int dtype, int ny, int nx, double fdx, double shift, double a0, double b0,
                                 double a1, double b1, void* win, void* xf, void* yf, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1) return fail(h, PB_ERR_INVALID, "bad window shape");
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) radial_window_kernel<float><<<g, 256, 0, st>>>(ny, nx, fdx, shift, a0, b0, a1, b1, (float*)win, (float*)xf, (float*)yf);
-    else radial_window_kernel<double><<<g, 256, 0, st>>>(ny, nx, fdx, shift, a0, b0, a1, b1, (double*)win, (double*)xf, (double*)yf);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        radial_window_kernel<R><<<g, 256, 0, st>>>(ny, nx, fdx, shift, a0, b0, a1, b1, (R*)win, (R*)xf, (R*)yf);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

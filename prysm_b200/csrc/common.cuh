@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
+#include <algorithm>
 #include <cstdint>
 #include <complex>
 #include <cstdio>
@@ -126,6 +127,31 @@ struct NvtxRange {
     if (!h) return PB_ERR_INVALID;                           \
     pb::DeviceGuard pb_guard_(h->device);                    \
     pb::NvtxRange pb_range_(__func__)
+
+// PB_ENTER for an entry point whose `dtype` selects fp32 (PB_C64) or fp64 (PB_C128) data and which takes `stream`
+#define PB_ENTER_REAL(hh)                                                                                      \
+    PB_ENTER(hh);                                                                                              \
+    if (dtype != PB_C64 && dtype != PB_C128) return pb::fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
+
+// blocks of a grid-stride launch over n items: enough to cover them, at most 16 per SM
+inline int grid_for(long long n, int threads, int sm_count) {
+    const long long g = (n + threads - 1) / threads;
+    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
+}
+
+#define PB_GRID_STRIDE(i, n) \
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (n); i += (long long)gridDim.x * blockDim.x)
+
+// calls f(float{}) for PB_C64 and f(double{}) for PB_C128; false for any other dtype.  A launch pair is written once
+// as with_real(dtype, [&](auto r) { using R = decltype(r); kernel<R><<<...>>>(...); }), with PB_LAUNCH_CHECK after
+// the call: it returns an error code, which the void lambda cannot.
+template <typename F>
+bool with_real(int dtype, F&& f) {
+    if (dtype == PB_C64) { f(float{}); return true; }
+    if (dtype == PB_C128) { f(double{}); return true; }
+    return false;
+}
 
 // true the first time a kernel is seen on this handle: the caller then sets its opt-in attributes
 inline bool attr_needed(Handle* h, const void* fn) { return h->attr_done.insert(fn).second; }

@@ -159,11 +159,6 @@ __global__ void dm_gather_kernel(const void* __restrict__ in, bool cplx_in, int 
     }
 }
 
-inline int grid_for(long long n, int threads, int sm_count) {
-    const long long g = (n + threads - 1) / threads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 // both axes of the prefilter into `coef` (ny, nx) fp64, through `tmp` (ny, nx) fp64
 template <typename R>
 int spline_prefilter(Handle* h, const void* in, bool cplx_in, int ny, int nx, double* tmp, double* coef, cudaStream_t st) {
@@ -186,25 +181,23 @@ int spline_prefilter(Handle* h, const void* in, bool cplx_in, int ny, int nx, do
 
 using namespace pb;
 
-#define PB_DM_ENTER(hh)                                                                                   \
-    PB_ENTER(hh);                                                                                         \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_spline_prefilter(pb_handle_t hh, int dtype, const void* in, int in_complex, int ny, int nx, double* coef,
                                    void* stream) {
-    PB_DM_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (!in || !coef || ny < 1 || nx < 1) return fail(h, PB_ERR_INVALID, "bad prefilter arguments");
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 1, (size_t)ny * nx * sizeof(double), &tmp));
-    if (dtype == PB_C64) return spline_prefilter<float>(h, in, in_complex != 0, ny, nx, (double*)tmp, coef, st);
-    return spline_prefilter<double>(h, in, in_complex != 0, ny, nx, (double*)tmp, coef, st);
+    int rc = PB_OK;
+    with_real(dtype, [&](auto r) {
+        rc = spline_prefilter<decltype(r)>(h, in, in_complex != 0, ny, nx, (double*)tmp, coef, st);
+    });
+    return rc;
 }
 
 extern "C" int pb_warp(pb_handle_t hh, int dtype, const void* in, int in_complex, int ny, int nx, const void* xc,
                        const void* yc, int coord_dtype, const double* matrix_host, int oy, int ox, double scale, void* out,
                        void* stream) {
-    PB_DM_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (!in || !out || ny < 1 || nx < 1 || oy < 0 || ox < 0) return fail(h, PB_ERR_INVALID, "bad warp arguments");
     if ((xc == nullptr) != (yc == nullptr)) return fail(h, PB_ERR_INVALID, "give both coordinate arrays or neither");
     if (!xc && !matrix_host) return fail(h, PB_ERR_INVALID, "warp needs coordinate arrays or a projection matrix");
@@ -216,49 +209,48 @@ extern "C" int pb_warp(pb_handle_t hh, int dtype, const void* in, int in_complex
     Mat3 M{};
     if (!xc) for (int i = 0; i < 9; ++i) M.m[i] = matrix_host[i];
     const int g = grid_for((long long)oy * ox, 256, h->sm_count);
-    if (dtype == PB_C64) {
-        PB_TRY(spline_prefilter<float>(h, in, in_complex != 0, ny, nx, (double*)tmp, (double*)coef, st));
-        if (coord_dtype == PB_C64)
-            spline_interp_kernel<float, float><<<g, 256, 0, st>>>((const double*)coef, ny, nx, (const float*)xc, (const float*)yc, M,
-                                                                  oy, ox, scale, (float*)out);
-        else
-            spline_interp_kernel<float, double><<<g, 256, 0, st>>>((const double*)coef, ny, nx, (const double*)xc, (const double*)yc,
-                                                                   M, oy, ox, scale, (float*)out);
-    } else {
-        PB_TRY(spline_prefilter<double>(h, in, in_complex != 0, ny, nx, (double*)tmp, (double*)coef, st));
-        if (coord_dtype == PB_C64)
-            spline_interp_kernel<double, float><<<g, 256, 0, st>>>((const double*)coef, ny, nx, (const float*)xc, (const float*)yc,
-                                                                   M, oy, ox, scale, (double*)out);
-        else
-            spline_interp_kernel<double, double><<<g, 256, 0, st>>>((const double*)coef, ny, nx, (const double*)xc,
-                                                                    (const double*)yc, M, oy, ox, scale, (double*)out);
-    }
+    int rc = PB_OK;
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        rc = spline_prefilter<R>(h, in, in_complex != 0, ny, nx, (double*)tmp, (double*)coef, st);
+        if (rc != PB_OK) return;
+        with_real(coord_dtype, [&](auto c) {
+            using C = decltype(c);
+            spline_interp_kernel<R, C><<<g, 256, 0, st>>>((const double*)coef, ny, nx, (const C*)xc, (const C*)yc, M, oy, ox,
+                                                          scale, (R*)out);
+        });
+    });
+    PB_TRY(rc);
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_dm_scatter(pb_handle_t hh, int dtype, const void* act, int nay, int nax, int ny, int nx, int y0, int sy,
                              int x0, int sx, void* poke, void* stream) {
-    PB_DM_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (!act || !poke || nay < 1 || nax < 1 || ny < 1 || nx < 1 || sy < 1 || sx < 1 || y0 < 0 || x0 < 0 ||
         y0 + (long long)(nay - 1) * sy >= ny || x0 + (long long)(nax - 1) * sx >= nx)
         return fail(h, PB_ERR_INVALID, "actuator lattice does not fit the poke grid");
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) dm_scatter_kernel<float><<<g, 256, 0, st>>>((const float*)act, nay, nax, ny, nx, y0, sy, x0, sx, (float*)poke);
-    else dm_scatter_kernel<double><<<g, 256, 0, st>>>((const double*)act, nay, nax, ny, nx, y0, sy, x0, sx, (double*)poke);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        dm_scatter_kernel<R><<<g, 256, 0, st>>>((const R*)act, nay, nax, ny, nx, y0, sy, x0, sx, (R*)poke);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_dm_gather(pb_handle_t hh, int dtype, const void* in, int in_complex, int ny, int nx, int nay, int nax, int y0,
                             int sy, int x0, int sx, void* act, void* stream) {
-    PB_DM_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (!in || !act || nay < 1 || nax < 1 || ny < 1 || nx < 1 || sy < 1 || sx < 1 || y0 < 0 || x0 < 0 ||
         y0 + (long long)(nay - 1) * sy >= ny || x0 + (long long)(nax - 1) * sx >= nx)
         return fail(h, PB_ERR_INVALID, "actuator lattice does not fit the array");
     const int g = grid_for((long long)nay * nax, 256, h->sm_count);
-    if (dtype == PB_C64) dm_gather_kernel<float><<<g, 256, 0, st>>>(in, in_complex != 0, nx, nay, nax, y0, sy, x0, sx, (float*)act);
-    else dm_gather_kernel<double><<<g, 256, 0, st>>>(in, in_complex != 0, nx, nay, nax, y0, sy, x0, sx, (double*)act);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        dm_gather_kernel<R><<<g, 256, 0, st>>>(in, in_complex != 0, nx, nay, nax, y0, sy, x0, sx, (R*)act);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

@@ -6,12 +6,6 @@
 
 namespace pb {
 
-static inline int grid_for(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;  // grid-stride beyond a few waves
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
 // out[i] = amp * exp(2 pi i kturns opd) over the n elements of a dense array of rows of nx; opd and amp are read with
 // row pitch ld (elements)
 template <typename R>
@@ -34,8 +28,10 @@ __global__ void phase_screen_kernel(const void* amp, int amp_kind, const R* __re
 int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, const void* opd, double kturns, long long count,
                         long long nx, long long ld, void* out, cudaStream_t st) {
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) phase_screen_kernel<float><<<g, 256, 0, st>>>(amp, amp_kind, (const float*)opd, kturns, count, nx, ld, (float2*)out);
-    else phase_screen_kernel<double><<<g, 256, 0, st>>>(amp, amp_kind, (const double*)opd, kturns, count, nx, ld, (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        phase_screen_kernel<R><<<g, 256, 0, st>>>(amp, amp_kind, (const R*)opd, kturns, count, nx, ld, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -231,39 +227,36 @@ __global__ void mdft_basis_kernel(const double* __restrict__ f, int m, const dou
 
 using namespace pb;
 
-#define PB_HANDLE(hh)                                   \
-    PB_ENTER(hh);                      \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_phase_screen(pb_handle_t hh, int dtype, const void* amp, int amp_kind, const void* opd,
                                double kscale, long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (count <= 0) return PB_OK;
     return launch_phase_screen(h, dtype, amp, amp_kind, opd, kscale / (2.0 * M_PI), count, count, count, out, st);
 }
 
 extern "C" int pb_intensity(pb_handle_t hh, int dtype, const void* in, long long count, double weight, int accumulate,
                             void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) intensity_kernel<float><<<g, 256, 0, st>>>((const float2*)in, count, (float)weight, accumulate, (float*)out);
-    else intensity_kernel<double><<<g, 256, 0, st>>>((const double2*)in, count, weight, accumulate, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        intensity_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)in, count, (R)weight, accumulate, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_binary(pb_handle_t hh, int dtype, int op, const void* a, const void* b, double s_re, double s_im,
                          int reverse, long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (op < 0 || op > 3 || !a || !out) return fail(h, PB_ERR_INVALID, "bad binary-op arguments");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64)
-        binary_kernel<float><<<g, 256, 0, st>>>(op, (const float2*)a, (const float2*)b, make_float2((float)s_re, (float)s_im), reverse, count, (float2*)out);
-    else
-        binary_kernel<double><<<g, 256, 0, st>>>(op, (const double2*)a, (const double2*)b, make_double2(s_re, s_im), reverse, count, (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        binary_kernel<R><<<g, 256, 0, st>>>(op, (const cplx<R>*)a, (const cplx<R>*)b, mk<R>((R)s_re, (R)s_im), reverse, count, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -271,35 +264,31 @@ extern "C" int pb_binary(pb_handle_t hh, int dtype, int op, const void* a, const
 extern "C" int pb_mul_outer(pb_handle_t hh, int dtype, const void* in, long long in_ld, int ny, int nx, const void* vy,
                             int conj_y, const void* vx, int conj_x, double scale, void* out, long long out_ld,
                             void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny <= 0 || nx <= 0) return PB_OK;
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64)
-        mul_outer_kernel<float><<<g, 256, 0, st>>>((const float2*)in, in_ld, ny, nx, (const float2*)vy, conj_y,
-                                                   (const float2*)vx, conj_x, (float)scale, (float2*)out, out_ld);
-    else
-        mul_outer_kernel<double><<<g, 256, 0, st>>>((const double2*)in, in_ld, ny, nx, (const double2*)vy, conj_y,
-                                                    (const double2*)vx, conj_x, scale, (double2*)out, out_ld);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        mul_outer_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)in, in_ld, ny, nx, (const cplx<R>*)vy, conj_y, (const cplx<R>*)vx,
+                                               conj_x, (R)scale, (cplx<R>*)out, out_ld);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_weighted_sum(pb_handle_t hh, int dtype, const void* modes, int k, long long count,
                                const double* weights_host, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (k < 1 || count <= 0 || !weights_host) return fail(h, PB_ERR_INVALID, "bad mode count / weights");
     const int g = grid_for(count, 256, h->sm_count);
     for (int k0 = 0; k0 < k; k0 += PB_MAX_MODES) {
         const int kk = std::min(PB_MAX_MODES, k - k0);
-        if (dtype == PB_C64) {
-            ModeWeights<float> w;
-            for (int i = 0; i < kk; ++i) w.w[i] = (float)weights_host[k0 + i];
-            weighted_sum_kernel<float><<<g, 256, 0, st>>>((const float*)modes + (long long)k0 * count, kk, count, w, k0 > 0, (float*)out);
-        } else {
-            ModeWeights<double> w;
-            for (int i = 0; i < kk; ++i) w.w[i] = weights_host[k0 + i];
-            weighted_sum_kernel<double><<<g, 256, 0, st>>>((const double*)modes + (long long)k0 * count, kk, count, w, k0 > 0, (double*)out);
-        }
+        with_real(dtype, [&](auto r) {
+            using R = decltype(r);
+            ModeWeights<R> w;
+            for (int i = 0; i < kk; ++i) w.w[i] = (R)weights_host[k0 + i];
+            weighted_sum_kernel<R><<<g, 256, 0, st>>>((const R*)modes + (long long)k0 * count, kk, count, w, k0 > 0, (R*)out);
+        });
         PB_LAUNCH_CHECK(h);
     }
     return PB_OK;
@@ -307,28 +296,30 @@ extern "C" int pb_weighted_sum(pb_handle_t hh, int dtype, const void* modes, int
 
 extern "C" int pb_otf_normalize(pb_handle_t hh, int dtype, const void* D, int ny, int nx, int which, void* mtf,
                                 void* ptf, void* otf, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1) return fail(h, PB_ERR_INVALID, "bad shape");
     const long long n = (long long)ny * nx, centre = (long long)(ny / 2) * nx + nx / 2;
     const int g = grid_for(n, 256, h->sm_count);
-    if (dtype == PB_C64)
-        otf_normalize_kernel<float><<<g, 256, 0, st>>>((const float2*)D, n, centre, which, (float*)mtf, (float*)ptf, (float2*)otf);
-    else
-        otf_normalize_kernel<double><<<g, 256, 0, st>>>((const double2*)D, n, centre, which, (double*)mtf, (double*)ptf, (double2*)otf);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        otf_normalize_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)D, n, centre, which, (R*)mtf, (R*)ptf, (cplx<R>*)otf);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_moments(pb_handle_t hh, int dtype, const void* data, int ny, int nx, double* sums_host,
                           void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || !sums_host) return fail(h, PB_ERR_INVALID, "bad shape");
     void* d = nullptr;
     PB_TRY(ensure_scratch(h, 2, 3 * sizeof(double), &d));
     PB_CUDA(h, cudaMemsetAsync(d, 0, 3 * sizeof(double), st));
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) moments_kernel<float><<<g, 256, 0, st>>>((const float*)data, ny, nx, (double*)d);
-    else moments_kernel<double><<<g, 256, 0, st>>>((const double*)data, ny, nx, (double*)d);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        moments_kernel<R><<<g, 256, 0, st>>>((const R*)data, ny, nx, (double*)d);
+    });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(sums_host, d, 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
     PB_CUDA(h, cudaStreamSynchronize(st));
@@ -337,7 +328,7 @@ extern "C" int pb_moments(pb_handle_t hh, int dtype, const void* data, int ny, i
 
 extern "C" int pb_encircled_energy(pb_handle_t hh, int dtype, const void* mtf, int ny, int nx, double df,
                                    const double* radii_mm_host, int nr, double* out_host, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nr < 1 || !mtf || !radii_mm_host || !out_host) return fail(h, PB_ERR_INVALID, "bad encircled-energy arguments");
     void* d = nullptr;
     PB_TRY(ensure_scratch(h, 2, (size_t)2 * nr * sizeof(double), &d));
@@ -347,8 +338,10 @@ extern "C" int pb_encircled_energy(pb_handle_t hh, int dtype, const void* mtf, i
     PB_CUDA(h, cudaMemsetAsync(dout, 0, nr * sizeof(double), st));
     const int gx = (int)std::min<long long>(((long long)ny * nx + 255) / 256, (long long)h->sm_count * 4);
     dim3 g(gx, nr);
-    if (dtype == PB_C64) encircled_energy_kernel<float><<<g, 256, 0, st>>>((const float*)mtf, ny, nx, df, dr, dout);
-    else encircled_energy_kernel<double><<<g, 256, 0, st>>>((const double*)mtf, ny, nx, df, dr, dout);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        encircled_energy_kernel<R><<<g, 256, 0, st>>>((const R*)mtf, ny, nx, df, dr, dout);
+    });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, dout, nr * sizeof(double), cudaMemcpyDeviceToHost, st));
     PB_CUDA(h, cudaStreamSynchronize(st));
@@ -359,13 +352,18 @@ int pb::czt_plan_impl(Handle* h, pb_handle_t hh, int dtype, int N, int M, int K,
                       double f0, double df, void* b, void* post, void* H, void* Hadj, void* hk, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int n = std::max(K, std::max(N, M));
-    if (dtype == PB_C64) czt_plan_kernel<float><<<(n + 255) / 256, 256, 0, st>>>(N, M, K, shift, alpha, sign, xc, f0, df, (float2*)b, (float2*)post, (float2*)hk);
-    else czt_plan_kernel<double><<<(n + 255) / 256, 256, 0, st>>>(N, M, K, shift, alpha, sign, xc, f0, df, (double2*)b, (double2*)post, (double2*)hk);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        czt_plan_kernel<R><<<(n + 255) / 256, 256, 0, st>>>(N, M, K, shift, alpha, sign, xc, f0, df, (cplx<R>*)b, (cplx<R>*)post,
+                                                           (cplx<R>*)hk);
+    });
     PB_LAUNCH_CHECK(h);
     PB_TRY(pb_fft1(hh, dtype, hk, 1, K, K, 1, K, -1, 1.0, H, K, stream));   // H = FFT_K(h)
     if (Hadj) {
-        if (dtype == PB_C64) czt_hadj_kernel<float><<<(K + 255) / 256, 256, 0, st>>>(N, K, (const float2*)H, (float2*)Hadj);
-        else czt_hadj_kernel<double><<<(K + 255) / 256, 256, 0, st>>>(N, K, (const double2*)H, (double2*)Hadj);
+        with_real(dtype, [&](auto r) {
+            using R = decltype(r);
+            czt_hadj_kernel<R><<<(K + 255) / 256, 256, 0, st>>>(N, K, (const cplx<R>*)H, (cplx<R>*)Hadj);
+        });
         PB_LAUNCH_CHECK(h);
     }
     return PB_OK;
@@ -373,7 +371,7 @@ int pb::czt_plan_impl(Handle* h, pb_handle_t hh, int dtype, int N, int M, int K,
 
 extern "C" int pb_czt_plan(pb_handle_t hh, int dtype, int N, int M, int K, double shift, double alpha, int sign, double xc,
                            double f0, double df, void* b, void* post, void* H, void* Hadj, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     (void)st;
     if (N < 1 || M < 1 || K < N + M - 1 || (sign != 1 && sign != -1) || !b || !post || !H || !Hadj)
         return fail(h, PB_ERR_INVALID, "bad czt plan arguments");
@@ -384,16 +382,14 @@ extern "C" int pb_czt_plan(pb_handle_t hh, int dtype, int N, int M, int K, doubl
 
 extern "C" int pb_angular_spectrum_vectors(pb_handle_t hh, int dtype, int ky, int kx, double wvl_um, double dx_mm,
                                            double z_mm, void* ty, void* tx, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ky < 1 || kx < 1) return fail(h, PB_ERR_INVALID, "bad shape");
     const double w = wvl_um / 1e3;
-    if (dtype == PB_C64) {
-        as_vector_kernel<float><<<(ky + 255) / 256, 256, 0, st>>>(ky, w, dx_mm, z_mm, (float2*)ty);
-        as_vector_kernel<float><<<(kx + 255) / 256, 256, 0, st>>>(kx, w, dx_mm, z_mm, (float2*)tx);
-    } else {
-        as_vector_kernel<double><<<(ky + 255) / 256, 256, 0, st>>>(ky, w, dx_mm, z_mm, (double2*)ty);
-        as_vector_kernel<double><<<(kx + 255) / 256, 256, 0, st>>>(kx, w, dx_mm, z_mm, (double2*)tx);
-    }
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        as_vector_kernel<R><<<(ky + 255) / 256, 256, 0, st>>>(ky, w, dx_mm, z_mm, (cplx<R>*)ty);
+        as_vector_kernel<R><<<(kx + 255) / 256, 256, 0, st>>>(kx, w, dx_mm, z_mm, (cplx<R>*)tx);
+    });
     PB_LAUNCH_CHECK(h);
     h->launches++;
     return PB_OK;
@@ -401,7 +397,7 @@ extern "C" int pb_angular_spectrum_vectors(pb_handle_t hh, int dtype, int ky, in
 
 extern "C" int pb_mdft_basis(pb_handle_t hh, int dtype, const double* f_host, int m, const double* x_host, int n,
                              int sign, void* E, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (m < 1 || n < 1 || !f_host || !x_host || (sign != 1 && sign != -1)) return fail(h, PB_ERR_INVALID, "bad basis arguments");
     void* d = nullptr;
     PB_TRY(ensure_scratch(h, 2, (size_t)(m + n) * sizeof(double), &d));
@@ -411,8 +407,10 @@ extern "C" int pb_mdft_basis(pb_handle_t hh, int dtype, const double* f_host, in
     PB_CUDA(h, cudaMemcpyAsync(df, f_host, m * sizeof(double), cudaMemcpyHostToDevice, st));
     PB_CUDA(h, cudaMemcpyAsync(dxv, x_host, n * sizeof(double), cudaMemcpyHostToDevice, st));
     const int g = grid_for((long long)m * n, 256, h->sm_count);
-    if (dtype == PB_C64) mdft_basis_kernel<float><<<g, 256, 0, st>>>(df, m, dxv, n, sign, (float2*)E);
-    else mdft_basis_kernel<double><<<g, 256, 0, st>>>(df, m, dxv, n, sign, (double2*)E);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        mdft_basis_kernel<R><<<g, 256, 0, st>>>(df, m, dxv, n, sign, (cplx<R>*)E);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

@@ -95,11 +95,6 @@ __global__ void sdf_combine_kernel(int op, const R* __restrict__ a, const R* __r
     }
 }
 
-inline int grid_for(long long n, int threads, int sm_count) {
-    const long long g = (n + threads - 1) / threads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 }  // namespace
 
 }  // namespace pb
@@ -109,8 +104,7 @@ using namespace pb;
 extern "C" int pb_sdf(pb_handle_t hh, int dtype, int kind, const void* x, const void* y, int separable, int ny, int nx,
                       const double* params_host, int nparams, const double* verts_host, int nverts, int mask, void* out,
                       void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (kind < PB_SDF_POLYGON || kind > PB_SDF_OFFSET_CIRCLE) return fail(h, PB_ERR_INVALID, "unknown shape kind");
     if (ny < 0 || nx < 0 || nparams < 0 || nparams > 8 || nverts < 0 || (nparams && !params_host) || (nverts && !verts_host))
         return fail(h, PB_ERR_INVALID, "bad shape arguments");
@@ -124,26 +118,27 @@ extern "C" int pb_sdf(pb_handle_t hh, int dtype, int kind, const void* x, const 
     s.nv = nverts;
     for (int i = 0; i < nparams; ++i) s.p[i] = params_host[i];
     for (int i = 0; i < 2 * nverts; ++i) s.v[i] = verts_host[i];
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
     const void* yy = kind == PB_SDF_ANNULUS ? nullptr : y;
-    if (dtype == PB_C64) sdf_kernel<float><<<g, 256, 0, st>>>((const float*)x, (const float*)yy, separable, ny, nx, s, mask, out);
-    else sdf_kernel<double><<<g, 256, 0, st>>>((const double*)x, (const double*)yy, separable, ny, nx, s, mask, out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        sdf_kernel<R><<<g, 256, 0, st>>>((const R*)x, (const R*)yy, separable, ny, nx, s, mask, out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_sdf_combine(pb_handle_t hh, int dtype, int op, const void* a, const void* b, long long count, void* out,
                               void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (op < PB_SDF_UNION || op > PB_SDF_SUBTRACT) return fail(h, PB_ERR_INVALID, "unknown combine op");
     if (count <= 0) return PB_OK;
     if (!a || !b || !out) return fail(h, PB_ERR_INVALID, "null pointer");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) sdf_combine_kernel<float><<<g, 256, 0, st>>>(op, (const float*)a, (const float*)b, count, (float*)out);
-    else sdf_combine_kernel<double><<<g, 256, 0, st>>>(op, (const double*)a, (const double*)b, count, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        sdf_combine_kernel<R><<<g, 256, 0, st>>>(op, (const R*)a, (const R*)b, count, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

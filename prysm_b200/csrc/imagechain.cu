@@ -10,12 +10,6 @@
 
 namespace pb {
 
-static inline int grid_for(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
 template <typename R>
 __global__ void pack_complex_kernel(const R* __restrict__ re, const R* __restrict__ im, const double* __restrict__ im_scale,
                                     long long n, cplx<R>* __restrict__ out) {
@@ -111,33 +105,32 @@ __global__ void separable_tf_kernel(int kind, const R* __restrict__ fxv, const R
 
 using namespace pb;
 
-#define PB_HANDLE(hh)                                   \
-    PB_ENTER(hh);                      \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_pack_complex(pb_handle_t hh, int dtype, const void* re, const void* im, const double* im_scale_dev,
                                long long count, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!re || !out) return fail(h, PB_ERR_INVALID, "null pointer");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) pack_complex_kernel<float><<<g, 256, 0, st>>>((const float*)re, (const float*)im, im_scale_dev, count, (float2*)out);
-    else pack_complex_kernel<double><<<g, 256, 0, st>>>((const double*)re, (const double*)im, im_scale_dev, count, (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        pack_complex_kernel<R><<<g, 256, 0, st>>>((const R*)re, (const R*)im, im_scale_dev, count, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_balance_scale(pb_handle_t hh, int dtype, const void* a, const void* b, long long count, double* s_dev,
                                 void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !b || !s_dev || count <= 0) return fail(h, PB_ERR_INVALID, "bad balance arguments");
     void* d = nullptr;
     PB_TRY(ensure_scratch(h, 2, 2 * sizeof(double), &d));
     PB_CUDA(h, cudaMemsetAsync(d, 0, 2 * sizeof(double), st));
     const int g = (int)std::min<long long>((count + 255) / 256, (long long)h->sm_count * 4);
-    if (dtype == PB_C64) norms2_kernel<float><<<g, 256, 0, st>>>((const float*)a, (const float*)b, count, (double*)d);
-    else norms2_kernel<double><<<g, 256, 0, st>>>((const double*)a, (const double*)b, count, (double*)d);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        norms2_kernel<R><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, (double*)d);
+    });
     balance_finalize_kernel<<<1, 1, 0, st>>>((const double*)d, s_dev);
     PB_LAUNCH_CHECK(h);
     h->launches++;
@@ -146,47 +139,55 @@ extern "C" int pb_balance_scale(pb_handle_t hh, int dtype, const void* a, const 
 
 extern "C" int pb_packed_spectrum_product(pb_handle_t hh, int dtype, const void* Z, int ny, int nx, double scale,
                                           const double* im_scale_dev, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!Z || !out || ny < 1 || nx < 1 || Z == out) return fail(h, PB_ERR_INVALID, "bad spectrum-product arguments (out must not alias Z)");
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) packed_spectrum_product_kernel<float><<<g, 256, 0, st>>>((const float2*)Z, ny, nx, (float)scale, im_scale_dev, (float2*)out);
-    else packed_spectrum_product_kernel<double><<<g, 256, 0, st>>>((const double2*)Z, ny, nx, scale, im_scale_dev, (double2*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        packed_spectrum_product_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)Z, ny, nx, (R)scale, im_scale_dev, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_bindown(pb_handle_t hh, int dtype, const void* in, int ny, int nx, int fy, int fx, int mean, void* out,
                           void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!in || !out || fy < 1 || fx < 1 || ny < fy || nx < fx || ny % fy || nx % fx)
         return fail(h, PB_ERR_INVALID, "array shape must be a positive integer multiple of the binning factor");
     const int oy = ny / fy, ox = nx / fx;
     const double scale = mean ? 1.0 / ((double)fy * fx) : 1.0;
     const int g = grid_for((long long)oy * ox, 256, h->sm_count);
-    if (dtype == PB_C64) bindown_kernel<float><<<g, 256, 0, st>>>((const float*)in, oy, ox, fy, fx, (float)scale, (float*)out);
-    else bindown_kernel<double><<<g, 256, 0, st>>>((const double*)in, oy, ox, fy, fx, scale, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        bindown_kernel<R><<<g, 256, 0, st>>>((const R*)in, oy, ox, fy, fx, (R)scale, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_tile(pb_handle_t hh, int dtype, const void* in, int ny, int nx, int fy, int fx, double scale, void* out,
                        void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!in || !out || fy < 1 || fx < 1 || ny < 1 || nx < 1) return fail(h, PB_ERR_INVALID, "bad tile arguments");
     const int g = grid_for((long long)ny * fy * nx * fx, 256, h->sm_count);
-    if (dtype == PB_C64) tile_kernel<float><<<g, 256, 0, st>>>((const float*)in, ny, nx, fy, fx, (float)scale, (float*)out);
-    else tile_kernel<double><<<g, 256, 0, st>>>((const double*)in, ny, nx, fy, fx, scale, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        tile_kernel<R><<<g, 256, 0, st>>>((const R*)in, ny, nx, fy, fx, (R)scale, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_separable_tf(pb_handle_t hh, int dtype, int kind, const void* fx, const void* fy, int ny, int nx, double wx,
                                double wy, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!fx || !fy || !out || ny < 1 || nx < 1 || kind < 0 || kind > 1) return fail(h, PB_ERR_INVALID, "bad transfer-function arguments");
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) separable_tf_kernel<float><<<g, 256, 0, st>>>(kind, (const float*)fx, (const float*)fy, ny, nx, wx, wy, (float*)out);
-    else separable_tf_kernel<double><<<g, 256, 0, st>>>(kind, (const double*)fx, (const double*)fy, ny, nx, wx, wy, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        separable_tf_kernel<R><<<g, 256, 0, st>>>(kind, (const R*)fx, (const R*)fy, ny, nx, wx, wy, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

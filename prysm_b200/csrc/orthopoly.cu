@@ -35,15 +35,6 @@ struct P1Plan {
 };
 static_assert(sizeof(P1Plan) <= 32764, "the 1-D plan must fit the kernel parameter space");
 
-static inline int o_grid(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
-#define PB_GRID_STRIDE(i, n) \
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (n); i += (long long)gridDim.x * blockDim.x)
-
 // MODE 0: planes of P_n(a) or dP_n/dx (out0, (planes, n));  MODE 1: the radial sum z = sum w P(u), u = 2 (a^2 + b^2) / R^2
 // - 1, into out0, and with DER dz/dx, dz/dy into out1, out2 (jacobi_radial_sum(_der_xy))
 template <typename R, int MODE, bool DER>
@@ -274,12 +265,11 @@ static void build_p1plan(int fam, double alpha, double beta, std::vector<P1Term>
 template <int MODE, bool DER>
 static void launch_p1(int dtype, int g, cudaStream_t st, const void* a, const void* b, long long count, const P1Plan& pl,
                       double rsq, double inv_rsq, void* o0, void* o1, void* o2) {
-    if (dtype == PB_C64)
-        poly1d_kernel<float, MODE, DER><<<g, 256, 0, st>>>((const float*)a, (const float*)b, count, pl, rsq, inv_rsq,
-                                                           (float*)o0, (float*)o1, (float*)o2);
-    else
-        poly1d_kernel<double, MODE, DER><<<g, 256, 0, st>>>((const double*)a, (const double*)b, count, pl, rsq, inv_rsq,
-                                                            (double*)o0, (double*)o1, (double*)o2);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        poly1d_kernel<R, MODE, DER><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, rsq, inv_rsq, (R*)o0, (R*)o1,
+                                                       (R*)o2);
+    });
 }
 
 static int run_p1_seq(Handle* h, int dtype, int fam, double alpha, double beta, const void* x, long long count,
@@ -287,7 +277,7 @@ static int run_p1_seq(Handle* h, int dtype, int fam, double alpha, double beta, 
     P1Plan pl;
     build_p1plan(fam, alpha, beta, terms, pl);
     if (count <= 0) return PB_OK;
-    const int g = o_grid(count, 256, h->sm_count);
+    const int g = grid_for(count, 256, h->sm_count);
     if (der) launch_p1<0, true>(dtype, g, st, x, nullptr, count, pl, 1.0, 1.0, out, nullptr, nullptr);
     else launch_p1<0, false>(dtype, g, st, x, nullptr, count, pl, 1.0, 1.0, out, nullptr, nullptr);
     PB_LAUNCH_CHECK(h);
@@ -298,14 +288,9 @@ static int run_p1_seq(Handle* h, int dtype, int fam, double alpha, double beta, 
 
 using namespace pb;
 
-#define PB_REAL_DTYPE()                                                                                         \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_jacobi_seq(pb_handle_t hh, int dtype, const void* x, long long count, int nmax, double alpha, double beta,
                              const int* slots_host, void* out, void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (!x || !out || !slots_host || nmax < 0) return fail(h, PB_ERR_INVALID, "bad jacobi arguments");
     if (nmax > PB_JAC_MAX) return fail(h, PB_ERR_UNSUPPORTED, "jacobi order above 120");
     if (count <= 0) return PB_OK;
@@ -319,8 +304,7 @@ extern "C" int pb_jacobi_seq(pb_handle_t hh, int dtype, const void* x, long long
 
 extern "C" int pb_poly_seq(pb_handle_t hh, int dtype, int family, int kind, double alpha, double beta, const void* x,
                            long long count, int k, const int* n_host, void* out, void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (family < PB_POLY_JACOBI || family > PB_POLY_DICKSON2 || kind < PB_POLY_VALUE || kind > PB_POLY_VALUE_DER)
         return fail(h, PB_ERR_INVALID, "poly: bad family or kind");
     if (!x || !out || k < 1 || !n_host) return fail(h, PB_ERR_INVALID, "bad poly arguments");
@@ -358,8 +342,7 @@ extern "C" int pb_poly_seq(pb_handle_t hh, int dtype, int family, int kind, doub
 extern "C" int pb_jacobi_radial_sum(pb_handle_t hh, int dtype, double alpha, double beta, const void* x, const void* y,
                                     long long count, int k, const int* n_host, const double* coefs_host, double radius,
                                     void* z, void* dzdx, void* dzdy, void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (!x || !y || !z || k < 0 || (k > 0 && (!n_host || !coefs_host)) || (!dzdx != !dzdy))
         return fail(h, PB_ERR_INVALID, "bad jacobi radial sum arguments");
     std::vector<P1Term> terms;
@@ -372,7 +355,7 @@ extern "C" int pb_jacobi_radial_sum(pb_handle_t hh, int dtype, double alpha, dou
     P1Plan pl;
     build_p1plan(PB_POLY_JACOBI, alpha, beta, terms, pl);
     if (count <= 0) return PB_OK;
-    const int g = o_grid(count, 256, h->sm_count);
+    const int g = grid_for(count, 256, h->sm_count);
     const double rsq = radius * radius, inv_rsq = 1.0 / rsq;
     if (dzdx) launch_p1<1, true>(dtype, g, st, x, y, count, pl, rsq, inv_rsq, z, dzdx, dzdy);
     else launch_p1<1, false>(dtype, g, st, x, y, count, pl, rsq, inv_rsq, z, nullptr, nullptr);
@@ -382,8 +365,7 @@ extern "C" int pb_jacobi_radial_sum(pb_handle_t hh, int dtype, double alpha, dou
 
 extern "C" int pb_jacobi_clenshaw(pb_handle_t hh, int dtype, double alpha, double beta, const void* x, long long count,
                                   int len, const double* s_host, int j, int table, void* out, void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (!x || !out || len < 1 || !s_host || j < 0) return fail(h, PB_ERR_INVALID, "bad clenshaw arguments");
     if (j > PB_CLEN_J) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: derivative order above 8");
     if (len > PB_JAC_MAX + 1) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: more than 121 coefficients");
@@ -397,9 +379,11 @@ extern "C" int pb_jacobi_clenshaw(pb_handle_t hh, int dtype, double alpha, doubl
         pl.A[nn] = abc[0]; pl.B[nn] = abc[1]; pl.C1[nn] = abc1[2];
     }
     if (count <= 0) return PB_OK;
-    const int g = o_grid(count, 256, h->sm_count);
-    if (dtype == PB_C64) clenshaw_kernel<float><<<g, 256, 0, st>>>((const float*)x, count, pl, (float*)out);
-    else clenshaw_kernel<double><<<g, 256, 0, st>>>((const double*)x, count, pl, (double*)out);
+    const int g = grid_for(count, 256, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        clenshaw_kernel<R><<<g, 256, 0, st>>>((const R*)x, count, pl, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -407,8 +391,7 @@ extern "C" int pb_jacobi_clenshaw(pb_handle_t hh, int dtype, double alpha, doubl
 extern "C" int pb_xy_seq(pb_handle_t hh, int dtype, const void* x, const void* y, long long count, long long nx,
                          int separable, int k, const int* m_host, const int* n_host, const int* kind_host, void* out,
                          void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (!x || !y || !out || k < 1 || !m_host || !n_host || !kind_host || (separable && nx < 1))
         return fail(h, PB_ERR_INVALID, "bad xy arguments");
     if (k > PB_XY_PLANES) return fail(h, PB_ERR_UNSUPPORTED, "xy: more than 1024 planes");
@@ -420,9 +403,11 @@ extern "C" int pb_xy_seq(pb_handle_t hh, int dtype, const void* x, const void* y
         pl.m[q] = (short)m_host[q]; pl.nn[q] = (short)n_host[q]; pl.kind[q] = (unsigned char)kind_host[q];
     }
     if (count <= 0) return PB_OK;
-    const int g = o_grid(count, 256, h->sm_count);
-    if (dtype == PB_C64) xy_kernel<float><<<g, 256, 0, st>>>((const float*)x, (const float*)y, count, pl, (float*)out);
-    else xy_kernel<double><<<g, 256, 0, st>>>((const double*)x, (const double*)y, count, pl, (double*)out);
+    const int g = grid_for(count, 256, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        xy_kernel<R><<<g, 256, 0, st>>>((const R*)x, (const R*)y, count, pl, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -430,8 +415,7 @@ extern "C" int pb_xy_seq(pb_handle_t hh, int dtype, const void* x, const void* y
 extern "C" int pb_tensor_sum(pb_handle_t hh, int dtype, int basis, const void* x, const void* y, long long count, long long nx,
                              int separable, int k, const int* m_host, const int* n_host, const double* coefs_host,
                              double x_norm, double y_norm, void* z, void* dzdx, void* dzdy, void* stream) {
-    PB_ENTER(hh);
-    PB_REAL_DTYPE();
+    PB_ENTER_REAL(hh);
     if (basis < PB_TSUM_MONOMIAL || basis > PB_TSUM_CHEBY1 || !x || !y || !z || k < 0 ||
         (k > 0 && (!m_host || !n_host || !coefs_host)) || (!dzdx != !dzdy) || (separable && nx < 1))
         return fail(h, PB_ERR_INVALID, "bad tensor sum arguments");
@@ -449,14 +433,12 @@ extern "C" int pb_tensor_sum(pb_handle_t hh, int dtype, int basis, const void* x
     std::fill(pl.c, pl.c + PB_TSUM_COEFS, 0.0);
     for (int q = 0; q < k; ++q) pl.c[n_host[q] * (maxm + 1) + m_host[q]] += coefs_host[q];
     if (count <= 0) return PB_OK;
-    const int g = o_grid(count, 256, h->sm_count);
-    if (dtype == PB_C64) {
-        if (dzdx) tsum_kernel<float, true><<<g, 256, 0, st>>>((const float*)x, (const float*)y, count, pl, (float*)z, (float*)dzdx, (float*)dzdy);
-        else tsum_kernel<float, false><<<g, 256, 0, st>>>((const float*)x, (const float*)y, count, pl, (float*)z, nullptr, nullptr);
-    } else {
-        if (dzdx) tsum_kernel<double, true><<<g, 256, 0, st>>>((const double*)x, (const double*)y, count, pl, (double*)z, (double*)dzdx, (double*)dzdy);
-        else tsum_kernel<double, false><<<g, 256, 0, st>>>((const double*)x, (const double*)y, count, pl, (double*)z, nullptr, nullptr);
-    }
+    const int g = grid_for(count, 256, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        if (dzdx) tsum_kernel<R, true><<<g, 256, 0, st>>>((const R*)x, (const R*)y, count, pl, (R*)z, (R*)dzdx, (R*)dzdy);
+        else tsum_kernel<R, false><<<g, 256, 0, st>>>((const R*)x, (const R*)y, count, pl, (R*)z, nullptr, nullptr);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

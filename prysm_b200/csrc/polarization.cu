@@ -62,11 +62,6 @@ __device__ __forceinline__ double ld_real(const void* p, int type, long long i) 
 
 template <typename R> __device__ __forceinline__ double ld_plain(const R* __restrict__ p, long long i) { return (double)p[i]; }
 
-inline int grid_for(long long groups, int sm_count) {
-    const long long g = (groups + kThreads - 1) / kThreads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 // ---- pb_jones_planar ---------------------------------------------------------------------------------------------
 // strided (rows, cols, 2, 2) of any real or complex type -> 4 planes; one thread per V pixels
 template <typename T, bool CPLX, typename R, int V>
@@ -331,24 +326,16 @@ using namespace pb;
 template <typename F>
 static int jones_launch(Handle* h, int dtype, bool pairs, long long n, F&& f) {
     if (dtype == PB_C64 && pairs) f(float(), std::integral_constant<int, 2>(), n / 2);
-    else if (dtype == PB_C64) f(float(), std::integral_constant<int, 1>(), n);
-    else f(double(), std::integral_constant<int, 1>(), n);
+    else with_real(dtype, [&](auto r) { f(r, std::integral_constant<int, 1>(), n); });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
-#define PB_JONES_ENTER(hh)                                                                                    \
-    PB_ENTER(hh);                                                                                             \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");                                       \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
-#define PB_JONES_GRID(groups) grid_for(groups, h->sm_count), kThreads, 0, st
-
 extern "C" int pb_jones_planar(pb_handle_t hh, int dtype, const void* src, int src_type, long long rows, long long cols,
                                long long s_row, long long s_col, long long s_i, long long s_j, void* out, void* stream) {
     const long long n = rows < 0 || cols < 0 ? -1 : rows * cols;
-    PB_JONES_ENTER(hh);
+    PB_ENTER_REAL(hh);
+    if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     if (src_type < PB_JONES_SRC_F32 || src_type > PB_JONES_SRC_C128) return fail(h, PB_ERR_INVALID, "bad Jones source type");
     if (n == 0) return PB_OK;
     if (!src || !out) return fail(h, PB_ERR_INVALID, "null pointer");
@@ -356,29 +343,31 @@ extern "C" int pb_jones_planar(pb_handle_t hh, int dtype, const void* src, int s
         using R = decltype(r);
         constexpr int V = decltype(v)::value;
         cplx<R>* o = reinterpret_cast<cplx<R>*>(out);
+        const int g = grid_for(groups, kThreads, h->sm_count);
         switch (src_type) {
             case PB_JONES_SRC_F32:
-                jones_planar_kernel<float, false, R, V><<<PB_JONES_GRID(groups)>>>((const float*)src, cols, s_row, s_col, s_i,
-                                                                                    s_j, groups, n, o);
+                jones_planar_kernel<float, false, R, V><<<g, kThreads, 0, st>>>((const float*)src, cols, s_row, s_col, s_i, s_j,
+                                                                                 groups, n, o);
                 break;
             case PB_JONES_SRC_F64:
-                jones_planar_kernel<double, false, R, V><<<PB_JONES_GRID(groups)>>>((const double*)src, cols, s_row, s_col,
-                                                                                     s_i, s_j, groups, n, o);
+                jones_planar_kernel<double, false, R, V><<<g, kThreads, 0, st>>>((const double*)src, cols, s_row, s_col, s_i,
+                                                                                  s_j, groups, n, o);
                 break;
             case PB_JONES_SRC_C64:
-                jones_planar_kernel<float, true, R, V><<<PB_JONES_GRID(groups)>>>((const float*)src, cols, s_row, s_col, s_i,
-                                                                                   s_j, groups, n, o);
+                jones_planar_kernel<float, true, R, V><<<g, kThreads, 0, st>>>((const float*)src, cols, s_row, s_col, s_i, s_j,
+                                                                                groups, n, o);
                 break;
             default:
-                jones_planar_kernel<double, true, R, V><<<PB_JONES_GRID(groups)>>>((const double*)src, cols, s_row, s_col,
-                                                                                    s_i, s_j, groups, n, o);
+                jones_planar_kernel<double, true, R, V><<<g, kThreads, 0, st>>>((const double*)src, cols, s_row, s_col, s_i,
+                                                                                 s_j, groups, n, o);
         }
     });
 }
 
 extern "C" int pb_jones_product(pb_handle_t hh, int dtype, int mode, long long n, int a_kind, const void* a, int a_op,
                                 int b_kind, const void* b, int b_op, const double* consts_host, void* out, void* stream) {
-    PB_JONES_ENTER(hh);
+    PB_ENTER_REAL(hh);
+    if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     auto kind_ok = [](int k) { return k >= PB_JONES_CONST && k <= PB_JONES_SCALAR_REAL; };
     auto op_ok = [](int o) { return o == PB_JONES_OP_N || o == PB_JONES_OP_H; };
     if ((mode != PB_JONES_MATMUL && mode != PB_JONES_HADAMARD) || !kind_ok(a_kind) || !kind_ok(b_kind) || !op_ok(a_op) ||
@@ -395,14 +384,16 @@ extern "C" int pb_jones_product(pb_handle_t hh, int dtype, int mode, long long n
                                     b_kind == PB_JONES_SCALAR_REAL ? nullptr : b});
     return jones_launch(h, dtype, pairs, n, [&](auto r, auto v, long long groups) {
         using R = decltype(r);
-        jones_product_kernel<R, decltype(v)::value><<<PB_JONES_GRID(groups)>>>(mode, groups, n, a_kind, a, a_op, b_kind, b,
-                                                                              b_op, k, reinterpret_cast<cplx<R>*>(out));
+        const int g = grid_for(groups, kThreads, h->sm_count);
+        jones_product_kernel<R, decltype(v)::value><<<g, kThreads, 0, st>>>(mode, groups, n, a_kind, a, a_op, b_kind, b, b_op, k,
+                                                                           reinterpret_cast<cplx<R>*>(out));
     });
 }
 
 extern "C" int pb_jones_elements(pb_handle_t hh, int dtype, int kind, long long n, const void* plane, int plane_type,
                                  const double* params_host, int nparams, void* out, void* stream) {
-    PB_JONES_ENTER(hh);
+    PB_ENTER_REAL(hh);
+    if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     static const int need[] = {8, 2, 2, 2, 3};
     if (kind < PB_JONES_FILL || kind > PB_JONES_VVR || nparams < need[kind] || nparams > 8 ||
         (plane && plane_type != PB_JONES_SRC_F32 && plane_type != PB_JONES_SRC_F64) || (kind == PB_JONES_FILL && plane))
@@ -413,14 +404,16 @@ extern "C" int pb_jones_elements(pb_handle_t hh, int dtype, int kind, long long 
     std::copy(params_host, params_host + nparams, p.v);
     return jones_launch(h, dtype, pairs_ok(n, {out}), n, [&](auto r, auto v, long long groups) {
         using R = decltype(r);
-        jones_elements_kernel<R, decltype(v)::value><<<PB_JONES_GRID(groups)>>>(kind, groups, n, plane, plane_type, p,
-                                                                               reinterpret_cast<cplx<R>*>(out));
+        const int g = grid_for(groups, kThreads, h->sm_count);
+        jones_elements_kernel<R, decltype(v)::value><<<g, kThreads, 0, st>>>(kind, groups, n, plane, plane_type, p,
+                                                                            reinterpret_cast<cplx<R>*>(out));
     });
 }
 
 extern "C" int pb_jones_reduce(pb_handle_t hh, int dtype, int kind, long long n, const void* a, const void* b, void* out,
                                void* stream) {
-    PB_JONES_ENTER(hh);
+    PB_ENTER_REAL(hh);
+    if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     if (kind < PB_JONES_MUELLER || kind > PB_JONES_PAULI) return fail(h, PB_ERR_INVALID, "bad Jones reduction");
     if (n == 0) return PB_OK;
     if (!a || !out || (kind == PB_JONES_KRON && !b)) return fail(h, PB_ERR_INVALID, "null pointer");
@@ -429,7 +422,8 @@ extern "C" int pb_jones_reduce(pb_handle_t hh, int dtype, int kind, long long n,
                        (reinterpret_cast<uintptr_t>(out) & 7) == 0;
     return jones_launch(h, dtype, pairs, n, [&](auto r, auto v, long long groups) {
         using R = decltype(r);
-        jones_reduce_kernel<R, decltype(v)::value><<<PB_JONES_GRID(groups)>>>(
+        const int g = grid_for(groups, kThreads, h->sm_count);
+        jones_reduce_kernel<R, decltype(v)::value><<<g, kThreads, 0, st>>>(
             kind, groups, n, reinterpret_cast<const cplx<R>*>(a), reinterpret_cast<const cplx<R>*>(b), out);
     });
 }

@@ -39,12 +39,6 @@ struct QPlan {
 };
 static_assert(sizeof(QPlan) <= 32764, "the qpoly plan must fit the kernel parameter space");
 
-static inline int q_grid(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
 #define PB_Q_INV_SQRT19 0.22941573387056177   // 1 / sqrt(19)
 
 // KIND 0: values (a = r or x of Q-bfs / Q-con, b = t);  1: d/dr (and d/dt of 2D-Q);  2: d/dx, d/dy (a = x, b = y)
@@ -353,10 +347,10 @@ static int build_qterms(Handle* h, int family, int k, const int* n_host, const i
 template <int KIND, int MODE>
 static void launch_q(int dtype, int g, cudaStream_t st, const void* a, const void* b, long long count, const QPlan& pl,
                      void* o0, void* o1, void* o2) {
-    if (dtype == PB_C64)
-        qpoly_kernel<float, KIND, MODE><<<g, 256, 0, st>>>((const float*)a, (const float*)b, count, pl, (float*)o0, (float*)o1, (float*)o2);
-    else
-        qpoly_kernel<double, KIND, MODE><<<g, 256, 0, st>>>((const double*)a, (const double*)b, count, pl, (double*)o0, (double*)o1, (double*)o2);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        qpoly_kernel<R, KIND, MODE><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, (R*)o0, (R*)o1, (R*)o2);
+    });
 }
 
 }  // namespace pb
@@ -365,8 +359,7 @@ using namespace pb;
 
 extern "C" int pb_qpoly_seq(pb_handle_t hh, int dtype, int family, int kind, const void* a, const void* b, long long count,
                             int k, const int* n_host, const int* m_host, void* out0, void* out1, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (family < PB_QPOLY_BFS || family > PB_QPOLY_2D || kind < PB_QPOLY_VALUE || kind > PB_QPOLY_DER_XY)
         return fail(h, PB_ERR_INVALID, "qpoly: bad family or kind");
     if (family != PB_QPOLY_2D && kind == PB_QPOLY_DER_XY) return fail(h, PB_ERR_INVALID, "qpoly: Cartesian derivatives are 2D-Q only");
@@ -378,8 +371,7 @@ extern "C" int pb_qpoly_seq(pb_handle_t hh, int dtype, int family, int kind, con
     QPlan pl;
     PB_TRY(build_qplan(h, terms, 0, pl));
     if (count <= 0) return PB_OK;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = q_grid(count, 256, h->sm_count);
+    const int g = grid_for(count, 256, h->sm_count);
     const void* bb = family == PB_QPOLY_2D ? b : nullptr;
     if (kind == PB_QPOLY_VALUE) launch_q<0, 0>(dtype, g, st, a, bb, count, pl, out0, nullptr, nullptr);
     else if (kind == PB_QPOLY_DER) launch_q<1, 0>(dtype, g, st, a, bb, count, pl, out0, out1, nullptr);
@@ -391,8 +383,7 @@ extern "C" int pb_qpoly_seq(pb_handle_t hh, int dtype, int family, int kind, con
 extern "C" int pb_qpoly_sum(pb_handle_t hh, int dtype, int family, const void* u, const void* t, long long count, int k,
                             const int* n_host, const int* m_host, const double* coefs_host, void* z, void* dzdr, void* dzdt,
                             void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (family < PB_QPOLY_BFS || family > PB_QPOLY_2D) return fail(h, PB_ERR_INVALID, "qpoly: bad family");
     if (!u || k < 0 || (k > 0 && (!n_host || !coefs_host || (family == PB_QPOLY_2D && !m_host))))
         return fail(h, PB_ERR_INVALID, "bad qpoly sum arguments");
@@ -403,8 +394,7 @@ extern "C" int pb_qpoly_sum(pb_handle_t hh, int dtype, int family, const void* u
     QPlan pl;
     PB_TRY(build_qplan(h, terms, 1, pl));
     if (count <= 0) return PB_OK;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = q_grid(count, 256, h->sm_count);
+    const int g = grid_for(count, 256, h->sm_count);
     const void* tt = family == PB_QPOLY_2D ? t : nullptr;
     if (dzdr || dzdt) launch_q<1, 1>(dtype, g, st, u, tt, count, pl, z, dzdr, dzdt);
     else launch_q<0, 1>(dtype, g, st, u, tt, count, pl, z, nullptr, nullptr);

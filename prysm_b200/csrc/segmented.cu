@@ -186,11 +186,6 @@ __global__ void segment_adjoint_final_kernel(int nseg, int nmodes, int nchunk, c
 
 using namespace pb;
 
-#define PB_SEG_ENTER(hh)                                                                                      \
-    PB_ENTER(hh);                                                                                             \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 static inline int tile_count(int ny, int nx, int tiles_y, int tiles_x) {
     return (tiles_y == (ny + kTY - 1) / kTY && tiles_x == (nx + kTX - 1) / kTX) ? tiles_y * tiles_x : -1;
 }
@@ -198,21 +193,18 @@ static inline int tile_count(int ny, int nx, int tiles_y, int tiles_x) {
 extern "C" int pb_hex_segments(pb_handle_t hh, int dtype, const void* x, const void* y, int ny, int nx, int tiles_y, int tiles_x,
                                const int* tile_ptr, const int* tile_seg, const long long* seg, const double* geo, int nverts,
                                double dx, void* cover, void* local_x, void* local_y, void* amp, void* stream) {
-    PB_SEG_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nverts < 3 || nverts > kMaxSides || !(dx > 0.0))
         return fail(h, PB_ERR_INVALID, "bad segment raster arguments");
     const int nt = tile_count(ny, nx, tiles_y, tiles_x);
     if (nt < 0) return fail(h, PB_ERR_INVALID, "tile grid does not match the array");
     if (!x || !y || !tile_ptr || !tile_seg || !seg || !geo || !cover || !local_x || !local_y || !amp)
         return fail(h, PB_ERR_INVALID, "null pointer");
-    if (dtype == PB_C64)
-        hex_raster_kernel<float><<<nt, kThreads, 0, st>>>((const float*)x, (const float*)y, ny, nx, tiles_x, tile_ptr, tile_seg, seg,
-                                                          geo, nverts, dx, (float*)cover, (float*)local_x, (float*)local_y,
-                                                          (float*)amp);
-    else
-        hex_raster_kernel<double><<<nt, kThreads, 0, st>>>((const double*)x, (const double*)y, ny, nx, tiles_x, tile_ptr, tile_seg,
-                                                           seg, geo, nverts, dx, (double*)cover, (double*)local_x,
-                                                           (double*)local_y, (double*)amp);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        hex_raster_kernel<R><<<nt, kThreads, 0, st>>>((const R*)x, (const R*)y, ny, nx, tiles_x, tile_ptr, tile_seg, seg, geo, nverts,
+                                                      dx, (R*)cover, (R*)local_x, (R*)local_y, (R*)amp);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -220,20 +212,18 @@ extern "C" int pb_hex_segments(pb_handle_t hh, int dtype, const void* x, const v
 extern "C" int pb_segment_compose(pb_handle_t hh, int dtype, int ny, int nx, int tiles_y, int tiles_x, const int* tile_ptr,
                                   const int* tile_seg, const long long* seg, const void* masks, const void* bases, int nmodes,
                                   const double* coefs, long long coef_stride, int ncoef, void* out, void* stream) {
-    PB_SEG_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nmodes < 0 || ncoef < 0 || coef_stride < nmodes) return fail(h, PB_ERR_INVALID, "bad compose arguments");
     const int nt = tile_count(ny, nx, tiles_y, tiles_x);
     if (nt < 0) return fail(h, PB_ERR_INVALID, "tile grid does not match the array");
     if (!tile_ptr || !tile_seg || !seg || !masks || !out || (nmodes > 0 && ncoef > 0 && (!bases || !coefs)))
         return fail(h, PB_ERR_INVALID, "null pointer");
     if (ncoef == 0 || nmodes == 0) return PB_OK;
-    if (dtype == PB_C64)
-        segment_compose_kernel<float><<<nt, kThreads, 0, st>>>(ny, nx, tiles_x, tile_ptr, tile_seg, seg, (const float*)masks,
-                                                               (const float*)bases, nmodes, coefs, coef_stride, ncoef, (float*)out);
-    else
-        segment_compose_kernel<double><<<nt, kThreads, 0, st>>>(ny, nx, tiles_x, tile_ptr, tile_seg, seg, (const double*)masks,
-                                                                (const double*)bases, nmodes, coefs, coef_stride, ncoef,
-                                                                (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        segment_compose_kernel<R><<<nt, kThreads, 0, st>>>(ny, nx, tiles_x, tile_ptr, tile_seg, seg, (const R*)masks, (const R*)bases,
+                                                           nmodes, coefs, coef_stride, ncoef, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -241,22 +231,23 @@ extern "C" int pb_segment_compose(pb_handle_t hh, int dtype, int ny, int nx, int
 extern "C" int pb_segment_compose_adjoint(pb_handle_t hh, int dtype, int ny, int nx, int nseg, const long long* seg,
                                           const void* masks, const void* bases, int nmodes, const void* opdbar, int nchunk,
                                           double* partial, void* out, void* stream) {
-    PB_SEG_ENTER(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nseg < 0 || nmodes < 0 || nchunk < 1 || nseg > 65535)
         return fail(h, PB_ERR_INVALID, "bad compose adjoint arguments");
     if ((long long)nseg * nmodes == 0) return PB_OK;
     if (!seg || !masks || !bases || !opdbar || !partial || !out) return fail(h, PB_ERR_INVALID, "null pointer");
     const dim3 grid(nchunk, nseg);
-    if (dtype == PB_C64)
-        segment_adjoint_partial_kernel<float><<<grid, kThreads, 0, st>>>(nx, seg, (const float*)masks, (const float*)bases, nmodes,
-                                                                         (const float*)opdbar, nchunk, partial);
-    else
-        segment_adjoint_partial_kernel<double><<<grid, kThreads, 0, st>>>(nx, seg, (const double*)masks, (const double*)bases,
-                                                                          nmodes, (const double*)opdbar, nchunk, partial);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        segment_adjoint_partial_kernel<R><<<grid, kThreads, 0, st>>>(nx, seg, (const R*)masks, (const R*)bases, nmodes,
+                                                                     (const R*)opdbar, nchunk, partial);
+    });
     PB_LAUNCH_CHECK(h);
     const int n = nseg * nmodes, g = (n + 255) / 256;
-    if (dtype == PB_C64) segment_adjoint_final_kernel<float><<<g, 256, 0, st>>>(nseg, nmodes, nchunk, partial, (float*)out);
-    else segment_adjoint_final_kernel<double><<<g, 256, 0, st>>>(nseg, nmodes, nchunk, partial, (double*)out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        segment_adjoint_final_kernel<R><<<g, 256, 0, st>>>(nseg, nmodes, nchunk, partial, (R*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

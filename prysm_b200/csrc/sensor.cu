@@ -16,11 +16,6 @@ namespace {
 
 constexpr int kSensorThreads = 256;
 
-inline int sensor_grid(long long n, int sm_count) {
-    long long g = (n + kSensorThreads - 1) / kSensorThreads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 // ---- Philox4x32-10 -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
@@ -432,13 +427,6 @@ bool with_bytes(int bytes, F&& f) {
 }
 
 template <typename F>
-bool with_real(int dtype, F&& f) {
-    if (dtype == PB_C64) { f(float{}); return true; }
-    if (dtype == PB_C128) { f(double{}); return true; }
-    return false;
-}
-
-template <typename F>
 bool with_sensor_type(int type, F&& f) {
     switch (type) {
         case PB_SENSOR_F32: f(float{}); return true;
@@ -469,7 +457,7 @@ extern "C" int pb_expose(pb_handle_t hh, int dtype, const void* aerial, long lon
     p.fwc = params_host[4]; p.scaling = params_host[5]; p.cap = params_host[6];
     p.lut_len = lut_len;
     p.key = make_uint2((uint32_t)key, (uint32_t)(key >> 32));
-    const int g = sensor_grid(n, h->sm_count);
+    const int g = grid_for(n, kSensorThreads, h->sm_count);
     bool ok = false;
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
@@ -498,7 +486,7 @@ extern "C" int pb_apply_lut(pb_handle_t hh, int code_bytes, const void* codes, l
     if (!codes || !lut || !out || (check && !flags) || lut_len < 1 || n < 0) return fail(h, PB_ERR_INVALID, "bad lut arguments");
     if (n == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = sensor_grid(n, h->sm_count);
+    const int g = grid_for(n, kSensorThreads, h->sm_count);
     bool ok = false;
     with_bytes(code_bytes, [&](auto code) {
         using Code = decltype(code);
@@ -523,7 +511,7 @@ extern "C" int pb_pixel(pb_handle_t hh, int dtype, const void* x, long long xsr,
     if (!x || !y || !out || n < 0 || nx < 1 || n % nx) return fail(h, PB_ERR_INVALID, "bad pixel arguments");
     if (n == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = sensor_grid(n, h->sm_count);
+    const int g = grid_for(n, kSensorThreads, h->sm_count);
     if (!with_real(dtype, [&](auto r) {
             using R = decltype(r);
             pixel_kernel<R><<<g, kSensorThreads, 0, st>>>((const R*)x, xsr, xsc, (const R*)y, ysr, ysc, n, nx, wx, wy,
@@ -548,7 +536,7 @@ extern "C" int pb_bayer_interleave(pb_handle_t hh, int elem_bytes, const void* c
     }
     if (M * N == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = sensor_grid(M * N, h->sm_count);
+    const int g = grid_for(M * N, kSensorThreads, h->sm_count);
     if (!with_bytes(elem_bytes, [&](auto e) {
             using T = decltype(e);
             interleave_kernel<T><<<g, kSensorThreads, 0, st>>>(src, half, M, N, (T*)out, out_ld);
@@ -565,7 +553,7 @@ extern "C" int pb_demosaic_deinterlace(pb_handle_t hh, int in_type, const void* 
     const long long m2 = m / 2, n2 = n / 2;
     if (m2 * n2 == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = sensor_grid(m2 * n2, h->sm_count);
+    const int g = grid_for(m2 * n2, kSensorThreads, h->sm_count);
     const int r_site = bggr ? 3 : 0, b_site = bggr ? 0 : 3;
     bool ok = false;
     with_sensor_type(in_type, [&](auto i) {
@@ -596,7 +584,7 @@ extern "C" int pb_white_balance(pb_handle_t hh, int dtype, void* a, long long n,
         g4.g[pl] = pl < nplanes ? gains_host[pl] : 1.0;
         g4.sat[pl] = sat_host && pl < nplanes ? sat_host[pl] : 1.0;
     }
-    const int g = std::min(sensor_grid(n, h->sm_count), (int)PB_WB_MAX_BLOCKS);
+    const int g = std::min(grid_for(n, kSensorThreads, h->sm_count), (int)PB_WB_MAX_BLOCKS);
     double* ratio = nullptr;
     if (!with_real(dtype, [&](auto r) {
             using T = decltype(r);
@@ -646,7 +634,7 @@ extern "C" int pb_bayer_assemble(pb_handle_t hh, int dtype, const void* rp, cons
     if (!rp || !g2p || !bp || !g1 || !out || n < 0) return fail(h, PB_ERR_INVALID, "bad assemble arguments");
     if (n == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int g = sensor_grid(n, h->sm_count);
+    const int g = grid_for(n, kSensorThreads, h->sm_count);
     if (!with_real(dtype, [&](auto r) {
             using R = decltype(r);
             assemble_kernel<R><<<g, kSensorThreads, 0, st>>>((const cplx<R>*)rp, (const cplx<R>*)g2p, (const cplx<R>*)bp,

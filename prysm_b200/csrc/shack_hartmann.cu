@@ -234,11 +234,6 @@ __global__ void __launch_bounds__(kThreads) reconstruct_kernel(
     if (tid == 0) out[(long long)f * K + k] = (S)part[0];
 }
 
-inline int grid_for(long long n, int sm_count) {
-    const long long g = (n + kThreads - 1) / kThreads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 }  // namespace
 
 }  // namespace pb
@@ -248,9 +243,7 @@ using namespace pb;
 extern "C" int pb_lenslet_screen(pb_handle_t hh, int dtype, const void* x, const void* y, int H, int W, int ncols,
                                  int nrows, const double* centres, const int* cand, int kind, const double* params_host,
                                  double two_efl, double kphase, void* out, void* stream) {
-    PB_ENTER(hh);
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (H < 0 || W < 0 || ncols < 0 || nrows < 0 || kind < PB_LENSLET_RECT || kind > PB_LENSLET_CIRCLE)
         return fail(h, PB_ERR_INVALID, "bad lenslet screen arguments");
     if ((long long)H * W == 0) return PB_OK;
@@ -260,15 +253,12 @@ extern "C" int pb_lenslet_screen(pb_handle_t hh, int dtype, const void* x, const
     std::copy(params_host, params_host + 4, p.v);
     const int2* cx = reinterpret_cast<const int2*>(cand);
     const int2* cy = cx + W;
-    const int grid = grid_for((long long)H * W, h->sm_count);
-    if (dtype == PB_C64)
-        lenslet_screen_kernel<float><<<grid, kThreads, 0, st>>>((const float*)x, (const float*)y, H, W, centres,
-                                                                centres + ncols, cx, cy, kind, p, two_efl, kphase,
-                                                                (float2*)out);
-    else
-        lenslet_screen_kernel<double><<<grid, kThreads, 0, st>>>((const double*)x, (const double*)y, H, W, centres,
-                                                                 centres + ncols, cx, cy, kind, p, two_efl, kphase,
-                                                                 (double2*)out);
+    const int grid = grid_for((long long)H * W, kThreads, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        lenslet_screen_kernel<R><<<grid, kThreads, 0, st>>>((const R*)x, (const R*)y, H, W, centres, centres + ncols, cx, cy, kind,
+                                                            p, two_efl, kphase, (cplx<R>*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

@@ -12,15 +12,6 @@
 
 namespace pb {
 
-static inline int grid_for(long long n, int threads, int sm_count) {
-    long long g = (n + threads - 1) / threads;
-    long long cap = (long long)sm_count * 16;
-    return (int)std::max<long long>(1, std::min(g, cap));
-}
-
-#define PB_GRID_STRIDE(i, n) \
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (n); i += (long long)gridDim.x * blockDim.x)
-
 __device__ inline float mul_rn(float a, float b) { return __fmul_rn(a, b); }       // one rounding per operation, like numpy
 __device__ inline double mul_rn(double a, double b) { return __dmul_rn(a, b); }
 
@@ -273,41 +264,42 @@ static int build_terms(Handle* h, int k, const int* n_host, const int* m_host, c
 
 using namespace pb;
 
-#define PB_HANDLE(hh)                                   \
-    PB_ENTER(hh);                      \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128"); \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
 extern "C" int pb_xy_grid(pb_handle_t hh, int dtype, int ny, int nx, double dx, void* x, void* y, void* r, void* t, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1) return fail(h, PB_ERR_INVALID, "bad grid shape");
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
-    if (dtype == PB_C64) xy_grid_kernel<float><<<g, 256, 0, st>>>(ny, nx, dx, (float*)x, (float*)y, (float*)r, (float*)t);
-    else xy_grid_kernel<double><<<g, 256, 0, st>>>(ny, nx, dx, (double*)x, (double*)y, (double*)r, (double*)t);
+    with_real(dtype, [&](auto real) {
+        using R = decltype(real);
+        xy_grid_kernel<R><<<g, 256, 0, st>>>(ny, nx, dx, (R*)x, (R*)y, (R*)r, (R*)t);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_cart_to_polar(pb_handle_t hh, int dtype, const void* x, const void* y, long long count, void* r, void* t,
                                 void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!x || !y) return fail(h, PB_ERR_INVALID, "null coordinates");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) cart_to_polar_kernel<float><<<g, 256, 0, st>>>((const float*)x, (const float*)y, count, (float*)r, (float*)t);
-    else cart_to_polar_kernel<double><<<g, 256, 0, st>>>((const double*)x, (const double*)y, count, (double*)r, (double*)t);
+    with_real(dtype, [&](auto real) {
+        using R = decltype(real);
+        cart_to_polar_kernel<R><<<g, 256, 0, st>>>((const R*)x, (const R*)y, count, (R*)r, (R*)t);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_circle(pb_handle_t hh, int dtype, const void* r, long long count, double radius, double aa_dx, void* out,
                          void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!r || !out) return fail(h, PB_ERR_INVALID, "null pointer");
     if (count <= 0) return PB_OK;
     const int g = grid_for(count, 256, h->sm_count);
-    if (dtype == PB_C64) circle_kernel<float><<<g, 256, 0, st>>>((const float*)r, count, (float)radius, (float)aa_dx, out);
-    else circle_kernel<double><<<g, 256, 0, st>>>((const double*)r, count, radius, aa_dx, out);
+    with_real(dtype, [&](auto real) {
+        using R = decltype(real);
+        circle_kernel<R><<<g, 256, 0, st>>>((const R*)r, count, (R)radius, (R)aa_dx, out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -318,20 +310,18 @@ static int run_zernike(Handle* h, int dtype, int polar, const void* a, const voi
     const int g = grid_for(count, 256, h->sm_count);
     int launches = 0;
     if ((MODE == 1 || MODE == 4) && terms.empty()) {      // all weights zero: the sum (and its slopes) is zero
-        PB_CUDA(h, cudaMemsetAsync(out, 0, (size_t)count * (dtype == PB_C64 ? 4 : 8) * (MODE == 4 ? 3 : 1), st));
+        PB_CUDA(h, cudaMemsetAsync(out, 0, (size_t)count * rsize(dtype) * (MODE == 4 ? 3 : 1), st));
         return PB_OK;
     }
     while (!terms.empty()) {
         ZernPlan pl;
         PB_TRY(next_plan(terms, pl));
         const int acc = launches > 0;
-        if (dtype == PB_C64) {
-            if (polar) zernike_kernel<float, MODE, true><<<g, 256, 0, st>>>((const float*)a, (const float*)b, count, pl, acc, (float*)out);
-            else zernike_kernel<float, MODE, false><<<g, 256, 0, st>>>((const float*)a, (const float*)b, count, pl, acc, (float*)out);
-        } else {
-            if (polar) zernike_kernel<double, MODE, true><<<g, 256, 0, st>>>((const double*)a, (const double*)b, count, pl, acc, (double*)out);
-            else zernike_kernel<double, MODE, false><<<g, 256, 0, st>>>((const double*)a, (const double*)b, count, pl, acc, (double*)out);
-        }
+        with_real(dtype, [&](auto r) {
+            using R = decltype(r);
+            if (polar) zernike_kernel<R, MODE, true><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, (R*)out);
+            else zernike_kernel<R, MODE, false><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, (R*)out);
+        });
         PB_LAUNCH_CHECK(h);
         ++launches;
     }
@@ -340,7 +330,7 @@ static int run_zernike(Handle* h, int dtype, int polar, const void* a, const voi
 
 extern "C" int pb_zernike_seq(pb_handle_t hh, int dtype, int polar, const void* a, const void* b, long long count, int k,
                               const int* n_host, const int* m_host, int norm, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !b || !out || k < 1 || !n_host || !m_host) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
     if (k > 32767) return fail(h, PB_ERR_UNSUPPORTED, "more than 32767 modes");
     if (count <= 0) return PB_OK;
@@ -352,7 +342,7 @@ extern "C" int pb_zernike_seq(pb_handle_t hh, int dtype, int polar, const void* 
 extern "C" int pb_zernike_sum(pb_handle_t hh, int dtype, int polar, const void* a, const void* b, long long count, int k,
                               const int* n_host, const int* m_host, const double* coefs_host, int norm, void* out,
                               void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !b || !out || k < 0 || (k > 0 && (!n_host || !m_host || !coefs_host))) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
     if (count <= 0) return PB_OK;
     std::vector<HostTerm> terms;
@@ -369,7 +359,7 @@ static int zernike_fits(Handle* h, const std::vector<HostTerm>& terms) {
 
 extern "C" int pb_zernike_der(pb_handle_t hh, int dtype, int cartesian, const void* a, const void* b, long long count, int k,
                               const int* n_host, const int* m_host, int norm, void* out, void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!a || !b || !out || k < 1 || !n_host || !m_host) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
     if (k > 16383) return fail(h, PB_ERR_UNSUPPORTED, "more than 16383 modes");
     std::vector<HostTerm> terms;
@@ -383,7 +373,7 @@ extern "C" int pb_zernike_der(pb_handle_t hh, int dtype, int cartesian, const vo
 extern "C" int pb_zernike_sum_der_xy(pb_handle_t hh, int dtype, const void* x, const void* y, long long count, int k,
                                      const int* n_host, const int* m_host, const double* coefs_host, int norm, void* out,
                                      void* stream) {
-    PB_HANDLE(hh);
+    PB_ENTER_REAL(hh);
     if (!x || !y || !out || k < 0 || (k > 0 && (!n_host || !m_host || !coefs_host))) return fail(h, PB_ERR_INVALID, "bad zernike arguments");
     std::vector<HostTerm> terms, merged;
     PB_TRY(build_terms(h, k, n_host, m_host, coefs_host, norm, terms));

@@ -21,11 +21,6 @@ constexpr int kOvMax = 256;                // mode pointers per pb_overlap launc
 constexpr int kPsiMax = 64;                // frames of pb_psi
 constexpr double kEulerGamma = 0.57721566490153286061;
 
-inline int grid_for(long long groups, int sm_count) {
-    const long long g = (groups + kThreads - 1) / kThreads;
-    return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
-}
-
 // ---- Bessel functions ----------------------------------------------------------------------------------------------
 // J_l(x), x >= 0.  Orders 0 and 1 are CUDA's j0 / j1.  Above: forward recurrence from them where x > l (stable
 // there), Miller's backward recurrence below, normalised by J0 + 2 (J2 + J4 + ...) = 1 and rescaled against overflow.
@@ -338,17 +333,9 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 using namespace pb;
 
-#define PB_WFS_ENTER(hh)                                                                                      \
-    PB_ENTER(hh);                                                                                             \
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream)
-
-#define PB_WFS_DTYPE()                                                                                        \
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128")
-
 extern "C" int pb_lp_modes(pb_handle_t hh, int dtype, const void* r, const void* t, long long n, double a, int nmodes,
                            const double* plan_host, void* out, void* stream) {
-    PB_WFS_ENTER(hh);
-    PB_WFS_DTYPE();
+    PB_ENTER_REAL(hh);
     if (n < 0 || nmodes < 0 || !(a > 0)) return fail(h, PB_ERR_INVALID, "bad LP mode arguments");
     if (n == 0 || nmodes == 0) return PB_OK;
     if (!r || !out || !plan_host) return fail(h, PB_ERR_INVALID, "null pointer");
@@ -367,18 +354,16 @@ extern "C" int pb_lp_modes(pb_handle_t hh, int dtype, const void* r, const void*
             return fail(h, PB_ERR_INVALID, "bad LP mode plan entry");
         if (m.az != PB_LP_NONE && !t) return fail(h, PB_ERR_INVALID, "an azimuthal mode needs the angle grid");
     }
-    const int gx = grid_for(n, h->sm_count);
+    const int gx = grid_for(n, kThreads, h->sm_count);
     for (int p0 = 0; p0 < nmodes; p0 += kLpMax) {
         LpPlan plan{};
         const int np = std::min(kLpMax, nmodes - p0);
         std::copy(modes.begin() + p0, modes.begin() + p0 + np, plan.m);
         const dim3 grid(gx, np);
-        if (dtype == PB_C64)
-            lp_modes_kernel<float><<<grid, kThreads, 0, st>>>((const float*)r, (const float*)t, n, a, plan,
-                                                              (float*)out + (long long)p0 * n);
-        else
-            lp_modes_kernel<double><<<grid, kThreads, 0, st>>>((const double*)r, (const double*)t, n, a, plan,
-                                                               (double*)out + (long long)p0 * n);
+        with_real(dtype, [&](auto real) {
+            using R = decltype(real);
+            lp_modes_kernel<R><<<grid, kThreads, 0, st>>>((const R*)r, (const R*)t, n, a, plan, (R*)out + (long long)p0 * n);
+        });
         PB_LAUNCH_CHECK(h);
     }
     return PB_OK;
@@ -387,8 +372,7 @@ extern "C" int pb_lp_modes(pb_handle_t hh, int dtype, const void* r, const void*
 extern "C" int pb_overlap(pb_handle_t hh, int dtype, const void* E, long long n, int nmodes, const void* modes,
                           const void* const* mode_ptrs_host, int modes_complex, const double* ip_dev,
                           const double* ie_dev, void* partial, void* eta, void* c_out, void* stream) {
-    PB_WFS_ENTER(hh);
-    PB_WFS_DTYPE();
+    PB_ENTER_REAL(hh);
     if (n <= 0 || nmodes <= 0) return fail(h, PB_ERR_INVALID, "bad overlap sizes");
     if (!E || !partial || !eta || (!modes && !mode_ptrs_host)) return fail(h, PB_ERR_INVALID, "null pointer");
     const long long nchunk_ll = (n + PB_OVERLAP_CHUNK - 1) / PB_OVERLAP_CHUNK;
@@ -396,7 +380,7 @@ extern "C" int pb_overlap(pb_handle_t hh, int dtype, const void* E, long long n,
     const int nchunk = (int)nchunk_ll;
     double* part = reinterpret_cast<double*>(partial);
     double* part_e = part + (long long)nmodes * nchunk * 3;
-    const size_t esz = (dtype == PB_C64 ? 4 : 8) * (modes_complex ? 2 : 1);
+    const size_t esz = rsize(dtype) * (modes_complex ? 2 : 1);
     for (int p0 = 0; p0 < nmodes; p0 += kOvMax) {
         ModeTable tab{};
         const int np = std::min(kOvMax, nmodes - p0);
@@ -411,19 +395,15 @@ extern "C" int pb_overlap(pb_handle_t hh, int dtype, const void* E, long long n,
                 reinterpret_cast<const cplx<R>*>(E), n, np, p0, nchunk, tab, ip_dev == nullptr, ie_dev == nullptr, part,
                 part_e);
         };
-        if (dtype == PB_C64) {
-            if (modes_complex) go(float(), std::true_type()); else go(float(), std::false_type());
-        } else {
-            if (modes_complex) go(double(), std::true_type()); else go(double(), std::false_type());
-        }
+        with_real(dtype, [&](auto r) {
+            if (modes_complex) go(r, std::true_type()); else go(r, std::false_type());
+        });
         PB_LAUNCH_CHECK(h);
     }
-    if (dtype == PB_C64)
-        overlap_finish_kernel<float><<<nmodes, kThreads, 0, st>>>(part, part_e, nchunk, ip_dev, ie_dev, (float*)eta,
-                                                                  (float*)c_out);
-    else
-        overlap_finish_kernel<double><<<nmodes, kThreads, 0, st>>>(part, part_e, nchunk, ip_dev, ie_dev, (double*)eta,
-                                                                   (double*)c_out);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        overlap_finish_kernel<R><<<nmodes, kThreads, 0, st>>>(part, part_e, nchunk, ip_dev, ie_dev, (R*)eta, (R*)c_out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -431,32 +411,28 @@ extern "C" int pb_overlap(pb_handle_t hh, int dtype, const void* E, long long n,
 extern "C" int pb_wfs_combine(pb_handle_t hh, int dtype, long long n, const void* a, const void* b,
                               const double* coefs_host, const void* alpha_scale, const void* beta_scale, int real_out,
                               void* out, void* stream) {
-    PB_WFS_ENTER(hh);
-    PB_WFS_DTYPE();
+    PB_ENTER_REAL(hh);
     if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     if (n == 0) return PB_OK;
     if (!a || !out || !coefs_host) return fail(h, PB_ERR_INVALID, "null pointer");
     const double* k = coefs_host;
-    const int grid = grid_for(n, h->sm_count);
+    const int grid = grid_for(n, kThreads, h->sm_count);
     auto go = [&](auto r, auto ro) {
         using R = decltype(r);
         combine_kernel<R, decltype(ro)::value><<<grid, kThreads, 0, st>>>(
             n, reinterpret_cast<const cplx<R>*>(a), reinterpret_cast<const cplx<R>*>(b), k[0], k[1], k[2], k[3],
             reinterpret_cast<const R*>(alpha_scale), reinterpret_cast<const R*>(beta_scale), out);
     };
-    if (dtype == PB_C64) {
-        if (real_out) go(float(), std::true_type()); else go(float(), std::false_type());
-    } else {
-        if (real_out) go(double(), std::true_type()); else go(double(), std::false_type());
-    }
+    with_real(dtype, [&](auto r) {
+        if (real_out) go(r, std::true_type()); else go(r, std::false_type());
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
 extern "C" int pb_grating(pb_handle_t hh, int dtype, int kind, long long n, const void* x, double shift,
                           const double* params_host, int nparams, const void* E, void* out, void* stream) {
-    PB_WFS_ENTER(hh);
-    PB_WFS_DTYPE();
+    PB_ENTER_REAL(hh);
     if (n < 0 || (kind != PB_GRATING_SIN_AMP && kind != PB_GRATING_RECTANGLE) ||
         nparams != (kind == PB_GRATING_SIN_AMP ? 1 : 6))
         return fail(h, PB_ERR_INVALID, "bad grating arguments");
@@ -464,11 +440,11 @@ extern "C" int pb_grating(pb_handle_t hh, int dtype, int kind, long long n, cons
     if (!x || !out || !params_host) return fail(h, PB_ERR_INVALID, "null pointer");
     GratingParams p{};
     std::copy(params_host, params_host + nparams, p.v);
-    const int grid = grid_for(n, h->sm_count);
-    if (dtype == PB_C64)
-        grating_kernel<float><<<grid, kThreads, 0, st>>>(kind, n, (const float*)x, shift, p, (const float2*)E, out);
-    else
-        grating_kernel<double><<<grid, kThreads, 0, st>>>(kind, n, (const double*)x, shift, p, (const double2*)E, out);
+    const int grid = grid_for(n, kThreads, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        grating_kernel<R><<<grid, kThreads, 0, st>>>(kind, n, (const R*)x, shift, p, (const cplx<R>*)E, out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -476,7 +452,8 @@ extern "C" int pb_grating(pb_handle_t hh, int dtype, int kind, long long n, cons
 extern "C" int pb_psi(pb_handle_t hh, int frame_type, int nframes, const void* const* frames_host, const void* stack,
                       long long frame_stride, long long n, const double* s_host, const double* c_host, int num_type,
                       void* num, void* den, int phase_type, void* phase, void* stream) {
-    PB_WFS_ENTER(hh);
+    PB_ENTER(hh);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (frame_type < PB_PSI_F32 || frame_type > PB_PSI_I32 || nframes < 1 || nframes > kPsiMax || n < 0)
         return fail(h, PB_ERR_INVALID, "bad PSI arguments");
     const bool int_frames = frame_type == PB_PSI_U16 || frame_type == PB_PSI_I32;
@@ -508,7 +485,7 @@ extern "C" int pb_psi(pb_handle_t hh, int frame_type, int nframes, const void* c
         using NT = decltype(nt);
         using PT = decltype(pt);
         const long long groups = n / V;
-        psi_kernel<T, V, decltype(acc), NT, PT><<<grid_for(groups, h->sm_count), kThreads, 0, st>>>(
+        psi_kernel<T, V, decltype(acc), NT, PT><<<grid_for(groups, kThreads, h->sm_count), kThreads, 0, st>>>(
             nframes, groups, plan, (NT*)num, (NT*)den, (PT*)phase);
     };
     using one = std::integral_constant<int, 1>;
