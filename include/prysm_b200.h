@@ -32,6 +32,12 @@ typedef struct pb_handle_s* pb_handle_t;
 
 typedef enum { PB_C64 = 0, PB_C128 = 1 } pb_dtype;
 
+/* the element type of typed storage (frames, mosaics, Jones sources, slopes) in the entry points that take one */
+typedef enum {
+    PB_ELEM_F32 = 0, PB_ELEM_F64 = 1, PB_ELEM_C64 = 2, PB_ELEM_C128 = 3, PB_ELEM_U8 = 4, PB_ELEM_U16 = 5, PB_ELEM_U32 = 6,
+    PB_ELEM_I32 = 7, PB_ELEM_I64 = 8
+} pb_elem;
+
 typedef enum {
     PB_OK = 0,
     PB_ERR_INVALID = -1,      /* bad argument */
@@ -460,7 +466,7 @@ int pb_segment_compose_adjoint(pb_handle_t h, int dtype, int ny, int nx, int nse
 /* ---- Jones calculus (prysm/x/polarization.py) ----------------------------------------------------------------------
  * Element-planar layout: a Jones array of n pixels is 4 contiguous planes of n complex samples at dtype, plane 2*i + j
  * holding J[..., i, j]; Mueller and Kronecker arrays are 16 planes, plane 4*r + c (Mueller planes are real).
- * pb_jones_planar: src is a (rows, cols, 2, 2) array of src_type with strides s_row, s_col, s_i, s_j counted in
+ * pb_jones_planar: src is a (rows, cols, 2, 2) array of src_type (PB_ELEM_F32 / F64 / C64 / C128) with strides s_row, s_col, s_i, s_j counted in
  *   elements of src_type (one complex value is one element); out = its 4 planes (n = rows*cols), converted to dtype.
  * pb_jones_product: out = op_a(A) * op_b(B) per pixel, the 2x2 matrix product (PB_JONES_MATMUL) or the elementwise
  *   product (PB_JONES_HADAMARD).  An operand is a constant 2x2 (PB_JONES_CONST: four complex values from consts_host,
@@ -471,10 +477,9 @@ int pb_segment_compose_adjoint(pb_handle_t h, int dtype, int ny, int nx, int nse
  *   PB_JONES_FILL: 4 complex values (8 doubles);  PB_JONES_ROTATION: theta, scale (with a plane, theta = plane*scale);
  *   PB_JONES_RETARDER / PB_JONES_DIATTENUATOR: theta, retardance / alpha (a plane replaces the second);
  *   PB_JONES_VVR: charge, retardance, rotate, with the azimuth plane (required; it is not modified).
- *   plane: optional, n real values of plane_type PB_JONES_SRC_F32 or PB_JONES_SRC_F64.
+ *   plane: optional, n real values of plane_type PB_ELEM_F32 or PB_ELEM_F64.
  * pb_jones_reduce: PB_JONES_MUELLER: out = 16 real planes of real(U kron(conj a, a) U^-1);  PB_JONES_KRON: out = 16
  *   complex planes of kron(a, b);  PB_JONES_PAULI: out = 4 complex planes c0..c3. */
-typedef enum { PB_JONES_SRC_F32 = 0, PB_JONES_SRC_F64 = 1, PB_JONES_SRC_C64 = 2, PB_JONES_SRC_C128 = 3 } pb_jones_src;
 typedef enum { PB_JONES_CONST = 0, PB_JONES_PLANES = 1, PB_JONES_SCALAR = 2, PB_JONES_SCALAR_REAL = 3 } pb_jones_operand;
 typedef enum { PB_JONES_MATMUL = 0, PB_JONES_HADAMARD = 1 } pb_jones_mode;
 typedef enum { PB_JONES_OP_N = 0, PB_JONES_OP_H = 1 } pb_jones_op;
@@ -510,15 +515,14 @@ int pb_jones_reduce(pb_handle_t h, int dtype, int kind, long long n, const void*
  *   g itself (real) when E is NULL.  PB_GRATING_SIN_AMP params: prefix (g = 1 - (sin(prefix x) + 1) / 2 * 0.1);
  *   PB_GRATING_RECTANGLE params: period, edge, hi, lo, mid, eps (numpy's mod by period, hi below edge else lo, mid
  *   where |x mod period| < eps).
- * pb_psi: num = sum s_k g_k, den = sum c_k g_k over nframes <= 64 frames of frame_type (the host pointer array
- *   frames_host, or `stack` with frame_stride elements between frames) and phase = atan2(num, den).  Any of num,
- *   den and phase may be NULL.  Float frames: num_type = phase_type = frame_type.  Integer frames: phase_type =
- *   PB_PSI_F64 and num_type PB_PSI_I64 (integer weights, exact) or PB_PSI_F64. */
+ * pb_psi: num = sum s_k g_k, den = sum c_k g_k over nframes <= 64 frames of frame_type (PB_ELEM_F32 / F64 / U16 /
+ *   I32; the host pointer array frames_host, or `stack` with frame_stride elements between frames) and phase =
+ *   atan2(num, den).  Any of num, den and phase may be NULL.  Float frames: num_type = phase_type = frame_type.
+ *   Integer frames: phase_type = PB_ELEM_F64 and num_type PB_ELEM_I64 (integer weights, exact) or PB_ELEM_F64. */
 enum { PB_OVERLAP_CHUNK = 4096 };
 typedef enum { PB_LP_RULE_LP = 0, PB_LP_RULE_SMF = 1 } pb_lp_rule;
 typedef enum { PB_LP_NONE = 0, PB_LP_COS = 1, PB_LP_SIN = 2 } pb_lp_azimuth;
 typedef enum { PB_GRATING_SIN_AMP = 0, PB_GRATING_RECTANGLE = 1 } pb_grating_kind;
-typedef enum { PB_PSI_F32 = 0, PB_PSI_F64 = 1, PB_PSI_U16 = 2, PB_PSI_I32 = 3, PB_PSI_I64 = 4 } pb_psi_type;
 int pb_lp_modes(pb_handle_t h, int dtype, const void* r, const void* t, long long n, double a, int nmodes,
                 const double* plan_host, void* out, void* stream);
 int pb_overlap(pb_handle_t h, int dtype, const void* E, long long n, int nmodes, const void* modes,
@@ -550,15 +554,15 @@ int pb_psi(pb_handle_t h, int frame_type, int nframes, const void* const* frames
  *   1 top-right, 2 bottom-left, 3 bottom-right of each 2x2 cell) comes from planes_host[s] (row pitch ld_host[s]) at
  *   (y, x), or at (y / 2, x / 2) with half (recomposite).
  * pb_demosaic_deinterlace: (m / 2, n / 2, 3) = (R, (G1 + G2) / 2, B) of an even-sided mosaic with row pitch ld; the
- *   green sum is formed in in_type (wrapping for unsigned types), the halving in out_type (PB_SENSOR_F32 / F64).
+ *   green sum is formed in in_type (PB_ELEM_F32 / F64 / U8 / U16 / U32; wrapping for unsigned types), the halving in
+ *   out_type (PB_ELEM_F32 / F64).
  * pb_white_balance: a *= gain in place (a contiguous, real at dtype): gains_host[site] for a mosaic (kind 0, rows of
  *   nx) or gains_host[i % 3] for interleaved RGB (kind 1).  With sat_host, every gain is first divided by max(1,
  *   max_p(max(plane p) gains_p / sat_p)), computed on the device in work (fp64, 4 PB_WB_MAX_BLOCKS + 1 values).
- * pb_demosaic_malvar: (m, n, 3) RGB of out_type (PB_SENSOR_F32 from f32 / u8 / u16, or PB_SENSOR_F64) from an m x n
+ * pb_demosaic_malvar: (m, n, 3) RGB of out_type (PB_ELEM_F32 from f32 / u8 / u16, or PB_ELEM_F64) from an m x n
  *   mosaic of in_type with row pitch ld, rggb or bggr: Malvar-He-Cutler's 5x5 filters, scipy.ndimage's reflect
  *   boundary, accumulated in fp64.  One pass.
  * pb_bayer_assemble: (n, 3) = (Re rp, (Re g2p + g1) / 2, Re bp) for complex rp, g2p, bp and real g1 at dtype. */
-typedef enum { PB_SENSOR_F32 = 0, PB_SENSOR_F64 = 1, PB_SENSOR_U8 = 2, PB_SENSOR_U16 = 3, PB_SENSOR_U32 = 4 } pb_sensor_type;
 enum { PB_WB_MAX_BLOCKS = 1024 };
 int pb_expose(pb_handle_t h, int dtype, const void* aerial, long long n, long long nx, const void* prnu, long long prnu_sr,
               long long prnu_sc, const void* dcnu, long long dcnu_sr, long long dcnu_sc, const double* params_host,
@@ -589,18 +593,17 @@ int pb_bayer_assemble(pb_handle_t h, int dtype, const void* rp, const void* g2p,
  *   lenslet r^2.  kind: PB_LENSLET_RECT (|lx| <= w and |ly| <= h), PB_LENSLET_RECT_SWAP (|ly| <= w and |lx| <= h),
  *   PB_LENSLET_RECT_ROTATED (the same after rotating (lx, ly) by the angle in polar form), PB_LENSLET_CIRCLE
  *   (rsq <= lenslet r^2).
- * pb_subaperture_centroids: for nframes frames of frame_type ((H, W) each, frame_stride elements apart) and each
+ * pb_subaperture_centroids: for nframes frames of frame_type (PB_ELEM_F32 / F64 / U16 / I32; (H, W) each, frame_stride elements apart) and each
  *   subaperture (j, i): w = max(I - t, 0) with t = threshold max(I over the subaperture); disp (nframes, 2, nrows,
  *   ncols) = scale (sum w x / sum w - xc[i], sum w y / sum w - yc[j]), NaN where sum w = 0; flux (nframes, nrows, ncols) =
- *   sum I.  out_type: PB_SH_F64 for PB_SH_F64 frames, PB_SH_F32 otherwise; the sums are fp64 in a fixed order.
+ *   sum I.  out_type: PB_ELEM_F64 for PB_ELEM_F64 frames, PB_ELEM_F32 otherwise; the sums are fp64 in a fixed order.
  *   dtab (fp64, device): x of each grid column [W], y of each grid row [H], xc [ncols], yc [nrows].  itab (int32,
  *   device): owning lenslet column of each grid column or -1 [W], each lenslet column's owned grid columns as
  *   [lo, hi): lo [ncols] then hi [ncols], each lenslet row's owned grid rows: lo [nrows] then hi [nrows].  One launch.
  * pb_sh_reconstruct: out[f, k] = sum_m R[k, m] (slopes[f][idx[m]] - ref[m]) for nframes slope vectors frame_stride
  *   elements apart, R (K, M) and ref (M, optional) fp64 on the device, idx int32; slopes and out of dtype
- *   (PB_SH_F32 / PB_SH_F64), accumulated in fp64.  A NaN in a selected slope propagates. */
+ *   (PB_ELEM_F32 / PB_ELEM_F64), accumulated in fp64.  A NaN in a selected slope propagates. */
 typedef enum { PB_LENSLET_RECT = 0, PB_LENSLET_RECT_SWAP = 1, PB_LENSLET_RECT_ROTATED = 2, PB_LENSLET_CIRCLE = 3 } pb_lenslet_kind;
-typedef enum { PB_SH_F32 = 0, PB_SH_F64 = 1, PB_SH_U16 = 2, PB_SH_I32 = 3 } pb_sh_type;
 int pb_lenslet_screen(pb_handle_t h, int dtype, const void* x, const void* y, int H, int W, int ncols, int nrows,
                       const double* centres, const int* cand, int kind, const double* params_host, double two_efl,
                       double kphase, void* out, void* stream);

@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, '_lib', 'libprysm_b200.so')
 
 PB_C64, PB_C128 = 0, 1
+ELEM_F32, ELEM_F64, ELEM_C64, ELEM_C128, ELEM_U8, ELEM_U16, ELEM_U32, ELEM_I32, ELEM_I64 = range(9)
 IN_COMPLEX, IN_REAL, IN_AMP_OPD = 0, 1, 2
 AMP_NONE, AMP_REAL, AMP_U8 = 0, 1, 2
 OUT_COMPLEX, OUT_INTENSITY, OUT_ACCUMULATE = 0, 1, 2
@@ -139,7 +140,6 @@ SIGNATURES = {
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
 SDF_UNION, SDF_INTERSECT, SDF_SUBTRACT = range(3)
 SEGMENT_FIELDS, SEGMENT_TILE_Y, SEGMENT_TILE_X, SEGMENT_CHUNK = 6, 32, 64, 2048
-JONES_SRC_F32, JONES_SRC_F64, JONES_SRC_C64, JONES_SRC_C128 = range(4)
 JONES_CONST, JONES_PLANES, JONES_SCALAR, JONES_SCALAR_REAL = range(4)
 JONES_MATMUL, JONES_HADAMARD = range(2)
 JONES_OP_N, JONES_OP_H = range(2)
@@ -149,11 +149,8 @@ OVERLAP_CHUNK = 4096
 LP_RULE_LP, LP_RULE_SMF = range(2)
 LP_NONE, LP_COS, LP_SIN = range(3)
 GRATING_SIN_AMP, GRATING_RECTANGLE = range(2)
-PSI_F32, PSI_F64, PSI_U16, PSI_I32, PSI_I64 = range(5)
-SENSOR_F32, SENSOR_F64, SENSOR_U8, SENSOR_U16, SENSOR_U32 = range(5)
 WB_MAX_BLOCKS = 1024
 LENSLET_RECT, LENSLET_RECT_SWAP, LENSLET_RECT_ROTATED, LENSLET_CIRCLE = range(4)
-SH_F32, SH_F64, SH_U16, SH_I32 = range(4)
 QPOLY_BFS, QPOLY_CON, QPOLY_2D = range(3)
 QPOLY_VALUE, QPOLY_DER, QPOLY_DER_XY = range(3)
 QPOLY_NMAX = 64

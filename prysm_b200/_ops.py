@@ -1,7 +1,8 @@
 """Thin tensor-level wrappers over the C ABI: each function takes CUDA torch tensors (or host
 arrays, which are uploaded), allocates the output with torch's caching allocator and makes
 exactly one library call on torch's current stream.  PyTorch is plumbing here (device memory,
-streams); every kernel is in libprysm_b200.so.
+streams); every kernel is in libprysm_b200.so.  A wrapper makes its call through `_call`, which supplies the handle
+and stream and checks the status, and gets its output array from `_out`, which allocates it or validates the caller's.
 """
 import math
 import ctypes as C
@@ -16,6 +17,10 @@ _REAL_OF = {torch.complex64: torch.float32, torch.complex128: torch.float64}
 _CPLX_OF = {torch.float32: torch.complex64, torch.float64: torch.complex128}
 _CODE = {torch.complex64: capi.PB_C64, torch.complex128: capi.PB_C128,
          torch.float32: capi.PB_C64, torch.float64: capi.PB_C128}
+# pb_elem code of typed storage; each wrapper still decides which of these its entry point takes
+_ELEM = {torch.float32: capi.ELEM_F32, torch.float64: capi.ELEM_F64, torch.complex64: capi.ELEM_C64,
+         torch.complex128: capi.ELEM_C128, torch.uint8: capi.ELEM_U8, torch.uint16: capi.ELEM_U16,
+         torch.uint32: capi.ELEM_U32, torch.int32: capi.ELEM_I32, torch.int64: capi.ELEM_I64}
 
 _default_device = None
 
@@ -72,6 +77,12 @@ def _ctx(t):
     return capi.handle_for(t.device.index, stream), C.c_void_p(stream)
 
 
+def _call(fn, like, *args):
+    """fn(handle, *args, stream) on the handle and current stream of `like`'s device; a failed status raises."""
+    h, st = _ctx(like)
+    h.check(fn(h.ptr, *args, st))
+
+
 def _p(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
@@ -92,20 +103,50 @@ def _check_out(out, shape, dtype, device, name='out'):
     return out
 
 
-def _contiguous_out(out, shape, like):
-    """A new (shape) array of like's dtype, or the caller's `out` checked to be exactly that and contiguous (the
-    kernels that take it write a dense array)."""
+def _out(out, shape, dtype, device, contiguous=True, name='out'):
+    """A new (shape) array of dtype on device, or the caller's `out` checked to be exactly that, and contiguous when
+    `contiguous` (the kernel then writes a dense array; otherwise it takes the row pitch)."""
     if out is None:
-        return torch.empty(shape, dtype=like.dtype, device=like.device)
-    _check_out(out, shape, like.dtype, like.device)
-    if not out.is_contiguous():
-        raise ValueError('`out` must be contiguous')
+        return torch.empty(shape, dtype=dtype, device=device)
+    _check_out(out, shape, dtype, device, name)
+    if contiguous and not out.is_contiguous():
+        raise ValueError(f'`{name}` must be contiguous')
     return out
 
 
+def _amp_operand(amp, rdtype):
+    """(pb_amp_kind, tensor) of an optional amplitude: a bool / uint8 mask goes as bytes, anything else at rdtype."""
+    if amp is None:
+        return capi.AMP_NONE, None
+    if amp.dtype in (torch.bool, torch.uint8):
+        return capi.AMP_U8, amp.contiguous()
+    return capi.AMP_REAL, amp.to(rdtype).contiguous()
+
+
+def _field_operand(field):
+    """(src, pb_in_kind, complex dtype) of a transform input: a complex field as is, a real one as IN_REAL (float32
+    unless it is float64)."""
+    if field.is_complex():
+        return field, capi.IN_COMPLEX, field.dtype
+    src = field if field.dtype in _CPLX_OF else field.to(torch.float32)
+    return src, capi.IN_REAL, _CPLX_OF[src.dtype]
+
+
+# Host arrays for the library.  numpy allocates at least one byte for an empty array, so an empty sequence still gives
+# a valid pointer; the entry points read no element when its count is 0.
 def _darr(v):
     v = np.ascontiguousarray(v, dtype=np.float64)
     return v, v.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def _iarr(v):
+    v = np.ascontiguousarray(v, dtype=np.int32)
+    return v, v.ctypes.data_as(C.POINTER(C.c_int))
+
+
+def _nm(nms):
+    """the two int32 host arrays (n, m) of a sequence of (n, m) pairs"""
+    return _iarr([nm[0] for nm in nms]), _iarr([nm[1] for nm in nms])
 
 
 # ------------------------------------------------------------------------------------------
@@ -113,39 +154,22 @@ def fft2(field, k=None, *, dir=-1, scale=1.0, shift_in=False, shift_out=False, c
          out_kind=capi.OUT_COMPLEX, weight=1.0, out=None, amp=None, opd=None, kscale=0.0):
     """pb_fft2.  Either `field` (complex or real 2-D tensor) or (amp, opd, kscale)."""
     if opd is not None:
-        src = opd
-        in_kind = capi.IN_AMP_OPD
-        if amp is None:
-            amp_kind, amp_t = capi.AMP_NONE, None
-        elif amp.dtype in (torch.bool, torch.uint8):
-            amp_kind, amp_t = capi.AMP_U8, amp.contiguous()
-        else:
-            amp_kind, amp_t = capi.AMP_REAL, amp.to(opd.dtype).contiguous()
-        cdtype = _CPLX_OF[opd.dtype]
+        src, in_kind, cdtype = opd, capi.IN_AMP_OPD, _CPLX_OF[opd.dtype]
+        amp_kind, amp_t = _amp_operand(amp, opd.dtype)
     else:
-        src = field
+        src, in_kind, cdtype = _field_operand(field)
         amp_kind, amp_t = capi.AMP_NONE, None
-        if field.is_complex():
-            in_kind, cdtype = capi.IN_COMPLEX, field.dtype
-        else:
-            if field.dtype not in _CPLX_OF:
-                src = field.to(torch.float32)
-            in_kind, cdtype = capi.IN_REAL, _CPLX_OF[src.dtype]
     src = src.contiguous()
     ny, nx = src.shape
     ky, kx = (ny, nx) if k is None else k
     oy, ox = (ky, kx) if crop is None else crop
     odt = cdtype if out_kind == capi.OUT_COMPLEX else _REAL_OF[cdtype]
-    if out is None:
-        if out_kind == capi.OUT_ACCUMULATE:
-            raise ValueError('accumulate needs an existing `out` array')
-        out = torch.empty((oy, ox), dtype=odt, device=src.device)
-    else:
-        _check_out(out, (oy, ox), odt, src.device)
-    h, st = _ctx(src)
-    h.check(lib.pb_fft2(h.ptr, _CODE[cdtype], _p(src), in_kind, _p(amp_t), amp_kind, float(kscale),
-                        ny, nx, nx, ky, kx, int(dir), float(scale), int(shift_in), int(shift_out),
-                        _p(out), out_kind, float(weight), oy, ox, out.stride(0), st))
+    if out is None and out_kind == capi.OUT_ACCUMULATE:
+        raise ValueError('accumulate needs an existing `out` array')
+    out = _out(out, (oy, ox), odt, src.device, contiguous=False)
+    _call(lib.pb_fft2, src, _CODE[cdtype], _p(src), in_kind, _p(amp_t), amp_kind, float(kscale), ny, nx, nx, ky, kx,
+          int(dir), float(scale), int(shift_in), int(shift_out), _p(out), out_kind, float(weight), oy, ox,
+          out.stride(0))
     return out
 
 
@@ -154,39 +178,26 @@ def fft2_batch(fields, k=None, *, dir=-1, scale=1.0, shift_in=False, shift_out=F
     """pb_fft2_batch over a (B, ny, nx) stack -> (B, ky, kx): either `fields` (complex or real) or `opd` (B, ny, nx)
     with an optional amplitude that is (ny, nx) (shared) or (B, ny, nx).  `crop` = (oy, ox) keeps the centred
     window of each transform, as fft2's does (the adjoints of focus / unfocus)."""
-    amp_kind, amp_t, amp_bs = capi.AMP_NONE, None, 0
     if opd is not None:
         src = opd if opd.dtype in _CPLX_OF else opd.to(torch.float32)
         in_kind, cdtype = capi.IN_AMP_OPD, _CPLX_OF[src.dtype]
-        if amp is not None:
-            if amp.dtype in (torch.bool, torch.uint8):
-                amp_kind, amp_t = capi.AMP_U8, amp.contiguous()
-            else:
-                amp_kind, amp_t = capi.AMP_REAL, amp.to(src.dtype).contiguous()
-            amp_bs = amp_t.stride(0) if amp_t.ndim == 3 else 0
+        amp_kind, amp_t = _amp_operand(amp, src.dtype)
     else:
-        src = fields
-        if src.is_complex():
-            in_kind, cdtype = capi.IN_COMPLEX, src.dtype
-        else:
-            if src.dtype not in _CPLX_OF:
-                src = src.to(torch.float32)
-            in_kind, cdtype = capi.IN_REAL, _CPLX_OF[src.dtype]
+        src, in_kind, cdtype = _field_operand(fields)
+        amp_kind, amp_t = capi.AMP_NONE, None
+    amp_bs = amp_t.stride(0) if amp_t is not None and amp_t.ndim == 3 else 0
     src = src.contiguous()
     nb, ny, nx = src.shape
     ky, kx = (ny, nx) if k is None else k
     oy, ox = (ky, kx) if crop is None else crop
     odt = cdtype if out_kind == capi.OUT_COMPLEX else _REAL_OF[cdtype]
-    if out is None:
-        out = torch.empty((nb, oy, ox), dtype=odt, device=src.device)
-    else:
-        _check_out(out, (nb, oy, ox), odt, src.device)
-        if out.stride(1) < ox or (nb > 1 and out.stride(0) < (oy - 1) * out.stride(1) + ox):
-            raise ValueError('`out` rows / fields overlap')
-    h, st = _ctx(src)
-    h.check(lib.pb_fft2_batch(h.ptr, _CODE[cdtype], _p(src), in_kind, _p(amp_t), amp_kind, float(kscale), nb,
-                              src.stride(0), amp_bs, ny, nx, src.stride(1), ky, kx, int(dir), float(scale), int(shift_in),
-                              int(shift_out), _p(out), out_kind, 1.0, oy, ox, out.stride(1), out.stride(0), st))
+    given = out is not None
+    out = _out(out, (nb, oy, ox), odt, src.device, contiguous=False)
+    if given and (out.stride(1) < ox or (nb > 1 and out.stride(0) < (oy - 1) * out.stride(1) + ox)):
+        raise ValueError('`out` rows / fields overlap')
+    _call(lib.pb_fft2_batch, src, _CODE[cdtype], _p(src), in_kind, _p(amp_t), amp_kind, float(kscale), nb,
+          src.stride(0), amp_bs, ny, nx, src.stride(1), ky, kx, int(dir), float(scale), int(shift_in), int(shift_out),
+          _p(out), out_kind, 1.0, oy, ox, out.stride(1), out.stride(0))
     return out
 
 
@@ -199,9 +210,7 @@ def fft1(a, n=None, axis=-1, dir=-1, scale=1.0):
         n = a.shape[axis]
     oshape = (n, nx) if axis == 0 else (ny, n)
     out = torch.empty(oshape, dtype=a.dtype, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_fft1(h.ptr, _CODE[a.dtype], _p(a), ny, nx, nx, axis, int(n), int(dir), float(scale),
-                        _p(out), oshape[1], st))
+    _call(lib.pb_fft1, a, _CODE[a.dtype], _p(a), ny, nx, nx, axis, int(n), int(dir), float(scale), _p(out), oshape[1])
     return out
 
 
@@ -214,12 +223,10 @@ def axis_dft(a, n, axis, dir=-1, scale=1.0, pre_e=None, pre_e_conj=False, pre_b=
     if n_out is None:
         n_out = n - out_off
     oshape = (n_out, nx) if axis == 0 else (ny, n_out)
-    out = _contiguous_out(out, oshape, a)
-    h, st = _ctx(a)
-    h.check(lib.pb_axis_dft(h.ptr, _CODE[a.dtype], _p(a), ny, nx, nx, axis, int(n), int(dir), float(scale),
-                            _p(pre_e), int(pre_e_conj), _p(pre_b), int(pre_b_conj),
-                            _p(post_e), int(post_e_conj), _p(post_b), int(post_b_conj),
-                            int(out_off), int(n_out), _p(out), oshape[1], st))
+    out = _out(out, oshape, a.dtype, a.device)
+    _call(lib.pb_axis_dft, a, _CODE[a.dtype], _p(a), ny, nx, nx, axis, int(n), int(dir), float(scale), _p(pre_e),
+          int(pre_e_conj), _p(pre_b), int(pre_b_conj), _p(post_e), int(post_e_conj), _p(post_b), int(post_b_conj),
+          int(out_off), int(n_out), _p(out), oshape[1])
     return out
 
 
@@ -229,16 +236,14 @@ def czt_plan(N, M, K, shift, alpha, sign, xc, f0, df, cdtype, dev):
     post = torch.empty(M, dtype=cdtype, device=dev)
     H = torch.empty(K, dtype=cdtype, device=dev)
     Hadj = torch.empty(K, dtype=cdtype, device=dev)
-    h, st = _ctx(b)
-    h.check(lib.pb_czt_plan(h.ptr, _CODE[cdtype], int(N), int(M), int(K), float(shift), float(alpha), int(sign), float(xc),
-                            float(f0), float(df), _p(b), _p(post), _p(H), _p(Hadj), st))
+    _call(lib.pb_czt_plan, b, _CODE[cdtype], int(N), int(M), int(K), float(shift), float(alpha), int(sign), float(xc),
+          float(f0), float(df), _p(b), _p(post), _p(H), _p(Hadj))
     return b, post, H, Hadj
 
 
 def polychromatic_czt(amp, opd, m, K, units, plane):
     """pb_polychromatic_czt: plane += sum_i weight_i |CZT_i(amp exp(i kscale_i opd))|^2 for the rows of `units`
     (host float64 array (n_units, 8): kscale, shift, alpha, xc, f0, df, norm, weight) -- one library call for the loop."""
-    import numpy as np
     opd = opd.contiguous()
     n = opd.shape[0]
     if opd.ndim != 2 or opd.shape[1] != n:
@@ -246,28 +251,19 @@ def polychromatic_czt(amp, opd, m, K, units, plane):
     rdt = opd.dtype
     if rdt not in _CPLX_OF:
         raise ValueError('opd must be float32 or float64')
-    if amp is None:
-        amp_kind, amp_t = capi.AMP_NONE, None
-    elif amp.dtype in (torch.bool, torch.uint8):
-        amp_kind, amp_t = capi.AMP_U8, amp.contiguous()
-    else:
-        amp_kind, amp_t = capi.AMP_REAL, amp.to(rdt).contiguous()
+    amp_kind, amp_t = _amp_operand(amp, rdt)
     if amp_t is not None and tuple(amp_t.shape) != (n, n):
         raise ValueError('amplitude and OPD shapes differ')
-    _check_out(plane, (m, m), rdt, opd.device, name='plane')
-    if not plane.is_contiguous():
-        raise ValueError('`plane` must be contiguous')
-    units = np.ascontiguousarray(units, dtype=np.float64)
+    _out(plane, (m, m), rdt, opd.device, name='plane')
+    units, up = _darr(units)
     if units.ndim != 2 or units.shape[1] != 8:
         raise ValueError('units must have shape (n_units, 8)')
     code = _CODE[_CPLX_OF[rdt]]
     nbytes = int(lib.pb_polychromatic_czt_work_bytes(code, n, int(m), int(K)))
     work = torch.empty(nbytes + 256, dtype=torch.uint8, device=opd.device)
     off = (-work.data_ptr()) % 256
-    h, st = _ctx(opd)
-    import ctypes
-    h.check(lib.pb_polychromatic_czt(h.ptr, code, _p(amp_t), amp_kind, _p(opd), n, int(m), int(K), int(units.shape[0]),
-                                     units.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), work.data_ptr() + off, _p(plane), st))
+    _call(lib.pb_polychromatic_czt, opd, code, _p(amp_t), amp_kind, _p(opd), n, int(m), int(K), int(units.shape[0]), up,
+          work.data_ptr() + off, _p(plane))
     return plane
 
 
@@ -281,22 +277,17 @@ def czt_axis(a, K, axis, pre_e, H, post_e, out_off, n_out, scale=1.0, pre_conj=F
     ny, nx = a.shape
     axis = axis % 2
     oshape = (n_out, nx) if axis == 0 else (ny, n_out)
-    h, st = _ctx(a)
     if out_kind != capi.OUT_COMPLEX:     # |.|^2 (written or accumulated with `weight`) formed in the pass's store
-        rd = _REAL_OF[a.dtype]
-        if out is None:
-            if out_kind == capi.OUT_ACCUMULATE:
-                raise ValueError('accumulate needs an existing `out` array')
-            out = torch.empty(oshape, dtype=rd, device=a.device)
-        else:
-            _check_out(out, oshape, rd, a.device)
-        h.check(lib.pb_czt_axis_intensity(h.ptr, _CODE[a.dtype], _p(a), ny, nx, a.stride(0), axis, int(K), _p(pre_e),
-                                          int(pre_conj), _p(H), _p(post_e), int(post_conj), int(out_off), int(n_out),
-                                          float(scale), int(out_kind), float(weight), _p(out), out.stride(0), st))
+        if out is None and out_kind == capi.OUT_ACCUMULATE:
+            raise ValueError('accumulate needs an existing `out` array')
+        out = _out(out, oshape, _REAL_OF[a.dtype], a.device, contiguous=False)
+        _call(lib.pb_czt_axis_intensity, a, _CODE[a.dtype], _p(a), ny, nx, a.stride(0), axis, int(K), _p(pre_e),
+              int(pre_conj), _p(H), _p(post_e), int(post_conj), int(out_off), int(n_out), float(scale), int(out_kind),
+              float(weight), _p(out), out.stride(0))
         return out
-    out = _contiguous_out(out, oshape, a)
-    h.check(lib.pb_czt_axis(h.ptr, _CODE[a.dtype], _p(a), ny, nx, a.stride(0), axis, int(K), _p(pre_e), int(pre_conj), _p(H),
-                            _p(post_e), int(post_conj), int(out_off), int(n_out), float(scale), _p(out), oshape[1], st))
+    out = _out(out, oshape, a.dtype, a.device)
+    _call(lib.pb_czt_axis, a, _CODE[a.dtype], _p(a), ny, nx, a.stride(0), axis, int(K), _p(pre_e), int(pre_conj), _p(H),
+          _p(post_e), int(post_conj), int(out_off), int(n_out), float(scale), _p(out), oshape[1])
     return out
 
 
@@ -308,19 +299,18 @@ def angular_spectrum(field, k, ty=None, tx=None, tf=None, conj_tf=False, crop=No
     ny, nx = field.shape
     ky, kx = k
     oy, ox = (ky, kx) if crop is None else crop
-    out = _contiguous_out(out, (oy, ox), field)
+    out = _out(out, (oy, ox), field.dtype, field.device)
     if tf is not None:
         tf = tf.to(field.dtype).contiguous()
-    h, st = _ctx(field)
     if screen is not None:
         if tuple(screen.shape) != (ny, nx):
             raise ValueError(f'shape mismatch {(ny, nx)} vs {tuple(screen.shape)}')
         screen = ascomplex(screen).to(field.dtype).contiguous()
-        h.check(lib.pb_angular_spectrum_screen(h.ptr, _CODE[field.dtype], _p(field), _p(screen), int(conj_screen), ny, nx, ky,
-                                               kx, _p(ty), _p(tx), _p(tf), int(conj_tf), _p(out), oy, ox, st))
+        _call(lib.pb_angular_spectrum_screen, field, _CODE[field.dtype], _p(field), _p(screen), int(conj_screen), ny,
+              nx, ky, kx, _p(ty), _p(tx), _p(tf), int(conj_tf), _p(out), oy, ox)
         return out
-    h.check(lib.pb_angular_spectrum(h.ptr, _CODE[field.dtype], _p(field), ny, nx, ky, kx, _p(ty), _p(tx), _p(tf),
-                                    int(conj_tf), _p(out), oy, ox, st))
+    _call(lib.pb_angular_spectrum, field, _CODE[field.dtype], _p(field), ny, nx, ky, kx, _p(ty), _p(tx), _p(tf),
+          int(conj_tf), _p(out), oy, ox)
     return out
 
 
@@ -345,9 +335,7 @@ def angular_spectrum_vectors(shape, wvl, dx, z, cdtype, dev):
             return hit
     ty = torch.empty(ky, dtype=cdtype, device=dev)
     tx = torch.empty(kx, dtype=cdtype, device=dev)
-    h, st = _ctx(ty)
-    h.check(lib.pb_angular_spectrum_vectors(h.ptr, _CODE[cdtype], ky, kx, float(wvl), float(dx), float(z),
-                                            _p(ty), _p(tx), st))
+    _call(lib.pb_angular_spectrum_vectors, ty, _CODE[cdtype], ky, kx, float(wvl), float(dx), float(z), _p(ty), _p(tx))
     if key is not None:
         _AS_VECTORS[key] = (ty, tx)
         while len(_AS_VECTORS) > 8:
@@ -360,8 +348,7 @@ def mdft_basis(f, x, sign, cdtype, dev):
     f, fp = _darr(f)
     x, xp = _darr(x)
     E = torch.empty((len(f), len(x)), dtype=cdtype, device=dev)
-    h, st = _ctx(E)
-    h.check(lib.pb_mdft_basis(h.ptr, _CODE[cdtype], fp, len(f), xp, len(x), int(sign), _p(E), st))
+    _call(lib.pb_mdft_basis, E, _CODE[cdtype], fp, len(f), xp, len(x), int(sign), _p(E))
     return E
 
 
@@ -374,9 +361,8 @@ def cgemm(A, B, opA=capi.OP_N, opB=capi.OP_N, alpha=1.0):
         raise ValueError(f'matmul: inner dimensions {k} and {kb} differ')
     A, B = A.contiguous(), B.contiguous()
     out = torch.empty((m, n), dtype=A.dtype, device=A.device)
-    h, st = _ctx(A)
-    h.check(lib.pb_cgemm(h.ptr, _CODE[A.dtype], opA, opB, m, n, k, float(alpha), _p(A), A.shape[1], _p(B), B.shape[1],
-                         _p(out), n, st))
+    _call(lib.pb_cgemm, A, _CODE[A.dtype], opA, opB, m, n, k, float(alpha), _p(A), A.shape[1], _p(B), B.shape[1],
+          _p(out), n)
     return out
 
 
@@ -388,12 +374,11 @@ def mdft_apply(Ey, Ex, a, norm, adjoint, left_first, out=None):
     if tuple(a.shape) != want:
         raise ValueError(f'array of shape {tuple(a.shape)} does not match the executor ({want})')
     oshape = (ny, nx) if adjoint else (my, mx)
-    out = _contiguous_out(out, oshape, a)
+    out = _out(out, oshape, a.dtype, a.device)
     nwork = lib.pb_mdft_work_elems(my, ny, mx, nx, int(adjoint), int(left_first))
     work = torch.empty(nwork, dtype=a.dtype, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_mdft_apply(h.ptr, _CODE[a.dtype], _p(Ey), _p(Ex), my, ny, mx, nx, _p(a), _p(out), float(norm),
-                              int(adjoint), int(left_first), _p(work), st))
+    _call(lib.pb_mdft_apply, a, _CODE[a.dtype], _p(Ey), _p(Ex), my, ny, mx, nx, _p(a), _p(out), float(norm),
+          int(adjoint), int(left_first), _p(work))
     return out
 
 
@@ -406,8 +391,7 @@ def mdft_tc_expand(E):
     m, n = E.shape
     hi = torch.empty((2 * m, 2 * n), dtype=torch.float32, device=E.device)
     lo = torch.empty_like(hi)
-    h, st = _ctx(E)
-    h.check(lib.pb_mdft_tc_expand(h.ptr, _p(E), m, n, _p(hi), _p(lo), st))
+    _call(lib.pb_mdft_tc_expand, E, _p(E), m, n, _p(hi), _p(lo))
     return hi, lo
 
 
@@ -424,11 +408,10 @@ def mdft_tc_apply(ex_hi, ex_lo, ey_hi, ey_lo, a, norm, out=None):
     a = _tc_aligned(a)
     if tuple(a.shape) != (ny, nx):
         raise ValueError(f'array of shape {tuple(a.shape)} does not match the executor ({(ny, nx)})')
-    out = _contiguous_out(out, (my, mx), a)
+    out = _out(out, (my, mx), a.dtype, a.device)
     work = torch.empty(lib.pb_mdft_tc_work_bytes(my, ny, mx, nx), dtype=torch.uint8, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_mdft_tc_apply(h.ptr, _p(ex_hi), _p(ex_lo), _p(ey_hi), _p(ey_lo), my, ny, mx, nx, _p(a), _p(out),
-                                 float(norm), _p(work), st))
+    _call(lib.pb_mdft_tc_apply, a, _p(ex_hi), _p(ex_lo), _p(ey_hi), _p(ey_lo), my, ny, mx, nx, _p(a), _p(out),
+          float(norm), _p(work))
     return out
 
 
@@ -436,30 +419,17 @@ def phase_screen(amp, opd, kscale):
     opd = opd.contiguous()
     if opd.dtype not in _CPLX_OF:
         opd = opd.to(torch.float32)
-    if amp is None:
-        amp_kind, amp_t = capi.AMP_NONE, None
-    elif amp.dtype in (torch.bool, torch.uint8):
-        amp_kind, amp_t = capi.AMP_U8, amp.contiguous()
-    else:
-        amp_kind, amp_t = capi.AMP_REAL, amp.to(opd.dtype).contiguous()
+    amp_kind, amp_t = _amp_operand(amp, opd.dtype)
     out = torch.empty(opd.shape, dtype=_CPLX_OF[opd.dtype], device=opd.device)
-    h, st = _ctx(opd)
-    h.check(lib.pb_phase_screen(h.ptr, _CODE[opd.dtype], _p(amp_t), amp_kind, _p(opd), float(kscale), opd.numel(),
-                                _p(out), st))
+    _call(lib.pb_phase_screen, opd, _CODE[opd.dtype], _p(amp_t), amp_kind, _p(opd), float(kscale), opd.numel(), _p(out))
     return out
 
 
 def intensity(field, weight=1.0, out=None):
     field = field.contiguous()
     acc = out is not None
-    if out is None:
-        out = torch.empty(field.shape, dtype=_REAL_OF[field.dtype], device=field.device)
-    else:
-        _check_out(out, field.shape, _REAL_OF[field.dtype], field.device)
-        if not out.is_contiguous():
-            raise ValueError('`out` must be contiguous')
-    h, st = _ctx(field)
-    h.check(lib.pb_intensity(h.ptr, _CODE[field.dtype], _p(field), field.numel(), float(weight), int(acc), _p(out), st))
+    out = _out(out, field.shape, _REAL_OF[field.dtype], field.device)
+    _call(lib.pb_intensity, field, _CODE[field.dtype], _p(field), field.numel(), float(weight), int(acc), _p(out))
     return out
 
 
@@ -477,9 +447,7 @@ def binary(op, a, b, reverse=False):
     else:
         s, b = complex(b), None
     out = torch.empty_like(a)
-    h, st = _ctx(a)
-    h.check(lib.pb_binary(h.ptr, _CODE[a.dtype], _BINOPS[op], _p(a), _p(b), s.real, s.imag, int(reverse), a.numel(),
-                          _p(out), st))
+    _call(lib.pb_binary, a, _CODE[a.dtype], _BINOPS[op], _p(a), _p(b), s.real, s.imag, int(reverse), a.numel(), _p(out))
     return out
 
 
@@ -488,13 +456,9 @@ def mul_outer(a, vy=None, vx=None, conj_y=False, conj_x=False, scale=1.0, out=No
     if a.stride(1) != 1:
         a = a.contiguous()
     ny, nx = a.shape
-    if out is None:
-        out = torch.empty((ny, nx), dtype=a.dtype, device=a.device)
-    else:
-        _check_out(out, (ny, nx), a.dtype, a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_mul_outer(h.ptr, _CODE[a.dtype], _p(a), a.stride(0), ny, nx, _p(vy), int(conj_y), _p(vx),
-                             int(conj_x), float(scale), _p(out), out.stride(0), st))
+    out = _out(out, (ny, nx), a.dtype, a.device, contiguous=False)
+    _call(lib.pb_mul_outer, a, _CODE[a.dtype], _p(a), a.stride(0), ny, nx, _p(vy), int(conj_y), _p(vx), int(conj_x),
+          float(scale), _p(out), out.stride(0))
     return out
 
 
@@ -503,8 +467,7 @@ def weighted_sum(modes, weights):
     k = modes.shape[0]
     w, wp = _darr(weights)
     out = torch.empty(modes.shape[1:], dtype=modes.dtype, device=modes.device)
-    h, st = _ctx(modes)
-    h.check(lib.pb_weighted_sum(h.ptr, _CODE[modes.dtype], _p(modes), k, out.numel(), wp, _p(out), st))
+    _call(lib.pb_weighted_sum, modes, _CODE[modes.dtype], _p(modes), k, out.numel(), wp, _p(out))
     return out
 
 
@@ -515,8 +478,7 @@ def otf_normalize(D, which):
     mtf = torch.empty((ny, nx), dtype=rd, device=D.device) if which & 1 else None
     ptf = torch.empty((ny, nx), dtype=rd, device=D.device) if which & 2 else None
     otf = torch.empty((ny, nx), dtype=D.dtype, device=D.device) if which & 4 else None
-    h, st = _ctx(D)
-    h.check(lib.pb_otf_normalize(h.ptr, _CODE[D.dtype], _p(D), ny, nx, which, _p(mtf), _p(ptf), _p(otf), st))
+    _call(lib.pb_otf_normalize, D, _CODE[D.dtype], _p(D), ny, nx, which, _p(mtf), _p(ptf), _p(otf))
     return mtf, ptf, otf
 
 
@@ -525,8 +487,7 @@ def encircled_energy(mtf, df, radii_mm):
     ny, nx = mtf.shape
     r, rp = _darr(radii_mm)
     out = (C.c_double * len(r))()
-    h, st = _ctx(mtf)
-    h.check(lib.pb_encircled_energy(h.ptr, _CODE[mtf.dtype], _p(mtf), ny, nx, float(df), rp, len(r), out, st))
+    _call(lib.pb_encircled_energy, mtf, _CODE[mtf.dtype], _p(mtf), ny, nx, float(df), rp, len(r), out)
     return np.array(out[:])
 
 
@@ -536,8 +497,7 @@ def moments(data):
         data = data.to(torch.float32)
     ny, nx = data.shape
     sums = (C.c_double * 3)()
-    h, st = _ctx(data)
-    h.check(lib.pb_moments(h.ptr, _CODE[data.dtype], _p(data), ny, nx, sums, st))
+    _call(lib.pb_moments, data, _CODE[data.dtype], _p(data), ny, nx, sums)
     return sums[0], sums[1], sums[2]
 
 
@@ -563,16 +523,11 @@ def mask_multiply(a, m=None, *, b=None, w=None, conj=False, one_minus=False, rea
     w = None if w is None else same(asdevice(w), 'window').to(rd).contiguous()
     flags = (capi.MASK_CONJ if conj else 0) | (capi.MASK_ONE_MINUS if one_minus else 0) | \
             (capi.MASK_REAL_OUT if real_out else 0)
-    if out is None:
-        out = torch.empty(a.shape, dtype=rd if real_out else a.dtype, device=a.device)
-    else:
-        _check_out(out, a.shape, rd if real_out else a.dtype, a.device)
-        if not out.is_contiguous():
-            raise ValueError('`out` must be contiguous')
+    if out is not None:
         flags |= capi.MASK_ACCUMULATE
-    h, st = _ctx(a)
-    h.check(lib.pb_mask_multiply(h.ptr, _CODE[a.dtype], _p(a), _p(b), _p(m), kind, flags, _p(w), float(scale),
-                                 a.numel(), _p(out), st))
+    out = _out(out, a.shape, rd if real_out else a.dtype, a.device)
+    _call(lib.pb_mask_multiply, a, _CODE[a.dtype], _p(a), _p(b), _p(m), kind, flags, _p(w), float(scale), a.numel(),
+          _p(out))
     return out
 
 
@@ -583,9 +538,8 @@ def field_adjoint(mode, field, bar, opd, kscale):
     field = None if field is None else field.to(bar.dtype).contiguous()
     opd = None if opd is None else asdevice(opd).to(rd).contiguous()
     out = torch.empty(bar.shape, dtype=bar.dtype if mode == 0 else rd, device=bar.device)
-    h, st = _ctx(bar)
-    h.check(lib.pb_field_adjoint(h.ptr, _CODE[bar.dtype], int(mode), _p(field), _p(bar), _p(opd), float(kscale),
-                                 bar.numel(), _p(out), st))
+    _call(lib.pb_field_adjoint, bar, _CODE[bar.dtype], int(mode), _p(field), _p(bar), _p(opd), float(kscale),
+          bar.numel(), _p(out))
     return out
 
 
@@ -593,9 +547,8 @@ def component(which, field):
     """re / im / angle / abs of a complex tensor as a contiguous real tensor (pb_component)."""
     field = field.contiguous()
     out = torch.empty(field.shape, dtype=_REAL_OF[field.dtype], device=field.device)
-    h, st = _ctx(field)
-    h.check(lib.pb_component(h.ptr, _CODE[field.dtype], {'real': 0, 'imag': 1, 'angle': 2, 'abs': 3}[which], _p(field),
-                             field.numel(), _p(out), st))
+    _call(lib.pb_component, field, _CODE[field.dtype], {'real': 0, 'imag': 1, 'angle': 2, 'abs': 3}[which], _p(field),
+          field.numel(), _p(out))
     return out
 
 
@@ -607,8 +560,7 @@ def dot(a, b, w=None):
         raise ValueError(f'shape mismatch {tuple(a.shape)} vs {tuple(b.shape)}')
     w = None if w is None else asdevice(w).to(_REAL_OF[a.dtype]).contiguous()
     out = (C.c_double * 2)()
-    h, st = _ctx(a)
-    h.check(lib.pb_dot(h.ptr, _CODE[a.dtype], _p(a), _p(b), _p(w), a.numel(), out, st))
+    _call(lib.pb_dot, a, _CODE[a.dtype], _p(a), _p(b), _p(w), a.numel(), out)
     return complex(out[0], out[1])
 
 
@@ -621,8 +573,7 @@ def mode_projection(modes, bar):
     if tuple(bar.shape) != tuple(modes.shape[1:]):
         raise ValueError(f'shape mismatch: modes {tuple(modes.shape)} vs gradient {tuple(bar.shape)}')
     out = (C.c_double * (2 * k))()
-    h, st = _ctx(modes)
-    h.check(lib.pb_mode_projection(h.ptr, _CODE[modes.dtype], _p(modes), k, bar.numel(), _p(bar), int(cplx), out, st))
+    _call(lib.pb_mode_projection, modes, _CODE[modes.dtype], _p(modes), k, bar.numel(), _p(bar), int(cplx), out)
     v = np.array(out[:]).reshape(k, 2)
     return v[:, 0] + 1j * v[:, 1] if cplx else v[:, 0].copy()
 
@@ -636,8 +587,7 @@ def otf_adjoint_seed(which, bar, D):
     if tuple(bar.shape) != (ny, nx):
         raise ValueError(f'shape mismatch: gradient {tuple(bar.shape)} vs transform {(ny, nx)}')
     out = torch.empty_like(D)
-    h, st = _ctx(D)
-    h.check(lib.pb_otf_adjoint_seed(h.ptr, _CODE[D.dtype], int(which), _p(bar), _p(D), ny, nx, _p(out), st))
+    _call(lib.pb_otf_adjoint_seed, D, _CODE[D.dtype], int(which), _p(bar), _p(D), ny, nx, _p(out))
     return out
 
 
@@ -648,8 +598,7 @@ def encircled_energy_adjoint_seed(shape, df, radii_mm, ee_bar, rdtype, dev):
     if len(r) != len(b):
         raise ValueError('one gradient value per radius is required')
     out = torch.empty((ny, nx), dtype=rdtype, device=dev)
-    h, st = _ctx(out)
-    h.check(lib.pb_encircled_energy_adjoint_seed(h.ptr, _CODE[rdtype], ny, nx, float(df), rp, bp, len(r), _p(out), st))
+    _call(lib.pb_encircled_energy_adjoint_seed, out, _CODE[rdtype], ny, nx, float(df), rp, bp, len(r), _p(out))
     return out
 
 
@@ -657,8 +606,7 @@ def vortex_phase(charge, xf, yf):
     xf = xf.contiguous()
     yf = yf.to(xf.dtype).contiguous()
     out = torch.empty(xf.shape, dtype=_CPLX_OF[xf.dtype], device=xf.device)
-    h, st = _ctx(xf)
-    h.check(lib.pb_vortex_phase(h.ptr, _CODE[xf.dtype], int(charge), _p(xf), _p(yf), xf.numel(), _p(out), st))
+    _call(lib.pb_vortex_phase, xf, _CODE[xf.dtype], int(charge), _p(xf), _p(yf), xf.numel(), _p(out))
     return out
 
 
@@ -675,9 +623,8 @@ def resample_bilinear(cmap, xf, yf, cx, cy, dx, fill):
     else:
         fs = complex(fill)
     out = torch.empty(xf.shape, dtype=cd, device=xf.device)
-    h, st = _ctx(xf)
-    h.check(lib.pb_resample_bilinear(h.ptr, _CODE[cd], _p(cmap), ny, nx, _p(xf), _p(yf), xf.numel(), float(cx), float(cy),
-                                     float(dx), _p(fill_t), fs.real, fs.imag, _p(out), st))
+    _call(lib.pb_resample_bilinear, xf, _CODE[cd], _p(cmap), ny, nx, _p(xf), _p(yf), xf.numel(), float(cx), float(cy),
+          float(dx), _p(fill_t), fs.real, fs.imag, _p(out))
     return out
 
 
@@ -687,15 +634,9 @@ def radial_window(shape, fdx, shift, here, nxt, rdtype, dev):
     win, xf, yf = (torch.empty((ny, nx), dtype=rdtype, device=dev) for _ in range(3))
     a0, b0 = here if here is not None else (-1.0, 0.0)
     a1, b1 = nxt if nxt is not None else (-1.0, 0.0)
-    h, st = _ctx(win)
-    h.check(lib.pb_radial_window(h.ptr, _CODE[rdtype], ny, nx, float(fdx), float(shift), float(a0), float(b0), float(a1),
-                                 float(b1), _p(win), _p(xf), _p(yf), st))
+    _call(lib.pb_radial_window, win, _CODE[rdtype], ny, nx, float(fdx), float(shift), float(a0), float(b0), float(a1),
+          float(b1), _p(win), _p(xf), _p(yf))
     return win, xf, yf
-
-
-def _iarr(v):
-    v = np.ascontiguousarray(v, dtype=np.int32)
-    return v, v.ctypes.data_as(C.POINTER(C.c_int))
 
 
 def xy_grid(shape, dx, rdtype, dev, want='xy'):
@@ -703,9 +644,8 @@ def xy_grid(shape, dx, rdtype, dev, want='xy'):
     ny, nx = shape
     out = {k: torch.empty((ny, nx), dtype=rdtype, device=dev) for k in want}
     any_t = next(iter(out.values()))
-    h, st = _ctx(any_t)
-    h.check(lib.pb_xy_grid(h.ptr, _CODE[rdtype], ny, nx, float(dx), _p(out.get('x')), _p(out.get('y')), _p(out.get('r')),
-                           _p(out.get('t')), st))
+    _call(lib.pb_xy_grid, any_t, _CODE[rdtype], ny, nx, float(dx), _p(out.get('x')), _p(out.get('y')), _p(out.get('r')),
+          _p(out.get('t')))
     return out
 
 
@@ -713,8 +653,7 @@ def cart_to_polar(x, y):
     x = x.contiguous()
     y = y.to(x.dtype).contiguous()
     r, t = torch.empty_like(x), torch.empty_like(x)
-    h, st = _ctx(x)
-    h.check(lib.pb_cart_to_polar(h.ptr, _CODE[x.dtype], _p(x), _p(y), x.numel(), _p(r), _p(t), st))
+    _call(lib.pb_cart_to_polar, x, _CODE[x.dtype], _p(x), _p(y), x.numel(), _p(r), _p(t))
     return r, t
 
 
@@ -722,8 +661,7 @@ def circle(r, radius, aa_dx=0.0):
     """bool mask r - radius <= 0, or with aa_dx > 0 the one-sample grey-edge coverage (pb_circle)."""
     r = r.contiguous()
     out = torch.empty(r.shape, dtype=r.dtype if aa_dx > 0 else torch.bool, device=r.device)
-    h, st = _ctx(r)
-    h.check(lib.pb_circle(h.ptr, _CODE[r.dtype], _p(r), r.numel(), float(radius), float(aa_dx), _p(out), st))
+    _call(lib.pb_circle, r, _CODE[r.dtype], _p(r), r.numel(), float(radius), float(aa_dx), _p(out))
     return out
 
 
@@ -738,8 +676,7 @@ def jacobi_seq(ns, alpha, beta, x):
     out = torch.empty((len(ns),) + tuple(x.shape), dtype=x.dtype, device=x.device)
     if not ns:
         return out
-    h, st = _ctx(x)
-    h.check(lib.pb_jacobi_seq(h.ptr, _CODE[x.dtype], _p(x), x.numel(), nmax, float(alpha), float(beta), sp, _p(out), st))
+    _call(lib.pb_jacobi_seq, x, _CODE[x.dtype], _p(x), x.numel(), nmax, float(alpha), float(beta), sp, _p(out))
     return out
 
 
@@ -750,11 +687,9 @@ def zernike_seq(nms, a, b, norm, polar):
     out = torch.empty((k,) + tuple(a.shape), dtype=a.dtype, device=a.device)
     if k == 0:
         return out
-    n, nptr = _iarr([nm[0] for nm in nms])
-    m, mptr = _iarr([nm[1] for nm in nms])
-    h, st = _ctx(a)
-    h.check(lib.pb_zernike_seq(h.ptr, _CODE[a.dtype], int(polar), _p(a), _p(b), a.numel(), k, nptr, mptr, int(bool(norm)),
-                               _p(out), st))
+    (n, nptr), (m, mptr) = _nm(nms)
+    _call(lib.pb_zernike_seq, a, _CODE[a.dtype], int(polar), _p(a), _p(b), a.numel(), k, nptr, mptr, int(bool(norm)),
+          _p(out))
     return out
 
 
@@ -763,12 +698,10 @@ def zernike_sum(coefs, nms, a, b, norm, polar):
     b = b.to(a.dtype).contiguous()
     k = len(nms)
     out = torch.empty(a.shape, dtype=a.dtype, device=a.device)
-    n, nptr = _iarr([nm[0] for nm in nms])
-    m, mptr = _iarr([nm[1] for nm in nms])
+    (n, nptr), (m, mptr) = _nm(nms)
     c, cptr = _darr(np.asarray(coefs, dtype=np.float64)[:k])
-    h, st = _ctx(a)
-    h.check(lib.pb_zernike_sum(h.ptr, _CODE[a.dtype], int(polar), _p(a), _p(b), a.numel(), k, nptr, mptr, cptr,
-                               int(bool(norm)), _p(out), st))
+    _call(lib.pb_zernike_sum, a, _CODE[a.dtype], int(polar), _p(a), _p(b), a.numel(), k, nptr, mptr, cptr,
+          int(bool(norm)), _p(out))
     return out
 
 
@@ -777,8 +710,7 @@ def balance_scale(a, b):
     a = a.contiguous()
     b = b.to(a.dtype).contiguous()
     s = torch.empty(1, dtype=torch.float64, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_balance_scale(h.ptr, _CODE[a.dtype], _p(a), _p(b), a.numel(), _p(s), st))
+    _call(lib.pb_balance_scale, a, _CODE[a.dtype], _p(a), _p(b), a.numel(), _p(s))
     return s
 
 
@@ -788,8 +720,7 @@ def pack_complex(re, im=None, im_scale=None):
         re = re.to(torch.float32)
     im = None if im is None else im.to(re.dtype).contiguous()
     out = torch.empty(re.shape, dtype=_CPLX_OF[re.dtype], device=re.device)
-    h, st = _ctx(re)
-    h.check(lib.pb_pack_complex(h.ptr, _CODE[re.dtype], _p(re), _p(im), _p(im_scale), re.numel(), _p(out), st))
+    _call(lib.pb_pack_complex, re, _CODE[re.dtype], _p(re), _p(im), _p(im_scale), re.numel(), _p(out))
     return out
 
 
@@ -798,8 +729,7 @@ def packed_spectrum_product(Z, scale=1.0, im_scale=None):
     Z = Z.contiguous()
     ny, nx = Z.shape
     out = torch.empty_like(Z)
-    h, st = _ctx(Z)
-    h.check(lib.pb_packed_spectrum_product(h.ptr, _CODE[Z.dtype], _p(Z), ny, nx, float(scale), _p(im_scale), _p(out), st))
+    _call(lib.pb_packed_spectrum_product, Z, _CODE[Z.dtype], _p(Z), ny, nx, float(scale), _p(im_scale), _p(out))
     return out
 
 
@@ -814,8 +744,7 @@ def bindown(a, fy, fx, mean):
     a = _real2d(a)
     ny, nx = a.shape
     out = torch.empty((ny // max(fy, 1), nx // max(fx, 1)), dtype=a.dtype, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_bindown(h.ptr, _CODE[a.dtype], _p(a), ny, nx, int(fy), int(fx), int(bool(mean)), _p(out), st))
+    _call(lib.pb_bindown, a, _CODE[a.dtype], _p(a), ny, nx, int(fy), int(fx), int(bool(mean)), _p(out))
     return out
 
 
@@ -823,8 +752,7 @@ def tile(a, fy, fx, scale):
     a = _real2d(a)
     ny, nx = a.shape
     out = torch.empty((ny * fy, nx * fx), dtype=a.dtype, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_tile(h.ptr, _CODE[a.dtype], _p(a), ny, nx, int(fy), int(fx), float(scale), _p(out), st))
+    _call(lib.pb_tile, a, _CODE[a.dtype], _p(a), ny, nx, int(fy), int(fx), float(scale), _p(out))
     return out
 
 
@@ -832,9 +760,8 @@ def separable_tf(kind, fx, fy, wx, wy):
     fx = _real2d(fx).reshape(-1)
     fy = _real2d(fy).to(fx.dtype).reshape(-1)
     out = torch.empty((fy.numel(), fx.numel()), dtype=fx.dtype, device=fx.device)
-    h, st = _ctx(fx)
-    h.check(lib.pb_separable_tf(h.ptr, _CODE[fx.dtype], int(kind), _p(fx), _p(fy), fy.numel(), fx.numel(), float(wx), float(wy),
-                                _p(out), st))
+    _call(lib.pb_separable_tf, fx, _CODE[fx.dtype], int(kind), _p(fx), _p(fy), fy.numel(), fx.numel(), float(wx),
+          float(wy), _p(out))
     return out
 
 
@@ -854,8 +781,7 @@ def spline_prefilter(a):
     a, cplx_in = _real_or_complex2d(a)
     ny, nx = a.shape
     out = torch.empty((ny, nx), dtype=torch.float64, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_spline_prefilter(h.ptr, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, _p(out), st))
+    _call(lib.pb_spline_prefilter, a, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, _p(out))
     return out
 
 
@@ -878,16 +804,10 @@ def warp(img, xc=None, yc=None, matrix=None, shape=None, scale=1.0, out=None):
         cd = torch.float64 if torch.float64 in (xc_t.dtype, yc_t.dtype) else torch.float32
         xc_t, yc_t = xc_t.to(cd).contiguous(), yc_t.to(cd).contiguous()
         oshape, cdt = tuple(xc_t.shape), _CODE[cd]
-    if out is None:
-        out = torch.empty(oshape, dtype=rd, device=img.device)
-    else:
-        _check_out(out, oshape, rd, img.device)
-        if not out.is_contiguous():
-            raise ValueError('`out` must be contiguous')
+    out = _out(out, oshape, rd, img.device)
     oy, ox = (oshape[0], int(np.prod(oshape[1:]))) if len(oshape) else (1, 1)
-    h, st = _ctx(img)
-    h.check(lib.pb_warp(h.ptr, _CODE[img.dtype], _p(img), int(cplx_in), ny, nx, _p(xc_t), _p(yc_t), cdt, mp, oy, ox,
-                        float(scale), _p(out), st))
+    _call(lib.pb_warp, img, _CODE[img.dtype], _p(img), int(cplx_in), ny, nx, _p(xc_t), _p(yc_t), cdt, mp, oy, ox,
+          float(scale), _p(out))
     return out
 
 
@@ -898,8 +818,7 @@ def dm_scatter(act, shape, lattice):
     ny, nx = shape
     y0, sy, x0, sx = lattice
     out = torch.empty((ny, nx), dtype=act.dtype, device=act.device)
-    h, st = _ctx(act)
-    h.check(lib.pb_dm_scatter(h.ptr, _CODE[act.dtype], _p(act), nay, nax, ny, nx, y0, sy, x0, sx, _p(out), st))
+    _call(lib.pb_dm_scatter, act, _CODE[act.dtype], _p(act), nay, nax, ny, nx, y0, sy, x0, sx, _p(out))
     return out
 
 
@@ -910,8 +829,7 @@ def dm_gather(a, nact, lattice):
     nay, nax = nact
     y0, sy, x0, sx = lattice
     out = torch.empty((nay, nax), dtype=_REAL_OF.get(a.dtype, a.dtype), device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_dm_gather(h.ptr, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, nay, nax, y0, sy, x0, sx, _p(out), st))
+    _call(lib.pb_dm_gather, a, _CODE[a.dtype], _p(a), int(cplx_in), ny, nx, nay, nax, y0, sy, x0, sx, _p(out))
     return out
 
 
@@ -945,9 +863,8 @@ def sdf(kind, x, y, params=(), verts=None, mask=False):
     if len(v) // 2 > SDF_MAX_VERTICES:
         raise ValueError(f'{len(v) // 2} polygon vertices or spider vanes: at most {SDF_MAX_VERTICES} are supported')
     v, vp = _darr(v)
-    h, st = _ctx(x)
-    h.check(lib.pb_sdf(h.ptr, _CODE[x.dtype], int(kind), _p(x), _p(y), separable, int(ny), int(nx), pp, len(p), vp,
-                       len(v) // 2, int(bool(mask)), _p(out), st))
+    _call(lib.pb_sdf, x, _CODE[x.dtype], int(kind), _p(x), _p(y), separable, int(ny), int(nx), pp, len(p), vp,
+          len(v) // 2, int(bool(mask)), _p(out))
     return out
 
 
@@ -958,8 +875,7 @@ def sdf_combine(op, a, b):
     if a.shape != b.shape:
         a, b = (t.contiguous() for t in torch.broadcast_tensors(a, b))
     out = torch.empty_like(a)
-    h, st = _ctx(a)
-    h.check(lib.pb_sdf_combine(h.ptr, _CODE[a.dtype], int(op), _p(a), _p(b), a.numel(), _p(out), st))
+    _call(lib.pb_sdf_combine, a, _CODE[a.dtype], int(op), _p(a), _p(b), a.numel(), _p(out))
     return out
 
 
@@ -970,9 +886,8 @@ def hex_segments(x, y, tiles, seg, geo, nverts, dx, total):
     ty, tx, ptr, lst = tiles
     cover, lx, ly = (torch.empty(total, dtype=x.dtype, device=x.device) for _ in range(3))
     amp = torch.empty((ny, nx), dtype=x.dtype, device=x.device)
-    h, st = _ctx(x)
-    h.check(lib.pb_hex_segments(h.ptr, _CODE[x.dtype], _p(x), _p(y), ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(geo),
-                                int(nverts), float(dx), _p(cover), _p(lx), _p(ly), _p(amp), st))
+    _call(lib.pb_hex_segments, x, _CODE[x.dtype], _p(x), _p(y), ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(geo),
+          int(nverts), float(dx), _p(cover), _p(lx), _p(ly), _p(amp))
     return cover, lx, ly, amp
 
 
@@ -981,9 +896,8 @@ def segment_compose(tiles, seg, masks, bases, nmodes, coefs, ncoef, out):
     contiguous (n, nmodes) float64 device tensor."""
     ny, nx = out.shape
     ty, tx, ptr, lst = tiles
-    h, st = _ctx(out)
-    h.check(lib.pb_segment_compose(h.ptr, _CODE[out.dtype], ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(masks), _p(bases),
-                                   int(nmodes), _p(coefs), int(nmodes), int(ncoef), _p(out), st))
+    _call(lib.pb_segment_compose, out, _CODE[out.dtype], ny, nx, ty, tx, _p(ptr), _p(lst), _p(seg), _p(masks),
+          _p(bases), int(nmodes), _p(coefs), int(nmodes), int(ncoef), _p(out))
     return out
 
 
@@ -993,24 +907,17 @@ def segment_compose_adjoint(seg, nseg, masks, bases, nmodes, opdbar, max_window)
     nchunk = max(1, -(-int(max_window) // capi.SEGMENT_CHUNK))
     partial = torch.empty(max(1, nseg * nchunk * nmodes), dtype=torch.float64, device=opdbar.device)
     out = torch.empty((nseg, nmodes), dtype=opdbar.dtype, device=opdbar.device)
-    h, st = _ctx(opdbar)
-    h.check(lib.pb_segment_compose_adjoint(h.ptr, _CODE[opdbar.dtype], ny, nx, int(nseg), _p(seg), _p(masks), _p(bases),
-                                           int(nmodes), _p(opdbar), nchunk, _p(partial), _p(out), st))
+    _call(lib.pb_segment_compose_adjoint, opdbar, _CODE[opdbar.dtype], ny, nx, int(nseg), _p(seg), _p(masks), _p(bases),
+          int(nmodes), _p(opdbar), nchunk, _p(partial), _p(out))
     return out
-
-
-_JONES_SRC = {torch.float32: capi.JONES_SRC_F32, torch.float64: capi.JONES_SRC_F64,
-              torch.complex64: capi.JONES_SRC_C64, torch.complex128: capi.JONES_SRC_C128}
 
 
 def jones_planar(src, cdtype, out=None):
     """A (rows, cols, 2, 2) device tensor of any strides, real or complex -> its 4 element planes (4, rows, cols) at
     `cdtype` (pb_jones_planar)."""
     rows, cols = src.shape[:2]
-    if out is None:
-        out = torch.empty((4, rows, cols), dtype=cdtype, device=src.device)
-    h, st = _ctx(src)
-    h.check(lib.pb_jones_planar(h.ptr, _CODE[cdtype], _p(src), _JONES_SRC[src.dtype], rows, cols, *src.stride(), _p(out), st))
+    out = _out(out, (4, rows, cols), cdtype, src.device)
+    _call(lib.pb_jones_planar, src, _CODE[cdtype], _p(src), _ELEM[src.dtype], rows, cols, *src.stride(), _p(out))
     return out
 
 
@@ -1020,25 +927,22 @@ def jones_product(mode, n, a, b, out, consts=None):
     (ak, at, ao), (bk, bt, bo) = a, b
     c = np.zeros(16) if consts is None else np.asarray(consts, dtype=np.complex128).view(np.float64)
     c, cp = _darr(c)
-    h, st = _ctx(out)
-    h.check(lib.pb_jones_product(h.ptr, _CODE[out.dtype], int(mode), int(n), int(ak), _p(at), int(ao), int(bk), _p(bt),
-                                 int(bo), cp, _p(out), st))
+    _call(lib.pb_jones_product, out, _CODE[out.dtype], int(mode), int(n), int(ak), _p(at), int(ao), int(bk), _p(bt),
+          int(bo), cp, _p(out))
     return out
 
 
 def jones_elements(kind, n, params, out, plane=None):
     """4 planes of one Jones constructor over n pixels (pb_jones_elements); plane: optional real device tensor."""
     p, pp = _darr(np.asarray(params, dtype=np.float64).reshape(-1))
-    ptype = _JONES_SRC[plane.dtype] if plane is not None else 0
-    h, st = _ctx(out)
-    h.check(lib.pb_jones_elements(h.ptr, _CODE[out.dtype], int(kind), int(n), _p(plane), ptype, pp, len(p), _p(out), st))
+    ptype = _ELEM[plane.dtype] if plane is not None else 0
+    _call(lib.pb_jones_elements, out, _CODE[out.dtype], int(kind), int(n), _p(plane), ptype, pp, len(p), _p(out))
     return out
 
 
 def jones_reduce(kind, n, a, out, b=None):
     """Mueller (16 real planes), Kronecker (16 complex planes) or Pauli (4 planes) of 4-plane operands (pb_jones_reduce)."""
-    h, st = _ctx(a)
-    h.check(lib.pb_jones_reduce(h.ptr, _CODE[a.dtype], int(kind), int(n), _p(a), _p(b), _p(out), st))
+    _call(lib.pb_jones_reduce, a, _CODE[a.dtype], int(kind), int(n), _p(a), _p(b), _p(out))
     return out
 
 
@@ -1047,15 +951,10 @@ def lp_modes(r, t, a, plan, out=None):
     (P, 6) host array of l, ld, U, W, rule, az rows."""
     r = r.contiguous()
     t = None if t is None else t.to(r.dtype).contiguous()
-    plan = np.ascontiguousarray(plan, dtype=np.float64).reshape(-1, 6)
+    plan, pp = _darr(np.asarray(plan, dtype=np.float64).reshape(-1, 6))
     P = plan.shape[0]
-    if out is None:
-        out = torch.empty((P, *r.shape), dtype=r.dtype, device=r.device)
-    else:
-        _check_out(out, (P, *r.shape), r.dtype, r.device)
-    pp = plan.ctypes.data_as(C.POINTER(C.c_double))
-    h, st = _ctx(r)
-    h.check(lib.pb_lp_modes(h.ptr, _CODE[r.dtype], _p(r), _p(t), r.numel(), float(a), P, pp, _p(out), st))
+    out = _out(out, (P, *r.shape), r.dtype, r.device, contiguous=False)
+    _call(lib.pb_lp_modes, r, _CODE[r.dtype], _p(r), _p(t), r.numel(), float(a), P, pp, _p(out))
     return out
 
 
@@ -1087,9 +986,8 @@ def overlap(E, modes, ip=None, ie=None, want_c=False):
     work = torch.empty(nchunk * (3 * P + 1), dtype=torch.float64, device=E.device)
     eta = torch.empty(P, dtype=rd, device=E.device)
     c = torch.empty((), dtype=rd, device=E.device) if want_c else None
-    h, st = _ctx(E)
-    h.check(lib.pb_overlap(h.ptr, _CODE[E.dtype], _p(E), n, P, _p(packed), ptrs, int(mc), _p(ip), _p(ie), _p(work),
-                           _p(eta), _p(c), st))
+    _call(lib.pb_overlap, E, _CODE[E.dtype], _p(E), n, P, _p(packed), ptrs, int(mc), _p(ip), _p(ie), _p(work), _p(eta),
+          _p(c))
     del keep
     return eta, c
 
@@ -1108,9 +1006,7 @@ def wfs_combine(a, alpha=1.0, b=None, beta=1.0, alpha_scale=None, beta_scale=Non
     sa = None if alpha_scale is None else alpha_scale.to(rd).contiguous()
     sb = None if beta_scale is None else beta_scale.to(rd).contiguous()
     out = torch.empty(a.shape, dtype=rd if real_out else a.dtype, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_wfs_combine(h.ptr, _CODE[a.dtype], a.numel(), _p(a), _p(b), kp, _p(sa), _p(sb), int(real_out),
-                               _p(out), st))
+    _call(lib.pb_wfs_combine, a, _CODE[a.dtype], a.numel(), _p(a), _p(b), kp, _p(sa), _p(sb), int(real_out), _p(out))
     return out
 
 
@@ -1123,14 +1019,8 @@ def grating(kind, x, params, shift=0.0, E=None):
             raise ValueError(f'shape mismatch {tuple(E.shape)} vs grid {tuple(x.shape)}')
     p, pp = _darr(params)
     out = torch.empty(x.shape, dtype=x.dtype if E is None else E.dtype, device=x.device)
-    h, st = _ctx(x)
-    h.check(lib.pb_grating(h.ptr, _CODE[x.dtype], int(kind), x.numel(), _p(x), float(shift), pp, len(p), _p(E),
-                           _p(out), st))
+    _call(lib.pb_grating, x, _CODE[x.dtype], int(kind), x.numel(), _p(x), float(shift), pp, len(p), _p(E), _p(out))
     return out
-
-
-_PSI_TYPE = {torch.float32: capi.PSI_F32, torch.float64: capi.PSI_F64, torch.uint16: capi.PSI_U16,
-             torch.int32: capi.PSI_I32, torch.int64: capi.PSI_I64}
 
 
 def psi(frames, s, c, num_dtype, phase_dtype, want_num=True, want_phase=True):
@@ -1146,7 +1036,7 @@ def psi(frames, s, c, num_dtype, phase_dtype, want_num=True, want_phase=True):
             if f.shape != f0.shape or f.dtype != f0.dtype or f.device != f0.device:
                 raise ValueError('every frame must have one shape, dtype and device')
         ptrs = (C.c_void_p * N)(*[f.data_ptr() for f in keep])
-    if f0.dtype not in _PSI_TYPE or f0.dtype == torch.int64:
+    if f0.dtype not in (torch.float32, torch.float64, torch.uint16, torch.int32):
         raise ValueError(f'frames of {f0.dtype} are not supported (float32, float64, uint16, int32)')
     shape, n = tuple(f0.shape), f0.numel()
     s, sp = _darr(s)
@@ -1156,15 +1046,12 @@ def psi(frames, s, c, num_dtype, phase_dtype, want_num=True, want_phase=True):
     num = torch.empty(shape, dtype=num_dtype, device=f0.device) if want_num else None
     den = torch.empty(shape, dtype=num_dtype, device=f0.device) if want_num else None
     phase = torch.empty(shape, dtype=phase_dtype, device=f0.device) if want_phase else None
-    h, st = _ctx(f0)
-    h.check(lib.pb_psi(h.ptr, _PSI_TYPE[f0.dtype], N, ptrs, _p(stack), n, n, sp, cp, _PSI_TYPE[num_dtype], _p(num),
-                       _p(den), _PSI_TYPE[phase_dtype], _p(phase), st))
+    _call(lib.pb_psi, f0, _ELEM[f0.dtype], N, ptrs, _p(stack), n, n, sp, cp, _ELEM[num_dtype], _p(num), _p(den),
+          _ELEM[phase_dtype], _p(phase))
     del keep
     return num, den, phase
 
 
-_SENSOR_TYPE = {torch.float32: capi.SENSOR_F32, torch.float64: capi.SENSOR_F64, torch.uint8: capi.SENSOR_U8,
-                torch.uint16: capi.SENSOR_U16, torch.uint32: capi.SENSOR_U32}
 _CODE_BYTES = {torch.uint8: 1, torch.uint16: 2, torch.uint32: 4}
 
 
@@ -1206,10 +1093,9 @@ def expose(aerial, prnu, dcnu, params, frames, key, code_dtype, lut=None):
     pp, pr, pc = views[0] or (None, 0, 0)
     dp, dr, dc = views[1] or (None, 0, 0)
     prm, prmp = _darr(params)
-    h, st = _ctx(aerial)
-    h.check(lib.pb_expose(h.ptr, _CODE[aerial.dtype], _p(aerial), n, nx, _p(pp), pr, pc, _p(dp), dr, dc, prmp,
-                          int(frames), int(key), _CODE_BYTES[code_dtype], _p(lut_t),
-                          0 if lut_t is None else lut_t.numel(), odt.itemsize, _p(out), _p(flags), st))
+    _call(lib.pb_expose, aerial, _CODE[aerial.dtype], _p(aerial), n, nx, _p(pp), pr, pc, _p(dp), dr, dc, prmp,
+          int(frames), int(key), _CODE_BYTES[code_dtype], _p(lut_t), 0 if lut_t is None else lut_t.numel(),
+          odt.itemsize, _p(out), _p(flags))
     return out, _flags_read(flags, 2 if lut_t is not None else 1)
 
 
@@ -1219,9 +1105,8 @@ def apply_lut(codes, lut, check):
     lut = lut.contiguous()
     out = torch.empty(codes.shape, dtype=lut.dtype, device=codes.device)
     flags = torch.zeros(2, dtype=torch.int32, device=codes.device) if check else None
-    h, st = _ctx(codes)
-    h.check(lib.pb_apply_lut(h.ptr, _CODE_BYTES[codes.dtype], _p(codes), codes.numel(), _p(lut), lut.numel(),
-                             lut.dtype.itemsize, int(bool(check)), _p(out), _p(flags), st))
+    _call(lib.pb_apply_lut, codes, _CODE_BYTES[codes.dtype], _p(codes), codes.numel(), _p(lut), lut.numel(),
+          lut.dtype.itemsize, int(bool(check)), _p(out), _p(flags))
     if check and codes.numel():
         f = _flags_read(flags, 2)
         if f[0] & 4:
@@ -1237,9 +1122,8 @@ def pixel(x, y, wx, wy):
     out = torch.empty(shape, dtype=torch.uint8, device=x.device)
     n = math.prod(shape)
     if n:
-        h, st = _ctx(x)
-        h.check(lib.pb_pixel(h.ptr, _CODE[x.dtype], _p(xv), xr, xc, _p(yv), yr, yc, n, shape[-1] if shape else 1,
-                             float(wx), float(wy), _p(out), st))
+        _call(lib.pb_pixel, x, _CODE[x.dtype], _p(xv), xr, xc, _p(yv), yr, yc, n, shape[-1] if shape else 1, float(wx),
+              float(wy), _p(out))
     return out.view(torch.bool)
 
 
@@ -1249,17 +1133,15 @@ def bayer_interleave(planes, half, out):
     M, N = out.shape
     ptrs = (C.c_void_p * 4)(*[None if p is None else p.data_ptr() for p in planes])
     lds = (C.c_longlong * 4)(*[0 if p is None else p.stride(0) for p in planes])
-    h, st = _ctx(out)
-    h.check(lib.pb_bayer_interleave(h.ptr, out.element_size(), ptrs, lds, int(half), M, N, _p(out), out.stride(0), st))
+    _call(lib.pb_bayer_interleave, out, out.element_size(), ptrs, lds, int(half), M, N, _p(out), out.stride(0))
     return out
 
 
 def demosaic_deinterlace(img, bggr, out_dtype):
     m, n = img.shape
     out = torch.empty((m // 2, n // 2, 3), dtype=out_dtype, device=img.device)
-    h, st = _ctx(img)
-    h.check(lib.pb_demosaic_deinterlace(h.ptr, _SENSOR_TYPE[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
-                                        _SENSOR_TYPE[out_dtype], _p(out), st))
+    _call(lib.pb_demosaic_deinterlace, img, _ELEM[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
+          _ELEM[out_dtype], _p(out))
     return out
 
 
@@ -1269,24 +1151,21 @@ def white_balance(a, kind, gains, sat=None):
     g, gp = _darr(gains)
     s, sp = (None, None) if sat is None else _darr(sat)
     work = None if sat is None else torch.empty(4 * capi.WB_MAX_BLOCKS + 1, dtype=torch.float64, device=a.device)
-    h, st = _ctx(a)
-    h.check(lib.pb_white_balance(h.ptr, _CODE[a.dtype], _p(a), a.numel(), a.shape[-1] if kind == 0 else 3, int(kind),
-                                 gp, sp, _p(work), st))
+    _call(lib.pb_white_balance, a, _CODE[a.dtype], _p(a), a.numel(), a.shape[-1] if kind == 0 else 3, int(kind), gp, sp,
+          _p(work))
     return a
 
 
 def demosaic_malvar(img, bggr, out_dtype):
     m, n = img.shape
     out = torch.empty((m, n, 3), dtype=out_dtype, device=img.device)
-    h, st = _ctx(img)
-    h.check(lib.pb_demosaic_malvar(h.ptr, _SENSOR_TYPE[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
-                                   _SENSOR_TYPE[out_dtype], _p(out), st))
+    _call(lib.pb_demosaic_malvar, img, _ELEM[img.dtype], _p(img), m, n, img.stride(0), int(bggr),
+          _ELEM[out_dtype], _p(out))
     return out
 
 
 def bayer_assemble(rp, g2p, bp, g1, out):
-    h, st = _ctx(g1)
-    h.check(lib.pb_bayer_assemble(h.ptr, _CODE[g1.dtype], _p(rp), _p(g2p), _p(bp), _p(g1), g1.numel(), _p(out), st))
+    _call(lib.pb_bayer_assemble, g1, _CODE[g1.dtype], _p(rp), _p(g2p), _p(bp), _p(g1), g1.numel(), _p(out))
     return out
 
 
@@ -1296,30 +1175,23 @@ def lenslet_screen(x, y, centres, cand, kind, params, two_efl, kphase, ncols, nr
     H, W = x.shape
     out = torch.empty((H, W), dtype=_CPLX_OF[x.dtype], device=x.device)
     prm, prmp = _darr(params)
-    h, st = _ctx(x)
-    h.check(lib.pb_lenslet_screen(h.ptr, _CODE[x.dtype], _p(x), _p(y), H, W, int(ncols), int(nrows), _p(centres),
-                                  _p(cand), int(kind), prmp, float(two_efl), float(kphase), _p(out), st))
+    _call(lib.pb_lenslet_screen, x, _CODE[x.dtype], _p(x), _p(y), H, W, int(ncols), int(nrows), _p(centres), _p(cand),
+          int(kind), prmp, float(two_efl), float(kphase), _p(out))
     return out
-
-
-_SH_TYPE = {torch.float32: capi.SH_F32, torch.float64: capi.SH_F64, torch.uint16: capi.SH_U16,
-            torch.int32: capi.SH_I32}
 
 
 def subaperture_centroids(frames, dtab, itab, ncols, nrows, threshold, scale=1.0):
     """(disp (F, 2, nrows, ncols) times scale, flux (F, nrows, ncols)) of an (F, H, W) stack in one launch
     (pb_subaperture_centroids); float64 for float64 frames, float32 otherwise."""
-    if frames.dtype not in _SH_TYPE:
+    if frames.dtype not in (torch.float32, torch.float64, torch.uint16, torch.int32):
         raise ValueError(f'frames of {frames.dtype} are not supported (float32, float64, uint16, int32)')
     frames = frames.contiguous()
     F, H, W = frames.shape
     odt = torch.float64 if frames.dtype == torch.float64 else torch.float32
     disp = torch.empty((F, 2, nrows, ncols), dtype=odt, device=frames.device)
     flux = torch.empty((F, nrows, ncols), dtype=odt, device=frames.device)
-    h, st = _ctx(frames)
-    h.check(lib.pb_subaperture_centroids(h.ptr, _SH_TYPE[frames.dtype], _p(frames), F, H, W, H * W, int(ncols),
-                                         int(nrows), _p(dtab), _p(itab), float(threshold), float(scale), _SH_TYPE[odt], _p(disp),
-                                         _p(flux), st))
+    _call(lib.pb_subaperture_centroids, frames, _ELEM[frames.dtype], _p(frames), F, H, W, H * W, int(ncols),
+          int(nrows), _p(dtab), _p(itab), float(threshold), float(scale), _ELEM[odt], _p(disp), _p(flux))
     return disp, flux
 
 
@@ -1335,9 +1207,8 @@ def sh_reconstruct(slopes, idx, ref, R, frame_shape):
     F = slopes.shape[0]
     K, M = R.shape
     out = torch.empty((F, K), dtype=slopes.dtype, device=slopes.device)
-    h, st = _ctx(slopes)
-    h.check(lib.pb_sh_reconstruct(h.ptr, _SH_TYPE[slopes.dtype], _p(slopes), F, math.prod(frame_shape), _p(idx),
-                                  _p(ref), _p(R), K, M, _p(out), st))
+    _call(lib.pb_sh_reconstruct, slopes, _ELEM[slopes.dtype], _p(slopes), F, math.prod(frame_shape), _p(idx),
+          _p(ref), _p(R), K, M, _p(out))
     return out
 
 
@@ -1355,9 +1226,8 @@ def qpoly_seq(family, kind, ns, ms, a, b=None):
         return (out0, out1) if pair else out0
     n, nptr = _iarr(ns)
     m, mptr = _iarr(ms) if ms is not None else (None, C.POINTER(C.c_int)())
-    h, st = _ctx(a)
-    h.check(lib.pb_qpoly_seq(h.ptr, _CODE[a.dtype], int(family), int(kind), _p(a), _p(b), a.numel(), k, nptr, mptr,
-                             _p(out0), _p(out1), st))
+    _call(lib.pb_qpoly_seq, a, _CODE[a.dtype], int(family), int(kind), _p(a), _p(b), a.numel(), k, nptr, mptr, _p(out0),
+          _p(out1))
     return (out0, out1) if pair else out0
 
 
@@ -1371,19 +1241,18 @@ def qpoly_sum(family, ns, ms, coefs, u, t=None, want_der=False):
     dr = torch.empty_like(u) if want_der else None
     dt = torch.empty_like(u) if want_der and family == capi.QPOLY_2D else None
     k = len(ns)
-    n, nptr = _iarr(ns if k else [0])
-    m, mptr = _iarr(ms if ms is not None and k else [0])
-    c, cptr = _darr(coefs if k else [0.0])
-    h, st = _ctx(u)
-    h.check(lib.pb_qpoly_sum(h.ptr, _CODE[u.dtype], int(family), _p(u), _p(t), u.numel(), k, nptr, mptr, cptr, _p(z),
-                             _p(dr), _p(dt), st))
+    n, nptr = _iarr(ns)
+    m, mptr = _iarr([] if ms is None else ms)      # read for 2D-Q only
+    c, cptr = _darr(coefs)
+    _call(lib.pb_qpoly_sum, u, _CODE[u.dtype], int(family), _p(u), _p(t), u.numel(), k, nptr, mptr, cptr, _p(z), _p(dr),
+          _p(dt))
     return z, dr, dt
 
 
 def qpoly_tables(family, m, nmax):
     """(nmax + 1, 7) fp64 recurrence tables from the host C++ the kernels are planned with (pb_qpoly_tables)."""
-    out = np.zeros((nmax + 1, 7), dtype=np.float64)
-    rc = lib.pb_qpoly_tables(int(family), int(m), int(nmax), out.ctypes.data_as(C.POINTER(C.c_double)))
+    out, op = _darr(np.zeros((nmax + 1, 7)))
+    rc = lib.pb_qpoly_tables(int(family), int(m), int(nmax), op)
     if rc != 0:
         raise ValueError(f'pb_qpoly_tables(family={family}, m={m}, nmax={nmax}) failed with status {rc}')
     return out
@@ -1398,9 +1267,8 @@ def poly_seq(family, kind, ns, x, alpha=0.0, beta=0.0):
     out = torch.empty(((2 if both else 1) * k,) + tuple(x.shape), dtype=x.dtype, device=x.device)
     if k:
         n, nptr = _iarr(ns)
-        h, st = _ctx(x)
-        h.check(lib.pb_poly_seq(h.ptr, _CODE[x.dtype], int(family), int(kind), float(alpha), float(beta), _p(x), x.numel(),
-                                k, nptr, _p(out), st))
+        _call(lib.pb_poly_seq, x, _CODE[x.dtype], int(family), int(kind), float(alpha), float(beta), _p(x), x.numel(),
+              k, nptr, _p(out))
     return (out[:k], out[k:]) if both else out
 
 
@@ -1412,11 +1280,10 @@ def jacobi_radial_sum(coefs, ns, alpha, beta, x, y, radius, want_der):
     dx = torch.empty_like(x) if want_der else None
     dy = torch.empty_like(x) if want_der else None
     k = len(ns)
-    n, nptr = _iarr(ns if k else [0])
-    c, cptr = _darr(coefs if k else [0.0])
-    h, st = _ctx(x)
-    h.check(lib.pb_jacobi_radial_sum(h.ptr, _CODE[x.dtype], float(alpha), float(beta), _p(x), _p(y), x.numel(), k, nptr,
-                                     cptr, float(radius), _p(z), _p(dx), _p(dy), st))
+    n, nptr = _iarr(ns)
+    c, cptr = _darr(coefs)
+    _call(lib.pb_jacobi_radial_sum, x, _CODE[x.dtype], float(alpha), float(beta), _p(x), _p(y), x.numel(), k, nptr,
+          cptr, float(radius), _p(z), _p(dx), _p(dy))
     return z, dx, dy
 
 
@@ -1426,11 +1293,10 @@ def jacobi_clenshaw(s, alpha, beta, x, j, table, out=None):
     x = x.contiguous()
     N = max(len(s), 2)
     shape = ((j + 1, N) + tuple(x.shape)) if table else tuple(x.shape)
-    out = _contiguous_out(out, shape, x)
-    c, cptr = _darr(s if len(s) else [0.0])
-    h, st = _ctx(x)
-    h.check(lib.pb_jacobi_clenshaw(h.ptr, _CODE[x.dtype], float(alpha), float(beta), _p(x), x.numel(), len(s), cptr,
-                                   int(j), int(bool(table)), _p(out), st))
+    out = _out(out, shape, x.dtype, x.device)
+    c, cptr = _darr(s)
+    _call(lib.pb_jacobi_clenshaw, x, _CODE[x.dtype], float(alpha), float(beta), _p(x), x.numel(), len(s), cptr, int(j),
+          int(bool(table)), _p(out))
     return out
 
 
@@ -1442,11 +1308,9 @@ def zernike_der(nms, a, b, norm, cartesian):
     out = torch.empty((k, 2) + tuple(a.shape), dtype=a.dtype, device=a.device)
     if k == 0:
         return out
-    n, nptr = _iarr([nm[0] for nm in nms])
-    m, mptr = _iarr([nm[1] for nm in nms])
-    h, st = _ctx(a)
-    h.check(lib.pb_zernike_der(h.ptr, _CODE[a.dtype], int(bool(cartesian)), _p(a), _p(b), a.numel(), k, nptr, mptr,
-                               int(bool(norm)), _p(out), st))
+    (n, nptr), (m, mptr) = _nm(nms)
+    _call(lib.pb_zernike_der, a, _CODE[a.dtype], int(bool(cartesian)), _p(a), _p(b), a.numel(), k, nptr, mptr,
+          int(bool(norm)), _p(out))
     return out
 
 
@@ -1456,12 +1320,10 @@ def zernike_sum_der_xy(coefs, nms, x, y, norm):
     y = y.to(x.dtype).contiguous()
     k = len(nms)
     out = torch.empty((3,) + tuple(x.shape), dtype=x.dtype, device=x.device)
-    n, nptr = _iarr([nm[0] for nm in nms] if k else [0])
-    m, mptr = _iarr([nm[1] for nm in nms] if k else [0])
-    c, cptr = _darr(coefs if k else [0.0])
-    h, st = _ctx(x)
-    h.check(lib.pb_zernike_sum_der_xy(h.ptr, _CODE[x.dtype], _p(x), _p(y), x.numel(), k, nptr, mptr, cptr,
-                                      int(bool(norm)), _p(out), st))
+    (n, nptr), (m, mptr) = _nm(nms)
+    c, cptr = _darr(coefs)
+    _call(lib.pb_zernike_sum_der_xy, x, _CODE[x.dtype], _p(x), _p(y), x.numel(), k, nptr, mptr, cptr, int(bool(norm)),
+          _p(out))
     return out
 
 
@@ -1477,9 +1339,8 @@ def xy_seq(ms, ns, kinds, x, y, shape, separable):
     m, mptr = _iarr(ms)
     n, nptr = _iarr(ns)
     kd, kptr = _iarr(kinds)
-    h, st = _ctx(x)
-    h.check(lib.pb_xy_seq(h.ptr, _CODE[x.dtype], _p(x), _p(y), math.prod(shape), int(shape[-1]) if separable else 1,
-                          int(bool(separable)), k, mptr, nptr, kptr, _p(out), st))
+    _call(lib.pb_xy_seq, x, _CODE[x.dtype], _p(x), _p(y), math.prod(shape), int(shape[-1]) if separable else 1,
+          int(bool(separable)), k, mptr, nptr, kptr, _p(out))
     return out
 
 
@@ -1491,13 +1352,12 @@ def tensor_sum(basis, coefs, ms, ns, x, y, shape, separable, want_der, x_norm=1.
     dx = torch.empty_like(z) if want_der else None
     dy = torch.empty_like(z) if want_der else None
     k = len(ms)
-    m, mptr = _iarr(ms if k else [0])
-    n, nptr = _iarr(ns if k else [0])
-    c, cptr = _darr(coefs if k else [0.0])
-    h, st = _ctx(x)
-    h.check(lib.pb_tensor_sum(h.ptr, _CODE[x.dtype], int(basis), _p(x), _p(y), math.prod(shape),
-                              int(shape[-1]) if separable else 1, int(bool(separable)), k, mptr, nptr, cptr,
-                              float(x_norm), float(y_norm), _p(z), _p(dx), _p(dy), st))
+    m, mptr = _iarr(ms)
+    n, nptr = _iarr(ns)
+    c, cptr = _darr(coefs)
+    _call(lib.pb_tensor_sum, x, _CODE[x.dtype], int(basis), _p(x), _p(y), math.prod(shape),
+          int(shape[-1]) if separable else 1, int(bool(separable)), k, mptr, nptr, cptr, float(x_norm), float(y_norm),
+          _p(z), _p(dx), _p(dy))
     return z, dx, dy
 
 

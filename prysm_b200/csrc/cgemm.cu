@@ -127,10 +127,9 @@ using namespace pb;
 
 extern "C" int pb_cgemm(pb_handle_t hh, int dtype, int opA, int opB, int m, int n, int k, double alpha, const void* A,
                         long long lda, const void* B, long long ldb, void* C, long long ldc, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (m < 1 || n < 1 || k < 1 || opA < 0 || opA > 3 || opB < 0 || opB > 3) return fail(h, PB_ERR_INVALID, "bad gemm arguments");
-    return cgemm_simt(h, dtype, opA, opB, m, n, k, alpha, A, lda, B, ldb, C, ldc, reinterpret_cast<cudaStream_t>(stream));
+    return cgemm_simt(h, dtype, opA, opB, m, n, k, alpha, A, lda, B, ldb, C, ldc, st);
 }
 
 extern "C" long long pb_mdft_work_elems(int my, int ny, int mx, int nx, int adjoint, int left_first) {
@@ -141,10 +140,8 @@ extern "C" long long pb_mdft_work_elems(int my, int ny, int mx, int nx, int adjo
 extern "C" int pb_mdft_apply(pb_handle_t hh, int dtype, const void* Ey, const void* Ex, int my, int ny, int mx, int nx,
                              const void* a, void* out, double norm, int adjoint, int left_first, void* work,
                              void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (my < 1 || ny < 1 || mx < 1 || nx < 1 || !Ey || !Ex || !a || !out || !work) return fail(h, PB_ERR_INVALID, "bad mdft arguments");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (!adjoint) {
         if (left_first) {  // (Ey @ a) @ Ex^T
             PB_TRY(cgemm_simt(h, dtype, 0, 0, my, nx, ny, 1.0, Ey, ny, a, nx, work, nx, st));

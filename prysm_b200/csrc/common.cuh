@@ -153,6 +153,34 @@ bool with_real(int dtype, F&& f) {
     return false;
 }
 
+// calls f with a value of the element type a pb_elem code names (float, double, float2, double2, uint8_t, uint16_t,
+// uint32_t, int32_t, int64_t); false for an unknown code.  An entry point that takes only some types skips the others
+// with `if constexpr` inside f, so that no kernel is instantiated for them, and reports them after the call.
+template <typename F>
+bool with_elem(int type, F&& f) {
+    switch (type) {
+        case PB_ELEM_F32: f(float{}); return true;
+        case PB_ELEM_F64: f(double{}); return true;
+        case PB_ELEM_C64: f(float2{}); return true;
+        case PB_ELEM_C128: f(double2{}); return true;
+        case PB_ELEM_U8: f(uint8_t{}); return true;
+        case PB_ELEM_U16: f(uint16_t{}); return true;
+        case PB_ELEM_U32: f(uint32_t{}); return true;
+        case PB_ELEM_I32: f(int32_t{}); return true;
+        case PB_ELEM_I64: f(int64_t{}); return true;
+        default: return false;
+    }
+}
+
+// bytes of one element of a pb_elem type; 0 for an unknown code
+inline size_t elem_size(int type) {
+    size_t s = 0;
+    with_elem(type, [&](auto t) { s = sizeof(t); });
+    return s;
+}
+
+template <typename T, typename... U> constexpr bool is_one_of = (std::is_same<T, U>::value || ...);
+
 // true the first time a kernel is seen on this handle: the caller then sets its opt-in attributes
 inline bool attr_needed(Handle* h, const void* fn) { return h->attr_done.insert(fn).second; }
 

@@ -188,8 +188,7 @@ extern "C" int pb_fft2(pb_handle_t hh, int dtype, const void* in, int in_kind, c
                        double kscale, int ny, int nx, long long in_ld, int ky, int kx, int dir, double scale,
                        int shift_in, int shift_out, void* out, int out_kind, double weight, int oy, int ox,
                        long long out_ld, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || ky < ny || kx < nx) return fail(h, PB_ERR_INVALID, "need 1 <= n <= k on both axes");
     if (oy < 1 || ox < 1 || oy > ky || ox > kx) return fail(h, PB_ERR_INVALID, "crop window must fit the transform");
     if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
@@ -198,7 +197,6 @@ extern "C" int pb_fft2(pb_handle_t hh, int dtype, const void* in, int in_kind, c
     if (in_ld < nx || out_ld < ox) return fail(h, PB_ERR_INVALID, "row pitch smaller than the row");
     Fft2Args a{dtype, in, in_kind, amp, amp_kind, kscale / (2.0 * M_PI), ny, nx, in_ld, ky, kx, dir, scale,
                shift_in, shift_out, out, out_kind, weight, oy, ox, out_ld};
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     int rc = try_tuned_fft2(h, a.dtype, a.in, a.in_kind, a.amp, a.amp_kind, a.kturns, a.ny, a.nx, a.in_ld, a.ky,
                             a.kx, a.dir, a.scale, a.shift_in, a.shift_out, a.out, a.out_kind, a.weight, a.oy, a.ox,
                             a.out_ld, st);
@@ -227,7 +225,7 @@ extern "C" int pb_fft2_batch(pb_handle_t hh, int dtype, const void* in, int in_k
                                   out_bs, st);
     if (rc != PB_ERR_UNSUPPORTED) return rc;
     // shapes outside the fused kernels: one field at a time through the generic passes
-    const size_t rsz = dtype == PB_C64 ? 4 : 8;
+    const size_t rsz = rsize(dtype);
     const size_t in_elt = in_kind == PB_IN_COMPLEX ? 2 * rsz : rsz;
     const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : rsz;
     const size_t out_elt = out_kind == PB_OUT_COMPLEX ? 2 * rsz : rsz;
@@ -243,11 +241,9 @@ extern "C" int pb_fft2_batch(pb_handle_t hh, int dtype, const void* in, int in_k
 
 extern "C" int pb_fft1(pb_handle_t hh, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int n,
                        int dir, double scale, void* out, long long out_ld, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || n < 1 || (axis != 0 && axis != 1)) return fail(h, PB_ERR_INVALID, "bad shape / axis");
     if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     AxisPass p;
     p.dtype = dtype; p.in = in; p.dir = dir; p.scale = scale; p.out = out;
     p.Llog = n; p.in_off = 0; p.rot_in = 0; p.n_out = n; p.crop_off = 0; p.rot_out = 0;
@@ -265,12 +261,10 @@ extern "C" int pb_axis_dft(pb_handle_t hh, int dtype, const void* in, int ny, in
                            int dir, double scale, const void* pre_e, int pre_e_conj, const void* pre_b, int pre_b_conj,
                            const void* post_e, int post_e_conj, const void* post_b, int post_b_conj, int out_off,
                            int n_out, void* out, long long out_ld, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || n < 1 || (axis != 0 && axis != 1)) return fail(h, PB_ERR_INVALID, "bad shape / axis");
     if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
     if (out_off < 0 || n_out < 1 || out_off + n_out > n) return fail(h, PB_ERR_INVALID, "output window outside the transform");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     AxisPass p;
     p.dtype = dtype; p.in = in; p.dir = dir; p.scale = scale; p.out = out;
     p.Llog = n; p.n_out = n_out; p.crop_off = out_off;
@@ -288,12 +282,10 @@ extern "C" int pb_axis_dft(pb_handle_t hh, int dtype, const void* in, int ny, in
 
 int pb::czt_axis_impl(Handle* h, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int K,
                          const void* pre_e, int pre_conj, const void* H, const void* post_e, int post_conj, int out_off,
-                         int n_out, double scale, int out_kind, double weight, void* out, long long out_ld, void* stream) {
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+                         int n_out, double scale, int out_kind, double weight, void* out, long long out_ld, cudaStream_t st) {
     if (ny < 1 || nx < 1 || K < 1 || (axis != 0 && axis != 1) || !H) return fail(h, PB_ERR_INVALID, "bad czt arguments");
     if (out_off < 0 || n_out < 1 || out_off + n_out > K) return fail(h, PB_ERR_INVALID, "output window outside the transform");
     if (!is_pow2(K)) return fail(h, PB_ERR_INVALID, "the Bluestein length K must be a power of two");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int nline = axis == 1 ? ny : nx, n_in = std::min(axis == 1 ? nx : ny, K);
     AxisPass f;  // fused: (in * pre) -> FFT_K -> * H -> IFFT_K -> window -> * post
     f.dtype = dtype; f.in = in; f.dir = -1; f.out = out; f.scale = scale / K;
@@ -327,9 +319,9 @@ int pb::czt_axis_impl(Handle* h, int dtype, const void* in, int ny, int nx, long
 extern "C" int pb_czt_axis(pb_handle_t hh, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int K,
                            const void* pre_e, int pre_conj, const void* H, const void* post_e, int post_conj, int out_off,
                            int n_out, double scale, void* out, long long out_ld, void* stream) {
-    PB_ENTER(hh);
+    PB_ENTER_REAL(hh);
     return czt_axis_impl(h, dtype, in, ny, nx, in_ld, axis, K, pre_e, pre_conj, H, post_e, post_conj, out_off, n_out, scale,
-                         PB_OUT_COMPLEX, 1.0, out, out_ld, stream);
+                         PB_OUT_COMPLEX, 1.0, out, out_ld, st);
 }
 
 extern "C" int pb_czt_axis_intensity(pb_handle_t hh, int dtype, const void* in, int ny, int nx, long long in_ld, int axis,
@@ -338,14 +330,15 @@ extern "C" int pb_czt_axis_intensity(pb_handle_t hh, int dtype, const void* in, 
                                      void* out, long long out_ld, void* stream) {
     PB_ENTER(hh);
     if (out_kind != PB_OUT_INTENSITY && out_kind != PB_OUT_ACCUMULATE) return fail(h, PB_ERR_INVALID, "out_kind must be intensity or accumulate");
+    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
     return czt_axis_impl(h, dtype, in, ny, nx, in_ld, axis, K, pre_e, pre_conj, H, post_e, post_conj, out_off, n_out, scale,
-                         out_kind, weight, out, out_ld, stream);
+                         out_kind, weight, out, out_ld, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// dtype is checked by the entry points
 static int angular_spectrum_impl(Handle* h, int dtype, const void* in, int ny, int nx, int ky, int kx, const void* ty,
                                  const void* tx, const void* tf, int conj_tf, const void* screen, int conj_screen, void* out,
                                  int oy, int ox, cudaStream_t st) {
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
     if (ny < 1 || nx < 1 || ky < ny || kx < nx || oy < 1 || ox < 1 || oy > ky || ox > kx)
         return fail(h, PB_ERR_INVALID, "bad shapes");
     if (!tf && (!ty || !tx)) return fail(h, PB_ERR_INVALID, "need tf or both ty and tx");
@@ -401,9 +394,8 @@ static int angular_spectrum_impl(Handle* h, int dtype, const void* in, int ny, i
 extern "C" int pb_angular_spectrum(pb_handle_t hh, int dtype, const void* in, int ny, int nx, int ky, int kx,
                                    const void* ty, const void* tx, const void* tf, int conj_tf, void* out, int oy,
                                    int ox, void* stream) {
-    PB_ENTER(hh);
-    return angular_spectrum_impl(h, dtype, in, ny, nx, ky, kx, ty, tx, tf, conj_tf, nullptr, 0, out, oy, ox,
-                                 reinterpret_cast<cudaStream_t>(stream));
+    PB_ENTER_REAL(hh);
+    return angular_spectrum_impl(h, dtype, in, ny, nx, ky, kx, ty, tx, tf, conj_tf, nullptr, 0, out, oy, ox, st);
 }
 
 extern "C" int pb_angular_spectrum_screen(pb_handle_t hh, int dtype, const void* in, const void* screen, int conj_screen,
@@ -411,6 +403,7 @@ extern "C" int pb_angular_spectrum_screen(pb_handle_t hh, int dtype, const void*
                                           int conj_tf, void* out, int oy, int ox, void* stream) {
     PB_ENTER(hh);
     if (!screen) return fail(h, PB_ERR_INVALID, "null screen");
+    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
     return angular_spectrum_impl(h, dtype, in, ny, nx, ky, kx, ty, tx, tf, conj_tf, screen, conj_screen, out, oy, ox,
                                  reinterpret_cast<cudaStream_t>(stream));
 }

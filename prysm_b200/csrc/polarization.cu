@@ -57,7 +57,7 @@ __device__ __forceinline__ void st_real(R* __restrict__ p, long long g, const do
 }
 
 __device__ __forceinline__ double ld_real(const void* p, int type, long long i) {
-    return type == PB_JONES_SRC_F32 ? (double)reinterpret_cast<const float*>(p)[i] : reinterpret_cast<const double*>(p)[i];
+    return type == PB_ELEM_F32 ? (double)reinterpret_cast<const float*>(p)[i] : reinterpret_cast<const double*>(p)[i];
 }
 
 template <typename R> __device__ __forceinline__ double ld_plain(const R* __restrict__ p, long long i) { return (double)p[i]; }
@@ -336,31 +336,22 @@ extern "C" int pb_jones_planar(pb_handle_t hh, int dtype, const void* src, int s
     const long long n = rows < 0 || cols < 0 ? -1 : rows * cols;
     PB_ENTER_REAL(hh);
     if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
-    if (src_type < PB_JONES_SRC_F32 || src_type > PB_JONES_SRC_C128) return fail(h, PB_ERR_INVALID, "bad Jones source type");
+    if (src_type < PB_ELEM_F32 || src_type > PB_ELEM_C128) return fail(h, PB_ERR_INVALID, "bad Jones source type");
     if (n == 0) return PB_OK;
     if (!src || !out) return fail(h, PB_ERR_INVALID, "null pointer");
     return jones_launch(h, dtype, pairs_ok(n, {out}), n, [&](auto r, auto v, long long groups) {
         using R = decltype(r);
         constexpr int V = decltype(v)::value;
-        cplx<R>* o = reinterpret_cast<cplx<R>*>(out);
         const int g = grid_for(groups, kThreads, h->sm_count);
-        switch (src_type) {
-            case PB_JONES_SRC_F32:
-                jones_planar_kernel<float, false, R, V><<<g, kThreads, 0, st>>>((const float*)src, cols, s_row, s_col, s_i, s_j,
-                                                                                 groups, n, o);
-                break;
-            case PB_JONES_SRC_F64:
-                jones_planar_kernel<double, false, R, V><<<g, kThreads, 0, st>>>((const double*)src, cols, s_row, s_col, s_i,
-                                                                                  s_j, groups, n, o);
-                break;
-            case PB_JONES_SRC_C64:
-                jones_planar_kernel<float, true, R, V><<<g, kThreads, 0, st>>>((const float*)src, cols, s_row, s_col, s_i, s_j,
-                                                                                groups, n, o);
-                break;
-            default:
-                jones_planar_kernel<double, true, R, V><<<g, kThreads, 0, st>>>((const double*)src, cols, s_row, s_col, s_i,
-                                                                                 s_j, groups, n, o);
-        }
+        with_elem(src_type, [&](auto t) {
+            using T = decltype(t);
+            if constexpr (is_one_of<T, float, double, float2, double2>) {
+                // a complex source is read as interleaved scalars
+                using S = std::conditional_t<is_one_of<T, float, float2>, float, double>;
+                jones_planar_kernel<S, is_one_of<T, float2, double2>, R, V><<<g, kThreads, 0, st>>>(
+                    (const S*)src, cols, s_row, s_col, s_i, s_j, groups, n, reinterpret_cast<cplx<R>*>(out));
+            }
+        });
     });
 }
 
@@ -396,7 +387,7 @@ extern "C" int pb_jones_elements(pb_handle_t hh, int dtype, int kind, long long 
     if (n < 0) return fail(h, PB_ERR_INVALID, "negative pixel count");
     static const int need[] = {8, 2, 2, 2, 3};
     if (kind < PB_JONES_FILL || kind > PB_JONES_VVR || nparams < need[kind] || nparams > 8 ||
-        (plane && plane_type != PB_JONES_SRC_F32 && plane_type != PB_JONES_SRC_F64) || (kind == PB_JONES_FILL && plane))
+        (plane && plane_type != PB_ELEM_F32 && plane_type != PB_ELEM_F64) || (kind == PB_JONES_FILL && plane))
         return fail(h, PB_ERR_INVALID, "bad Jones element arguments");
     if (n == 0) return PB_OK;
     if (!out || !params_host || (kind == PB_JONES_VVR && !plane)) return fail(h, PB_ERR_INVALID, "null pointer");

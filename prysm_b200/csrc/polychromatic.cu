@@ -35,14 +35,13 @@ extern "C" long long pb_polychromatic_czt_work_bytes(int dtype, int n, int m, in
 
 extern "C" int pb_polychromatic_czt(pb_handle_t hh, int dtype, const void* amp, int amp_kind, const void* opd, int n, int m,
                                     int K, int n_units, const double* units, void* work, void* plane, void* stream) {
-    PB_ENTER(hh);
-    if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
+    PB_ENTER_REAL(hh);
     if (n < 1 || m < 1 || K < n + m - 1 || !is_pow2(K) || n_units < 0 || !opd || !work || !plane || (n_units > 0 && !units))
         return fail(h, PB_ERR_INVALID, "bad polychromatic czt arguments");
     if ((uintptr_t)work & 255) return fail(h, PB_ERR_INVALID, "work must be 256-byte aligned");
     if (n_units == 0) return PB_OK;
     PB_TRY(ensure_side(h));
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream), sd = h->side;
+    cudaStream_t sd = h->side;
     cudaEvent_t ev_fork = h->side_ev[0];
     cudaEvent_t ev_plan[2] = {h->side_ev[1], h->side_ev[2]}, ev_used[2] = {h->side_ev[3], h->side_ev[4]};
     const size_t cs = csize(dtype);
@@ -77,9 +76,9 @@ extern "C" int pb_polychromatic_czt(pb_handle_t hh, int dtype, const void* amp, 
         PB_TRY(pb_phase_screen(hh, dtype, amp, amp_kind, opd, u[0], count, field, stream));
         PB_CUDA(h, cudaStreamWaitEvent(st, ev_plan[j], 0));   // join: every plan is waited for before the call returns
         PB_TRY(czt_axis_impl(h, dtype, field, n, n, n, 1, K, b[j], 0, H[j], post[j], 0, n - 1, m, 1.0, PB_OUT_COMPLEX, 1.0,
-                             mid, m, stream));
+                             mid, m, st));
         PB_TRY(czt_axis_impl(h, dtype, mid, n, m, m, 0, K, b[j], 0, H[j], post[j], 0, n - 1, m, u[6], PB_OUT_ACCUMULATE, u[7],
-                             plane, m, stream));
+                             plane, m, st));
         PB_CUDA(h, cudaEventRecord(ev_used[j], st));
     }
     return PB_OK;

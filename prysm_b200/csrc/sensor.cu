@@ -426,18 +426,6 @@ bool with_bytes(int bytes, F&& f) {
     }
 }
 
-template <typename F>
-bool with_sensor_type(int type, F&& f) {
-    switch (type) {
-        case PB_SENSOR_F32: f(float{}); return true;
-        case PB_SENSOR_F64: f(double{}); return true;
-        case PB_SENSOR_U8: f(uint8_t{}); return true;
-        case PB_SENSOR_U16: f(uint16_t{}); return true;
-        case PB_SENSOR_U32: f(uint32_t{}); return true;
-        default: return false;
-    }
-}
-
 }  // namespace
 
 extern "C" int pb_expose(pb_handle_t hh, int dtype, const void* aerial, long long n, long long nx, const void* prnu,
@@ -556,11 +544,11 @@ extern "C" int pb_demosaic_deinterlace(pb_handle_t hh, int in_type, const void* 
     const int g = grid_for(m2 * n2, kSensorThreads, h->sm_count);
     const int r_site = bggr ? 3 : 0, b_site = bggr ? 0 : 3;
     bool ok = false;
-    with_sensor_type(in_type, [&](auto i) {
+    with_elem(in_type, [&](auto i) {
         using In = decltype(i);
-        with_sensor_type(out_type, [&](auto o) {
+        with_elem(out_type, [&](auto o) {
             using Out = decltype(o);
-            if constexpr (std::is_floating_point<Out>::value) {
+            if constexpr (is_one_of<In, float, double, uint8_t, uint16_t, uint32_t> && std::is_floating_point<Out>::value) {
                 deinterlace_kernel<In, Out><<<g, kSensorThreads, 0, st>>>((const In*)img, m2, n2, ld, r_site, b_site, (Out*)out);
                 ok = true;
             }
@@ -610,14 +598,14 @@ extern "C" int pb_demosaic_malvar(pb_handle_t hh, int in_type, const void* img, 
     const dim3 grid((unsigned)((n + kMalvarTX - 1) / kMalvarTX), (unsigned)((m + kMalvarTY - 1) / kMalvarTY));
     const dim3 block(kMalvarTX, kMalvarRows);
     bool ok = false;
-    with_sensor_type(in_type, [&](auto i) {
+    with_elem(in_type, [&](auto i) {
         using In = decltype(i);
-        if constexpr (!std::is_same<In, uint32_t>::value) {
+        if constexpr (is_one_of<In, float, double, uint8_t, uint16_t>) {
             using S = typename std::conditional<std::is_same<In, double>::value, double, float>::type;
-            if (out_type == PB_SENSOR_F32 && !std::is_same<In, double>::value) {
+            if (out_type == PB_ELEM_F32 && !std::is_same<In, double>::value) {
                 malvar_kernel<In, S, float><<<grid, block, 0, st>>>((const In*)img, m, n, ld, bggr, (float*)out);
                 ok = true;
-            } else if (out_type == PB_SENSOR_F64) {
+            } else if (out_type == PB_ELEM_F64) {
                 malvar_kernel<In, S, double><<<grid, block, 0, st>>>((const In*)img, m, n, ld, bggr, (double*)out);
                 ok = true;
             }

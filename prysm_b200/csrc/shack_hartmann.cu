@@ -269,39 +269,36 @@ extern "C" int pb_subaperture_centroids(pb_handle_t hh, int frame_type, const vo
                                         void* flux, void* stream) {
     PB_ENTER(hh);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (frame_type < PB_SH_F32 || frame_type > PB_SH_I32 || nframes < 0 || H < 0 || W < 0 || ncols < 0 || nrows < 0 ||
-        frame_stride < (long long)H * W || !std::isfinite(threshold) || !std::isfinite(scale))
+    const bool type_ok = frame_type == PB_ELEM_F32 || frame_type == PB_ELEM_F64 || frame_type == PB_ELEM_U16 ||
+                         frame_type == PB_ELEM_I32;
+    if (!type_ok || nframes < 0 || H < 0 || W < 0 || ncols < 0 || nrows < 0 || frame_stride < (long long)H * W ||
+        !std::isfinite(threshold) || !std::isfinite(scale))
         return fail(h, PB_ERR_INVALID, "bad centroid arguments");
-    if (out_type != (frame_type == PB_SH_F64 ? PB_SH_F64 : PB_SH_F32))
+    if (out_type != (frame_type == PB_ELEM_F64 ? PB_ELEM_F64 : PB_ELEM_F32))
         return fail(h, PB_ERR_INVALID, "centroids are float64 for float64 frames and float32 otherwise");
     if (nframes == 0 || ncols == 0 || nrows == 0) return PB_OK;
     if (nrows > 65535) return fail(h, PB_ERR_UNSUPPORTED, "more than 65535 lenslet rows");
     if (nframes > 65535) return fail(h, PB_ERR_UNSUPPORTED, "more than 65535 frames in one call");
     if (!frames || !dtab || !itab || !disp || !flux) return fail(h, PB_ERR_INVALID, "null pointer");
-    static const size_t fsz[] = {4, 8, 2, 4};
-    const size_t vbytes = fsz[frame_type] * kCentroidVec;
+    const size_t fsz = elem_size(frame_type), vbytes = fsz * kCentroidVec;
     auto smem_for = [&](int v) { return (5 * (size_t)ncols + 3 * (size_t)kThreads * v) * sizeof(double); };
     const bool vec = W % kCentroidVec == 0 && reinterpret_cast<uintptr_t>(frames) % vbytes == 0 &&
-                     (frame_stride * fsz[frame_type]) % vbytes == 0 && smem_for(kCentroidVec) <= kCentroidSmemMax;
+                     (frame_stride * fsz) % vbytes == 0 && smem_for(kCentroidVec) <= kCentroidSmemMax;
     const size_t smem = smem_for(vec ? kCentroidVec : 1);
     if (smem > kCentroidSmemMax) return fail(h, PB_ERR_UNSUPPORTED, "too many lenslet columns");
     const dim3 grid(nrows, nframes);
-    auto go = [&](auto t, auto o) {
+    with_elem(frame_type, [&](auto t) {
         using T = decltype(t);
-        using O = decltype(o);
-        if (vec)
-            centroid_kernel<T, O, kCentroidVec><<<grid, kThreads, smem, st>>>(
-                (const T*)frames, H, W, frame_stride, ncols, nrows, dtab, itab, threshold, scale, (O*)disp, (O*)flux);
-        else
-            centroid_kernel<T, O, 1><<<grid, kThreads, smem, st>>>(
-                (const T*)frames, H, W, frame_stride, ncols, nrows, dtab, itab, threshold, scale, (O*)disp, (O*)flux);
-    };
-    switch (frame_type) {
-        case PB_SH_F32: go(float(), float()); break;
-        case PB_SH_F64: go(double(), double()); break;
-        case PB_SH_U16: go((unsigned short)0, float()); break;
-        default: go(int(), float());
-    }
+        if constexpr (is_one_of<T, float, double, uint16_t, int32_t>) {
+            using O = std::conditional_t<std::is_same<T, double>::value, double, float>;
+            if (vec)
+                centroid_kernel<T, O, kCentroidVec><<<grid, kThreads, smem, st>>>(
+                    (const T*)frames, H, W, frame_stride, ncols, nrows, dtab, itab, threshold, scale, (O*)disp, (O*)flux);
+            else
+                centroid_kernel<T, O, 1><<<grid, kThreads, smem, st>>>(
+                    (const T*)frames, H, W, frame_stride, ncols, nrows, dtab, itab, threshold, scale, (O*)disp, (O*)flux);
+        }
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
@@ -311,18 +308,17 @@ extern "C" int pb_sh_reconstruct(pb_handle_t hh, int dtype, const void* slopes, 
                                  void* stream) {
     PB_ENTER(hh);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (dtype != PB_SH_F32 && dtype != PB_SH_F64) return fail(h, PB_ERR_INVALID, "slopes must be float32 or float64");
+    if (dtype != PB_ELEM_F32 && dtype != PB_ELEM_F64) return fail(h, PB_ERR_INVALID, "slopes must be float32 or float64");
     if (nframes < 0 || K < 0 || M < 0 || frame_stride < 0) return fail(h, PB_ERR_INVALID, "bad reconstruct sizes");
     if (nframes == 0 || K == 0) return PB_OK;
     if (nframes > 65535) return fail(h, PB_ERR_UNSUPPORTED, "more than 65535 frames in one call");
     if (!slopes || !out || (M > 0 && (!idx || !R))) return fail(h, PB_ERR_INVALID, "null pointer");
     const dim3 grid(K, nframes);
-    if (dtype == PB_SH_F32)
-        reconstruct_kernel<float><<<grid, kThreads, 0, st>>>((const float*)slopes, frame_stride, idx, ref, R, K, M,
-                                                             (float*)out);
-    else
-        reconstruct_kernel<double><<<grid, kThreads, 0, st>>>((const double*)slopes, frame_stride, idx, ref, R, K, M,
-                                                              (double*)out);
+    with_elem(dtype, [&](auto t) {
+        using T = decltype(t);
+        if constexpr (std::is_floating_point<T>::value)
+            reconstruct_kernel<T><<<grid, kThreads, 0, st>>>((const T*)slopes, frame_stride, idx, ref, R, K, M, (T*)out);
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

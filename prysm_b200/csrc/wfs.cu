@@ -454,31 +454,30 @@ extern "C" int pb_psi(pb_handle_t hh, int frame_type, int nframes, const void* c
                       void* num, void* den, int phase_type, void* phase, void* stream) {
     PB_ENTER(hh);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (frame_type < PB_PSI_F32 || frame_type > PB_PSI_I32 || nframes < 1 || nframes > kPsiMax || n < 0)
+    const bool int_frames = frame_type == PB_ELEM_U16 || frame_type == PB_ELEM_I32;
+    if ((frame_type != PB_ELEM_F32 && frame_type != PB_ELEM_F64 && !int_frames) || nframes < 1 || nframes > kPsiMax || n < 0)
         return fail(h, PB_ERR_INVALID, "bad PSI arguments");
-    const bool int_frames = frame_type == PB_PSI_U16 || frame_type == PB_PSI_I32;
     // output types follow numpy: float frames keep their type; integer frames give int64 (integer weights) or
     // float64 sums and a float64 phase
-    const bool types_ok = int_frames ? ((num_type == PB_PSI_I64 || num_type == PB_PSI_F64) && phase_type == PB_PSI_F64)
+    const bool types_ok = int_frames ? ((num_type == PB_ELEM_I64 || num_type == PB_ELEM_F64) && phase_type == PB_ELEM_F64)
                                      : (num_type == frame_type && phase_type == frame_type);
     if (!types_ok) return fail(h, PB_ERR_INVALID, "PSI output types do not follow the frame type");
     if (n == 0) return PB_OK;
     if (!s_host || !c_host || (!frames_host && !stack) || (!num && !den && !phase))
         return fail(h, PB_ERR_INVALID, "null pointer");
-    static const size_t fsz[] = {4, 8, 2, 4};
+    const size_t fsz = elem_size(frame_type);
     PsiPlan plan{};
     bool vec = true;
     for (int k = 0; k < nframes; ++k) {
         plan.s[k] = s_host[k];
         plan.c[k] = c_host[k];
-        plan.f[k] = frames_host ? frames_host[k] : static_cast<const char*>(stack) + (size_t)k * frame_stride * fsz[frame_type];
+        plan.f[k] = frames_host ? frames_host[k] : static_cast<const char*>(stack) + (size_t)k * frame_stride * fsz;
         if (!plan.f[k]) return fail(h, PB_ERR_INVALID, "null frame pointer");
         vec = vec && aligned16(plan.f[k]);
-        if (num_type == PB_PSI_I64 && (plan.s[k] != rint(plan.s[k]) || plan.c[k] != rint(plan.c[k])))
+        if (num_type == PB_ELEM_I64 && (plan.s[k] != rint(plan.s[k]) || plan.c[k] != rint(plan.c[k])))
             return fail(h, PB_ERR_INVALID, "int64 PSI sums need integer weights");
     }
-    const int vw = (int)(16 / fsz[frame_type]);
-    vec = vec && n % vw == 0 && aligned16(num) && aligned16(den) && aligned16(phase);
+    vec = vec && n % (long long)(16 / fsz) == 0 && aligned16(num) && aligned16(den) && aligned16(phase);
     auto go = [&](auto t, auto v, auto acc, auto nt, auto pt) {
         using T = decltype(t);
         constexpr int V = decltype(v)::value;
@@ -488,24 +487,22 @@ extern "C" int pb_psi(pb_handle_t hh, int frame_type, int nframes, const void* c
         psi_kernel<T, V, decltype(acc), NT, PT><<<grid_for(groups, kThreads, h->sm_count), kThreads, 0, st>>>(
             nframes, groups, plan, (NT*)num, (NT*)den, (PT*)phase);
     };
-    using one = std::integral_constant<int, 1>;
     auto dispatch = [&](auto t, auto vv) {
         using T = decltype(t);
         if constexpr (std::is_floating_point<T>::value) {
             go(t, vv, double(), T(), T());
         } else {
-            if (num_type == PB_PSI_I64) go(t, vv, (long long)0, (long long)0, double());
+            if (num_type == PB_ELEM_I64) go(t, vv, (long long)0, (long long)0, double());
             else go(t, vv, double(), double(), double());
         }
     };
-    switch (frame_type) {
-        case PB_PSI_F32: vec ? dispatch(float(), std::integral_constant<int, 4>()) : dispatch(float(), one()); break;
-        case PB_PSI_F64: vec ? dispatch(double(), std::integral_constant<int, 2>()) : dispatch(double(), one()); break;
-        case PB_PSI_U16:
-            vec ? dispatch((unsigned short)0, std::integral_constant<int, 8>()) : dispatch((unsigned short)0, one());
-            break;
-        default: vec ? dispatch(int(), std::integral_constant<int, 4>()) : dispatch(int(), one());
-    }
+    with_elem(frame_type, [&](auto t) {
+        using T = decltype(t);
+        if constexpr (is_one_of<T, float, double, uint16_t, int32_t>) {
+            if (vec) dispatch(t, std::integral_constant<int, 16 / sizeof(T)>());
+            else dispatch(t, std::integral_constant<int, 1>());
+        }
+    });
     PB_LAUNCH_CHECK(h);
     return PB_OK;
 }

@@ -9,10 +9,36 @@ import pytest
 from conftest import ROOT
 
 
-def header_symbols():
+def _header_code():
     src = open(os.path.join(ROOT, 'include', 'prysm_b200.h')).read()
-    src = re.sub(r'/\*.*?\*/', '', src, flags=re.S)
-    return sorted(set(re.findall(r'\b(pb_[a-z0-9_]+)\s*\(', src)))
+    return re.sub(r'/\*.*?\*/', '', src, flags=re.S)
+
+
+def header_symbols():
+    return sorted(set(re.findall(r'\b(pb_[a-z0-9_]+)\s*\(', _header_code())))
+
+
+def header_prototypes():
+    """name -> [restype, parameter types...] of every prototype in the header, as C type text"""
+    protos = {}
+    for ret, name, params in re.findall(r'^([A-Za-z_][\w ]*?\**)\s*(pb_[a-z0-9_]+)\s*\(([^)]*)\)\s*;', _header_code(),
+                                        flags=re.M):
+        params = [' '.join(p.split()) for p in params.split(',')] if params.strip() not in ('', 'void') else []
+        # drop the parameter name, keep its type (every parameter in the header is named)
+        protos[name] = [ret.strip()] + [re.sub(r'\b\w+$', '', p).strip() for p in params]
+    return protos
+
+
+def _ctype_of(c_type):
+    if '*' in c_type or c_type == 'pb_handle_t':
+        return 'pointer'
+    return {'int': ctypes.c_int, 'long long': ctypes.c_longlong, 'double': ctypes.c_double}[c_type]
+
+
+def _ctypes_kind(t):
+    if t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer):
+        return 'pointer'
+    return t
 
 
 def test_library_exports_every_header_symbol():
@@ -23,6 +49,15 @@ def test_library_exports_every_header_symbol():
     for n in names:
         assert hasattr(lib, n), f'{n} declared in the header but not exported'
     assert sorted(_capi.SIGNATURES) == names, 'ctypes SIGNATURES and the header diverge'
+    # an int / long long slip at one position passes garbage in the upper half of a register: compare every position
+    protos = header_prototypes()
+    assert sorted(protos) == names
+    for name, (res, args) in _capi.SIGNATURES.items():
+        want = [_ctype_of(t) for t in protos[name]]
+        got = [_ctypes_kind(t) for t in [res] + list(args)]
+        assert len(got) == len(want), f'{name}: {len(args)} ctypes arguments, the header has {len(want) - 1}'
+        for i, (g, w) in enumerate(zip(got, want)):
+            assert g == w, f'{name}: ' + ('return type' if i == 0 else f'argument {i - 1}') + f' is {g}, the header says {w}'
 
 
 def test_version_and_null_handle_are_safe():
@@ -64,6 +99,8 @@ def test_python_constants_match_the_header_enums():
              'PB_OUT_ACCUMULATE': _capi.OUT_ACCUMULATE, 'PB_MASK_REAL': _capi.MASK_REAL, 'PB_MASK_COMPLEX': _capi.MASK_COMPLEX,
              'PB_MASK_CONJ': _capi.MASK_CONJ, 'PB_MASK_ONE_MINUS': _capi.MASK_ONE_MINUS, 'PB_MASK_REAL_OUT': _capi.MASK_REAL_OUT,
              'PB_MASK_ACCUMULATE': _capi.MASK_ACCUMULATE}
+    for e in ('F32', 'F64', 'C64', 'C128', 'U8', 'U16', 'U32', 'I32', 'I64'):
+        pairs['PB_ELEM_' + e] = getattr(_capi, 'ELEM_' + e)
     for name, val in pairs.items():
         assert enums[name] == val, name
     assert enums['PB_OK'] == 0 and enums['PB_ERR_INVALID'] == -1      # Handle.check maps -1 to ValueError
