@@ -2,8 +2,9 @@
 
     python oracle/install_reference.py [SRC]        (SRC: a prysm source checkout; default $PRYSM_REFERENCE)
 
-oracle/_ref is git-ignored.  The drop-in tests (tests/test_gpu_dropin.py, tests/test_backend_binding.py) and
-`bench.py --impl reference` import the reference from there; they skip or fail loudly where it was not installed.
+oracle/_ref is git-ignored.  The tests and tools/bench_*.py import the reference from there through
+oracle/reference.py (which a PRYSM_REFERENCE checkout overrides), and `bench.py --impl reference` imports it directly;
+they skip or fail loudly where it was not installed.
 The package is copied file for file and checked to be identical to its source: nothing in it is changed."""
 import filecmp
 import os

@@ -21,6 +21,7 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
         sys.path.insert(0, _p)
 
 import prysm_oracle as O  # noqa: E402
+import reference  # noqa: E402
 
 
 def warp(img, xnew, ynew):
@@ -220,22 +221,19 @@ def run_case(DMcls, name, shape, kw, to_numpy=np.asarray):
 
 def main():
     """Write tests/golden/dm.npz from the unmodified reference at fp64."""
-    ref = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
-    from prysm.conf import config
-    from prysm.x.dm import DM as RefDM
-    config.precision = 64
-    sys.path.insert(0, os.path.join(ROOT, 'oracle'))
-    from make_golden import save
-    g = {}
-    for name, (shape, kw) in SMALL_CASES.items():
-        for k, v in run_case(RefDM, name, shape, kw).items():
-            g[f'{name}_{k}'] = v
-    for name, (shape, kw) in LARGE_CASES.items():
-        res = run_case(RefDM, name, shape, kw)
-        for k, v in res.items():
-            g.update(summarize(f'{name}_{k}', v) if v.size > 4096 else {f'{name}_{k}': v})
+    with reference.loaded():
+        from prysm.conf import config
+        from prysm.x.dm import DM as RefDM
+        config.precision = 64
+        from make_golden import save
+        g = {}
+        for name, (shape, kw) in SMALL_CASES.items():
+            for k, v in run_case(RefDM, name, shape, kw).items():
+                g[f'{name}_{k}'] = v
+        for name, (shape, kw) in LARGE_CASES.items():
+            res = run_case(RefDM, name, shape, kw)
+            for k, v in res.items():
+                g.update(summarize(f'{name}_{k}', v) if v.size > 4096 else {f'{name}_{k}': v})
     save('dm.npz', g)
 
 

@@ -20,6 +20,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 SHAPE = (61, 80)           # (rows, cols): non-square, odd rows
 PROP_N = 256               # the reference's test_make_propagation_polarized (tests/x/test_polarization.py:129-183)
 VVC_N = 128                # the vector vortex coronagraph
@@ -178,11 +180,7 @@ def run(pol, prop, g, to_numpy=np.asarray, asarray=np.asarray):
     return out
 
 
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
     from prysm.conf import config
     from prysm.x import polarization as pol
     from prysm import propagation as prop
@@ -191,17 +189,19 @@ def reference_modules(ref=None):
 
 
 def reference_outputs():
-    pol, prop = reference_modules()
-    g = inputs()
-    out = run(pol, prop, g)
-    out['diattenuator_plane'] = diattenuator_plane(pol, g['alpha'])
-    return out
+    with reference.loaded():
+        pol, prop = reference_modules()
+        g = inputs()
+        out = run(pol, prop, g)
+        out['diattenuator_plane'] = diattenuator_plane(pol, g['alpha'])
+        return out
 
 
 def main():
     """Write tests/golden/polarization*.npz from the unmodified reference."""
-    from make_golden import save
-    save('polarization.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('polarization.npz', reference_outputs())
 
 
 if __name__ == '__main__':

@@ -26,6 +26,7 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle'), HERE):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
 from qpoly_oracle import grids  # noqa: E402  (the same two grids)
 
 NS = [0, 1, 2, 3, 5, 8, 13, 21, 30, 34]      # ascending: the reference's 1-D sequences assume it
@@ -91,11 +92,7 @@ def xypsf_inputs():
     return amp, u, w, dx
 
 
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
     from prysm.conf import config
     from prysm import polynomials
     from prysm.propagation import Wavefront
@@ -149,16 +146,17 @@ def run(m):
 
 def reference_outputs():
     import warnings
-    m = reference_modules()
-    with warnings.catch_warnings():
+    with reference.loaded(), warnings.catch_warnings():
+        m = reference_modules()
         warnings.simplefilter('ignore')
         return run(m)
 
 
 def main():
     """Write tests/golden/polynomials*.npz from the unmodified reference."""
-    from make_golden import save
-    save('polynomials.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('polynomials.npz', reference_outputs())
 
 
 if __name__ == '__main__':

@@ -23,6 +23,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 NMAX = 64                   # the engine's order limit (PB_QPOLY_NMAX)
 TAB_M = 20
 NS = [0, 1, 2, 3, 5, 8, 12]  # ascending: the reference's 1-D sequences assume it
@@ -68,11 +70,7 @@ def psf_inputs():
     return amp, u, t, dx
 
 
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
     from prysm.conf import config
     from prysm.polynomials import qpoly
     from prysm.propagation import Wavefront
@@ -126,16 +124,17 @@ def run(m):
 
 def reference_outputs():
     import warnings
-    m = reference_modules()
-    with warnings.catch_warnings():
+    with reference.loaded(), warnings.catch_warnings():
+        m = reference_modules()
         warnings.simplefilter('ignore')
         return run(m)
 
 
 def main():
     """Write tests/golden/qpoly*.npz from the unmodified reference."""
-    from make_golden import save
-    save('qpoly.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('qpoly.npz', reference_outputs())
 
 
 if __name__ == '__main__':

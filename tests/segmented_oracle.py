@@ -21,6 +21,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 SHAPE = (61, 80)           # (rows, cols): non-square, odd rows
 DX = 0.0371
 
@@ -257,35 +259,32 @@ def run_large(S, poly, name, x, y, to_numpy=np.asarray):
 
 def main():
     """Write tests/golden/segmented*.npz from the unmodified reference."""
-    ref = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
-    from prysm.conf import config
-    from prysm import geometry as G, segmented as S, polynomials as P
-    from make_golden import save
-    g = {}
-    for prec in (64, 32):
-        dt = np.float64 if prec == 64 else np.float32
-        config.precision = prec
-        x, y = (a.astype(np.float64) for a in grid(SHAPE, DX, dt))
-        r = np.hypot(x, y)
-        for k, v in geometry_cases(G, x, y, r).items():
-            g[f'geom{prec}_{k}'] = np.asarray(v)
-        for name, case in HEX_CASES.items():
-            xx, yy = (a.astype(np.float64) for a in grid(case[0], case[1], dt))
-            if prec == 32:       # the windows of the promoted grid must be those of the float32 grid
-                cha32 = S.CompositeHexagonalAperture(*grid(case[0], case[1], dt), case[2], case[3], case[4],
-                                                     segment_angle=case[5], exclude=case[6])
-            res, cha = run_hex(S, P, name, xx, yy)
-            if prec == 32:
-                assert cha32.windows == cha.windows, name
-            for k, v in res.items():
-                g[f'hex{prec}_{name}_{k}'] = v
-        for name, (n, diameter, *_rest) in LARGE_CASES.items():
-            xx, yy = (a.astype(np.float64) for a in large_grid(n, diameter, dt))
-            for k, v in run_large(S, P, name, xx, yy).items():
-                g[f'large{prec}_{k}'] = v
-    config.precision = 64
+    with reference.loaded():
+        from prysm.conf import config
+        from prysm import geometry as G, segmented as S, polynomials as P
+        from make_golden import save
+        g = {}
+        for prec in (64, 32):
+            dt = np.float64 if prec == 64 else np.float32
+            config.precision = prec
+            x, y = (a.astype(np.float64) for a in grid(SHAPE, DX, dt))
+            r = np.hypot(x, y)
+            for k, v in geometry_cases(G, x, y, r).items():
+                g[f'geom{prec}_{k}'] = np.asarray(v)
+            for name, case in HEX_CASES.items():
+                xx, yy = (a.astype(np.float64) for a in grid(case[0], case[1], dt))
+                if prec == 32:       # the windows of the promoted grid must be those of the float32 grid
+                    cha32 = S.CompositeHexagonalAperture(*grid(case[0], case[1], dt), case[2], case[3], case[4],
+                                                         segment_angle=case[5], exclude=case[6])
+                res, cha = run_hex(S, P, name, xx, yy)
+                if prec == 32:
+                    assert cha32.windows == cha.windows, name
+                for k, v in res.items():
+                    g[f'hex{prec}_{name}_{k}'] = v
+            for name, (n, diameter, *_rest) in LARGE_CASES.items():
+                xx, yy = (a.astype(np.float64) for a in large_grid(n, diameter, dt))
+                for k, v in run_large(S, P, name, xx, yy).items():
+                    g[f'large{prec}_{k}'] = v
     save('segmented.npz', g)
 
 

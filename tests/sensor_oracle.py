@@ -20,6 +20,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 SHAPES = ((2, 2), (3, 5), (4, 4), (7, 9), (64, 96), (257, 130))
 SMALL = SHAPES[:4]
 CFAS = ('rggb', 'BGGR', 'RgGb', 'bggr')          # mixed case: every function but assemble_superresolved lower-cases
@@ -131,11 +133,7 @@ def run(det, bayer, g, to_numpy=np.asarray, asarray=np.asarray):
     return out
 
 
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
     from prysm.conf import config
     from prysm import bayer, detector
     config.precision = 64
@@ -144,8 +142,8 @@ def reference_modules(ref=None):
 
 def reference_outputs():
     import warnings
-    det, bayer = reference_modules()
-    with warnings.catch_warnings():
+    with reference.loaded(), warnings.catch_warnings():
+        det, bayer = reference_modules()
         warnings.simplefilter('ignore')
         np.random.seed(0)                  # the deterministic exposures still draw (zero-variance) noise
         return run(det, bayer, inputs())
@@ -153,8 +151,9 @@ def reference_outputs():
 
 def main():
     """Write tests/golden/sensor*.npz from the unmodified reference."""
-    from make_golden import save
-    save('sensor.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('sensor.npz', reference_outputs())
 
 
 if __name__ == '__main__':

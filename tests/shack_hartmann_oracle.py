@@ -24,6 +24,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 WAVELENGTH = 0.55
 NEAR_ANGLE_ULPS = 8
 # name -> (grid samples (rows, cols), dx, pitch, n, efl, aperture, aperture_kwargs, shift)
@@ -114,11 +116,7 @@ def centroids_numpy(frames, x, y, pitch, n, shift=False, threshold=0.0):
 
 
 # ---- the reference -------------------------------------------------------------------------------------------------
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
     from prysm.conf import config
     from prysm.x import shack_hartmann as sh
     from prysm import geometry, segmented
@@ -182,16 +180,17 @@ def run(m, to_numpy=_np):
 
 def reference_outputs():
     import warnings
-    m = reference_modules()
-    with warnings.catch_warnings():
+    with reference.loaded(), warnings.catch_warnings():
+        m = reference_modules()
         warnings.simplefilter('ignore')
         return run(m)
 
 
 def main():
     """Write tests/golden/shack_hartmann*.npz from the unmodified reference."""
-    from make_golden import save
-    save('shack_hartmann.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('shack_hartmann.npz', reference_outputs())
 
 
 if __name__ == '__main__':

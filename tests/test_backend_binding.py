@@ -1,28 +1,19 @@
 """CPU: set_backend_to_b200() re-binds prysm's hot-path names and set_backend_to_defaults() restores them.
 Runs only where the unmodified reference was installed into oracle/_ref (oracle/install_reference.py) or
 PRYSM_REFERENCE names a prysm source checkout."""
-import os
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_INSTALLED = os.path.join(ROOT, 'oracle', '_ref')      # oracle/install_reference.py (the unmodified reference)
-REF = os.environ.get('PRYSM_REFERENCE', _INSTALLED)
+import reference
 
 
 @pytest.fixture()
 def prysm_pkg():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    sys.dont_write_bytecode = True
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm.propagation  # noqa: F401
         import prysm
         yield prysm
-    finally:
-        sys.path.remove(REF)
 
 
 def test_rebinding_round_trip(prysm_pkg):

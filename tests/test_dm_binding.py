@@ -1,26 +1,18 @@
 """CPU: set_backend_to_b200() re-binds prysm.x.dm.DM and prysm.coordinates.warp, and set_backend_to_defaults()
 restores them.  Runs where the unmodified reference is installed in oracle/_ref or PRYSM_REFERENCE names one."""
-import os
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture()
 def prysm_pkg():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    sys.dont_write_bytecode = True
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm
         import prysm.x.dm  # noqa: F401
         yield prysm
-    finally:
-        sys.path.remove(REF)
 
 
 def test_dm_and_warp_rebinding_round_trip(prysm_pkg):

@@ -9,16 +9,9 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf
+from gpu_fixtures import pb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    return prysm_b200
 
 
 def crand(shape, seed, dt=torch.float32):

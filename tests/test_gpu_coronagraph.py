@@ -11,6 +11,7 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf, load_golden
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 HeNe = 0.6328
@@ -20,19 +21,6 @@ TOL64 = 1e-12
 @pytest.fixture(scope='module')
 def gold():
     return load_golden('coronagraph.npz')
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
-
-
-def host(t):
-    return t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
 
 
 def setprec(pb, prec):

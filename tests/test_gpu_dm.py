@@ -1,18 +1,14 @@
 """GPU: the deformable mirror and the cubic-spline warp (prysm_b200.dm, prysm_b200.coordinates.warp) against the
 reference's fp64 fixtures (tests/golden/dm.npz), scipy, the dot-product identity, graph capture and determinism."""
-import os
-import sys
-
 import numpy as np
 import pytest
 from scipy import ndimage
 
 from conftest import load_golden, rel_linf, within
 import dm_oracle as D
+import reference
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, 'oracle', '_ref')
 TOL = {32: 1e-6, 64: 1e-12}
 # 2048^2 tilted with upsample 0.75 at fp32: two 2048^2 transforms, the spline warp and the 2048 -> 1536 matrix DFT on
 # the 3xTF32 tensor-core path; measured 1.0e-6 on an H100, so this one case is held at 1.5e-6
@@ -153,16 +149,13 @@ def test_graph_replay_and_repeated_calls_are_bit_identical(precision):
 
 @pytest.fixture(scope='module')
 def prysm_ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed (run oracle/install_reference.py)')
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm
         import prysm.x.dm  # noqa: F401
         import prysm.propagation  # noqa: F401
         yield prysm
-    finally:
-        sys.path.remove(REF)
 
 
 def dm_user_code(ifn, act):

@@ -7,30 +7,25 @@ results are compared at the north-star tolerance.  The reference is imported fro
 it from a prysm source checkout (oracle/install_reference.py).
 """
 import os
-import sys
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, 'oracle', '_ref')
+import reference
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope='module')
 def prysm_ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed (run oracle/install_reference.py)')
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm
         import prysm.propagation  # noqa: F401
         import prysm.otf  # noqa: F401
-        assert os.path.realpath(prysm.__file__).startswith(os.path.realpath(REF))
+        assert os.path.realpath(prysm.__file__).startswith(os.path.realpath(reference.REF))
         yield prysm
-    finally:
-        sys.path.remove(REF)
 
 
 def rel(a, b):

@@ -7,17 +7,9 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf
+from gpu_fixtures import pb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
 
 
 @pytest.mark.parametrize('shape,Q,prec', [((1024, 1024), 1, 32), ((2048, 2048), 1, 32), ((256, 256), 2, 32), ((96, 80), 1, 32),

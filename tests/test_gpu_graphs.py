@@ -4,18 +4,15 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_fixtures import pb  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 HeNe = 0.6328
 
 
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    prysm_b200.config.precision = 32
-    yield prysm_b200
-    prysm_b200.config.precision = 64
+@pytest.fixture(scope='module', autouse=True)
+def precision_32(pb):
+    pb.config.precision = 32
 
 
 def crand(shape, seed):

@@ -8,6 +8,7 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf, load_golden
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 ZOOMS = (0.5, 2, (2, 1.5))
@@ -16,19 +17,6 @@ ZOOMS = (0.5, 2, (2, 1.5))
 @pytest.fixture(scope='module')
 def gold():
     return load_golden('imagechain.npz')
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def setprec(pb, prec):

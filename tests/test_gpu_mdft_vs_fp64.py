@@ -44,6 +44,7 @@ import torch
 import prysm_oracle as O
 import test_host_mdft_routes as R
 from conftest import ROOT, rel_linf, within
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -516,15 +517,10 @@ def record_hits(pred, dtype=0, adjoint=False):
 
 
 # ---- fixtures and inputs ------------------------------------------------------------------------------------------
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    prev = prysm_b200.config.precision
-    prysm_b200.config.precision = 32
-    yield prysm_b200
-    prysm_b200.config.precision = prev
+@pytest.fixture(scope='module', autouse=True)
+def precision_32(pb):
+    pb.config.precision = 32
+    yield
     _PUPIL.clear()
     path = os.environ.get('PB_MDFT_TEST_HITS')
     if CHILD and path:
@@ -562,10 +558,6 @@ def geometry(shape):
     x, fx = coords(nx, mx, 0.37)
     y, fy = coords(ny, my, 0.53)
     return x, y, fx, fy
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def gemm_ref(Ey, Ex, a, adjoint):

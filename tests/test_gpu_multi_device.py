@@ -5,17 +5,16 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_fixtures import pb  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
+@pytest.fixture(scope='module', autouse=True)
+def two_devices_at_precision_32(pb):
+    if torch.cuda.device_count() < 2:
         pytest.skip('needs two CUDA devices in one process')
-    import prysm_b200
-    prysm_b200.config.precision = 32
-    yield prysm_b200
-    prysm_b200.config.precision = 64
+    pb.config.precision = 32
 
 
 def test_two_devices_one_process(pb):

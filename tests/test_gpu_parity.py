@@ -11,24 +11,13 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf, load_golden, within
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 HeNe = 0.6328
 TOL64 = 1e-12
 TOL32 = 1e-6
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    return prysm_b200
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def Qof(v):

@@ -9,21 +9,10 @@ import pytest
 import torch
 from scipy.special import j1
 
+from gpu_fixtures import pb, host  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 PARAMS = [(10.0, 1.000, 0.5), (10.0, 1.000, 1.0), (3.00, 1.125, 3.0)]
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    prysm_b200.config.precision = 64
-    return prysm_b200
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def centre_slices(a, dx):

@@ -3,30 +3,23 @@
 engine's scalar calls, the layout and launch bookkeeping, adjoint identities, and the drop-in path executed against
 the unmodified reference."""
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden, rel_linf, within
+from gpu_fixtures import pb  # noqa: F401
 import polarization_oracle as O
+import reference
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(O.ROOT, 'oracle', '_ref')
 BOUND = {32: 1e-6, 64: 1e-12}
 # The coronagraph's final plane is what the vortex lets through: its peak is 20x below that of the same chain without
 # the vortex (1.00 against 20.3 in the fixture case), so the fp32 transforms' error, ~1e-7 of the field they carry,
 # is ~2e-6 of the suppressed output.  Measured on an H100: 2.0e-6 (final plane), 1.3e-6 (its sums of |.|).
 BOUND_SUPPRESSED_32 = 3e-6
-
-
-@pytest.fixture(scope='module')
-def pb():
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
 
 
 @pytest.fixture(scope='module')
@@ -198,13 +191,12 @@ def polarized_user_code():
 
 
 def test_dropin_add_jones_propagation(pb):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed')
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm.propagation as pprop
         import prysm.x.polarization  # noqa: F401
-        assert os.path.realpath(pprop.__file__).startswith(os.path.realpath(REF))
+        assert os.path.realpath(pprop.__file__).startswith(os.path.realpath(reference.REF))
         from prysm_b200 import mathops
         saved = {n: getattr(pprop, n) for n in prysm.x.polarization.supported_propagation_funcs}
         try:
@@ -222,5 +214,3 @@ def test_dropin_add_jones_propagation(pb):
         for i, (g, w) in enumerate(zip(got, want)):
             assert g.shape == w.shape
             within(f'polarization_dropin_{i}', rel_linf(g, w), 1e-6)
-    finally:
-        sys.path.remove(REF)

@@ -10,16 +10,9 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf
+from gpu_fixtures import pb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    return prysm_b200
 
 
 def reference_sum(amp, opd, wvls, wts, dx, efl, fdx, M, kind):

@@ -13,6 +13,7 @@ import torch
 
 from conftest import load_golden, within
 import polynomials_oracle as O
+from gpu_fixtures import host
 
 pytestmark = pytest.mark.gpu
 FP32_BOUND = 5.3e-6      # measured 3.5e-6 (H100 80GB HBM3, 700 W)
@@ -29,10 +30,6 @@ def P():
         pytest.skip('needs a CUDA device')
     from prysm_b200 import polynomials
     return polynomials
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def dev(a, dt=np.float64):

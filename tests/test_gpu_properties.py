@@ -3,30 +3,17 @@ runs the same examples) -- ragged / odd / prime sizes, fractional Q, shifted foc
 Tolerances: complex128 1e-11, complex64 2e-6 (relative L-inf vs the fp64 oracle)."""
 import numpy as np
 import pytest
-import torch
 from hypothesis import given, settings, strategies as st, HealthCheck
 
 import prysm_oracle as O
 from conftest import rel_linf
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 HeNe = 0.6328
 SETTINGS = dict(max_examples=20, deadline=None, derandomize=True,
                 suppress_health_check=[HealthCheck.too_slow, HealthCheck.function_scoped_fixture])
 shapes = st.tuples(st.integers(1, 40), st.integers(1, 40))
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def crand(rng, shape, cdt):

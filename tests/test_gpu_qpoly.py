@@ -12,6 +12,7 @@ import torch
 
 from conftest import load_golden, within
 import qpoly_oracle as O
+from gpu_fixtures import host
 
 pytestmark = pytest.mark.gpu
 FP32_BOUND = 3.5e-6      # measured 2.3e-6 (H100 80GB HBM3, 700 W)
@@ -28,10 +29,6 @@ def Q():
         pytest.skip('needs a CUDA device')
     from prysm_b200 import qpoly
     return qpoly
-
-
-def host(t):
-    return t.detach().cpu().numpy()
 
 
 def plane_err(got, ref):

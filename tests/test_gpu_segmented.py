@@ -1,18 +1,14 @@
 """GPU: the signed-distance geometry and CompositeHexagonalAperture (prysm_b200.geometry, prysm_b200.segmented)
 against the reference's fixtures (tests/golden/segmented*.npz), the adjoint's dot-product identity, graph capture
 and determinism, and a JWST pupil end to end through focus."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from conftest import load_golden, rel_linf, within
+import reference
 import segmented_oracle as O
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, 'oracle', '_ref')
 TOL = {32: 1e-6, 64: 1e-12}
 
 
@@ -240,16 +236,13 @@ def test_graph_replay_and_repeated_calls_are_bit_identical():
 
 @pytest.fixture(scope='module')
 def prysm_ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed (run oracle/install_reference.py)')
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         import prysm
         import prysm.segmented  # noqa: F401
         import prysm.propagation  # noqa: F401
         yield prysm
-    finally:
-        sys.path.remove(REF)
 
 
 def jwst_pupil(geometry, segmented, polynomials, x, y, c):

@@ -3,8 +3,6 @@ detector cases against the reference's fixtures (tests/golden/sensor*.npz, writt
 random part of Detector.expose against exact distributions (chi-square, moments), for independence and for
 reproducibility under numpy's global seed; and the reference's own user code through the drop-in switch."""
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -12,19 +10,13 @@ import torch
 from scipy import stats
 
 from conftest import load_golden, rel_linf
+from gpu_fixtures import pb  # noqa: F401
+import reference
 import sensor_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(O.ROOT, 'oracle', '_ref')
 ROUNDED = ('malvar_', 'superres_', 'wbpre_1', 'wbpost_1')      # fp64 sums or descaled gains: 1e-12, not bit-exact
-
-
-@pytest.fixture(scope='module')
-def pb():
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
 
 
 @pytest.fixture(scope='module')
@@ -268,20 +260,14 @@ def test_expose_lut_is_fused_and_matches_apply_lut(pb):
 
 # ---- drop-in ----------------------------------------------------------------------------------------------------------
 def _with_reference(fn):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed')
-    before = set(sys.modules)
-    sys.path.insert(0, REF)
-    try:
-        return fn()
-    finally:
-        from prysm_b200 import mathops
-        mathops.set_backend_to_defaults()
-        for name in set(sys.modules) - before:
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
+    from prysm_b200 import mathops
+    with reference.loaded():
+        try:
+            return fn()
+        finally:
+            mathops.set_backend_to_defaults()
 
 
 def test_dropin_image_simulation_chain(pb):

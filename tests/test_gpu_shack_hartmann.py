@@ -2,19 +2,17 @@
 fixtures (tests/golden/shack_hartmann*.npz, written by tests/shack_hartmann_oracle.py), spot_centroids against its numpy
 statement, the physics of a tilted beam, a calibrated modal loop with its CUDA-graph capture, the drop-in path with
 the unmodified reference, and a Detector.expose frame straight into the slopes."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden, within
+from gpu_fixtures import pb  # noqa: F401
+import reference
 import shack_hartmann_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(O.ROOT, 'oracle', '_ref')
 # Measured on an H100 SXM (700 W, 1980 MHz); each bound is the measured figure x 1.5.
 # fp32 screens against the fp64 fixtures, away from the samples whose mask the float32 grid itself flips: 1.03e-5
 # (circle_shift; the others 4.1e-6 to 7.0e-6), mostly the float32 grid's own rounding of rsq.
@@ -24,13 +22,6 @@ BOUND_SCREEN_32 = 1.55e-5
 BOUND_TILT = 0.21
 # worst coefficient error of the calibrated Noll 2-11 loop at ~50 nm RMS: 0.340 nm
 BOUND_LOOP_NM = 0.51
-
-
-@pytest.fixture(scope='module')
-def pb():
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
 
 
 @pytest.fixture(scope='module')
@@ -336,26 +327,21 @@ def test_exposed_frame_goes_straight_into_slopes(pb):
 def test_dropin_reference_user_code(pb, golden):
     """The reference's own shack_hartmann and Wavefront code, run through set_backend_to_b200(), gives the fixtures
     (the reference's numpy results) within 1e-6."""
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed')
-    before = set(sys.modules)
-    m = O.reference_modules(REF)
     from prysm_b200 import mathops
-    try:
-        mathops.set_backend_to_b200()
-        assert m.sh.shack_hartmann is pb.shack_hartmann.shack_hartmann
-        import warnings
-        with warnings.catch_warnings():
-            warnings.simplefilter('ignore')
-            mine = O.run(m, to_numpy=to_numpy)
-    finally:
-        mathops.set_backend_to_defaults()
-        for name in set(sys.modules) - before:
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
-        pb.config.precision = 64
+    with reference.loaded():
+        m = O.reference_modules()
+        try:
+            mathops.set_backend_to_b200()
+            assert m.sh.shack_hartmann is pb.shack_hartmann.shack_hartmann
+            import warnings
+            with warnings.catch_warnings():
+                warnings.simplefilter('ignore')
+                mine = O.run(m, to_numpy=to_numpy)
+        finally:
+            mathops.set_backend_to_defaults()
+            pb.config.precision = 64
     for k in sorted(golden):
         if k.startswith('near_'):
             continue

@@ -2,21 +2,13 @@
 pb_angular_spectrum, against numpy fp64 and against the generic shared-memory kernel."""
 import numpy as np
 import pytest
-import torch
 
 import prysm_oracle as O
 from conftest import rel_linf
+from gpu_fixtures import pb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 HeNe = 0.6328
-
-
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    return prysm_b200
 
 
 def crand(shape, seed):

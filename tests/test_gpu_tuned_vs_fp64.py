@@ -57,6 +57,7 @@ import torch
 
 import prysm_oracle as O
 from conftest import rel_linf, within
+from gpu_fixtures import pb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -347,15 +348,10 @@ def run_axis(chk, case, fn, expect):
 
 
 # ---- fixtures -----------------------------------------------------------------------------------------------------
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    prev = prysm_b200.config.precision
-    prysm_b200.config.precision = 32
-    yield prysm_b200
-    prysm_b200.config.precision = prev
+@pytest.fixture(scope='module', autouse=True)
+def precision_32(pb):
+    pb.config.precision = 32
+    yield
     _REF.clear()
     _HOST.clear()
 

@@ -2,8 +2,6 @@
 (tests/golden/wfs*.npz, written by tests/wfs_oracle.py), the Bessel ratios against scipy, the determinism and graph
 capture of the coupling reduction and of a whole SRI forward model, the launch count of a PSI reconstruction, and the
 drop-in path executed against the unmodified reference."""
-import os
-import sys
 import types
 
 import numpy as np
@@ -12,11 +10,12 @@ import torch
 from scipy import special
 
 from conftest import load_golden, rel_linf, within
+from gpu_fixtures import pb  # noqa: F401
+import reference
 import wfs_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(O.ROOT, 'oracle', '_ref')
 BOUND = {32: 1e-6, 64: 1e-12}
 # Camera intensities at fp32 are squared fields after two matrix DFTs per arm, so the transforms' ~5e-7 field error
 # doubles.  Measured on an H100 (700 W, 1980 MHz): SRI 1.68e-6 (phase pi/2) and 1.44e-6 (phase 0), ronchi PS/PDI along x
@@ -24,13 +23,6 @@ BOUND = {32: 1e-6, 64: 1e-12}
 BOUND_INTENSITY_32 = 3e-6
 INTENSITIES = ('sri_I_', 'pdi_ronchi_x_0', 'pdi_ronchi_x_60', 'pdi_ratio_I2')
 EXACT = ('pdi_ronchi_x_grating', 'pdi_ronchi_y_grating', 'rect1', 'rect2')
-
-
-@pytest.fixture(scope='module')
-def pb():
-    import prysm_b200
-    yield prysm_b200
-    prysm_b200.config.precision = 64
 
 
 @pytest.fixture(scope='module')
@@ -224,26 +216,21 @@ def test_degroot_is_one_launch(pb):
 def test_dropin_reference_user_code(pb, golden):
     """The reference's own SRI, PS/PDI, PSI and multimode_coupling code, run through set_backend_to_b200(), gives the
     fixtures (the reference's numpy results) within 1e-6."""
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('oracle/_ref is not installed')
-    before = set(sys.modules)
-    m = O.reference_modules(REF)
     from prysm_b200 import mathops
-    try:
-        mathops.set_backend_to_b200()
-        assert m.sri.SelfReferencedInterferometer is pb.sri.SelfReferencedInterferometer
-        assert m.fibers.multimode_coupling is pb.fibers.multimode_coupling
-        import warnings
-        with warnings.catch_warnings():
-            warnings.simplefilter('ignore')
-            mine = O.run(m, O.inputs(), to_numpy=to_numpy)
-    finally:
-        mathops.set_backend_to_defaults()
-        for name in set(sys.modules) - before:
-            if name.split('.')[0] in ('prysm', 'skimage'):
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
+    with reference.loaded(also=('skimage',)):
+        m = O.reference_modules()
+        try:
+            mathops.set_backend_to_b200()
+            assert m.sri.SelfReferencedInterferometer is pb.sri.SelfReferencedInterferometer
+            assert m.fibers.multimode_coupling is pb.fibers.multimode_coupling
+            import warnings
+            with warnings.catch_warnings():
+                warnings.simplefilter('ignore')
+                mine = O.run(m, O.inputs(), to_numpy=to_numpy)
+        finally:
+            mathops.set_backend_to_defaults()
     for k in ('fam_V10_keys',):
         assert np.array_equal(mine[k], golden[k])
     bad = {}

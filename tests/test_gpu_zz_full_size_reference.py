@@ -14,27 +14,18 @@ inside the north-star 1e-6.  Measured by this test on an H100 (windows / strided
     C5 final CZT focus   measured 5.0e-7            bound 6.5e-7      (reference fp32: 2.5e-5)"""
 import numpy as np
 import pytest
-import torch
 
 import prysm_oracle as O
 from conftest import load_golden, within
+from gpu_fixtures import pb, host  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 HeNe = 0.6328
 
 
-@pytest.fixture(scope='module')
-def pb():
-    if not torch.cuda.is_available():
-        pytest.skip('needs a CUDA device')
-    import prysm_b200
-    prysm_b200.config.precision = 32
-    yield prysm_b200
-    prysm_b200.config.precision = 64
-
-
-def host(t):
-    return t.detach().cpu().numpy()
+@pytest.fixture(scope='module', autouse=True)
+def precision_32(pb):
+    pb.config.precision = 32
 
 
 def test_c4_czt_fields_and_incoherent_sum_vs_reference(pb):

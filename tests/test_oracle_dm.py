@@ -1,18 +1,13 @@
 """CPU: the fp64 DM restatement (tests/dm_oracle.py) replays the reference's fixtures (tests/golden/dm.npz), the host-side
 lattice and projection matrices of prysm_b200.dm match the reference's own functions, and scipy's warp rules that the
 spline kernel reproduces are pinned."""
-import os
-import sys
-
 import numpy as np
 import pytest
 from scipy import ndimage
 
 from conftest import load_golden, rel_linf
 import dm_oracle as D
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -22,17 +17,13 @@ def golden():
 
 @pytest.fixture(scope='module')
 def ref_dm():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    sys.dont_write_bytecode = True
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         import prysm.x.dm as rdm
         config.precision = 64
         yield rdm
-    finally:
-        sys.path.remove(REF)
 
 
 @pytest.mark.parametrize('name', sorted(D.SMALL_CASES))

@@ -1,14 +1,11 @@
 """CPU: the reference, where it is installed (oracle/_ref), re-derives every polarization fixture
 (tests/golden/polarization*.npz) from the inputs tests/polarization_oracle.py builds."""
-import os
-
 import numpy as np
 import pytest
 
 from conftest import load_golden
 import polarization_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -24,18 +21,9 @@ def test_fixture_inputs_are_deterministic():
 
 
 def test_reference_rederives_the_fixtures(golden):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    import sys
-    before = set(sys.modules)
-    try:
-        mine = O.reference_outputs()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules do not stay importable as `prysm`
-            if name == 'prysm' or name.startswith('prysm.'):
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
+    mine = O.reference_outputs()
     assert sorted(mine) == sorted(golden)
     for k, v in golden.items():
         np.testing.assert_array_equal(np.asarray(mine[k]), v, err_msg=k)

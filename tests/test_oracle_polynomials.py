@@ -1,16 +1,12 @@
 """CPU: the reference, where it is installed (oracle/_ref), re-derives every orthogonal-polynomial fixture
 (tests/golden/polynomials*.npz) bit for bit, and the host-only index helpers (xy_j_to_mn, ansi_j_to_nm, nm_to_ansi_j,
 nm_to_fringe, beside noll_to_nm and fringe_to_nm) equal the reference's over a range."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from conftest import load_golden
 import polynomials_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -20,17 +16,10 @@ def golden():
 
 @pytest.fixture(scope='module')
 def ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    before = set(sys.modules)
-    try:
+    with reference.loaded():
         yield O.reference_modules()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules do not stay
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
 
 
 @pytest.fixture(scope='module')

@@ -2,16 +2,12 @@
 (tests/golden/qpoly*.npz) bit for bit; the engine's C++ recurrence tables (pb_qpoly_tables, the ones its kernels are
 planned with) match the reference's scalar functions; and the host-only Q2d_nm_c_to_a_b keeps the reference's
 semantics."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from conftest import load_golden
 import qpoly_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -21,17 +17,10 @@ def golden():
 
 @pytest.fixture(scope='module')
 def ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    before = set(sys.modules)
-    try:
+    with reference.loaded():
         yield O.reference_modules()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules do not stay
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
 
 
 @pytest.fixture(scope='module')

@@ -1,17 +1,12 @@
 """CPU: the fp64 restatement of the geometry and of compose_opd (tests/segmented_oracle.py) replays the reference's
 fixtures (tests/golden/segmented*.npz), and the engine's host tables of CompositeHexagonalAperture (windows, centres,
 ids, the keys that decide which segments share a basis) match the fixtures and, where it is installed, the reference."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from conftest import load_golden, rel_linf
 import segmented_oracle as O
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -21,17 +16,12 @@ def golden():
 
 @pytest.fixture(scope='module')
 def ref():
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    sys.dont_write_bytecode = True
-    sys.path.insert(0, REF)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         from prysm import segmented
         yield config, segmented
-    finally:
-        config.precision = 64
-        sys.path.remove(REF)
 
 
 def dtype_of(prec):

@@ -2,34 +2,18 @@
 from the inputs tests/sensor_oracle.py builds; the Malvar filters the engine uses are the reference's and are symmetric
 under a 180-degree rotation, so the engine's correlation equals scipy's convolution."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from conftest import load_golden
 import sensor_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
 def golden():
     return load_golden('sensor.npz')
-
-
-def _reference(fn):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
-        pytest.skip('reference prysm not installed')
-    before = set(sys.modules)
-    try:
-        return fn()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules do not stay
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
 
 
 def test_fixture_inputs_are_deterministic():
@@ -40,7 +24,9 @@ def test_fixture_inputs_are_deterministic():
 
 
 def test_reference_rederives_the_fixtures(golden):
-    mine = _reference(O.reference_outputs)
+    if not reference.installed():
+        pytest.skip('reference prysm not installed')
+    mine = O.reference_outputs()
     assert sorted(mine) == sorted(golden)
     for k, v in golden.items():
         got = np.asarray(mine[k])
@@ -64,13 +50,12 @@ def test_fixtures_cover_every_bayer_function_and_the_error_cases(golden):
 
 def test_malvar_filters_are_the_references_and_point_symmetric():
     from prysm_b200 import bayer as ours
-
-    def ref_kernels():
-        sys.path.insert(0, REF)
+    if not reference.installed():
+        pytest.skip('reference prysm not installed')
+    with reference.loaded():
         from prysm import bayer
-        return {'G_at_R_or_B': bayer.kernel_G_at_R_or_B, 'R_at_G_in_RB': bayer.kernel_R_at_G_in_RB,
-                'R_at_G_in_BR': bayer.kernel_R_at_G_in_BR, 'R_at_B_in_BB': bayer.kernel_R_at_B_in_BB}
-    ref = _reference(ref_kernels)
+        ref = {'G_at_R_or_B': bayer.kernel_G_at_R_or_B, 'R_at_G_in_RB': bayer.kernel_R_at_G_in_RB,
+               'R_at_G_in_BR': bayer.kernel_R_at_G_in_BR, 'R_at_B_in_BB': bayer.kernel_R_at_B_in_BB}
     assert sorted(ref) == sorted(ours.MALVAR_KERNELS)
     for name, k in ours.MALVAR_KERNELS.items():
         np.testing.assert_array_equal(k, np.asarray(ref[name], dtype=np.float64), err_msg=name)

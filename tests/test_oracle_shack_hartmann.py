@@ -2,8 +2,6 @@
 (tests/golden/shack_hartmann*.npz) bit for bit; the fixtures pin the reference's multi-claimed edges; and the numpy
 statement of spot_centroids (tests/shack_hartmann_oracle.py) agrees with an independent per-subaperture
 scipy.ndimage.center_of_mass."""
-import os
-import sys
 import warnings
 
 import numpy as np
@@ -12,8 +10,7 @@ from scipy import ndimage
 
 from conftest import load_golden
 import shack_hartmann_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -22,17 +19,9 @@ def golden():
 
 
 def test_reference_rederives_the_fixtures(golden):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    before = set(sys.modules)
-    try:
-        mine = O.reference_outputs()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules do not stay
-            if name.split('.')[0] == 'prysm':
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
+    mine = O.reference_outputs()
     assert sorted(mine) == sorted(golden)
     for k, v in golden.items():
         np.testing.assert_array_equal(np.asarray(mine[k]), v, err_msg=k)

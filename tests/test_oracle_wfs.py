@@ -1,17 +1,13 @@
 """CPU: the reference, where it is installed (oracle/_ref), re-derives every wavefront-sensing fixture
 (tests/golden/wfs*.npz) from the inputs tests/wfs_oracle.py builds; the engine's host mode finder matches the fixtures
 and cutoff theory."""
-import os
-import sys
-
 import numpy as np
 import pytest
 from scipy import special
 
 from conftest import load_golden
 import wfs_oracle as O
-
-REF = os.environ.get('PRYSM_REFERENCE', os.path.join(O.ROOT, 'oracle', '_ref'))
+import reference
 
 
 @pytest.fixture(scope='module')
@@ -42,17 +38,9 @@ def test_fixture_grid_spacings_are_float32_exact():
 
 
 def test_reference_rederives_the_fixtures(golden):
-    if not os.path.isdir(os.path.join(REF, 'prysm')):
+    if not reference.installed():
         pytest.skip('reference prysm not installed')
-    before = set(sys.modules)
-    try:
-        mine = O.reference_outputs()
-    finally:
-        for name in set(sys.modules) - before:      # the reference's modules (and the skimage stub) do not stay
-            if name.split('.')[0] in ('prysm', 'skimage'):
-                del sys.modules[name]
-        if REF in sys.path:
-            sys.path.remove(REF)
+    mine = O.reference_outputs()
     assert sorted(mine) == sorted(golden)
     for k, v in golden.items():
         np.testing.assert_array_equal(np.asarray(mine[k]), v, err_msg=k)

@@ -26,6 +26,8 @@ for _p in (ROOT, os.path.join(ROOT, 'oracle')):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import reference  # noqa: E402
+
 V_FIND = (0.5, 2.3, 3.0, 10, 20)
 LP = dict(V=10, a=4.0, dx=0.375, shape=(64, 72))          # out to 3a along y
 SMF = dict(V=2.3, a=0.975, dx=0.0625, n=96)
@@ -191,15 +193,13 @@ def run(m, g, to_numpy=_np, asarray=np.asarray, modes10=None, reference=False):
     return out
 
 
-def reference_modules(ref=None):
-    ref = ref or os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-    if ref not in sys.path:
-        sys.path.insert(0, ref)
-    sys.dont_write_bytecode = True
+def reference_modules():
+    """Call inside reference.loaded(also=('skimage',)): the skimage stub goes with the reference's modules."""
     if 'skimage.restoration._unwrap_2d' not in sys.modules:      # prysm.x.psi imports it; unwrap_phase is not used
-        for name in ('skimage', 'skimage.restoration', 'skimage.restoration._unwrap_2d'):
-            sys.modules.setdefault(name, types.ModuleType(name))
-        sys.modules['skimage.restoration._unwrap_2d'].unwrap_2d = None
+        stub = types.ModuleType('skimage.restoration._unwrap_2d')
+        stub.unwrap_2d = None
+        for mod in (types.ModuleType('skimage'), types.ModuleType('skimage.restoration'), stub):
+            sys.modules.setdefault(mod.__name__, mod)
     from prysm.conf import config
     from prysm.x import fibers, sri, pdi, psi
     from prysm.propagation import Wavefront
@@ -209,16 +209,17 @@ def reference_modules(ref=None):
 
 def reference_outputs():
     import warnings
-    m = reference_modules()
-    with warnings.catch_warnings():
+    with reference.loaded(also=('skimage',)), warnings.catch_warnings():
+        m = reference_modules()
         warnings.simplefilter('ignore')
         return run(m, inputs(), reference=True)
 
 
 def main():
     """Write tests/golden/wfs*.npz from the unmodified reference."""
-    from make_golden import save
-    save('wfs.npz', reference_outputs())
+    with reference.loaded():
+        from make_golden import save      # imports the reference
+        save('wfs.npz', reference_outputs())
 
 
 if __name__ == '__main__':

@@ -12,23 +12,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import prysm_b200 as pb  # noqa: E402
+from benchlib import timed  # noqa: E402
 from prysm_b200 import _ops, propagation as P  # noqa: E402
 
 HeNe = 0.6328
-
-
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    l0 = _ops.launch_count()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / reps, (_ops.launch_count() - l0) / reps
 
 
 gen = torch.Generator(device='cuda').manual_seed(1)
@@ -51,15 +38,19 @@ for prec in (32, 64):
     for kind in ('mdft', 'czt'):
         ex = P.prepare_executor(10.0 / n, n, 1.0, m, HeNe, 100.0, kind=kind)
         tc = kind == 'mdft' and getattr(ex, '_tc', None) is not None and getattr(ex, '_tc_adj', None) is not None
-        us, nl = timeit(lambda: P.to_fpm_and_back(w, fpm, ex))
+        us, nl = timed(lambda: P.to_fpm_and_back(w, fpm, ex), 20)
+        us *= 1e6
         print(f'[p{prec}] to_fpm_and_back {n}^2<->{m}^2 {kind}{" (wgmma both legs)" if tc else ""}: {us:.0f} us, {nl:.0f} launches')
-        us, nl = timeit(lambda: P.babinet(w, lyot, fpm, ex))
+        us, nl = timed(lambda: P.babinet(w, lyot, fpm, ex), 20)
+        us *= 1e6
         print(f'[p{prec}] babinet         {n}^2<->{m}^2 {kind}: {us:.0f} us, {nl:.0f} launches')
         step = pb.graphs.capture(lambda w_: P.babinet(w_, lyot, fpm, ex), w)
-        us, _ = timeit(lambda: step(w))
+        us, _ = timed(lambda: step(w), 20)
+        us *= 1e6
         print(f'[p{prec}] babinet         {n}^2<->{m}^2 {kind}, CUDA graph replay: {us:.0f} us')
         g = crand((n, n), cdt)
-        us, nl = timeit(lambda: P.babinet_adjoint(g, lyot, fpm, ex))
+        us, nl = timed(lambda: P.babinet_adjoint(g, lyot, fpm, ex), 20)
+        us *= 1e6
         print(f'[p{prec}] babinet_adjoint {n}^2<->{m}^2 {kind}: {us:.0f} us, {nl:.0f} launches')
     # the reference's vortex rig (tests/test_propagation.py:463-541): 384^2 pupil, 640^2 + 5 x 256^2 focal levels
     npup, nd, pdx, efl = 384, 320, 0.05, 100.0
@@ -68,14 +59,17 @@ for prec in (32, 64):
     vm = P.vortex_phase_mask(2)
     for kind in ('mdft', 'czt'):
         mex = P.prepare_multiresolution(pdx, npup, period / (2 * nd), 2 * nd, HeNe, efl, num_levels=6, fine_samples=256, kind=kind)
-        us, nl = timeit(lambda: P.to_fpm_and_back_multiresolution(pupil, vm, mex))
+        us, nl = timed(lambda: P.to_fpm_and_back_multiresolution(pupil, vm, mex), 20)
+        us *= 1e6
         print(f'[p{prec}] vortex 6-level multiresolution 384^2 {kind}: {us:.0f} us, {nl:.0f} launches')
-        us, nl = timeit(lambda: P.to_fpm_and_back_multiresolution_adjoint(pupil, vm, mex))
+        us, nl = timed(lambda: P.to_fpm_and_back_multiresolution_adjoint(pupil, vm, mex), 20)
+        us *= 1e6
         print(f'[p{prec}] vortex 6-level multiresolution adjoint 384^2 {kind}: {us:.0f} us, {nl:.0f} launches')
         step = pb.graphs.capture(lambda w_: P.to_fpm_and_back_multiresolution(w_, vm, mex), pupil)
         ref = P.to_fpm_and_back_multiresolution(pupil, vm, mex)
         err = float((step(pupil) - ref).abs().max() / ref.abs().max())
-        us, _ = timeit(lambda: step(pupil))
+        us, _ = timed(lambda: step(pupil), 20)
+        us *= 1e6
         print(f'[p{prec}] vortex 6-level multiresolution 384^2 {kind}, CUDA graph replay: {us:.0f} us (max diff vs eager {err:.1e})')
     # modal phase-retrieval gradient (docs/source/how-tos/Differentiable Optical Models.ipynb): 512^2 pupil -> 256^2 PSF, 19 modes
     npup, npsf = 512, 256
@@ -98,6 +92,7 @@ for prec in (32, 64):
         pbar = wf.from_amp_and_phase_adjoint_phase(wbar)
         return pb.polynomials.sum_of_2d_modes_adjoint(basis, pbar)
 
-    us, nl = timeit(cost_grad)
+    us, nl = timed(cost_grad, 20)
+    us *= 1e6
     print(f'[p{prec}] modal phase-retrieval cost+gradient 512^2 -> 256^2, 19 modes: {us:.0f} us, {nl:.0f} launches')
     ex = None

@@ -11,34 +11,20 @@ oracle/_ref holds it.  The card's name and power limit are printed with the numb
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
 import prysm_b200 as pb  # noqa: E402
+import reference  # noqa: E402
+from benchlib import card, timed  # noqa: E402
 from prysm_b200 import _ops  # noqa: E402
 
 SIZES = ((512, 48, 8), (1024, 48, 16), (2048, 64, 24))
 VARIANTS = (('flat', dict()), ('tilt', dict(rot=(5, 0, 10))), ('tilt_up075', dict(rot=(5, 0, 10), upsample=0.75)))
-
-
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    l0 = _ops.launch_count()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / reps, (_ops.launch_count() - l0) / reps
 
 
 def ifn_for(n, sep):
@@ -47,11 +33,9 @@ def ifn_for(n, sep):
 
 
 def reference_render_us(n, nact, sep, kw, reps=3):
-    ref = os.path.join(ROOT, 'oracle', '_ref')
-    if not os.path.isdir(os.path.join(ref, 'prysm')):
+    if not reference.installed():
         return None
-    sys.path.insert(0, ref)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         from prysm.x.dm import DM
         config.precision = 32
@@ -62,17 +46,6 @@ def reference_render_us(n, nact, sep, kw, reps=3):
         for _ in range(reps):
             dm.render()
         return (time.perf_counter() - t0) / reps * 1e6
-    finally:
-        sys.path.remove(ref)
-
-
-def card():
-    try:
-        r = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return torch.cuda.get_device_name()
 
 
 def main():
@@ -85,9 +58,10 @@ def main():
     for n, nact, sep in SIZES:
         x = pb.asdevice(np.random.default_rng(1).standard_normal((n, n)).astype(np.float32))
         xc = _ops.fft2(x)
-        pair_us, _ = timeit(lambda: _ops.fft2(_ops.fft2(xc, dir=-1, shift_in=True), dir=+1, shift_out=True))
+        pair_s, _ = timed(lambda: _ops.fft2(_ops.fft2(xc, dir=-1, shift_in=True), dir=+1, shift_out=True), 20)
         Mfwd, Mifwd = pb.dm.projection_matrices((n, n), (5, 0, 10))
-        warp_us, warp_launches = timeit(lambda: _ops.warp(x, matrix=Mifwd))
+        warp_s, warp_launches = timed(lambda: _ops.warp(x, matrix=Mifwd), 20)
+        pair_us, warp_us = pair_s * 1e6, warp_s * 1e6
         # prefilter: read fp32 input, write + read fp64 intermediate, write + read fp64 coefficients; interpolation
         # writes fp32 (the 4 x 4 taps mostly hit L1 / L2): the least traffic of the two passes and the gather
         warp_bytes = n * n * (4 + 8 + 8 + 8 + 8 + 4)
@@ -96,9 +70,10 @@ def main():
         for vname, kw in VARIANTS:
             dm = pb.dm.DM(ifn_for(n, sep), Nout=n, Nact=nact, sep=sep, **kw)
             dm.update(np.random.default_rng(0).uniform(-1, 1, (nact, nact)).astype(np.float32))
-            r_us, r_l = timeit(dm.render)
+            r_s, r_l = timed(dm.render, 20)
             g = dm.render().clone()
-            a_us, a_l = timeit(lambda: dm.render_adjoint(g))
+            a_s, a_l = timed(lambda: dm.render_adjoint(g), 20)
+            r_us, a_us = r_s * 1e6, a_s * 1e6
             ref_us = reference_render_us(n, nact, sep, kw)
             row = dict(n=n, nact=nact, sep=sep, variant=vname, render_us=r_us, render_launches=r_l, adjoint_us=a_us,
                        adjoint_launches=a_l, fft2_pair_us=pair_us, warp_us=warp_us, warp_gbs=warp_bytes / warp_us / 1e3,

@@ -20,6 +20,8 @@ import os
 import subprocess
 import sys
 
+from benchlib import card
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 N, Q, BATCH = 2048, 2, 16
 K = N * Q
@@ -111,16 +113,6 @@ for name, fn in cases.items():
                  'launches_per_call': (_ops.launch_count() - l0) / reps}
 print('RESULT', json.dumps(res))
 '''
-
-
-def card():
-    q = 'name,power.limit,clocks.sm,clocks.max.sm'
-    try:
-        r = subprocess.run(['nvidia-smi', f'--query-gpu={q}', '--format=csv,noheader', '-i', '0'],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return 'nvidia-smi unavailable'
 
 
 def run_child(root, src):

@@ -10,21 +10,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import prysm_b200 as pb  # noqa: E402
+from benchlib import timed  # noqa: E402
 from prysm_b200 import _ops, convolution as CV, fttools as FT  # noqa: E402
-
-
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    l0 = _ops.launch_count()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / reps, (_ops.launch_count() - l0) / reps
 
 
 pb.config.precision = 32
@@ -32,18 +19,22 @@ gen = torch.Generator(device='cuda').manual_seed(3)
 for n in (2048, 4096):
     o = torch.rand((n, n), generator=gen, device='cuda')
     h = torch.rand((n, n), generator=gen, device='cuda')
-    us, nl = timeit(lambda: CV.conv(o, h))
+    us, nl = timed(lambda: CV.conv(o, h), 20)
+    us *= 1e6
     print(f'conv real x real {n}^2 (packed: 1 forward + 1 inverse FFT): {us:.0f} us, {nl:.0f} launches')
 
     def three_fft():
         O = _ops.fft2(o, (n, n), dir=-1, shift_in=True)
         H = _ops.fft2(h, (n, n), dir=-1, shift_in=True)
         return _ops.fft2(_ops.binary('mul', O, H), (n, n), dir=+1, scale=1.0 / (n * n), shift_out=True)
-    us, nl = timeit(three_fft)
+    us, nl = timed(three_fft, 20)
+    us *= 1e6
     print(f'conv real x real {n}^2 the reference way (3 FFTs + product): {us:.0f} us, {nl:.0f} launches')
     tf = torch.rand((n, n), generator=gen, device='cuda')
-    us, nl = timeit(lambda: CV.apply_transfer_functions(o, 1.0, [tf, tf]))
+    us, nl = timed(lambda: CV.apply_transfer_functions(o, 1.0, [tf, tf]), 20)
+    us *= 1e6
     print(f'apply_transfer_functions {n}^2, 2 array TFs: {us:.0f} us, {nl:.0f} launches')
 f = torch.rand((1024, 1024), generator=gen, device='cuda')
-us, nl = timeit(lambda: FT.fourier_resample(f, 2))
+us, nl = timed(lambda: FT.fourier_resample(f, 2), 20)
+us *= 1e6
 print(f'fourier_resample 1024^2 -> 2048^2 (plan rebuilt per call, like the reference): {us:.0f} us, {nl:.0f} launches')

@@ -15,52 +15,23 @@ The card name, power limit and current SM clock are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) * 1e3 / iters       # us per call
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
 
 
 def alternate(fa, fb, iters, rounds=5):
     """Median over `rounds` of (fa, fb) timed back to back."""
     ta, tb = [], []
     for _ in range(rounds):
-        ta.append(timed(fa, iters))
-        tb.append(timed(fb, iters))
+        ta.append(timed(fa, iters, warm=1)[0] * 1e6)
+        tb.append(timed(fb, iters, warm=1)[0] * 1e6)
     return float(np.median(ta)), float(np.median(tb))
-
-
-def host_once(fn):
-    t0 = time.perf_counter()
-    fn()
-    return (time.perf_counter() - t0) * 1e6
 
 
 def main():
@@ -118,7 +89,7 @@ def main():
     }
     res['kernels_4096'] = {}
     for name, (fn, bpp) in kernels.items():
-        t = timed(fn, args.iters)
+        t = timed(fn, args.iters, warm=1)[0] * 1e6
         gbs = bpp * px / (t * 1e-6) / 1e9
         res['kernels_4096'][name] = {'us': t, 'bytes_per_pixel': bpp, 'GB/s': gbs,
                                      'share_of_3.35TB/s': gbs * 1e9 / HBM_BYTES_PER_S}
@@ -127,23 +98,22 @@ def main():
 
     # ---- the reference's host path
     if not args.no_reference:
-        ref = os.path.join(ROOT, 'oracle', '_ref')
-        sys.path.insert(0, ref)
-        from prysm.x import polarization as rpol
-        from prysm import propagation as rprop
-        hr = {}
-        n = 2048
-        Jh = (rng.standard_normal((n, n, 2, 2)) + 1j * rng.standard_normal((n, n, 2, 2)))
-        hr['jones_focus_2048_Q2_us'] = host_once(lambda: rpol.jones_adapter(rprop.focus)(Jh, 2))
-        n, m = 1024, 256
-        rex = rprop.prepare_executor(10.0 / n, (n, n), 0.55 * 100 / 10 / 2, (m, m), 0.55, 100.0, kind='mdft')
-        Jm = Jh[:n, :n].copy()
-        hr['jones_focus_dft_1024_256_us'] = host_once(lambda: rpol.jones_adapter(rprop.focus_dft)(Jm, rex))
-        Kh = Jh[::-1].copy()
-        th = rng.uniform(-np.pi, np.pi, Jh.shape[:2])
-        hr['matmul_2048_us'] = host_once(lambda: Jh @ Kh)
-        hr['vector_vortex_retarder_2048_us'] = host_once(lambda: rpol.vector_vortex_retarder(2, th.copy()))
-        hr['jones_to_mueller_2048_us'] = host_once(lambda: rpol.jones_to_mueller(Jh))
+        with reference.loaded():
+            from prysm.x import polarization as rpol
+            from prysm import propagation as rprop
+            hr = {}
+            n = 2048
+            Jh = (rng.standard_normal((n, n, 2, 2)) + 1j * rng.standard_normal((n, n, 2, 2)))
+            hr['jones_focus_2048_Q2_us'] = 1e6 * host_time(lambda: rpol.jones_adapter(rprop.focus)(Jh, 2))
+            n, m = 1024, 256
+            rex = rprop.prepare_executor(10.0 / n, (n, n), 0.55 * 100 / 10 / 2, (m, m), 0.55, 100.0, kind='mdft')
+            Jm = Jh[:n, :n].copy()
+            hr['jones_focus_dft_1024_256_us'] = 1e6 * host_time(lambda: rpol.jones_adapter(rprop.focus_dft)(Jm, rex))
+            Kh = Jh[::-1].copy()
+            th = rng.uniform(-np.pi, np.pi, Jh.shape[:2])
+            hr['matmul_2048_us'] = 1e6 * host_time(lambda: Jh @ Kh)
+            hr['vector_vortex_retarder_2048_us'] = 1e6 * host_time(lambda: rpol.vector_vortex_retarder(2, th.copy()))
+            hr['jones_to_mueller_2048_us'] = 1e6 * host_time(lambda: rpol.jones_to_mueller(Jh))
         res['reference_host_fp64'] = hr
     line = json.dumps(res)
     print(line)

@@ -15,49 +15,20 @@ name, power limit and current and maximum SM clocks are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import warnings
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
+
 SIZES = (512, 2048)
 LEG_NS = list(range(41))
 XY_MNS = [(m, n) for m in range(11) for n in range(11) if m + n <= 10]
 assert len(XY_MNS) == 66
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e-3
-
-
-def host_time(fn):
-    t0 = time.perf_counter()
-    fn()
-    return time.perf_counter() - t0
 
 
 def grid(N):
@@ -70,11 +41,9 @@ def coefficients(k, seed):
 
 
 def reference_times(N, nms):
-    ref = os.path.join(ROOT, 'oracle', '_ref')
-    if not os.path.isdir(os.path.join(ref, 'prysm')):
+    if not reference.installed():
         return None
-    sys.path.insert(0, ref)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         from prysm import polynomials as p
         config.precision = 64
@@ -86,10 +55,6 @@ def reference_times(N, nms):
                     'zernike_nm_der_xy_seq_s': host_time(lambda: p.zernike_nm_der_xy_seq(nms, x, y)),
                     'zernike_sum_der_xy_s': host_time(lambda: p.zernike_sum_der_xy(zc, nms, x, y)),
                     'xy_sum_der_xy_s': host_time(lambda: p.xy_sum_der_xy(xc, XY_MNS, x, y))}
-    finally:
-        sys.path.remove(ref)
-        for name in [m for m in sys.modules if m.split('.')[0] == 'prysm']:
-            del sys.modules[name]
 
 
 def main():
@@ -111,13 +76,13 @@ def main():
         for dt, name in ((torch.float64, 'fp64'), (torch.float32, 'fp32')):
             x, y = (torch.as_tensor(v).to('cuda', dt) for v in (xh, yh))
             es, px = x.element_size(), N * N
-            row[f'legendre_seq_{name}_s'] = timed(lambda: P.legendre_seq(LEG_NS, x), args.iters)
+            row[f'legendre_seq_{name}_s'] = timed(lambda: P.legendre_seq(LEG_NS, x), args.iters)[0]
             row[f'legendre_seq_{name}_floor_s'] = (len(LEG_NS) + 1) * px * es / HBM_BYTES_PER_S
-            row[f'zernike_nm_der_xy_seq_{name}_s'] = timed(lambda: P.zernike_nm_der_xy_seq(nms, x, y), args.iters)
+            row[f'zernike_nm_der_xy_seq_{name}_s'] = timed(lambda: P.zernike_nm_der_xy_seq(nms, x, y), args.iters)[0]
             row[f'zernike_nm_der_xy_seq_{name}_floor_s'] = (2 * len(nms) + 2) * px * es / HBM_BYTES_PER_S
-            row[f'zernike_sum_der_xy_{name}_s'] = timed(lambda: P.zernike_sum_der_xy(zc, nms, x, y), args.iters)
+            row[f'zernike_sum_der_xy_{name}_s'] = timed(lambda: P.zernike_sum_der_xy(zc, nms, x, y), args.iters)[0]
             row[f'zernike_sum_der_xy_{name}_floor_s'] = 5 * px * es / HBM_BYTES_PER_S
-            row[f'xy_sum_der_xy_{name}_s'] = timed(lambda: P.xy_sum_der_xy(xc, XY_MNS, x, y), args.iters)
+            row[f'xy_sum_der_xy_{name}_s'] = timed(lambda: P.xy_sum_der_xy(xc, XY_MNS, x, y), args.iters)[0]
             row[f'xy_sum_der_xy_{name}_floor_s'] = 3 * px * es / HBM_BYTES_PER_S
             del x, y
             torch.cuda.empty_cache()

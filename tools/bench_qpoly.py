@@ -14,48 +14,19 @@ maximum SM clocks are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import warnings
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
+
 SIZES = (512, 2048)
 NMS = [(n, m) for m in range(-6, 7) for n in range(9)]          # 13 x 9 = 117 modes
 assert len(NMS) == 117
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e-3
-
-
-def host_time(fn):
-    t0 = time.perf_counter()
-    fn()
-    return time.perf_counter() - t0
 
 
 def polar(N):
@@ -70,11 +41,9 @@ def coefficients():
 
 
 def reference_times(N):
-    ref = os.path.join(ROOT, 'oracle', '_ref')
-    if not os.path.isdir(os.path.join(ref, 'prysm')):
+    if not reference.installed():
         return None
-    sys.path.insert(0, ref)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         from prysm.polynomials import qpoly as q
         config.precision = 64
@@ -85,10 +54,6 @@ def reference_times(N):
             return {'Q2d_seq_s': host_time(lambda: q.Q2d_seq(NMS, r, t)),
                     'Q2d_der_xy_seq_s': host_time(lambda: q.Q2d_der_xy_seq(NMS, x, y)),
                     'compute_z_zprime_Q2d_s': host_time(lambda: q.compute_z_zprime_Q2d(cm0, ams, bms, r, t))}
-    finally:
-        sys.path.remove(ref)
-        for name in [m for m in sys.modules if m.split('.')[0] == 'prysm']:
-            del sys.modules[name]
 
 
 def main():
@@ -109,11 +74,12 @@ def main():
             x, y, r, t = (torch.as_tensor(v).to('cuda', dt) for v in (xh, yh, rh, th))
             es = x.element_size()
             cm0, ams, bms = Q.Q2d_nm_c_to_a_b(NMS, coefficients())
-            row[f'Q2d_seq_{name}_s'] = timed(lambda: Q.Q2d_seq(NMS, r, t), args.iters)
+            row[f'Q2d_seq_{name}_s'] = timed(lambda: Q.Q2d_seq(NMS, r, t), args.iters)[0]
             row[f'Q2d_seq_{name}_floor_s'] = (len(NMS) + 2) * N * N * es / HBM_BYTES_PER_S
-            row[f'Q2d_der_xy_seq_{name}_s'] = timed(lambda: Q.Q2d_der_xy_seq(NMS, x, y), args.iters)
+            row[f'Q2d_der_xy_seq_{name}_s'] = timed(lambda: Q.Q2d_der_xy_seq(NMS, x, y), args.iters)[0]
             row[f'Q2d_der_xy_seq_{name}_floor_s'] = (2 * len(NMS) + 2) * N * N * es / HBM_BYTES_PER_S
-            row[f'compute_z_zprime_Q2d_{name}_s'] = timed(lambda: Q.compute_z_zprime_Q2d(cm0, ams, bms, r, t), args.iters)
+            row[f'compute_z_zprime_Q2d_{name}_s'] = timed(lambda: Q.compute_z_zprime_Q2d(cm0, ams, bms, r, t),
+                                                          args.iters)[0]
             row[f'compute_z_zprime_Q2d_{name}_floor_s'] = 5 * N * N * es / HBM_BYTES_PER_S
             del x, y, r, t
             torch.cuda.empty_cache()

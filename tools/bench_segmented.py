@@ -12,16 +12,17 @@ accumulated into), plus every segment's mask and every unique basis read once; t
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, timed  # noqa: E402
+
 NMS = [(0, 0), (1, 1), (1, -1), (2, 0), (2, -2), (2, 2), (3, -1), (3, 1), (3, -3), (3, 3), (4, 0)]
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
 L2_BYTES = 50 * 2 ** 20
 
 
@@ -40,30 +41,7 @@ CASES = {   # name -> (n, diameter, rings, segment flat-to-flat, gap, exclude)
 }
 
 
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def time_events(fn, iters):
-    import torch
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / iters * 1e3        # us
-
-
-def run_case(name, iters, precision, reference):
+def run_case(name, iters, precision, with_reference):
     import torch
     import prysm_b200 as pb
     n, diameter, rings, diam, gap, exclude = CASES[name]
@@ -84,8 +62,8 @@ def run_case(name, iters, precision, reference):
     c = pb.asdevice(np.random.default_rng(1).standard_normal((nseg, len(NMS))) * 1e-2)
     out = torch.zeros_like(cha.x)
     g = torch.randn_like(cha.x)
-    us_fwd = time_events(lambda: cha.compose_opd(c, out=out), iters)
-    us_adj = time_events(lambda: cha.compose_opd_adjoint(g), iters)
+    us_fwd = timed(lambda: cha.compose_opd(c, out=out), iters, warm=5)[0] * 1e6
+    us_adj = timed(lambda: cha.compose_opd_adjoint(g), iters, warm=5)[0] * 1e6
     esize = cha.x.element_size()
     nunique = len({b.data_ptr() for b in cha.opd_bases})
     base_bytes = cha._bases.numel() * esize
@@ -98,27 +76,24 @@ def run_case(name, iters, precision, reference):
                compose_bytes=fwd_bytes, compose_GBps=fwd_bytes / us_fwd / 1e3,
                compose_hbm_bound_us=fwd_bytes / HBM_BYTES_PER_S * 1e6, adjoint_GBps=adj_bytes / us_adj / 1e3,
                bound='memory (bytes / HBM bandwidth; under 1 flop per byte)')
-    if reference:
-        ref = os.environ.get('PRYSM_REFERENCE', os.path.join(ROOT, 'oracle', '_ref'))
-        sys.path.insert(0, ref)
-        from prysm.conf import config
-        from prysm import segmented as S, polynomials as P, coordinates as C
-        config.precision = precision
-        xr, yr = C.make_xy_grid(n, diameter=diameter)
-        t0 = time.perf_counter()
-        rc = S.CompositeHexagonalAperture(xr, yr, rings, diam, gap, exclude=exclude)
-        res['reference_constructor_s'] = time.perf_counter() - t0
-        t0 = time.perf_counter()
-        rc.prepare_opd_bases(P.zernike_nm_seq, NMS)
-        res['reference_prepare_opd_bases_s'] = time.perf_counter() - t0
-        ch = c.cpu().numpy()
-        rc.compose_opd(ch)
-        t0 = time.perf_counter()
-        for _ in range(3):
+    if with_reference:
+        with reference.loaded():
+            from prysm.conf import config
+            from prysm import segmented as S, polynomials as P, coordinates as C
+            config.precision = precision
+            xr, yr = C.make_xy_grid(n, diameter=diameter)
+            t0 = time.perf_counter()
+            rc = S.CompositeHexagonalAperture(xr, yr, rings, diam, gap, exclude=exclude)
+            res['reference_constructor_s'] = time.perf_counter() - t0
+            t0 = time.perf_counter()
+            rc.prepare_opd_bases(P.zernike_nm_seq, NMS)
+            res['reference_prepare_opd_bases_s'] = time.perf_counter() - t0
+            ch = c.cpu().numpy()
             rc.compose_opd(ch)
-        res['reference_compose_opd_ms'] = (time.perf_counter() - t0) / 3 * 1e3
-        config.precision = 64
-        sys.path.remove(ref)
+            t0 = time.perf_counter()
+            for _ in range(3):
+                rc.compose_opd(ch)
+            res['reference_compose_opd_ms'] = (time.perf_counter() - t0) / 3 * 1e3
     pb.config.precision = 64
     return res
 

@@ -16,47 +16,18 @@ current and maximum SM clocks are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import warnings
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
+
 N = 2048
 M_RAW, N_RAW = 3072, 4096
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e-3
-
-
-def host_time(fn):
-    t0 = time.perf_counter()
-    fn()
-    return time.perf_counter() - t0
 
 
 def main():
@@ -65,17 +36,20 @@ def main():
     ap.add_argument('--no-reference', action='store_true')
     ap.add_argument('--out')
     args = ap.parse_args()
+    if args.no_reference:
+        return run(args, None)
+    with reference.loaded():
+        from prysm import bayer as rbayer, detector as rdet
+        return run(args, (rdet, rbayer))
+
+
+def run(args, ref):
+    """Every case, each beside the reference modules' call (ref: detector, bayer) when ref is not None."""
     import torch
     import prysm_b200 as pb
     if not torch.cuda.is_available():
         raise SystemExit('bench_sensor needs a CUDA device')
     rng = np.random.default_rng(0)
-    ref = None
-    if not args.no_reference:
-        sys.path.insert(0, os.path.join(ROOT, 'oracle', '_ref'))
-        from prysm import bayer as rbayer, detector as rdet
-        ref = (rdet, rbayer)
-
     results = []
 
     def record(name, seconds, nbytes, ref_fn=None):
@@ -102,7 +76,7 @@ def main():
                     continue
                 cam = pb.detector.Detector(0.5, 3.0, 100, 60_000, 15.0, 12, 1.0, prnu=prnu_d, dcnu=dcnu_d,
                                            lut=lut_d if with_lut else None)
-                t = timed(lambda: cam.expose(aerial_d, frames=frames), args.iters)
+                t = timed(lambda: cam.expose(aerial_d, frames=frames), args.iters)[0]
                 out_bytes = 4 if with_lut else 2
                 nbytes = 3 * N * N * 4 + frames * N * N * out_bytes
                 ref_fn = None
@@ -117,20 +91,20 @@ def main():
     pb.config.precision = 32
     for name, raw in (('float32', raw_f32), ('uint16', raw_u16)):
         d = pb.asdevice(raw)
-        t = timed(lambda: pb.bayer.demosaic_malvar(d, 'rggb'), args.iters)
+        t = timed(lambda: pb.bayer.demosaic_malvar(d, 'rggb'), args.iters)[0]
         nbytes = raw.nbytes + M_RAW * N_RAW * 3 * 4
         ref_fn = None
         if ref is not None:
             ref_fn = (lambda raw=raw: ref[1].demosaic_malvar(raw, 'rggb'))
         record(f'demosaic_malvar_{M_RAW}x{N_RAW}_{name}', t, nbytes, ref_fn)
     d = pb.asdevice(raw_f32)
-    t = timed(lambda: pb.bayer.wb_prescale(d, 1.0, 1.0, 1.0, 1.0, safe=True, saturation=1e9), args.iters)
+    t = timed(lambda: pb.bayer.wb_prescale(d, 1.0, 1.0, 1.0, 1.0, safe=True, saturation=1e9), args.iters)[0]
     record(f'wb_prescale_safe_{M_RAW}x{N_RAW}_float32', t, 3 * raw_f32.nbytes,
            None if ref is None else (lambda: ref[1].wb_prescale(raw_f32.copy(), 1.9, 1.0, 1.0, 1.6, safe=True,
                                                                  saturation=4000)))
     planes = [pb.asdevice((rng.random((M_RAW, N_RAW))).astype(np.float32)) for _ in range(4)]
     out = torch.empty((M_RAW, N_RAW), dtype=torch.float32, device=planes[0].device)
-    t = timed(lambda: pb.bayer.composite_bayer(*planes, output=out), args.iters)
+    t = timed(lambda: pb.bayer.composite_bayer(*planes, output=out), args.iters)[0]
     hp = [p.cpu().numpy() for p in planes]
     record(f'composite_bayer_{M_RAW}x{N_RAW}_float32', t, 2 * raw_f32.nbytes,
            None if ref is None else (lambda: ref[1].composite_bayer(*hp)))

@@ -16,55 +16,24 @@ maximum SM clocks are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import warnings
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
+
 CONFIGS = ((512, 16), (2048, 64))
 DX, PITCH_SAMPLES, EFL, WVL = 0.01, 32, 20.0, 0.55
 
 
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e-3
-
-
-def host_time(fn):
-    t0 = time.perf_counter()
-    fn()
-    return time.perf_counter() - t0
-
-
 def reference_screen_times(N, n, pitch):
-    ref = os.path.join(ROOT, 'oracle', '_ref')
-    if not os.path.isdir(os.path.join(ref, 'prysm')):
+    if not reference.installed():
         return None
-    sys.path.insert(0, ref)
-    try:
+    with reference.loaded():
         from prysm.conf import config
         from prysm.coordinates import make_xy_grid
         from prysm.geometry import circle
@@ -76,10 +45,6 @@ def reference_screen_times(N, n, pitch):
             return {'rectangle': host_time(lambda: shack_hartmann(pitch, n, EFL, WVL, x, y)),
                     'circle_shift': host_time(lambda: shack_hartmann(pitch, n, EFL, WVL, x, y, aperture=circle,
                                                                      shift=True))}
-    finally:
-        sys.path.remove(ref)
-        for name in [m for m in sys.modules if m.split('.')[0] == 'prysm']:
-            del sys.modules[name]
 
 
 def main():
@@ -100,25 +65,25 @@ def main():
         for prec in (64, 32):
             pb.config.precision = prec
             x, y = pb.coordinates.make_xy_grid(N, dx=DX)
-            row[f'screen_rect_fp{prec}_s'] = timed(lambda: S.shack_hartmann(pitch, n, EFL, WVL, x, y), args.iters)
+            row[f'screen_rect_fp{prec}_s'] = timed(lambda: S.shack_hartmann(pitch, n, EFL, WVL, x, y), args.iters)[0]
             plan = S._plan_for(pitch, n, x, y, False)
             row[f'screen_rect_kernel_fp{prec}_s'] = timed(lambda: S._screen(plan, pitch, EFL, WVL, x, y, S.rectangle, None),
-                                                          args.iters)
+                                                          args.iters)[0]
             row[f'screen_bytes_fp{prec}'] = x.numel() * x.element_size() * 4      # x, y read; complex written
             row[f'screen_circle_shift_fp{prec}_s'] = timed(
-                lambda: S.shack_hartmann(pitch, n, EFL, WVL, x, y, aperture=pb.geometry.circle, shift=True), args.iters)
+                lambda: S.shack_hartmann(pitch, n, EFL, WVL, x, y, aperture=pb.geometry.circle, shift=True), args.iters)[0]
             sh = S.ShackHartmann(pitch, n, EFL, WVL, x, y, shift=True)
             wave = pb.Wavefront(torch.ones_like(x).to(pb.config.complex_dtype), WVL, DX)
-            row[f'forward_model_fp{prec}_s'] = timed(lambda: sh.forward_model(wave), args.iters)
+            row[f'forward_model_fp{prec}_s'] = timed(lambda: sh.forward_model(wave), args.iters)[0]
         pb.config.precision = 64
         x, y = pb.coordinates.make_xy_grid(N, dx=DX)
         sh = S.ShackHartmann(pitch, n, EFL, WVL, x, y, shift=True)
         I = sh.forward_model(pb.Wavefront(torch.ones_like(x).to(torch.complex128), WVL, DX)).data
         frame = np.round(I.cpu().numpy() / float(I.max()) * 60000).astype(np.uint16)
         stack = pb.asdevice(np.repeat(frame[None], 16, axis=0))
-        t = timed(lambda: sh.centroids(stack, 0.0), args.iters)
+        t = timed(lambda: sh.centroids(stack, 0.0), args.iters)[0]
         row['centroids_16_u16_s'] = t
-        row['centroids_16_u16_threshold_s'] = timed(lambda: sh.centroids(stack, 0.1), args.iters)
+        row['centroids_16_u16_threshold_s'] = timed(lambda: sh.centroids(stack, 0.1), args.iters)[0]
         row['centroids_16_u16_bytes'] = stack.numel() * 2
         row['centroids_16_u16_bound_s'] = stack.numel() * 2 / HBM_BYTES_PER_S
         # the reconstructor of Noll 2-11 over the full grid (tilt, focus, astigmatism, coma, trefoil, spherical)
@@ -131,8 +96,8 @@ def main():
         sh.calibrate(modes, 1.0)
         s1 = sh.slopes(I)
         s16 = s1[None].repeat(16, 1, 1, 1).contiguous()
-        row['reconstruct_1_s'] = timed(lambda: sh.reconstruct(s1), args.iters)
-        row['reconstruct_16_s'] = timed(lambda: sh.reconstruct(s16), args.iters)
+        row['reconstruct_1_s'] = timed(lambda: sh.reconstruct(s1), args.iters)[0]
+        row['reconstruct_16_s'] = timed(lambda: sh.reconstruct(s16), args.iters)[0]
         row['valid_subapertures'] = int(sh.valid.sum())
         if not args.no_reference:
             row['reference_screen_s'] = reference_screen_times(N, n, pitch)

@@ -6,25 +6,12 @@ import os
 import sys
 
 import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import prysm_b200 as pb  # noqa: E402
-from prysm_b200 import _ops, coordinates as C, geometry as G, polynomials as Z, propagation as P  # noqa: E402
-
-
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / reps
+from benchlib import timed  # noqa: E402
+from prysm_b200 import coordinates as C, geometry as G, polynomials as Z, propagation as P  # noqa: E402
 
 
 for prec in (32, 64):
@@ -35,18 +22,18 @@ for prec in (32, 64):
     r, t = C.cart_to_polar(x, y)
     nms = [Z.noll_to_nm(j) for j in range(2, 38)]
     coefs = np.random.default_rng(1).normal(0, 30, 36)
-    us = timeit(lambda: C.make_xy_grid(N, diameter=2.0))
+    us = timed(lambda: C.make_xy_grid(N, diameter=2.0), 20)[0] * 1e6
     print(f'[p{prec}] make_xy_grid {N}^2: {us:.1f} us ({2 * N * N * b / us / 1e3:.0f} GB/s written)')
-    us = timeit(lambda: C.cart_to_polar(x, y))
+    us = timed(lambda: C.cart_to_polar(x, y), 20)[0] * 1e6
     print(f'[p{prec}] cart_to_polar {N}^2: {us:.1f} us ({4 * N * N * b / us / 1e3:.0f} GB/s r+w)')
-    us = timeit(lambda: G.circle(1.0, r))
+    us = timed(lambda: G.circle(1.0, r), 20)[0] * 1e6
     print(f'[p{prec}] circle {N}^2: {us:.1f} us')
-    us = timeit(lambda: Z.zernike_nm_seq(nms, r, t))
+    us = timed(lambda: Z.zernike_nm_seq(nms, r, t), 20)[0] * 1e6
     print(f'[p{prec}] zernike_nm_seq 36 modes {N}^2: {us:.1f} us ({38 * N * N * b / us / 1e3:.0f} GB/s r+w)')
-    us = timeit(lambda: Z.zernike_sum(coefs, nms, x, y))
+    us = timed(lambda: Z.zernike_sum(coefs, nms, x, y), 20)[0] * 1e6
     print(f'[p{prec}] zernike_sum 36 modes {N}^2 (coefficients -> OPD, no basis): {us:.1f} us ({3 * N * N * b / us / 1e3:.0f} GB/s r+w)')
     basis = Z.zernike_nm_seq(nms, r, t)
-    us = timeit(lambda: Z.sum_of_2d_modes(basis, coefs))
+    us = timed(lambda: Z.sum_of_2d_modes(basis, coefs), 20)[0] * 1e6
     print(f'[p{prec}] sum_of_2d_modes over the stored 36-mode basis {N}^2: {us:.1f} us ({37 * N * N * b / us / 1e3:.0f} GB/s r+w)')
     amp = G.circle(1.0, r)
 
@@ -54,6 +41,6 @@ for prec in (32, 64):
         opd = Z.zernike_sum(coefs, nms, x, y)
         return P.Wavefront.from_amp_and_phase(amp, opd, 0.6328, 2.0 / N).focus(100.0, Q=2)
     if prec == 32:
-        us = timeit(model)
+        us = timed(model, 20)[0] * 1e6
         print(f'[p{prec}] coefficients -> OPD -> pupil -> focus {N}^2 -> {2 * N}^2: {us:.1f} us')
     del basis

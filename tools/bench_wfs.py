@@ -15,45 +15,16 @@ card name, power limit and current SM clock are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import types
 import warnings
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f'unknown ({e})'
-
-
-def timed(fn, iters):
-    import torch
-    fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) * 1e3 / iters       # us per call
-
-
-def host_once(fn):
-    t0 = time.perf_counter()
-    fn()
-    return (time.perf_counter() - t0) * 1e6
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
+import reference  # noqa: E402
+from benchlib import HBM_BYTES_PER_S, card, host_time, timed  # noqa: E402
 
 
 def cases(m, xp, asarray):
@@ -100,7 +71,7 @@ def main():
     calls, nmodes = cases(eng, None, pb.asdevice)
     res = {'card': card(), 'precision': 32, 'iters': args.iters, 'modes_V20': nmodes, 'engine_us': {}, 'reference_us': {}}
     for k, fn in calls.items():
-        res['engine_us'][k] = timed(fn, args.iters)
+        res['engine_us'][k] = timed(fn, args.iters, warm=1)[0] * 1e6
     N = 2048
     for k, nbytes in (('psi13_2048_f32', 13 * N * N * 4 + N * N * 4), ('psi13_2048_u16', 13 * N * N * 2 + N * N * 8)):
         bound = nbytes / HBM_BYTES_PER_S * 1e6
@@ -112,12 +83,12 @@ def main():
     if not args.no_reference:
         sys.path.insert(0, os.path.join(ROOT, 'tests'))
         import wfs_oracle as O
-        m = O.reference_modules(os.path.join(ROOT, 'oracle', '_ref'))
-        with warnings.catch_warnings():
+        with reference.loaded(also=('skimage',)), warnings.catch_warnings():
+            m = O.reference_modules()
             warnings.simplefilter('ignore')
             ref_calls, _ = cases(m, np, np.asarray)
             for k, fn in ref_calls.items():
-                res['reference_us'][k] = host_once(fn)
+                res['reference_us'][k] = host_time(fn) * 1e6
         res['speedup'] = {k: res['reference_us'][k] / res['engine_us'][k] for k in res['reference_us']}
     line = json.dumps(res)
     print(line)
