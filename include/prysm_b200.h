@@ -692,6 +692,50 @@ int pb_tensor_sum(pb_handle_t h, int dtype, int basis, const void* x, const void
                   int separable, int k, const int* m_host, const int* n_host, const double* coefs_host, double x_norm,
                   double y_norm, void* z, void* dzdx, void* dzdy, void* stream);
 
+/* ---- Thin-film stacks (prysm/thinfilm.py multilayer_stack_rt, prysm/x/coatings stack.py and diff.py) ---------------
+ * One thread per sample; the transfer-matrix chain runs in fp64 registers whatever dtype is, and outputs are rounded
+ * once to dtype (PB_C64: complex64 / float32, PB_C128: complex128 / float64).  Layers are ambient side first.
+ * Operands (HOST array in[PB_TF_NOPS] of device pointers, all fp64): wavelength and angle of incidence (radians) real,
+ *   ambient index, substrate index and the per-layer index complex128, the per-layer thickness real.  Each is indexed
+ *   over a collapsed calculation shape of ndim <= 4 dims (HOST shape[ndim], outermost first; count = its product):
+ *   operand q reads element  sum_j idx_j strides[5 q + j]  (+ layer * strides[5 q + 4] for the per-layer operands),
+ *   strides in elements, 0 where it broadcasts, slots j >= ndim ignored.
+ * pb_stack_eval: the angle is theta_scale times the angle operand (pi / 180 for degrees).  Mode PB_TF_THINFILM
+ *   assembles r, t as multilayer_stack_rt (nlayers >= 1; only the r and t outputs); PB_TF_COATINGS uses the
+ *   admittance form of the coatings engine (nlayers >= 0).  flags is a bit mask of 1 << PB_TF_OUT_*; out[PB_TF_OUT_*] (HOST array of PB_TF_NOUT device pointers) is read for the bits set:
+ *   r, t, eta0, eta_sub complex (count); E, H complex and Esq = |E|^2 real (nlayers + 1, count), E and H the tangential
+ *   fields at every boundary; REFL = |r|^2, TRANS real (count); ABS real (nlayers, count) by flux telescoping.
+ *   The field outputs are staged in fp64 before t scales them: in the outputs for PB_C128, in the handle's scratch for
+ *   PB_C64.
+ * pb_stack_grad: the thickness (PB_TF_GRAD_THICKNESS) and / or index (PB_TF_GRAD_INDEX) gradient of a scalar merit whose
+ *   cotangents are the seeds (HOST array of 4 device pointers, fp64, NULL when absent): dR, dT (count), dA
+ *   (nlayers, count), dEsq (nlayers + 1, count).  E and H are the complex128 boundary fields pb_stack_eval wrote in
+ *   coatings mode.  grad: (nlayers) of dtype's real type, or (2, nlayers) thickness first when both kinds are asked.
+ *   The sample sum is per-warp partials in the handle's scratch added in a fixed order by a second launch: no atomics,
+ *   so repeated calls are bit-identical.
+ * pb_field_at_depth: E, H (complex, nz) at depths z (fp64, nz) of a stack of nlayers >= 1 at one wavelength and angle:
+ *   zb (fp64, nlayers + 1) the boundary depths, n (complex128, nlayers) the layer indices, E_b and H_b (complex128,
+ *   nlayers + 1) the boundary fields pb_stack_eval wrote for that sample. */
+typedef enum { PB_TF_THINFILM = 0, PB_TF_COATINGS = 1 } pb_tf_mode;
+typedef enum { PB_TF_POL_S = 0, PB_TF_POL_P = 1 } pb_tf_pol;
+typedef enum {
+    PB_TF_IN_WVL = 0, PB_TF_IN_THETA = 1, PB_TF_IN_N0 = 2, PB_TF_IN_NSUB = 3, PB_TF_IN_N = 4, PB_TF_IN_D = 5,
+    PB_TF_NOPS = 6
+} pb_tf_operand;
+typedef enum {
+    PB_TF_OUT_R = 0, PB_TF_OUT_T = 1, PB_TF_OUT_E = 2, PB_TF_OUT_H = 3, PB_TF_OUT_REFL = 4, PB_TF_OUT_TRANS = 5,
+    PB_TF_OUT_ABS = 6, PB_TF_OUT_ESQ = 7, PB_TF_OUT_ETA0 = 8, PB_TF_OUT_ETASUB = 9, PB_TF_NOUT = 10
+} pb_tf_output;
+typedef enum { PB_TF_GRAD_THICKNESS = 1, PB_TF_GRAD_INDEX = 2 } pb_tf_grad_kind;
+int pb_stack_eval(pb_handle_t h, int dtype, int mode, int pol, int flags, int nlayers, int ndim, const long long* shape,
+                  const long long* strides, const void* const* in, double theta_scale, void* const* out, void* stream);
+int pb_stack_grad(pb_handle_t h, int dtype, int pol, int kinds, int nlayers, int ndim, const long long* shape,
+                  const long long* strides, const void* const* in, const void* E, const void* H, const void* const* seeds,
+                  void* grad, void* stream);
+int pb_field_at_depth(pb_handle_t h, int dtype, int pol, int nlayers, const void* z, long long nz, const void* zb,
+                      const void* n, double n0_re, double n0_im, double wvl, double theta0, const void* E_b,
+                      const void* H_b, void* E, void* H, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -135,6 +135,11 @@ SIGNATURES = {
     'pb_xy_seq': (_i, [_vp, _i, _vp, _vp, _ll, _ll, _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), _vp, _vp]),
     'pb_tensor_sum': (_i, [_vp, _i, _i, _vp, _vp, _ll, _ll, _i, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_d), _d, _d,
                            _vp, _vp, _vp, _vp]),
+    'pb_stack_eval': (_i, [_vp, _i, _i, _i, _i, _i, _i, C.POINTER(_ll), C.POINTER(_ll), C.POINTER(_vp), _d,
+                           C.POINTER(_vp), _vp]),
+    'pb_stack_grad': (_i, [_vp, _i, _i, _i, _i, _i, C.POINTER(_ll), C.POINTER(_ll), C.POINTER(_vp), _vp, _vp,
+                           C.POINTER(_vp), _vp, _vp]),
+    'pb_field_at_depth': (_i, [_vp, _i, _i, _i, _vp, _ll, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _vp, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -160,6 +165,13 @@ POLY_VALUE, POLY_DER, POLY_VALUE_DER = range(3)
 POLY_NMAX = 120
 CLENSHAW_JMAX = 8
 TSUM_MONOMIAL, TSUM_CHEBY1 = range(2)
+TF_THINFILM, TF_COATINGS = range(2)
+TF_POL_S, TF_POL_P = range(2)
+TF_IN_WVL, TF_IN_THETA, TF_IN_N0, TF_IN_NSUB, TF_IN_N, TF_IN_D, TF_NOPS = range(7)
+(TF_OUT_R, TF_OUT_T, TF_OUT_E, TF_OUT_H, TF_OUT_REFL, TF_OUT_TRANS, TF_OUT_ABS, TF_OUT_ESQ, TF_OUT_ETA0, TF_OUT_ETASUB,
+ TF_NOUT) = range(11)
+TF_GRAD_THICKNESS, TF_GRAD_INDEX = 1, 2
+TF_DIMS = 4
 
 
 def load_library(path=LIB_PATH):

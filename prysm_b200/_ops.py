@@ -1361,6 +1361,109 @@ def tensor_sum(basis, coefs, ms, ns, x, y, shape, separable, want_der, x_norm=1.
     return z, dx, dy
 
 
+def tf_layout(ops):
+    """(broadcast calculation shape, collapsed shape, (TF_NOPS * 5) int64 host strides) of the six thin-film operands
+    (wavelength, angle, ambient index, substrate index, layer index, layer thickness: fp64 / complex128 device tensors,
+    the last two with a leading layer axis).  Dims that are contiguous in every operand are merged; a broadcast that
+    still needs more than TF_DIMS dims is refused with ValueError."""
+    calc = [tuple(t.shape[1:]) if q in (capi.TF_IN_N, capi.TF_IN_D) else tuple(t.shape) for q, t in enumerate(ops)]
+    bshape = np.broadcast_shapes(*calc)
+    nd = len(bshape)
+    st = []
+    for q, (t, c) in enumerate(zip(ops, calc)):
+        tst = t.stride()[1:] if q in (capi.TF_IN_N, capi.TF_IN_D) else t.stride()
+        pad = nd - len(c)
+        st.append([0 if j < pad or c[j - pad] == 1 else tst[j - pad] for j in range(nd)])
+    dims, cst = [], [[] for _ in ops]
+    for j in range(nd):
+        if bshape[j] == 1:
+            continue
+        if dims and all(s[-1] == st[q][j] * bshape[j] for q, s in enumerate(cst)):
+            dims[-1] *= bshape[j]
+            for q, s in enumerate(cst):
+                s[-1] = st[q][j]
+            continue
+        dims.append(bshape[j])
+        for q, s in enumerate(cst):
+            s.append(st[q][j])
+    if len(dims) > capi.TF_DIMS:
+        raise ValueError(f'thin-film operands broadcast to {bshape}, which needs {len(dims)} dims after merging the '
+                         f'contiguous ones; at most {capi.TF_DIMS} are supported')
+    strides = np.zeros((capi.TF_NOPS, capi.TF_DIMS + 1), dtype=np.int64)
+    for q, s in enumerate(cst):
+        strides[q, :len(s)] = s
+        if q in (capi.TF_IN_N, capi.TF_IN_D) and ops[q].shape[0] != 1:
+            strides[q, capi.TF_DIMS] = ops[q].stride(0)
+    return bshape, dims, strides
+
+
+def tf_nlayers(ops):
+    """layers of the thin-film operands: the index and thickness layer axes broadcast"""
+    return max(int(ops[capi.TF_IN_N].shape[0]), int(ops[capi.TF_IN_D].shape[0])) \
+        if min(ops[capi.TF_IN_N].shape[0], ops[capi.TF_IN_D].shape[0]) else 0
+
+
+def _tf_args(ops):
+    bshape, dims, strides = tf_layout(ops)
+    shp = np.asarray(dims if dims else [1], dtype=np.int64)
+    ins = (C.c_void_p * capi.TF_NOPS)(*[t.data_ptr() for t in ops])
+    keep = (shp, strides, ins)
+    return bshape, len(dims), shp.ctypes.data_as(C.POINTER(C.c_longlong)), \
+        strides.ctypes.data_as(C.POINTER(C.c_longlong)), C.cast(ins, C.POINTER(C.c_void_p)), keep
+
+
+def stack_eval(mode, pol, ops, outputs, rdtype, theta_scale=1.0):
+    """{TF_OUT_* code: device array} for the codes in `outputs`, from one pb_stack_eval launch: r, t, eta0, eta_sub
+    complex of the broadcast shape, E, H, Esq (N + 1, *shape), REFL, TRANS (shape), ABS (N, *shape), in rdtype's
+    precision."""
+    nlayers = tf_nlayers(ops)
+    bshape, nd, shp, stp, inp, keep = _tf_args(ops)
+    cdtype = _CPLX_OF[rdtype]
+    lead = {capi.TF_OUT_E: nlayers + 1, capi.TF_OUT_H: nlayers + 1, capi.TF_OUT_ESQ: nlayers + 1,
+            capi.TF_OUT_ABS: nlayers}
+    cplx = (capi.TF_OUT_R, capi.TF_OUT_T, capi.TF_OUT_E, capi.TF_OUT_H, capi.TF_OUT_ETA0, capi.TF_OUT_ETASUB)
+    dev = ops[0].device
+    res = {}
+    for code in outputs:
+        shape = ((lead[code],) if code in lead else ()) + tuple(bshape)
+        res[code] = torch.empty(shape, dtype=cdtype if code in cplx else rdtype, device=dev)
+    live = [q for q in res if res[q].numel()]        # an empty output (no layers, or no samples) is not written
+    if not live:
+        return res
+    outs = (C.c_void_p * capi.TF_NOUT)(*[res[q].data_ptr() if q in live else None for q in range(capi.TF_NOUT)])
+    flags = sum(1 << q for q in live)
+    _call(lib.pb_stack_eval, ops[0], _CODE[rdtype], int(mode), int(pol), flags, nlayers, nd, shp, stp, inp,
+          float(theta_scale), C.cast(outs, C.POINTER(C.c_void_p)))
+    return res
+
+
+def stack_grad(pol, kinds, ops, E, H, seeds, rdtype):
+    """(N,) thickness or index gradient, or (2, N) both, summed over the samples (pb_stack_grad).  E, H: the complex128
+    boundary fields of stack_eval; seeds: dR, dT, dA, dEsq as contiguous fp64 device arrays of the full shapes, or
+    None."""
+    nlayers = tf_nlayers(ops)
+    bshape, nd, shp, stp, inp, keep = _tf_args(ops)
+    both = kinds == capi.TF_GRAD_THICKNESS | capi.TF_GRAD_INDEX
+    grad = torch.empty(((2,) if both else ()) + (nlayers,), dtype=rdtype, device=E.device)
+    if nlayers == 0:
+        return grad
+    sp = (C.c_void_p * 4)(*[None if s is None else s.data_ptr() for s in seeds])
+    _call(lib.pb_stack_grad, E, _CODE[rdtype], int(pol), int(kinds), nlayers, nd, shp, stp, inp, _p(E), _p(H),
+          C.cast(sp, C.POINTER(C.c_void_p)), _p(grad))
+    return grad
+
+
+def field_at_depth(pol, z, zb, n, n0, wvl, theta0, Eb, Hb, cdtype):
+    """E, H (complex, like z) at depths z inside a stack (pb_field_at_depth): z, zb fp64, n, Eb, Hb complex128."""
+    z = z.contiguous()
+    E = torch.empty(z.shape, dtype=cdtype, device=z.device)
+    H = torch.empty_like(E)
+    n0 = complex(n0)
+    _call(lib.pb_field_at_depth, z, _CODE[cdtype], int(pol), int(n.shape[0]), _p(z), z.numel(), _p(zb), _p(n),
+          n0.real, n0.imag, float(wvl), float(theta0), _p(Eb), _p(Hb), _p(E), _p(H))
+    return E, H
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

@@ -1,0 +1,525 @@
+// Thin-film stacks on the device: the characteristic-matrix chain of prysm/thinfilm.py (multilayer_stack_rt) and of
+// prysm/x/coatings (stack.py: r, t, boundary fields, R / T / per-layer A; diff.py: thickness and index gradients), and
+// the field at arbitrary depth.
+//
+// One thread per sample (wavelength, angle, pixel).  The forward pass is one sweep from the substrate to the ambient
+// side, v_N = [1, eta_sub], v_k = M_k v_{k+1}, (B, C) = v_0, the suffix products of the reference applied to a vector;
+// the boundary fields are f_k = t v_k.  The gradient reads f_k back and runs the reverse sweep
+// vbar_{k+1} += M_k^H vbar_k, Mbar_k = vbar_k v_{k+1}^H: v_{k+1} is never recovered from v_k by inverting M_k, which
+// through an absorbing or evanescent layer would amplify the rounding error by about exp(2 |Im beta|).
+// Every operand is fp64 and all arithmetic is fp64 in registers; the outputs are rounded once to the storage type.
+#include <cmath>
+
+#include "common.cuh"
+
+namespace pb {
+
+#define PB_TF_DIMS 4
+#define PB_TF_THREADS 256
+
+struct TfOut { void* p[PB_TF_NOUT]; };
+
+struct TfOps {
+    long long shape[PB_TF_DIMS];                 // collapsed calculation shape, padded with 1 in front
+    long long st[PB_TF_NOPS][PB_TF_DIMS + 1];    // per operand: calculation strides, then the layer stride
+    const void* p[PB_TF_NOPS];
+    double theta_scale;          // radians per unit of the angle operand
+    int nlayers, pol;
+};
+
+// complex helpers with numpy's rules, so that signed zeros on the branch cut of the square root come out as the
+// reference's do: Smith's division (numpy's complex divide) and the C99 principal square root
+__device__ inline double2 tf_div(double2 a, double2 b) {
+    if (fabs(b.x) >= fabs(b.y)) {
+        const double rat = b.y / b.x, scl = 1.0 / (b.x + b.y * rat);
+        return make_double2((a.x + a.y * rat) * scl, (a.y - a.x * rat) * scl);
+    }
+    const double rat = b.x / b.y, scl = 1.0 / (b.y + b.x * rat);
+    return make_double2((a.x * rat + a.y) * scl, (a.y * rat - a.x) * scl);
+}
+
+__device__ inline double2 tf_sqrt(double2 z) {
+    if (z.x == 0.0 && z.y == 0.0) return make_double2(0.0, z.y);
+    const double t = sqrt((fabs(z.x) + hypot(z.x, z.y)) * 0.5);
+    if (z.x >= 0.0) return make_double2(t, z.y / (2.0 * t));
+    return make_double2(fabs(z.y) / (2.0 * t), copysign(t, z.y));
+}
+
+__device__ inline double2 tf_scale(double2 a, double s) { return make_double2(a.x * s, a.y * s); }
+
+// _cos_snell (thinfilm.py:75-80): sqrt(1 - sint^2) on the principal branch, negated for a real sint > 1
+__device__ inline double2 tf_cos_snell(double2 n0, double2 n, double sin0) {
+    const double2 q = tf_div(n0, n);
+    const double2 s = make_double2(q.x * sin0 - q.y * 0.0, q.x * 0.0 + q.y * sin0);
+    const double2 s2 = cmul(s, s);
+    double2 c = tf_sqrt(make_double2(1.0 - s2.x, 0.0 - s2.y));
+    if (s.y == 0.0 && s.x > 1.0) c = make_double2(-c.x, -c.y);
+    return c;
+}
+
+// tilted admittance: n / cos (p) or n cos (s)
+__device__ inline double2 tf_admittance(double2 n, double2 cost, int pol) {
+    return pol == PB_TF_POL_P ? tf_div(n, cost) : cmul(n, cost);
+}
+
+// sin and cos of a complex argument
+__device__ inline void tf_sincos(double2 b, double2* sb, double2* cb) {
+    // sincospi has no slow-path argument reduction (a call that costs registers); b.x / pi adds one rounding,
+    // a phase error of |b.x| * 1e-16
+    double s, c;
+    sincospi(b.x * M_1_PI, &s, &c);
+    // cosh and sinh of |Im b| from one expm1 (sinh stays accurate for small |Im b|, and e^|Im b| never cancels), the
+    // sign restored after: cosh is even and sinh odd.  Im b < 0 is an evanescent layer under total internal reflection.
+    const double em1 = expm1(fabs(b.y)), e = 1.0 + em1;
+    const double ch = 0.5 * (e + 1.0 / e), sh = copysign(0.5 * em1 * (1.0 + 1.0 / e), b.y);
+    *sb = make_double2(s * ch, c * sh);
+    *cb = make_double2(c * ch, -s * sh);
+}
+
+struct TfSample {
+    long long off_n, off_d;      // offsets of the per-layer operands at layer 0
+    double wvl, sin0, cos0;
+    double2 n0, nsub;
+};
+
+__device__ inline TfSample tf_sample(const TfOps& op, long long i) {
+    long long idx[PB_TF_DIMS];
+    for (int j = PB_TF_DIMS - 1; j >= 0; --j) {
+        idx[j] = i % op.shape[j];
+        i /= op.shape[j];
+    }
+    long long off[PB_TF_NOPS];
+    for (int q = 0; q < PB_TF_NOPS; ++q) {
+        off[q] = 0;
+        for (int j = 0; j < PB_TF_DIMS; ++j) off[q] += idx[j] * op.st[q][j];
+    }
+    TfSample s;
+    s.off_n = off[PB_TF_IN_N];
+    s.off_d = off[PB_TF_IN_D];
+    s.wvl = ((const double*)op.p[PB_TF_IN_WVL])[off[PB_TF_IN_WVL]];
+    sincos(((const double*)op.p[PB_TF_IN_THETA])[off[PB_TF_IN_THETA]] * op.theta_scale, &s.sin0, &s.cos0);
+    s.n0 = ((const double2*)op.p[PB_TF_IN_N0])[off[PB_TF_IN_N0]];
+    s.nsub = ((const double2*)op.p[PB_TF_IN_NSUB])[off[PB_TF_IN_NSUB]];
+    return s;
+}
+
+// layer k of a sample: index, cos theta_k, phase thickness beta, admittance eta and thickness
+struct TfLayer { double2 n, cost, beta, eta; double d; };
+
+__device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k) {
+    TfLayer L;
+    L.n = ((const double2*)op.p[PB_TF_IN_N])[s.off_n + (long long)k * op.st[PB_TF_IN_N][PB_TF_DIMS]];
+    L.d = ((const double*)op.p[PB_TF_IN_D])[s.off_d + (long long)k * op.st[PB_TF_IN_D][PB_TF_DIMS]];
+    L.cost = tf_cos_snell(s.n0, L.n, s.sin0);
+    L.beta = tf_scale(cmul(tf_scale(L.n, 2.0 * M_PI * L.d), L.cost), 1.0 / s.wvl);
+    L.eta = tf_admittance(L.n, L.cost, op.pol);
+    return L;
+}
+
+// v <- M v with M = [[cos b, -i sin b / eta], [-i eta sin b, cos b]]
+__device__ inline void tf_apply(double2 sb, double2 cb, double2 eta, double2& v0, double2& v1) {
+    const double2 mis = make_double2(sb.y, -sb.x);               // -i sin b
+    const double2 a = cadd(cmul(cb, v0), cmul(tf_div(mis, eta), v1));
+    const double2 b = cadd(cmul(cmul(mis, eta), v0), cmul(cb, v1));
+    v0 = a; v1 = b;
+}
+
+__device__ inline double tf_abs2(double2 a) { return a.x * a.x + a.y * a.y; }
+
+// fp64 staging of the field outputs before they are scaled by t: |v_k| grows like e^|Im beta| through an absorbing or
+// evanescent layer and geometrically through a long high-contrast stack, which would overflow float32.  For fp64
+// outputs the stage is the output itself.
+struct TfStage { double2* E; double2* H; double* Esq; double* A; };
+
+template <typename R, int MODE>
+__global__ void stack_eval_kernel(const TfOps op, long long count, TfOut o, TfStage sg) {
+    const int N = op.nlayers;
+    const bool fields = sg.E || sg.H || sg.Esq || sg.A;
+    PB_GRID_STRIDE(i, count) {
+        const TfSample s = tf_sample(op, i);
+        const double2 nsub = s.nsub;
+        const double2 cos_sub = tf_cos_snell(s.n0, nsub, s.sin0);
+        const double2 eta_sub = tf_admittance(nsub, cos_sub, op.pol);
+        double2 v0, v1;
+        if (MODE == PB_TF_THINFILM && op.pol == PB_TF_POL_P) { v0 = cos_sub; v1 = nsub; }
+        else { v0 = make_double2(1.0, 0.0); v1 = MODE == PB_TF_THINFILM ? cmul(nsub, cos_sub) : eta_sub; }
+        // v_k, |v_k,E|^2 and the flux differences are staged in fp64 and scaled by t or |t|^2 once v_0 (hence t)
+        // is known
+        double g_below = 0.0;
+        if (fields) {
+            const long long ob = (long long)N * count + i;
+            if (sg.E) sg.E[ob] = v0;
+            if (sg.H) sg.H[ob] = v1;
+            if (sg.Esq) sg.Esq[ob] = tf_abs2(v0);
+            g_below = cmulc(v0, v1).x;
+        }
+        for (int k = N - 1; k >= 0; --k) {
+            const TfLayer L = tf_layer(op, s, k);
+            double2 sb, cb;
+            tf_sincos(L.beta, &sb, &cb);
+            tf_apply(sb, cb, L.eta, v0, v1);
+            if (fields) {
+                const long long ok = (long long)k * count + i;
+                if (sg.E) sg.E[ok] = v0;
+                if (sg.H) sg.H[ok] = v1;
+                if (sg.Esq) sg.Esq[ok] = tf_abs2(v0);
+                const double g = cmulc(v0, v1).x;
+                if (sg.A) sg.A[ok] = g - g_below;
+                g_below = g;
+            }
+        }
+        double2 r, t;
+        if (MODE == PB_TF_THINFILM) {
+            // multilayer_stack_rt (thinfilm.py:295-311): term1 = 1 / (2 n0 cos0)
+            const double2 term1 = tf_div(make_double2(1.0, 0.0), tf_scale(s.n0, 2.0 * s.cos0));
+            const double2 a = op.pol == PB_TF_POL_P ? s.n0 : tf_scale(s.n0, s.cos0);
+            const double2 q1 = op.pol == PB_TF_POL_P ? tf_scale(v1, s.cos0) : v1;
+            const double2 aq = cmul(a, v0);
+            const double2 A00 = cmul(term1, cadd(aq, q1)), A10 = cmul(term1, csub(aq, q1));
+            r = tf_div(A10, A00);
+            t = tf_div(make_double2(1.0, 0.0), A00);
+        } else {
+            const double2 eta0 = tf_admittance(s.n0, make_double2(s.cos0, 0.0), op.pol);
+            const double2 eb = cmul(eta0, v0);
+            const double2 den = cadd(eb, v1);
+            r = tf_div(csub(eb, v1), den);
+            t = tf_div(tf_scale(eta0, 2.0), den);
+            if (o.p[PB_TF_OUT_ETA0]) ((cplx<R>*)o.p[PB_TF_OUT_ETA0])[i] = mk<R>((R)eta0.x, (R)eta0.y);
+            if (o.p[PB_TF_OUT_ETASUB]) ((cplx<R>*)o.p[PB_TF_OUT_ETASUB])[i] = mk<R>((R)eta_sub.x, (R)eta_sub.y);
+            if (o.p[PB_TF_OUT_TRANS]) ((R*)o.p[PB_TF_OUT_TRANS])[i] = (R)(eta_sub.x / eta0.x * tf_abs2(t));
+            if (fields) {
+                const double t2 = tf_abs2(t), fscale = t2 / eta0.x;
+                cplx<R>* const Eo = (cplx<R>*)o.p[PB_TF_OUT_E];
+                cplx<R>* const Ho = (cplx<R>*)o.p[PB_TF_OUT_H];
+                R* const Esq = (R*)o.p[PB_TF_OUT_ESQ];
+                R* const Ab = (R*)o.p[PB_TF_OUT_ABS];
+                for (int k = 0; k <= N; ++k) {
+                    const long long ok = (long long)k * count + i;
+                    if (Eo) { const double2 v = cmul(t, sg.E[ok]); Eo[ok] = mk<R>((R)v.x, (R)v.y); }
+                    if (Ho) { const double2 v = cmul(t, sg.H[ok]); Ho[ok] = mk<R>((R)v.x, (R)v.y); }
+                    if (Esq) Esq[ok] = (R)(sg.Esq[ok] * t2);
+                    if (Ab && k < N) Ab[ok] = (R)(sg.A[ok] * fscale);
+                }
+            }
+        }
+        if (o.p[PB_TF_OUT_R]) ((cplx<R>*)o.p[PB_TF_OUT_R])[i] = mk<R>((R)r.x, (R)r.y);
+        if (o.p[PB_TF_OUT_T]) ((cplx<R>*)o.p[PB_TF_OUT_T])[i] = mk<R>((R)t.x, (R)t.y);
+        if (o.p[PB_TF_OUT_REFL]) ((R*)o.p[PB_TF_OUT_REFL])[i] = (R)tf_abs2(r);
+    }
+}
+
+// cotangent of boundary field k from the field seeds (diff.py:204-224): flux_k = Re(E_k conj H_k) / Re(eta0) enters
+// A_k with +1 and A_{k-1} with -1
+__device__ inline void tf_field_bar(const double* dA, const double* dEsq, int N, long long count, long long i, int k,
+                                    double inv_re0, double2 E, double2 H, double2& Eb, double2& Hb) {
+    double fb = 0.0;
+    if (dA) {
+        if (k < N) fb += dA[(long long)k * count + i];
+        if (k > 0) fb -= dA[(long long)(k - 1) * count + i];
+    }
+    fb *= inv_re0;
+    Eb = tf_scale(H, fb);
+    Hb = tf_scale(E, fb);
+    if (dEsq) Eb = cadd(Eb, tf_scale(E, 2.0 * dEsq[(long long)k * count + i]));
+}
+
+__device__ inline double warp_sum(double v) {
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_down_sync(0xffffffffu, v, d);
+    return v;
+}
+
+// One warp-uniform pass per 32 samples.  Each layer's contribution is summed over the warp and added by lane 0 to the
+// warp's own slot partial[(2 k + kind) * W + warp], written on the warp's first pass: no atomics, a fixed order.
+__global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOps op, long long count, int kinds,
+                                                                    const double2* __restrict__ E, const double2* __restrict__ H,
+                                                                    const double* __restrict__ dR, const double* __restrict__ dT,
+                                                                    const double* __restrict__ dA, const double* __restrict__ dEsq,
+                                                                    double* __restrict__ partial) {
+    const int N = op.nlayers;
+    const long long W = (long long)gridDim.x * (blockDim.x / 32);
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const bool fseed = dA || dEsq;
+    for (long long base = warp * 32; base < count; base += W * 32) {
+        const bool first = base == warp * 32;
+        const bool act = base + lane < count;
+        const long long i = act ? base + lane : count - 1;
+        const TfSample s = tf_sample(op, i);
+        const double2 nsub = s.nsub;
+        const double2 eta_sub = tf_admittance(nsub, tf_cos_snell(s.n0, nsub, s.sin0), op.pol);
+        const double2 eta0 = tf_admittance(s.n0, make_double2(s.cos0, 0.0), op.pol);
+        const double inv_re0 = 1.0 / eta0.x;
+        const double2 t = E[(long long)N * count + i];                  // f_N = t [1, eta_sub]
+        const double2 inv_t = tf_div(make_double2(1.0, 0.0), t);
+        const double2 B = cmul(E[i], inv_t), C = cmul(H[i], inv_t);
+        const double2 eb = cmul(eta0, B);
+        const double2 den = cadd(eb, C);
+        const double2 r = tf_div(csub(eb, C), den);
+        // amplitude cotangents (diff.py:191-201)
+        double2 rb = make_double2(0.0, 0.0), tb = make_double2(0.0, 0.0);
+        if (dR) rb = tf_scale(r, 2.0 * dR[i]);
+        if (dT) tb = tf_scale(t, 2.0 * (eta_sub.x * inv_re0) * dT[i]);
+        // f_k = t v_k: tbar += sum_k v_k^H fbar_k
+        if (fseed) {
+            for (int k = 0; k <= N; ++k) {
+                const long long ok = (long long)k * count + i;
+                const double2 e = E[ok], hh = H[ok];
+                double2 eb2, hb2;
+                tf_field_bar(dA, dEsq, N, count, i, k, inv_re0, e, hh, eb2, hb2);
+                tb = cadd(tb, cadd(cmulc(eb2, cmul(e, inv_t)), cmulc(hb2, cmul(hh, inv_t))));
+            }
+        }
+        // (B, C) = v_0 (diff.py:162-188): holomorphic partials of r and t
+        const double2 inv_den = tf_div(make_double2(1.0, 0.0), den);
+        const double2 dr_dB = cmul(cmul(eta0, make_double2(1.0 - r.x, -r.y)), inv_den);
+        const double2 dr_dC = cmul(make_double2(-1.0 - r.x, -r.y), inv_den);
+        const double2 dt_dB = cmul(make_double2(-(t.x * eta0.x - t.y * eta0.y), -(t.x * eta0.y + t.y * eta0.x)), inv_den);
+        const double2 dt_dC = cmul(make_double2(-t.x, -t.y), inv_den);
+        double2 vb0 = cadd(cmulc(rb, dr_dB), cmulc(tb, dt_dB));
+        double2 vb1 = cadd(cmulc(rb, dr_dC), cmulc(tb, dt_dC));
+        const double2 ct = cconj(t);
+        if (fseed) {
+            double2 eb2, hb2;
+            tf_field_bar(dA, dEsq, N, count, i, 0, inv_re0, E[i], H[i], eb2, hb2);
+            vb0 = cadd(vb0, cmul(ct, eb2));
+            vb1 = cadd(vb1, cmul(ct, hb2));
+        }
+        const double2 n0sq_sin2 = tf_scale(cmul(s.n0, s.n0), s.sin0 * s.sin0);
+        for (int k = 0; k < N; ++k) {
+            const TfLayer L = tf_layer(op, s, k);
+            double2 sb, cb;
+            tf_sincos(L.beta, &sb, &cb);
+            const long long o1 = (long long)(k + 1) * count + i;
+            const double2 e1 = E[o1], h1 = H[o1];
+            const double2 w0 = cmul(e1, inv_t), w1 = cmul(h1, inv_t);       // v_{k+1}
+            // Mbar = vbar v_{k+1}^H
+            const double2 m00 = cmulc(vb0, w0), m01 = cmulc(vb0, w1), m10 = cmulc(vb1, w0), m11 = cmulc(vb1, w1);
+            // char_matrix_vjp (diff.py:22-60): c = sum conj(dM) * Mbar
+            const double2 ieta = tf_div(make_double2(1.0, 0.0), L.eta);
+            const double2 icb = make_double2(cb.y, -cb.x);                 // -i cos b
+            const double2 dB01 = cmul(icb, ieta), dB10 = cmul(icb, L.eta);
+            const double2 cbeta = csub(cadd(cmulc(m01, dB01), cmulc(m10, dB10)), cadd(cmulc(m00, sb), cmulc(m11, sb)));
+            const double2 isb = make_double2(-sb.y, sb.x);                 // i sin b
+            const double2 dE01 = cmul(isb, cmul(ieta, ieta)), dE10 = make_double2(-isb.x, -isb.y);
+            const double2 ceta = cadd(cmulc(m01, dE01), cmulc(m10, dE10));
+            double gth = 0.0, gix = 0.0;
+            if (kinds & PB_TF_GRAD_THICKNESS) {
+                // dbeta/dd = 2 pi n cos / wvl (diff.py:110, 307)
+                const double2 dbdd = tf_scale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
+                gth = cmulc(dbdd, cbeta).x;
+            }
+            if (kinds & PB_TF_GRAD_INDEX) {
+                // diff.py:328-339: dcos/dn = n0^2 sin0^2 / (n^3 cos)
+                const double2 n2 = cmul(L.n, L.n);
+                const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
+                const double2 ndc = cmul(L.n, dcdn);
+                const double2 dbdn = tf_scale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
+                const double2 dedn = op.pol == PB_TF_POL_P
+                    ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
+                    : cadd(L.cost, ndc);
+                gix = cmulc(dbdn, cbeta).x + cmulc(dedn, ceta).x;
+            }
+            // vbar_{k+1} = M_k^H vbar_k (+ conj(t) fbar_{k+1})
+            const double2 mis = make_double2(sb.y, -sb.x);
+            const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
+            const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
+            const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
+            vb0 = nb0; vb1 = nb1;
+            if (fseed) {
+                double2 eb2, hb2;
+                tf_field_bar(dA, dEsq, N, count, i, k + 1, inv_re0, e1, h1, eb2, hb2);
+                vb0 = cadd(vb0, cmul(ct, eb2));
+                vb1 = cadd(vb1, cmul(ct, hb2));
+            }
+            for (int kind = 0; kind < 2; ++kind) {
+                if (!(kinds & (1 << kind))) continue;
+                const double v = warp_sum(act ? (kind == 0 ? gth : gix) : 0.0);
+                if (lane == 0) {
+                    double* p = partial + (long long)(2 * k + kind) * W + warp;
+                    *p = first ? v : *p + v;
+                }
+            }
+        }
+    }
+}
+
+// grad[row, k] = sum over the first nw warps of partial[(2 k + kind) * W + w], in a fixed order
+template <typename R>
+__global__ void __launch_bounds__(PB_TF_THREADS) stack_grad_reduce_kernel(const double* __restrict__ partial, long long W,
+                                                                           long long nw, int N, int kinds, R* __restrict__ grad) {
+    __shared__ double sh[PB_TF_THREADS];
+    const int k = blockIdx.x % N, kind = blockIdx.x / N;
+    if (!(kinds & (1 << kind))) return;
+    const int row = kinds == (PB_TF_GRAD_THICKNESS | PB_TF_GRAD_INDEX) ? kind : 0;
+    const double* p = partial + (long long)(2 * k + kind) * W;
+    double acc = 0.0;
+    for (long long w = threadIdx.x; w < nw; w += blockDim.x) acc += p[w];
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (int d = blockDim.x / 2; d > 0; d >>= 1) {
+        if ((int)threadIdx.x < d) sh[threadIdx.x] += sh[threadIdx.x + d];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) grad[(long long)row * N + k] = (R)sh[0];
+}
+
+// stack.py:252-301: searchsorted(Z, z, 'right') - 1 clipped to [0, N - 1], then the partial layer below z applied to
+// the field at the layer's substrate-side boundary
+template <typename R>
+__global__ void __launch_bounds__(PB_TF_THREADS) field_at_depth_kernel(const double* __restrict__ z, long long nz,
+                                                                        const double* __restrict__ zb, int N,
+                                                                        const double2* __restrict__ nl, double2 n0,
+                                                                        double wvl, double sin0, int pol,
+                                                                        const double2* __restrict__ Eb,
+                                                                        const double2* __restrict__ Hb,
+                                                                        cplx<R>* __restrict__ Eo, cplx<R>* __restrict__ Ho) {
+    PB_GRID_STRIDE(i, nz) {
+        const double zi = z[i];
+        int lo = 0, hi = N + 1;                       // first boundary with zb > zi
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (zb[mid] <= zi) lo = mid + 1;
+            else hi = mid;
+        }
+        const int li = min(max(lo - 1, 0), N - 1);
+        const double2 n = nl[li];
+        const double2 cost = tf_cos_snell(n0, n, sin0);
+        const double2 eta = tf_admittance(n, cost, pol);
+        const double2 beta = tf_scale(cmul(tf_scale(n, 2.0 * M_PI * (zb[li + 1] - zi)), cost), 1.0 / wvl);
+        double2 sb, cb;
+        tf_sincos(beta, &sb, &cb);
+        double2 v0 = Eb[li + 1], v1 = Hb[li + 1];
+        tf_apply(sb, cb, eta, v0, v1);
+        Eo[i] = mk<R>((R)v0.x, (R)v0.y);
+        Ho[i] = mk<R>((R)v1.x, (R)v1.y);
+    }
+}
+
+static int tf_ops(Handle* h, int pol, int nlayers, int ndim, const long long* shape, const long long* strides,
+                  const void* const* in, TfOps& op, long long& count) {
+    if (pol != PB_TF_POL_S && pol != PB_TF_POL_P) return fail(h, PB_ERR_INVALID, "thinfilm: pol must be PB_TF_POL_S or P");
+    if (nlayers < 0) return fail(h, PB_ERR_INVALID, "thinfilm: nlayers must be >= 0");
+    if (ndim < 0 || ndim > PB_TF_DIMS) return fail(h, PB_ERR_INVALID, "thinfilm: the calculation shape has at most 4 dims");
+    if ((ndim && !shape) || !strides || !in) return fail(h, PB_ERR_INVALID, "thinfilm: missing shape, strides or operands");
+    count = 1;
+    for (int j = 0; j < PB_TF_DIMS; ++j) {
+        const int src = j - (PB_TF_DIMS - ndim);
+        op.shape[j] = src >= 0 ? shape[src] : 1;
+        if (op.shape[j] < 0) return fail(h, PB_ERR_INVALID, "thinfilm: negative extent");
+        count *= op.shape[j];
+    }
+    for (int q = 0; q < PB_TF_NOPS; ++q) {
+        op.p[q] = in[q];
+        const bool layered = q == PB_TF_IN_N || q == PB_TF_IN_D;
+        if (!in[q] && (!layered || nlayers > 0)) return fail(h, PB_ERR_INVALID, "thinfilm: missing operand");
+        for (int j = 0; j < PB_TF_DIMS; ++j) {
+            const int src = j - (PB_TF_DIMS - ndim);
+            op.st[q][j] = src >= 0 ? strides[5 * q + src] : 0;
+        }
+        op.st[q][PB_TF_DIMS] = layered ? strides[5 * q + PB_TF_DIMS] : 0;
+    }
+    op.nlayers = nlayers;
+    op.pol = pol;
+    op.theta_scale = 1.0;
+    return PB_OK;
+}
+
+}  // namespace pb
+
+using namespace pb;
+
+extern "C" int pb_stack_eval(pb_handle_t hh, int dtype, int mode, int pol, int flags, int nlayers, int ndim,
+                             const long long* shape, const long long* strides, const void* const* in, double theta_scale,
+                             void* const* out, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (mode != PB_TF_THINFILM && mode != PB_TF_COATINGS) return fail(h, PB_ERR_INVALID, "thinfilm: bad mode");
+    if (flags <= 0 || flags >= (1 << PB_TF_NOUT) || !out) return fail(h, PB_ERR_INVALID, "thinfilm: no output");
+    if (mode == PB_TF_THINFILM && (flags & ~(1 << PB_TF_OUT_R | 1 << PB_TF_OUT_T)))
+        return fail(h, PB_ERR_INVALID, "thinfilm: multilayer_stack_rt mode writes r and t only");
+    if (mode == PB_TF_THINFILM && nlayers < 1) return fail(h, PB_ERR_INVALID, "thinfilm: at least one film layer");
+    TfOps op;
+    long long count;
+    PB_TRY(tf_ops(h, pol, nlayers, ndim, shape, strides, in, op, count));
+    op.theta_scale = theta_scale;
+    TfOut o;
+    for (int q = 0; q < PB_TF_NOUT; ++q) {
+        o.p[q] = (flags >> q & 1) ? out[q] : nullptr;
+        if ((flags >> q & 1) && !out[q]) return fail(h, PB_ERR_INVALID, "thinfilm: an output asked for is NULL");
+    }
+    if (count == 0) return PB_OK;
+    TfStage sg{(double2*)o.p[PB_TF_OUT_E], (double2*)o.p[PB_TF_OUT_H], (double*)o.p[PB_TF_OUT_ESQ],
+               (double*)o.p[PB_TF_OUT_ABS]};
+    if (dtype == PB_C64 && (sg.E || sg.H || sg.Esq || sg.A)) {
+        // float outputs: the stage lives in the handle's scratch, one fp64 array per field output
+        const size_t nb = (size_t)(nlayers + 1) * count, na = (size_t)nlayers * count;
+        const size_t bytes = (sg.E ? 16 * nb : 0) + (sg.H ? 16 * nb : 0) + (sg.Esq ? 8 * nb : 0) + (sg.A ? 8 * na : 0);
+        void* base = nullptr;
+        PB_TRY(ensure_scratch(h, 2, bytes, &base));
+        char* p = (char*)base;
+        if (sg.E) { sg.E = (double2*)p; p += 16 * nb; }
+        if (sg.H) { sg.H = (double2*)p; p += 16 * nb; }
+        if (sg.Esq) { sg.Esq = (double*)p; p += 8 * nb; }
+        if (sg.A) sg.A = (double*)p;
+    }
+    const int g = grid_for(count, PB_TF_THREADS, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        if (mode == PB_TF_THINFILM) stack_eval_kernel<R, PB_TF_THINFILM><<<g, PB_TF_THREADS, 0, st>>>(op, count, o, sg);
+        else stack_eval_kernel<R, PB_TF_COATINGS><<<g, PB_TF_THREADS, 0, st>>>(op, count, o, sg);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+extern "C" int pb_stack_grad(pb_handle_t hh, int dtype, int pol, int kinds, int nlayers, int ndim, const long long* shape,
+                             const long long* strides, const void* const* in, const void* E, const void* H,
+                             const void* const* seeds, void* grad, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (kinds < 1 || kinds > (PB_TF_GRAD_THICKNESS | PB_TF_GRAD_INDEX)) return fail(h, PB_ERR_INVALID, "thinfilm: bad gradient kind");
+    if (!E || !H || !seeds || !grad) return fail(h, PB_ERR_INVALID, "thinfilm: missing fields, seeds or output");
+    TfOps op;
+    long long count;
+    PB_TRY(tf_ops(h, pol, nlayers, ndim, shape, strides, in, op, count));
+    if (nlayers == 0) return PB_OK;
+    const int ng = (kinds & PB_TF_GRAD_THICKNESS ? 1 : 0) + (kinds & PB_TF_GRAD_INDEX ? 1 : 0);
+    if (count == 0) {
+        PB_CUDA(h, cudaMemsetAsync(grad, 0, (size_t)ng * nlayers * rsize(dtype), st));
+        return PB_OK;
+    }
+    const int g = grid_for(count, PB_TF_THREADS, h->sm_count);
+    const long long W = (long long)g * (PB_TF_THREADS / 32);
+    const long long nw = std::min<long long>(W, (count + 31) / 32);     // warps that had at least one sample
+    void* partial = nullptr;
+    PB_TRY(ensure_scratch(h, 2, (size_t)2 * nlayers * W * sizeof(double), &partial));
+    stack_grad_kernel<<<g, PB_TF_THREADS, 0, st>>>(op, count, kinds, (const double2*)E, (const double2*)H,
+                                                   (const double*)seeds[0], (const double*)seeds[1],
+                                                   (const double*)seeds[2], (const double*)seeds[3], (double*)partial);
+    PB_LAUNCH_CHECK(h);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        stack_grad_reduce_kernel<R><<<2 * nlayers, PB_TF_THREADS, 0, st>>>((const double*)partial, W, nw, nlayers, kinds,
+                                                                           (R*)grad);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+extern "C" int pb_field_at_depth(pb_handle_t hh, int dtype, int pol, int nlayers, const void* z, long long nz,
+                                 const void* zb, const void* n, double n0_re, double n0_im, double wvl, double theta0,
+                                 const void* E_b, const void* H_b, void* E, void* H, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (pol != PB_TF_POL_S && pol != PB_TF_POL_P) return fail(h, PB_ERR_INVALID, "thinfilm: pol must be PB_TF_POL_S or P");
+    if (nlayers < 1) return fail(h, PB_ERR_INVALID, "field_at_depth requires at least one layer");
+    if (nz < 0 || !z || !zb || !n || !E_b || !H_b || !E || !H) return fail(h, PB_ERR_INVALID, "bad field_at_depth arguments");
+    if (nz == 0) return PB_OK;
+    const int g = grid_for(nz, PB_TF_THREADS, h->sm_count);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        field_at_depth_kernel<R><<<g, PB_TF_THREADS, 0, st>>>((const double*)z, nz, (const double*)zb, nlayers,
+                                                              (const double2*)n, make_double2(n0_re, n0_im), wvl,
+                                                              sin(theta0), pol, (const double2*)E_b, (const double2*)H_b,
+                                                              (cplx<R>*)E, (cplx<R>*)H);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}

@@ -20,6 +20,7 @@ touches numpy `exp` or eager tensor arithmetic.
 import importlib
 
 from . import bayer as _bayer
+from . import coatings as _coat
 from . import convolution as _conv
 from . import coordinates as _coords
 from . import detector as _det
@@ -35,6 +36,7 @@ from . import psf as _psf
 from . import psi as _psi
 from . import shack_hartmann as _sh
 from . import sri as _sri
+from . import thinfilm as _tf
 
 # prysm module -> {attribute: replacement}
 _PROPAGATION_FUNCS = (
@@ -46,6 +48,8 @@ _CORONAGRAPH_FUNCS = (
     'to_fpm_and_back', 'to_fpm_and_back_adjoint', 'to_fpm_and_back_multiresolution',
     'to_fpm_and_back_multiresolution_adjoint', 'babinet', 'babinet_adjoint', 'vortex_phase_mask', 'prepare_measured_fpm',
 )
+_COATINGS_STACK_FUNCS = ('stack_rt', 'RTA', 'internal_fields', 'field_at_depth')
+_COATINGS_DIFF_FUNCS = ('forward_eval', 'ForwardEval', 'thickness_gradient', 'index_gradient')
 _TARGETS = {
     'prysm.propagation.fft': {n: getattr(_prop, n) for n in ('focus', 'unfocus', 'focus_adjoint', 'unfocus_adjoint')},
     'prysm.propagation.angular_spectrum': {n: getattr(_prop, n) for n in (
@@ -93,6 +97,12 @@ _TARGETS = {
     'prysm.bayer': {n: getattr(_bayer, n) for n in (
         'wb_prescale', 'wb_postscale', 'composite_bayer', 'decomposite_bayer', 'recomposite_bayer',
         'demosaic_deinterlace', 'assemble_superresolved', 'demosaic_malvar')},
+    # thin films: merit, problem, needle and monitoring bind these names at import time and do numpy arithmetic on
+    # the results, so they keep the reference's host engine
+    'prysm.thinfilm': {'multilayer_stack_rt': _tf.multilayer_stack_rt},
+    'prysm.x.coatings': {n: getattr(_coat, n) for n in _COATINGS_STACK_FUNCS + _COATINGS_DIFF_FUNCS},
+    'prysm.x.coatings.stack': {n: getattr(_coat, n) for n in _COATINGS_STACK_FUNCS},
+    'prysm.x.coatings.diff': {n: getattr(_coat, n) for n in _COATINGS_DIFF_FUNCS},
 }
 
 _saved = {}  # (module name, attribute) -> original
