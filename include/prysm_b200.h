@@ -73,7 +73,10 @@ long long pb_launch_count(pb_handle_t h);
  * can tell which specialisation a call ran.  route = kind << 28 | L << 8 | flags:
  *   PB_ROUTE_AXIS_REG     axis_reg_kernel<L, INV, COLS, TP, RT, PM, DENSE>; flags INV | COLS << 1 | RT << 2 | PM << 3 |
  *                         DENSE << 4
- *   PB_ROUTE_AXIS_GENERIC the generic shared-memory axis pass, any length (L = 0, flags = 0)
+ *   PB_ROUTE_AXIS_GENERIC the generic shared-memory axis pass: every launch on L = 0, flags = 0, and each launch also
+ *                         on its power-of-two length L, flags DTYPE | COLS << 1 (DTYPE: PB_C64 / PB_C128; COLS: a
+ *                         column pass, consecutive lines adjacent in memory).  A Bluestein axis is two launches at its
+ *                         padded length.
  *   PB_ROUTE_FOCUS_V2     focus_col4_kernel / focus_row4_kernel of N = L; flags INV (two kernels per field)
  *   PB_ROUTE_MDFT_TC      wgmma_gemm_kernel of the tensor-core matrix DFT; L = split-K pieces (1 when not split);
  *                         flags STREAMK | STAGE2 << 1 | PARTIALS << 2 (PARTIALS: writes split-K partial planes)

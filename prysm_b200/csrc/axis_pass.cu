@@ -142,6 +142,13 @@ __global__ void __launch_bounds__(512) axis_pass_kernel(const AxisPass p, const 
 
 static int pow2ceil(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 
+int generic_max_len(const Handle* h, int dtype) {
+    const long long cap = h->max_smem_optin, elem = csize(dtype);
+    int L = 1;
+    while ((long long)2 * L * elem <= cap) L <<= 1;
+    return L;
+}
+
 template <typename R>
 static int launch_generic(Handle* h, const AxisPass& p, cudaStream_t st) {
     const int L = p.L;
@@ -172,7 +179,8 @@ static int launch_generic(Handle* h, const AxisPass& p, cudaStream_t st) {
     const int grid = (p.nb + T - 1) / T;
     axis_pass_kernel<R><<<grid, threads, smem, st>>>(p, T, ilog2(L), reinterpret_cast<const cplx<R>*>(tw));
     PB_LAUNCH_CHECK(h);
-    h->route_launches[route_code(PB_ROUTE_AXIS_GENERIC, 0, 0)]++;
+    h->route_launches[route_code(PB_ROUTE_AXIS_GENERIC, 0, 0)]++;  // every generic launch
+    h->route_launches[route_code(PB_ROUTE_AXIS_GENERIC, L, p.dtype | p.batch_contiguous << 1)]++;
     return PB_OK;
 }
 

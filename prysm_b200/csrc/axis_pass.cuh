@@ -55,4 +55,8 @@ struct AxisPass {
 // L must be a power of two here (Bluestein is composed one level up).
 int launch_axis_pass(Handle* h, const AxisPass& p, cudaStream_t s);
 
+// Largest power-of-two L the generic pass takes at dtype: one line of L elements must fit one CTA's opt-in shared
+// memory (232,448 B on an H100: 16384 complex64 or 8192 complex128 points).
+int generic_max_len(const Handle* h, int dtype);
+
 }  // namespace pb

@@ -103,6 +103,15 @@ static int get_chirp_filter(Handle* h, int n, int dtype, int dir, const void** o
 // ---------------------------------------------------------------------------------------
 static int axis_dft(Handle* h, AxisPass p, cudaStream_t st) {
     const int n = p.Llog;
+    // refused before any launch, in terms of the length the caller asked for (Bluestein runs at M ~ 2n)
+    const int lmax = generic_max_len(h, p.dtype);
+    if (n > lmax || (!is_pow2(n) && bluestein_len(n) > lmax)) {
+        const char* name = p.dtype == PB_C64 ? "complex64" : "complex128";
+        return fail(h, PB_ERR_UNSUPPORTED,
+                    std::string(name) + " FFT of length " + std::to_string(n) + " does not fit one CTA's shared memory (" +
+                        std::to_string(h->max_smem_optin) + " B): " + name + " takes any length up to " +
+                        std::to_string(lmax / 2) + " and powers of two up to " + std::to_string(lmax));
+    }
     if (is_pow2(n)) {
         p.L = n;
         return launch_axis_pass(h, p, st);

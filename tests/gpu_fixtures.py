@@ -1,4 +1,5 @@
-"""The fixture and helper the GPU tests share: `from gpu_fixtures import pb, host`."""
+"""The fixture and helpers the GPU tests share: `from gpu_fixtures import pb, host`, and the per-route launch counters
+(pb_route_launch_count) that pin which transform kernels a call ran: `routes_of(fn, codes)`."""
 import numpy as np
 import pytest
 import torch
@@ -18,3 +19,25 @@ def pb():
 
 def host(t):
     return t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+
+
+def _handle():
+    from prysm_b200 import _capi
+    return _capi.handle_for(torch.cuda.current_device(), torch.cuda.current_stream().cuda_stream)
+
+
+def route_counts(codes):
+    """launches so far on each route of `codes` ({key: route code}), and of every kernel of the handle under 'all'"""
+    h = _handle()
+    out = {k: h.route_launch_count(c) for k, c in codes.items()}
+    out['all'] = h.launch_count()
+    return out
+
+
+def routes_of(fn, codes):
+    """fn()'s result and the launches it made, per key of `codes` and 'all' (only the keys it used)"""
+    torch.cuda.synchronize()
+    c0 = route_counts(codes)
+    res = fn()
+    c1 = route_counts(codes)
+    return res, {k: c1[k] - c0[k] for k in c0 if c1[k] != c0[k]}

@@ -58,6 +58,7 @@ import torch
 import prysm_oracle as O
 from conftest import rel_linf, within
 from gpu_fixtures import pb  # noqa: F401
+from gpu_fixtures import routes_of as _routes_of
 
 pytestmark = pytest.mark.gpu
 
@@ -301,37 +302,26 @@ AXIS_ALL = [(L, inv, cols, rt, pm, dense) for L in (1024, 2048, 4096) for inv in
             for rt in (False, True) for pm in (False, True) for dense in (False, True)]
 
 
-def _handle():
-    from prysm_b200 import _capi
-    return _capi.handle_for(torch.cuda.current_device(), torch.cuda.current_stream().cuda_stream)
-
-
 def axis_code(k):
     from prysm_b200 import _capi
     L, inv, cols, rt, pm, dense = k
     return _capi.route_code(_capi.ROUTE_AXIS_REG, L, int(inv) | int(cols) << 1 | int(rt) << 2 | int(pm) << 3 | int(dense) << 4)
 
 
-def route_counts():
-    """launches so far of every axis_reg_kernel instantiation, of the generic axis pass and of the focus pair"""
+def route_codes():
+    """every axis_reg_kernel instantiation, the generic axis pass (all lengths) and the focus pair"""
     from prysm_b200 import _capi
-    h = _handle()
-    out = {k: h.route_launch_count(axis_code(k)) for k in AXIS_ALL}
-    out['generic'] = h.route_launch_count(_capi.route_code(_capi.ROUTE_AXIS_GENERIC))
+    codes = {k: axis_code(k) for k in AXIS_ALL}
+    codes['generic'] = _capi.route_code(_capi.ROUTE_AXIS_GENERIC)
     for N in NS:
         for inv in (0, 1):
-            out[('focus', N, inv)] = h.route_launch_count(_capi.route_code(_capi.ROUTE_FOCUS_V2, N, inv))
-    out['all'] = h.launch_count()
-    return out
+            codes[('focus', N, inv)] = _capi.route_code(_capi.ROUTE_FOCUS_V2, N, inv)
+    return codes
 
 
 def routes_of(fn):
     """fn()'s result and the launches it made, per route (only the routes it used)"""
-    torch.cuda.synchronize()
-    c0 = route_counts()
-    res = fn()
-    c1 = route_counts()
-    return res, {k: c1[k] - c0[k] for k in c0 if c1[k] != c0[k]}
+    return _routes_of(fn, route_codes())
 
 
 def run_axis(chk, case, fn, expect):
