@@ -1,4 +1,4 @@
-// Handle lifetime, scratch arenas, error reporting.
+// Handle lifetime, scratch arenas, tensor-map encoding, error reporting.
 #include "common.cuh"
 
 namespace pb {
@@ -20,6 +20,27 @@ int ensure_scratch(Handle* h, int slot, size_t bytes, void** out) {
         h->scratch_bytes[slot] = want;
     }
     *out = h->scratch[slot];
+    return PB_OK;
+}
+
+int encode_tensor_map(Handle* h, CUtensorMap* map, CUtensorMapDataType type, int rank, const void* base,
+                      const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
+                      CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2) {
+    typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static EncodeTiledFn fn = nullptr;   // a driver entry point: process-wide, not per device
+    if (!fn) {
+        cudaDriverEntryPointQueryResult q;
+        void* f = nullptr;
+        PB_CUDA(h, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q));
+        if (!f || q != cudaDriverEntryPointSuccess) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled not available");
+        fn = reinterpret_cast<EncodeTiledFn>(f);
+    }
+    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    CUresult r = fn(map, type, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
     return PB_OK;
 }
 

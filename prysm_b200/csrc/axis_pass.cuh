@@ -52,6 +52,14 @@ struct AxisPass {
     int roundtrip = 0;
 };
 
+// Points p at nlines lines of row-major planes with row pitches in_ld and out_ld (elements): axis 1 runs the pass along
+// the rows (one line per row), axis 0 along the columns (one line per column, consecutive lines adjacent in memory).
+inline void along(AxisPass& p, int axis, int nlines, long long in_ld, long long out_ld) {
+    p.nb = nlines;
+    if (axis == 1) { p.ibs = in_ld; p.ies = 1; p.obs = out_ld; p.oes = 1; p.batch_contiguous = 0; }
+    else { p.ibs = 1; p.ies = in_ld; p.obs = 1; p.oes = out_ld; p.batch_contiguous = 1; }
+}
+
 // L must be a power of two here (Bluestein is composed one level up).
 int launch_axis_pass(Handle* h, const AxisPass& p, cudaStream_t s);
 

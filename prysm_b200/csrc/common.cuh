@@ -224,6 +224,19 @@ int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, con
 int get_twiddles(Handle* h, int n, int dtype, const void** out);
 // upload a host fp64 complex table in the precision of key.dtype and cache it in the handle
 int upload_table(Handle* h, const TwKey& key, const std::vector<std::complex<double>>& t, const void** out);
+// the handle's device table `key`; on a miss, build(t) fills the empty host table t, which upload_table then uploads
+template <typename F>
+int cached_table(Handle* h, const TwKey& key, F&& build, const void** out) {
+    auto it = h->tables.find(key);
+    if (it != h->tables.end()) { *out = it->second; return PB_OK; }
+    std::vector<std::complex<double>> t;
+    build(t);
+    return upload_table(h, key, t, out);
+}
+// cuTensorMapEncodeTiled (resolved once per process) with unit element strides, no interleave and no out-of-bounds fill
+int encode_tensor_map(Handle* h, CUtensorMap* map, CUtensorMapDataType type, int rank, const void* base,
+                      const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
+                      CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2);
 
 inline bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 inline int ilog2(int n) { int l = 0; while ((1 << l) < n) ++l; return l; }

@@ -52,50 +52,44 @@ int upload_table(Handle* h, const TwKey& key, const std::vector<std::complex<dou
 }
 
 int get_twiddles(Handle* h, int n, int dtype, const void** out) {
-    TwKey key{n, dtype, TW_ROOTS};
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) { *out = it->second; return PB_OK; }
-    std::vector<std::complex<double>> t(n);
-    for (int k = 0; k < n; ++k) {
-        // exact octant symmetry is not needed; long double keeps the table correctly rounded
-        const long double ang = -2.0L * 3.14159265358979323846264338327950288L * k / n;
-        t[k] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
-    }
-    return upload_table(h, key, t, out);
+    return cached_table(h, {n, dtype, TW_ROOTS}, [n](auto& t) {
+        t.resize(n);
+        for (int k = 0; k < n; ++k) {
+            // exact octant symmetry is not needed; long double keeps the table correctly rounded
+            const long double ang = -2.0L * 3.14159265358979323846264338327950288L * k / n;
+            t[k] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
+        }
+    }, out);
 }
 
 static int bluestein_len(int n) { int m = 1; while (m < 2 * n - 1) m <<= 1; return m; }
 
 // chirp c[j] = exp(dir*pi*i*j^2/n), j^2 reduced mod 2n exactly
 static int get_chirp(Handle* h, int n, int dtype, int dir, const void** out) {
-    TwKey key{n, dtype, dir < 0 ? TW_CHIRP_FWD : TW_CHIRP_INV};
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) { *out = it->second; return PB_OK; }
-    std::vector<std::complex<double>> t(n);
-    for (int j = 0; j < n; ++j) {
-        const long long r = ((long long)j * j) % (2LL * n);
-        const long double ang = dir * 3.14159265358979323846264338327950288L * r / n;
-        t[j] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
-    }
-    return upload_table(h, key, t, out);
+    return cached_table(h, {n, dtype, dir < 0 ? TW_CHIRP_FWD : TW_CHIRP_INV}, [n, dir](auto& t) {
+        t.resize(n);
+        for (int j = 0; j < n; ++j) {
+            const long long r = ((long long)j * j) % (2LL * n);
+            const long double ang = dir * 3.14159265358979323846264338327950288L * r / n;
+            t[j] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
+        }
+    }, out);
 }
 
 // spectrum of the Bluestein filter g[d mod M] = conj(c[|d|]), |d| < n
 static int get_chirp_filter(Handle* h, int n, int dtype, int dir, const void** out) {
-    TwKey key{n, dtype, dir < 0 ? TW_FILTER_FWD : TW_FILTER_INV};
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) { *out = it->second; return PB_OK; }
-    const int M = bluestein_len(n);
-    std::vector<std::complex<double>> g(M, {0.0, 0.0});
-    for (int d = 0; d < n; ++d) {
-        const long long r = ((long long)d * d) % (2LL * n);
-        const long double ang = -dir * 3.14159265358979323846264338327950288L * r / n;
-        std::complex<double> v((double)cosl(ang), (double)sinl(ang));
-        g[d] = v;
-        if (d) g[M - d] = v;
-    }
-    host_fft_pow2(g, -1);
-    return upload_table(h, key, g, out);
+    return cached_table(h, {n, dtype, dir < 0 ? TW_FILTER_FWD : TW_FILTER_INV}, [n, dir](auto& g) {
+        const int M = bluestein_len(n);
+        g.assign(M, {0.0, 0.0});
+        for (int d = 0; d < n; ++d) {
+            const long long r = ((long long)d * d) % (2LL * n);
+            const long double ang = -dir * 3.14159265358979323846264338327950288L * r / n;
+            std::complex<double> v((double)cosl(ang), (double)sinl(ang));
+            g[d] = v;
+            if (d) g[M - d] = v;
+        }
+        host_fft_pow2(g, -1);
+    }, out);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -155,38 +149,65 @@ static int axis_dft(Handle* h, AxisPass p, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------
 // pb_fft2
 // ---------------------------------------------------------------------------------------
-struct Fft2Args {
-    int dtype;
-    const void* in; int in_kind; const void* amp; int amp_kind; double kturns;
-    int ny, nx; long long in_ld;
-    int ky, kx, dir; double scale; int shift_in, shift_out;
-    void* out; int out_kind; double weight; int oy, ox; long long out_ld;
-};
-
+// one field (a.batch is ignored)
 static int fft2_generic(Handle* h, const Fft2Args& a, cudaStream_t st) {
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 0, (size_t)a.ny * a.ox * csize(a.dtype), &tmp));
     AxisPass x;  // rows: only the ny populated rows are transformed (zero rows stay implicit)
     x.dtype = a.dtype;
-    x.in = a.in; x.in_kind = a.in_kind; x.amp = a.amp; x.amp_kind = a.amp_kind; x.kturns = a.kturns;
-    x.ibs = a.in_ld; x.ies = 1; x.nb = a.ny;
+    x.in = a.in; x.in_kind = a.in_kind; x.amp = a.amp; x.amp_kind = a.amp_kind; x.kturns = a.kturns();
+    along(x, 1, a.ny, a.in_ld, a.ox);
     x.Llog = a.kx; x.n_in = a.nx; x.in_off = ceil_half(a.kx - a.nx); x.rot_in = a.shift_in ? a.kx / 2 : 0;
     x.dir = a.dir;
-    x.out = tmp; x.obs = a.ox; x.oes = 1;
+    x.out = tmp;
     x.n_out = a.ox; x.crop_off = ceil_half(a.kx - a.ox); x.rot_out = a.shift_out ? a.kx / 2 : 0;
-    x.batch_contiguous = 0;
     PB_TRY(axis_dft(h, x, st));
 
     AxisPass y;  // columns
     y.dtype = a.dtype;
-    y.in = tmp; y.ibs = 1; y.ies = a.ox; y.nb = a.ox;
+    y.in = tmp;
+    along(y, 0, a.ox, a.ox, a.out_ld);
     y.Llog = a.ky; y.n_in = a.ny; y.in_off = ceil_half(a.ky - a.ny); y.rot_in = a.shift_in ? a.ky / 2 : 0;
     y.dir = a.dir;
-    y.out = a.out; y.obs = 1; y.oes = a.out_ld;
+    y.out = a.out;
     y.n_out = a.oy; y.crop_off = ceil_half(a.ky - a.oy); y.rot_out = a.shift_out ? a.ky / 2 : 0;
     y.scale = a.scale; y.out_kind = a.out_kind; y.weight = a.weight;
-    y.batch_contiguous = 1;
     return axis_dft(h, y, st);
+}
+
+// pb_fft2 and pb_fft2_batch after their prologue (handle, dtype, batch >= 1): the fused focus pair where it covers the
+// call, else one field at a time through the generic passes
+static int fft2_run(Handle* h, const Fft2Args& a, cudaStream_t st) {
+    if (a.ny < 1 || a.nx < 1 || a.ky < a.ny || a.kx < a.nx) return fail(h, PB_ERR_INVALID, "need 1 <= n <= k on both axes");
+    if (a.oy < 1 || a.ox < 1 || a.oy > a.ky || a.ox > a.kx) return fail(h, PB_ERR_INVALID, "crop window must fit the transform");
+    if (a.dir != -1 && a.dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
+    if (!a.in || !a.out) return fail(h, PB_ERR_INVALID, "null array pointer");
+    if (a.in_kind < 0 || a.in_kind > 2 || a.out_kind < 0 || a.out_kind > 2) return fail(h, PB_ERR_INVALID, "bad in/out kind");
+    if (a.in_ld < a.nx || a.out_ld < a.ox) return fail(h, PB_ERR_INVALID, "row pitch smaller than the row");
+    if (a.batch > 1 && (a.in_bs < (long long)(a.ny - 1) * a.in_ld + a.nx || a.out_bs < (long long)(a.oy - 1) * a.out_ld + a.ox))
+        return fail(h, PB_ERR_INVALID, "batch stride smaller than one field");
+    int rc = try_tuned_fft2_batch(h, a, st);
+    if (rc != PB_ERR_UNSUPPORTED) return rc;
+    for (int b = 0; b < a.batch; ++b) PB_TRY(fft2_generic(h, a.field(b), st));
+    return PB_OK;
+}
+
+// pb_fft1 and pb_axis_dft after their prologue: one transform of length n along `axis` of an (ny, nx) plane
+static int plane_axis_dft(Handle* h, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int n, int dir,
+                          double scale, const void* pre_e, int pre_e_conj, const void* pre_b, int pre_b_conj,
+                          const void* post_e, int post_e_conj, const void* post_b, int post_b_conj, int out_off,
+                          int n_out, void* out, long long out_ld, cudaStream_t st) {
+    if (ny < 1 || nx < 1 || n < 1 || (axis != 0 && axis != 1)) return fail(h, PB_ERR_INVALID, "bad shape / axis");
+    if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
+    if (out_off < 0 || n_out < 1 || out_off + n_out > n) return fail(h, PB_ERR_INVALID, "output window outside the transform");
+    AxisPass p;
+    p.dtype = dtype; p.in = in; p.dir = dir; p.scale = scale; p.out = out;
+    p.Llog = n; p.n_out = n_out; p.crop_off = out_off;
+    p.pre_e = pre_e; p.pre_e_conj = pre_e_conj; p.pre_b = pre_b; p.pre_b_conj = pre_b_conj;
+    p.post_e = post_e; p.post_e_conj = post_e_conj; p.post_off = out_off; p.post_b = post_b; p.post_b_conj = post_b_conj;
+    along(p, axis, axis == 1 ? ny : nx, in_ld, out_ld);
+    p.n_in = std::min(axis == 1 ? nx : ny, n);
+    return axis_dft(h, p, st);
 }
 
 }  // namespace pb
@@ -198,19 +219,8 @@ extern "C" int pb_fft2(pb_handle_t hh, int dtype, const void* in, int in_kind, c
                        int shift_in, int shift_out, void* out, int out_kind, double weight, int oy, int ox,
                        long long out_ld, void* stream) {
     PB_ENTER_REAL(hh);
-    if (ny < 1 || nx < 1 || ky < ny || kx < nx) return fail(h, PB_ERR_INVALID, "need 1 <= n <= k on both axes");
-    if (oy < 1 || ox < 1 || oy > ky || ox > kx) return fail(h, PB_ERR_INVALID, "crop window must fit the transform");
-    if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
-    if (!in || !out) return fail(h, PB_ERR_INVALID, "null array pointer");
-    if (in_kind < 0 || in_kind > 2 || out_kind < 0 || out_kind > 2) return fail(h, PB_ERR_INVALID, "bad in/out kind");
-    if (in_ld < nx || out_ld < ox) return fail(h, PB_ERR_INVALID, "row pitch smaller than the row");
-    Fft2Args a{dtype, in, in_kind, amp, amp_kind, kscale / (2.0 * M_PI), ny, nx, in_ld, ky, kx, dir, scale,
-               shift_in, shift_out, out, out_kind, weight, oy, ox, out_ld};
-    int rc = try_tuned_fft2(h, a.dtype, a.in, a.in_kind, a.amp, a.amp_kind, a.kturns, a.ny, a.nx, a.in_ld, a.ky,
-                            a.kx, a.dir, a.scale, a.shift_in, a.shift_out, a.out, a.out_kind, a.weight, a.oy, a.ox,
-                            a.out_ld, st);
-    if (rc != PB_ERR_UNSUPPORTED) return rc;
-    return fft2_generic(h, a, st);
+    return fft2_run(h, {dtype, in, in_kind, amp, amp_kind, kscale, 1, 0, 0, ny, nx, in_ld, ky, kx, dir, scale, shift_in,
+                        shift_out, out, out_kind, weight, oy, ox, out_ld, 0}, st);
 }
 
 extern "C" int pb_fft2_batch(pb_handle_t hh, int dtype, const void* in, int in_kind, const void* amp, int amp_kind,
@@ -220,50 +230,16 @@ extern "C" int pb_fft2_batch(pb_handle_t hh, int dtype, const void* in, int in_k
     PB_ENTER(hh);
     if (batch < 1) return fail(h, PB_ERR_INVALID, "batch must be >= 1");
     if (dtype != PB_C64 && dtype != PB_C128) return fail(h, PB_ERR_INVALID, "dtype must be PB_C64 or PB_C128");
-    if (ny < 1 || nx < 1 || ky < ny || kx < nx) return fail(h, PB_ERR_INVALID, "need 1 <= n <= k on both axes");
-    if (oy < 1 || ox < 1 || oy > ky || ox > kx) return fail(h, PB_ERR_INVALID, "crop window must fit the transform");
-    if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
-    if (!in || !out) return fail(h, PB_ERR_INVALID, "null array pointer");
-    if (in_kind < 0 || in_kind > 2 || out_kind < 0 || out_kind > 2) return fail(h, PB_ERR_INVALID, "bad in/out kind");
-    if (in_ld < nx || out_ld < ox) return fail(h, PB_ERR_INVALID, "row pitch smaller than the row");
-    if (batch > 1 && (in_bs < (long long)(ny - 1) * in_ld + nx || out_bs < (long long)(oy - 1) * out_ld + ox))
-        return fail(h, PB_ERR_INVALID, "batch stride smaller than one field");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = try_tuned_fft2_batch(h, dtype, in, in_kind, amp, amp_kind, kscale / (2.0 * M_PI), batch, in_bs, amp_bs, ny, nx,
-                                  in_ld, ky, kx, dir, scale, shift_in, shift_out, out, out_kind, weight, oy, ox, out_ld,
-                                  out_bs, st);
-    if (rc != PB_ERR_UNSUPPORTED) return rc;
-    // shapes outside the fused kernels: one field at a time through the generic passes
-    const size_t rsz = rsize(dtype);
-    const size_t in_elt = in_kind == PB_IN_COMPLEX ? 2 * rsz : rsz;
-    const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : rsz;
-    const size_t out_elt = out_kind == PB_OUT_COMPLEX ? 2 * rsz : rsz;
-    for (int b = 0; b < batch; ++b) {
-        Fft2Args a{dtype, reinterpret_cast<const char*>(in) + (size_t)b * in_bs * in_elt, in_kind,
-                   amp ? reinterpret_cast<const char*>(amp) + (size_t)b * amp_bs * amp_elt : nullptr, amp_kind,
-                   kscale / (2.0 * M_PI), ny, nx, in_ld, ky, kx, dir, scale, shift_in, shift_out,
-                   reinterpret_cast<char*>(out) + (size_t)b * out_bs * out_elt, out_kind, weight, oy, ox, out_ld};
-        PB_TRY(fft2_generic(h, a, st));
-    }
-    return PB_OK;
+    return fft2_run(h, {dtype, in, in_kind, amp, amp_kind, kscale, batch, in_bs, amp_bs, ny, nx, in_ld, ky, kx, dir, scale,
+                        shift_in, shift_out, out, out_kind, weight, oy, ox, out_ld, out_bs},
+                    reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int pb_fft1(pb_handle_t hh, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int n,
                        int dir, double scale, void* out, long long out_ld, void* stream) {
     PB_ENTER_REAL(hh);
-    if (ny < 1 || nx < 1 || n < 1 || (axis != 0 && axis != 1)) return fail(h, PB_ERR_INVALID, "bad shape / axis");
-    if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
-    AxisPass p;
-    p.dtype = dtype; p.in = in; p.dir = dir; p.scale = scale; p.out = out;
-    p.Llog = n; p.in_off = 0; p.rot_in = 0; p.n_out = n; p.crop_off = 0; p.rot_out = 0;
-    if (axis == 1) {
-        p.nb = ny; p.ibs = in_ld; p.ies = 1; p.n_in = nx < n ? nx : n;
-        p.obs = out_ld; p.oes = 1; p.batch_contiguous = 0;
-    } else {
-        p.nb = nx; p.ibs = 1; p.ies = in_ld; p.n_in = ny < n ? ny : n;
-        p.obs = 1; p.oes = out_ld; p.batch_contiguous = 1;
-    }
-    return axis_dft(h, p, st);
+    return plane_axis_dft(h, dtype, in, ny, nx, in_ld, axis, n, dir, scale, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                          0, n, out, out_ld, st);
 }
 
 extern "C" int pb_axis_dft(pb_handle_t hh, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int n,
@@ -271,22 +247,8 @@ extern "C" int pb_axis_dft(pb_handle_t hh, int dtype, const void* in, int ny, in
                            const void* post_e, int post_e_conj, const void* post_b, int post_b_conj, int out_off,
                            int n_out, void* out, long long out_ld, void* stream) {
     PB_ENTER_REAL(hh);
-    if (ny < 1 || nx < 1 || n < 1 || (axis != 0 && axis != 1)) return fail(h, PB_ERR_INVALID, "bad shape / axis");
-    if (dir != -1 && dir != 1) return fail(h, PB_ERR_INVALID, "dir must be -1 or +1");
-    if (out_off < 0 || n_out < 1 || out_off + n_out > n) return fail(h, PB_ERR_INVALID, "output window outside the transform");
-    AxisPass p;
-    p.dtype = dtype; p.in = in; p.dir = dir; p.scale = scale; p.out = out;
-    p.Llog = n; p.n_out = n_out; p.crop_off = out_off;
-    p.pre_e = pre_e; p.pre_e_conj = pre_e_conj; p.pre_b = pre_b; p.pre_b_conj = pre_b_conj;
-    p.post_e = post_e; p.post_e_conj = post_e_conj; p.post_off = out_off; p.post_b = post_b; p.post_b_conj = post_b_conj;
-    if (axis == 1) {
-        p.nb = ny; p.ibs = in_ld; p.ies = 1; p.n_in = nx < n ? nx : n;
-        p.obs = out_ld; p.oes = 1; p.batch_contiguous = 0;
-    } else {
-        p.nb = nx; p.ibs = 1; p.ies = in_ld; p.n_in = ny < n ? ny : n;
-        p.obs = 1; p.oes = out_ld; p.batch_contiguous = 1;
-    }
-    return axis_dft(h, p, st);
+    return plane_axis_dft(h, dtype, in, ny, nx, in_ld, axis, n, dir, scale, pre_e, pre_e_conj, pre_b, pre_b_conj, post_e,
+                          post_e_conj, post_b, post_b_conj, out_off, n_out, out, out_ld, st);
 }
 
 int pb::czt_axis_impl(Handle* h, int dtype, const void* in, int ny, int nx, long long in_ld, int axis, int K,
@@ -298,29 +260,29 @@ int pb::czt_axis_impl(Handle* h, int dtype, const void* in, int ny, int nx, long
     const int nline = axis == 1 ? ny : nx, n_in = std::min(axis == 1 ? nx : ny, K);
     AxisPass f;  // fused: (in * pre) -> FFT_K -> * H -> IFFT_K -> window -> * post
     f.dtype = dtype; f.in = in; f.dir = -1; f.out = out; f.scale = scale / K;
-    f.L = K; f.Llog = K; f.n_in = n_in; f.n_out = n_out; f.crop_off = out_off; f.nb = nline;
+    f.L = K; f.Llog = K; f.n_in = n_in; f.n_out = n_out; f.crop_off = out_off;
     f.pre_e = pre_e; f.pre_e_conj = pre_conj;
     f.post_e = H;
     f.post_e2 = post_e; f.post_e2_conj = post_conj;
-    if (axis == 1) { f.ibs = in_ld; f.ies = 1; f.obs = out_ld; f.oes = 1; f.batch_contiguous = 0; }
-    else { f.ibs = 1; f.ies = in_ld; f.obs = 1; f.oes = out_ld; f.batch_contiguous = 1; }
+    along(f, axis, nline, in_ld, out_ld);
     f.roundtrip = 1;
     f.out_kind = out_kind; f.weight = weight;
     int rc = try_tuned_axis_pass(h, f, st);
     if (rc != PB_ERR_UNSUPPORTED) return rc;
-    // two passes through a (lines x K) scratch
+    // two passes through a (lines x K) scratch: K-element rows along axis 1, nline-element rows along axis 0
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 1, (size_t)nline * K * csize(dtype), &tmp));
+    const long long tmp_ld = axis == 1 ? K : nline;
     AxisPass a = f;
     a.roundtrip = 0; a.post_e2 = nullptr; a.out = tmp; a.n_out = K; a.crop_off = 0; a.scale = 1.0;
     a.out_kind = PB_OUT_COMPLEX; a.weight = 1.0;
-    if (axis == 1) { a.obs = K; a.oes = 1; } else { a.obs = 1; a.oes = nline; }
+    along(a, axis, nline, in_ld, tmp_ld);
     PB_TRY(axis_dft(h, a, st));
     AxisPass b;
     b.dtype = dtype; b.in = tmp; b.dir = +1; b.out = out; b.scale = scale / K;
-    b.Llog = K; b.n_in = K; b.n_out = n_out; b.crop_off = out_off; b.nb = nline;
+    b.Llog = K; b.n_in = K; b.n_out = n_out; b.crop_off = out_off;
     b.post_e = post_e; b.post_e_conj = post_conj; b.post_off = out_off;
-    b.ibs = a.obs; b.ies = a.oes; b.obs = f.obs; b.oes = f.oes; b.batch_contiguous = f.batch_contiguous;
+    along(b, axis, nline, tmp_ld, out_ld);
     b.out_kind = out_kind; b.weight = weight;
     return axis_dft(h, b, st);
 }
@@ -357,45 +319,46 @@ static int angular_spectrum_impl(Handle* h, int dtype, const void* in, int ny, i
     PB_TRY(ensure_scratch(h, 0, (size_t)ky * kx * cs, &t0));
     PB_TRY(ensure_scratch(h, 1, (size_t)ky * kx * cs, &t1));
     AxisPass p;  // rows forward (times the phase screen, if any): ny populated rows -> t0 (ny, kx)
-    p.dtype = dtype; p.in = in; p.ibs = nx; p.ies = 1; p.nb = ny;
+    p.dtype = dtype; p.in = in;
+    along(p, 1, ny, nx, kx);
     p.pre_mat = screen; p.pmi_bs = nx; p.pmi_es = 1; p.pre_mat_conj = conj_screen;
     p.Llog = kx; p.n_in = nx; p.in_off = ceil_half(kx - nx);
-    p.dir = -1; p.out = t0; p.obs = kx; p.oes = 1; p.n_out = kx;
+    p.dir = -1; p.out = t0; p.n_out = kx;
     PB_TRY(axis_dft(h, p, st));
-    if (!tf && dtype == PB_C64) {  // separable TF: forward * TF * inverse along y in ONE tuned pass, if it is covered
-        AxisPass f;
-        f.dtype = dtype; f.in = t0; f.ibs = 1; f.ies = kx; f.nb = kx;
+    bool fused = false;
+    if (!tf && dtype == PB_C64 && is_pow2(ky)) {  // separable TF: forward * TF * inverse along y in ONE tuned pass, if it is covered
+        AxisPass f;  // -> t1 (oy, kx)
+        f.dtype = dtype; f.in = t0;
+        along(f, 0, kx, kx, kx);
         f.L = ky; f.Llog = ky; f.n_in = ny; f.in_off = ceil_half(ky - ny);
-        f.dir = -1; f.out = t1; f.obs = 1; f.oes = kx; f.n_out = oy; f.crop_off = ceil_half(ky - oy); f.batch_contiguous = 1;
+        f.dir = -1; f.out = t1; f.n_out = oy; f.crop_off = ceil_half(ky - oy);
         f.post_e = ty; f.post_e_conj = conj_tf; f.post_b = tx; f.post_b_conj = conj_tf;
         f.roundtrip = 1;
-        int frc = is_pow2(ky) ? try_tuned_axis_pass(h, f, st) : PB_ERR_UNSUPPORTED;
-        if (frc == PB_OK) {
-            AxisPass s2;  // rows inverse from t1 (oy, kx), keep the ox centred columns, 1/(ky*kx)
-            s2.dtype = dtype; s2.in = t1; s2.ibs = kx; s2.ies = 1; s2.nb = oy;
-            s2.Llog = kx; s2.n_in = kx; s2.dir = +1;
-            s2.out = out; s2.obs = ox; s2.oes = 1; s2.n_out = ox; s2.crop_off = ceil_half(kx - ox);
-            s2.scale = 1.0 / ((double)ky * (double)kx);
-            return axis_dft(h, s2, st);
-        }
-        if (frc != PB_ERR_UNSUPPORTED) return frc;
+        const int frc = try_tuned_axis_pass(h, f, st);
+        if (frc != PB_OK && frc != PB_ERR_UNSUPPORTED) return frc;
+        fused = frc == PB_OK;
     }
-    AxisPass q;  // columns forward, times the transfer function -> t1 (ky, kx)
-    q.dtype = dtype; q.in = t0; q.ibs = 1; q.ies = kx; q.nb = kx;
-    q.Llog = ky; q.n_in = ny; q.in_off = ceil_half(ky - ny);
-    q.dir = -1; q.out = t1; q.obs = 1; q.oes = kx; q.n_out = ky; q.batch_contiguous = 1;
-    if (tf) { q.post_mat = tf; q.pm_bs = 1; q.pm_es = kx; q.pm_conj = conj_tf; }
-    else { q.post_e = ty; q.post_e_conj = conj_tf; q.post_b = tx; q.post_b_conj = conj_tf; }
-    PB_TRY(axis_dft(h, q, st));
-    AxisPass r;  // columns inverse, keep the oy centred rows -> t0 (oy, kx)
-    r.dtype = dtype; r.in = t1; r.ibs = 1; r.ies = kx; r.nb = kx;
-    r.Llog = ky; r.n_in = ky; r.dir = +1;
-    r.out = t0; r.obs = 1; r.oes = kx; r.n_out = oy; r.crop_off = ceil_half(ky - oy); r.batch_contiguous = 1;
-    PB_TRY(axis_dft(h, r, st));
-    AxisPass s;  // rows inverse, keep the ox centred columns, 1/(ky*kx)
-    s.dtype = dtype; s.in = t0; s.ibs = kx; s.ies = 1; s.nb = oy;
+    if (!fused) {
+        AxisPass q;  // columns forward, times the transfer function -> t1 (ky, kx)
+        q.dtype = dtype; q.in = t0;
+        along(q, 0, kx, kx, kx);
+        q.Llog = ky; q.n_in = ny; q.in_off = ceil_half(ky - ny);
+        q.dir = -1; q.out = t1; q.n_out = ky;
+        if (tf) { q.post_mat = tf; q.pm_bs = 1; q.pm_es = kx; q.pm_conj = conj_tf; }
+        else { q.post_e = ty; q.post_e_conj = conj_tf; q.post_b = tx; q.post_b_conj = conj_tf; }
+        PB_TRY(axis_dft(h, q, st));
+        AxisPass r;  // columns inverse, keep the oy centred rows -> t0 (oy, kx)
+        r.dtype = dtype; r.in = t1;
+        along(r, 0, kx, kx, kx);
+        r.Llog = ky; r.n_in = ky; r.dir = +1;
+        r.out = t0; r.n_out = oy; r.crop_off = ceil_half(ky - oy);
+        PB_TRY(axis_dft(h, r, st));
+    }
+    AxisPass s;  // rows inverse from the (oy, kx) result of the column passes, keep the ox centred columns, 1/(ky*kx)
+    s.dtype = dtype; s.in = fused ? t1 : t0;
+    along(s, 1, oy, kx, ox);
     s.Llog = kx; s.n_in = kx; s.dir = +1;
-    s.out = out; s.obs = ox; s.oes = 1; s.n_out = ox; s.crop_off = ceil_half(kx - ox);
+    s.out = out; s.n_out = ox; s.crop_off = ceil_half(kx - ox);
     s.scale = 1.0 / ((double)ky * (double)kx);
     return axis_dft(h, s, st);
 }

@@ -2,7 +2,6 @@
 // lanes, the two-exchange FFT_L skeleton, async-copy / TMA plumbing, and the geometry of the focus pipeline.
 // Everything device-side lives in an anonymous namespace (each translation unit gets its own copy).
 #pragma once
-#include <cstdlib>
 #include <algorithm>
 #include "fft_tuned.cuh"
 
@@ -421,16 +420,14 @@ template <int L>
 int get_col4_plan(Handle* h, const float2** out) {
     using G4 = Geo4<L>;
     using G = Geo<L>;
-    const TwKey key{L, PB_C64, TW_FOCUS_PLAN};
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) { *out = reinterpret_cast<const float2*>(it->second); return PB_OK; }
-    std::vector<std::complex<double>> tab(G4::PLANLEN);
-    for (int k = 0; k < 16; ++k)
-        for (int t = 0; t < G::NT; ++t) tab[G4::TW1 + k * G::NT + t] = host_tw((long long)t * k, L);
-    for (int k = 1; k < 16; ++k)
-        for (int m = 0; m < G::NT / 16; ++m) tab[G4::TW2 + (k - 1) * (G::NT / 16) + m] = host_tw(16LL * m * k, L);
     const void* d = nullptr;
-    PB_TRY(upload_table(h, key, tab, &d));
+    PB_TRY(cached_table(h, {L, PB_C64, TW_FOCUS_PLAN}, [](auto& tab) {
+        tab.resize(G4::PLANLEN);
+        for (int k = 0; k < 16; ++k)
+            for (int t = 0; t < G::NT; ++t) tab[G4::TW1 + k * G::NT + t] = host_tw((long long)t * k, L);
+        for (int k = 1; k < 16; ++k)
+            for (int m = 0; m < G::NT / 16; ++m) tab[G4::TW2 + (k - 1) * (G::NT / 16) + m] = host_tw(16LL * m * k, L);
+    }, &d));
     *out = reinterpret_cast<const float2*>(d);
     return PB_OK;
 }

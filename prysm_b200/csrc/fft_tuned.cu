@@ -358,29 +358,14 @@ __global__ void __launch_bounds__(4 * L / 16) focus_row4_kernel(const __grid_con
 
 
 // ---- TMA descriptors, cached in the handle by (base pointer, geometry) -----------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 int get_map_c64(Handle* h, const MapKey& key, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
                 const cuuint32_t* box, const CUtensorMap** out) {
     auto it = h->maps.find(key);
     if (it != h->maps.end()) { *out = &it->second; return PB_OK; }
-    static EncodeTiledFn fn = nullptr;   // a driver entry point: process-wide, not per device
-    if (!fn) {
-        cudaDriverEntryPointQueryResult q;
-        void* f = nullptr;
-        PB_CUDA(h, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q));
-        if (!f || q != cudaDriverEntryPointSuccess) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-        fn = reinterpret_cast<EncodeTiledFn>(f);
-    }
-    if (h->maps.size() > 256) h->maps.clear();
     CUtensorMap m;
-    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_UINT64, (cuuint32_t)rank, const_cast<void*>(key.base), dims, strides_bytes, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
+    PB_TRY(encode_tensor_map(h, &m, CU_TENSOR_MAP_DATA_TYPE_UINT64, rank, key.base, dims, strides_bytes, box,
+                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B));
+    if (h->maps.size() > 256) h->maps.clear();
     *out = &(h->maps[key] = m);
     return PB_OK;
 }
@@ -717,22 +702,16 @@ __global__ void __launch_bounds__((COLS ? TP : 1) * L / 16, (RT && (!COLS || TP 
 template <int L>
 int get_plain_plan(Handle* h, const float2** tw1, const float2** tw2) {
     using G = Geo<L>;
-    const TwKey key{L, PB_C64, TW_PLAIN_PLAN};
-    const float2* base = nullptr;
-    auto it = h->tables.find(key);
-    if (it != h->tables.end()) base = reinterpret_cast<const float2*>(it->second);
-    else {
-        std::vector<std::complex<double>> tab(15 * G::NT + 15 * (G::NT / 16));
+    const void* d = nullptr;
+    PB_TRY(cached_table(h, {L, PB_C64, TW_PLAIN_PLAN}, [](auto& tab) {
+        tab.resize(15 * G::NT + 15 * (G::NT / 16));
         for (int k = 1; k < 16; ++k)
             for (int t = 0; t < G::NT; ++t) tab[(k - 1) * G::NT + t] = host_tw((long long)t * k, L);
         for (int k = 1; k < 16; ++k)
             for (int m = 0; m < G::NT / 16; ++m) tab[15 * G::NT + (k - 1) * (G::NT / 16) + m] = host_tw(16LL * m * k, L);
-        const void* d = nullptr;
-        PB_TRY(upload_table(h, key, tab, &d));
-        base = reinterpret_cast<const float2*>(d);
-    }
-    *tw1 = base;
-    *tw2 = base + 15 * G::NT;
+    }, &d));
+    *tw1 = reinterpret_cast<const float2*>(d);
+    *tw2 = *tw1 + 15 * G::NT;
     return PB_OK;
 }
 
@@ -799,8 +778,6 @@ int dispatch_axis_reg(Handle* h, const AxisPass& p0, cudaStream_t st) {
 }  // namespace
 
 int try_tuned_axis_pass(Handle* h, const AxisPass& p, cudaStream_t st) {
-    static const bool disabled = getenv("PB_DISABLE_TUNED") != nullptr || getenv("PB_DISABLE_TUNED_AXIS") != nullptr;
-    if (disabled) return PB_ERR_UNSUPPORTED;
     if (p.dtype != PB_C64 || p.in_kind == PB_IN_AMP_OPD) return PB_ERR_UNSUPPORTED;
     if (p.out_kind != PB_OUT_COMPLEX && !p.roundtrip) return PB_ERR_UNSUPPORTED;   // |.|^2 stores: round-trip epilogue only
     if (p.pre_e2 || (p.post_e2 && !p.roundtrip) || p.post_mat) return PB_ERR_UNSUPPORTED;
@@ -815,80 +792,66 @@ int try_tuned_axis_pass(Handle* h, const AxisPass& p, cudaStream_t st) {
     }
 }
 
-int try_tuned_fft2_batch(Handle* h, int dtype, const void* in, int in_kind, const void* amp, int amp_kind, double kturns,
-                         int batch, long long in_bs, long long amp_bs, int ny, int nx, long long in_ld, int ky, int kx, int dir,
-                         double scale, int shift_in, int shift_out, void* out, int out_kind, double weight, int oy, int ox,
-                         long long out_ld, long long out_bs, cudaStream_t st) {
-    static const bool disabled = getenv("PB_DISABLE_TUNED") != nullptr;
-    if (disabled) return PB_ERR_UNSUPPORTED;
-    if (dtype != PB_C64 || ny != nx || ky != 2 * ny || kx != 2 * nx || !shift_in || !shift_out || oy != ky || ox != kx)
+int try_tuned_fft2_batch(Handle* h, const Fft2Args& a, cudaStream_t st) {
+    if (a.dtype != PB_C64 || a.ny != a.nx || a.ky != 2 * a.ny || a.kx != 2 * a.nx || !a.shift_in || !a.shift_out ||
+        a.oy != a.ky || a.ox != a.kx)
         return PB_ERR_UNSUPPORTED;
-    if (nx != 512 && nx != 1024 && nx != 2048) return PB_ERR_UNSUPPORTED;
-    if (in_kind == PB_IN_REAL) return PB_ERR_UNSUPPORTED;
-    if (out_kind == PB_OUT_COMPLEX ? (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 15) : (out_ld & 1) || (out_bs & 1) || ((uintptr_t)out & 7))
+    const int N = a.nx;
+    if (N != 512 && N != 1024 && N != 2048) return PB_ERR_UNSUPPORTED;
+    if (a.in_kind == PB_IN_REAL) return PB_ERR_UNSUPPORTED;
+    if ((a.out_ld & 1) || (a.out_bs & 1) || ((uintptr_t)a.out & (a.out_kind == PB_OUT_COMPLEX ? 15 : 7)))
         return PB_ERR_UNSUPPORTED;  // vector stores need aligned rows
-    const int N = nx;
     // Inputs tensor TMA can gather (complex, 16-byte aligned base, even pitches) go to the pair as they are; every other
     // one is first written as a dense aligned field in scratch slot 1, one field at a time
-    const bool staged = in_kind != PB_IN_COMPLEX || ((uintptr_t)in & 15) || (in_ld & 1) || (in_bs & 1);
+    const bool staged = a.in_kind != PB_IN_COMPLEX || ((uintptr_t)a.in & 15) || (a.in_ld & 1) || (a.in_bs & 1);
     // the fields of a stack alternate between two intermediates (field f: buffer f mod 2), so that a column kernel never
     // writes what the row kernel before it reads (focus_col4_kernel)
-    const int nbuf = batch > 1 ? 2 : 1;
+    const int nbuf = a.batch > 1 ? 2 : 1;
     const size_t field_bytes = (size_t)N * N * sizeof(float2);
     void* tmp = nullptr;
     PB_TRY(ensure_scratch(h, 0, nbuf * 2 * field_bytes, &tmp));
     void* stage = nullptr;
     if (staged) PB_TRY(ensure_scratch(h, 1, field_bytes, &stage));
     // the column kernels' tile counters, one per buffer: zeroed once here, then by each field's row kernel
-    const TwKey key{2, PB_C64, TW_TILE_COUNTERS};
-    auto it = h->tables.find(key);
-    const void* d = it != h->tables.end() ? it->second : nullptr;
-    if (!d) PB_TRY(upload_table(h, key, std::vector<std::complex<double>>(1), &d));   // one complex64 zero = two counters
+    const void* d = nullptr;
+    PB_TRY(cached_table(h, {2, PB_C64, TW_TILE_COUNTERS}, [](auto& t) { t.resize(1); }, &d));   // one complex64 zero = two counters
     unsigned int* ctr = reinterpret_cast<unsigned int*>(const_cast<void*>(d));
-    const size_t in_elt = in_kind == PB_IN_COMPLEX ? sizeof(float2) : sizeof(float);
-    const size_t amp_elt = amp_kind == PB_AMP_U8 ? 1 : sizeof(float);
-    const size_t out_elt = out_kind == PB_OUT_COMPLEX ? sizeof(float2) : sizeof(float);
     // fields after the first of an unstaged stack: the column kernel follows this call's previous row kernel
     // (programmatic dependent launch, see launch_focus2); it may gather its input early unless the input stack overlaps
     // the output stack.  A staged field's column kernel is launched plainly, after its staging launch, which is plain too
     // and so follows the previous field's row kernel.
-    const uintptr_t in_lo = (uintptr_t)in, in_hi = in_lo + (size_t)((long long)(batch - 1) * in_bs + (long long)(ny - 1) * in_ld + nx) * in_elt;
-    const uintptr_t out_lo = (uintptr_t)out, out_hi = out_lo + (size_t)((long long)(batch - 1) * out_bs + (long long)(ky - 1) * out_ld + kx) * out_elt;
+    const uintptr_t in_lo = (uintptr_t)a.in,
+                    in_hi = in_lo + (size_t)((long long)(a.batch - 1) * a.in_bs + (long long)(a.ny - 1) * a.in_ld + a.nx) * a.in_elt();
+    const uintptr_t out_lo = (uintptr_t)a.out,
+                    out_hi = out_lo + (size_t)((long long)(a.batch - 1) * a.out_bs + (long long)(a.ky - 1) * a.out_ld + a.kx) * a.out_elt();
     const int col_dep_next = staged ? 0 : (in_hi <= out_lo || out_hi <= in_lo) ? 2 : 1;
-    for (int b = 0; b < batch; ++b) {
+    for (int b = 0; b < a.batch; ++b) {
+        const Fft2Args f = a.field(b);
         FocusParams p = {};
-        p.in = reinterpret_cast<const char*>(in) + (size_t)b * in_bs * in_elt;   // (16-byte aligned if not staged: in_bs is even)
-        p.in_ld = in_ld;
+        p.in = f.in;   // (16-byte aligned if not staged: in_bs is even)
+        p.in_ld = a.in_ld;
         if (staged) {
-            if (in_kind == PB_IN_AMP_OPD) {
-                const void* a = amp ? reinterpret_cast<const char*>(amp) + (size_t)b * amp_bs * amp_elt : nullptr;
-                PB_TRY(launch_phase_screen(h, PB_C64, a, amp_kind, p.in, kturns, (long long)N * N, N, in_ld, stage, st));
+            if (a.in_kind == PB_IN_AMP_OPD) {
+                PB_TRY(launch_phase_screen(h, PB_C64, f.amp, a.amp_kind, p.in, a.kturns(), (long long)N * N, N, a.in_ld, stage, st));
             } else {
-                PB_CUDA(h, cudaMemcpy2DAsync(stage, N * sizeof(float2), p.in, in_ld * sizeof(float2), N * sizeof(float2), N,
+                PB_CUDA(h, cudaMemcpy2DAsync(stage, N * sizeof(float2), p.in, a.in_ld * sizeof(float2), N * sizeof(float2), N,
                                              cudaMemcpyDeviceToDevice, st));
             }
             p.in = stage;
             p.in_ld = N;
         }
         p.tmp = reinterpret_cast<float2*>(reinterpret_cast<char*>(tmp) + (size_t)(b % nbuf) * 2 * field_bytes);
-        p.out = reinterpret_cast<char*>(out) + (size_t)b * out_bs * out_elt;
-        p.out_ld = out_ld; p.out_kind = out_kind; p.scale = (float)scale; p.weight = (float)weight;
-        p.out_bs = out_bs;
+        p.out = f.out;
+        p.out_ld = a.out_ld; p.out_kind = a.out_kind; p.scale = (float)a.scale; p.weight = (float)a.weight;
+        p.out_bs = a.out_bs;
         p.tile_ctr = ctr + (b % nbuf);
         const int cd = b > 0 ? col_dep_next : 0;
         int rc;
-        if (dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
+        if (a.dir < 0) rc = N == 512 ? launch_focus2<512, false>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, false>(h, p, cd, st) : launch_focus2<2048, false>(h, p, cd, st);
         else rc = N == 512 ? launch_focus2<512, true>(h, p, cd, st) : N == 1024 ? launch_focus2<1024, true>(h, p, cd, st) : launch_focus2<2048, true>(h, p, cd, st);
         if (rc != PB_OK) return rc;
     }
     return PB_OK;
-}
-
-int try_tuned_fft2(Handle* h, int dtype, const void* in, int in_kind, const void* amp, int amp_kind, double kturns,
-                   int ny, int nx, long long in_ld, int ky, int kx, int dir, double scale, int shift_in, int shift_out,
-                   void* out, int out_kind, double weight, int oy, int ox, long long out_ld, cudaStream_t st) {
-    return try_tuned_fft2_batch(h, dtype, in, in_kind, amp, amp_kind, kturns, 1, 0, 0, ny, nx, in_ld, ky, kx, dir, scale,
-                                shift_in, shift_out, out, out_kind, weight, oy, ox, out_ld, 0, st);
 }
 
 

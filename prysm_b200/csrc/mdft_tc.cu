@@ -367,28 +367,12 @@ __global__ void reduce_splits_kernel(const float* __restrict__ ws, int splits, i
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 int make_map(Handle* h, CUtensorMap* map, const void* base, long long rows, long long cols, int box_rows) {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        cudaDriverEntryPointQueryResult q;
-        void* f = nullptr;
-        PB_CUDA(h, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q));
-        if (!f || q != cudaDriverEntryPointSuccess) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-        fn = reinterpret_cast<EncodeTiledFn>(f);
-    }
     const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     const cuuint64_t gstr[1] = {(cuuint64_t)cols * sizeof(float)};
     const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstr, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(h, PB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
-    return PB_OK;
+    return encode_tensor_map(h, map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // C'(M x N) = A'(M x K) @ B'(N x K)^T on the tensor cores; see GemmParams for the output modes.  Split-K: `splits`
