@@ -61,6 +61,21 @@ __global__ void mul_outer_kernel(const cplx<R>* __restrict__ in, long long in_ld
     }
 }
 
+// Complex division in fp64, rounded once to R by the caller: x * w with w = conj(y) / |y|^2.  For float operands the
+// fp64 |y|^2 neither overflows nor goes subnormal anywhere in the float range (in R = float it overflows above
+// |y| ~ 1.8e19 and loses bits below ~1e-19); for double operands it holds for 1e-154 < |y| < 1e154 (DESIGN.md §4.4).
+// One fp64 reciprocal per divisor: no slower than the two float divisions it replaces.
+template <typename R>
+__device__ inline double2 crecip_fp64(cplx<R> y) {
+    const double yx = y.x, yy = y.y, inv = 1.0 / (yx * yx + yy * yy);
+    return make_double2(yx * inv, -yy * inv);
+}
+
+template <typename R>
+__device__ inline double2 cmul_fp64(cplx<R> x, double2 w) {
+    return make_double2((double)x.x * w.x - (double)x.y * w.y, (double)x.x * w.y + (double)x.y * w.x);
+}
+
 // out = a (op) b, or with b == nullptr a (op) scalar; reverse swaps the operands.  op: 0 mul, 1 div, 2 add, 3 sub
 template <typename R>
 __global__ void binary_kernel(int op, const cplx<R>* __restrict__ a, const cplx<R>* __restrict__ b, cplx<R> sc,
@@ -70,7 +85,7 @@ __global__ void binary_kernel(int op, const cplx<R>* __restrict__ a, const cplx<
         if (reverse) { cplx<R> t = x; x = y; y = t; }
         cplx<R> r;
         if (op == 0) r = cmul(x, y);
-        else if (op == 1) { const R d = y.x * y.x + y.y * y.y; r = cmulc(x, y); r.x /= d; r.y /= d; }
+        else if (op == 1) { const double2 q = cmul_fp64<R>(x, crecip_fp64<R>(y)); r = mk<R>((R)q.x, (R)q.y); }
         else if (op == 2) r = cadd(x, y);
         else r = csub(x, y);
         out[i] = r;
@@ -93,12 +108,10 @@ __global__ void weighted_sum_kernel(const R* __restrict__ modes, int k, long lon
 template <typename R>
 __global__ void otf_normalize_kernel(const cplx<R>* __restrict__ D, long long n, long long centre, int which,
                                      R* __restrict__ mtf, R* __restrict__ ptf, cplx<R>* __restrict__ otf) {
-    const cplx<R> c = D[centre];
-    const R den = c.x * c.x + c.y * c.y;
+    const double2 w = crecip_fp64<R>(D[centre]);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        cplx<R> v = D[i];
-        cplx<R> q = cmulc(v, c);  // v * conj(c)
-        q.x /= den; q.y /= den;
+        const double2 qd = cmul_fp64<R>(D[i], w);
+        const cplx<R> q = mk<R>((R)qd.x, (R)qd.y);      // the quotient, rounded once to R
         if (which & 1) mtf[i] = hypot(q.x, q.y);
         if (which & 2) ptf[i] = atan2(q.y, q.x);
         if (which & 4) otf[i] = q;
