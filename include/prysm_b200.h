@@ -83,7 +83,12 @@ long long pb_launch_count(pb_handle_t h);
  *   PB_ROUTE_MDFT_REDUCE  reduce_splits_kernel, the sum of the split-K partial planes; L = pieces, flags = 0
  *   PB_ROUTE_CGEMM        cgemm_kernel<R, OPA, OPB> of the CUDA-core GEMM (pb_cgemm, pb_mdft_apply); L = 0,
  *                         flags DTYPE | OPA << 1 | OPB << 3 (DTYPE: PB_C64 / PB_C128; OP as in pb_cgemm)
- * Returns -1 for a NULL handle. */
+ *   PB_ROUTE_CENTROID     centroid_kernel<T, O, V> of pb_subaperture_centroids; L = V (grid columns per thread: 4, or
+ *                         1 for a row length or frame alignment that rules out vector loads, or more than 614 lenslet
+ *                         columns), flags = the frame's pb_elem_type
+ *   PB_ROUTE_PSI          psi_kernel of pb_psi; L = V (samples per thread: 16 / element size, or 1 for a misaligned
+ *                         frame or output or an n that is not a multiple of it), flags = 1 for int64 sums, else 0
+ * The key is a 32-bit int: kinds 8 and up set its sign bit.  Returns -1 for a NULL handle. */
 typedef enum {
     PB_ROUTE_AXIS_REG = 1,
     PB_ROUTE_AXIS_GENERIC = 2,
@@ -91,7 +96,9 @@ typedef enum {
     PB_ROUTE_FOCUS_V2 = 4,
     PB_ROUTE_MDFT_TC = 5,
     PB_ROUTE_MDFT_REDUCE = 6,
-    PB_ROUTE_CGEMM = 7
+    PB_ROUTE_CGEMM = 7,
+    PB_ROUTE_CENTROID = 8,
+    PB_ROUTE_PSI = 9
 } pb_route_kind;
 long long pb_route_launch_count(pb_handle_t h, int route);
 

@@ -22,11 +22,13 @@ ROUTE_AXIS_REG, ROUTE_AXIS_GENERIC, ROUTE_FOCUS_V2 = 1, 2, 4
 # and the name stays so that code written against it keeps working
 ROUTE_FOCUS_V1 = 3
 ROUTE_MDFT_TC, ROUTE_MDFT_REDUCE, ROUTE_CGEMM = 5, 6, 7
+ROUTE_CENTROID, ROUTE_PSI = 8, 9
 
 
 def route_code(kind, L=0, flags=0):
-    """the `route` argument of pb_route_launch_count"""
-    return kind << 28 | L << 8 | flags
+    """the `route` argument of pb_route_launch_count: the 32-bit int the C side forms (kinds 8 and up are negative)"""
+    code = (kind << 28 | L << 8 | flags) & 0xFFFFFFFF
+    return code - (1 << 32) if code >> 31 else code
 
 _vp, _i, _ll, _d = C.c_void_p, C.c_int, C.c_longlong, C.c_double
 

@@ -204,8 +204,10 @@ inline int fail(Handle* h, int code, const std::string& msg) {
         (h)->launches++;                                                                      \
     } while (0)
 
-// key of Handle::route_launches (pb_route_launch_count)
-constexpr int route_code(int kind, int L, int flags) { return kind << 28 | L << 8 | flags; }
+// key of Handle::route_launches (pb_route_launch_count); kinds 8 and up set the sign bit, so the key is formed unsigned
+constexpr int route_code(int kind, int L, int flags) {
+    return (int)((unsigned)kind << 28 | (unsigned)L << 8 | (unsigned)flags);
+}
 
 #define PB_TRY(expr)               \
     do {                           \

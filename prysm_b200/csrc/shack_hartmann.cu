@@ -75,10 +75,12 @@ __global__ void __launch_bounds__(kThreads) lenslet_screen_kernel(
 // One CTA per (lenslet row j, frame f).  It reads the rows of j's band whole: thread t takes grid columns
 // c0 + V t .. c0 + V t + V - 1 of each chunk of V kThreads columns, loads them as one vector per row and sums down the
 // band, so a warp's load of one row is 32 V contiguous elements (V = 4: 256 bytes of uint16, 512 of float32).  The
-// column sums go through shared memory to the lenslet columns, each of which one thread sums in column order.  With a
-// threshold a first sweep finds each subaperture's maximum (order-free) before the weighted sums.  The sums of a
-// column and of a lenslet do not depend on V, so every V gives the same bits; V = 1 serves rows whose length or
-// alignment does not allow vector loads.
+// column sums go through shared memory to the lenslet columns, each of which one thread sums in column order, carrying
+// its sums from one chunk to the next.  With a threshold a first sweep finds each subaperture's maximum (order-free)
+// before the weighted sums.  The sums of a column and of a lenslet do not depend on V, so every V gives the same bits.
+// V = 1 serves rows whose length is not a multiple of 4, frames whose start or stride is not aligned to a vector, and
+// rows of more than 614 lenslets: the shared memory holds 5 ncols + 3 kThreads V doubles, at most 48 KB, so V = 4 takes
+// ncols <= 614 and V = 1 ncols <= 1075; more lenslet columns are refused.
 //
 // dtab (fp64): x of each grid column [W], y of each grid row [H], lenslet centres xc [ncols], yc [nrows].
 // itab (int32): owner lenslet column of each grid column or -1 [W], owned grid-column range of each lenslet column
@@ -300,6 +302,7 @@ extern "C" int pb_subaperture_centroids(pb_handle_t hh, int frame_type, const vo
         }
     });
     PB_LAUNCH_CHECK(h);
+    h->route_launches[route_code(PB_ROUTE_CENTROID, vec ? kCentroidVec : 1, frame_type)]++;
     return PB_OK;
 }
 

@@ -24,11 +24,17 @@ constexpr double kEulerGamma = 0.57721566490153286061;
 // ---- Bessel functions ----------------------------------------------------------------------------------------------
 // J_l(x), x >= 0.  Orders 0 and 1 are CUDA's j0 / j1.  Above: forward recurrence from them where x > l (stable
 // there), Miller's backward recurrence below, normalised by J0 + 2 (J2 + J4 + ...) = 1 and rescaled against overflow.
-// (CUDA's jn returns NaN at x = 0 and carries ~1e-14 absolute error at moderate x.)
+// (CUDA's jn returns NaN at x = 0 and carries ~1e-14 absolute error at moderate x.)  Below x = 1e-20 the leading term
+// of the series, (x/2)^l / l!, is J_l to a relative 1e-40; Miller's rescaling by 1e-100 per step cannot keep up there
+// once j * 2 / x passes 1e100, so the recurrence would overflow to NaN.
 __device__ double bessel_j(int l, double x) {
     if (l == 0) return j0(x);
     if (l == 1) return j1(x);
-    if (x < 1e-100) return 0.0;                  // below any representable J_l, l >= 2
+    if (x < 1e-20) {
+        double t = 1.0;
+        for (int k = 1; k <= l; ++k) t *= 0.5 * x / k;
+        return t;
+    }
     const double tox = 2.0 / x;
     if (x > l) {
         double bjm = j0(x), bj = j1(x);
@@ -232,10 +238,12 @@ __global__ void __launch_bounds__(kThreads) overlap_finish_kernel(const double* 
         double t[4] = {0.0, 0.0, 0.0, 0.0};
         for (int w = 0; w < kThreads / 32; ++w)
             for (int k = 0; k < 4; ++k) t[k] += sh[w][k];
+        // eta = q^2 with q = |sum conj(M) E| / sqrt(I_p I_E) <= 1: formed without squaring a sum, so fields far from
+        // unit magnitude (|E| ~ 1e150 or 1e-150 in fp64) neither overflow nor underflow
         const double ip = ip_in ? ip_in[p] : t[2], ie = ie_in ? ie_in[0] : t[3];
-        const double e = (t[0] * t[0] + t[1] * t[1]) / (ip * ie);
-        eta[p] = (R)e;
-        if (c_out && p == 0) c_out[0] = (R)sqrt(ie * e);
+        const double q = hypot(t[0], t[1]) / sqrt(ip) / sqrt(ie);
+        eta[p] = (R)(q * q);
+        if (c_out && p == 0) c_out[0] = (R)(sqrt(ie) * q);
     }
 }
 
@@ -486,6 +494,7 @@ extern "C" int pb_psi(pb_handle_t hh, int frame_type, int nframes, const void* c
         const long long groups = n / V;
         psi_kernel<T, V, decltype(acc), NT, PT><<<grid_for(groups, kThreads, h->sm_count), kThreads, 0, st>>>(
             nframes, groups, plan, (NT*)num, (NT*)den, (PT*)phase);
+        h->route_launches[route_code(PB_ROUTE_PSI, V, std::is_same<decltype(acc), long long>::value)]++;
     };
     auto dispatch = [&](auto t, auto vv) {
         using T = decltype(t);
