@@ -72,12 +72,14 @@ struct ZernPlan {
 // MODE 2 (POLAR): out[k][0|1][i] = w dZ_k/dr, w dZ_k/dt  (zernike_nm_der_seq)
 // MODE 3: out[k][0|1][i] = w dZ_k/dx, w dZ_k/dy  (zernike_nm_der_xy_seq)
 // MODE 4: out[0|1|2][i] (+)= W, dW/dx, dW/dy of W = sum w Z_k  (zernike_sum_der_xy)
+// MODES 1 and 4 split over several plans carry the partial sums from launch to launch in the fp64 `stage` (the output
+// itself for fp64 storage, so neither `stage` nor `out` is __restrict__) and round to R once, in the `last` launch.
 // POLAR: inputs are (r, t); otherwise Cartesian (x, y) with r = hypot, cos t = x/r, sin t = y/r.  The derivative modes
 // carry dP_j/dx2 beside P_j (seed (|m| + 2)/2, the differentiated recurrence); MODE 2 forms r^|m|, r^(|m|-1) and
 // cos / sin(|m| t) per group, MODES 3 and 4 C_k, S_k = Re, Im (x + iy)^k for k = |m| and |m| - 1, finite at the origin.
 template <typename R, int MODE, bool POLAR>
 __global__ void zernike_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, const __grid_constant__ ZernPlan pl,
-                               int accumulate, R* __restrict__ out) {
+                               int accumulate, int last, double* stage, R* out) {
     constexpr bool DER = MODE >= 2, XY = MODE >= 3;
     PB_GRID_STRIDE(i, n) {
         double r = 0.0, c1 = 1.0, s1 = 0.0, xv = 0.0, yv = 0.0, tv = 0.0;
@@ -176,12 +178,17 @@ __global__ void zernike_kernel(const R* __restrict__ a, const R* __restrict__ b,
                 accy += 4.0 * yv * dH + am * (Sb * hc1 - Sa * hs1);
             }
         }
-        if constexpr (MODE == 1) out[i] = accumulate ? (R)((double)out[i] + acc) : (R)acc;
+        if constexpr (MODE == 1) {
+            if (accumulate) acc += stage[i];
+            if (last) out[i] = (R)acc;
+            else stage[i] = acc;
+        }
         if constexpr (MODE == 4) {
             if (accumulate) {
-                acc += (double)out[i]; accx += (double)out[n + i]; accy += (double)out[2 * n + i];
+                acc += stage[i]; accx += stage[n + i]; accy += stage[2 * n + i];
             }
-            out[i] = (R)acc; out[n + i] = (R)accx; out[2 * n + i] = (R)accy;
+            if (last) { out[i] = (R)acc; out[n + i] = (R)accx; out[2 * n + i] = (R)accy; }
+            else { stage[i] = acc; stage[n + i] = accx; stage[2 * n + i] = accy; }
         }
     }
 }
@@ -304,6 +311,13 @@ extern "C" int pb_circle(pb_handle_t hh, int dtype, const void* r, long long cou
     return PB_OK;
 }
 
+// a radial order no plan can hold is refused before the first of several launches
+static int zernike_fits(Handle* h, const std::vector<HostTerm>& terms) {
+    for (const HostTerm& t : terms)
+        if (t.nj + 1 > PB_ZERN_STEPS) return fail(h, PB_ERR_UNSUPPORTED, "zernike: (n - |m|)/2 above 71");
+    return PB_OK;
+}
+
 template <int MODE>
 static int run_zernike(Handle* h, int dtype, int polar, const void* a, const void* b, long long count,
                        std::vector<HostTerm>& terms, void* out, cudaStream_t st) {
@@ -313,14 +327,24 @@ static int run_zernike(Handle* h, int dtype, int polar, const void* a, const voi
         PB_CUDA(h, cudaMemsetAsync(out, 0, (size_t)count * rsize(dtype) * (MODE == 4 ? 3 : 1), st));
         return PB_OK;
     }
+    double* stage = nullptr;
     while (!terms.empty()) {
         ZernPlan pl;
         PB_TRY(next_plan(terms, pl));
-        const int acc = launches > 0;
+        const int acc = launches > 0, last = terms.empty();
+        if ((MODE == 1 || MODE == 4) && !last && !stage) {
+            // the partial sums of a split call stay in fp64 until the last launch rounds them once
+            if (dtype == PB_C128) stage = (double*)out;
+            else {
+                void* p = nullptr;
+                PB_TRY(ensure_scratch(h, 2, (size_t)count * sizeof(double) * (MODE == 4 ? 3 : 1), &p));
+                stage = (double*)p;
+            }
+        }
         with_real(dtype, [&](auto r) {
             using R = decltype(r);
-            if (polar) zernike_kernel<R, MODE, true><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, (R*)out);
-            else zernike_kernel<R, MODE, false><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, (R*)out);
+            if (polar) zernike_kernel<R, MODE, true><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, last, stage, (R*)out);
+            else zernike_kernel<R, MODE, false><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, pl, acc, last, stage, (R*)out);
         });
         PB_LAUNCH_CHECK(h);
         ++launches;
@@ -336,6 +360,7 @@ extern "C" int pb_zernike_seq(pb_handle_t hh, int dtype, int polar, const void* 
     if (count <= 0) return PB_OK;
     std::vector<HostTerm> terms;
     PB_TRY(build_terms(h, k, n_host, m_host, nullptr, norm, terms));
+    PB_TRY(zernike_fits(h, terms));
     return run_zernike<0>(h, dtype, polar, a, b, count, terms, out, st);
 }
 
@@ -347,14 +372,8 @@ extern "C" int pb_zernike_sum(pb_handle_t hh, int dtype, int polar, const void* 
     if (count <= 0) return PB_OK;
     std::vector<HostTerm> terms;
     PB_TRY(build_terms(h, k, n_host, m_host, coefs_host, norm, terms));
+    PB_TRY(zernike_fits(h, terms));
     return run_zernike<1>(h, dtype, polar, a, b, count, terms, out, st);
-}
-
-// a radial order no plan can hold is refused before the first of several launches
-static int zernike_fits(Handle* h, const std::vector<HostTerm>& terms) {
-    for (const HostTerm& t : terms)
-        if (t.nj + 1 > PB_ZERN_STEPS) return fail(h, PB_ERR_UNSUPPORTED, "zernike: (n - |m|)/2 above 71");
-    return PB_OK;
 }
 
 extern "C" int pb_zernike_der(pb_handle_t hh, int dtype, int cartesian, const void* a, const void* b, long long count, int k,
