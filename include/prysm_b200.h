@@ -746,6 +746,50 @@ int pb_field_at_depth(pb_handle_t h, int dtype, int pol, int nlayers, const void
                       const void* n, double n0_re, double n0_im, double wvl, double theta0, const void* E_b,
                       const void* H_b, void* E, void* H, void* stream);
 
+/* ---- PSF / MTF analysis (prysm/_richdata.py, prysm/coordinates.py uniform_cart_to_polar, prysm/psf.py, prysm/otf.py) --
+ * Data is (ny, nx) on the fp64 ascending axes xax (nx) and yax (ny), device arrays.  Every sampling entry point uses one
+ * linear interpolator, scipy's RegularGridInterpolator(method='linear'): interval = the largest i with axis[i] <= p
+ * clipped to [0, n - 2]; fp64 weights; the four corners summed in scipy's order without fused multiply-add, so a NaN
+ * at any corner gives NaN even at weight 0; a point outside the axes gives `fill`.  An axis of one sample has weight 0.
+ * The polar lattice is uniform_cart_to_polar's: rho_j = linspace(0, rmax, nx), phi_i = linspace(0, 2 pi, ny), the
+ * point (rho_j cos phi_i, rho_j sin phi_i), fill 0, all in fp64; it is (ny, nx), phi along rows.
+ * pb_interp2d_linear: type PB_ELEM_F32 / F64 / C64 / C128; rows of data are ld elements apart.  mode PB_INTERP_POINTS:
+ *   out[k] = f(px[k], py[k]) (fp64 device arrays, count points); PB_INTERP_POLAR: out (ny, nx) = f on the lattice
+ *   (px, py, count and fill unused).  out has data's type.  One launch.
+ * pb_azimuthal_stats: type PB_ELEM_F32 / F64, data dense.  For every rho column j of the lattice, the statistics over
+ *   phi that `stats` (a mask of pb_az_stat) asks for, ignoring NaN, into row log2(bit) of out (6, nx) of data's type:
+ *   count, mean, variance (ddof 0, two passes), min, max, median (the mean of the two middle values for an even count).
+ *   A column without a number gives NaN (count 0).  One launch; one block per column holds its ny samples in shared
+ *   memory, so ny <= PB_AZ_MAX_NY (else PB_ERR_INVALID before any launch).  fp64 arithmetic, fixed-order reductions.
+ * pb_polar_crossings: estimate_size's core.  The level is metric (relative = 0) or metric * the lattice maximum
+ *   (relative != 0; NaN if any lattice sample is NaN).  Along each phi row, the first (last = 0) or last i with
+ *   (v[i] > level) != (v[i + 1] > level) gives the radius rho_i + frac (rho_{i+1} - rho_i), frac = (level - v[i]) /
+ *   (v[i + 1] - v[i]), 0 where v[i + 1] == v[i].  result (HOST, 2): the number of rows that cross, and the fixed-order
+ *   fp64 mean of their radii.  Up to four launches in the handle's scratch; the call waits for them.
+ * pb_analytic_radial: out[k] = f(x[k]) in fp64, rounded once to out_type (in_type, out_type PB_ELEM_F32 / F64);
+ *   a = wavelength, b = F/#.  jinc(u) = j1(u) / u, 0.5 for |u| < 1e-8; core(s) = (2 / pi)(acos s - s sqrt(1 - s^2)).
+ *   PB_AR_AIRYDISK (2 jinc(u))^2 and PB_AR_AIRYDISK_EFIELD 2 jinc(u), u = x pi / a / b;  PB_AR_AIRYDISK_FT core(min(|x| /
+ *   (1 / (a b)), 1));  PB_AR_DIFFLIM_MTF core(min(|x / (1 / (a / 1000 b))|, 1));  PB_AR_DIFFLIM_NORMALIZED core(min(x,
+ *   1));  PB_AR_EE_CIRCULAR 1 - J0(p)^2 - J1(p)^2, p = x pi / b / a.  One launch. */
+typedef enum { PB_INTERP_POINTS = 0, PB_INTERP_POLAR = 1 } pb_interp_mode;
+typedef enum {
+    PB_AZ_COUNT = 1, PB_AZ_MEAN = 2, PB_AZ_VAR = 4, PB_AZ_MIN = 8, PB_AZ_MAX = 16, PB_AZ_MEDIAN = 32, PB_AZ_ALL = 63
+} pb_az_stat;
+typedef enum { PB_AZ_MAX_NY = 28672 } pb_az_limit;
+typedef enum {
+    PB_AR_AIRYDISK = 0, PB_AR_AIRYDISK_EFIELD = 1, PB_AR_AIRYDISK_FT = 2, PB_AR_DIFFLIM_MTF = 3, PB_AR_DIFFLIM_NORMALIZED = 4,
+    PB_AR_EE_CIRCULAR = 5
+} pb_analytic_kind;
+int pb_interp2d_linear(pb_handle_t h, int type, const void* data, int ny, int nx, long long ld, const double* xax,
+                       const double* yax, int mode, const double* px, const double* py, long long count, double rmax,
+                       double fill, void* out, void* stream);
+int pb_azimuthal_stats(pb_handle_t h, int type, const void* data, int ny, int nx, const double* xax, const double* yax,
+                       double rmax, int stats, void* out, void* stream);
+int pb_polar_crossings(pb_handle_t h, int type, const void* data, int ny, int nx, const double* xax, const double* yax,
+                       double rmax, double metric, int relative, int last, double* result, void* stream);
+int pb_analytic_radial(pb_handle_t h, int in_type, int out_type, int kind, const void* x, long long count, double a,
+                       double b, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -142,6 +142,10 @@ SIGNATURES = {
     'pb_stack_grad': (_i, [_vp, _i, _i, _i, _i, _i, C.POINTER(_ll), C.POINTER(_ll), C.POINTER(_vp), _vp, _vp,
                            C.POINTER(_vp), _vp, _vp]),
     'pb_field_at_depth': (_i, [_vp, _i, _i, _i, _vp, _ll, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _vp, _vp, _vp]),
+    'pb_interp2d_linear': (_i, [_vp, _i, _vp, _i, _i, _ll, _vp, _vp, _i, _vp, _vp, _ll, _d, _d, _vp, _vp]),
+    'pb_azimuthal_stats': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _d, _i, _vp, _vp]),
+    'pb_polar_crossings': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _d, _d, _i, _i, C.POINTER(_d), _vp]),
+    'pb_analytic_radial': (_i, [_vp, _i, _i, _i, _vp, _ll, _d, _d, _vp, _vp]),
 }
 
 SDF_POLYGON, SDF_SPIDER, SDF_RECTANGLE, SDF_FILLET_RECTANGLE, SDF_ANNULUS, SDF_OFFSET_CIRCLE = range(6)
@@ -174,6 +178,11 @@ TF_IN_WVL, TF_IN_THETA, TF_IN_N0, TF_IN_NSUB, TF_IN_N, TF_IN_D, TF_NOPS = range(
  TF_NOUT) = range(11)
 TF_GRAD_THICKNESS, TF_GRAD_INDEX = 1, 2
 TF_DIMS = 4
+INTERP_POINTS, INTERP_POLAR = range(2)
+AZ_COUNT, AZ_MEAN, AZ_VAR, AZ_MIN, AZ_MAX, AZ_MEDIAN = 1, 2, 4, 8, 16, 32
+AZ_ALL = 63
+AZ_MAX_NY = 28672
+AR_AIRYDISK, AR_AIRYDISK_EFIELD, AR_AIRYDISK_FT, AR_DIFFLIM_MTF, AR_DIFFLIM_NORMALIZED, AR_EE_CIRCULAR = range(6)
 
 
 def load_library(path=LIB_PATH):

@@ -1464,6 +1464,72 @@ def field_at_depth(pol, z, zb, n, n0, wvl, theta0, Eb, Hb, cdtype):
     return E, H
 
 
+def _analysis_data(data, types):
+    """data as a dense 2-D tensor of one of `types`; anything else is refused before any launch"""
+    if not isinstance(data, torch.Tensor) or data.ndim != 2:
+        raise ValueError(f'data must be a 2-D CUDA tensor, got {getattr(data, "shape", type(data))}')
+    if data.dtype not in types:
+        raise ValueError(f'data of {data.dtype} is not supported ({", ".join(str(t) for t in types)})')
+    return data.contiguous()
+
+
+def interp2d_linear(data, xax, yax, px=None, py=None, rmax=None, fill=0.0, ld=None):
+    """Linear interpolation of (ny, nx) data on the fp64 axes xax, yax (pb_interp2d_linear): at the fp64 points (px, py)
+    -- out has px's shape -- or, with rmax, on the (ny, nx) polar lattice of uniform_cart_to_polar.  `ld` is the row
+    pitch of a strided data view (one row or column of a larger array)."""
+    if ld is None:
+        data = _analysis_data(data, (torch.float32, torch.float64, torch.complex64, torch.complex128))
+        ld = data.shape[1]
+    ny, nx = data.shape
+    if rmax is not None:
+        out = torch.empty((ny, nx), dtype=data.dtype, device=data.device)
+        _call(lib.pb_interp2d_linear, data, _ELEM[data.dtype], _p(data), ny, nx, ld, _p(xax), _p(yax),
+              capi.INTERP_POLAR, None, None, 0, float(rmax), 0.0, _p(out))
+        return out
+    shape = px.shape
+    px, py = px.reshape(-1).contiguous(), py.reshape(-1).contiguous()
+    out = torch.empty(shape, dtype=data.dtype, device=data.device)
+    _call(lib.pb_interp2d_linear, data, _ELEM[data.dtype], _p(data), ny, nx, ld, _p(xax), _p(yax), capi.INTERP_POINTS,
+          _p(px), _p(py), px.numel(), 0.0, float(fill), _p(out))
+    return out
+
+
+def azimuthal_stats(data, xax, yax, rmax, stats):
+    """(6, nx) of data's dtype: rows count, mean, var, min, max, median over phi of each rho column of the polar lattice,
+    the rows `stats` (a mask of AZ_*) asks for filled, in one launch (pb_azimuthal_stats)."""
+    data = _analysis_data(data, (torch.float32, torch.float64))
+    ny, nx = data.shape
+    if ny > capi.AZ_MAX_NY:
+        raise ValueError(f'azimuthal statistics hold a column on chip: at most {capi.AZ_MAX_NY} phi samples (rows), '
+                         f'got {ny}')
+    out = torch.full((6, nx), float('nan'), dtype=data.dtype, device=data.device)
+    _call(lib.pb_azimuthal_stats, data, _ELEM[data.dtype], _p(data), ny, nx, _p(xax), _p(yax), float(rmax), int(stats),
+          _p(out))
+    return out
+
+
+def polar_crossings(data, xax, yax, rmax, metric, relative, last):
+    """(rows that cross, mean crossing radius) of estimate_size on the polar lattice (pb_polar_crossings); the call
+    waits for the device."""
+    data = _analysis_data(data, (torch.float32, torch.float64))
+    ny, nx = data.shape
+    res = (C.c_double * 2)()
+    _call(lib.pb_polar_crossings, data, _ELEM[data.dtype], _p(data), ny, nx, _p(xax), _p(yax), float(rmax),
+          float(metric), int(bool(relative)), int(bool(last)), res)
+    return int(res[0]), res[1]
+
+
+def analytic_radial(kind, x, a, b, out_dtype):
+    """f(x) of one AR_* kind elementwise in fp64, stored as out_dtype (pb_analytic_radial); a = wavelength, b = F/#."""
+    if x.dtype not in (torch.float32, torch.float64):
+        x = x.to(torch.float64)
+    x = x.contiguous()
+    out = torch.empty(x.shape, dtype=out_dtype, device=x.device)
+    _call(lib.pb_analytic_radial, x, _ELEM[x.dtype], _ELEM[out_dtype], int(kind), _p(x), x.numel(), float(a), float(b),
+          _p(out))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

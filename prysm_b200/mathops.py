@@ -15,6 +15,9 @@ prysm/propagation/wavefront.py:59-166): `from_amp_and_phase`, `phase_screen`, `t
 reference's own classes, so user code that imported `Wavefront` before the switch keeps working and never
 touches numpy `exp` or eager tensor arithmetic.
 
+The reference's `RichData` class gets `slices`, `exact_polar`, `exact_xy`, `exact_x` and `exact_y` that run on the
+device when its `data` is a CUDA tensor (what the re-bound `mtf_from_psf` returns) and call the originals otherwise.
+
 `set_backend_to_defaults()` restores every name it replaced.
 """
 import importlib
@@ -71,8 +74,9 @@ _TARGETS = {
     'prysm.otf': {n: getattr(_otf, n) for n in (
         'transform_psf', 'transform_psf_adjoint', 'mtf_from_psf', 'ptf_from_psf', 'otf_from_psf', 'mtf_ptf_otf_from_psf',
         'mtf_from_psf_adjoint', 'ptf_from_psf_adjoint', 'otf_from_psf_adjoint', 'encircled_energy',
-        'encircled_energy_adjoint')},
-    'prysm.psf': {'centroid': _psf.centroid},
+        'encircled_energy_adjoint', 'diffraction_limited_mtf', 'analytical_encircled_energy_circular_aperture')},
+    'prysm.psf': {n: getattr(_psf, n) for n in (
+        'centroid', 'estimate_size', 'fwhm', 'one_over_e', 'one_over_e_sq', 'airydisk', 'airydisk_efield', 'airydisk_ft')},
     'prysm.polynomials': {'sum_of_2d_modes': _poly.sum_of_2d_modes, 'sum_of_2d_modes_adjoint': _poly.sum_of_2d_modes_adjoint},
     'prysm.polynomials.fitting': {'sum_of_2d_modes': _poly.sum_of_2d_modes,
                                   'sum_of_2d_modes_adjoint': _poly.sum_of_2d_modes_adjoint},
@@ -198,6 +202,54 @@ def _patch_wavefront_class():
         setattr(cls, name, desc)
 
 
+def _richdata_patches():
+    """Methods that replace the sampling members of the reference's RichData class: with a CUDA tensor as `data` they
+    run the engine on the object's own x / y axes; otherwise (a host RichData, an Interferogram, ...) they call the
+    reference's original, so host objects behave exactly as before."""
+    import torch
+    from . import _richdata as ours
+    ref = importlib.import_module('prysm._richdata').RichData
+
+    def on_device(self):
+        return isinstance(self.data, torch.Tensor) and self.data.is_cuda
+
+    def make(name, engine):
+        orig = getattr(ref, name)
+
+        def f(self, *args, **kwargs):
+            if on_device(self):
+                return engine(self, *args, **kwargs)
+            return orig(self, *args, **kwargs)
+        f.__name__ = name
+        f.__doc__ = orig.__doc__
+        return f
+
+    def slices(self, twosided=None):
+        if twosided is None:
+            twosided = self._default_twosided
+        return ours.Slices(data=self.data, x=self.x[0], y=self.y[..., 0], twosided=twosided)
+
+    engines = {
+        'slices': slices,
+        'exact_polar': lambda self, rho, phi=None: ours.exact_polar(self.data, self.x, self.y, rho, phi),
+        'exact_xy': lambda self, x, y=None: ours.exact_xy(self.data, self.x, self.y, x, y),
+        'exact_x': lambda self, x: ours.exact_x(self.data, self.x, self.y, x),
+        'exact_y': lambda self, y: ours.exact_y(self.data, self.x, self.y, y),
+    }
+    return ref, {n: make(n, e) for n, e in engines.items()}
+
+
+def _patch_richdata_class():
+    try:
+        cls, patches = _richdata_patches()
+    except ImportError:
+        return
+    for name, fn in patches.items():
+        if (cls, name) not in _saved_cls:
+            _saved_cls[(cls, name)] = cls.__dict__.get(name, _MISSING)
+            setattr(cls, name, fn)
+
+
 def set_backend_to_b200(device=None):
     """Route prysm's propagation hot path through the H100 engine.  Call after `import prysm`
     (like the reference's own set_backend_to_* helpers).  Arrays handed to the re-bound functions may be
@@ -230,6 +282,7 @@ def set_backend_to_b200(device=None):
             if hasattr(mod, attr):
                 setattr(mod, attr, new)
     _patch_wavefront_class()
+    _patch_richdata_class()
     return sorted(_saved)
 
 

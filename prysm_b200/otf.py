@@ -125,3 +125,23 @@ def encircled_energy(psf, dx, radius, return_more=False):
     out = _ops.encircled_energy(mtf.data, mtf.dx, radii)
     out = float(out[0]) if scalar else out
     return (out, data) if return_more else out
+
+
+def analytical_encircled_energy_circular_aperture(fno, wavelength, points):
+    """1 - J0(p)^2 - J1(p)^2, p = points pi / fno / wavelength (prysm/otf.py:474-493), one kernel."""
+    from . import _capi
+    from .psf import analytic
+    return analytic(_capi.AR_EE_CIRCULAR, points, wavelength, fno)
+
+
+def diffraction_limited_mtf(fno, wavelength, frequencies=None, samples=128):
+    """The MTF of a circular pupil at frequencies [cy/mm], or (frequencies, mtf) at `samples` frequencies from 0 to
+    the extinction 1 / (wavelength / 1000 fno) when none are given (prysm/otf.py:496-543), one kernel."""
+    import numpy as np
+    from . import _capi
+    from .psf import analytic
+    if frequencies is None:
+        extinction = 1 / (wavelength / 1000 * fno)
+        nf = np.linspace(0, 1, samples)
+        return _ops.asdevice(nf * extinction), analytic(_capi.AR_DIFFLIM_NORMALIZED, nf, 0.0, 0.0)
+    return analytic(_capi.AR_DIFFLIM_MTF, frequencies, wavelength, fno)
