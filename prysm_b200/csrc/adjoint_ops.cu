@@ -69,27 +69,6 @@ __global__ void component_kernel(int which, const cplx<R>* __restrict__ in, long
     }
 }
 
-__device__ inline void block_sum2(double& re, double& im, double* dst) {
-    for (int o = 16; o; o >>= 1) {
-        re += __shfl_down_sync(0xffffffffu, re, o);
-        im += __shfl_down_sync(0xffffffffu, im, o);
-    }
-    __shared__ double sh[2][32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) { sh[0][wid] = re; sh[1][wid] = im; }
-    __syncthreads();
-    if (wid == 0) {
-        const int nw = blockDim.x >> 5;
-        re = lane < nw ? sh[0][lane] : 0.0;
-        im = lane < nw ? sh[1][lane] : 0.0;
-        for (int o = 16; o; o >>= 1) {
-            re += __shfl_down_sync(0xffffffffu, re, o);
-            im += __shfl_down_sync(0xffffffffu, im, o);
-        }
-        if (lane == 0) { atomicAdd(&dst[0], re); atomicAdd(&dst[1], im); }
-    }
-}
-
 // sums[0..1] += sum w * a * conj(b)
 template <typename R>
 __global__ void dot_kernel(const cplx<R>* __restrict__ a, const cplx<R>* __restrict__ b, const R* __restrict__ w, long long n,
@@ -101,7 +80,9 @@ __global__ void dot_kernel(const cplx<R>* __restrict__ a, const cplx<R>* __restr
         re += ww * ((double)x.x * y.x + (double)x.y * y.y);
         im += ww * ((double)x.y * y.x - (double)x.x * y.y);
     }
-    block_sum2(re, im, sums);
+    double v[2] = {re, im};
+    block_reduce<256>(v, OpAdd{});
+    if (threadIdx.x == 0) { atomicAdd(&sums[0], v[0]); atomicAdd(&sums[1], v[1]); }
 }
 
 // sums[2k..2k+1] += sum modes[k][i] * bar[i]      (bar real or complex)
@@ -119,7 +100,9 @@ __global__ void mode_projection_kernel(const R* __restrict__ modes, long long n,
             re += mv * reinterpret_cast<const R*>(bar)[i];
         }
     }
-    block_sum2(re, im, sums + 2 * blockIdx.y);
+    double v[2] = {re, im};
+    block_reduce<256>(v, OpAdd{});
+    if (threadIdx.x == 0) { atomicAdd(&sums[2 * blockIdx.y], v[0]); atomicAdd(&sums[2 * blockIdx.y + 1], v[1]); }
 }
 
 // which 1 (mtf): S = sum bar*|D|;  2 (ptf): S = sum bar;  4 (otf): S = sum conj(D)*bar
@@ -138,7 +121,9 @@ __global__ void otf_adjoint_reduce_kernel(int which, const void* __restrict__ ba
             else re += g;
         }
     }
-    block_sum2(re, im, sums);
+    double v[2] = {re, im};
+    block_reduce<256>(v, OpAdd{});
+    if (threadIdx.x == 0) { atomicAdd(&sums[0], v[0]); atomicAdd(&sums[1], v[1]); }
 }
 
 template <typename R>
@@ -222,9 +207,6 @@ __global__ void resample_bilinear_kernel(const cplx<R>* __restrict__ map, int ny
         out[i] = mk<R>((R)re, (R)im);
     }
 }
-
-__device__ inline float mul_add_rn(float a, float b, float c) { return __fadd_rn(__fmul_rn(a, b), c); }     // two roundings,
-__device__ inline double mul_add_rn(double a, double b, double c) { return __dadd_rn(__dmul_rn(a, b), c); }  // like numpy
 
 __device__ inline double smootherstep(double t) {
     t = fmin(fmax(t, 0.0), 1.0);

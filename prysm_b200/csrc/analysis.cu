@@ -111,31 +111,6 @@ __global__ void interp_polar_kernel(const T* __restrict__ d, Grid g, double rmax
     }
 }
 
-// ---- fixed-order block reductions (blockDim.x == AN_THREADS) --------------------------------------------------------
-template <typename Op>
-__device__ inline double block_reduce(double v, Op op, double* sh) {
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    for (int o = 16; o; o >>= 1) v = op(v, __shfl_down_sync(0xffffffffu, v, o));
-    __syncthreads();                 // sh may still be read by the previous reduction
-    if (lane == 0) sh[wid] = v;
-    __syncthreads();
-    if (wid == 0) {
-        v = sh[lane < AN_THREADS / 32 ? lane : 0];
-        for (int o = AN_THREADS / 64; o; o >>= 1) {
-            const double w = __shfl_down_sync(0xffffffffu, v, o);
-            if (lane < o) v = op(v, w);
-        }
-        if (lane == 0) sh[0] = v;
-    }
-    __syncthreads();
-    return sh[0];
-}
-struct OpAdd { __device__ double operator()(double a, double b) const { return a + b; } };
-struct OpMin { __device__ double operator()(double a, double b) const { return fmin(a, b); } };   // NaN ignored
-struct OpMax { __device__ double operator()(double a, double b) const { return fmax(a, b); } };
-// NaN propagates (ndarray.max)
-struct OpMaxNan { __device__ double operator()(double a, double b) const { return (isnan(a) || a > b) ? a : b; } };
-
 // order-preserving key of a double; NaN above everything
 __device__ inline unsigned long long order_key(double v) {
     if (isnan(v)) return ~0ull;
@@ -195,7 +170,6 @@ template <typename R>
 __global__ void __launch_bounds__(AN_THREADS) azimuthal_stats_kernel(const R* __restrict__ d, Grid g, double rmax,
                                                                      int stats, R* __restrict__ out) {
     extern __shared__ double s[];
-    __shared__ double red[AN_THREADS / 32];
     __shared__ unsigned hist[256];
     __shared__ unsigned long long shk;
     __shared__ int shr;
@@ -206,20 +180,20 @@ __global__ void __launch_bounds__(AN_THREADS) azimuthal_stats_kernel(const R* __
         s[i] = v;
         if (!isnan(v)) { cnt += 1; sum += v; mn = fmin(mn, v); mx = fmax(mx, v); }
     }
-    cnt = block_reduce(cnt, OpAdd{}, red);
-    sum = block_reduce(sum, OpAdd{}, red);
+    cnt = block_reduce<AN_THREADS>(cnt, OpAdd{});
+    sum = block_reduce<AN_THREADS>(sum, OpAdd{});
     const double mean = cnt > 0 ? sum / cnt : CUDART_NAN;
     const long long col = j;
     const long long nxo = g.nx;
-    if (stats & PB_AZ_MIN) { mn = block_reduce(mn, OpMin{}, red); if (threadIdx.x == 0) out[3 * nxo + col] = (R)(cnt > 0 ? mn : CUDART_NAN); }
-    if (stats & PB_AZ_MAX) { mx = block_reduce(mx, OpMax{}, red); if (threadIdx.x == 0) out[4 * nxo + col] = (R)(cnt > 0 ? mx : CUDART_NAN); }
+    if (stats & PB_AZ_MIN) { mn = block_reduce<AN_THREADS>(mn, OpMin{}); if (threadIdx.x == 0) out[3 * nxo + col] = (R)(cnt > 0 ? mn : CUDART_NAN); }
+    if (stats & PB_AZ_MAX) { mx = block_reduce<AN_THREADS>(mx, OpMax{}); if (threadIdx.x == 0) out[4 * nxo + col] = (R)(cnt > 0 ? mx : CUDART_NAN); }
     if (stats & PB_AZ_VAR) {
         double ss = 0;
         for (int i = threadIdx.x; i < n; i += AN_THREADS) {
             const double v = s[i];
             if (!isnan(v)) { const double e = v - mean; ss += e * e; }
         }
-        ss = block_reduce(ss, OpAdd{}, red);
+        ss = block_reduce<AN_THREADS>(ss, OpAdd{});
         if (threadIdx.x == 0) out[2 * nxo + col] = (R)(cnt > 0 ? ss / cnt : CUDART_NAN);
     }
     if (threadIdx.x == 0) {
@@ -242,21 +216,19 @@ __global__ void __launch_bounds__(AN_THREADS) azimuthal_stats_kernel(const R* __
 template <typename R>
 __global__ void __launch_bounds__(AN_THREADS) lattice_rowmax_kernel(const R* __restrict__ d, Grid g, double rmax,
                                                                     double* __restrict__ rowmax) {
-    __shared__ double red[AN_THREADS / 32];
     const int i = blockIdx.x;
     double m = -CUDART_INF;
     for (int j = threadIdx.x; j < g.nx; j += AN_THREADS) m = OpMaxNan{}(m, lattice_at(d, g, rmax, i, j));
-    m = block_reduce(m, OpMaxNan{}, red);
+    m = block_reduce<AN_THREADS>(m, OpMaxNan{});
     if (threadIdx.x == 0) rowmax[i] = m;
 }
 
 // t = metric (absolute) or metric * max(rowmax) (relative), into *t
 __global__ void __launch_bounds__(AN_THREADS) crossing_level_kernel(const double* __restrict__ rowmax, int n, double metric,
                                                                     int relative, double* __restrict__ t) {
-    __shared__ double red[AN_THREADS / 32];
     double m = -CUDART_INF;
     for (int i = threadIdx.x; i < n; i += AN_THREADS) m = OpMaxNan{}(m, rowmax[i]);
-    m = block_reduce(m, OpMaxNan{}, red);
+    m = block_reduce<AN_THREADS>(m, OpMaxNan{});
     if (threadIdx.x == 0) *t = relative ? __dmul_rn(metric, m) : metric;
 }
 
@@ -300,14 +272,13 @@ __global__ void __launch_bounds__(AN_THREADS) crossing_kernel(const R* __restric
 // res[0] = number of rows that cross, res[1] = the mean of their radii (fixed order)
 __global__ void __launch_bounds__(AN_THREADS) crossing_mean_kernel(const double* __restrict__ radius, int n,
                                                                    double* __restrict__ res) {
-    __shared__ double red[AN_THREADS / 32];
     double c = 0, s = 0;
     for (int i = threadIdx.x; i < n; i += AN_THREADS) {
         const double r = radius[i];
         if (!isnan(r)) { c += 1; s += r; }
     }
-    c = block_reduce(c, OpAdd{}, red);
-    s = block_reduce(s, OpAdd{}, red);
+    c = block_reduce<AN_THREADS>(c, OpAdd{});
+    s = block_reduce<AN_THREADS>(s, OpAdd{});
     if (threadIdx.x == 0) { res[0] = c; res[1] = c > 0 ? s / c : CUDART_NAN; }
 }
 

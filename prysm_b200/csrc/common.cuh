@@ -1,4 +1,4 @@
-// Shared declarations for libprysm_b200: handle, error plumbing, complex helpers.
+// Shared declarations for libprysm_b200: handle, error plumbing, complex helpers, fixed-order device reductions.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -33,6 +33,99 @@ template <typename C> __host__ __device__ inline C cmulc(C a, C b) {  // a * con
 template <typename C> __host__ __device__ inline C cadd(C a, C b) { C c; c.x = a.x + b.x; c.y = a.y + b.y; return c; }
 template <typename C> __host__ __device__ inline C csub(C a, C b) { C c; c.x = a.x - b.x; c.y = a.y - b.y; return c; }
 template <typename C> __host__ __device__ inline C cconj(C a) { a.y = -a.y; return a; }
+template <typename C> __host__ __device__ inline C cscale(C a, decltype(a.x) s) { a.x *= s; a.y *= s; return a; }
+
+// one rounding per operation and no contraction into an fma, like numpy
+__device__ inline float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ inline double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ inline float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ inline double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ inline float mul_add_rn(float a, float b, float c) { return __fadd_rn(__fmul_rn(a, b), c); }
+__device__ inline double mul_add_rn(double a, double b, double c) { return __dadd_rn(__dmul_rn(a, b), c); }
+
+// ---- fixed-order reductions: each combines the same values in the same order on every call ----------------------
+struct OpAdd { __device__ double operator()(double a, double b) const { return a + b; } };
+struct OpMin { __device__ double operator()(double a, double b) const { return fmin(a, b); } };   // NaN ignored
+struct OpMax { __device__ double operator()(double a, double b) const { return fmax(a, b); } };   // NaN ignored
+// NaN propagates (ndarray.max)
+struct OpMaxNan { __device__ double operator()(double a, double b) const { return (isnan(a) || a > b) ? a : b; } };
+
+// the fold of v over the warp, in lane 0
+template <typename Op>
+__device__ inline double warp_reduce(double v, Op op) {
+    for (int o = 16; o; o >>= 1) v = op(v, __shfl_down_sync(0xffffffffu, v, o));
+    return v;
+}
+template <int N, typename Op>
+__device__ inline void warp_reduce(double (&v)[N], Op op) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = warp_reduce(v[k], op);
+}
+
+// the shared memory of block_reduce: one array per (THREADS, N) in a kernel whatever the op, so that the reductions
+// of a kernel take no more shared memory than one of them
+template <int THREADS, int N>
+__device__ inline double (&block_reduce_smem())[N][THREADS / 32] {
+    __shared__ double sh[N][THREADS / 32];
+    return sh;
+}
+
+// the fold of each v[k] over the block (blockDim.x == THREADS), given to every thread: each warp folds, then warp 0
+// folds the THREADS / 32 warp results
+template <int THREADS, int N, typename Op>
+__device__ inline void block_reduce(double (&v)[N], Op op) {
+    double (&sh)[N][THREADS / 32] = block_reduce_smem<THREADS, N>();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    warp_reduce(v, op);
+    __syncthreads();                 // sh may still be read by the previous reduction
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) sh[k][wid] = v[k];
+    __syncthreads();
+    if (wid == 0) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+            double x = sh[k][lane < THREADS / 32 ? lane : 0];
+            for (int o = THREADS / 64; o; o >>= 1) {
+                const double w = __shfl_down_sync(0xffffffffu, x, o);
+                if (lane < o) x = op(x, w);
+            }
+            if (lane == 0) sh[k][0] = x;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = sh[k][0];
+}
+template <int THREADS, typename Op>
+__device__ inline double block_reduce(double v, Op op) {
+    double a[1] = {v};
+    block_reduce<THREADS>(a, op);
+    return a[0];
+}
+
+// sh[w][k] = the fold of v[k] over warp w (blockDim.x == THREADS), then a block barrier; the caller combines the
+// THREADS / 32 partials of each value in the order it needs
+template <int THREADS, int N, typename Op>
+__device__ inline void warp_partials(double (&v)[N], Op op, double (&sh)[THREADS / 32][N]) {
+    warp_reduce(v, op);
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) sh[threadIdx.x >> 5][k] = v[k];
+    __syncthreads();
+}
+
+// the sum of v over the block (blockDim.x == THREADS, a power of two) by a halving tree in sh, given to every thread
+template <int THREADS>
+__device__ inline double tree_sum(double v, double* sh) {
+    sh[threadIdx.x] = v;
+    __syncthreads();
+    for (int d = THREADS / 2; d > 0; d >>= 1) {
+        if ((int)threadIdx.x < d) sh[threadIdx.x] += sh[threadIdx.x + d];
+        __syncthreads();
+    }
+    return sh[0];
+}
 
 // exp(2*pi*i*turns) with the argument reduced in fp64 before the sincos.
 __device__ inline float2 expi_turns(double turns, float) {

@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(256) spline_interp_kernel(const double* __rest
                                                             const C* __restrict__ xc, const C* __restrict__ yc, Mat3 M,
                                                             int oy, int ox, double scale, R* __restrict__ out) {
     const long long total = (long long)oy * ox;
-    for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(q, total) {
         double cx, cy;
         if (xc) {
             cx = (double)xc[q];
@@ -135,7 +135,7 @@ template <typename R>
 __global__ void dm_scatter_kernel(const R* __restrict__ act, int nay, int nax, int ny, int nx, int y0, int sy, int x0,
                                   int sx, R* __restrict__ poke) {
     const long long total = (long long)ny * nx;
-    for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(q, total) {
         const int y = (int)(q / nx), x = (int)(q - (long long)y * nx);
         const int dy = y - y0, dx = x - x0;
         R v = R(0);
@@ -152,7 +152,7 @@ template <typename R>
 __global__ void dm_gather_kernel(const void* __restrict__ in, bool cplx_in, int nx, int nay, int nax, int y0, int sy,
                                  int x0, int sx, R* __restrict__ act) {
     const long long total = (long long)nay * nax;
-    for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(q, total) {
         const int ay = (int)(q / nax), ax = (int)(q - (long long)ay * nax);
         const long long idx = (long long)(y0 + ay * sy) * nx + (x0 + ax * sx);
         act[q] = (R)load_real<R>(in, cplx_in, idx);

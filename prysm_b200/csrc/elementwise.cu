@@ -11,7 +11,7 @@ namespace pb {
 template <typename R>
 __global__ void phase_screen_kernel(const void* amp, int amp_kind, const R* __restrict__ opd, double kturns,
                                     long long n, long long nx, long long ld, cplx<R>* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const long long s = ld == nx ? i : i / nx * ld + i % nx;
         R a = R(1);
         if (amp_kind == PB_AMP_REAL) a = reinterpret_cast<const R*>(amp)[s];
@@ -39,7 +39,7 @@ int launch_phase_screen(Handle* h, int dtype, const void* amp, int amp_kind, con
 template <typename R>
 __global__ void intensity_kernel(const cplx<R>* __restrict__ in, long long n, R weight, int accumulate,
                                  R* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         cplx<R> v = in[i];
         R I = v.x * v.x + v.y * v.y;
         if (accumulate) out[i] += weight * I; else out[i] = weight * I;
@@ -51,7 +51,7 @@ __global__ void mul_outer_kernel(const cplx<R>* __restrict__ in, long long in_ld
                                  const cplx<R>* __restrict__ vy, int conj_y, const cplx<R>* __restrict__ vx,
                                  int conj_x, R scale, cplx<R>* __restrict__ out, long long out_ld) {
     const long long n = (long long)ny * nx;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int y = (int)(i / nx), x = (int)(i - (long long)y * nx);
         cplx<R> v = in[y * in_ld + x];
         if (vy) { cplx<R> m = vy[y]; v = conj_y ? cmulc(v, m) : cmul(v, m); }
@@ -80,7 +80,7 @@ __device__ inline double2 cmul_fp64(cplx<R> x, double2 w) {
 template <typename R>
 __global__ void binary_kernel(int op, const cplx<R>* __restrict__ a, const cplx<R>* __restrict__ b, cplx<R> sc,
                               int reverse, long long n, cplx<R>* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         cplx<R> x = a[i], y = b ? b[i] : sc;
         if (reverse) { cplx<R> t = x; x = y; y = t; }
         cplx<R> r;
@@ -98,7 +98,7 @@ template <typename R> struct ModeWeights { R w[PB_MAX_MODES]; };
 template <typename R>
 __global__ void weighted_sum_kernel(const R* __restrict__ modes, int k, long long n, ModeWeights<R> w, int accumulate,
                                     R* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         R acc = accumulate ? out[i] : R(0);
         for (int m = 0; m < k; ++m) acc += w.w[m] * modes[(long long)m * n + i];
         out[i] = acc;
@@ -109,7 +109,7 @@ template <typename R>
 __global__ void otf_normalize_kernel(const cplx<R>* __restrict__ D, long long n, long long centre, int which,
                                      R* __restrict__ mtf, R* __restrict__ ptf, cplx<R>* __restrict__ otf) {
     const double2 w = crecip_fp64<R>(D[centre]);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const double2 qd = cmul_fp64<R>(D[i], w);
         const cplx<R> q = mk<R>((R)qd.x, (R)qd.y);      // the quotient, rounded once to R
         if (which & 1) mtf[i] = hypot(q.x, q.y);
@@ -120,32 +120,15 @@ __global__ void otf_normalize_kernel(const cplx<R>* __restrict__ D, long long n,
 
 template <typename R>
 __global__ void moments_kernel(const R* __restrict__ d, int ny, int nx, double* __restrict__ sums) {
-    double s0 = 0, sy = 0, sx = 0;
+    double s[3] = {0, 0, 0};     // sum v, sum v y, sum v x
     const long long n = (long long)ny * nx;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int y = (int)(i / nx), x = (int)(i - (long long)y * nx);
         const double v = (double)d[i];
-        s0 += v; sy += v * y; sx += v * x;
+        s[0] += v; s[1] += v * y; s[2] += v * x;
     }
-    for (int o = 16; o; o >>= 1) {
-        s0 += __shfl_down_sync(0xffffffffu, s0, o);
-        sy += __shfl_down_sync(0xffffffffu, sy, o);
-        sx += __shfl_down_sync(0xffffffffu, sx, o);
-    }
-    __shared__ double sh[3][32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) { sh[0][wid] = s0; sh[1][wid] = sy; sh[2][wid] = sx; }
-    __syncthreads();
-    if (wid == 0) {
-        const int nw = blockDim.x >> 5;
-        s0 = lane < nw ? sh[0][lane] : 0; sy = lane < nw ? sh[1][lane] : 0; sx = lane < nw ? sh[2][lane] : 0;
-        for (int o = 16; o; o >>= 1) {
-            s0 += __shfl_down_sync(0xffffffffu, s0, o);
-            sy += __shfl_down_sync(0xffffffffu, sy, o);
-            sx += __shfl_down_sync(0xffffffffu, sx, o);
-        }
-        if (lane == 0) { atomicAdd(&sums[0], s0); atomicAdd(&sums[1], sy); atomicAdd(&sums[2], sx); }
-    }
+    block_reduce<256>(s, OpAdd{});
+    if (threadIdx.x == 0) { atomicAdd(&sums[0], s[0]); atomicAdd(&sums[1], s[1]); atomicAdd(&sums[2], s[2]); }
 }
 
 // Baliga & Cohn encircled energy: r * sum( MTF * J1(2 pi r nu) / nu ) * dnu^2 on the fftrange*df grid, nu(0) -> 1e-16
@@ -156,23 +139,15 @@ __global__ void encircled_energy_kernel(const R* __restrict__ mtf, int ny, int n
     const double r = radii[blockIdx.y];
     const long long n = (long long)ny * nx;
     double acc = 0.0;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int y = (int)(i / nx), x = (int)(i - (long long)y * nx);
         const double fy = (double)(y - ny / 2) * df, fx = (double)(x - nx / 2) * df;
         double nu = hypot(fx, fy);
         if (nu == 0.0) nu = 1e-16;
         acc += (double)mtf[i] * j1(6.283185307179586476925 * r * nu) / nu;
     }
-    for (int o = 16; o; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
-    __shared__ double sh[32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) sh[wid] = acc;
-    __syncthreads();
-    if (wid == 0) {
-        acc = lane < (blockDim.x >> 5) ? sh[lane] : 0.0;
-        for (int o = 16; o; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
-        if (lane == 0) atomicAdd(&out[blockIdx.y], acc * r * df * df);
-    }
+    acc = block_reduce<256>(acc, OpAdd{});
+    if (threadIdx.x == 0) atomicAdd(&out[blockIdx.y], acc * r * df * df);
 }
 
 // Bluestein pieces of one CZT axis built on the device from scalars (prysm/fttools.py:372-389, 277-281):
@@ -230,7 +205,7 @@ template <typename R>
 __global__ void mdft_basis_kernel(const double* __restrict__ f, int m, const double* __restrict__ x, int n, int sign,
                                   cplx<R>* __restrict__ E) {
     const long long tot = (long long)m * n;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < tot; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, tot) {
         const int j = (int)(i / n), l = (int)(i - (long long)j * n);
         E[i] = expi_turns(sign * f[j] * x[l], R(0));
     }

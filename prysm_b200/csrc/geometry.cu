@@ -65,7 +65,7 @@ template <typename R>
 __global__ void __launch_bounds__(256) sdf_kernel(const R* __restrict__ x, const R* __restrict__ y, int separable, int ny,
                                                   int nx, const __grid_constant__ SdfShape s, int mask, void* __restrict__ out) {
     const long long n = (long long)ny * nx;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         double xv, yv;
         if (separable) {
             const int iy = (int)(i / nx);
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(256) sdf_kernel(const R* __restrict__ x, const
 // minimum / maximum do, whatever the argument order.
 template <typename R>
 __global__ void sdf_combine_kernel(int op, const R* __restrict__ a, const R* __restrict__ b, long long n, R* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const R u = a[i], v = op == PB_SDF_SUBTRACT ? -b[i] : b[i];
         R r;
         if (u != u) r = u;

@@ -14,29 +14,20 @@ template <typename R>
 __global__ void pack_complex_kernel(const R* __restrict__ re, const R* __restrict__ im, const double* __restrict__ im_scale,
                                     long long n, cplx<R>* __restrict__ out) {
     const R s = im_scale ? (R)*im_scale : R(1);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    PB_GRID_STRIDE(i, n)
         out[i] = mk<R>(re[i], im ? s * im[i] : R(0));
 }
 
 // sums[0] += sum a^2, sums[1] += sum b^2
 template <typename R>
 __global__ void norms2_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, double* __restrict__ sums) {
-    double sa = 0, sb = 0;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    double s[2] = {0, 0};
+    PB_GRID_STRIDE(i, n) {
         const double x = a[i], y = b[i];
-        sa += x * x; sb += y * y;
+        s[0] += x * x; s[1] += y * y;
     }
-    for (int o = 16; o; o >>= 1) { sa += __shfl_down_sync(0xffffffffu, sa, o); sb += __shfl_down_sync(0xffffffffu, sb, o); }
-    __shared__ double sh[2][32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) { sh[0][wid] = sa; sh[1][wid] = sb; }
-    __syncthreads();
-    if (wid == 0) {
-        const int nw = blockDim.x >> 5;
-        sa = lane < nw ? sh[0][lane] : 0.0; sb = lane < nw ? sh[1][lane] : 0.0;
-        for (int o = 16; o; o >>= 1) { sa += __shfl_down_sync(0xffffffffu, sa, o); sb += __shfl_down_sync(0xffffffffu, sb, o); }
-        if (lane == 0) { atomicAdd(&sums[0], sa); atomicAdd(&sums[1], sb); }
-    }
+    block_reduce<256>(s, OpAdd{});
+    if (threadIdx.x == 0) { atomicAdd(&sums[0], s[0]); atomicAdd(&sums[1], s[1]); }
 }
 
 __global__ void balance_finalize_kernel(const double* __restrict__ sums, double* __restrict__ s) {
@@ -49,7 +40,7 @@ __global__ void packed_spectrum_product_kernel(const cplx<R>* __restrict__ Z, in
                                                const double* __restrict__ im_scale, cplx<R>* __restrict__ out) {
     const long long n = (long long)ny * nx;
     if (im_scale) scale = (R)((double)scale / *im_scale);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int ky = (int)(i / nx), kx = (int)(i - (long long)ky * nx);
         const int my = ky ? ny - ky : 0, mx = kx ? nx - kx : 0;
         const cplx<R> a = Z[i], b = Z[(long long)my * nx + mx];
@@ -67,7 +58,7 @@ template <typename R>
 __global__ void bindown_kernel(const R* __restrict__ in, int oy, int ox, int fy, int fx, R scale, R* __restrict__ out) {
     const long long n = (long long)oy * ox;
     const long long in_ld = (long long)ox * fx;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int y = (int)(i / ox), x = (int)(i - (long long)y * ox);
         const R* p = in + (long long)y * fy * in_ld + (long long)x * fx;
         double acc = 0.0;
@@ -80,7 +71,7 @@ __global__ void bindown_kernel(const R* __restrict__ in, int oy, int ox, int fy,
 template <typename R>
 __global__ void tile_kernel(const R* __restrict__ in, int ny, int nx, int fy, int fx, R scale, R* __restrict__ out) {
     const long long ox = (long long)nx * fx, n = (long long)ny * fy * ox;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const long long y = i / ox, x = i - y * ox;
         out[i] = scale * in[(y / fy) * nx + x / fx];
     }
@@ -91,7 +82,7 @@ template <typename R>
 __global__ void separable_tf_kernel(int kind, const R* __restrict__ fxv, const R* __restrict__ fyv, int ny, int nx, double wx,
                                     double wy, R* __restrict__ out) {
     const long long n = (long long)ny * nx;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int y = (int)(i / nx), x = (int)(i - (long long)y * nx);
         const double ax = (double)fxv[x] * wx, ay = (double)fyv[y] * wy;
         double v;

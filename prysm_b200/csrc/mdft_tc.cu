@@ -341,7 +341,7 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // complex basis E (m,n) -> real expansion (2m, 2n), hi and lo
 __global__ void expand_basis_kernel(const float2* __restrict__ E, int m, int n, float* __restrict__ hi, float* __restrict__ lo) {
     const long long tot = (long long)m * n;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < tot; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, tot) {
         const int j = (int)(i / n), l = (int)(i - (long long)j * n);
         const float2 e = E[i];
         const long long r0 = (long long)(2 * j) * (2 * n) + 2 * l, r1 = r0 + 2 * n;
@@ -356,7 +356,7 @@ __global__ void expand_basis_kernel(const float2* __restrict__ E, int m, int n, 
 __global__ void reduce_splits_kernel(const float* __restrict__ ws, int splits, int my, int mx, float norm, float2* __restrict__ out) {
     const long long tot = (long long)my * mx;
     const long long plane = (long long)2 * my * mx;
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < tot; e += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(e, tot) {
         const int i = (int)(e / mx), j = (int)(e - (long long)i * mx);
         float re = 0.f, im = 0.f;
         for (int s = 0; s < splits; ++s) {

@@ -47,7 +47,7 @@ template <typename R, int KIND, int MODE>
 __global__ void qpoly_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, const __grid_constant__ QPlan pl,
                              R* __restrict__ out0, R* __restrict__ out1, R* __restrict__ out2) {
     constexpr bool DER = KIND != 0;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         double r = 0.0, x = 0.0, y = 0.0, u, tv = 0.0;
         if (KIND == 2) {
             x = a[i]; y = b[i];

@@ -138,7 +138,6 @@ __global__ void __launch_bounds__(kThreads) segment_adjoint_partial_kernel(int n
     const Win win = load_win(seg, s);
     const long long hw = (long long)win.h * win.w;
     const long long q0 = (long long)b * PB_SEGMENT_CHUNK, q1 = std::min(hw, q0 + PB_SEGMENT_CHUNK);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int k0 = 0; k0 < nmodes; k0 += kModeBlock) {
         double acc[kModeBlock];
 #pragma unroll
@@ -152,13 +151,7 @@ __global__ void __launch_bounds__(kThreads) segment_adjoint_partial_kernel(int n
             for (int kk = 0; kk < kModeBlock; ++kk)
                 if (k0 + kk < nmodes) acc[kk] += gm * (double)bp[(long long)(k0 + kk) * hw];
         }
-#pragma unroll
-        for (int kk = 0; kk < kModeBlock; ++kk) {
-            double v = acc[kk];
-            for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-            if (lane == 0) red[warp][kk] = v;
-        }
-        __syncthreads();
+        warp_partials<kThreads>(acc, OpAdd{}, red);
         if (threadIdx.x < kModeBlock && k0 + threadIdx.x < nmodes) {
             double v = 0.0;
             for (int w = 0; w < kThreads / 32; ++w) v += red[w][threadIdx.x];

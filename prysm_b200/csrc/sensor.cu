@@ -109,13 +109,6 @@ struct PoissonPlan {
     }
 };
 
-template <typename R> __device__ __forceinline__ R mul_rn(R a, R b);
-template <> __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-template <> __device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-template <typename R> __device__ __forceinline__ R add_rn(R a, R b);
-template <> __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-template <> __device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-
 struct ExposeParams {
     long long n, nx;                     // pixels; the image is viewed as (n / nx, nx)
     long long prnu_sr, prnu_sc, dcnu_sr, dcnu_sc;
@@ -134,7 +127,7 @@ __global__ void __launch_bounds__(kSensorThreads) expose_kernel(const R* __restr
                                                                 unsigned int* __restrict__ flags) {
     // np.iinfo('l').max - sqrt(np.iinfo('l').max) * 10, in fp64 as numpy forms it
     const double lam_max = 9223372036854775807.0 - sqrt(9223372036854775807.0) * 10.0;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < p.n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, p.n) {
         // electrons = aerial * t [* prnu] + dark [* dcnu], every step rounded in R as numpy does
         R e = mul_rn(aerial[i], (R)p.t);
         R d = (R)p.dark;
@@ -182,7 +175,7 @@ __global__ void __launch_bounds__(kSensorThreads) expose_kernel(const R* __restr
 template <typename Code, typename Out>
 __global__ void lut_kernel(const Code* __restrict__ codes, long long n, const Out* __restrict__ lut, long long lut_len,
                            int check, Out* __restrict__ out, unsigned int* __restrict__ flags) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         long long c = (long long)codes[i];
         if (check && c >= lut_len) {
             atomicOr(flags, 4u);
@@ -198,7 +191,7 @@ __global__ void lut_kernel(const Code* __restrict__ codes, long long n, const Ou
 template <typename R>
 __global__ void pixel_kernel(const R* __restrict__ x, long long xsr, long long xsc, const R* __restrict__ y, long long ysr,
                              long long ysc, long long n, long long nx, double wx, double wy, uint8_t* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const long long r = i / nx, c = i - r * nx;
         const double xv = (double)x[r * xsr + c * xsc], yv = (double)y[r * ysr + c * ysc];
         out[i] = (xv <= wx) & (xv >= -wx) & (yv <= wy) & (yv >= -wy);
@@ -216,7 +209,7 @@ struct Planes4 { const void* p[4]; long long ld[4]; };
 template <typename T>
 __global__ void interleave_kernel(Planes4 src, int half, long long M, long long N, T* __restrict__ out, long long out_ld) {
     const long long n = M * N;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const long long y = i / N, x = i - y * N;
         const int s = cfa_site(y, x);
         const long long sy = half ? y >> 1 : y, sx = half ? x >> 1 : x;
@@ -229,7 +222,7 @@ template <typename In, typename Out>
 __global__ void deinterlace_kernel(const In* __restrict__ img, long long m2, long long n2, long long ld, int r_site,
                                    int b_site, Out* __restrict__ out) {
     const long long n = m2 * n2;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const long long y = i / n2, x = i - y * n2;
         const In* c = img + 2 * y * ld + 2 * x;
         const In v[4] = {c[0], c[1], c[ld], c[ld + 1]};
@@ -254,7 +247,7 @@ template <typename T>
 __global__ void wb_plane_max_kernel(const T* __restrict__ a, long long n, long long nx, int kind,
                                     double* __restrict__ partial) {
     double mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         const int pl = wb_plane(kind, i, nx);
         mx[pl] = fmax(mx[pl], (double)a[i]);
     }
@@ -305,7 +298,7 @@ __global__ void wb_scale_kernel(T* __restrict__ a, long long n, long long nx, in
     const double r = ratio ? *ratio : 1.0;
 #pragma unroll
     for (int pl = 0; pl < 4; ++pl) gain[pl] = (T)(ratio ? g.g[pl] / r : g.g[pl]);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    PB_GRID_STRIDE(i, n)
         a[i] = a[i] * gain[wb_plane(kind, i, nx)];
 }
 
@@ -399,7 +392,7 @@ __global__ void __launch_bounds__(kMalvarTX * kMalvarRows) malvar_kernel(const I
 template <typename R>
 __global__ void assemble_kernel(const cplx<R>* __restrict__ rp, const cplx<R>* __restrict__ g2p, const cplx<R>* __restrict__ bp,
                                 const R* __restrict__ g1, long long n, R* __restrict__ out) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    PB_GRID_STRIDE(i, n) {
         out[3 * i + 0] = rp[i].x;
         out[3 * i + 1] = (g2p[i].x + g1[i]) / R(2);
         out[3 * i + 2] = bp[i].x;

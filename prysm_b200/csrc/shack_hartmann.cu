@@ -227,13 +227,8 @@ __global__ void __launch_bounds__(kThreads) reconstruct_kernel(
         if (ref) v -= ref[m];
         a += row[m] * v;
     }
-    part[tid] = a;
-    __syncthreads();
-    for (int w = kThreads / 2; w > 0; w >>= 1) {
-        if (tid < w) part[tid] += part[tid + w];
-        __syncthreads();
-    }
-    if (tid == 0) out[(long long)f * K + k] = (S)part[0];
+    a = tree_sum<kThreads>(a, part);
+    if (tid == 0) out[(long long)f * K + k] = (S)a;
 }
 
 }  // namespace

@@ -12,9 +12,6 @@
 
 namespace pb {
 
-__device__ inline float mul_rn(float a, float b) { return __fmul_rn(a, b); }       // one rounding per operation, like numpy
-__device__ inline double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-
 // x = (ix - nx/2)*dx, y = (iy - ny/2)*dx in working precision (prysm/coordinates.py:344-378); r, t from them
 template <typename R>
 __global__ void xy_grid_kernel(int ny, int nx, double dx, R* __restrict__ x, R* __restrict__ y, R* __restrict__ r, R* __restrict__ t) {

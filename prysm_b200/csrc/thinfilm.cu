@@ -45,8 +45,6 @@ __device__ inline double2 tf_sqrt(double2 z) {
     return make_double2(fabs(z.y) / (2.0 * t), copysign(t, z.y));
 }
 
-__device__ inline double2 tf_scale(double2 a, double s) { return make_double2(a.x * s, a.y * s); }
-
 // _cos_snell (thinfilm.py:75-80): sqrt(1 - sint^2) on the principal branch, negated for a real sint > 1
 __device__ inline double2 tf_cos_snell(double2 n0, double2 n, double sin0) {
     const double2 q = tf_div(n0, n);
@@ -111,7 +109,7 @@ __device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k) {
     L.n = ((const double2*)op.p[PB_TF_IN_N])[s.off_n + (long long)k * op.st[PB_TF_IN_N][PB_TF_DIMS]];
     L.d = ((const double*)op.p[PB_TF_IN_D])[s.off_d + (long long)k * op.st[PB_TF_IN_D][PB_TF_DIMS]];
     L.cost = tf_cos_snell(s.n0, L.n, s.sin0);
-    L.beta = tf_scale(cmul(tf_scale(L.n, 2.0 * M_PI * L.d), L.cost), 1.0 / s.wvl);
+    L.beta = cscale(cmul(cscale(L.n, 2.0 * M_PI * L.d), L.cost), 1.0 / s.wvl);
     L.eta = tf_admittance(L.n, L.cost, op.pol);
     return L;
 }
@@ -171,9 +169,9 @@ __global__ void stack_eval_kernel(const TfOps op, long long count, TfOut o, TfSt
         double2 r, t;
         if (MODE == PB_TF_THINFILM) {
             // multilayer_stack_rt (thinfilm.py:295-311): term1 = 1 / (2 n0 cos0)
-            const double2 term1 = tf_div(make_double2(1.0, 0.0), tf_scale(s.n0, 2.0 * s.cos0));
-            const double2 a = op.pol == PB_TF_POL_P ? s.n0 : tf_scale(s.n0, s.cos0);
-            const double2 q1 = op.pol == PB_TF_POL_P ? tf_scale(v1, s.cos0) : v1;
+            const double2 term1 = tf_div(make_double2(1.0, 0.0), cscale(s.n0, 2.0 * s.cos0));
+            const double2 a = op.pol == PB_TF_POL_P ? s.n0 : cscale(s.n0, s.cos0);
+            const double2 q1 = op.pol == PB_TF_POL_P ? cscale(v1, s.cos0) : v1;
             const double2 aq = cmul(a, v0);
             const double2 A00 = cmul(term1, cadd(aq, q1)), A10 = cmul(term1, csub(aq, q1));
             r = tf_div(A10, A00);
@@ -183,7 +181,7 @@ __global__ void stack_eval_kernel(const TfOps op, long long count, TfOut o, TfSt
             const double2 eb = cmul(eta0, v0);
             const double2 den = cadd(eb, v1);
             r = tf_div(csub(eb, v1), den);
-            t = tf_div(tf_scale(eta0, 2.0), den);
+            t = tf_div(cscale(eta0, 2.0), den);
             if (o.p[PB_TF_OUT_ETA0]) ((cplx<R>*)o.p[PB_TF_OUT_ETA0])[i] = mk<R>((R)eta0.x, (R)eta0.y);
             if (o.p[PB_TF_OUT_ETASUB]) ((cplx<R>*)o.p[PB_TF_OUT_ETASUB])[i] = mk<R>((R)eta_sub.x, (R)eta_sub.y);
             if (o.p[PB_TF_OUT_TRANS]) ((R*)o.p[PB_TF_OUT_TRANS])[i] = (R)(eta_sub.x / eta0.x * tf_abs2(t));
@@ -218,14 +216,9 @@ __device__ inline void tf_field_bar(const double* dA, const double* dEsq, int N,
         if (k > 0) fb -= dA[(long long)(k - 1) * count + i];
     }
     fb *= inv_re0;
-    Eb = tf_scale(H, fb);
-    Hb = tf_scale(E, fb);
-    if (dEsq) Eb = cadd(Eb, tf_scale(E, 2.0 * dEsq[(long long)k * count + i]));
-}
-
-__device__ inline double warp_sum(double v) {
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_down_sync(0xffffffffu, v, d);
-    return v;
+    Eb = cscale(H, fb);
+    Hb = cscale(E, fb);
+    if (dEsq) Eb = cadd(Eb, cscale(E, 2.0 * dEsq[(long long)k * count + i]));
 }
 
 // One warp-uniform pass per 32 samples.  Each layer's contribution is summed over the warp and added by lane 0 to the
@@ -257,8 +250,8 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
         const double2 r = tf_div(csub(eb, C), den);
         // amplitude cotangents (diff.py:191-201)
         double2 rb = make_double2(0.0, 0.0), tb = make_double2(0.0, 0.0);
-        if (dR) rb = tf_scale(r, 2.0 * dR[i]);
-        if (dT) tb = tf_scale(t, 2.0 * (eta_sub.x * inv_re0) * dT[i]);
+        if (dR) rb = cscale(r, 2.0 * dR[i]);
+        if (dT) tb = cscale(t, 2.0 * (eta_sub.x * inv_re0) * dT[i]);
         // f_k = t v_k: tbar += sum_k v_k^H fbar_k
         if (fseed) {
             for (int k = 0; k <= N; ++k) {
@@ -284,7 +277,7 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
             vb0 = cadd(vb0, cmul(ct, eb2));
             vb1 = cadd(vb1, cmul(ct, hb2));
         }
-        const double2 n0sq_sin2 = tf_scale(cmul(s.n0, s.n0), s.sin0 * s.sin0);
+        const double2 n0sq_sin2 = cscale(cmul(s.n0, s.n0), s.sin0 * s.sin0);
         for (int k = 0; k < N; ++k) {
             const TfLayer L = tf_layer(op, s, k);
             double2 sb, cb;
@@ -305,7 +298,7 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
             double gth = 0.0, gix = 0.0;
             if (kinds & PB_TF_GRAD_THICKNESS) {
                 // dbeta/dd = 2 pi n cos / wvl (diff.py:110, 307)
-                const double2 dbdd = tf_scale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
+                const double2 dbdd = cscale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
                 gth = cmulc(dbdd, cbeta).x;
             }
             if (kinds & PB_TF_GRAD_INDEX) {
@@ -313,7 +306,7 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
                 const double2 n2 = cmul(L.n, L.n);
                 const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
                 const double2 ndc = cmul(L.n, dcdn);
-                const double2 dbdn = tf_scale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
+                const double2 dbdn = cscale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
                 const double2 dedn = op.pol == PB_TF_POL_P
                     ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
                     : cadd(L.cost, ndc);
@@ -333,7 +326,7 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
             }
             for (int kind = 0; kind < 2; ++kind) {
                 if (!(kinds & (1 << kind))) continue;
-                const double v = warp_sum(act ? (kind == 0 ? gth : gix) : 0.0);
+                const double v = warp_reduce(act ? (kind == 0 ? gth : gix) : 0.0, OpAdd{});
                 if (lane == 0) {
                     double* p = partial + (long long)(2 * k + kind) * W + warp;
                     *p = first ? v : *p + v;
@@ -354,13 +347,8 @@ __global__ void __launch_bounds__(PB_TF_THREADS) stack_grad_reduce_kernel(const 
     const double* p = partial + (long long)(2 * k + kind) * W;
     double acc = 0.0;
     for (long long w = threadIdx.x; w < nw; w += blockDim.x) acc += p[w];
-    sh[threadIdx.x] = acc;
-    __syncthreads();
-    for (int d = blockDim.x / 2; d > 0; d >>= 1) {
-        if ((int)threadIdx.x < d) sh[threadIdx.x] += sh[threadIdx.x + d];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) grad[(long long)row * N + k] = (R)sh[0];
+    acc = tree_sum<PB_TF_THREADS>(acc, sh);
+    if (threadIdx.x == 0) grad[(long long)row * N + k] = (R)acc;
 }
 
 // stack.py:252-301: searchsorted(Z, z, 'right') - 1 clipped to [0, N - 1], then the partial layer below z applied to
@@ -385,7 +373,7 @@ __global__ void __launch_bounds__(PB_TF_THREADS) field_at_depth_kernel(const dou
         const double2 n = nl[li];
         const double2 cost = tf_cos_snell(n0, n, sin0);
         const double2 eta = tf_admittance(n, cost, pol);
-        const double2 beta = tf_scale(cmul(tf_scale(n, 2.0 * M_PI * (zb[li + 1] - zi)), cost), 1.0 / wvl);
+        const double2 beta = cscale(cmul(cscale(n, 2.0 * M_PI * (zb[li + 1] - zi)), cost), 1.0 / wvl);
         double2 sb, cb;
         tf_sincos(beta, &sb, &cb);
         double2 v0 = Eb[li + 1], v1 = Hb[li + 1];

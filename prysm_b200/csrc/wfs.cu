@@ -154,19 +154,6 @@ __global__ void __launch_bounds__(kThreads) lp_modes_kernel(const R* __restrict_
 // ---- pb_overlap ----------------------------------------------------------------------------------------------------
 struct ModeTable { const void* p[kOvMax]; };
 
-template <int N>
-__device__ __forceinline__ void block_sum(double (&v)[N], double (*sh)[N]) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
-    if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < N; ++k) sh[warp][k] = v[k];
-    __syncthreads();
-}
-
 // stage 1: block (chunk, group) sums sum conj(M_p) E, sum |M_p|^2 of its eight modes over PB_OVERLAP_CHUNK pixels;
 // the blocks of the first group of the first launch also sum |E|^2
 template <typename R, bool MC>
@@ -203,7 +190,7 @@ __global__ void __launch_bounds__(kThreads) overlap_partial_kernel(const cplx<R>
             }
         }
     }
-    block_sum<NV>(acc, sh);
+    warp_partials<kThreads>(acc, OpAdd{}, sh);
     const int v = threadIdx.x;
     if (v < NV) {
         double s = 0.0;
@@ -233,7 +220,7 @@ __global__ void __launch_bounds__(kThreads) overlap_finish_kernel(const double* 
         if (!ip_in) s[2] += q[2];
         if (!ie_in) s[3] += part_e[k];
     }
-    block_sum<4>(s, sh);
+    warp_partials<kThreads>(s, OpAdd{}, sh);
     if (threadIdx.x == 0) {
         double t[4] = {0.0, 0.0, 0.0, 0.0};
         for (int w = 0; w < kThreads / 32; ++w)
