@@ -765,7 +765,8 @@ int pb_field_at_depth(pb_handle_t h, int dtype, int pol, int nlayers, const void
  *   (relative != 0; NaN if any lattice sample is NaN).  Along each phi row, the first (last = 0) or last i with
  *   (v[i] > level) != (v[i + 1] > level) gives the radius rho_i + frac (rho_{i+1} - rho_i), frac = (level - v[i]) /
  *   (v[i + 1] - v[i]), 0 where v[i + 1] == v[i].  result (HOST, 2): the number of rows that cross, and the fixed-order
- *   fp64 mean of their radii.  Up to four launches in the handle's scratch; the call waits for them.
+ *   fp64 mean of their radii.  A crossing next to a NaN sample counts and has a NaN radius, so the mean is NaN; only
+ *   rows without a transition stay out.  Up to four launches in the handle's scratch; the call waits for them.
  * pb_analytic_radial: out[k] = f(x[k]) in fp64, rounded once to out_type (in_type, out_type PB_ELEM_F32 / F64);
  *   a = wavelength, b = F/#.  jinc(u) = j1(u) / u, 0.5 for |u| < 1e-8; core(s) = (2 / pi)(acos s - s sqrt(1 - s^2)).
  *   PB_AR_AIRYDISK (2 jinc(u))^2 and PB_AR_AIRYDISK_EFIELD 2 jinc(u), u = x pi / a / b;  PB_AR_AIRYDISK_FT core(min(|x| /

@@ -232,7 +232,8 @@ __global__ void __launch_bounds__(AN_THREADS) crossing_level_kernel(const double
     if (threadIdx.x == 0) *t = relative ? __dmul_rn(metric, m) : metric;
 }
 
-// one block per phi row: the first (last = 0) or last crossing of the level along rho, as a radius; NaN if none.
+// one block per phi row: the first (last = 0) or last crossing of the level along rho, as a radius; +inf if the row
+// never crosses.  A crossing next to a NaN sample is a crossing with a NaN radius, as in the reference's loop.
 // Thread k scans the contiguous samples [k L, (k + 1) L] (the shared end sample is interpolated twice).
 template <typename R>
 __global__ void __launch_bounds__(AN_THREADS) crossing_kernel(const R* __restrict__ d, Grid g, double rmax,
@@ -261,7 +262,7 @@ __global__ void __launch_bounds__(AN_THREADS) crossing_kernel(const R* __restric
     if (found >= 0) { if (last) atomicMax(&shj, found); else atomicMin(&shj, found); }   // integer: order-free
     __syncthreads();
     const int jj = shj;
-    if (threadIdx.x == 0 && (jj < 0 || jj == INT_MAX)) radius[i] = CUDART_NAN;
+    if (threadIdx.x == 0 && (jj < 0 || jj == INT_MAX)) radius[i] = CUDART_INF;
     if (found >= 0 && found == jj) {
         const double frac = y1 == y0 ? 0.0 : __ddiv_rn(__dsub_rn(t, y0), __dsub_rn(y1, y0));
         const double r0 = linspace0(rmax, n, jj), r1 = linspace0(rmax, n, jj + 1);
@@ -269,13 +270,14 @@ __global__ void __launch_bounds__(AN_THREADS) crossing_kernel(const R* __restric
     }
 }
 
-// res[0] = number of rows that cross, res[1] = the mean of their radii (fixed order)
+// res[0] = number of rows that cross, res[1] = the mean of their radii (fixed order); a NaN radius makes it NaN, as
+// np.mean does
 __global__ void __launch_bounds__(AN_THREADS) crossing_mean_kernel(const double* __restrict__ radius, int n,
                                                                    double* __restrict__ res) {
     double c = 0, s = 0;
     for (int i = threadIdx.x; i < n; i += AN_THREADS) {
         const double r = radius[i];
-        if (!isnan(r)) { c += 1; s += r; }
+        if (r != CUDART_INF) { c += 1; s += r; }
     }
     c = block_reduce<AN_THREADS>(c, OpAdd{});
     s = block_reduce<AN_THREADS>(s, OpAdd{});
