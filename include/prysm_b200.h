@@ -217,9 +217,10 @@ int pb_angular_spectrum_vectors(pb_handle_t h, int dtype, int ky, int kx, double
 int pb_mdft_basis(pb_handle_t h, int dtype, const double* f_host, int m, const double* x_host,
                   int n, int sign, void* E, void* stream);
 
-/* C(m,n) = alpha * opA(A) * opB(B); op: 0 = as is, 1 = transpose, 2 = conjugate transpose,
- * 3 = conjugate.  A is (m,k) after op, B is (k,n) after op.  Complex, row-major.
+/* C(m,n) = alpha * opA(A) * opB(B); op (pb_op): PB_OP_N as is, PB_OP_T transpose, PB_OP_H conjugate transpose,
+ * PB_OP_C conjugate.  A is (m,k) after op, B is (k,n) after op.  Complex, row-major.
  * Replaces the `@` chains of MDFT.__call__ / adjoint (prysm/fttools.py:201-228). */
+typedef enum { PB_OP_N = 0, PB_OP_T = 1, PB_OP_H = 2, PB_OP_C = 3 } pb_op;
 int pb_cgemm(pb_handle_t h, int dtype, int opA, int opB, int m, int n, int k, double alpha,
              const void* A, long long lda, const void* B, long long ldb, void* C, long long ldc,
              void* stream);
@@ -357,7 +358,7 @@ int pb_circle(pb_handle_t h, int dtype, const void* r, long long count, double r
               void* out, void* stream);
 /* Jacobi polynomials P_j^(alpha,beta)(x), j = 0..nmax, by the three-term recurrence of
  * prysm/polynomials/jacobi.py:13-39, 147-175; order j is written to out[slots_host[j]] (a (n_out, count) real
- * array) when slots_host[j] >= 0.  nmax <= 120. */
+ * array) when slots_host[j] >= 0.  nmax <= PB_POLY_NMAX (120). */
 int pb_jacobi_seq(pb_handle_t h, int dtype, const void* x, long long count, int nmax, double alpha,
                   double beta, const int* slots_host, void* out, void* stream);
 /* Zernike polynomials Z_n^m = norm * P_{(n-|m|)/2}^{(0,|m|)}(2r^2-1) * r^|m| * {cos(m t), sin(|m| t)} for k HOST
@@ -434,7 +435,7 @@ int pb_dm_gather(pb_handle_t h, int dtype, const void* in, int in_complex, int n
  *                             (geometry.py:656-696)
  *     PB_SDF_ANNULUS          x = r (y unused); params = inner radius, outer radius        (geometry.py:375-395)
  *     PB_SDF_OFFSET_CIRCLE    params = radius, cx, cy                                       (geometry.py:627-653)
- *   At most 8 params and 128 vertices / vanes.
+ *   At most 8 params and PB_SDF_MAX_VERTICES (128) vertices / vanes: the shape travels in kernel-parameter space.
  * pb_sdf_combine: out = min(a, b) (PB_SDF_UNION), max(a, b) (PB_SDF_INTERSECT) or max(a, -b) (PB_SDF_SUBTRACT)
  *   (geometry.py:37-93).
  * Segments: the DEVICE table `seg` has PB_SEGMENT_FIELDS int64 per segment: window row y0, column x0, height, width, the
@@ -455,6 +456,7 @@ typedef enum {
     PB_SDF_OFFSET_CIRCLE = 5
 } pb_sdf_kind;
 typedef enum { PB_SDF_UNION = 0, PB_SDF_INTERSECT = 1, PB_SDF_SUBTRACT = 2 } pb_sdf_op;
+enum { PB_SDF_MAX_VERTICES = 128 };
 typedef enum {
     PB_SEGMENT_FIELDS = 6, PB_SEGMENT_TILE_Y = 32, PB_SEGMENT_TILE_X = 64, PB_SEGMENT_CHUNK = 2048
 } pb_segment_layout;
@@ -625,7 +627,7 @@ int pb_sh_reconstruct(pb_handle_t h, int dtype, const void* slopes, int nframes,
 
 /* ---- Forbes polynomials (prysm/polynomials/qpoly.py) ------------------------------------------------------------
  * family: PB_QPOLY_BFS (Q-bfs, oe-18-19-19700), PB_QPOLY_CON (Q-con, oe-18-13-13851), PB_QPOLY_2D (2D-Q, oe-20-3-2483;
- * m = 0 is Q-bfs, m < 0 a sine term).  Orders are limited to n <= 64 and |m| <= 64, a call to 256 recurrence steps
+ * m = 0 is Q-bfs, m < 0 a sine term).  Orders are limited to n and |m| <= PB_QPOLY_NMAX (64), a call to 256 recurrence steps
  * (the sum over its recurrences -- one for Q-bfs / Q-con, one per |m| for 2D-Q -- of the highest n + 1) and a basis
  * call to 1024 modes; outside these PB_ERR_UNSUPPORTED, n < 0 PB_ERR_INVALID, both before any launch.  Each call is
  * one kernel, one thread per sample, every recurrence run once in fp64 registers.
@@ -644,6 +646,7 @@ int pb_sh_reconstruct(pb_handle_t h, int dtype, const void* slopes, int nframes,
  *   PB_QPOLY_2D (m >= 1): A, B, C (abc_q2d, NaN where its denominator is 0), G, F, g, f (G_q2d, F_q2d, g_q2d, f_q2d). */
 typedef enum { PB_QPOLY_BFS = 0, PB_QPOLY_CON = 1, PB_QPOLY_2D = 2 } pb_qpoly_family;
 typedef enum { PB_QPOLY_VALUE = 0, PB_QPOLY_DER = 1, PB_QPOLY_DER_XY = 2 } pb_qpoly_kind;
+enum { PB_QPOLY_NMAX = 64 };
 int pb_qpoly_seq(pb_handle_t h, int dtype, int family, int kind, const void* a, const void* b, long long count, int k,
                  const int* n_host, const int* m_host, void* out0, void* out1, void* stream);
 int pb_qpoly_sum(pb_handle_t h, int dtype, int family, const void* u, const void* t, long long count, int k,
@@ -653,8 +656,8 @@ int pb_qpoly_tables(int family, int m, int nmax, double* out);
 
 /* ---- Orthogonal polynomials, Zernike derivatives and polynomial sums (prysm/polynomials) ---------------------------
  * The 1-D families are one three-term recurrence P_k = (A_k x + B_k) P_{k-1} - C_k P_{k-2}, run once per sample in
- * fp64 registers by one kernel; outputs are rounded once to dtype.  Orders are limited to 0 <= n <= 120: n < 0 is
- * PB_ERR_INVALID, n > 120 PB_ERR_UNSUPPORTED, both before any launch.  Each call is one launch.
+ * fp64 registers by one kernel; outputs are rounded once to dtype.  Orders are limited to 0 <= n <= PB_POLY_NMAX (120):
+ * n < 0 is PB_ERR_INVALID, n > PB_POLY_NMAX PB_ERR_UNSUPPORTED, both before any launch.  Each call is one launch.
  * pb_jacobi_seq (above) is served by the same kernel.
  * pb_poly_seq: k HOST orders n_host in any order, repeats allowed; alpha is Jacobi's and Laguerre's alpha and Dickson's
  *   alpha, beta Jacobi's beta (ignored otherwise).
@@ -666,8 +669,8 @@ int pb_qpoly_tables(int family, int m, int nmax, double* out);
  * pb_jacobi_radial_sum: z = sum_q coefs[q] P_{n_q}^(alpha,beta)(u), u = 2 (x^2 + y^2) / radius^2 - 1, zero coefficients
  *   skipped; with dzdx and dzdy (both or neither) also dz/du 4x / radius^2 and dz/du 4y / radius^2, dz/du by the
  *   differentiated recurrence in the same pass.  (jacobi_radial_sum, jacobi_radial_sum_der_xy.)
- * pb_jacobi_clenshaw: Clenshaw's backward recurrence over the len (<= 121) HOST coefficients s_host for the sum and its
- *   first j (<= 8) derivatives, N = max(len, 2); table != 0: every alpha plane (jj, n) into out (j + 1, N, count), rows
+ * pb_jacobi_clenshaw: Clenshaw's backward recurrence over the len (<= PB_POLY_NMAX + 1) HOST coefficients s_host for the
+ *   sum and its first j (<= PB_CLENSHAW_JMAX, 8) derivatives, N = max(len, 2); table != 0: every alpha plane (jj, n) into out (j + 1, N, count), rows
  *   jj > len - 1 zero; table = 0: the sum alone into out (count).  (jacobi_sum_clenshaw, jacobi_sum_clenshaw_der.)
  * pb_zernike_der: the (n, m) pairs' derivatives into out (k, 2, count): cartesian = 0, (a, b) = (r, t): dZ/dr, dZ/dt;
  *   cartesian = 1, (a, b) = (x, y): dZ/dx, dZ/dy through Re / Im (x + iy)^|m|, finite at the origin.  norm as
@@ -685,6 +688,7 @@ typedef enum {
 } pb_poly_family;
 typedef enum { PB_POLY_VALUE = 0, PB_POLY_DER = 1, PB_POLY_VALUE_DER = 2 } pb_poly_kind;
 typedef enum { PB_TSUM_MONOMIAL = 0, PB_TSUM_CHEBY1 = 1 } pb_tsum_basis;
+enum { PB_POLY_NMAX = 120, PB_CLENSHAW_JMAX = 8 };
 int pb_poly_seq(pb_handle_t h, int dtype, int family, int kind, double alpha, double beta, const void* x, long long count,
                 int k, const int* n_host, void* out, void* stream);
 int pb_jacobi_radial_sum(pb_handle_t h, int dtype, double alpha, double beta, const void* x, const void* y, long long count,
@@ -707,8 +711,9 @@ int pb_tensor_sum(pb_handle_t h, int dtype, int basis, const void* x, const void
  * once to dtype (PB_C64: complex64 / float32, PB_C128: complex128 / float64).  Layers are ambient side first.
  * Operands (HOST array in[PB_TF_NOPS] of device pointers, all fp64): wavelength and angle of incidence (radians) real,
  *   ambient index, substrate index and the per-layer index complex128, the per-layer thickness real.  Each is indexed
- *   over a collapsed calculation shape of ndim <= 4 dims (HOST shape[ndim], outermost first; count = its product):
- *   operand q reads element  sum_j idx_j strides[5 q + j]  (+ layer * strides[5 q + 4] for the per-layer operands),
+ *   over a collapsed calculation shape of ndim <= PB_TF_DIMS (4) dims (HOST shape[ndim], outermost first; count = its
+ *   product): operand q reads element  sum_j idx_j strides[5 q + j]  (+ layer * strides[5 q + 4] for the per-layer
+ *   operands),
  *   strides in elements, 0 where it broadcasts, slots j >= ndim ignored.
  * pb_stack_eval: the angle is theta_scale times the angle operand (pi / 180 for degrees).  Mode PB_TF_THINFILM
  *   assembles r, t as multilayer_stack_rt (nlayers >= 1; only the r and t outputs); PB_TF_COATINGS uses the
@@ -737,6 +742,7 @@ typedef enum {
     PB_TF_OUT_ABS = 6, PB_TF_OUT_ESQ = 7, PB_TF_OUT_ETA0 = 8, PB_TF_OUT_ETASUB = 9, PB_TF_NOUT = 10
 } pb_tf_output;
 typedef enum { PB_TF_GRAD_THICKNESS = 1, PB_TF_GRAD_INDEX = 2 } pb_tf_grad_kind;
+enum { PB_TF_DIMS = 4 };
 int pb_stack_eval(pb_handle_t h, int dtype, int mode, int pol, int flags, int nlayers, int ndim, const long long* shape,
                   const long long* strides, const void* const* in, double theta_scale, void* const* out, void* stream);
 int pb_stack_grad(pb_handle_t h, int dtype, int pol, int kinds, int nlayers, int ndim, const long long* shape,

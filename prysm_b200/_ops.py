@@ -840,9 +840,6 @@ def _real_pair(x, y):
     return x.to(rd).contiguous(), (None if y is None else y.to(rd).contiguous())
 
 
-SDF_MAX_VERTICES = 128      # the shape travels in kernel-parameter space (csrc/geometry.cu)
-
-
 def sdf(kind, x, y, params=(), verts=None, mask=False):
     """One signed-distance shape (pb_sdf) on a pair of (ny, nx) grids, or on the separable row (nx values) and
     column (ny values) that optimize_xy_separable reduces them to; y is None for the annulus (x is then r, any
@@ -860,8 +857,9 @@ def sdf(kind, x, y, params=(), verts=None, mask=False):
     out = torch.empty(oshape, dtype=torch.bool if mask else x.dtype, device=x.device)
     p, pp = _darr(np.asarray(params, dtype=np.float64).reshape(-1))
     v = np.zeros(0) if verts is None else np.asarray(verts, dtype=np.float64).reshape(-1)
-    if len(v) // 2 > SDF_MAX_VERTICES:
-        raise ValueError(f'{len(v) // 2} polygon vertices or spider vanes: at most {SDF_MAX_VERTICES} are supported')
+    if len(v) // 2 > capi.SDF_MAX_VERTICES:
+        raise ValueError(f'{len(v) // 2} polygon vertices or spider vanes: at most {capi.SDF_MAX_VERTICES} are '
+                         'supported')
     v, vp = _darr(v)
     _call(lib.pb_sdf, x, _CODE[x.dtype], int(kind), _p(x), _p(y), separable, int(ny), int(nx), pp, len(p), vp,
           len(v) // 2, int(bool(mask)), _p(out))

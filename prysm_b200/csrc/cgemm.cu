@@ -8,14 +8,14 @@ namespace pb {
 
 template <typename R, int OP>
 __device__ __forceinline__ cplx<R> ld_a(const cplx<R>* __restrict__ A, long long lda, int i, int kk) {
-    cplx<R> v = (OP == 0 || OP == 3) ? A[(long long)i * lda + kk] : A[(long long)kk * lda + i];
-    if (OP >= 2) v.y = -v.y;
+    cplx<R> v = (OP == PB_OP_N || OP == PB_OP_C) ? A[(long long)i * lda + kk] : A[(long long)kk * lda + i];
+    if (OP == PB_OP_H || OP == PB_OP_C) v.y = -v.y;
     return v;
 }
 template <typename R, int OP>
 __device__ __forceinline__ cplx<R> ld_b(const cplx<R>* __restrict__ B, long long ldb, int kk, int j) {
-    cplx<R> v = (OP == 0 || OP == 3) ? B[(long long)kk * ldb + j] : B[(long long)j * ldb + kk];
-    if (OP >= 2) v.y = -v.y;
+    cplx<R> v = (OP == PB_OP_N || OP == PB_OP_C) ? B[(long long)kk * ldb + j] : B[(long long)j * ldb + kk];
+    if (OP == PB_OP_H || OP == PB_OP_C) v.y = -v.y;
     return v;
 }
 
@@ -36,14 +36,14 @@ __global__ void __launch_bounds__(256) cgemm_kernel(int M, int N, int K, R alpha
     for (int k0 = 0; k0 < K; k0 += BK) {
         for (int e = tid; e < BM * BK; e += 256) {
             int ii, kk;
-            if (OPA == 0 || OPA == 3) { kk = e % BK; ii = e / BK; } else { ii = e % BM; kk = e / BM; }
+            if (OPA == PB_OP_N || OPA == PB_OP_C) { kk = e % BK; ii = e / BK; } else { ii = e % BM; kk = e / BM; }
             cplx<R> v = mk<R>(R(0), R(0));
             if (i0 + ii < M && k0 + kk < K) v = ld_a<R, OPA>(A, lda, i0 + ii, k0 + kk);
             Ar[kk][ii] = v.x; Ai[kk][ii] = v.y;
         }
         for (int e = tid; e < BN * BK; e += 256) {
             int jj, kk;
-            if (OPB == 0 || OPB == 3) { jj = e % BN; kk = e / BN; } else { kk = e % BK; jj = e / BK; }
+            if (OPB == PB_OP_N || OPB == PB_OP_C) { jj = e % BN; kk = e / BN; } else { kk = e % BK; jj = e / BK; }
             cplx<R> v = mk<R>(R(0), R(0));
             if (j0 + jj < N && k0 + kk < K) v = ld_b<R, OPB>(B, ldb, k0 + kk, j0 + jj);
             Br[kk][jj] = v.x; Bi[kk][jj] = v.y;
@@ -91,10 +91,10 @@ template <typename R, int OPA>
 static void launch_b(int opB, dim3 g, cudaStream_t st, int M, int N, int K, R alpha, const cplx<R>* A, long long lda,
                      const cplx<R>* B, long long ldb, cplx<R>* C, long long ldc) {
     switch (opB) {
-        case 0: cgemm_kernel<R, OPA, 0><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        case 1: cgemm_kernel<R, OPA, 1><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        case 2: cgemm_kernel<R, OPA, 2><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        default: cgemm_kernel<R, OPA, 3><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_N: cgemm_kernel<R, OPA, PB_OP_N><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_T: cgemm_kernel<R, OPA, PB_OP_T><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_H: cgemm_kernel<R, OPA, PB_OP_H><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        default: cgemm_kernel<R, OPA, PB_OP_C><<<g, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
     }
 }
 
@@ -102,10 +102,10 @@ template <typename R>
 static void launch_ab(int opA, int opB, dim3 g, cudaStream_t st, int M, int N, int K, R alpha, const cplx<R>* A,
                       long long lda, const cplx<R>* B, long long ldb, cplx<R>* C, long long ldc) {
     switch (opA) {
-        case 0: launch_b<R, 0>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        case 1: launch_b<R, 1>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        case 2: launch_b<R, 2>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
-        default: launch_b<R, 3>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_N: launch_b<R, PB_OP_N>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_T: launch_b<R, PB_OP_T>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        case PB_OP_H: launch_b<R, PB_OP_H>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
+        default: launch_b<R, PB_OP_C>(opB, g, st, M, N, K, alpha, A, lda, B, ldb, C, ldc); break;
     }
 }
 
@@ -128,7 +128,8 @@ using namespace pb;
 extern "C" int pb_cgemm(pb_handle_t hh, int dtype, int opA, int opB, int m, int n, int k, double alpha, const void* A,
                         long long lda, const void* B, long long ldb, void* C, long long ldc, void* stream) {
     PB_ENTER_REAL(hh);
-    if (m < 1 || n < 1 || k < 1 || opA < 0 || opA > 3 || opB < 0 || opB > 3) return fail(h, PB_ERR_INVALID, "bad gemm arguments");
+    if (m < 1 || n < 1 || k < 1 || opA < PB_OP_N || opA > PB_OP_C || opB < PB_OP_N || opB > PB_OP_C)
+        return fail(h, PB_ERR_INVALID, "bad gemm arguments");
     return cgemm_simt(h, dtype, opA, opB, m, n, k, alpha, A, lda, B, ldb, C, ldc, st);
 }
 
@@ -144,16 +145,16 @@ extern "C" int pb_mdft_apply(pb_handle_t hh, int dtype, const void* Ey, const vo
     if (my < 1 || ny < 1 || mx < 1 || nx < 1 || !Ey || !Ex || !a || !out || !work) return fail(h, PB_ERR_INVALID, "bad mdft arguments");
     if (!adjoint) {
         if (left_first) {  // (Ey @ a) @ Ex^T
-            PB_TRY(cgemm_simt(h, dtype, 0, 0, my, nx, ny, 1.0, Ey, ny, a, nx, work, nx, st));
-            return cgemm_simt(h, dtype, 0, 1, my, mx, nx, norm, work, nx, Ex, nx, out, mx, st);
+            PB_TRY(cgemm_simt(h, dtype, PB_OP_N, PB_OP_N, my, nx, ny, 1.0, Ey, ny, a, nx, work, nx, st));
+            return cgemm_simt(h, dtype, PB_OP_N, PB_OP_T, my, mx, nx, norm, work, nx, Ex, nx, out, mx, st);
         }
-        PB_TRY(cgemm_simt(h, dtype, 0, 1, ny, mx, nx, 1.0, a, nx, Ex, nx, work, mx, st));
-        return cgemm_simt(h, dtype, 0, 0, my, mx, ny, norm, Ey, ny, work, mx, out, mx, st);
+        PB_TRY(cgemm_simt(h, dtype, PB_OP_N, PB_OP_T, ny, mx, nx, 1.0, a, nx, Ex, nx, work, mx, st));
+        return cgemm_simt(h, dtype, PB_OP_N, PB_OP_N, my, mx, ny, norm, Ey, ny, work, mx, out, mx, st);
     }
     if (left_first) {  // (Ey^H @ g) @ conj(Ex)
-        PB_TRY(cgemm_simt(h, dtype, 2, 0, ny, mx, my, 1.0, Ey, ny, a, mx, work, mx, st));
-        return cgemm_simt(h, dtype, 0, 3, ny, nx, mx, norm, work, mx, Ex, nx, out, nx, st);
+        PB_TRY(cgemm_simt(h, dtype, PB_OP_H, PB_OP_N, ny, mx, my, 1.0, Ey, ny, a, mx, work, mx, st));
+        return cgemm_simt(h, dtype, PB_OP_N, PB_OP_C, ny, nx, mx, norm, work, mx, Ex, nx, out, nx, st);
     }
-    PB_TRY(cgemm_simt(h, dtype, 0, 3, my, nx, mx, 1.0, a, mx, Ex, nx, work, nx, st));
-    return cgemm_simt(h, dtype, 2, 0, ny, nx, my, norm, Ey, ny, work, nx, out, nx, st);
+    PB_TRY(cgemm_simt(h, dtype, PB_OP_N, PB_OP_C, my, nx, mx, 1.0, a, mx, Ex, nx, work, nx, st));
+    return cgemm_simt(h, dtype, PB_OP_H, PB_OP_N, ny, nx, my, norm, Ey, ny, work, nx, out, nx, st);
 }

@@ -13,12 +13,10 @@ namespace pb {
 
 namespace {
 
-constexpr int kMaxVerts = 128;     // polygon vertices / spider vanes per launch (kernel-parameter space)
-
 struct SdfShape {
     int kind, nv;
     double p[8];
-    double v[2 * kMaxVerts];       // polygon: (x, y) per vertex; spider: (cos, sin) per vane
+    double v[2 * PB_SDF_MAX_VERTICES];     // polygon: (x, y) per vertex; spider: (cos, sin) per vane
 };
 
 __device__ __forceinline__ double box_distance(double qx, double qy) {
@@ -108,7 +106,7 @@ extern "C" int pb_sdf(pb_handle_t hh, int dtype, int kind, const void* x, const 
     if (kind < PB_SDF_POLYGON || kind > PB_SDF_OFFSET_CIRCLE) return fail(h, PB_ERR_INVALID, "unknown shape kind");
     if (ny < 0 || nx < 0 || nparams < 0 || nparams > 8 || nverts < 0 || (nparams && !params_host) || (nverts && !verts_host))
         return fail(h, PB_ERR_INVALID, "bad shape arguments");
-    if (nverts > kMaxVerts) return fail(h, PB_ERR_UNSUPPORTED, "more than 128 polygon vertices or spider vanes");
+    if (nverts > PB_SDF_MAX_VERTICES) return fail(h, PB_ERR_UNSUPPORTED, "more than 128 polygon vertices or spider vanes");
     if ((kind == PB_SDF_POLYGON || kind == PB_SDF_SPIDER) && nverts < 1)
         return fail(h, PB_ERR_INVALID, "a polygon needs vertices and a spider vanes");
     if ((long long)ny * nx == 0) return PB_OK;

@@ -17,9 +17,7 @@
 
 namespace pb {
 
-#define PB_JAC_MAX 120             // highest order of a 1-D recurrence
 #define PB_POLY_PLANES 1024        // output planes per 1-D call
-#define PB_CLEN_J 8                // highest derivative order of jacobi_sum_clenshaw_der
 #define PB_XY_PLANES 1024          // output planes per XY-monomial call
 #define PB_TSUM_COEFS 1024         // (max m + 1) (max n + 1) of a tensor-product sum
 
@@ -29,7 +27,7 @@ struct P1Step { double A, B, C, wv, wd; short e0, e1, pad0, pad1; };
 struct P1Plan {
     int seed, nmax;
     double p0, s1a, s1b, dp1;      // P_0; P_1 = s1a + s1b (x - 1)/2 (SEED_JACOBI) or s1a x + s1b; dP_1/dx
-    P1Step s[PB_JAC_MAX + 1];      // order k: (A, B, C) of the step that makes P_k (k >= 2), sum weights, planes [e0, e1)
+    P1Step s[PB_POLY_NMAX + 1];    // order k: (A, B, C) of the step that makes P_k (k >= 2), sum weights, planes [e0, e1)
     int ent[PB_POLY_PLANES];       // plane << 1 | (1: the derivative track)
     double scale[PB_POLY_PLANES];
 };
@@ -88,7 +86,8 @@ __global__ void poly1d_kernel(const R* __restrict__ a, const R* __restrict__ b, 
 // n > M - jj.  table: every plane (jj, n) of out (j+1, N, count);  otherwise alpha_0[0] alone into out (count).
 struct ClenPlan {
     int N, M, j, table;
-    double s[PB_JAC_MAX + 1], A[PB_JAC_MAX + 1], B[PB_JAC_MAX + 1], C1[PB_JAC_MAX + 1];   // C1[n] = C_{n+1}
+    double s[PB_POLY_NMAX + 1], A[PB_POLY_NMAX + 1], B[PB_POLY_NMAX + 1];
+    double C1[PB_POLY_NMAX + 1];   // C1[n] = C_{n+1}
 };
 static_assert(sizeof(ClenPlan) <= 32764, "the Clenshaw plan must fit the kernel parameter space");
 
@@ -96,13 +95,13 @@ template <typename R>
 __global__ void clenshaw_kernel(const R* __restrict__ x, long long n, const __grid_constant__ ClenPlan pl, R* __restrict__ out) {
     PB_GRID_STRIDE(i, n) {
         const double xv = x[i];
-        double a1[PB_CLEN_J + 1], a2[PB_CLEN_J + 1];
+        double a1[PB_CLENSHAW_JMAX + 1], a2[PB_CLENSHAW_JMAX + 1];
 #pragma unroll
-        for (int jj = 0; jj <= PB_CLEN_J; ++jj) { a1[jj] = 0.0; a2[jj] = 0.0; }
+        for (int jj = 0; jj <= PB_CLENSHAW_JMAX; ++jj) { a1[jj] = 0.0; a2[jj] = 0.0; }
         for (int k = pl.N - 1; k >= 0; --k) {
             const double lin = pl.A[k] * xv + pl.B[k];
 #pragma unroll
-            for (int jj = PB_CLEN_J; jj >= 0; --jj) {
+            for (int jj = PB_CLENSHAW_JMAX; jj >= 0; --jj) {
                 if (jj > pl.j) continue;
                 double v = 0.0;
                 if (k <= pl.M - jj) {
@@ -292,7 +291,7 @@ extern "C" int pb_jacobi_seq(pb_handle_t hh, int dtype, const void* x, long long
                              const int* slots_host, void* out, void* stream) {
     PB_ENTER_REAL(hh);
     if (!x || !out || !slots_host || nmax < 0) return fail(h, PB_ERR_INVALID, "bad jacobi arguments");
-    if (nmax > PB_JAC_MAX) return fail(h, PB_ERR_UNSUPPORTED, "jacobi order above 120");
+    if (nmax > PB_POLY_NMAX) return fail(h, PB_ERR_UNSUPPORTED, "jacobi order above 120");
     if (count <= 0) return PB_OK;
     std::vector<P1Term> terms;
     for (int j = 0; j <= nmax; ++j)
@@ -311,7 +310,7 @@ extern "C" int pb_poly_seq(pb_handle_t hh, int dtype, int family, int kind, doub
     if ((long long)k * (kind == PB_POLY_VALUE_DER ? 2 : 1) > PB_POLY_PLANES) return fail(h, PB_ERR_UNSUPPORTED, "poly: more than 1024 planes");
     for (int q = 0; q < k; ++q) {
         if (n_host[q] < 0) return fail(h, PB_ERR_INVALID, "poly: order n must be >= 0");
-        if (n_host[q] > PB_JAC_MAX) return fail(h, PB_ERR_UNSUPPORTED, "poly: order above 120");
+        if (n_host[q] > PB_POLY_NMAX) return fail(h, PB_ERR_UNSUPPORTED, "poly: order above 120");
     }
     // the derivative by order shift, as the reference forms it: Jacobi 0.5 (n + a + b + 1) P_{n-1}^(a+1, b+1),
     // Hermite kind n P_{n-1}, Laguerre -L_{n-1}^(a+1); an order-0 plane is 0 P_0
@@ -348,7 +347,7 @@ extern "C" int pb_jacobi_radial_sum(pb_handle_t hh, int dtype, double alpha, dou
     std::vector<P1Term> terms;
     for (int q = 0; q < k; ++q) {
         if (n_host[q] < 0) return fail(h, PB_ERR_INVALID, "poly: order n must be >= 0");
-        if (n_host[q] > PB_JAC_MAX) return fail(h, PB_ERR_UNSUPPORTED, "poly: order above 120");
+        if (n_host[q] > PB_POLY_NMAX) return fail(h, PB_ERR_UNSUPPORTED, "poly: order above 120");
         if (coefs_host[q] == 0.0) continue;                          // jacobi.py:386 skips zero weights
         terms.push_back({n_host[q], -1, 0, 0.0, coefs_host[q], coefs_host[q]});
     }
@@ -367,8 +366,8 @@ extern "C" int pb_jacobi_clenshaw(pb_handle_t hh, int dtype, double alpha, doubl
                                   int len, const double* s_host, int j, int table, void* out, void* stream) {
     PB_ENTER_REAL(hh);
     if (!x || !out || len < 1 || !s_host || j < 0) return fail(h, PB_ERR_INVALID, "bad clenshaw arguments");
-    if (j > PB_CLEN_J) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: derivative order above 8");
-    if (len > PB_JAC_MAX + 1) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: more than 121 coefficients");
+    if (j > PB_CLENSHAW_JMAX) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: derivative order above 8");
+    if (len > PB_POLY_NMAX + 1) return fail(h, PB_ERR_UNSUPPORTED, "clenshaw: more than 121 coefficients");
     ClenPlan pl;
     pl.M = len - 1; pl.N = std::max(len, 2); pl.j = j; pl.table = table ? 1 : 0;
     for (int nn = 0; nn < pl.N; ++nn) {

@@ -17,7 +17,6 @@
 
 namespace pb {
 
-#define PB_QPOLY_NMAX 64          // highest radial order n, and highest |m| of 2D-Q
 #define PB_QPOLY_STEPS 256        // recurrence steps per call: the sum over groups of (highest n + 1)
 #define PB_QPOLY_ENTRIES 1024     // output planes per basis call
 

@@ -14,7 +14,6 @@
 
 namespace pb {
 
-#define PB_TF_DIMS 4
 #define PB_TF_THREADS 256
 
 struct TfOut { void* p[PB_TF_NOUT]; };

@@ -30,9 +30,9 @@ CEIL = 1e4
 # ---- launch and plan rules (mirrors of csrc/common.cuh, orthopoly.cu, synthesis.cu and qpoly.cu) --------------------
 THREADS = 256
 BLOCKS_PER_SM = 16
-JAC_MAX = 120                   # PB_JAC_MAX: highest order of a 1-D recurrence
+JAC_MAX = 120                   # PB_POLY_NMAX: highest order of a 1-D recurrence
 POLY_PLANES = 1024              # PB_POLY_PLANES: output planes per 1-D call (VALUE_DER counts 2 per order)
-CLEN_J = 8                      # PB_CLEN_J: highest Clenshaw derivative order
+CLEN_J = 8                      # PB_CLENSHAW_JMAX: highest Clenshaw derivative order
 CLEN_LEN = JAC_MAX + 1          # Clenshaw coefficients
 XY_PLANES = 1024                # PB_XY_PLANES
 XY_ORDER = 32767                # highest XY order (a short)

@@ -89,21 +89,30 @@ def test_product_never_imports_the_oracle():
 
 
 def test_python_constants_match_the_header_enums():
-    """The integer codes the ctypes layer passes are the enum values the header declares."""
+    """The integer codes the ctypes layer passes are the enum values the header declares: every PB_NAME is
+    _capi.NAME, except PB_C64 and PB_C128, which keep their names."""
     from prysm_b200 import _capi
     src = open(os.path.join(ROOT, 'include', 'prysm_b200.h')).read()
     enums = {k: int(v) for k, v in re.findall(r'\b(PB_[A-Z0-9_]+)\s*=\s*(-?\d+)', src)}
-    pairs = {'PB_C64': _capi.PB_C64, 'PB_C128': _capi.PB_C128, 'PB_IN_COMPLEX': _capi.IN_COMPLEX, 'PB_IN_REAL': _capi.IN_REAL,
-             'PB_IN_AMP_OPD': _capi.IN_AMP_OPD, 'PB_AMP_NONE': _capi.AMP_NONE, 'PB_AMP_REAL': _capi.AMP_REAL,
-             'PB_AMP_U8': _capi.AMP_U8, 'PB_OUT_COMPLEX': _capi.OUT_COMPLEX, 'PB_OUT_INTENSITY': _capi.OUT_INTENSITY,
-             'PB_OUT_ACCUMULATE': _capi.OUT_ACCUMULATE, 'PB_MASK_REAL': _capi.MASK_REAL, 'PB_MASK_COMPLEX': _capi.MASK_COMPLEX,
-             'PB_MASK_CONJ': _capi.MASK_CONJ, 'PB_MASK_ONE_MINUS': _capi.MASK_ONE_MINUS, 'PB_MASK_REAL_OUT': _capi.MASK_REAL_OUT,
-             'PB_MASK_ACCUMULATE': _capi.MASK_ACCUMULATE}
-    for e in ('F32', 'F64', 'C64', 'C128', 'U8', 'U16', 'U32', 'I32', 'I64'):
-        pairs['PB_ELEM_' + e] = getattr(_capi, 'ELEM_' + e)
-    for name, val in pairs.items():
-        assert enums[name] == val, name
+    assert len(enums) >= 152
+    for name, val in enums.items():
+        assert getattr(_capi, name if name in ('PB_C64', 'PB_C128') else name[3:]) == val, name
     assert enums['PB_OK'] == 0 and enums['PB_ERR_INVALID'] == -1      # Handle.check maps -1 to ValueError
+
+
+@pytest.mark.parametrize('decl', ['int pb_g(pb_handle_t h, float x);', 'enum { PB_A = 1, PB_B };',
+                                  'int pb_g(int n) { return n; }'])
+def test_read_header_refuses_what_it_cannot_bind(tmp_path, decl):
+    """A C type without a ctypes mapping, an enumerator without a literal value or a declaration the reader cannot
+    parse fails the import: the binding never guesses an argument type or a code."""
+    from prysm_b200 import _capi
+    path = tmp_path / 'api.h'
+    path.write_text('enum { PB_K = -2 };\nlong long pb_f(pb_handle_t h, const double* x, int n, double s);\n')
+    assert _capi.read_header(str(path)) == (
+        {'pb_f': (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_double])}, {'PB_K': -2})
+    path.write_text(path.read_text() + decl + '\n')
+    with pytest.raises(ImportError, match=re.escape(str(path))):
+        _capi.read_header(str(path))
 
 
 def test_only_tests_smoke_and_bench_touch_the_oracle():
