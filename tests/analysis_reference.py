@@ -15,31 +15,20 @@ import os
 
 import numpy as np
 
-LDBL = np.longdouble
-assert np.finfo(LDBL).nmant >= 63, 'the references need an 80-bit long double'
+from accuracy import LDBL, grid_for, sweep  # noqa: F401
+
 EPS = np.finfo(np.float64).eps
 
 # ---- launch rules (mirrors of csrc/analysis.cu and csrc/common.cuh) ------------------------------------------------
 AN_THREADS = 256                # AN_THREADS: threads of every analysis block
 AZ_MAX_NY = 28672               # PB_AZ_MAX_NY: phi samples of one column held in shared memory
-BLOCKS_PER_SM = 16              # grid_for's cap
 AZ_LAUNCHES = 1                 # pb_azimuthal_stats: one launch whatever the mask
 INTERP_LAUNCHES = 1
 ANALYTIC_LAUNCHES = 1
 
 
-def grid_for(n, sm_count, threads=AN_THREADS):
-    """csrc/common.cuh grid_for: ceil(n / threads) blocks, at least 1, at most sm_count * 16"""
-    return max(1, min((n + threads - 1) // threads, sm_count * BLOCKS_PER_SM))
-
-
-def grid_cap(sm_count):
-    """items one sweep of a capped grid-stride launch covers"""
-    return sm_count * BLOCKS_PER_SM * AN_THREADS
-
-
 def sweep_counts(sm_count):
-    c = grid_cap(sm_count)
+    c = sweep(sm_count)
     return (1, c - 1, c, c + 1, 3 * c)
 
 

@@ -11,9 +11,7 @@ defects, so that tests/test_host_generic_reference.py can show that the ceilings
 import numpy as np
 import scipy.fft as sfft
 
-assert np.finfo(np.longdouble).nmant >= 63, (
-    'the generic-axis reference needs an 80-bit long double (x86-64); this host has '
-    f'{np.finfo(np.longdouble).nmant + 1} mantissa bits')
+from accuracy import ld
 
 LD = np.clongdouble
 PI_LD = np.longdouble('3.14159265358979323846264338327950288')
@@ -74,12 +72,6 @@ def merge(*counts):
 
 
 # ---- the long-double reference --------------------------------------------------------------------------------------
-def ld(a):
-    """the exact values the device got, as long double"""
-    a = np.asarray(a)
-    return a.astype(LD if np.iscomplexobj(a) else np.longdouble)
-
-
 def fft_ld(a, n=None, axis=-1, inverse=False):
     """numpy's fft(a, n, axis) (inverse: unnormalised, sign +) in long double"""
     a = ld(a)

@@ -1,5 +1,6 @@
-"""The fixture and helpers the GPU tests share: `from gpu_fixtures import pb, host`, and the per-route launch counters
-(pb_route_launch_count) that pin which transform kernels a call ran: `routes_of(fn, codes)`."""
+"""The fixture and helpers the GPU tests share: `from gpu_fixtures import pb, dev, host`, seeded inputs (`crand`), the
+launch counters: all kernels (`launches(pb, fn)`) and per route (pb_route_launch_count), which pin which transform
+kernels a call ran (`routes_of(fn, codes)`)."""
 import numpy as np
 import pytest
 import torch
@@ -17,8 +18,31 @@ def pb():
     prysm_b200.mathops.set_backend_to_defaults()
 
 
+def dev(a):
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
 def host(t):
     return t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+
+
+def crand(shape, seed, dtype=np.complex128, scale=1.0):
+    """a seeded complex Gaussian, drawn in fp64 and rounded to `dtype`"""
+    rng = np.random.default_rng(seed)
+    return ((rng.standard_normal(shape) + 1j * rng.standard_normal(shape)) * scale).astype(dtype)
+
+
+def sm_count():
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+def launches(pb, fn):
+    """fn()'s result and the kernels it launched"""
+    torch.cuda.synchronize()
+    c0 = pb._ops.launch_count()
+    res = fn()
+    torch.cuda.synchronize()
+    return res, pb._ops.launch_count() - c0
 
 
 def _handle():

@@ -18,8 +18,7 @@ a kernel with one deliberate fault; tests/test_host_poly_reference.py shows the 
 """
 import numpy as np
 
-LDBL = np.longdouble
-assert np.finfo(LDBL).nmant >= 63, 'the references need an 80-bit long double'
+from accuracy import LDBL, THREADS, grid_for, sweep  # noqa: F401
 U53 = 2.0 ** -53
 U24 = 2.0 ** -24
 
@@ -28,8 +27,6 @@ U24 = 2.0 ** -24
 CEIL = 1e4
 
 # ---- launch and plan rules (mirrors of csrc/common.cuh, orthopoly.cu, synthesis.cu and qpoly.cu) --------------------
-THREADS = 256
-BLOCKS_PER_SM = 16
 JAC_MAX = 120                   # PB_POLY_NMAX: highest order of a 1-D recurrence
 POLY_PLANES = 1024              # PB_POLY_PLANES: output planes per 1-D call (VALUE_DER counts 2 per order)
 CLEN_J = 8                      # PB_CLENSHAW_JMAX: highest Clenshaw derivative order
@@ -48,16 +45,6 @@ Q_ENTRIES = 1024                # PB_QPOLY_ENTRIES
 FAMILIES = ('jacobi', 'cheby1', 'cheby2', 'cheby3', 'cheby4', 'legendre', 'hermite_he', 'hermite_h', 'laguerre',
             'dickson1', 'dickson2')      # the order of capi.POLY_*
 SHIFTED = ('jacobi', 'hermite_he', 'hermite_h', 'laguerre')   # POLY_DER by a shifted order, as the reference forms it
-
-
-def grid_for(n, sm_count, threads=THREADS):
-    """csrc/common.cuh grid_for: ceil(n / threads) blocks, at least 1, at most 16 per SM"""
-    return max(1, min((n + threads - 1) // threads, sm_count * BLOCKS_PER_SM))
-
-
-def sweep(sm_count):
-    """samples one grid-stride sweep covers"""
-    return BLOCKS_PER_SM * sm_count * THREADS
 
 
 def sweep_counts(sm_count):

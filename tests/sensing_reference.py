@@ -21,8 +21,7 @@ import os
 import numpy as np
 import scipy.special as sps
 
-LDBL = np.longdouble
-assert np.finfo(LDBL).nmant >= 63, 'the references need an 80-bit long double'
+from accuracy import LDBL
 
 # ---- launch rules (mirrors of csrc/wfs.cu and csrc/shack_hartmann.cu) ----------------------------------------------
 THREADS = 256                   # kThreads of both files

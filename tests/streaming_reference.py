@@ -22,6 +22,7 @@ import scipy.ndimage as ndi
 import scipy.special as sps
 
 import generic_reference as G
+from accuracy import LDBL, THREADS, grid_for, ld, sweep  # noqa: F401
 from generic_reference import LD, PB_C64, PB_C128, expi_ld, phase_field_ld, centred_ft2_ld  # noqa: F401
 
 RDT = {PB_C64: np.float32, PB_C128: np.float64}
@@ -30,17 +31,10 @@ DT_NAME = G.DT_NAME
 CEIL_ELEM = G.CEILING                 # relative L-inf of an elementwise output: a few ulps of R
 CEIL_RED = 1e-13                      # |got - ref| / sum|terms| of an fp64-accumulated reduction, both dtypes
 CEIL_EE = 1e-12                       # encircled energy: the same over ee_ref's majorant, j1 error included
-LDBL = np.longdouble
 
 
 # ---- launch geometry (mirrors of the C++) --------------------------------------------------------------------------
-THREADS = 256
 PB_MAX_MODES = 64                     # csrc/elementwise.cu: #define PB_MAX_MODES 64 (weights per weighted_sum launch)
-
-
-def grid_for(n, sm_count, threads=THREADS):
-    """csrc/common.cuh grid_for: ceil(n / threads) blocks, at least 1, at most sm_count * 16"""
-    return max(1, min((n + threads - 1) // threads, sm_count * 16))
 
 
 def reduction_grid(n, sm_count, threads=THREADS):
@@ -54,11 +48,6 @@ def mode_projection_gx(n, k, sm_count, threads=THREADS):
     return min((n + threads - 1) // threads, max(1, sm_count * 4 // k))
 
 
-def elementwise_cap(sm_count):
-    """samples one sweep of a grid_for launch covers"""
-    return sm_count * 16 * THREADS
-
-
 def reduction_cap(sm_count):
     return sm_count * 4 * THREADS
 
@@ -68,7 +57,7 @@ def shapes(sm_count):
     1 x n and n x 1), 1 x 1, 1 x n, n x 1, a partial warp, an odd shape, and two that take many sweeps"""
     out = {'1x1': (1, 1), '1xn': (1, 1000), 'nx1': (1000, 1), '31x33': (31, 33), '1023x769': (1023, 769),
            '2048sq': (2048, 2048), '4096sq': (4096, 4096)}
-    for tag, cap in (('red', reduction_cap(sm_count)), ('elem', elementwise_cap(sm_count))):
+    for tag, cap in (('red', reduction_cap(sm_count)), ('elem', sweep(sm_count))):
         out.update({f'{tag}-1': (1, cap - 1), tag: (cap, 1), f'{tag}+1': (1, cap + 1)})
     return out
 
@@ -84,7 +73,7 @@ def rel_linf(got, ref):
     if not np.all(np.isfinite(got)):
         return math.inf
     den = float(np.abs(ref).max())
-    return float(np.abs(G.ld(got) - ref).max()) / (den if den > 0 else 1.0)
+    return float(np.abs(ld(got) - ref).max()) / (den if den > 0 else 1.0)
 
 
 def red_fig(got, ref, cond):
@@ -93,11 +82,7 @@ def red_fig(got, ref, cond):
     if not np.all(np.isfinite(got)):
         return math.inf
     cond = np.where(cond > 0, cond, 1)
-    return float(np.max(np.abs(G.ld(got) - ref) / cond))
-
-
-def ld(a):
-    return G.ld(a)
+    return float(np.max(np.abs(ld(got) - ref) / cond))
 
 
 # ---- reductions -----------------------------------------------------------------------------------------------------

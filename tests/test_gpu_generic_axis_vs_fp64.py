@@ -43,9 +43,10 @@ import scipy.fft as sfft
 import torch
 
 import generic_reference as G
-from conftest import within
+from accuracy import Ledger
 from generic_reference import PB_C64, PB_C128, DT_NAME, CEILING, LD
-from gpu_fixtures import pb  # noqa: F401
+from gpu_fixtures import pb, dev, host  # noqa: F401
+from gpu_fixtures import crand as _crand
 from gpu_fixtures import routes_of
 
 pytestmark = pytest.mark.gpu
@@ -543,16 +544,13 @@ MEASURED = {
 }
 
 
-def bound(name, dt):
-    case, metric = name.rsplit('/', 1)
-    m = MEASURED.get(case, {}).get(metric)
-    if m is None:
-        return CEILING[dt]
-    return min(1.5 * m, CEILING[dt]) if m > 0 else float(np.nextafter(0.0, 1.0))
+CEIL_OF = {DT_NAME[dt]: CEILING[dt] for dt in DTYPES}
+# a figure's worst over its test; one test per figure name in the whole file, so that MEASURED keeps every figure (not
+# the last of several)
+LEDGER = Ledger(MEASURED, lambda name: CEIL_OF[name.split('/', 1)[0]], per_test=True, one_test_per_name=True)
 
 
 # ---- which kernels ran ----------------------------------------------------------------------------------------------
-RECORDED = {}       # figure name -> the test that recorded it
 HIT = set()          # (L, dtype, cols) of every generic launch an extended-precision-checked case made
 _CODES = {}
 
@@ -575,65 +573,32 @@ def codes():
     return _CODES
 
 
-class Checker:
-    """Compares whole arrays with their long-double references; `done()` records every figure with conftest.within and
-    fails with all that are over their bounds and every case that ran other kernels than it should."""
+def run(case, fn, expect, others=0):
+    """fn() for its result; it must launch exactly `expect` ({(L, dtype, cols): n}) on the generic pass, nothing on
+    the register engine or the focus pair, and `others` launches of other kernels"""
+    res, used = routes_of(fn, codes())
+    gen = {k[1:]: v for k, v in used.items() if isinstance(k, tuple) and k[0] == 'g'}
+    tuned = sorted(str(k) for k in used if isinstance(k, tuple) and k[0] != 'g')
+    ngen = sum(gen.values())
+    LEDGER.route(gen == expect, f'{case}: generic launches {gen}, expected {expect}')
+    LEDGER.route(not tuned, f'{case}: tuned kernels ran: {tuned}')
+    LEDGER.route(used.get('generic', 0) == ngen, f'{case}: total generic counter {used.get("generic", 0)} != {ngen}')
+    LEDGER.route(used.get('all', 0) == ngen + others, f'{case}: {used.get("all", 0)} launches, expected {ngen + others}')
+    HIT.update(gen)
+    return res
 
-    def __init__(self):
-        self.figs = {}
-        self.dts = {}
-        self.bad = []
 
-    def route(self, ok, msg):
-        if not ok:
-            self.bad.append(msg)
-
-    def run(self, case, fn, expect, others=0):
-        """fn() for its result; it must launch exactly `expect` ({(L, dtype, cols): n}) on the generic pass, nothing
-        on the register engine or the focus pair, and `others` launches of other kernels"""
-        res, used = routes_of(fn, codes())
-        gen = {k[1:]: v for k, v in used.items() if isinstance(k, tuple) and k[0] == 'g'}
-        tuned = sorted(str(k) for k in used if isinstance(k, tuple) and k[0] != 'g')
-        ngen = sum(gen.values())
-        self.route(gen == expect, f'{case}: generic launches {gen}, expected {expect}')
-        self.route(not tuned, f'{case}: tuned kernels ran: {tuned}')
-        self.route(used.get('generic', 0) == ngen, f'{case}: total generic counter {used.get("generic", 0)} != {ngen}')
-        self.route(used.get('all', 0) == ngen + others, f'{case}: {used.get("all", 0)} launches, expected {ngen + others}')
-        HIT.update(gen)
-        return res
-
-    def add(self, case, dt, got, ref):
-        got = got.detach().cpu().numpy() if torch.is_tensor(got) else np.asarray(got)
-        assert got.shape == ref.shape, (case, got.shape, ref.shape)
-        for metric, v in (('linf', G.rel_linf(got, ref)), ('l2', G.rel_l2(got, ref))):
-            name = f'{DT_NAME[dt]}/{case}/{metric}'
-            self.figs[name] = max(v, self.figs.get(name, 0.0))
-            self.dts[name] = dt
-
-    def done(self):
-        bad = []
-        for name, v in self.figs.items():
-            # one test per figure name in the whole file, so that MEASURED keeps every figure (not the last of several)
-            test = os.environ.get('PYTEST_CURRENT_TEST', '').split(' ')[0]
-            assert RECORDED.setdefault(name, test) == test, f'{name} is recorded by {RECORDED[name]} and {test}'
-            # every figure has its measurement: a new case is held to 1.5x its own figure, not to the ceiling
-            if name.rsplit('/', 1)[0] not in MEASURED and not os.environ.get('PB_TEST_MEASUREMENTS'):
-                bad.append(f'{name}: {v:.3e} has no MEASURED entry (record it with PB_TEST_MEASUREMENTS)')
-            try:
-                within(name, v, bound(name, self.dts[name]))
-            except AssertionError as e:
-                bad.append(str(e))
-        assert not bad + self.bad, '\n'.join(bad + self.bad)
+def add(case, dt, got, ref):
+    """the whole array against its long-double reference: rel_linf and the relative L2 error"""
+    got = host(got)
+    assert got.shape == ref.shape, (case, got.shape, ref.shape)
+    for metric, v in (('linf', G.rel_linf(got, ref)), ('l2', G.rel_l2(got, ref))):
+        LEDGER.record(f'{DT_NAME[dt]}/{case}/{metric}', v)
 
 
 # ---- inputs -----------------------------------------------------------------------------------------------------------
 def crand(shape, seed, dt):
-    rng = np.random.default_rng(seed)
-    return (rng.standard_normal(shape) + 1j * rng.standard_normal(shape)).astype(G.CPLX[dt])
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    return _crand(shape, seed, G.CPLX[dt])
 
 
 def lines_for(n):
@@ -662,18 +627,17 @@ def test_fft1_every_length(pb, dt, axis, d):
     from prysm_b200 import _ops
     cols = int(axis == 0)
     lens = [n for n in pow2_lengths(dt) if not (dt == PB_C64 and n in TUNED)] + list(bluestein_lengths(dt))
-    chk = Checker()
     for n in lens:
         for nl in lines_for(n):
             shape = (nl, n) if axis == 1 else (n, nl)
             a = crand(shape, n * 7 + nl + dt, dt)
             x = dev(a)
             case = f'fft1_{ROWS_COLS[cols]}_{"inv" if d > 0 else "fwd"}/{n}'
-            got = chk.run(f'{case}x{nl}', lambda: _ops.fft1(x, axis=axis, dir=d, scale=1.0 / n if d > 0 else 1.0),
-                          G.axis_launches(n, dt, cols))
+            got = run(f'{case}x{nl}', lambda: _ops.fft1(x, axis=axis, dir=d, scale=1.0 / n if d > 0 else 1.0),
+                      G.axis_launches(n, dt, cols))
             ref = G.fft_ld(a, axis=axis, inverse=d > 0) / (n if d > 0 else 1)
-            chk.add(case, dt, got, ref)
-    chk.done()
+            add(case, dt, got, ref)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('axis', (1, 0))
@@ -682,14 +646,13 @@ def test_fft1_pad_and_truncate(pb, dt, axis):
     """n longer than the input (zero pad) and shorter (truncation), power-of-two and Bluestein n"""
     from prysm_b200 import _ops
     cols = int(axis == 0)
-    chk = Checker()
     for n, m in ((1000, 995), (1000, 1007), (512, 300), (512, 700), (97, 1), (2047, 2100)):
         shape = (5, m) if axis == 1 else (m, 5)
         a = crand(shape, n + m, dt)
         x = dev(a)
-        got = chk.run(f'pad/{n}/{m}', lambda: _ops.fft1(x, n, axis=axis), G.axis_launches(n, dt, cols))
-        chk.add(f'fft1_pad_truncate_{ROWS_COLS[cols]}/{n}_{m}', dt, got, G.fft_ld(a, n, axis=axis))
-    chk.done()
+        got = run(f'pad/{n}/{m}', lambda: _ops.fft1(x, n, axis=axis), G.axis_launches(n, dt, cols))
+        add(f'fft1_pad_truncate_{ROWS_COLS[cols]}/{n}_{m}', dt, got, G.fft_ld(a, n, axis=axis))
+    LEDGER.done()
 
 
 # ---- fft2 compositions ---------------------------------------------------------------------------------------------
@@ -711,16 +674,15 @@ FFT2_CASES = [  # (ny, nx), (ky, kx), crop, shift
 def test_fft2_pad_shift_crop(pb, dt):
     """centred pad (in_off), shift_in / shift_out at odd and even k, odd and even crops, both directions"""
     from prysm_b200 import _ops
-    chk = Checker()
     for i, (n, k, crop, shift) in enumerate(FFT2_CASES):
         a = crand(n, 40 + i, dt)
         x = dev(a)
         for d in (-1, 1):
             case = f'fft2_{"inv" if d > 0 else "fwd"}/{n[0]}x{n[1]}_{k[0]}x{k[1]}'
-            got = chk.run(case, lambda: _ops.fft2(x, k, dir=d, shift_in=shift, shift_out=shift, crop=crop),
-                          fft2_launches(k, dt))
-            chk.add(case, dt, got, G.centred_ft2_ld(a, k, inverse=d > 0, crop=crop, shift=shift))
-    chk.done()
+            got = run(case, lambda: _ops.fft2(x, k, dir=d, shift_in=shift, shift_out=shift, crop=crop),
+                      fft2_launches(k, dt))
+            add(case, dt, got, G.centred_ft2_ld(a, k, inverse=d > 0, crop=crop, shift=shift))
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('dt', DTYPES)
@@ -735,29 +697,28 @@ def test_fft2_output_and_input_kinds(pb, dt):
     launches = fft2_launches(k, dt)
     ref = G.centred_ft2_ld(a, k, crop=crop)
     inten = ref.real ** 2 + ref.imag ** 2
-    chk = Checker()
-    got = chk.run('intensity', lambda: _ops.fft2(x, k, shift_in=True, shift_out=True, crop=crop,
-                                                   out_kind=capi.OUT_INTENSITY), launches)
-    chk.add('fft2_intensity', dt, got, inten)
+    got = run('intensity', lambda: _ops.fft2(x, k, shift_in=True, shift_out=True, crop=crop,
+                                               out_kind=capi.OUT_INTENSITY), launches)
+    add('fft2_intensity', dt, got, inten)
     acc0 = torch.rand(crop, generator=torch.Generator(device='cuda').manual_seed(5), device='cuda', dtype=RDT[dt])
-    got = chk.run('accumulate', lambda: _ops.fft2(x, k, shift_in=True, shift_out=True, crop=crop, weight=WEIGHT,
-                                                    out_kind=capi.OUT_ACCUMULATE, out=acc0.clone()), launches)
-    chk.add('fft2_accumulate', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * inten)
+    got = run('accumulate', lambda: _ops.fft2(x, k, shift_in=True, shift_out=True, crop=crop, weight=WEIGHT,
+                                                out_kind=capi.OUT_ACCUMULATE, out=acc0.clone()), launches)
+    add('fft2_accumulate', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * inten)
 
     r = np.random.default_rng(51).standard_normal(n).astype(NPR[dt])
-    got = chk.run('real', lambda: _ops.fft2(dev(r), k, shift_in=True, shift_out=True), launches)
-    chk.add('fft2_real_input', dt, got, G.centred_ft2_ld(r.astype(LD), k))
+    got = run('real', lambda: _ops.fft2(dev(r), k, shift_in=True, shift_out=True), launches)
+    add('fft2_real_input', dt, got, G.centred_ft2_ld(r.astype(LD), k))
 
     rng = np.random.default_rng(52)
     opd = (300.0 * rng.standard_normal(n)).astype(NPR[dt])
     ampr = rng.uniform(0.2, 1.0, n).astype(NPR[dt])
     ampu = (rng.random(n) > 0.3)
     for name, amp in (('none', None), ('real', ampr), ('u8', ampu)):
-        got = chk.run(f'opd_{name}', lambda: _ops.fft2(None, k, dir=-1, shift_in=True, shift_out=True, crop=crop,
-                                                       opd=dev(opd), amp=None if amp is None else dev(amp),
-                                                       kscale=KSCALE), launches)
-        chk.add(f'fft2_opd_amp_{name}', dt, got, G.centred_ft2_ld(G.phase_field_ld(opd, KSCALE, amp), k, crop=crop))
-    chk.done()
+        got = run(f'opd_{name}', lambda: _ops.fft2(None, k, dir=-1, shift_in=True, shift_out=True, crop=crop,
+                                                   opd=dev(opd), amp=None if amp is None else dev(amp),
+                                                   kscale=KSCALE), launches)
+        add(f'fft2_opd_amp_{name}', dt, got, G.centred_ft2_ld(G.phase_field_ld(opd, KSCALE, amp), k, crop=crop))
+    LEDGER.done()
 
 
 # ---- public entry points at precision 64 ---------------------------------------------------------------------------
@@ -779,7 +740,6 @@ def test_public_focus_family(pb, N, Q):
     K = math.ceil(N * Q)
     Nb = int(K // Q)
     dt = PB_C128
-    chk = Checker()
     fwd = fft2_launches((K, K), dt)
     if K <= 1024:
         a = crand((N, N), N + int(10 * Q), dt)
@@ -801,12 +761,12 @@ def test_public_focus_family(pb, N, Q):
         tag = 'impulses'
     x, y = dev(a), dev(g)
     case = f'{tag}/{N}_q{Q}'
-    chk.add(f'focus/{case}', dt, chk.run(f'focus/{case}', lambda: P.focus(x, Q), fwd), ref_f(False))
-    chk.add(f'unfocus/{case}', dt, chk.run(f'unfocus/{case}', lambda: P.unfocus(x, Q), fwd), ref_f(True))
-    chk.add(f'focus_adjoint/{case}', dt, chk.run(f'focus_adjoint/{case}', lambda: P.focus_adjoint(y, Q), fwd), ref_a(True))
-    chk.add(f'unfocus_adjoint/{case}', dt, chk.run(f'unfocus_adjoint/{case}', lambda: P.unfocus_adjoint(y, Q), fwd),
-            ref_a(False))
-    chk.done()
+    add(f'focus/{case}', dt, run(f'focus/{case}', lambda: P.focus(x, Q), fwd), ref_f(False))
+    add(f'unfocus/{case}', dt, run(f'unfocus/{case}', lambda: P.unfocus(x, Q), fwd), ref_f(True))
+    add(f'focus_adjoint/{case}', dt, run(f'focus_adjoint/{case}', lambda: P.focus_adjoint(y, Q), fwd), ref_a(True))
+    add(f'unfocus_adjoint/{case}', dt, run(f'unfocus_adjoint/{case}', lambda: P.unfocus_adjoint(y, Q), fwd),
+        ref_a(False))
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('N,Q', [(255, 2), (256, 1.5), (500, 2)])
@@ -819,21 +779,20 @@ def test_public_focus_intensity_and_psf(pb, N, Q):
     a = crand((N, N), N + 3, dt)
     ref = G.centred_ft2_ld(a, (K, K)) / K
     inten = ref.real ** 2 + ref.imag ** 2
-    chk = Checker()
     x = dev(a)
-    chk.add(f'focus_intensity/{N}_q{Q}', dt, chk.run('fi', lambda: P.focus_intensity(x, Q), fwd), inten)
+    add(f'focus_intensity/{N}_q{Q}', dt, run('fi', lambda: P.focus_intensity(x, Q), fwd), inten)
     acc0 = torch.rand((K, K), generator=torch.Generator(device='cuda').manual_seed(N), device='cuda', dtype=torch.float64)
-    got = chk.run('fia', lambda: P.focus_intensity(x, Q, weight=WEIGHT, out=acc0.clone()), fwd)
-    chk.add(f'focus_intensity_accumulate/{N}_q{Q}', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * inten)
+    got = run('fia', lambda: P.focus_intensity(x, Q, weight=WEIGHT, out=acc0.clone()), fwd)
+    add(f'focus_intensity_accumulate/{N}_q{Q}', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * inten)
     rng = np.random.default_rng(N)
     opd = 200.0 * rng.standard_normal((N, N))
     amp = rng.uniform(0.0, 1.0, (N, N))
     wvl = 0.6328
     kscale = P.phase_prefix(wvl).imag
     ref = G.centred_ft2_ld(G.phase_field_ld(opd, kscale, amp), (K, K)) / K
-    got = chk.run('psf', lambda: P.psf_from_amp_and_phase(dev(amp), dev(opd), wvl, Q), fwd)
-    chk.add(f'psf_from_amp_and_phase/{N}_q{Q}', dt, got, ref.real ** 2 + ref.imag ** 2)
-    chk.done()
+    got = run('psf', lambda: P.psf_from_amp_and_phase(dev(amp), dev(opd), wvl, Q), fwd)
+    add(f'psf_from_amp_and_phase/{N}_q{Q}', dt, got, ref.real ** 2 + ref.imag ** 2)
+    LEDGER.done()
 
 
 # ---- fft2_batch, one field at a time --------------------------------------------------------------------------------
@@ -848,7 +807,6 @@ def test_fft2_batch_fallback(pb, dt):
     shared = rng.random(n) > 0.25
     per = rng.uniform(0.1, 1.0, (nb,) + n).astype(NPR[dt])
     launches = {key: nb * v for key, v in fft2_launches(k, dt).items()}
-    chk = Checker()
     for name, amp in (('shared_u8', shared), ('per_field_real', per)):
         big0 = torch.full((nb + 1, k[0] + 2, k[1] + 5), 7.0, dtype=TDT[dt], device='cuda')
 
@@ -859,14 +817,14 @@ def test_fft2_batch_fallback(pb, dt):
                             kscale=KSCALE, out=out)
             inside = torch.zeros(big.shape, dtype=torch.bool, device='cuda')
             inside[:nb, 1:k[0] + 1, 3:k[1] + 3] = True
-            chk.route(torch.equal(big[~inside], big0[~inside]), f'{name}: a store outside the output windows')
+            LEDGER.route(torch.equal(big[~inside], big0[~inside]), f'{name}: a store outside the output windows')
             return out
-        got = chk.run(name, fn, launches)
+        got = run(name, fn, launches)
         for b in range(nb):
             ab = amp if amp.ndim == 2 else amp[b]
             ref = G.centred_ft2_ld(G.phase_field_ld(opd[b], KSCALE, ab), k) / 17
-            chk.add(f'fft2_batch_{name}', dt, got[b], ref)
-    chk.done()
+            add(f'fft2_batch_{name}', dt, got[b], ref)
+    LEDGER.done()
 
 
 # ---- axis_dft: fused multipliers and output windows ---------------------------------------------------------------
@@ -877,7 +835,6 @@ def test_axis_dft_multipliers(pb, dt, axis):
     lengths (on a Bluestein axis the user's multipliers ride as pre_e2 / post_e2 next to the chirp)"""
     from prysm_b200 import _ops
     cols = int(axis == 0)
-    chk = Checker()
     for n in (256, 1000, 97):
         nl = 11
         m = n - 3
@@ -888,15 +845,15 @@ def test_axis_dft_multipliers(pb, dt, axis):
         f = lambda v, c: np.conj(v) if c else v   # noqa: E731
         for conj in (0, 1, 2, 4, 8, 15):          # bits: pre_e, pre_b, post_e, post_b conjugated
             pc, pbc, qc, qbc = conj & 1, (conj >> 1) & 1, (conj >> 2) & 1, (conj >> 3) & 1
-            got = chk.run(f'axis_dft/{n}/{conj}', lambda: _ops.axis_dft(
+            got = run(f'axis_dft/{n}/{conj}', lambda: _ops.axis_dft(
                 dev(a), n, axis, dir=-1, scale=0.5, pre_e=dev(pre_e), pre_e_conj=bool(pc), pre_b=dev(pre_b),
                 pre_b_conj=bool(pbc), post_e=dev(post_e), post_e_conj=bool(qc), post_b=dev(post_b),
                 post_b_conj=bool(qbc), out_off=off, n_out=no), G.axis_launches(n, dt, cols))
             u = G.ld(a) if axis == 1 else G.ld(a).T
             u = u * G.ld(f(pre_e, pc))[:m] * G.ld(f(pre_b, pbc))[:, None]
             U = G.fft_ld(u, n)[:, off:off + no] * G.ld(f(post_e, qc)) * G.ld(f(post_b, qbc))[:, None] * LD(0.5)
-            chk.add(f'axis_dft_{ROWS_COLS[cols]}/{n}', dt, got, U if axis == 1 else U.T)
-    chk.done()
+            add(f'axis_dft_{ROWS_COLS[cols]}/{n}', dt, got, U if axis == 1 else U.T)
+    LEDGER.done()
 
 
 # ---- CZT, the two-pass fallback ------------------------------------------------------------------------------------
@@ -912,7 +869,6 @@ def test_czt_axis(pb, dt):
     columns, against the long-double transform of the plan vectors the device built"""
     from prysm_b200 import _ops
     capi = _ops.capi
-    chk = Checker()
     for K in czt_Ks(dt):
         N, M = K // 2, K // 2
         plan = _ops.czt_plan(N, M, K, 0.0, 0.37 / N, -1, 0.0, -M / 2 * 0.9, 0.9, TDT[dt], 'cuda')
@@ -926,25 +882,25 @@ def test_czt_axis(pb, dt):
             u = G.ld(a) if axis == 1 else G.ld(a).T
             V = G.fft_ld(G.fft_ld(u * b, K) * H, inverse=True)[:, N - 1:N - 1 + M] * post * LD(0.5) / K
             tr = (lambda z: z) if axis == 1 else (lambda z: z.T)
-            got = chk.run(f'czt/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5), two)
-            chk.add(f'czt/{K}', dt, got, tr(V))
+            got = run(f'czt/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5), two)
+            add(f'czt/{K}', dt, got, tr(V))
             inten = V.real ** 2 + V.imag ** 2
-            got = chk.run(f'czti/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5,
-                                                               out_kind=capi.OUT_INTENSITY), two)
-            chk.add(f'czt_intensity/{K}', dt, got, tr(inten))
+            got = run(f'czti/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5,
+                                                           out_kind=capi.OUT_INTENSITY), two)
+            add(f'czt_intensity/{K}', dt, got, tr(inten))
             acc0 = torch.rand(tuple(tr(inten).shape), generator=torch.Generator(device='cuda').manual_seed(K),
                               device='cuda', dtype=RDT[dt])
-            got = chk.run(f'czta/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5,
-                                                               out_kind=capi.OUT_ACCUMULATE, weight=WEIGHT,
-                                                               out=acc0.clone()), two)
-            chk.add(f'czt_accumulate/{K}', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * tr(inten))
+            got = run(f'czta/{K}', lambda: _ops.czt_axis(dev(a), K, axis, bd, Hd, postd, N - 1, M, 0.5,
+                                                           out_kind=capi.OUT_ACCUMULATE, weight=WEIGHT,
+                                                           out=acc0.clone()), two)
+            add(f'czt_accumulate/{K}', dt, got, G.ld(acc0.cpu().numpy()) + WEIGHT * tr(inten))
             g = crand((nl, M) if axis == 1 else (M, nl), K + 5 + axis, dt)
             w = G.ld(g) if axis == 1 else G.ld(g).T
             V = G.fft_ld(G.fft_ld(w * np.conj(post), K) * Hadj, inverse=True)[:, :N] * np.conj(b) / K
-            got = chk.run(f'czt_adj/{K}', lambda: _ops.czt_axis(dev(g), K, axis, postd, Hadjd, bd, 0, N, 1.0,
-                                                                  pre_conj=True, post_conj=True), two)
-            chk.add(f'czt_adjoint/{K}', dt, got, tr(V))
-    chk.done()
+            got = run(f'czt_adj/{K}', lambda: _ops.czt_axis(dev(g), K, axis, postd, Hadjd, bd, 0, N, 1.0,
+                                                              pre_conj=True, post_conj=True), two)
+            add(f'czt_adjoint/{K}', dt, got, tr(V))
+    LEDGER.done()
 
 
 # ---- angular spectrum ------------------------------------------------------------------------------------------------
@@ -957,7 +913,6 @@ def test_angular_spectrum(pb, dt):
     """the full transfer-function matrix (post_mat) and the separable vectors (post_e, post_b), plain and conjugated,
     with and without a phase screen, cropped and not"""
     from prysm_b200 import _ops
-    chk = Checker()
     for n, k in AS_CASES[dt]:
         ty, tx = _ops.angular_spectrum_vectors(k, 0.6328, 0.01, 25.0, TDT[dt], 'cuda')
         T = np.outer(G.ld(ty.cpu().numpy()), G.ld(tx.cpu().numpy()))
@@ -977,15 +932,15 @@ def test_angular_spectrum(pb, dt):
             y0, x0 = -(-(k[0] - cr[0]) // 2), -(-(k[1] - cr[1]) // 2)
             return out[y0:y0 + cr[0], x0:x0 + cr[1]]
         for conj in (False, True):
-            got = chk.run('as_vec', lambda: _ops.angular_spectrum(x, k, ty=ty, tx=tx, conj_tf=conj), launches)
-            chk.add(f'as_vectors/{k[0]}x{k[1]}', dt, got, ref(G.ld(a), T, conj, None))
-            got = chk.run('as_mat', lambda: _ops.angular_spectrum(x, k, tf=dev(tf), conj_tf=conj, crop=crop), launches)
-            chk.add(f'as_matrix/{k[0]}x{k[1]}', dt, got, ref(G.ld(a), G.ld(tf), conj, crop))
-            got = chk.run('as_screen', lambda: _ops.angular_spectrum(x, k, ty=ty, tx=tx, screen=sd, conj_screen=conj),
-                          launches)
+            got = run('as_vec', lambda: _ops.angular_spectrum(x, k, ty=ty, tx=tx, conj_tf=conj), launches)
+            add(f'as_vectors/{k[0]}x{k[1]}', dt, got, ref(G.ld(a), T, conj, None))
+            got = run('as_mat', lambda: _ops.angular_spectrum(x, k, tf=dev(tf), conj_tf=conj, crop=crop), launches)
+            add(f'as_matrix/{k[0]}x{k[1]}', dt, got, ref(G.ld(a), G.ld(tf), conj, crop))
+            got = run('as_screen', lambda: _ops.angular_spectrum(x, k, ty=ty, tx=tx, screen=sd, conj_screen=conj),
+                      launches)
             sc = np.conj(G.ld(s)) if conj else G.ld(s)
-            chk.add(f'as_screen/{k[0]}x{k[1]}', dt, got, ref(G.ld(a) * sc, T, False, None))
-    chk.done()
+            add(f'as_screen/{k[0]}x{k[1]}', dt, got, ref(G.ld(a) * sc, T, False, None))
+    LEDGER.done()
 
 
 def _pad(a, k):
@@ -1081,12 +1036,11 @@ def test_polychromatic_psf_czt(pb):
         ref += np.longdouble(wt) * (out.real ** 2 + out.imag ** 2)
     K = 256                                       # next_fast_len(N + M - 1), one plan per wavelength for both axes
     per_wvl = {(K, dt, 0): 3, (K, dt, 1): 2}      # H = FFT_K(h), then a CZT axis of two passes each way
-    chk = Checker()
-    got = chk.run('polychromatic_czt', lambda: pb.polychromatic.polychromatic_psf(
+    got = run('polychromatic_czt', lambda: pb.polychromatic.polychromatic_psf(
         dev(amp), dev(opd), wvls, wts, dx, efl, fdx, M, kind='czt', shard=False),
         {k: v * len(wvls) for k, v in per_wvl.items()}, others=2 * len(wvls))   # the plan and phase-screen kernels
-    chk.add('polychromatic_psf_czt/128_64', dt, got, ref)
-    chk.done()
+    add('polychromatic_psf_czt/128_64', dt, got, ref)
+    LEDGER.done()
 
 
 # ---- the shared-memory edge ----------------------------------------------------------------------------------------
@@ -1099,11 +1053,10 @@ def test_shared_memory_edge(pb, dt, axis):
     from prysm_b200 import _ops
     cols = int(axis == 0)
     lmax = G.max_pow2_len(dt)
-    chk = Checker()
     for n in (lmax, lmax // 2 - 1):
         a = crand((3, n) if axis == 1 else (n, 3), n + 9, dt)
-        got = chk.run(f'edge/{n}', lambda: _ops.fft1(dev(a), axis=axis), G.axis_launches(n, dt, cols))
-        chk.add(f'edge_accepted_{ROWS_COLS[cols]}/{n}', dt, got, G.fft_ld(a, axis=axis))
+        got = run(f'edge/{n}', lambda: _ops.fft1(dev(a), axis=axis), G.axis_launches(n, dt, cols))
+        add(f'edge_accepted_{ROWS_COLS[cols]}/{n}', dt, got, G.fft_ld(a, axis=axis))
     for n in (2 * lmax, lmax // 2 + 1):
         assert not G.accepts(n, dt)
         a = dev(crand((3, n) if axis == 1 else (n, 3), n, dt))
@@ -1117,9 +1070,9 @@ def test_shared_memory_edge(pb, dt, axis):
         torch.cuda.synchronize()
         assert torch.equal(out.view(RDT[dt]), before.view(RDT[dt])), 'a refused call wrote to `out`'
         b = crand((3, 1000) if axis == 1 else (1000, 3), 3, dt)
-        got = chk.run('after_refusal', lambda: _ops.fft1(dev(b), axis=axis), G.axis_launches(1000, dt, cols))
-        chk.add(f'after_refusal_{ROWS_COLS[cols]}/1000', dt, got, G.fft_ld(b, axis=axis))
-    chk.done()
+        got = run('after_refusal', lambda: _ops.fft1(dev(b), axis=axis), G.axis_launches(1000, dt, cols))
+        add(f'after_refusal_{ROWS_COLS[cols]}/1000', dt, got, G.fft_ld(b, axis=axis))
+    LEDGER.done()
 
 
 def _whole_module_selected(session):
@@ -1143,3 +1096,10 @@ def test_zz_every_reachable_length_was_hit(pb, request):
     want = {(L, dt, cols) for dt in DTYPES for L in pow2_lengths(dt) for cols in (0, 1)}
     assert not want - HIT, sorted(want - HIT)
     assert not HIT - want, sorted(HIT - want)
+
+
+def test_zz_every_figure_has_a_measurement():
+    """a figure this session reached that has no MEASURED entry is held to the bare ceiling, a bound nobody measured"""
+    if os.environ.get('PB_TEST_MEASUREMENTS'):
+        pytest.skip('recording figures')
+    assert not LEDGER.missing(), f'no MEASURED entry (record them with PB_TEST_MEASUREMENTS): {LEDGER.missing()}'

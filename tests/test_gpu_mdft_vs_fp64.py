@@ -43,8 +43,9 @@ import torch
 
 import prysm_oracle as O
 import test_host_mdft_routes as R
+from accuracy import Ledger, rel_l2
 from conftest import ROOT, rel_linf, within
-from gpu_fixtures import pb, host  # noqa: F401
+from gpu_fixtures import pb, crand, host, routes_of, sm_count  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -407,18 +408,9 @@ MEASURED = {
 }
 
 
-def bound(name):
-    """1.5x the measured figure (at most 1e-6 for complex64); a figure measured as exact stays exact"""
-    case, metric = name.rsplit('/', 1)
-    m = MEASURED.get(case, {}).get(metric)
-    if m is None:
-        return NORTH_STAR
-    cap = float('inf') if '/c128' in case else NORTH_STAR
-    return min(1.5 * m, cap) if m > 0 else float(np.nextafter(0.0, 1.0))
-
-
-def rel_l2(a, b):
-    return float(np.linalg.norm((a - b).ravel()) / np.linalg.norm(b.ravel()))
+# a case's figure is the worst over its inputs, within its test.  The cap of 1e-6 is for complex64: every complex128
+# figure is a few 1e-15, so it never binds there, and holds a complex128 figure with no entry to 1e-6 as well.
+LEDGER = Ledger(MEASURED, NORTH_STAR, per_test=True)
 
 
 def worst_tile(got, ref):
@@ -432,37 +424,14 @@ def worst_tile(got, ref):
     return int(i), int(j), float(t[i, j]) / max(float(np.abs(ref).max()), 1e-300)
 
 
-class Checker:
-    """Compares whole arrays with their references; a case's figure is the worst over its inputs.  `done()` records every
-    figure with conftest.within and fails with all that are over their bounds, each with its worst tile."""
-
-    def __init__(self):
-        self.worst = {}
-        self.routes = []
-
-    def route(self, ok, msg):
-        if not ok:
-            self.routes.append(msg)
-
-    def add(self, case, got, ref, note=None, what=''):
-        figs = {'linf': rel_linf(got, ref), 'l2': rel_l2(got, ref)}
-        for k, v in figs.items():
-            name = f'{case}{SUFFIX}/{k}'
-            if name not in self.worst or v > self.worst[name][0]:
-                i, j, tv = worst_tile(got, ref)
-                detail = f'{what}: worst 128 x 128 output tile ({i}, {j}) at {tv:.3e}'
-                if note is not None:
-                    detail += '; ' + note(i, j)
-                self.worst[name] = (v, detail)
-
-    def done(self):
-        bad = []
-        for name, (v, detail) in self.worst.items():
-            try:
-                within(name, v, bound(name))
-            except AssertionError as e:
-                bad.append(f'{e} ({detail})')
-        assert not bad + self.routes, '\n'.join(bad + self.routes)
+def add(case, got, ref, note=None, what=''):
+    """the whole array against its reference: rel_linf and the relative L2 error, each noted with its worst tile"""
+    i, j, tv = worst_tile(got, ref)
+    detail = f'{what}: worst 128 x 128 output tile ({i}, {j}) at {tv:.3e}'
+    if note is not None:
+        detail += '; ' + note(i, j)
+    for k, v in (('linf', rel_linf(got, ref)), ('l2', rel_l2(got, ref))):
+        LEDGER.record(f'{case}{SUFFIX}/{k}', v, detail)
 
 
 # ---- which kernels ran --------------------------------------------------------------------------------------------
@@ -470,38 +439,13 @@ HIT = set()     # ('tc', stage, form, pieces), ('reduce', pieces), ('cgemm', dty
 ROUTE_KEYS = ([R.route_code(R.ROUTE_MDFT_TC, L, f) for L in (1, 2, 4, 8) for f in range(8)]
               + [R.route_code(R.ROUTE_MDFT_REDUCE, L) for L in (1, 2, 4, 8)]
               + [R.cgemm_code(d, a, b) for d in (0, 1) for a in range(4) for b in range(4)])
-
-
-def _handle():
-    from prysm_b200 import _capi
-    return _capi.handle_for(torch.cuda.current_device(), torch.cuda.current_stream().cuda_stream)
-
-
-def route_counts():
-    h = _handle()
-    out = {k: h.route_launch_count(k) for k in ROUTE_KEYS}
-    out['all'] = h.launch_count()
-    return out
-
-
-def routes_of(fn):
-    """fn()'s result and the launches it made, per route (only the routes it used)"""
-    torch.cuda.synchronize()
-    c0 = route_counts()
-    res = fn()
-    torch.cuda.synchronize()
-    c1 = route_counts()
-    return res, {k: c1[k] - c0[k] for k in c0 if c1[k] != c0[k]}
+ROUTE_CODES = {k: k for k in ROUTE_KEYS}      # routes_of's {key: route code}: each route is its own key
 
 
 def expect(launches):
     want = dict(launches)
     want['all'] = sum(launches.values())
     return want
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
 def record_hits(pred, dtype=0, adjoint=False):
@@ -526,11 +470,6 @@ def precision_32(pb):
     if CHILD and path:
         with open(path, 'w') as fh:
             json.dump(sorted(HIT, key=str), fh)
-
-
-def crand(shape, seed, dtype=np.complex64):
-    rng = np.random.default_rng(seed)
-    return (rng.standard_normal(shape) + 1j * rng.standard_normal(shape)).astype(dtype)
 
 
 _PUPIL = {}
@@ -631,33 +570,33 @@ def test_executor_vs_fp64(pb, shape, sign, direction):
     note = stage_note(pred, shape, adjoint, sms)
     fn_of = (lambda a: (lambda: ex.adjoint(a))) if adjoint else (lambda a: (lambda: ex(a)))
     base = f'mdft/{shape_id(shape)}/{direction}'
-    chk = Checker()
 
     def run(inp, what):
         a = torch.from_numpy(inp).cuda()
-        got, used = routes_of(fn_of(a))
-        chk.route(used == expect(pred[2]), f'{base}/{what}: launches per route {used}, predicted {expect(pred[2])}')
+        got, used = routes_of(fn_of(a), ROUTE_CODES)
+        LEDGER.route(used == expect(pred[2]), f'{base}/{what}: launches per route {used}, predicted {expect(pred[2])}')
         g = host(got)
         if streamk:
-            chk.route(np.array_equal(host(fn_of(a)()), g), f'{base}/{what}: stream-K result differs between two applies')
+            LEDGER.route(np.array_equal(host(fn_of(a)()), g), f'{base}/{what}: stream-K result differs between two applies')
         return g
 
-    inputs = {'gauss': crand((rows, cols), sum(shape) + 17 * (sign + 1)), 'ones': np.ones((rows, cols), np.complex64)}
+    inputs = {'gauss': crand((rows, cols), sum(shape) + 17 * (sign + 1), np.complex64),
+              'ones': np.ones((rows, cols), np.complex64)}
     if max(rows, cols) <= 4096:
         inputs['pupil'] = pupil(rows, cols)
     for name, inp in inputs.items():
         g = run(inp, f'{name}, sign {sign:+d}')
         a128 = inp.astype(np.complex128)
-        chk.add(f'{base}/{name}/gemm', g, gemm_ref(Ey, Ex, inp, adjoint), note, f'{name}, sign {sign:+d}')
-        chk.add(f'{base}/{name}/e2e', g, (ref_ex.adjoint if adjoint else ref_ex)(a128), note, f'{name}, sign {sign:+d}')
+        add(f'{base}/{name}/gemm', g, gemm_ref(Ey, Ex, inp, adjoint), note, f'{name}, sign {sign:+d}')
+        add(f'{base}/{name}/e2e', g, (ref_ex.adjoint if adjoint else ref_ex)(a128), note, f'{name}, sign {sign:+d}')
     for pname, p in impulse_points(rows, cols).items():
         inp = np.zeros((rows, cols), np.complex64)
         inp[p] = 1.0
         g = run(inp, f'impulse {pname}, sign {sign:+d}')
-        chk.add(f'{base}/impulse/gemm', g, impulse_ref(Ey, Ex, p, adjoint), note, f'impulse {pname}, sign {sign:+d}')
-        chk.add(f'{base}/impulse/e2e', g, impulse_ref(ref_ex.Ey, ref_ex.Ex, p, adjoint), note,
-                f'impulse {pname}, sign {sign:+d}')
-    chk.done()
+        add(f'{base}/impulse/gemm', g, impulse_ref(Ey, Ex, p, adjoint), note, f'impulse {pname}, sign {sign:+d}')
+        add(f'{base}/impulse/e2e', g, impulse_ref(ref_ex.Ey, ref_ex.Ex, p, adjoint), note,
+            f'impulse {pname}, sign {sign:+d}')
+    LEDGER.done()
     record_hits(pred, 0, adjoint)
 
 
@@ -676,13 +615,9 @@ def test_switch_settings_in_child(pb, streamk, tmp_path):
     assert r.returncode == 0, f'child run under PB_MDFT_STREAMK={streamk} failed:\n{r.stdout[-6000:]}\n{r.stderr[-3000:]}'
     figures = json.loads(mfile.read_text())
     assert figures, 'the child run recorded no figures'
-    bad = []
     for name, d in sorted(figures.items()):
-        try:
-            within(name, d['measured'], bound(name))
-        except AssertionError as e:
-            bad.append(str(e))
-    assert not bad, '\n'.join(bad)
+        LEDGER.record(name, d['measured'])
+    LEDGER.done()
     HIT.update(tuple(h) for h in json.loads(hfile.read_text()))
 
 
@@ -695,17 +630,16 @@ def test_out_into_plane_of_a_stack(pb):
     x, y, fx, fy = geometry(shape)
     ex = pb.fttools.MDFT(x, y, fx, fy, -1, NORM)
     ref = O.MDFT(x, y, fx, fy, -1, NORM)
-    chk = Checker()
     for adjoint, (rows, cols), (orows, ocols) in ((False, (ny, nx), (my, mx)), (True, (my, mx), (ny, nx))):
-        inp = crand((rows, cols), 5 + adjoint)
+        inp = crand((rows, cols), 5 + adjoint, np.complex64)
         stack = torch.full((4, orows, ocols), float('nan'), dtype=torch.complex64, device='cuda')
         a = torch.from_numpy(inp).cuda()
         (ex._adjoint if adjoint else ex._forward)(a, out=stack[2])
         s = host(stack)
         assert np.isnan(np.delete(s, 2, axis=0)).all(), 'a plane other than the output plane was written'
         d = 'adjoint' if adjoint else 'forward'
-        chk.add(f'mdft/{shape_id(shape)}/{d}/out_plane2/e2e', s[2], (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)))
-    chk.done()
+        add(f'mdft/{shape_id(shape)}/{d}/out_plane2/e2e', s[2], (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)))
+    LEDGER.done()
 
 
 def test_misaligned_input(pb, monkeypatch):
@@ -725,20 +659,19 @@ def test_misaligned_input(pb, monkeypatch):
         seen.append((a.data_ptr(), out.data_ptr()))
         return out
     monkeypatch.setattr(_ops, '_tc_aligned', spy)
-    inp = crand((ny, nx), 3)
+    inp = crand((ny, nx), 3, np.complex64)
     flat = torch.empty(ny * nx + 1, dtype=torch.complex64, device='cuda')
     odd = flat[1:].view(ny, nx)
     odd.copy_(torch.from_numpy(inp))
     assert odd.data_ptr() % 16 == 8 and odd.is_contiguous()
-    chk = Checker()
-    chk.add(f'mdft/{shape_id(shape)}/forward/misaligned/e2e', host(ex(odd)), ref(inp.astype(np.complex128)))
+    add(f'mdft/{shape_id(shape)}/forward/misaligned/e2e', host(ex(odd)), ref(inp.astype(np.complex128)))
     (src, used), = seen
     assert src == odd.data_ptr() and used != src and used % 16 == 0, 'the misaligned input was not copied'
     aligned = torch.from_numpy(inp).cuda()
     same = host(ex(aligned))
     assert seen[1] == (aligned.data_ptr(), aligned.data_ptr()), 'an aligned input was copied'
     assert np.array_equal(same, host(ex(odd)))
-    chk.done()
+    LEDGER.done()
 
 
 # ---- the CUDA-core GEMM ---------------------------------------------------------------------------------------------
@@ -760,7 +693,7 @@ def stored_shape(rows, cols, op):
 
 def pb_cgemm(dtype, opA, opB, M, N, K, A, lda, B, ldb, Cm, ldc):
     from prysm_b200 import _capi
-    h = _handle()
+    h = _capi.handle_for(torch.cuda.current_device(), torch.cuda.current_stream().cuda_stream)
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     h.check(_capi.lib.pb_cgemm(h.ptr, dtype, opA, opB, M, N, K, float(ALPHA), C.c_void_p(A.data_ptr()), lda,
                                C.c_void_p(B.data_ptr()), ldb, C.c_void_p(Cm.data_ptr()), ldc, st))
@@ -774,7 +707,6 @@ def test_cgemm_op_pairs(pb, dtype, opA, opB):
     the fold; _ops.cgemm on contiguous operands"""
     from prysm_b200 import _ops
     name, npdt, tdt = DT[dtype]
-    chk = Checker()
     case = f'cgemm/{name}/{opA}{opB}'
     want = expect({R.cgemm_code(dtype, opA, opB): 1})
     for M, N in MN:
@@ -785,21 +717,22 @@ def test_cgemm_op_pairs(pb, dtype, opA, opB):
             Bh = crand((sb[0], ldb), N * 11 + K, npdt)
             A, B = torch.from_numpy(Ah).cuda(), torch.from_numpy(Bh).cuda()
             Cm = torch.full((M, ldc), float('nan'), dtype=tdt, device='cuda')
-            _, used = routes_of(lambda: pb_cgemm(dtype, opA, opB, M, N, K, A, lda, B, ldb, Cm, ldc))
-            chk.route(used == want, f'{case} M={M} N={N} K={K}: launches {used}, want {want}')
+            _, used = routes_of(lambda: pb_cgemm(dtype, opA, opB, M, N, K, A, lda, B, ldb, Cm, ldc), ROUTE_CODES)
+            LEDGER.route(used == want, f'{case} M={M} N={N} K={K}: launches {used}, want {want}')
             got = host(Cm)
             assert np.isnan(got[:, N:]).all(), f'{case} M={M} N={N} K={K}: the padding of C was written'
             a, b = op_host(Ah[:, :sa[1]].astype(np.complex128), opA), op_host(Bh[:, :sb[1]].astype(np.complex128), opB)
             alpha = float(np.float32(ALPHA)) if dtype == 0 else ALPHA
-            chk.add(case, got[:, :N], alpha * (a @ b), what=f'M={M} N={N} K={K}')
+            add(case, got[:, :N], alpha * (a @ b), what=f'M={M} N={N} K={K}')
     # the tensor-level wrapper: contiguous operands, alpha = 1
     Ah = crand(stored_shape(65, 80, opA), 1, npdt)
     Bh = crand(stored_shape(80, 63, opB), 2, npdt)
-    got, used = routes_of(lambda: _ops.cgemm(torch.from_numpy(Ah).cuda(), torch.from_numpy(Bh).cuda(), opA, opB))
-    chk.route(used == want, f'{case} _ops.cgemm: launches {used}, want {want}')
-    chk.add(case, host(got), op_host(Ah.astype(np.complex128), opA) @ op_host(Bh.astype(np.complex128), opB),
-            what='_ops.cgemm 65 x 63 x 80')
-    chk.done()
+    got, used = routes_of(lambda: _ops.cgemm(torch.from_numpy(Ah).cuda(), torch.from_numpy(Bh).cuda(), opA, opB),
+                          ROUTE_CODES)
+    LEDGER.route(used == want, f'{case} _ops.cgemm: launches {used}, want {want}')
+    add(case, host(got), op_host(Ah.astype(np.complex128), opA) @ op_host(Bh.astype(np.complex128), opB),
+        what='_ops.cgemm 65 x 63 x 80')
+    LEDGER.done()
     HIT.add(('cgemm', dtype, opA, opB))
 
 
@@ -820,7 +753,7 @@ def test_cgemm_c128_against_longdouble(pb):
     def err(c):
         return float((np.sqrt((c.real.astype(ld) - rr) ** 2 + (c.imag.astype(ld) - ri) ** 2)).max() / den)
     d, r = err(got), err(ALPHA * (Ah @ Bh))
-    within('cgemm/c128/longdouble/device/linf', d, bound('cgemm/c128/longdouble/device/linf'))
+    LEDGER.check('cgemm/c128/longdouble/device/linf', d)
     within('cgemm/c128/longdouble/numpy/linf', r, 1e-15)
 
 
@@ -837,18 +770,18 @@ def test_mdft_apply_branches(pb, dtype, adjoint, left_first):
     Ey = _ops.mdft_basis(fy, y, -1, tdt, torch.device('cuda'))
     Ex = _ops.mdft_basis(fx, x, -1, tdt, torch.device('cuda'))
     inp = crand((my, mx) if adjoint else (ny, nx), 9 + adjoint, npdt)
-    got, used = routes_of(lambda: _ops.mdft_apply(Ey, Ex, torch.from_numpy(inp).cuda(), NORM, adjoint, left_first))
+    got, used = routes_of(lambda: _ops.mdft_apply(Ey, Ex, torch.from_numpy(inp).cuda(), NORM, adjoint, left_first),
+                          ROUTE_CODES)
     want = {}
     for a, b in R.cgemm_pairs(adjoint, left_first):
         want[R.cgemm_code(dtype, a, b)] = want.get(R.cgemm_code(dtype, a, b), 0) + 1
-    chk = Checker()
-    chk.route(used == expect(want), f'launches {used}, want {expect(want)}')
+    LEDGER.route(used == expect(want), f'launches {used}, want {expect(want)}')
     case = f'mdft_apply/{name}/{"adjoint" if adjoint else "forward"}/{"left" if left_first else "right"}'
     g = host(got)
     ref = O.MDFT(x, y, fx, fy, -1, NORM)
-    chk.add(f'{case}/gemm', g, gemm_ref(host(Ey), host(Ex), inp, adjoint))
-    chk.add(f'{case}/e2e', g, (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)))
-    chk.done()
+    add(f'{case}/gemm', g, gemm_ref(host(Ey), host(Ex), inp, adjoint))
+    add(f'{case}/e2e', g, (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)))
+    LEDGER.done()
     HIT.add(('branch', dtype, adjoint, left_first))
     HIT.update(('cgemm', dtype, a, b) for a, b in R.cgemm_pairs(adjoint, left_first))
 
@@ -866,16 +799,15 @@ def test_ragged_complex64_executor(pb, direction):
     ref = O.MDFT(x, y, fx, fy, -1, NORM)
     Ey, Ex = host(ex.Ey), host(ex.Ex)
     rows, cols = (my, mx) if adjoint else (ny, nx)
-    chk = Checker()
-    for name, inp in (('gauss', crand((rows, cols), 23)), ('ones', np.ones((rows, cols), np.complex64))):
+    for name, inp in (('gauss', crand((rows, cols), 23, np.complex64)), ('ones', np.ones((rows, cols), np.complex64))):
         a = torch.from_numpy(inp).cuda()
-        got, used = routes_of(lambda: ex.adjoint(a) if adjoint else ex(a))
-        chk.route(used == expect(pred[2]), f'{name}: launches {used}, predicted {expect(pred[2])}')
+        got, used = routes_of(lambda: ex.adjoint(a) if adjoint else ex(a), ROUTE_CODES)
+        LEDGER.route(used == expect(pred[2]), f'{name}: launches {used}, predicted {expect(pred[2])}')
         g = host(got)
         case = f'mdft/{shape_id(shape)}/{direction}/{name}'
-        chk.add(f'{case}/gemm', g, gemm_ref(Ey, Ex, inp, adjoint), what=name)
-        chk.add(f'{case}/e2e', g, (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)), what=name)
-    chk.done()
+        add(f'{case}/gemm', g, gemm_ref(Ey, Ex, inp, adjoint), what=name)
+        add(f'{case}/e2e', g, (ref.adjoint if adjoint else ref)(inp.astype(np.complex128)), what=name)
+    LEDGER.done()
     record_hits(pred, 0, adjoint)
 
 
@@ -911,3 +843,10 @@ def test_every_route_was_checked(pb):
     need |= {('branch', d, adj, lf) for d in (0, 1) for adj in (False, True) for lf in (False, True)}
     missing = sorted(need - HIT, key=str)
     assert not missing, f'not run by an fp64-checked case: {missing}'
+
+
+def test_zz_every_figure_has_a_measurement():
+    """a figure this session reached that has no MEASURED entry is held to the bare ceiling, a bound nobody measured"""
+    if os.environ.get('PB_TEST_MEASUREMENTS'):
+        pytest.skip('recording figures')
+    assert not LEDGER.missing(), f'no MEASURED entry (record them with PB_TEST_MEASUREMENTS): {LEDGER.missing()}'

@@ -19,14 +19,15 @@ for float32 storage (the fp64 result rounded once), M the recurrence's majorant 
 poly_reference.CEIL, which tests/test_host_poly_reference.py shows every modelled defect exceeds by 10x or more.
 """
 import contextlib
+import os
 
 import numpy as np
 import pytest
 import torch
 
 import poly_reference as R
-from conftest import within
-from gpu_fixtures import pb  # noqa: F401
+from accuracy import Ledger
+from gpu_fixtures import pb, sm_count  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -103,16 +104,11 @@ MEASURED = {
     'zernike_sum_der_xy/noll20': 0.178,
 }
 
-FIGS = {}
-
-
-def check(name, value):
-    """a float32 figure is the error beyond the one rounding of the fp64 result, so it is held to the fp64 figure of
-    the same name: the kernels run the same fp64 arithmetic at both storage dtypes"""
-    FIGS[name] = max(float(value), FIGS.get(name, 0.0))
-    m = MEASURED.get(name.split('/', 1)[1])
-    bound = R.CEIL if m is None else (min(1.5 * m, R.CEIL) if m > 0 else float(np.nextafter(0.0, 1.0)))
-    within(name, FIGS[name], bound)
+# the worst figure of each name over the whole file.  A float32 figure is the error beyond the one rounding of the fp64
+# result, so it is held to the fp64 figure of the same name: the kernels run the same fp64 arithmetic at both storage
+# dtypes.
+LEDGER = Ledger(MEASURED, R.CEIL, key=lambda name: name.split('/', 1)[1])
+check = LEDGER.check
 
 
 class _NanTorch:
@@ -167,10 +163,6 @@ def dev(a, prec):
 
 def host(t):
     return t.detach().cpu().numpy().astype(np.float64)
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def family_params(fam):
@@ -540,3 +532,10 @@ def test_tensor_sum(pb, prec, separable, basis):
     assert R.tsum_refused([m for m, _ in over], [n for _, n in over])
     xd, yd = dev(xs, prec), dev(xs, prec)
     refused(pb, lambda: pb._ops.tensor_sum(bc, [1.0, 1.0], [40, 0], [0, 24], xd, yd, (xs.size,), False, False))
+
+
+def test_zz_every_figure_has_a_measurement():
+    """a figure this session reached that has no MEASURED entry is held to the bare ceiling, a bound nobody measured"""
+    if os.environ.get('PB_TEST_MEASUREMENTS'):
+        pytest.skip('recording figures')
+    assert not LEDGER.missing(), f'no MEASURED entry (record them with PB_TEST_MEASUREMENTS): {LEDGER.missing()}'

@@ -31,8 +31,9 @@ import pytest
 import torch
 
 import streaming_reference as S
-from conftest import within
-from gpu_fixtures import pb  # noqa: F401
+from accuracy import Ledger
+from gpu_fixtures import pb, dev, host, launches, sm_count  # noqa: F401
+from gpu_fixtures import crand as _crand
 from streaming_reference import PB_C64, PB_C128, CEIL_ELEM, CEIL_RED, CEIL_EE
 
 pytestmark = pytest.mark.gpu
@@ -150,8 +151,6 @@ MEASURED = {
     'c64/weighted_sum': 2.75e-07,
 }
 
-FIGS = {}
-
 # figures that move from run to run: the fp64 partial sums of these reductions meet in atomicAdd in whatever order the
 # blocks finish (the pack, product and conv figures through the balance scale, the seed centres through S).  Their
 # MEASURED entry is the largest of the recorded runs and their bound 3x it.
@@ -159,49 +158,33 @@ ATOMIC_ORDER = {'dot', 'dot_w', 'mode_projection', 'mode_projection_c', 'moments
                 'pack', 'packed_product', 'conv', 'otf_seed_1_centre', 'otf_seed_2_centre', 'otf_seed_4_centre'}
 
 
-def check(name, value, ceiling):
-    """record the largest figure of `name` seen so far with conftest.within against 1.5x its MEASURED value (3x for
-    the ATOMIC_ORDER figures), never above the ceiling"""
-    FIGS[name] = max(float(value), FIGS.get(name, 0.0))
-    m = MEASURED.get(name)
-    factor = 3.0 if name.split('/', 1)[1] in ATOMIC_ORDER else 1.5
-    bound = ceiling if m is None else (min(factor * m, ceiling) if m > 0 else float(np.nextafter(0.0, 1.0)))
-    within(name, FIGS[name], bound)
+REDUCTIONS = {'dot', 'dot_w', 'mode_projection', 'mode_projection_c', 'moments', 'balance_scale'}
+
+
+def ceiling(name):
+    dn, fig = name.split('/', 1)
+    if fig == 'encircled_energy':
+        return CEIL_EE
+    return CEIL_RED if fig in REDUCTIONS else CEIL_ELEM[PB_C64 if dn == DN[PB_C64] else PB_C128]
+
+
+# the largest figure of each name over the whole file, against 1.5x its MEASURED value (3x for the ATOMIC_ORDER
+# figures), never above the ceiling
+LEDGER = Ledger(MEASURED, ceiling, lambda name: 3.0 if name.split('/', 1)[1] in ATOMIC_ORDER else 1.5)
+check = LEDGER.check
 
 
 # ---- helpers ----------------------------------------------------------------------------------------------------------
-def sm():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
 def shape_of(name):
-    return S.shapes(sm())[name]
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def host(t):
-    return t.detach().cpu().numpy()
+    return S.shapes(sm_count())[name]
 
 
 def crand(shape, seed, dt, scale=1.0):
-    rng = np.random.default_rng(seed)
-    return ((rng.standard_normal(shape) + 1j * rng.standard_normal(shape)) * scale).astype(S.CDT[dt])
+    return _crand(shape, seed, S.CDT[dt], scale)
 
 
 def rand(shape, seed, dt, scale=1.0):
     return (np.random.default_rng(seed).standard_normal(shape) * scale).astype(S.RDT[dt])
-
-
-def launches(pb, fn):
-    """fn()'s result and the kernels it launched"""
-    torch.cuda.synchronize()
-    c0 = pb._ops.launch_count()
-    res = fn()
-    torch.cuda.synchronize()
-    return res, pb._ops.launch_count() - c0
 
 
 def wrap(a):
@@ -220,7 +203,7 @@ def test_dot(pb, dt, shape, weighted):
     got, n = launches(pb, lambda: pb._ops.dot(dev(a), dev(b), None if w is None else dev(w)))
     ref, cond = S.dot_ref(a, b, w)
     assert n == 1
-    check(f'{DN[dt]}/dot{"_w" if weighted else ""}', S.red_fig(got, ref, cond), CEIL_RED)
+    check(f'{DN[dt]}/dot{"_w" if weighted else ""}', S.red_fig(got, ref, cond))
 
 
 @pytest.mark.parametrize('cplx', (False, True))
@@ -228,16 +211,16 @@ def test_dot(pb, dt, shape, weighted):
 @pytest.mark.parametrize('dt', DTS)
 def test_mode_projection(pb, dt, k, cplx):
     """k = 1 and 64 take many blocks per mode; sm*4+1 modes leave one block to read a whole mode"""
-    k = sm() * 4 + 1 if k == 'sm*4+1' else int(k)
+    k = sm_count() * 4 + 1 if k == 'sm*4+1' else int(k)
     sh = (255, 383)
     modes = rand((k,) + sh, 4, dt)
     bar = crand(sh, 5, dt) if cplx else rand(sh, 5, dt)
     got, n = launches(pb, lambda: pb._ops.mode_projection(dev(modes), dev(bar)))
     ref, cond = S.mode_projection_ref(modes, bar)
     assert n == 1 and got.shape == (k,)
-    if k == sm() * 4 + 1:
-        assert S.mode_projection_gx(sh[0] * sh[1], k, sm()) == 1
-    check(f'{DN[dt]}/mode_projection{"_c" if cplx else ""}', S.red_fig(got, ref, cond), CEIL_RED)
+    if k == sm_count() * 4 + 1:
+        assert S.mode_projection_gx(sh[0] * sh[1], k, sm_count()) == 1
+    check(f'{DN[dt]}/mode_projection{"_c" if cplx else ""}', S.red_fig(got, ref, cond))
 
 
 @pytest.mark.parametrize('shape', S.SHAPE_NAMES)
@@ -248,7 +231,7 @@ def test_moments(pb, dt, shape):
     got, n = launches(pb, lambda: pb._ops.moments(dev(d)))
     ref, cond = S.moments_ref(d)
     assert n == 1
-    check(f'{DN[dt]}/moments', S.red_fig(np.array(got), ref, cond), CEIL_RED)
+    check(f'{DN[dt]}/moments', S.red_fig(np.array(got), ref, cond))
 
 
 @pytest.mark.parametrize('nr', (1, 40))
@@ -262,7 +245,7 @@ def test_encircled_energy(pb, dt, shape, nr):
     got, n = launches(pb, lambda: pb._ops.encircled_energy(dev(mtf), df, radii))
     ref, cond = S.ee_ref(mtf, df, radii)
     assert n == 1
-    check(f'{DN[dt]}/encircled_energy', S.red_fig(got, ref, cond), CEIL_EE)
+    check(f'{DN[dt]}/encircled_energy', S.red_fig(got, ref, cond))
 
 
 @pytest.mark.parametrize('shape', SMALL + ('red+1', 'elem+1', '2048sq'))
@@ -274,7 +257,7 @@ def test_balance_scale(pb, dt, shape):
     ref, (sa, sb) = S.balance_ref(a, b)
     assert n == 2
     # s = sqrt(sa / sb): its relative error is half the sum of the two sums' relative errors
-    check(f'{DN[dt]}/balance_scale', abs(float(host(got)[0]) - ref) / ref, CEIL_RED)
+    check(f'{DN[dt]}/balance_scale', abs(float(host(got)[0]) - ref) / ref)
 
 
 @pytest.mark.parametrize('dt', DTS)
@@ -314,7 +297,7 @@ def test_otf_normalize(pb, dt, which, shape):
     assert n == 1
     assert [g is not None for g in got] == [bool(which & 1), bool(which & 2), bool(which & 4)]
     for k, v in otf_figures(got, S.otf_normalize_ref(D), which).items():
-        check(f'{DN[dt]}/otf_normalize_{k}', v, CEIL_ELEM[dt])
+        check(f'{DN[dt]}/otf_normalize_{k}', v)
 
 
 @pytest.mark.parametrize('scale', (1e-22, 1.0, 1e21))
@@ -333,7 +316,7 @@ def test_otf_float32_psf_scale(pb, scale):
     assert np.all(np.isfinite(D))
     ref = S.otf_normalize_ref(D)
     for k, v in otf_figures((mtf.data, ptf.data, otf.data), ref, 7).items():
-        check(f'c64/otf_scale_{scale:g}_{k}', v, CEIL_ELEM[PB_C64])
+        check(f'c64/otf_scale_{scale:g}_{k}', v)
 
 
 @pytest.mark.parametrize('shape', ('1x1', '1xn', 'nx1', '31x33', '1023x769', '2048sq', 'red+1', 'elem+1'))
@@ -355,12 +338,12 @@ def test_otf_adjoint_seed(pb, dt, which, shape):
     # off the centre: relative to the largest term (the reduction does not enter)
     off = err.copy()
     off[c] = 0
-    check(f'{DN[dt]}/otf_seed_{which}', float(off.max() / np.abs(main).max()), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/otf_seed_{which}', float(off.max() / np.abs(main).max()))
     # the centre, relative to its first term and to its correction at the reduction's scale sum|terms| (the
     # correction is linear in S, and S is summed in an atomic order that varies from run to run); for a 1 x 1
     # plane the two terms cancel exactly (zero gradient)
     scale = abs(main[c]) + abs(corr) * Scond / max(abs(Sref), np.finfo(np.float64).tiny)
-    check(f'{DN[dt]}/otf_seed_{which}_centre', float(err[c] / scale), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/otf_seed_{which}_centre', float(err[c] / scale))
 
 
 @pytest.mark.parametrize('shape', ('1x1', '31x33', '1023x769', 'elem+1'))
@@ -372,8 +355,7 @@ def test_encircled_energy_adjoint_seed(pb, dt, shape):
     ee_bar = np.random.default_rng(16).standard_normal(40)
     got, n = launches(pb, lambda: pb._ops.encircled_energy_adjoint_seed(sh, df, radii, ee_bar, TR[dt], 'cuda'))
     assert n == 1
-    check(f'{DN[dt]}/ee_adjoint_seed', S.rel_linf(host(got), S.ee_adjoint_seed_ref(sh, df, radii, ee_bar)),
-          CEIL_ELEM[dt])
+    check(f'{DN[dt]}/ee_adjoint_seed', S.rel_linf(host(got), S.ee_adjoint_seed_ref(sh, df, radii, ee_bar)))
 
 
 # ---- elementwise ----------------------------------------------------------------------------------------------------
@@ -396,7 +378,7 @@ def test_mask_multiply_flags(pb, dt, flags, mcplx, with_b, with_w):
                                                        one_minus=one_minus, real_out=real_out, scale=0.7, out=o))
     assert n == 1 and got.is_complex() != real_out
     ref = S.mask_multiply_ref(a, m, b, w, conj, one_minus, real_out, 0.7, out0, rdt=S.RDT[dt])
-    check(f'{DN[dt]}/mask_multiply', S.rel_linf(host(got), ref), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/mask_multiply', S.rel_linf(host(got), ref))
 
 
 @pytest.mark.parametrize('shape', S.SHAPE_NAMES)
@@ -406,7 +388,7 @@ def test_mask_multiply_shapes(pb, dt, shape):
     a, m, w = crand(sh, 22, dt), crand(sh, 23, dt), rand(sh, 24, dt)
     got = pb._ops.mask_multiply(dev(a), dev(m), w=dev(w), conj=True, one_minus=True, scale=2.0)
     check(f'{DN[dt]}/mask_multiply_shapes',
-          S.rel_linf(host(got), S.mask_multiply_ref(a, m, None, w, True, True, False, 2.0)), CEIL_ELEM[dt])
+          S.rel_linf(host(got), S.mask_multiply_ref(a, m, None, w, True, True, False, 2.0)))
 
 
 @pytest.mark.parametrize('mode', (0, 1, 2))
@@ -426,7 +408,7 @@ def test_field_adjoint(pb, dt, shape, mode):
         assert np.all(g.real == 0)
     if mode == 1:
         assert np.all(g.reshape(-1)[::7] == 0)
-    check(f'{DN[dt]}/field_adjoint_{mode}', S.rel_linf(g, ref), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/field_adjoint_{mode}', S.rel_linf(g, ref))
 
 
 @pytest.mark.parametrize('which', ('real', 'imag', 'angle', 'abs'))
@@ -450,7 +432,7 @@ def test_component(pb, dt, shape, which):
         z = flat[:min(4, flat.size)]
         np.testing.assert_array_equal(g.reshape(-1)[:z.size], np.arctan2(z.imag, z.real))
         assert np.array_equal(np.signbit(g.reshape(-1)[:z.size]), np.signbit(np.arctan2(z.imag, z.real)))
-    check(f'{DN[dt]}/component_{which}', S.rel_linf(g, S.component_ref(which, v)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/component_{which}', S.rel_linf(g, S.component_ref(which, v)))
 
 
 @pytest.mark.parametrize('scalar', (False, True))
@@ -468,7 +450,7 @@ def test_binary(pb, dt, shape, op, reverse, scalar):
     # division: relative to each quotient (|a/b| spans decades), everything else: to max|ref|
     g = host(got)
     fig = float(np.max(np.abs(S.ld(g) - ref) / np.abs(ref))) if op == 'truediv' else S.rel_linf(g, ref)
-    check(f'{DN[dt]}/binary_{op}', fig, CEIL_ELEM[dt])
+    check(f'{DN[dt]}/binary_{op}', fig)
 
 
 @pytest.mark.parametrize('scale', ('tiny', 'huge'))
@@ -481,7 +463,7 @@ def test_truediv_range(pb, dt, scale):
     g = host(pb._ops.binary('truediv', dev(a), dev(b)))
     ref = S.binary_ref('truediv', a, b)
     fig = math.inf if not np.all(np.isfinite(g)) else float(np.max(np.abs(S.ld(g) - ref) / np.abs(ref)))
-    check(f'{DN[dt]}/truediv_{scale}', fig, CEIL_ELEM[dt])
+    check(f'{DN[dt]}/truediv_{scale}', fig)
 
 
 @pytest.mark.parametrize('dt', DTS)
@@ -495,7 +477,7 @@ def test_mul_outer_strided(pb, dt):
         got, n = launches(pb, lambda: pb._ops.mul_outer(a, dev(vy), dev(vx), cy, cx, 0.3, out=out))
         assert n == 1 and got.data_ptr() == out.data_ptr()
         ref = S.mul_outer_ref(big[50:250, 20:331], vy, vx, cy, cx, 0.3, rdt=S.RDT[dt])
-        check(f'{DN[dt]}/mul_outer', S.rel_linf(host(out), ref), CEIL_ELEM[dt])
+        check(f'{DN[dt]}/mul_outer', S.rel_linf(host(out), ref))
         ob = host(out_big)
         assert not ob[:5].any() and not ob[205:].any() and not ob[:, :7].any() and not ob[:, 318:].any()
 
@@ -511,7 +493,7 @@ def test_weighted_sum(pb, dt, k):
     ref = S.weighted_sum_ref(modes, w, S.RDT[dt])
     # a k-term sum in R: relative to the sum of the terms' magnitudes at each sample
     cond = np.tensordot(np.abs(S.ld(np.asarray(w).astype(S.RDT[dt]))), np.abs(S.ld(modes)), axes=1)
-    check(f'{DN[dt]}/weighted_sum', float(np.max(np.abs(S.ld(host(got)) - ref) / cond)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/weighted_sum', float(np.max(np.abs(S.ld(host(got)) - ref) / cond)))
 
 
 @pytest.mark.parametrize('charge', (1, 6))
@@ -521,7 +503,7 @@ def test_vortex_phase(pb, dt, charge):
     xf, yf = S.radial_axes_ref(sh, 0.013, 0.0, S.RDT[dt])
     got, n = launches(pb, lambda: pb._ops.vortex_phase(charge, dev(xf), dev(yf)))
     assert n == 1
-    check(f'{DN[dt]}/vortex', S.rel_linf(host(got), S.vortex_ref(charge, xf, yf)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/vortex', S.rel_linf(host(got), S.vortex_ref(charge, xf, yf)))
 
 
 @pytest.mark.parametrize('levels', ('outer', 'middle', 'inner'))
@@ -535,7 +517,7 @@ def test_radial_window(pb, dt, shape, levels):
     assert n == 1
     xr, yr = S.radial_axes_ref(sh, fdx, shift, S.RDT[dt])
     assert np.array_equal(host(xf), xr) and np.array_equal(host(yf), yr)
-    check(f'{DN[dt]}/radial_window', S.rel_linf(host(win), S.radial_window_ref(xr, yr, here, nxt)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/radial_window', S.rel_linf(host(win), S.radial_window_ref(xr, yr, here, nxt)))
 
 
 @pytest.mark.parametrize('dt', DTS)
@@ -562,7 +544,7 @@ def test_resample_bilinear_edges(pb, dt):
         ref = S.resample_ref(cmap, xf, yf, 0.0, 0.0, 1.0, ft if ft is not None else fill)
         assert g[0] == cmap[ny - 1, 0] and g[1] == cmap[0, nx - 1] and g[2] == cmap[hy, hx]
         assert np.array_equal(g[3:9], ref[3:9].astype(g.dtype))           # outside / NaN: the fill, exactly
-        check(f'{DN[dt]}/resample', S.rel_linf(g, ref), CEIL_ELEM[dt])
+        check(f'{DN[dt]}/resample', S.rel_linf(g, ref))
 
 
 @pytest.mark.parametrize('amp', ('none', 'real', 'u8'))
@@ -575,7 +557,7 @@ def test_phase_screen(pb, dt, shape, amp):
     a = {'none': None, 'real': np.abs(rand(sh, 42, dt)), 'u8': (rand(sh, 42, dt) > 0).astype(np.uint8)}[amp]
     got, n = launches(pb, lambda: pb._ops.phase_screen(None if a is None else dev(a), dev(opd), k))
     assert n == 1
-    check(f'{DN[dt]}/phase_screen', S.rel_linf(host(got), S.phase_field_ld(opd, k, a)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/phase_screen', S.rel_linf(host(got), S.phase_field_ld(opd, k, a)))
 
 
 @pytest.mark.parametrize('accumulate', (False, True))
@@ -588,7 +570,7 @@ def test_intensity(pb, dt, shape, accumulate):
     o = None if out0 is None else dev(out0)
     got, n = launches(pb, lambda: pb._ops.intensity(dev(v), 0.75, out=o))
     assert n == 1
-    check(f'{DN[dt]}/intensity', S.rel_linf(host(got), S.intensity_ref(v, 0.75, out0, S.RDT[dt])), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/intensity', S.rel_linf(host(got), S.intensity_ref(v, 0.75, out0, S.RDT[dt])))
 
 
 # ---- image chain ----------------------------------------------------------------------------------------------------
@@ -605,11 +587,11 @@ def test_pack_and_packed_product(pb, dt, shape):
     sv = float(host(s)[0])
     zh = host(zp)
     assert np.array_equal(zh.real, o)
-    check(f'{DN[dt]}/pack', S.rel_linf(zh.imag, S.ld(h) * S.ld(S.RDT[dt](sv))), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/pack', S.rel_linf(zh.imag, S.ld(h) * S.ld(S.RDT[dt](sv))))
     Z = np.asarray(S.ft2_ld(zh), S.CDT[dt])
     got, n = launches(pb, lambda: pb._ops.packed_spectrum_product(dev(Z), 0.5, s))
     assert n == 1
-    check(f'{DN[dt]}/packed_product', S.rel_linf(host(got), S.packed_product_ref(Z, 0.5, sv)), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/packed_product', S.rel_linf(host(got), S.packed_product_ref(Z, 0.5, sv)))
 
 
 @pytest.mark.parametrize('dt', DTS)
@@ -625,7 +607,7 @@ def test_conv_end_to_end(pb, dt):
     got = host(pb.convolution.conv(dev(o), dev(h)))
     import scipy.fft as sfft
     ref = sfft.fftshift(S.conv_ref(sfft.ifftshift(S.ld(o)), sfft.ifftshift(S.ld(h))))
-    check(f'{DN[dt]}/conv', S.rel_linf(got, ref), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/conv', S.rel_linf(got, ref))
 
 
 @pytest.mark.parametrize('f', ((1, 7), (7, 1), (3, 5)))
@@ -637,7 +619,7 @@ def test_bindown_and_tile(pb, dt, f):
         got, n = launches(pb, lambda: pb._ops.bindown(dev(a), fy, fx, mean))
         assert n == 1
         check(f'{DN[dt]}/bindown', S.red_fig(host(got).ravel(), S.bindown_ref(a, fy, fx, mean).ravel(),
-                                             S.bindown_ref(np.abs(a), fy, fx, mean).ravel()), CEIL_ELEM[dt])
+                                             S.bindown_ref(np.abs(a), fy, fx, mean).ravel()))
     small = rand((131, 97), 48, dt)
     got, n = launches(pb, lambda: pb._ops.tile(dev(small), fy, fx, 0.5))
     assert n == 1
@@ -657,7 +639,7 @@ def test_separable_tf(pb, dt, kind):
         if wx == 0 and wy == 0:
             assert np.all(g == 1)
         # sinc zeros: absolute error against the largest value
-        check(f'{DN[dt]}/separable_tf_{kind}', S.rel_linf(g, ref), CEIL_ELEM[dt])
+        check(f'{DN[dt]}/separable_tf_{kind}', S.rel_linf(g, ref))
 
 
 # ---- reverse pass through the public functions ----------------------------------------------------------------------
@@ -681,7 +663,7 @@ def test_otf_from_psf_adjoint(pb, dt, shape, which):
     fn = {1: pb.otf.mtf_from_psf_adjoint, 2: pb.otf.ptf_from_psf_adjoint, 4: pb.otf.otf_from_psf_adjoint}[which]
     got = host(fn(dev(bar), data=data))
     ref = S.transform_psf_adjoint_ld(S.otf_adjoint_seed_ref(which, bar, host(data))[0]).real
-    check(f'{DN[dt]}/psf_adjoint_{which}', S.rel_linf(got, ref), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/psf_adjoint_{which}', S.rel_linf(got, ref))
 
 
 @pytest.mark.parametrize('shape', ((256, 256), (255, 383)))
@@ -698,7 +680,7 @@ def test_encircled_energy_adjoint(pb, dt, shape):
     mtf_bar = host(pb._ops.encircled_energy_adjoint_seed(shape, 1000 / (shape[0] * dx), radii / 1e3, ee_bar, TR[dt],
                                                          'cuda'))
     ref = S.transform_psf_adjoint_ld(S.otf_adjoint_seed_ref(1, mtf_bar, host(data))[0]).real
-    check(f'{DN[dt]}/ee_adjoint', S.rel_linf(got, ref), CEIL_ELEM[dt])
+    check(f'{DN[dt]}/ee_adjoint', S.rel_linf(got, ref))
 
 
 # ---- beyond int32 ---------------------------------------------------------------------------------------------------
@@ -720,8 +702,8 @@ def test_moments_beyond_int32(pb):
 
 
 # ---- bookkeeping ----------------------------------------------------------------------------------------------------
-def test_zz_every_figure_has_a_measurement(pb):
+def test_zz_every_figure_has_a_measurement():
+    """a figure this session reached that has no MEASURED entry is held to the bare ceiling, a bound nobody measured"""
     if os.environ.get('PB_TEST_MEASUREMENTS'):
         pytest.skip('recording figures')
-    missing = sorted(k for k in FIGS if k not in MEASURED)
-    assert not missing, f'figures without a MEASURED entry (record them with PB_TEST_MEASUREMENTS): {missing}'
+    assert not LEDGER.missing(), f'no MEASURED entry (record them with PB_TEST_MEASUREMENTS): {LEDGER.missing()}'

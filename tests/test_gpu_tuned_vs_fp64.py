@@ -49,6 +49,7 @@ outside EXPECTED.  The last test asserts that every instantiation the Python API
 """
 import ctypes as C
 import math
+import os
 
 import numpy as np
 import pytest
@@ -56,8 +57,9 @@ import scipy.fft as sfft
 import torch
 
 import prysm_oracle as O
-from conftest import rel_linf, within
-from gpu_fixtures import pb  # noqa: F401
+from accuracy import Ledger, rel_l2
+from conftest import rel_linf
+from gpu_fixtures import pb, dev, host  # noqa: F401
 from gpu_fixtures import routes_of as _routes_of
 
 pytestmark = pytest.mark.gpu
@@ -244,54 +246,25 @@ MEASURED = {
 }
 
 
-def bound(name):
-    """1.5x the measured figure, at most 1e-6; a result that was exact (the focus of a centred impulse) stays exact"""
-    case, metric = name.rsplit('/', 1)
-    m = MEASURED.get(case, {}).get(metric)
-    if m is None:
-        return NORTH_STAR
-    return min(1.5 * m, NORTH_STAR) if m > 0 else float(np.nextafter(0.0, 1.0))
+# a case's figure is the worst over its fields, within its test; a result that was exact (the focus of a centred
+# impulse) stays exact
+LEDGER = Ledger(MEASURED, NORTH_STAR, per_test=True)
 
 
-def rel_l2(a, b):
-    return float(np.linalg.norm((a - b).ravel()) / np.linalg.norm(b.ravel()))
-
-
-class Checker:
-    """Compares whole arrays with their references; a case's figure is the worst over its fields.  `done()` records every
-    figure with conftest.within and then fails with all that are over their bounds, each under its own name."""
-
-    def __init__(self):
-        self.worst = {}
-        self.routes = []     # cases that did not run the kernels they are about
-
-    def route(self, ok, msg):
-        if not ok:
-            self.routes.append(msg)
-
-    def add(self, case, got, ref, rows=None, field=0):
-        got = got.detach().cpu().numpy() if torch.is_tensor(got) else np.asarray(got)
-        figs = {'linf': rel_linf(got, ref), 'l2': rel_l2(got, ref)}
-        if rows is not None:
-            rowmax = np.abs(got - ref).max(axis=1)
-            den = float(np.abs(ref).max())
-            for c, cname in enumerate(CLASSES):
-                sel = rowmax[rows == c]
-                if sel.size:
-                    figs[cname] = float(sel.max()) / den
-        for k, v in figs.items():
-            name = f'{case}/{k}'
-            if name not in self.worst or v > self.worst[name][0]:
-                self.worst[name] = (v, field)
-
-    def done(self):
-        bad = []
-        for name, (v, field) in self.worst.items():
-            try:
-                within(name, v, bound(name))
-            except AssertionError as e:
-                bad.append(f'{e} (worst field {field})')
-        assert not bad + self.routes, '\n'.join(bad + self.routes)
+def add(case, got, ref, rows=None, field=0):
+    """the whole array against its reference: rel_linf, the relative L2 error and, with `rows`, the figure of each
+    row class"""
+    got = host(got)
+    figs = {'linf': rel_linf(got, ref), 'l2': rel_l2(got, ref)}
+    if rows is not None:
+        rowmax = np.abs(got - ref).max(axis=1)
+        den = float(np.abs(ref).max())
+        for c, cname in enumerate(CLASSES):
+            sel = rowmax[rows == c]
+            if sel.size:
+                figs[cname] = float(sel.max()) / den
+    for k, v in figs.items():
+        LEDGER.record(f'{case}/{k}', v, f'worst field {field}')
 
 
 # ---- which kernels ran --------------------------------------------------------------------------------------------
@@ -324,15 +297,15 @@ def routes_of(fn):
     return _routes_of(fn, route_codes())
 
 
-def run_axis(chk, case, fn, expect):
+def run_axis(case, fn, expect):
     """fn() for its result: every instantiation in `expect` must have run, nothing but the register engine (no generic
     axis pass, no focus pair), and no instantiation outside EXPECTED"""
     res, used = routes_of(fn)
     hits = {k for k in used if isinstance(k, tuple) and k[0] != 'focus'}
     other = sorted(str(k) for k in used if k != 'all' and k not in hits)
-    chk.route(not other, f'{case}: other routes ran: {other}')
-    chk.route(hits <= EXPECTED, f'{case}: unexpected instantiations {sorted(hits - EXPECTED)}')
-    chk.route(set(expect) <= hits, f'{case}: {sorted(set(expect) - hits)} did not run; ran {sorted(hits)}')
+    LEDGER.route(not other, f'{case}: other routes ran: {other}')
+    LEDGER.route(hits <= EXPECTED, f'{case}: unexpected instantiations {sorted(hits - EXPECTED)}')
+    LEDGER.route(set(expect) <= hits, f'{case}: {sorted(set(expect) - hits)} did not run; ran {sorted(hits)}')
     HIT.update(hits)
     return res
 
@@ -438,16 +411,16 @@ def batch_call(ops, src, N, d, nb, in_bs, in_ld, out, kind, *, in_kind=None, amp
     return out
 
 
-def check_focus(chk, case, N, d, fn, refs, nlaunch, nscreen=0):
+def check_focus(case, N, d, fn, refs, nlaunch, nscreen=0):
     """fn() -> (nb, 2N, 2N) output; refs: {field: reference}; nlaunch: the launches of the focus pair of <N, INV> the
     call takes, and it launches nothing else but `nscreen` phase-screen kernels.  Outputs are bounded per row class of the
     tile-major intermediate."""
     got, used = routes_of(fn)
     want = {('focus', N, int(d > 0)): nlaunch, 'all': nlaunch + nscreen}
-    chk.route(used == want, f'{case}: launches per route {used}, the route takes {want}')
+    LEDGER.route(used == want, f'{case}: launches per route {used}, the route takes {want}')
     rows = row_classes(N)
     for b, ref in refs.items():
-        chk.add(case, got[b], ref, rows, b)
+        add(case, got[b], ref, rows, b)
 
 
 # ---- the fused focus pair (tensor-TMA input, one launch pair per field) -------------------------------------------
@@ -467,10 +440,9 @@ def test_v2_stack_every_field(pb, N, d, kind):
                                                                   dtype=torch.complex64 if kind == 'complex' else torch.float32)
         return batch_call(_ops, x, N, d, NSTACK, N * N, N, out, kind)
 
-    chk = Checker()
     refs = {b: derive(gauss_ref(N, b, d), kind, None if acc0h is None else acc0h[b]) for b in range(NSTACK)}
-    check_focus(chk, f'v2/{N}/{d:+d}/{kind}/stack5', N, d, fn, refs, 2 * NSTACK)
-    chk.done()
+    check_focus(f'v2/{N}/{d:+d}/{kind}/stack5', N, d, fn, refs, 2 * NSTACK)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('d', (-1, 1))
@@ -483,10 +455,9 @@ def test_v2_single_overlapping_padded(pb, N, d):
     K = 2 * N
     host = gauss_stack(N)
     x = torch.from_numpy(host).cuda()
-    chk = Checker()
     one = x[0].clone()
     fn = (lambda: (P.focus if d < 0 else P.unfocus)(one, 2)[None])
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/single', N, d, fn, {0: gauss_ref(N, 0, d)}, 2)
+    check_focus(f'v2/{N}/{d:+d}/complex/single', N, d, fn, {0: gauss_ref(N, 0, d)}, 2)
 
     buf = torch.zeros((NSTACK, K, K + N), dtype=torch.complex64, device='cuda')
     src = buf[:, :N, K:]
@@ -496,8 +467,8 @@ def test_v2_single_overlapping_padded(pb, N, d):
         out = buf[:, :, :K]
         batch_call(_ops, src, N, d, NSTACK, src.stride(0), src.stride(1), out, 'complex')
         return out
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/overlapping', N, d, inside,
-                {b: gauss_ref(N, b, d) for b in range(NSTACK)}, 2 * NSTACK)
+    check_focus(f'v2/{N}/{d:+d}/complex/overlapping', N, d, inside,
+           {b: gauss_ref(N, b, d) for b in range(NSTACK)}, 2 * NSTACK)
     assert torch.equal(src, x)
 
     big0 = acc_start((NSTACK, K + 3, K + 6), N + 2)
@@ -511,9 +482,9 @@ def test_v2_single_overlapping_padded(pb, N, d):
         outside[:, 1:K + 1, 2:K + 2] = False
         assert torch.equal(big[outside], big0[outside])      # no store outside the window
         return out
-    check_focus(chk, f'v2/{N}/{d:+d}/accumulate/padded', N, d, padded,
-                {b: derive(gauss_ref(N, b, d), 'accumulate', acc0h[b]) for b in range(NSTACK)}, 2 * NSTACK)
-    chk.done()
+    check_focus(f'v2/{N}/{d:+d}/accumulate/padded', N, d, padded,
+           {b: derive(gauss_ref(N, b, d), 'accumulate', acc0h[b]) for b in range(NSTACK)}, 2 * NSTACK)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('d', (-1, 1))
@@ -522,7 +493,6 @@ def test_v2_impulses(pb, N, d):
     """sums of impulses against their closed form (no FFT in the reference)"""
     from prysm_b200 import _ops
     px = impulse_pixels(N)
-    chk = Checker()
     for name, terms in IMPULSE_SUMS.items():
         a = np.zeros((N, N), dtype=np.complex64)
         for p, v in terms:
@@ -530,8 +500,8 @@ def test_v2_impulses(pb, N, d):
         x = torch.from_numpy(a).cuda()
         ref = impulse_focus(N, 2, [px[p] for p, _ in terms], [v for _, v in terms], inverse=d > 0)
         fn = (lambda: _ops.fft2(x, (2 * N, 2 * N), dir=d, scale=0.5 / N, shift_in=True, shift_out=True)[None])
-        check_focus(chk, f'v2/{N}/{d:+d}/complex/impulse_{name}', N, d, fn, {0: ref}, 2)
-    chk.done()
+        check_focus(f'v2/{N}/{d:+d}/complex/impulse_{name}', N, d, fn, {0: ref}, 2)
+    LEDGER.done()
 
 
 # ---- the fused focus pair, staged inputs (tensor TMA cannot gather them: staged field by field) ------------------------
@@ -546,15 +516,14 @@ def test_staged_misaligned_base_every_output_kind(pb, N, d):
     src.copy_(torch.from_numpy(gauss_stack(N)[0]))
     assert src.data_ptr() % 16 == 8
     acc0 = acc_start((K, K), N + 3)
-    chk = Checker()
     for kind in KINDS:
         def fn():
             out = acc0.clone() if kind == 'accumulate' else None
             return _ops.fft2(src, (K, K), dir=d, scale=1.0 / K, shift_in=True, shift_out=True,
                              out_kind=out_kind(_ops.capi, kind), weight=WEIGHT, out=out)[None]
         ref = derive(gauss_ref(N, 0, d), kind, acc0.cpu().numpy())
-        check_focus(chk, f'v2/{N}/{d:+d}/{kind}/staged_misaligned', N, d, fn, {0: ref}, 2)
-    chk.done()
+        check_focus(f'v2/{N}/{d:+d}/{kind}/staged_misaligned', N, d, fn, {0: ref}, 2)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('d', (-1, 1))
@@ -565,14 +534,13 @@ def test_staged_odd_pitches(pb, N, d):
     from prysm_b200 import _ops
     K = 2 * N
     host = gauss_stack(N)
-    chk = Checker()
     buf = torch.zeros((N, N + 1), dtype=torch.complex64, device='cuda')
     buf[:, :N] = torch.from_numpy(host[0])
 
     def odd_ld():
         out = torch.empty((1, K, K), dtype=torch.complex64, device='cuda')
         return batch_call(_ops, buf, N, d, 1, 0, N + 1, out, 'complex')
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/staged_odd_in_ld', N, d, odd_ld, {0: gauss_ref(N, 0, d)}, 2)
+    check_focus(f'v2/{N}/{d:+d}/complex/staged_odd_in_ld', N, d, odd_ld, {0: gauss_ref(N, 0, d)}, 2)
 
     order = (0, 1, 2, 3, 4, 4, 3, 2, 1)
     bs = N * N + 1
@@ -584,9 +552,9 @@ def test_staged_odd_pitches(pb, N, d):
         out = torch.empty((9, K, K), dtype=torch.complex64, device='cuda')
         return batch_call(_ops, src, N, d, 9, bs, N, out, 'complex')
     fields = range(9) if N < 2048 else (0, 4, 7, 8)
-    check_focus(chk, f'v2/{N}/{d:+d}/complex/staged_odd_in_bs_batch9', N, d, odd_bs,
-                {b: gauss_ref(N, order[b], d) for b in fields}, 18)
-    chk.done()
+    check_focus(f'v2/{N}/{d:+d}/complex/staged_odd_in_bs_batch9', N, d, odd_bs,
+           {b: gauss_ref(N, order[b], d) for b in fields}, 18)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('N', (512, 2048))
@@ -595,21 +563,20 @@ def test_staged_phase_screen_input(pb, N):
     OPD of ~1e4 nm (many waves: the fp64 phase range reduction); per-field real amplitudes, |.|^2 accumulated"""
     from prysm_b200 import _ops
     K = 2 * N
-    chk = Checker()
     fields = range(9) if N < 2048 else (0, 7, 8)
     opd_s, mask, _ = opd_stack(N, 9, 30.0)
     opd = torch.from_numpy(opd_s).cuda()
     fn = (lambda: _ops.fft2(None, (K, K), dir=1, scale=1.0 / K, shift_in=True, shift_out=True, opd=opd[0],
                             kscale=KSCALE)[None])
-    check_focus(chk, f'v2/{N}/+1/complex/staged_opd30_amp_none', N, 1, fn, {0: opd_ref(N, 9, 30.0, 'none', 0, 1)}, 2, 1)
+    check_focus(f'v2/{N}/+1/complex/staged_opd30_amp_none', N, 1, fn, {0: opd_ref(N, 9, 30.0, 'none', 0, 1)}, 2, 1)
 
     opd_l, mask_l, _ = opd_stack(N, 9, 1e4)
     opdl = torch.from_numpy(opd_l).cuda()
     m = torch.from_numpy(mask_l).cuda()
     fn = (lambda: _ops.fft2_batch(None, (K, K), dir=-1, scale=1.0 / K, shift_in=True, shift_out=True, amp=m, opd=opdl,
                                   kscale=KSCALE))
-    check_focus(chk, f'v2/{N}/-1/complex/staged_opd1e4_amp_u8_shared_batch9', N, -1, fn,
-                {b: opd_ref(N, 9, 1e4, 'mask', b, -1) for b in fields}, 18, 9)
+    check_focus(f'v2/{N}/-1/complex/staged_opd1e4_amp_u8_shared_batch9', N, -1, fn,
+           {b: opd_ref(N, 9, 1e4, 'mask', b, -1) for b in fields}, 18, 9)
 
     _, _, amps_s = opd_stack(N, 9, 30.0)
     amps = torch.from_numpy(amps_s).cuda()
@@ -620,9 +587,9 @@ def test_staged_phase_screen_input(pb, N):
         out = acc0.clone()
         return batch_call(_ops, opd, N, -1, 9, N * N, N, out, 'accumulate', in_kind=_ops.capi.IN_AMP_OPD, amp=amps,
                           amp_kind=_ops.capi.AMP_REAL, amp_bs=N * N)
-    check_focus(chk, f'v2/{N}/-1/accumulate/staged_opd30_amp_real_batch9', N, -1, fn2,
-                {b: derive(opd_ref(N, 9, 30.0, 'real', b, -1), 'accumulate', acc0h[b]) for b in fields}, 18, 9)
-    chk.done()
+    check_focus(f'v2/{N}/-1/accumulate/staged_opd30_amp_real_batch9', N, -1, fn2,
+           {b: derive(opd_ref(N, 9, 30.0, 'real', b, -1), 'accumulate', acc0h[b]) for b in fields}, 18, 9)
+    LEDGER.done()
 
 
 # ---- the register axis engine, through the public API ---------------------------------------------------------------
@@ -650,10 +617,6 @@ for _L in (1024, 2048, 4096):
         EXPECTED.add(_k(_L, False, True, rt=True, dense=True))
 
 
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 @pytest.mark.parametrize('n', (1024, 2048, 4096))
 def test_axis_plain_fft2(pb, n):
     """fft2 / ifft2: the DENSE row and column kernels at 2048 and 4096, the general ones at 1024"""
@@ -661,17 +624,16 @@ def test_axis_plain_fft2(pb, n):
     a = crand((n, n), 100 + n)
     d = dev(a)
     dense = n >= 2048
-    chk = Checker()
     with sfft.set_workers(-1):
         ref = sfft.fft2(a.astype(np.complex128))
-    got = run_axis(chk, f'axis/fft2/{n}', lambda: _ops.fft2(d, (n, n), dir=-1), rows_cols(n, False, dense))
-    chk.add(f'axis/fft2/{n}', got, ref)
+    got = run_axis(f'axis/fft2/{n}', lambda: _ops.fft2(d, (n, n), dir=-1), rows_cols(n, False, dense))
+    add(f'axis/fft2/{n}', got, ref)
     del ref
     with sfft.set_workers(-1):
         ref = sfft.ifft2(a.astype(np.complex128))
-    got = run_axis(chk, f'axis/ifft2/{n}', lambda: _ops.fft2(d, (n, n), dir=1, scale=1.0 / (n * n)), rows_cols(n, True, dense))
-    chk.add(f'axis/ifft2/{n}', got, ref)
-    chk.done()
+    got = run_axis(f'axis/ifft2/{n}', lambda: _ops.fft2(d, (n, n), dir=1, scale=1.0 / (n * n)), rows_cols(n, True, dense))
+    add(f'axis/ifft2/{n}', got, ref)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('n', (1024, 2048, 4096))
@@ -681,16 +643,15 @@ def test_axis_centred_and_cropped(pb, n):
     a = crand((n, n), 200 + n)
     d = dev(a)
     a2 = a.astype(np.complex128)
-    chk = Checker()
     with sfft.set_workers(-1):
         if n == 1024:
-            got = run_axis(chk, f'axis/focus_q1/{n}', lambda: P.focus(d, 1), rows_cols(n, False))
-            chk.add(f'axis/focus_q1/{n}', got, O.focus(a2, 1))
-        got = run_axis(chk, f'axis/focus_adjoint_q2/{n}', lambda: P.focus_adjoint(d, 2), rows_cols(n, True))
-        chk.add(f'axis/focus_adjoint_q2/{n}', got, O.focus_adjoint(a2, 2))
-        got = run_axis(chk, f'axis/unfocus_adjoint_q2/{n}', lambda: P.unfocus_adjoint(d, 2), rows_cols(n, False))
-        chk.add(f'axis/unfocus_adjoint_q2/{n}', got, O.unfocus_adjoint(a2, 2))
-    chk.done()
+            got = run_axis(f'axis/focus_q1/{n}', lambda: P.focus(d, 1), rows_cols(n, False))
+            add(f'axis/focus_q1/{n}', got, O.focus(a2, 1))
+        got = run_axis(f'axis/focus_adjoint_q2/{n}', lambda: P.focus_adjoint(d, 2), rows_cols(n, True))
+        add(f'axis/focus_adjoint_q2/{n}', got, O.focus_adjoint(a2, 2))
+        got = run_axis(f'axis/unfocus_adjoint_q2/{n}', lambda: P.unfocus_adjoint(d, 2), rows_cols(n, False))
+        add(f'axis/unfocus_adjoint_q2/{n}', got, O.unfocus_adjoint(a2, 2))
+    LEDGER.done()
 
 
 def test_axis_odd_width_and_line_counts(pb):
@@ -698,7 +659,6 @@ def test_axis_odd_width_and_line_counts(pb):
     counts of a one-axis transform"""
     from prysm_b200 import _ops
     n = 2048
-    chk = Checker()
 
     def centred(a, shape, crop=None):
         with sfft.set_workers(-1):
@@ -706,20 +666,20 @@ def test_axis_odd_width_and_line_counts(pb):
         return r if crop is None else O.crop_center(r, crop)
 
     a = crand((n, n), 301)
-    got = run_axis(chk, 'axis/fft2_centred_crop_odd_width/2048', lambda: _ops.fft2(dev(a), (n, n), dir=-1, shift_in=True, shift_out=True, crop=(n, n - 1)),
-                   rows_cols(n, False))
-    chk.add('axis/fft2_centred_crop_odd_width/2048', got, centred(a, (n, n), (n, n - 1)))
+    got = run_axis('axis/fft2_centred_crop_odd_width/2048', lambda: _ops.fft2(dev(a), (n, n), dir=-1, shift_in=True, shift_out=True, crop=(n, n - 1)),
+              rows_cols(n, False))
+    add('axis/fft2_centred_crop_odd_width/2048', got, centred(a, (n, n), (n, n - 1)))
     for rows in (1023, 1):
         b = crand((rows, n), 302 + rows)
-        got = run_axis(chk, f'axis/ifft2_rows{rows}/2048', lambda: _ops.fft2(dev(b), (n, n), dir=1, shift_in=True, shift_out=True), rows_cols(n, True))
+        got = run_axis(f'axis/ifft2_rows{rows}/2048', lambda: _ops.fft2(dev(b), (n, n), dir=1, shift_in=True, shift_out=True), rows_cols(n, True))
         with sfft.set_workers(-1):
             ref = sfft.fftshift(sfft.ifft2(sfft.ifftshift(O.pad2d(b.astype(np.complex128), out_shape=(n, n)))) * (n * n))
-        chk.add(f'axis/ifft2_rows{rows}/2048', got, ref)
+        add(f'axis/ifft2_rows{rows}/2048', got, ref)
     for cols in (3, 1):
         c = crand((4096, cols), 304 + cols)
-        got = run_axis(chk, f'axis/fft1_cols{cols}/4096', lambda: _ops.fft1(dev(c), axis=0, dir=-1), [_k(4096, False, True)])
-        chk.add(f'axis/fft1_cols{cols}/4096', got, sfft.fft(c.astype(np.complex128), axis=0))
-    chk.done()
+        got = run_axis(f'axis/fft1_cols{cols}/4096', lambda: _ops.fft1(dev(c), axis=0, dir=-1), [_k(4096, False, True)])
+        add(f'axis/fft1_cols{cols}/4096', got, sfft.fft(c.astype(np.complex128), axis=0))
+    LEDGER.done()
 
 
 WVL, DX, Z = HeNe, 0.01, 25.0
@@ -733,12 +693,11 @@ def test_axis_angular_spectrum(pb, n, Q):
     f = crand((n, n), 400 + n + Q)
     dense = Q == 1 and L >= 2048
     expect = [_k(L, False, False, dense=dense), _k(L, False, True, rt=True, dense=dense), _k(L, True, False, dense=L >= 2048)]
-    chk = Checker()
-    got = run_axis(chk, f'axis/angular_spectrum_q{Q}/{n}', lambda: P.angular_spectrum(dev(f), WVL, DX, Z, Q), expect)
+    got = run_axis(f'axis/angular_spectrum_q{Q}/{n}', lambda: P.angular_spectrum(dev(f), WVL, DX, Z, Q), expect)
     with sfft.set_workers(-1):
         ref = O.angular_spectrum(f.astype(np.complex128), WVL, DX, Z, Q)
-    chk.add(f'axis/angular_spectrum_q{Q}/{n}', got, ref)
-    chk.done()
+    add(f'axis/angular_spectrum_q{Q}/{n}', got, ref)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('L,Q', [(2048, 1), (1024, 2), (2048, 2), (4096, 2)])
@@ -747,12 +706,11 @@ def test_axis_angular_spectrum_adjoint(pb, L, Q):
     P = pb.propagation
     g = crand((L, L), 500 + L + Q)
     expect = [_k(L, False, False, dense=L >= 2048), _k(L, False, True, rt=True, dense=Q == 1 and L >= 2048)]
-    chk = Checker()
-    got = run_axis(chk, f'axis/angular_spectrum_adjoint_q{Q}/{L}', lambda: P.angular_spectrum_adjoint(dev(g), WVL, DX, Z, Q), expect)
+    got = run_axis(f'axis/angular_spectrum_adjoint_q{Q}/{L}', lambda: P.angular_spectrum_adjoint(dev(g), WVL, DX, Z, Q), expect)
     with sfft.set_workers(-1):
         ref = O.angular_spectrum_adjoint(g.astype(np.complex128), WVL, DX, Z, Q)
-    chk.add(f'axis/angular_spectrum_adjoint_q{Q}/{L}', got, ref)
-    chk.done()
+    add(f'axis/angular_spectrum_adjoint_q{Q}/{L}', got, ref)
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('n,Q', [(1024, 1), (2048, 1), (4096, 1), (512, 2), (1024, 2), (2048, 2)])
@@ -763,12 +721,11 @@ def test_axis_screened_free_space(pb, n, Q):
     f = crand((n, n), 600 + n + Q)
     rng = np.random.default_rng(700 + n)
     s = np.exp(1j * rng.uniform(0, 2 * np.pi, (n, n))).astype(np.complex64)
-    chk = Checker()
-    got = run_axis(chk, f'axis/screened_free_space_q{Q}/{n}', lambda: P.angular_spectrum(dev(f), WVL, DX, Z, Q, screen=dev(s)), [_k(L, False, False, pm=True, dense=Q == 1)])
+    got = run_axis(f'axis/screened_free_space_q{Q}/{n}', lambda: P.angular_spectrum(dev(f), WVL, DX, Z, Q, screen=dev(s)), [_k(L, False, False, pm=True, dense=Q == 1)])
     with sfft.set_workers(-1):
         ref = O.angular_spectrum(f.astype(np.complex128) * s.astype(np.complex128), WVL, DX, Z, Q)
-    chk.add(f'axis/screened_free_space_q{Q}/{n}', got, ref)
-    chk.done()
+    add(f'axis/screened_free_space_q{Q}/{n}', got, ref)
+    LEDGER.done()
 
 
 CZT_GEOMETRY = {1024: (512, 512), 2048: (1024, 1023), 4096: (2048, 1024)}   # K: (pupil samples N, focal samples M)
@@ -787,12 +744,11 @@ def test_axis_czt(pb, K):
     a = crand((N, N), 800 + K)
     g = crand((M, M), 900 + K)
     rt = [_k(K, False, False, rt=True), _k(K, False, True, rt=True)]
-    chk = Checker()
-    got = run_axis(chk, f'axis/czt/{K}', lambda: ex(dev(a)), rt)
-    chk.add(f'axis/czt/{K}', got, exo(a.astype(np.complex128)))
-    got = run_axis(chk, f'axis/czt_adjoint/{K}', lambda: ex.adjoint(dev(g)), rt)
-    chk.add(f'axis/czt_adjoint/{K}', got, exo.adjoint(g.astype(np.complex128)))
-    chk.done()
+    got = run_axis(f'axis/czt/{K}', lambda: ex(dev(a)), rt)
+    add(f'axis/czt/{K}', got, exo(a.astype(np.complex128)))
+    got = run_axis(f'axis/czt_adjoint/{K}', lambda: ex.adjoint(dev(g)), rt)
+    add(f'axis/czt_adjoint/{K}', got, exo.adjoint(g.astype(np.complex128)))
+    LEDGER.done()
 
 
 @pytest.mark.parametrize('K', (1024, 2048))
@@ -804,16 +760,22 @@ def test_axis_czt_intensity(pb, K):
     ref = exo(a.astype(np.complex128))
     inten = ref.real ** 2 + ref.imag ** 2
     rt = [_k(K, False, False, rt=True), _k(K, False, True, rt=True)]
-    chk = Checker()
-    got = run_axis(chk, f'axis/czt_intensity/{K}', lambda: ex.intensity(dev(a)), rt)
-    chk.add(f'axis/czt_intensity/{K}', got, inten)
+    got = run_axis(f'axis/czt_intensity/{K}', lambda: ex.intensity(dev(a)), rt)
+    add(f'axis/czt_intensity/{K}', got, inten)
     acc0 = acc_start((M, M), K)
-    got = run_axis(chk, f'axis/czt_intensity_accumulate/{K}', lambda: ex.intensity(dev(a), weight=WEIGHT, out=acc0.clone()), rt)
-    chk.add(f'axis/czt_intensity_accumulate/{K}', got, acc0.cpu().numpy().astype(np.float64) + WEIGHT * inten)
-    chk.done()
+    got = run_axis(f'axis/czt_intensity_accumulate/{K}', lambda: ex.intensity(dev(a), weight=WEIGHT, out=acc0.clone()), rt)
+    add(f'axis/czt_intensity_accumulate/{K}', got, acc0.cpu().numpy().astype(np.float64) + WEIGHT * inten)
+    LEDGER.done()
 
 
 def test_zz_every_reachable_instantiation_was_hit(pb):
     """runs last: every axis_reg_kernel instantiation the Python API can reach ran in an fp64-checked case above"""
     assert not EXPECTED - HIT, sorted(EXPECTED - HIT)
     assert not HIT - EXPECTED, sorted(HIT - EXPECTED)
+
+
+def test_zz_every_figure_has_a_measurement():
+    """a figure this session reached that has no MEASURED entry is held to the bare ceiling, a bound nobody measured"""
+    if os.environ.get('PB_TEST_MEASUREMENTS'):
+        pytest.skip('recording figures')
+    assert not LEDGER.missing(), f'no MEASURED entry (record them with PB_TEST_MEASUREMENTS): {LEDGER.missing()}'

@@ -24,7 +24,7 @@ def margin(name, fig, ceiling):
 # ---- launch rules --------------------------------------------------------------------------------------------------
 def test_launch_rules():
     assert A.grid_for(1, 132) == 1 and A.grid_for(10 ** 9, 132) == 132 * 16
-    assert A.grid_cap(132) == 540672 and A.sweep_counts(132)[-1] == 3 * 540672
+    assert A.sweep(132) == 540672 and A.sweep_counts(132)[-1] == 3 * 540672
     assert [A.chunk_len(n) for n in A.CROSS_NX] == [1, 1, 1, 2, 2, 16, 79]
     assert (A.crossing_launches(False), A.crossing_launches(True)) == (3, 4)
     assert A.AZ_MAX_NY * 8 == 224 * 1024

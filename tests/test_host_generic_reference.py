@@ -13,11 +13,7 @@ import scipy.fft as sfft
 
 import generic_reference as G
 from generic_reference import PB_C64, PB_C128
-
-
-def crand(shape, seed, cdt=np.complex128):
-    rng = np.random.default_rng(seed)
-    return (rng.standard_normal(shape) + 1j * rng.standard_normal(shape)).astype(cdt)
+from gpu_fixtures import crand
 
 
 # ---- the long-double helpers against closed forms -------------------------------------------------------------------

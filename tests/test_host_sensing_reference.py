@@ -7,12 +7,8 @@ import scipy.special as sps
 
 import sensing_reference as S
 from conftest import load_golden
+from gpu_fixtures import crand
 from test_gpu_sensing_vs_fp64 import CEIL
-
-
-def crand(shape, seed):
-    rng = np.random.default_rng(seed)
-    return rng.standard_normal(shape) + 1j * rng.standard_normal(shape)
 
 
 # ---- launch rules --------------------------------------------------------------------------------------------------

@@ -8,12 +8,8 @@ import pytest
 import scipy.special as sps
 
 import streaming_reference as S
+from gpu_fixtures import crand
 from streaming_reference import LD, LDBL, PB_C64, PB_C128, CEIL_ELEM, CEIL_RED
-
-
-def crand(shape, seed, cdt=np.complex128):
-    rng = np.random.default_rng(seed)
-    return (rng.standard_normal(shape) + 1j * rng.standard_normal(shape)).astype(cdt)
 
 
 def rand(shape, seed, dt=np.float64):
@@ -23,14 +19,14 @@ def rand(shape, seed, dt=np.float64):
 # ---- launch geometry ------------------------------------------------------------------------------------------------
 def test_launch_geometry():
     sm = 132
-    assert S.grid_for(1, sm) == 1 and S.grid_for(S.elementwise_cap(sm), sm) == sm * 16
-    assert S.grid_for(S.elementwise_cap(sm) + 1, sm) == sm * 16
+    assert S.grid_for(1, sm) == 1 and S.grid_for(S.sweep(sm), sm) == sm * 16
+    assert S.grid_for(S.sweep(sm) + 1, sm) == sm * 16
     assert S.reduction_grid(S.reduction_cap(sm) + 1, sm) == sm * 4
     assert S.mode_projection_gx(10 ** 6, 1, sm) == sm * 4
     assert S.mode_projection_gx(10 ** 6, sm * 4 + 1, sm) == 1
     assert tuple(S.shapes(sm)) == S.SHAPE_NAMES
     counts = {a * b for a, b in S.shapes(sm).values()}
-    for cap in (S.reduction_cap(sm), S.elementwise_cap(sm)):
+    for cap in (S.reduction_cap(sm), S.sweep(sm)):
         assert {cap - 1, cap, cap + 1} <= counts
     assert S.shapes(sm)['4096sq'] == (4096, 4096)
 
