@@ -752,6 +752,41 @@ int pb_field_at_depth(pb_handle_t h, int dtype, int pol, int nlayers, const void
                       const void* n, double n0_re, double n0_im, double wvl, double theta0, const void* E_b,
                       const void* H_b, void* E, void* H, void* stream);
 
+/* ---- Coating design (prysm/x/coatings merit.py and needle.py) on the thin-film chain above ---------------------------
+ * Operands: in[PB_CM_NOPS], strides[5 * PB_CM_NOPS] laid out as for pb_stack_eval; slots 0-5 are the six thin-film
+ *   operands, then target and weight (fp64) and, for pb_needle only, the needle index (complex128; NULL otherwise).
+ *   pol is PB_TF_POL_S, PB_TF_POL_P or PB_CM_POL_AVG: for avg one thread evaluates both polarisations, q is their mean
+ *   and each is seeded with 2 w (q - target) / 2.  The quantity q (PB_CM_Q_*) of a sample is
+ *   R; T; the absorptance of layer b0; |E|^2 at boundary b0; the largest |E|^2 over the nb boundaries of `blist`
+ *   (device int array of 2 nb: the boundaries, then 1 where that listing is the boundary's last, else 0; the seed goes
+ *   to the first maximum and only if its listing is the last); the mean of |E|^2 at boundaries b0 and b1.  Layer and
+ *   boundary indices are non-negative and in range.
+ * pb_coating_merit: flags (PB_CM_OUT_*) select the outputs: value (one fp64 device scalar) = sum of w (q - target)^2
+ *   over the count samples; residuals (count, dtype's real type) = sqrt(w) (q - target); grad (nlayers, or (2, nlayers)
+ *   thickness first when both kinds are asked) of the value.  With PB_CM_ACCUMULATE the value and the gradient are
+ *   added to what value and grad hold (the gradient in dtype's real type).  One sample launch, then one fixed-order
+ *   reduce launch when a value or gradient is asked; the forward vectors are staged in the handle's scratch, no
+ *   atomics, so repeated calls are bit-identical.
+ * pb_needle: P(z) of an R or T term at nz depths, summed over the samples.  zlist (device int array of nlayers + 1 +
+ *   nz) holds the start offset of each layer's run and then the depth indices grouped by layer j, the layer a depth is
+ *   evaluated in; zpart (fp64, (2, nz)) holds each depth's partial thicknesses z - Z_j, then Z_{j+1} - z.  P (nz, dtype's real type) is written, or added
+ *   to with accumulate != 0.  Two launches, no atomics. */
+typedef enum { PB_CM_IN_TARGET = 6, PB_CM_IN_WEIGHT = 7, PB_CM_IN_NEEDLE = 8, PB_CM_NOPS = 9 } pb_cm_operand;
+typedef enum {
+    PB_CM_Q_R = 0, PB_CM_Q_T = 1, PB_CM_Q_ABS = 2, PB_CM_Q_ESQ = 3, PB_CM_Q_PEAK = 4, PB_CM_Q_LAYER = 5
+} pb_cm_quantity;
+typedef enum { PB_CM_POL_AVG = 2 } pb_cm_pol;
+typedef enum {
+    PB_CM_OUT_VALUE = 1, PB_CM_OUT_RESIDUALS = 2, PB_CM_OUT_GRAD_THICKNESS = 4, PB_CM_OUT_GRAD_INDEX = 8,
+    PB_CM_ACCUMULATE = 16
+} pb_cm_flag;
+int pb_coating_merit(pb_handle_t h, int dtype, int quantity, int pol, int flags, int nlayers, int ndim,
+                     const long long* shape, const long long* strides, const void* const* in, int b0, int b1,
+                     const void* blist, int nb, void* value, void* residuals, void* grad, void* stream);
+int pb_needle(pb_handle_t h, int dtype, int quantity, int pol, int nlayers, int ndim, const long long* shape,
+              const long long* strides, const void* const* in, const void* zpart, long long nz, const void* zlist, void* P,
+              int accumulate, void* stream);
+
 /* ---- PSF / MTF analysis (prysm/_richdata.py, prysm/coordinates.py uniform_cart_to_polar, prysm/psf.py, prysm/otf.py) --
  * Data is (ny, nx) on the fp64 ascending axes xax (nx) and yax (ny), device arrays.  Every sampling entry point uses one
  * linear interpolator, scipy's RegularGridInterpolator(method='linear'): interval = the largest i with axis[i] <= p

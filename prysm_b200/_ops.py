@@ -1360,9 +1360,9 @@ def tensor_sum(basis, coefs, ms, ns, x, y, shape, separable, want_der, x_norm=1.
 
 
 def tf_layout(ops):
-    """(broadcast calculation shape, collapsed shape, (TF_NOPS * 5) int64 host strides) of the six thin-film operands
+    """(broadcast calculation shape, collapsed shape, (len(ops), 5) int64 host strides) of the six thin-film operands
     (wavelength, angle, ambient index, substrate index, layer index, layer thickness: fp64 / complex128 device tensors,
-    the last two with a leading layer axis).  Dims that are contiguous in every operand are merged; a broadcast that
+    the last two with a leading layer axis) and of any operands after them (per sample only).  Dims that are contiguous in every operand are merged; a broadcast that
     still needs more than TF_DIMS dims is refused with ValueError."""
     calc = [tuple(t.shape[1:]) if q in (capi.TF_IN_N, capi.TF_IN_D) else tuple(t.shape) for q, t in enumerate(ops)]
     bshape = np.broadcast_shapes(*calc)
@@ -1387,7 +1387,7 @@ def tf_layout(ops):
     if len(dims) > capi.TF_DIMS:
         raise ValueError(f'thin-film operands broadcast to {bshape}, which needs {len(dims)} dims after merging the '
                          f'contiguous ones; at most {capi.TF_DIMS} are supported')
-    strides = np.zeros((capi.TF_NOPS, capi.TF_DIMS + 1), dtype=np.int64)
+    strides = np.zeros((len(ops), capi.TF_DIMS + 1), dtype=np.int64)
     for q, s in enumerate(cst):
         strides[q, :len(s)] = s
         if q in (capi.TF_IN_N, capi.TF_IN_D) and ops[q].shape[0] != 1:
@@ -1404,7 +1404,7 @@ def tf_nlayers(ops):
 def _tf_args(ops):
     bshape, dims, strides = tf_layout(ops)
     shp = np.asarray(dims if dims else [1], dtype=np.int64)
-    ins = (C.c_void_p * capi.TF_NOPS)(*[t.data_ptr() for t in ops])
+    ins = (C.c_void_p * len(ops))(*[t.data_ptr() for t in ops])
     keep = (shp, strides, ins)
     return bshape, len(dims), shp.ctypes.data_as(C.POINTER(C.c_longlong)), \
         strides.ctypes.data_as(C.POINTER(C.c_longlong)), C.cast(ins, C.POINTER(C.c_void_p)), keep
@@ -1449,6 +1449,40 @@ def stack_grad(pol, kinds, ops, E, H, seeds, rdtype):
     _call(lib.pb_stack_grad, E, _CODE[rdtype], int(pol), int(kinds), nlayers, nd, shp, stp, inp, _p(E), _p(H),
           C.cast(sp, C.POINTER(C.c_void_p)), _p(grad))
     return grad
+
+
+def cm_layout(ops):
+    """(broadcast shape, ndim, shape, strides, operands, keep-alive) of the coating-design operands: the six thin-film
+    operands, target and weight, and optionally the needle index; the arrays are padded to CM_NOPS slots."""
+    bshape, dims, strides = tf_layout(ops)
+    full = np.zeros((capi.CM_NOPS, capi.TF_DIMS + 1), dtype=np.int64)
+    full[:len(ops)] = strides
+    shp = np.asarray(dims if dims else [1], dtype=np.int64)
+    ins = (C.c_void_p * capi.CM_NOPS)(*([t.data_ptr() for t in ops] + [None] * (capi.CM_NOPS - len(ops))))
+    return bshape, len(dims), shp, full, ins
+
+
+def coating_merit(quantity, pol, flags, ops, b0=0, b1=0, blist=None, value=None, residuals=None, grad=None,
+                  rdtype=torch.float64):
+    """One merit term (pb_coating_merit) over ops = the six thin-film operands, target and weight: the fp64 value
+    into `value` (a one-element device array), sqrt(w) (q - target) into `residuals` (count, rdtype) and the
+    gradient into `grad` (rdtype), each as `flags` (CM_OUT_*, CM_ACCUMULATE) asks."""
+    nlayers = tf_nlayers(ops)
+    bshape, nd, shp, strides, ins = cm_layout(ops)
+    nb = 0 if blist is None else blist.numel() // 2
+    _call(lib.pb_coating_merit, ops[0], _CODE[rdtype], int(quantity), int(pol), int(flags), nlayers, nd,
+          shp.ctypes.data_as(C.POINTER(C.c_longlong)), strides.ctypes.data_as(C.POINTER(C.c_longlong)),
+          C.cast(ins, C.POINTER(C.c_void_p)), int(b0), int(b1), _p(blist), nb, _p(value), _p(residuals), _p(grad))
+
+
+def needle(quantity, pol, ops, zpart, zlist, P, accumulate):
+    """P(z) of an R or T term (pb_needle): ops = the six thin-film operands, target, weight and the needle index;
+    zpart (2, nz) fp64 partial thicknesses, zlist the per-layer depth runs (int32), P (nz) written or added to."""
+    nlayers = tf_nlayers(ops)
+    bshape, nd, shp, strides, ins = cm_layout(ops)
+    _call(lib.pb_needle, ops[0], _CODE[P.dtype], int(quantity), int(pol), nlayers, nd,
+          shp.ctypes.data_as(C.POINTER(C.c_longlong)), strides.ctypes.data_as(C.POINTER(C.c_longlong)),
+          C.cast(ins, C.POINTER(C.c_void_p)), _p(zpart), int(zpart.shape[1]), _p(zlist), _p(P), int(bool(accumulate)))
 
 
 def field_at_depth(pol, z, zb, n, n0, wvl, theta0, Eb, Hb, cdtype):

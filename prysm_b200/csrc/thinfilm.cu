@@ -103,15 +103,17 @@ __device__ inline TfSample tf_sample(const TfOps& op, long long i) {
 // layer k of a sample: index, cos theta_k, phase thickness beta, admittance eta and thickness
 struct TfLayer { double2 n, cost, beta, eta; double d; };
 
-__device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k) {
+__device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k, int pol) {
     TfLayer L;
     L.n = ((const double2*)op.p[PB_TF_IN_N])[s.off_n + (long long)k * op.st[PB_TF_IN_N][PB_TF_DIMS]];
     L.d = ((const double*)op.p[PB_TF_IN_D])[s.off_d + (long long)k * op.st[PB_TF_IN_D][PB_TF_DIMS]];
     L.cost = tf_cos_snell(s.n0, L.n, s.sin0);
     L.beta = cscale(cmul(cscale(L.n, 2.0 * M_PI * L.d), L.cost), 1.0 / s.wvl);
-    L.eta = tf_admittance(L.n, L.cost, op.pol);
+    L.eta = tf_admittance(L.n, L.cost, pol);
     return L;
 }
+
+__device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k) { return tf_layer(op, s, k, op.pol); }
 
 // v <- M v with M = [[cos b, -i sin b / eta], [-i eta sin b, cos b]]
 __device__ inline void tf_apply(double2 sb, double2 cb, double2 eta, double2& v0, double2& v1) {
@@ -382,6 +384,383 @@ __global__ void __launch_bounds__(PB_TF_THREADS) field_at_depth_kernel(const dou
     }
 }
 
+
+// ---- coating design (prysm/x/coatings merit.py, needle.py) ------------------------------------------------------
+// One thread per sample runs, per polarisation, the forward sweep into a stage in the handle's scratch (v_k of every
+// boundary, unscaled), forms q and its seed in registers, and runs the reverse sweep of stack_grad_kernel with the
+// seed applied where the term puts it: no field or seed array goes through HBM.  The warp partials are summed in a
+// fixed order by a second launch.
+
+// both polarisations in one thread take about 164 registers: 3 blocks of 128 threads per SM, 12 warps, against 8 for
+// 256-thread blocks at that size
+constexpr int cm_threads(int npol) { return npol == 2 ? 128 : PB_TF_THREADS; }
+
+struct CmTerm {
+    int quantity, npol, b0, b1, nb;
+    const int* blist;              // nb boundaries, then nb "last listing" flags
+    const double* tgt;
+    const double* wgt;
+    long long st_tgt[PB_TF_DIMS], st_wgt[PB_TF_DIMS];
+    long long cpad;                // stage pitch: count rounded up to whole warps
+};
+
+__device__ inline long long cm_offset(const TfOps& op, const long long* st, long long i) {
+    long long off = 0;
+    for (int j = PB_TF_DIMS - 1; j >= 0; --j) {
+        off += (i % op.shape[j]) * st[j];
+        i /= op.shape[j];
+    }
+    return off;
+}
+
+// forward sweep of one polarisation into the stage V0 / V1 (boundary k at row k); returns r, t and the admittances
+struct CmFwd { double2 r, t, eta0; double t2; };
+
+// r and t from (B, C) = v_0; the reverse sweep recomputes them from the stage, with the same operations
+__device__ inline CmFwd cm_rt(const TfSample& s, int pol, double2 v0, double2 v1) {
+    CmFwd f;
+    f.eta0 = tf_admittance(s.n0, make_double2(s.cos0, 0.0), pol);
+    const double2 eb = cmul(f.eta0, v0);
+    const double2 den = cadd(eb, v1);
+    f.r = tf_div(csub(eb, v1), den);
+    f.t = tf_div(cscale(f.eta0, 2.0), den);
+    f.t2 = tf_abs2(f.t);
+    return f;
+}
+
+__device__ inline CmFwd cm_forward(const TfOps& op, const TfSample& s, int pol, double2* V0, double2* V1,
+                                   long long pitch, long long is) {
+    const int N = op.nlayers;
+    const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
+    double2 v0 = make_double2(1.0, 0.0), v1 = eta_sub;
+    V0[(long long)N * pitch + is] = v0;
+    V1[(long long)N * pitch + is] = v1;
+    for (int k = N - 1; k >= 0; --k) {
+        const TfLayer L = tf_layer(op, s, k, pol);
+        double2 sb, cb;
+        tf_sincos(L.beta, &sb, &cb);
+        tf_apply(sb, cb, L.eta, v0, v1);
+        V0[(long long)k * pitch + is] = v0;
+        V1[(long long)k * pitch + is] = v1;
+    }
+    return cm_rt(s, pol, v0, v1);
+}
+
+// q of one polarisation; for the peak, *arg is the list position of the first maximum (NaN counts as the maximum)
+__device__ inline double cm_quantity(const CmTerm& tm, const TfSample& s, int pol, const CmFwd& f, const double2* V0,
+                                     const double2* V1, long long pitch, long long is, int* arg) {
+    switch (tm.quantity) {
+    case PB_CM_Q_R: return tf_abs2(f.r);
+    case PB_CM_Q_T: {
+        const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
+        return eta_sub.x / f.eta0.x * f.t2;
+    }
+    case PB_CM_Q_ABS: {
+        const long long o = (long long)tm.b0 * pitch + is;
+        const double g0 = cmulc(V0[o], V1[o]).x, g1 = cmulc(V0[o + pitch], V1[o + pitch]).x;
+        return f.t2 * g0 / f.eta0.x - f.t2 * g1 / f.eta0.x;
+    }
+    case PB_CM_Q_ESQ: return f.t2 * tf_abs2(V0[(long long)tm.b0 * pitch + is]);
+    case PB_CM_Q_PEAK: {
+        double best = 0.0;
+        for (int j = 0; j < tm.nb; ++j) {
+            const double e = f.t2 * tf_abs2(V0[(long long)tm.blist[j] * pitch + is]);
+            if (j == 0 || (!isnan(best) && (e > best || isnan(e)))) { best = e; *arg = j; }
+        }
+        return best;
+    }
+    default:
+        return 0.5 * (f.t2 * tf_abs2(V0[(long long)tm.b0 * pitch + is]) + f.t2 * tf_abs2(V0[(long long)tm.b1 * pitch + is]));
+    }
+}
+
+// the field seed of boundary k (diff.py:204-224): fbar = (H cf + 2 ce E, E cf) with E = t v0, H = t v1
+struct CmSeed { int ka, kb; double cfa, cea, cfb, ceb; };
+
+__device__ inline void cm_field_bar(const CmSeed& sd, int k, double2 E, double2 H, double2& Eb, double2& Hb) {
+    double cf = 0.0, ce = 0.0;
+    if (k == sd.ka) { cf += sd.cfa; ce += sd.cea; }
+    if (k == sd.kb) { cf += sd.cfb; ce += sd.ceb; }
+    Eb = cadd(cscale(H, cf), cscale(E, 2.0 * ce));
+    Hb = cscale(E, cf);
+}
+
+// the reverse-sweep start of one polarisation: vbar_0 from the amplitude and field seeds of dq, and the field seeds
+__device__ inline void cm_seed(const CmTerm& tm, const TfSample& s, int pol, const CmFwd& f, double dq, int arg,
+                               const double2* V0, const double2* V1, long long pitch, long long is, CmSeed& sd,
+                               double2& vb0, double2& vb1) {
+    const double inv_re0 = 1.0 / f.eta0.x;
+    sd.ka = sd.kb = -1;
+    sd.cfa = sd.cea = sd.cfb = sd.ceb = 0.0;
+    double2 rb = make_double2(0.0, 0.0), tb = make_double2(0.0, 0.0);
+    if (tm.quantity == PB_CM_Q_R) rb = cscale(f.r, 2.0 * dq);
+    else if (tm.quantity == PB_CM_Q_T) {
+        const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
+        tb = cscale(f.t, 2.0 * (eta_sub.x * inv_re0) * dq);
+    } else if (tm.quantity == PB_CM_Q_ABS) {
+        sd.ka = tm.b0; sd.cfa = dq * inv_re0;
+        sd.kb = tm.b0 + 1; sd.cfb = -dq * inv_re0;
+    } else if (tm.quantity == PB_CM_Q_ESQ) {
+        sd.ka = tm.b0; sd.cea = dq;
+    } else if (tm.quantity == PB_CM_Q_PEAK) {
+        if (tm.blist[tm.nb + arg]) { sd.ka = tm.blist[arg]; sd.cea = dq; }
+    } else {
+        sd.ka = tm.b0; sd.cea = 0.5 * dq;
+        sd.kb = tm.b1; sd.ceb = 0.5 * dq;
+    }
+    // f_k = t v_k: tbar += v_k^H fbar_k at the seeded boundaries
+    for (int w = 0; w < 2; ++w) {
+        const int k = w == 0 ? sd.ka : (sd.kb == sd.ka ? -1 : sd.kb);
+        if (k < 0) continue;
+        const double2 v0 = V0[(long long)k * pitch + is], v1 = V1[(long long)k * pitch + is];
+        double2 eb2, hb2;
+        cm_field_bar(sd, k, cmul(f.t, v0), cmul(f.t, v1), eb2, hb2);
+        tb = cadd(tb, cadd(cmulc(eb2, v0), cmulc(hb2, v1)));
+    }
+    const double2 eb = cmul(f.eta0, V0[is]);
+    const double2 inv_den = tf_div(make_double2(1.0, 0.0), cadd(eb, V1[is]));
+    const double2 dr_dB = cmul(cmul(f.eta0, make_double2(1.0 - f.r.x, -f.r.y)), inv_den);
+    const double2 dr_dC = cmul(make_double2(-1.0 - f.r.x, -f.r.y), inv_den);
+    const double2 dt_dB = cmul(make_double2(-(f.t.x * f.eta0.x - f.t.y * f.eta0.y), -(f.t.x * f.eta0.y + f.t.y * f.eta0.x)),
+                               inv_den);
+    const double2 dt_dC = cmul(make_double2(-f.t.x, -f.t.y), inv_den);
+    vb0 = cadd(cmulc(rb, dr_dB), cmulc(tb, dt_dB));
+    vb1 = cadd(cmulc(rb, dr_dC), cmulc(tb, dt_dC));
+    if (sd.ka == 0 || sd.kb == 0) {
+        double2 eb2, hb2;
+        cm_field_bar(sd, 0, cmul(f.t, V0[is]), cmul(f.t, V1[is]), eb2, hb2);
+        const double2 ct = cconj(f.t);
+        vb0 = cadd(vb0, cmul(ct, eb2));
+        vb1 = cadd(vb1, cmul(ct, hb2));
+    }
+}
+
+// a / x for a real x, as numpy divides a complex array by a real one
+__device__ inline double2 cm_over(double2 a, double x) { return make_double2(a.x / x, a.y / x); }
+
+// lane 0 adds the warp's sum of v to its own slot p (written on the warp's first visit)
+__device__ inline void cm_warp_add(double v, bool act, int lane, bool first, double* p) {
+    v = warp_reduce(act ? v : 0.0, OpAdd{});
+    if (lane == 0) *p = first ? v : *p + v;
+}
+
+// partial rows: kind * N + k for the gradients, 2 N for the value
+template <int NPOL>
+__global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) coating_merit_kernel(const TfOps op, const CmTerm tm, long long count,
+                                                                       int flags, double2* __restrict__ V0,
+                                                                       double2* __restrict__ V1, double* __restrict__ partial,
+                                                                       void* __restrict__ resid, bool resid_f32) {
+    const int N = op.nlayers;
+    const long long W = (long long)gridDim.x * (blockDim.x / 32);
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const int kinds = (flags >> 2) & 3;
+    const long long pitch = tm.cpad;
+    for (long long base = warp * 32; base < count; base += W * 32) {
+        const bool first = base == warp * 32;
+        const bool act = base + lane < count;
+        const long long i = act ? base + lane : count - 1;
+        const long long is = base + lane;                      // this lane's own stage column
+        const TfSample s = tf_sample(op, i);
+        const double tg = tm.tgt[cm_offset(op, tm.st_tgt, i)], w = tm.wgt[cm_offset(op, tm.st_wgt, i)];
+        // the peak's list position per polarisation, 16 bits each (loops that are not unrolled keep it in a register)
+        unsigned args = 0;
+        double q = 0.0;
+#pragma unroll 1
+        for (int p = 0; p < NPOL; ++p) {
+            const int pol = NPOL == 2 ? p : op.pol;
+            double2* v0 = V0 + (long long)p * (N + 1) * pitch;
+            double2* v1 = V1 + (long long)p * (N + 1) * pitch;
+            const CmFwd f = cm_forward(op, s, pol, v0, v1, pitch, is);
+            int a = 0;
+            q += cm_quantity(tm, s, pol, f, v0, v1, pitch, is, &a);
+            args |= (unsigned)a << (16 * p);
+        }
+        q = q / NPOL;
+        const double d = q - tg;
+        if (flags & PB_CM_OUT_RESIDUALS && act) {
+            const double res = sqrt(w) * d;
+            if (resid_f32) ((float*)resid)[i] = (float)res;
+            else ((double*)resid)[i] = res;
+        }
+        if (flags & PB_CM_OUT_VALUE) cm_warp_add(w * (d * d), act, lane, first, partial + (long long)(2 * N) * W + warp);
+        if (!kinds) continue;
+        const double dq = 2.0 * w * d / NPOL;
+#pragma unroll 1
+        for (int p = 0; p < NPOL; ++p) {
+            const int pol = NPOL == 2 ? p : op.pol;
+            const double2* v0 = V0 + (long long)p * (N + 1) * pitch;
+            const double2* v1 = V1 + (long long)p * (N + 1) * pitch;
+            const CmFwd f = cm_rt(s, pol, v0[is], v1[is]);
+            CmSeed sd;
+            double2 vb0, vb1;
+            cm_seed(tm, s, pol, f, dq, (int)(args >> (16 * p) & 0xffffu), v0, v1, pitch, is, sd, vb0, vb1);
+            const double2 ct = cconj(f.t);
+            const double2 n0sq_sin2 = cscale(cmul(s.n0, s.n0), s.sin0 * s.sin0);
+            for (int k = 0; k < N; ++k) {
+                const TfLayer L = tf_layer(op, s, k, pol);
+                double2 sb, cb;
+                tf_sincos(L.beta, &sb, &cb);
+                const long long o1 = (long long)(k + 1) * pitch + is;
+                const double2 w0 = v0[o1], w1 = v1[o1];                         // v_{k+1}
+                const double2 m00 = cmulc(vb0, w0), m01 = cmulc(vb0, w1), m10 = cmulc(vb1, w0), m11 = cmulc(vb1, w1);
+                const double2 ieta = tf_div(make_double2(1.0, 0.0), L.eta);
+                const double2 icb = make_double2(cb.y, -cb.x);                 // -i cos b
+                const double2 dB01 = cmul(icb, ieta), dB10 = cmul(icb, L.eta);
+                const double2 cbeta = csub(cadd(cmulc(m01, dB01), cmulc(m10, dB10)), cadd(cmulc(m00, sb), cmulc(m11, sb)));
+                if (kinds & PB_TF_GRAD_THICKNESS) {
+                    const double2 dbdd = cscale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
+                    cm_warp_add(cmulc(dbdd, cbeta).x, act, lane, first && p == 0, partial + (long long)k * W + warp);
+                }
+                if (kinds & PB_TF_GRAD_INDEX) {
+                    const double2 isb = make_double2(-sb.y, sb.x);             // i sin b
+                    const double2 dE01 = cmul(isb, cmul(ieta, ieta)), dE10 = make_double2(-isb.x, -isb.y);
+                    const double2 ceta = cadd(cmulc(m01, dE01), cmulc(m10, dE10));
+                    const double2 n2 = cmul(L.n, L.n);
+                    const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
+                    const double2 ndc = cmul(L.n, dcdn);
+                    const double2 dbdn = cscale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
+                    const double2 dedn = pol == PB_TF_POL_P
+                        ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
+                        : cadd(L.cost, ndc);
+                    cm_warp_add(cmulc(dbdn, cbeta).x + cmulc(dedn, ceta).x, act, lane, first && p == 0,
+                                partial + (long long)(N + k) * W + warp);
+                }
+                // vbar_{k+1} = M_k^H vbar_k (+ conj(t) fbar_{k+1})
+                const double2 mis = make_double2(sb.y, -sb.x);
+                const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
+                const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
+                const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
+                vb0 = nb0; vb1 = nb1;
+                if (k + 1 == sd.ka || k + 1 == sd.kb) {
+                    double2 eb2, hb2;
+                    cm_field_bar(sd, k + 1, cmul(f.t, w0), cmul(f.t, w1), eb2, hb2);
+                    vb0 = cadd(vb0, cmul(ct, eb2));
+                    vb1 = cadd(vb1, cmul(ct, hb2));
+                }
+            }
+        }
+    }
+}
+
+// one block per partial row, the first nw warps summed in a fixed order: gradient rows into grad, the value row into
+// value (fp64); residuals rounded once to R
+// P[z] from the nz rows of needle partials, in the same fixed order
+template <typename R>
+__global__ void __launch_bounds__(PB_TF_THREADS) needle_reduce_kernel(const double* __restrict__ partial, long long W,
+                                                                       long long nw, int accumulate, R* __restrict__ P) {
+    __shared__ double sh[PB_TF_THREADS];
+    const double* p = partial + (long long)blockIdx.x * W;
+    double a = 0.0;
+    for (long long w = threadIdx.x; w < nw; w += blockDim.x) a += p[w];
+    a = tree_sum<PB_TF_THREADS>(a, sh);
+    if (threadIdx.x == 0) P[blockIdx.x] = accumulate ? P[blockIdx.x] + (R)a : (R)a;
+}
+
+template <typename R>
+__global__ void __launch_bounds__(PB_TF_THREADS) coating_merit_reduce_kernel(const double* __restrict__ partial,
+                                                                              long long W, long long nw, int N, int flags,
+                                                                              double* __restrict__ value,
+                                                                              R* __restrict__ grad) {
+    __shared__ double sh[PB_TF_THREADS];
+    const int row = blockIdx.x;
+    const bool acc = flags & PB_CM_ACCUMULATE;
+    const int kinds = (flags >> 2) & 3;
+    if (row < 2 * N) {
+        if (!(kinds & (1 << (row / N)))) return;
+    } else if (!(flags & PB_CM_OUT_VALUE)) return;
+    const double* p = partial + (long long)row * W;
+    double a = 0.0;
+    for (long long w = threadIdx.x; w < nw; w += blockDim.x) a += p[w];
+    a = tree_sum<PB_TF_THREADS>(a, sh);
+    if (threadIdx.x) return;
+    if (row == 2 * N) { *value = acc ? *value + a : a; return; }
+    const int kind = row / N, k = row % N;
+    R* g = grad + (kinds == (PB_TF_GRAD_THICKNESS | PB_TF_GRAD_INDEX) ? kind * N : 0) + k;
+    *g = acc ? *g + (R)a : (R)a;
+}
+
+struct NeedleStrides { long long st[PB_TF_DIMS]; };
+
+// P(z) of an R or T term (needle.py:18-91).  The assembled-matrix cotangent of diff.py's _rt_assembly_cotangent is
+// c_M = u w^H with u = (Bbar, Cbar) and w = (1, eta_sub), so Re tr(c_M^H L_j X R_{j+1}) = Re(vbar_j^H X v_{j+1}) with
+// X = M_top G M_bot: each (sample, depth) costs two characteristic matrices applied to a 2-vector.
+template <int NPOL>
+__global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) needle_kernel(const TfOps op, const CmTerm tm, const double2* __restrict__ nn,
+                                                                const NeedleStrides st_nn, long long count,
+                                                                const double* __restrict__ zpart, long long nz,
+                                                                const int* __restrict__ zlist,
+                                                                double2* __restrict__ V0, double2* __restrict__ V1,
+                                                                double* __restrict__ partial) {
+    const int N = op.nlayers;
+    const long long W = (long long)gridDim.x * (blockDim.x / 32);
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const long long pitch = tm.cpad;
+    const int* order = zlist + N + 1;
+    for (long long base = warp * 32; base < count; base += W * 32) {
+        const bool first = base == warp * 32;
+        const bool act = base + lane < count;
+        const long long i = act ? base + lane : count - 1;
+        const long long is = base + lane;
+        const TfSample s = tf_sample(op, i);
+        const double tg = tm.tgt[cm_offset(op, tm.st_tgt, i)], w = tm.wgt[cm_offset(op, tm.st_wgt, i)];
+        const double2 n = nn[cm_offset(op, st_nn.st, i)];
+        double q = 0.0;
+        int arg = 0;
+#pragma unroll 1
+        for (int p = 0; p < NPOL; ++p) {
+            const int pol = NPOL == 2 ? p : op.pol;
+            const CmFwd f = cm_forward(op, s, pol, V0 + (long long)p * (N + 1) * pitch,
+                                       V1 + (long long)p * (N + 1) * pitch, pitch, is);
+            q += cm_quantity(tm, s, pol, f, nullptr, nullptr, pitch, is, &arg);
+        }
+        q = q / NPOL;
+        const double dq = 2.0 * w * (q - tg) / NPOL;
+        const double2 cosn = tf_cos_snell(s.n0, n, s.sin0);
+#pragma unroll 1
+        for (int p = 0; p < NPOL; ++p) {
+            const int pol = NPOL == 2 ? p : op.pol;
+            const double2* v0 = V0 + (long long)p * (N + 1) * pitch;
+            const double2* v1 = V1 + (long long)p * (N + 1) * pitch;
+            CmSeed sd;
+            double2 vb0, vb1;
+            cm_seed(tm, s, pol, cm_rt(s, pol, v0[is], v1[is]), dq, 0, v0, v1, pitch, is, sd, vb0, vb1);
+            // the needle generator G = dbeta/dd [[0, -i / eta_n], [-i eta_n, 0]]
+            const double2 eta_n = tf_admittance(n, cosn, pol);
+            const double2 gdn = cm_over(cmul(cscale(n, 2.0 * M_PI), cosn), s.wvl);
+            const double2 g01 = cmul(gdn, tf_div(make_double2(0.0, -1.0), eta_n));
+            const double2 g10 = cmul(gdn, cmul(make_double2(0.0, -1.0), eta_n));
+            for (int k = 0; k < N; ++k) {
+                const TfLayer L = tf_layer(op, s, k, pol);
+                const long long o1 = (long long)(k + 1) * pitch + is;
+                const double2 w0 = v0[o1], w1 = v1[o1];                         // v_{k+1}
+                const double2 dbdd = cm_over(cmul(cscale(L.n, 2.0 * M_PI), L.cost), s.wvl);
+                for (int j = zlist[k]; j < zlist[k + 1]; ++j) {
+                    const int zi = order[j];
+                    // M_bot (the part of layer k below z), G, then M_top
+                    double2 x0 = w0, x1 = w1, sb, cb;
+                    tf_sincos(cscale(dbdd, zpart[nz + zi]), &sb, &cb);
+                    tf_apply(sb, cb, L.eta, x0, x1);
+                    const double2 y0 = cmul(g01, x1), y1 = cmul(g10, x0);
+                    x0 = y0; x1 = y1;
+                    tf_sincos(cscale(dbdd, zpart[zi]), &sb, &cb);
+                    tf_apply(sb, cb, L.eta, x0, x1);
+                    cm_warp_add(cmulc(x0, vb0).x + cmulc(x1, vb1).x, act, lane, first && p == 0,
+                                partial + (long long)zi * W + warp);
+                }
+                double2 sb, cb;
+                tf_sincos(L.beta, &sb, &cb);
+                const double2 mis = make_double2(sb.y, -sb.x);
+                const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
+                const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
+                const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
+                vb0 = nb0; vb1 = nb1;
+            }
+        }
+    }
+}
+
 static int tf_ops(Handle* h, int pol, int nlayers, int ndim, const long long* shape, const long long* strides,
                   const void* const* in, TfOps& op, long long& count) {
     if (pol != PB_TF_POL_S && pol != PB_TF_POL_P) return fail(h, PB_ERR_INVALID, "thinfilm: pol must be PB_TF_POL_S or P");
@@ -506,6 +885,142 @@ extern "C" int pb_field_at_depth(pb_handle_t hh, int dtype, int pol, int nlayers
                                                               (const double2*)n, make_double2(n0_re, n0_im), wvl,
                                                               sin(theta0), pol, (const double2*)E_b, (const double2*)H_b,
                                                               (cplx<R>*)E, (cplx<R>*)H);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+// the term of a pb_coating_merit / pb_needle call: the six thin-film operands through tf_ops, then target and weight
+static int cm_setup(Handle* h, int quantity, int pol, int nlayers, int ndim, const long long* shape,
+                    const long long* strides, const void* const* in, TfOps& op, CmTerm& tm, long long& count) {
+    if (quantity < PB_CM_Q_R || quantity > PB_CM_Q_LAYER) return fail(h, PB_ERR_INVALID, "coating merit: bad quantity");
+    if (pol != PB_TF_POL_S && pol != PB_TF_POL_P && pol != PB_CM_POL_AVG)
+        return fail(h, PB_ERR_INVALID, "coating merit: pol must be PB_TF_POL_S, P or PB_CM_POL_AVG");
+    if (!in || !strides) return fail(h, PB_ERR_INVALID, "coating merit: missing operands");
+    PB_TRY(tf_ops(h, pol == PB_CM_POL_AVG ? PB_TF_POL_S : pol, nlayers, ndim, shape, strides, in, op, count));
+    if (!in[PB_CM_IN_TARGET] || !in[PB_CM_IN_WEIGHT]) return fail(h, PB_ERR_INVALID, "coating merit: missing target or weight");
+    tm.quantity = quantity;
+    tm.npol = pol == PB_CM_POL_AVG ? 2 : 1;
+    tm.tgt = (const double*)in[PB_CM_IN_TARGET];
+    tm.wgt = (const double*)in[PB_CM_IN_WEIGHT];
+    for (int j = 0; j < PB_TF_DIMS; ++j) {
+        const int src = j - (PB_TF_DIMS - ndim);
+        tm.st_tgt[j] = src >= 0 ? strides[5 * PB_CM_IN_TARGET + src] : 0;
+        tm.st_wgt[j] = src >= 0 ? strides[5 * PB_CM_IN_WEIGHT + src] : 0;
+    }
+    tm.cpad = (count + 31) / 32 * 32;
+    tm.b0 = tm.b1 = tm.nb = 0;
+    tm.blist = nullptr;
+    return PB_OK;
+}
+
+// the handle's scratch as nrows * W fp64 warp partials, then the stage of npol * (nlayers + 1) boundary vectors
+static int cm_scratch(Handle* h, const CmTerm& tm, int nlayers, long long nrows, long long W, double** partial,
+                      double2** V0, double2** V1) {
+    const size_t pbytes = ((size_t)nrows * W * sizeof(double) + 255) / 256 * 256;
+    const size_t vn = (size_t)tm.npol * (nlayers + 1) * tm.cpad;
+    void* base = nullptr;
+    PB_TRY(ensure_scratch(h, 2, pbytes + 2 * vn * sizeof(double2), &base));
+    *partial = (double*)base;
+    *V0 = (double2*)((char*)base + pbytes);
+    *V1 = *V0 + vn;
+    return PB_OK;
+}
+
+extern "C" int pb_coating_merit(pb_handle_t hh, int dtype, int quantity, int pol, int flags, int nlayers, int ndim,
+                                const long long* shape, const long long* strides, const void* const* in, int b0, int b1,
+                                const void* blist, int nb, void* value, void* residuals, void* grad, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (flags <= 0 || flags >= 2 * PB_CM_ACCUMULATE || !(flags & ~PB_CM_ACCUMULATE))
+        return fail(h, PB_ERR_INVALID, "coating merit: no output");
+    if ((flags & PB_CM_OUT_VALUE && !value) || (flags & PB_CM_OUT_RESIDUALS && !residuals) ||
+        (flags & (PB_CM_OUT_GRAD_THICKNESS | PB_CM_OUT_GRAD_INDEX) && !grad))
+        return fail(h, PB_ERR_INVALID, "coating merit: an output asked for is NULL");
+    TfOps op;
+    CmTerm tm;
+    long long count;
+    PB_TRY(cm_setup(h, quantity, pol, nlayers, ndim, shape, strides, in, op, tm, count));
+    const int nbound = quantity == PB_CM_Q_ABS ? nlayers : nlayers + 1;
+    if (quantity == PB_CM_Q_ABS || quantity == PB_CM_Q_ESQ || quantity == PB_CM_Q_LAYER) {
+        if (b0 < 0 || b0 >= nbound || (quantity == PB_CM_Q_LAYER && (b1 < 0 || b1 >= nbound)))
+            return fail(h, PB_ERR_INVALID, "coating merit: layer or boundary index out of range");
+    }
+    if (quantity == PB_CM_Q_PEAK && (nb < 1 || !blist)) return fail(h, PB_ERR_INVALID, "coating merit: no boundaries");
+    tm.b0 = b0;
+    tm.b1 = b1;
+    tm.nb = quantity == PB_CM_Q_PEAK ? nb : 0;
+    tm.blist = (const int*)blist;
+    const int kinds = (flags >> 2) & 3;
+    const bool acc = flags & PB_CM_ACCUMULATE;
+    const int ng = (kinds & 1) + (kinds >> 1 & 1);
+    if (count == 0) {
+        if (!acc && (flags & PB_CM_OUT_VALUE)) PB_CUDA(h, cudaMemsetAsync(value, 0, sizeof(double), st));
+        if (!acc && kinds && nlayers) PB_CUDA(h, cudaMemsetAsync(grad, 0, (size_t)ng * nlayers * rsize(dtype), st));
+        return PB_OK;
+    }
+    const int nt = cm_threads(tm.npol);
+    const int g = grid_for(count, nt, h->sm_count);
+    const long long W = (long long)g * (nt / 32);
+    const long long nw = std::min<long long>(W, (count + 31) / 32);
+    double* partial;
+    double2 *V0, *V1;
+    PB_TRY(cm_scratch(h, tm, nlayers, 2LL * nlayers + 1, W, &partial, &V0, &V1));
+    if (tm.npol == 2) coating_merit_kernel<2><<<g, nt, 0, st>>>(op, tm, count, flags, V0, V1, partial, residuals,
+                                                                dtype == PB_C64);
+    else coating_merit_kernel<1><<<g, nt, 0, st>>>(op, tm, count, flags, V0, V1, partial, residuals, dtype == PB_C64);
+    PB_LAUNCH_CHECK(h);
+    if (!(flags & PB_CM_OUT_VALUE) && !(kinds && nlayers)) return PB_OK;
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        coating_merit_reduce_kernel<R><<<2 * nlayers + 1, PB_TF_THREADS, 0, st>>>(partial, W, nw, nlayers, flags,
+                                                                                   (double*)value, (R*)grad);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+extern "C" int pb_needle(pb_handle_t hh, int dtype, int quantity, int pol, int nlayers, int ndim, const long long* shape,
+                         const long long* strides, const void* const* in, const void* zpart, long long nz,
+                         const void* zlist, void* P, int accumulate, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (quantity != PB_CM_Q_R && quantity != PB_CM_Q_T)
+        return fail(h, PB_ERR_INVALID, "needle: the term must target R or T");
+    if (nlayers < 1) return fail(h, PB_ERR_INVALID, "needle: at least one layer");
+    if (nz < 0 || (nz && (!zpart || !zlist || !P))) return fail(h, PB_ERR_INVALID, "bad needle arguments");
+    TfOps op;
+    CmTerm tm;
+    long long count;
+    PB_TRY(cm_setup(h, quantity, pol, nlayers, ndim, shape, strides, in, op, tm, count));
+    if (!in[PB_CM_IN_NEEDLE]) return fail(h, PB_ERR_INVALID, "needle: missing needle index");
+    if (nz == 0) return PB_OK;
+    if (count == 0) {
+        if (!accumulate) PB_CUDA(h, cudaMemsetAsync(P, 0, (size_t)nz * rsize(dtype), st));
+        return PB_OK;
+    }
+    long long st_nn[PB_TF_DIMS];
+    for (int j = 0; j < PB_TF_DIMS; ++j) {
+        const int src = j - (PB_TF_DIMS - ndim);
+        st_nn[j] = src >= 0 ? strides[5 * PB_CM_IN_NEEDLE + src] : 0;
+    }
+    const int nt = cm_threads(tm.npol);
+    const int g = grid_for(count, nt, h->sm_count);
+    const long long W = (long long)g * (nt / 32);
+    const long long nw = std::min<long long>(W, (count + 31) / 32);
+    double* partial;
+    double2 *V0, *V1;
+    PB_TRY(cm_scratch(h, tm, nlayers, nz, W, &partial, &V0, &V1));
+    NeedleStrides ns;
+    for (int j = 0; j < PB_TF_DIMS; ++j) ns.st[j] = st_nn[j];
+    auto launch = [&](auto kern) {
+        kern<<<g, nt, 0, st>>>(op, tm, (const double2*)in[PB_CM_IN_NEEDLE], ns, count, (const double*)zpart, nz,
+                                          (const int*)zlist, V0, V1, partial);
+    };
+    if (tm.npol == 2) launch(needle_kernel<2>);
+    else launch(needle_kernel<1>);
+    PB_LAUNCH_CHECK(h);
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        needle_reduce_kernel<R><<<(unsigned)nz, PB_TF_THREADS, 0, st>>>(partial, W, nw, accumulate, (R*)P);
     });
     PB_LAUNCH_CHECK(h);
     return PB_OK;

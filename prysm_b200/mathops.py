@@ -53,6 +53,8 @@ _CORONAGRAPH_FUNCS = (
 )
 _COATINGS_STACK_FUNCS = ('stack_rt', 'RTA', 'internal_fields', 'field_at_depth')
 _COATINGS_DIFF_FUNCS = ('forward_eval', 'ForwardEval', 'thickness_gradient', 'index_gradient')
+_COATINGS_MERIT_NAMES = ('Reflectance', 'Transmittance', 'LayerAbsorptance', 'FieldIntensityAtBoundary',
+                         'PeakFieldAtInterfaces', 'FieldInLayer', 'MeritFunction', 'as_merit')
 _TARGETS = {
     'prysm.propagation.fft': {n: getattr(_prop, n) for n in ('focus', 'unfocus', 'focus_adjoint', 'unfocus_adjoint')},
     'prysm.propagation.angular_spectrum': {n: getattr(_prop, n) for n in (
@@ -101,12 +103,21 @@ _TARGETS = {
     'prysm.bayer': {n: getattr(_bayer, n) for n in (
         'wb_prescale', 'wb_postscale', 'composite_bayer', 'decomposite_bayer', 'recomposite_bayer',
         'demosaic_deinterlace', 'assemble_superresolved', 'demosaic_malvar')},
-    # thin films: merit, problem, needle and monitoring bind these names at import time and do numpy arithmetic on
-    # the results, so they keep the reference's host engine
+    # thin films.  The merit terms and the needle function run on the device.  The reference's refine, CoatingProblem
+    # and synthesize bind as_merit, the gradients and needle_function at import time and feed the results to host
+    # optimizer loops, so in those modules the names are re-bound to variants that hand back numpy (the evaluation is
+    # still on the device); insert_needle, cleanup and the optimizers stay the reference's.  monitoring keeps the
+    # reference's host engine.
     'prysm.thinfilm': {'multilayer_stack_rt': _tf.multilayer_stack_rt},
-    'prysm.x.coatings': {n: getattr(_coat, n) for n in _COATINGS_STACK_FUNCS + _COATINGS_DIFF_FUNCS},
+    'prysm.x.coatings': {n: getattr(_coat, n) for n in
+                         _COATINGS_STACK_FUNCS + _COATINGS_DIFF_FUNCS + _COATINGS_MERIT_NAMES + ('needle_function',)},
     'prysm.x.coatings.stack': {n: getattr(_coat, n) for n in _COATINGS_STACK_FUNCS},
     'prysm.x.coatings.diff': {n: getattr(_coat, n) for n in _COATINGS_DIFF_FUNCS},
+    'prysm.x.coatings.merit': {n: getattr(_coat, n) for n in _COATINGS_MERIT_NAMES},
+    'prysm.x.coatings.problem': {'as_merit': _coat._host_as_merit, 'thickness_gradient': _coat.thickness_gradient,
+                                 'index_gradient': _coat.index_gradient},
+    'prysm.x.coatings.refine': {'as_merit': _coat._host_as_merit},
+    'prysm.x.coatings.needle': {'as_merit': _coat._host_as_merit, 'needle_function': _coat._host_needle_function},
 }
 
 _saved = {}  # (module name, attribute) -> original
