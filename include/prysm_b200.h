@@ -832,6 +832,65 @@ int pb_polar_crossings(pb_handle_t h, int type, const void* data, int ny, int nx
 int pb_analytic_radial(pb_handle_t h, int in_type, int out_type, int kind, const void* x, long long count, double a,
                        double b, void* out, void* stream);
 
+/* ---- Interferometric metrology (prysm/interferogram.py, prysm/util.py, prysm/polynomials/fitting.py lstsq) ----------
+ * Real data of dtype's real type (PB_C64: fp32, PB_C128: fp64), dense (ny, nx) or n elements.  Every reduction
+ * accumulates in fp64 and folds per-block partials in block order in the last block to finish (an integer arrival
+ * counter in the handle's scratch, no float atomics), so repeated calls give the same bits.
+ * pb_nan_stats: res (DEVICE, 9 fp64) = finite count, sum, min, max and sum of squares of the finite values, NaN count,
+ *   mean, then sum |x - mean| and sum (x - mean)^2 over the finite values (pass 2 reads the mean from res).  Two launches.
+ * pb_masked_gram: modes (HOST array of k device pointers, NULL = the constant 1), each n elements; data n elements with
+ *   NaN (or inf) for pixels to ignore.  out (DEVICE, fp64) = the packed row-major upper triangle of the (k+1) x (k+1)
+ *   matrix [A d]^T [A d] over the finite pixels: A^T A, then A^T d in column k, and d^T d last.  1 <= k <= PB_GRAM_MAX_K.
+ *   One launch.
+ * pb_psd_prologue: the window w of make_window (PB_WIN_WELCH: 1 - |hypot(x, y) / rmax|^alpha on the fftrange * dx grid;
+ *   PB_WIN_HANN: np.outer(np.hanning(ny), np.hanning(nx)); PB_WIN_USER: the array `user`; PB_WIN_AUTO: Welch when every
+ *   sample of the four corner rectangles (HOST int[16], (y0, y1, x0, x1) each) is == 0, else Hann, decided on the
+ *   device into flags (DEVICE int[4])).  Writes `window` = w and / or `shifted` = fftshift(height * w) (either may be
+ *   NULL) and s2 (DEVICE fp64) = sum w^2.  One launch, two for PB_WIN_AUTO.
+ * pb_psd_epilogue: psd = ifftshift(|F|^2) / (s2 fs^2) for the complex (ny, nx) F = pb_fft2 of `shifted`.  One launch.
+ * pb_band_trapz: res (DEVICE fp64) = sum_ij wy_i wx_j psd_ij over the samples with flow <= r_ij <= fhigh, w = 1/2 on the
+ *   edges of an axis (0 for an axis of one sample), the trapezoid of bandlimited_rms without its dx^2; r is the array r
+ *   or, when r is NULL, hypot(fx[j], fy[i]) of the fp64 axes.  twod = 0: one trapezoid along the ny axis (nx = 1).
+ * pb_filter_h: out0 (and out1, with fcn1) = the factors `parts` (PB_FILT_*) asks for: W = hann2d(ny, nx), H =
+ *   ideal_lpf_iir2d(r, dx, fcn).  One launch.
+ * pb_filter_apply: H from the complex transforms Hl (and Hh) by typ (PB_FILT_LOWPASS |Hl|, HIGHPASS 1 - |Hl|, BANDPASS
+ *   1 - ((1 - |Hh|) + |Hl|), BANDREJECT (1 - |Hh|) + |Hl|); D *= H in place, or with D NULL H into the real Hout.
+ * pb_gradient2d: gx, gy = np.gradient(f, dx) (central inside, one-sided first order on the edges) and gr = hypot(gx, gy);
+ *   ny, nx >= 2.  One launch.
+ * pb_finite_bounds: box (HOST int[4]) = max(ny - i), max(i + 1), max(nx - j), max(j + 1) over the finite samples (all 0
+ *   when there is none).  One launch; the call waits for it.
+ * pb_metro_pointwise: out (may be x) = PB_PW_FILL NaN -> a; KEEP NaN where the byte mask m is 0; CLIP NaN where |x| > a;
+ *   RADIUS NaN where u / a > 1; SUB x - (a u + b v) (u NULL = 1, v NULL = 0); RHO2 rho^2 of np.linspace(-1, 1) axes whose steps
+ *   2 / (n - 1) are a (x) and b (y), x unused; REAL the real part of the complex x; AXPBY a u + b v (v NULL = 0, x unused); DIV x / a; WELCH
+ *   1 - |x / a|^b.  One launch. */
+typedef enum { PB_GRAM_MAX_K = 64 } pb_gram_limit;
+typedef enum { PB_WIN_AUTO = 0, PB_WIN_WELCH = 1, PB_WIN_HANN = 2, PB_WIN_USER = 3 } pb_window_kind;
+typedef enum { PB_FILT_W = 1, PB_FILT_H = 2 } pb_filter_part;
+typedef enum { PB_FILT_LOWPASS = 0, PB_FILT_HIGHPASS = 1, PB_FILT_BANDPASS = 2, PB_FILT_BANDREJECT = 3 } pb_filter_type;
+typedef enum {
+    PB_PW_FILL = 0, PB_PW_KEEP = 1, PB_PW_CLIP = 2, PB_PW_RADIUS = 3, PB_PW_SUB = 4, PB_PW_RHO2 = 5, PB_PW_REAL = 6,
+    PB_PW_AXPBY = 7, PB_PW_DIV = 8, PB_PW_WELCH = 9
+} pb_pointwise_op;
+int pb_nan_stats(pb_handle_t h, int dtype, const void* x, long long n, double* res, void* stream);
+int pb_masked_gram(pb_handle_t h, int dtype, const void* const* modes, int k, const void* data, long long n, double* out,
+                   void* stream);
+int pb_psd_prologue(pb_handle_t h, int dtype, const void* height, int ny, int nx, int kind, const void* user, double dx,
+                    double alpha, double rmax, const int* corners, void* shifted, void* window, double* s2, int* flags,
+                    void* stream);
+int pb_psd_epilogue(pb_handle_t h, int dtype, const void* F, int ny, int nx, const double* s2, double fs, void* psd,
+                    void* stream);
+int pb_band_trapz(pb_handle_t h, int dtype, const void* psd, const void* r, const double* fx, const double* fy, int ny,
+                  int nx, int twod, double flow, double fhigh, double* res, void* stream);
+int pb_filter_h(pb_handle_t h, int dtype, const void* r, int ny, int nx, int parts, double dx, double fcn0, double fcn1,
+                void* out0, void* out1, void* stream);
+int pb_filter_apply(pb_handle_t h, int dtype, void* D, const void* Hl, const void* Hh, long long n, int typ, void* Hout,
+                    void* stream);
+int pb_gradient2d(pb_handle_t h, int dtype, const void* f, int ny, int nx, double dx, void* gx, void* gy, void* gr,
+                  void* stream);
+int pb_finite_bounds(pb_handle_t h, int dtype, const void* x, int ny, int nx, int* box, void* stream);
+int pb_metro_pointwise(pb_handle_t h, int dtype, int op, const void* x, const void* u, const void* v, const void* m,
+                       int ny, int nx, double a, double b, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,6 +24,8 @@ Mirrors the reference's module layout for the path only:
                             ShackHartmann sensor with a modal reconstructor are engine extensions)
     prysm_b200.thinfilm / .coatings  <-> prysm.thinfilm.multilayer_stack_rt, prysm.x.coatings (stack_rt, RTA, internal
                             and depth fields, forward_eval with thickness and index gradients)
+    prysm_b200.util / .interferogram  <-> prysm.util statistics, prysm.interferogram (NaN-aware statistics, masked least
+                            squares, PSD and windows, band-limited RMS, filters, slopes and Interferogram's metrology)
     prysm_b200.graphs       CUDA-graph capture of launch-bound compositions (no reference counterpart)
 Every array operation is a call into libprysm_b200.so (hand-written sm_90a CUDA behind the C ABI
 of include/prysm_b200.h).  Importing this package without the built library raises ImportError.
@@ -32,7 +34,7 @@ from . import _capi  # noqa: F401  (fails loudly if the CUDA library is missing)
 from .conf import config  # noqa: F401
 from . import fttools, propagation, coronagraph, otf, psf, polynomials, polychromatic, mathops, graphs  # noqa: F401
 from . import coordinates, geometry, convolution, detector, dm, segmented, polarization  # noqa: F401
-from . import fibers, sri, pdi, psi, bayer, shack_hartmann, qpoly, thinfilm, coatings  # noqa: F401
+from . import fibers, sri, pdi, psi, bayer, shack_hartmann, qpoly, thinfilm, coatings, util, interferogram  # noqa: F401
 from ._capi import B200Error  # noqa: F401
 from .propagation import Wavefront  # noqa: F401
 from ._ops import asdevice, asnumpy, set_device  # noqa: F401

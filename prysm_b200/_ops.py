@@ -1562,6 +1562,171 @@ def analytic_radial(kind, x, a, b, out_dtype):
     return out
 
 
+# ---- interferometric metrology (pb_nan_stats ... pb_metro_pointwise) --------------------------------------------------
+def metro_data(data):
+    """data as a dense real CUDA tensor the metrology entry points take (fp32 / fp64; anything else is refused)"""
+    if not isinstance(data, torch.Tensor) or not data.is_cuda:
+        raise ValueError('metrology data must be a CUDA tensor')
+    if data.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f'metrology data of {data.dtype} is not supported (torch.float32, torch.float64)')
+    return data.contiguous()
+
+
+def nan_stats(x):
+    """(9,) fp64 host array: finite count, sum, min, max, sum of squares, NaN count, mean, sum |x - mean|,
+    sum (x - mean)^2 over the finite values of x (pb_nan_stats: two launches, one copy to the host)."""
+    x = metro_data(x)
+    res = torch.empty(9, dtype=torch.float64, device=x.device)
+    _call(lib.pb_nan_stats, x, _CODE[x.dtype], _p(x), x.numel(), _p(res))
+    return res.cpu().numpy()
+
+
+def masked_gram(modes, data):
+    """The packed upper triangle of [A d]^T [A d] over the finite pixels of data (pb_masked_gram), as a host fp64
+    array; modes is a sequence of tensors shaped like data (dtype data's), None for the constant 1."""
+    data = metro_data(data)
+    k = len(modes)
+    if not 1 <= k <= capi.GRAM_MAX_K:
+        raise ValueError(f'a masked least-squares fit takes 1 to {capi.GRAM_MAX_K} modes, got {k}')
+    keep = [None if m is None else m.to(data.dtype).contiguous() for m in modes]
+    for m in keep:
+        if m is not None and m.numel() != data.numel():
+            raise ValueError(f'mode of {m.numel()} samples against data of {data.numel()}')
+    ptrs = (C.c_void_p * k)(*[None if m is None else m.data_ptr() for m in keep])
+    out = torch.empty((k + 1) * (k + 2) // 2, dtype=torch.float64, device=data.device)
+    _call(lib.pb_masked_gram, data, _CODE[data.dtype], C.cast(ptrs, C.POINTER(C.c_void_p)), k, _p(data), data.numel(),
+          _p(out))
+    return out.cpu().numpy()
+
+
+def _same_shape(name, t, shape):
+    """refuse an operand the kernel would index densely over `shape` but which has another shape"""
+    if t is not None and tuple(t.shape) != tuple(shape):
+        raise ValueError(f'{name} of shape {tuple(t.shape)} does not match the data shape {tuple(shape)}')
+
+
+def psd_prologue(height, kind, user=None, dx=1.0, alpha=4.0, rmax=1.0, corners=None, want_shifted=True,
+                 want_window=False, shape=None, dtype=None):
+    """(shifted, window, s2) of pb_psd_prologue: fftshift(height * w) and / or w (None where not asked for), and the
+    device fp64 scalar sum w^2.  A user window must have height's shape."""
+    like = height if height is not None else user
+    if height is not None:
+        _same_shape('window', user, height.shape)
+        height = metro_data(height)
+        shape, dtype = height.shape, height.dtype
+    ny, nx = shape
+    dev = device() if like is None else like.device
+    if user is not None:
+        user = user.to(dtype).contiguous()
+    shifted = torch.empty((ny, nx), dtype=dtype, device=dev) if want_shifted else None
+    window = torch.empty((ny, nx), dtype=dtype, device=dev) if want_window else None
+    s2 = torch.empty(1, dtype=torch.float64, device=dev)
+    flags = torch.empty(4, dtype=torch.int32, device=dev)
+    cor, cp = _iarr(np.zeros(16) if corners is None else corners)
+    _call(lib.pb_psd_prologue, s2, _CODE[dtype], _p(height), ny, nx, int(kind), _p(user), float(dx), float(alpha),
+          float(rmax), cp if corners is not None else None, _p(shifted), _p(window), _p(s2), _p(flags))
+    return shifted, window, s2
+
+
+def psd_epilogue(F, s2, fs):
+    """ifftshift(|F|^2) / (s2 fs^2) (pb_psd_epilogue) of the complex transform F."""
+    ny, nx = F.shape
+    out = torch.empty((ny, nx), dtype=_REAL_OF[F.dtype], device=F.device)
+    _call(lib.pb_psd_epilogue, F, _CODE[F.dtype], _p(F), ny, nx, _p(s2), float(fs), _p(out))
+    return out
+
+
+def band_trapz(psd, r=None, fx=None, fy=None, flow=0.0, fhigh=np.inf):
+    """sum w_i w_j psd over flow <= r <= fhigh with trapezoid edge weights (pb_band_trapz), a host float; r is an
+    array like psd or None for hypot of the fp64 axes fx, fy.  1-D psd: one trapezoid."""
+    _same_shape('r', r, psd.shape)
+    psd = metro_data(psd)
+    twod = psd.ndim == 2
+    if twod and r is None and (fx.numel() != psd.shape[1] or fy.numel() != psd.shape[0]):
+        raise ValueError(f'frequency axes of {fx.numel()} and {fy.numel()} samples for a PSD of shape {tuple(psd.shape)}')
+    ny, nx = psd.shape if twod else (psd.numel(), 1)
+    if r is not None:
+        r = r.to(psd.dtype).contiguous()
+    res = torch.empty(1, dtype=torch.float64, device=psd.device)
+    _call(lib.pb_band_trapz, psd, _CODE[psd.dtype], _p(psd), _p(r), _p(fx), _p(fy), ny, nx, int(twod), float(flow),
+          float(fhigh), _p(res))
+    return float(res.cpu()[0])
+
+
+def filter_h(shape, parts, dtype, dev, r=None, dx=1.0, fcn0=0.0, fcn1=None):
+    """hann2d (FILT_W), ideal_lpf_iir2d (FILT_H) or their product over shape (pb_filter_h); with fcn1 a second array
+    at that cut-off from the same launch."""
+    ny, nx = shape
+    _same_shape('r', r, shape)
+    if r is not None:
+        r = r.to(dtype).contiguous()
+    out0 = torch.empty((ny, nx), dtype=dtype, device=dev)
+    out1 = torch.empty((ny, nx), dtype=dtype, device=dev) if fcn1 is not None else None
+    _call(lib.pb_filter_h, out0, _CODE[dtype], _p(r), ny, nx, int(parts), float(dx), float(fcn0),
+          float(0.0 if fcn1 is None else fcn1), _p(out0), _p(out1))
+    return out0, out1
+
+
+def filter_apply(typ, Hl, Hh=None, D=None):
+    """D *= H in place (returns D), or with D None the real H (pb_filter_apply)."""
+    for t in (Hh, D):
+        if t is not None and (t.dtype != Hl.dtype or t.shape != Hl.shape):
+            raise ValueError(f'filter transforms of {t.dtype} {tuple(t.shape)} and {Hl.dtype} {tuple(Hl.shape)} differ')
+    Hout = None if D is not None else torch.empty(Hl.shape, dtype=_REAL_OF[Hl.dtype], device=Hl.device)
+    _call(lib.pb_filter_apply, Hl, _CODE[Hl.dtype], _p(D), _p(Hl), _p(Hh), Hl.numel(), int(typ), _p(Hout))
+    return D if D is not None else Hout
+
+
+def gradient2d(f, dx):
+    """(gx, gy, hypot(gx, gy)) of np.gradient(f, dx) (pb_gradient2d)."""
+    f = metro_data(f)
+    ny, nx = f.shape
+    if ny < 2 or nx < 2:
+        raise ValueError('Shape of array too small to calculate a numerical gradient, at least (edge_order + 1) '
+                         'elements are required.')
+    gx, gy, gr = (torch.empty_like(f) for _ in range(3))
+    _call(lib.pb_gradient2d, f, _CODE[f.dtype], _p(f), ny, nx, float(dx), _p(gx), _p(gy), _p(gr))
+    return gx, gy, gr
+
+
+def finite_bounds(x):
+    """(first finite row, rows after the last finite one, first finite column, columns after the last finite one);
+    all zero without a finite sample (pb_finite_bounds, one launch, the call waits)."""
+    x = metro_data(x)
+    ny, nx = x.shape
+    box = (C.c_int * 4)()
+    _call(lib.pb_finite_bounds, x, _CODE[x.dtype], _p(x), ny, nx, box)
+    if box[0] == 0:
+        return 0, 0, 0, 0
+    return ny - box[0], ny - box[1], nx - box[2], nx - box[3]
+
+
+def metro_pointwise(op, x=None, u=None, v=None, m=None, a=0.0, b=0.0, out=None, shape=None, dtype=None):
+    """One PW_* op of pb_metro_pointwise; out may be x (in place).  u, v are cast to the output's dtype."""
+    like = x if x is not None else u
+    if dtype is None:
+        dtype = _REAL_OF.get(like.dtype, like.dtype) if like is not None else None
+    if shape is None:
+        shape = like.shape
+    dev = like.device if like is not None else device()
+    n = int(np.prod(shape))
+    for name, t, want in (('data', x, 2 * n if op == capi.PW_REAL else n), ('u', u, n), ('v', v, n), ('mask', m, n)):
+        if t is not None and t.numel() != want:
+            raise ValueError(f'{name} of {t.numel()} elements for an operation over {want} (shape {tuple(shape)})')
+    if x is not None:
+        x = x.contiguous()
+    u = None if u is None else u.to(dtype).contiguous()
+    v = None if v is None else v.to(dtype).contiguous()
+    if m is not None:
+        m = m.contiguous()
+        m = m.view(torch.uint8) if m.dtype == torch.bool else m.to(torch.uint8)
+    out = _out(out, tuple(shape), dtype, dev)
+    ny, nx = (shape[0], shape[1]) if len(shape) == 2 else (1, int(np.prod(shape)))
+    _call(lib.pb_metro_pointwise, out, _CODE[dtype], int(op), _p(x), _p(u), _p(v), _p(m), ny, nx, float(a), float(b),
+          _p(out))
+    return out
+
+
 def launch_count(dev=None):
     dev = device() if dev is None else torch.device(dev)
     return capi.launch_count(dev.index)

@@ -18,6 +18,11 @@ touches numpy `exp` or eager tensor arithmetic.
 The reference's `RichData` class gets `slices`, `exact_polar`, `exact_xy`, `exact_x` and `exact_y` that run on the
 device when its `data` is a CUDA tensor (what the re-bound `mtf_from_psf` returns) and call the originals otherwise.
 
+Interferometric metrology follows the same rule, because the reference's host `Interferogram` must behave exactly as
+before: the free functions of prysm.interferogram, prysm.util's statistics and prysm.polynomials' lstsq are re-bound to
+dispatchers that run the engine when their data argument is a CUDA tensor and call the original otherwise, and the
+reference's `Interferogram` class gets its metrology properties and methods patched the same way.
+
 `set_backend_to_defaults()` restores every name it replaced.
 """
 import importlib
@@ -30,6 +35,7 @@ from . import detector as _det
 from . import dm as _dm
 from . import fibers as _fib
 from . import fttools as _ft
+from . import interferogram as _ifg
 from . import otf as _otf
 from . import pdi as _pdi
 from . import polarization as _pol
@@ -119,6 +125,26 @@ _TARGETS = {
     'prysm.x.coatings.refine': {'as_merit': _coat._host_as_merit},
     'prysm.x.coatings.needle': {'as_merit': _coat._host_as_merit, 'needle_function': _coat._host_needle_function},
 }
+
+# names that run the engine only when their data argument (name, position) is a CUDA tensor: module -> {attribute:
+# (engine function, argument name, position)}
+_STATS = {n: (getattr(_ifg, n), 'array', 0) for n in ('mean', 'pv', 'rms', 'Sa', 'std')}
+_LSTSQ = {'lstsq': (_poly.lstsq, 'data', 1)}
+_DISPATCHED = {
+    'prysm.interferogram': {**_STATS, **_LSTSQ, 'fit_plane': (_ifg.fit_plane, 'z', 2),
+                            'fit_sphere': (_ifg.fit_sphere, 'z', 0), 'make_window': (_ifg.make_window, 'signal', 0),
+                            'psd': (_ifg.psd, 'height', 0), 'bandlimited_rms': (_ifg.bandlimited_rms, 'psd', 1),
+                            'window_2d_welch': (_ifg.window_2d_welch, 'r', 0),
+                            'ideal_lpf_iir2d': (_ifg.ideal_lpf_iir2d, 'r', 0),
+                            'designfilt2d': (_ifg.designfilt2d, 'r', 0)},
+    'prysm.util': _STATS,
+    'prysm.polynomials': _LSTSQ,
+    'prysm.polynomials.fitting': _LSTSQ,
+}
+_IFG_PROPERTIES = ('dropout_percentage', 'pv', 'rms', 'Sa', 'std', 'strehl')
+_IFG_METHODS = ('pvr', 'fill', 'crop', 'recenter', 'remove_piston', 'remove_tiptilt', 'remove_power', 'mask',
+                'strip_latcal', 'latcal', 'pad', 'spike_clip', 'psd', 'filter', 'bandlimited_rms',
+                'total_integrated_scatter', 'slope')
 
 _saved = {}  # (module name, attribute) -> original
 _saved_cls = {}  # (class, attribute) -> original descriptor (or _MISSING)
@@ -261,6 +287,121 @@ def _patch_richdata_class():
             setattr(cls, name, fn)
 
 
+def _on_device(v):
+    import torch
+    return isinstance(v, torch.Tensor) and v.is_cuda
+
+
+def _dispatch(engine, orig, argname, pos):
+    """orig with the engine in its place when the data argument is a CUDA tensor; reference RichData results"""
+    import functools
+    eng = _returning_reference_richdata(engine)
+
+    @functools.wraps(orig)
+    def f(*args, **kwargs):
+        v = args[pos] if len(args) > pos else kwargs.get(argname)
+        return eng(*args, **kwargs) if _on_device(v) else orig(*args, **kwargs)
+    f.__wrapped_engine__ = engine
+    return f
+
+
+def _with_reference_mode_sum(fn):
+    """A copy of the reference function fn whose call-time `from prysm.polynomials import ...` sees the reference's own
+    sum_of_2d_modes.  The reference's host pvr imports it at call time, and the engine's (numpy in, CUDA out), which
+    the backend binds in prysm.polynomials, would put its projection on the device.  The copy has its own globals and
+    import, so nothing shared is swapped while it runs."""
+    import builtins
+    import types
+    key = ('prysm.polynomials', 'sum_of_2d_modes')
+    if key not in _saved:
+        return fn
+    view = types.ModuleType(key[0])
+    view.__dict__.update(importlib.import_module(key[0]).__dict__)
+    view.sum_of_2d_modes = _saved[key]
+
+    def imp(name, globals=None, locals=None, fromlist=(), level=0):
+        if name == key[0] and fromlist and level == 0:
+            return view
+        return builtins.__import__(name, globals, locals, fromlist, level)
+    g = dict(fn.__globals__)
+    g['__builtins__'] = {**builtins.__dict__, '__import__': imp}
+    return types.FunctionType(fn.__code__, g, fn.__name__, fn.__defaults__, fn.__closure__)
+
+
+def _interferogram_patches():
+    """Members that replace the metrology of the reference's Interferogram class: with a CUDA tensor as `data` they run
+    the engine's Interferogram on the same data, dx and cached coordinates and write the results back (methods change
+    the object and return it, as the reference's do); otherwise they call the reference's original."""
+    from ._richdata import RichData as _OurRich
+    ref = importlib.import_module('prysm.interferogram').Interferogram
+    ref_rich = importlib.import_module('prysm._richdata').RichData
+    coords = ('_x', '_y', '_r', '_t')
+
+    def to_ours(self, with_coords=True):
+        """the engine's object on the same data; with_coords: the cached coordinates too (host ones are uploaded once:
+        back() leaves the device copies in the reference object)"""
+        o = _ifg.Interferogram.__new__(_ifg.Interferogram)
+        o.dx, o.wavelength, o._data = self.dx, self.wavelength, _ifg._real(self.data)
+        for c in coords:
+            v = getattr(self, c, None) if with_coords else None
+            setattr(o, c, None if v is None else _ifg._ops.asdevice(v))
+        o.intensity, o.meta, o._latcaled = self.intensity, self.meta, getattr(self, '_latcaled', False)
+        return o
+
+    def back(self, o):
+        self._data, self.dx, self._latcaled = o._data, o.dx, o._latcaled
+        self.interpf_x = self.interpf_y = self.interpf_2d = None
+        for c in coords:
+            setattr(self, c, getattr(o, c))
+
+    def conv(v):
+        if isinstance(v, _OurRich):
+            r = ref_rich(v.data, v.dx, v.wavelength)
+            for c in coords:
+                setattr(r, c, getattr(v, c))
+            r._default_twosided = v._default_twosided
+            return r
+        if isinstance(v, tuple):
+            return tuple(conv(e) for e in v)
+        return v
+
+    def method(name):
+        orig = getattr(ref, name)
+        host = _with_reference_mode_sum(orig) if name == 'pvr' else orig
+
+        def f(self, *args, **kwargs):
+            if not _on_device(self.data):
+                return host(self, *args, **kwargs)
+            o = to_ours(self)
+            r = getattr(o, name)(*args, **kwargs)
+            back(self, o)
+            return self if r is o else conv(r)
+        f.__name__ = name
+        f.__doc__ = orig.__doc__
+        return f
+
+    def prop(name):
+        orig = ref.__dict__[name]
+        # the statistics read no coordinates
+        return property(lambda self: getattr(to_ours(self, False), name) if _on_device(self.data) else orig.fget(self),
+                        doc=orig.__doc__)
+
+    out = {n: prop(n) for n in _IFG_PROPERTIES}
+    out.update({n: method(n) for n in _IFG_METHODS})
+    return ref, out
+
+
+def _patch_interferogram_class():
+    try:
+        cls, patches = _interferogram_patches()
+    except ImportError:
+        return
+    for name, fn in patches.items():
+        if (cls, name) not in _saved_cls:
+            _saved_cls[(cls, name)] = cls.__dict__.get(name, _MISSING)
+            setattr(cls, name, fn)
+
+
 def set_backend_to_b200(device=None):
     """Route prysm's propagation hot path through the H100 engine.  Call after `import prysm`
     (like the reference's own set_backend_to_* helpers).  Arrays handed to the re-bound functions may be
@@ -278,12 +419,14 @@ def set_backend_to_b200(device=None):
     # import every target before re-binding any: a module imported mid-way (prysm.x.dm binds fourier_resample,
     # apply_transfer_functions and warp at import time) would otherwise capture engine functions as its defaults
     mods = {}
-    for modname in _TARGETS:
+    for modname in [*_TARGETS, *_DISPATCHED]:
         try:
             mods[modname] = importlib.import_module(modname)
         except ImportError:
             continue
     for modname, mod in mods.items():
+        if modname not in _TARGETS:
+            continue
         repl = _TARGETS[modname]
         if modname in ('prysm.otf', 'prysm.x.psi'):   # these return RichData: hand back the reference's own container
             repl = {k: _returning_reference_richdata(v) for k, v in repl.items()}
@@ -292,8 +435,19 @@ def set_backend_to_b200(device=None):
                 _saved[(modname, attr)] = getattr(mod, attr)
             if hasattr(mod, attr):
                 setattr(mod, attr, new)
+    for modname, names in _DISPATCHED.items():
+        try:
+            mod = importlib.import_module(modname)
+        except ImportError:
+            continue
+        for attr, (engine, argname, pos) in names.items():
+            if not hasattr(mod, attr) or (modname, attr) in _saved:
+                continue
+            _saved[(modname, attr)] = orig = getattr(mod, attr)
+            setattr(mod, attr, _dispatch(engine, orig, argname, pos))
     _patch_wavefront_class()
     _patch_richdata_class()
+    _patch_interferogram_class()
     return sorted(_saved)
 
 

@@ -35,6 +35,31 @@ def sum_of_2d_modes_adjoint(modes, databar):
     return _ops.mode_projection(modes, _ops.asdevice(databar))
 
 
+def lstsq(modes, data):
+    """Least-squares fit of modes to data, ignoring the pixels where data is not finite (prysm/polynomials/fitting.py:
+    103-126).  One launch (pb_masked_gram) reduces [A d]^T [A d] over the finite pixels in fp64 with no compaction;
+    the (k, k) system is solved on the host with numpy.linalg.lstsq, whose minimum-norm answer equals pinv(A) d, so a
+    rank-deficient basis gets the reference's answer.  The normal equations square the condition number of A.  modes:
+    a (k, ...) array or a sequence of k arrays shaped like data, 1 <= k <= 64.  Returns the (k,) fp64 host array."""
+    data = _ops.asdevice(data)
+    if data.dtype not in (torch.float32, torch.float64):
+        data = data.to(torch.float64)
+    if isinstance(modes, torch.Tensor) or hasattr(modes, 'shape'):
+        modes = _ops.asdevice(modes)
+        mlist = [modes[k].reshape(-1) for k in range(modes.shape[0])]
+    else:
+        mlist = [None if m is None else _ops.asdevice(m).reshape(-1) for m in modes]
+    return solve_gram(_ops.masked_gram(mlist, data.reshape(-1)), len(mlist))
+
+
+def solve_gram(packed, k):
+    """numpy.linalg.lstsq of the normal equations held in the packed triangle pb_masked_gram writes"""
+    full = np.zeros((k + 1, k + 1))
+    full[np.triu_indices(k + 1)] = packed
+    G = np.triu(full[:k, :k]) + np.triu(full[:k, :k], 1).T
+    return np.linalg.lstsq(G, full[:k, k], rcond=None)[0]
+
+
 # ------------------------------------------------------------------------------------------
 # Jacobi / Zernike by recurrence
 # ------------------------------------------------------------------------------------------
