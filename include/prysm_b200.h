@@ -276,11 +276,11 @@ int pb_weighted_sum(pb_handle_t h, int dtype, const void* modes, int k, long lon
 int pb_otf_normalize(pb_handle_t h, int dtype, const void* D, int ny, int nx, int which,
                      void* mtf, void* ptf, void* otf, void* stream);
 /* Baliga-Cohn encircled energy of a real MTF array (ny,nx) with frequency spacing df [cy/mm] at nr radii
- * [mm] (HOST arrays in/out; synchronises the stream).  prysm/otf.py:319-414 */
+ * [mm] (HOST arrays in/out; synchronises the stream).  Deterministic.  prysm/otf.py:319-414 */
 int pb_encircled_energy(pb_handle_t h, int dtype, const void* mtf, int ny, int nx, double df,
                         const double* radii_mm_host, int nr, double* out_host, void* stream);
 /* moments of a real array: sums_host[0..2] = sum(d), sum(d*y), sum(d*x) (HOST doubles; this call
- * synchronises the stream).  prysm/psf.py:174-203 */
+ * synchronises the stream).  Deterministic.  prysm/psf.py:174-203 */
 int pb_moments(pb_handle_t h, int dtype, const void* data, int ny, int nx, double* sums_host,
                void* stream);
 
@@ -307,17 +307,17 @@ int pb_field_adjoint(pb_handle_t h, int dtype, int mode, const void* field, cons
  * (prysm/propagation/wavefront.py:153-166). */
 int pb_component(pb_handle_t h, int dtype, int which, const void* in, long long count, void* out,
                  void* stream);
-/* out_host[0..1] = sum w * a * conj(b) (w real or NULL; fp64 accumulation; synchronises the stream).
+/* out_host[0..1] = sum w * a * conj(b) (w real or NULL; fp64 accumulation, deterministic; synchronises the stream).
  * The reduction of thin_lens_adjoint (prysm/propagation/wavefront.py:244-280) and of <x, y> adjoint checks. */
 int pb_dot(pb_handle_t h, int dtype, const void* a, const void* b, const void* w, long long count,
            double* out_host, void* stream);
 /* out_host[2j..2j+1] = sum_n modes[j][n] * bar[n] for k real modes; bar real or complex (bar_complex).
- * sum_of_2d_modes_adjoint (prysm/polynomials/fitting.py:40-57).  Synchronises the stream. */
+ * sum_of_2d_modes_adjoint (prysm/polynomials/fitting.py:40-57).  Deterministic; synchronises the stream. */
 int pb_mode_projection(pb_handle_t h, int dtype, const void* modes, int k, long long count,
                        const void* bar, int bar_complex, double* out_host, void* stream);
 /* k-space gradient of mtf (which=1, bar real) / ptf (2, bar real) / otf (4, bar complex) _from_psf_adjoint given
- * the complex transform D (ny,nx), including the centre-normalisation term (prysm/otf.py:205-316); the caller
- * finishes with transform_psf_adjoint (pb_fft2, dir=+1) and takes the real part. */
+ * the complex transform D (ny,nx), including the centre-normalisation term (prysm/otf.py:205-316); deterministic.  The
+ * caller finishes with transform_psf_adjoint (pb_fft2, dir=+1) and takes the real part. */
 int pb_otf_adjoint_seed(pb_handle_t h, int dtype, int which, const void* bar, const void* D, int ny,
                         int nx, void* data_bar, void* stream);
 /* MTF-plane gradient of encircled_energy: mtf_bar = sum_r ee_bar[r]*r*J1(2 pi r nu)/nu*df^2, radii [mm] and
@@ -377,7 +377,7 @@ int pb_zernike_sum(pb_handle_t h, int dtype, int polar, const void* a, const voi
  * conv(obj, psf) of two REAL arrays (prysm/convolution.py:9-32) as one forward and one inverse transform:
  * pb_balance_scale: *s_dev (a DEVICE double) = sqrt(sum a^2 / sum b^2) (1 if either sum is 0 / not finite): the two
  *   arrays share one transform whose rounding error is relative to the larger of them, so the PSF is scaled to the
- *   object's norm for the round trip -- on the device, no host synchronisation;
+ *   object's norm for the round trip -- on the device, no host synchronisation; deterministic;
  * pb_pack_complex: out = re + i*s*im (im NULL -> 0; im_scale_dev NULL -> s = 1); pb_fft2 of that gives Z = O + i*s*H;
  * pb_packed_spectrum_product: out[k] = scale/s * (Z[k]^2 - conj(Z[-k])^2)/(4i) = scale * O[k]*H[k], indices modulo
  *   (ny, nx), unshifted spectrum order; out must not alias Z. */
@@ -448,9 +448,8 @@ int pb_dm_gather(pb_handle_t h, int dtype, const void* in, int in_complex, int n
  * pb_segment_compose: out (ny, nx) += sum over segments s < ncoef of mask_s * sum_k coefs[s*coef_stride + k] *
  *   base_{s,k} over its window (compose_opd), accumulated per sample in fp64 in segment order and rounded once; coefs
  *   is a DEVICE fp64 array.  No atomics.
- * pb_segment_compose_adjoint: out (nseg, nmodes) = sum over segment s's window of opdbar * mask_s * base_{s,k},
- *   through `partial` (DEVICE fp64, nseg * nchunk * nmodes) with nchunk * PB_SEGMENT_CHUNK >= every window's h*w:
- *   a fixed-order two-level reduction. */
+ * pb_segment_compose_adjoint: out (nseg, nmodes) = sum over segment s's window of opdbar * mask_s * base_{s,k}, with
+ *   nchunk * PB_SEGMENT_CHUNK >= every window's h*w: a fixed-order two-level reduction. */
 typedef enum {
     PB_SDF_POLYGON = 0, PB_SDF_SPIDER = 1, PB_SDF_RECTANGLE = 2, PB_SDF_FILLET_RECTANGLE = 3, PB_SDF_ANNULUS = 4,
     PB_SDF_OFFSET_CIRCLE = 5
@@ -473,7 +472,7 @@ int pb_segment_compose(pb_handle_t h, int dtype, int ny, int nx, int tiles_y, in
                        const double* coefs, long long coef_stride, int ncoef, void* out, void* stream);
 int pb_segment_compose_adjoint(pb_handle_t h, int dtype, int ny, int nx, int nseg, const long long* seg,
                                const void* masks, const void* bases, int nmodes, const void* opdbar, int nchunk,
-                               double* partial, void* out, void* stream);
+                               void* out, void* stream);
 
 /* ---- Jones calculus (prysm/x/polarization.py) ----------------------------------------------------------------------
  * Element-planar layout: a Jones array of n pixels is 4 contiguous planes of n complex samples at dtype, plane 2*i + j
@@ -517,9 +516,8 @@ int pb_jones_reduce(pb_handle_t h, int dtype, int kind, long long n, const void*
  * pb_overlap: for each of nmodes modes M_p (real or complex at dtype; packed (nmodes, n) in `modes`, or the host
  *   array mode_ptrs_host of nmodes device pointers when `modes` is NULL) and the complex field E (n values):
  *   eta[p] = |sum conj(M_p) E|^2 / (I_p I_E), I_p = sum |M_p|^2 (or ip_dev[p], fp64 on the device), I_E = sum |E|^2
- *   (or ie_dev[0]).  partial: fp64 device workspace of nchunk * (3 nmodes + 1) values, nchunk =
- *   ceil(n / PB_OVERLAP_CHUNK).  c_out (optional): sqrt(I_E eta[0]).  eta and c_out are dtype's real type.
- *   Deterministic: per-chunk partials summed in a fixed order.
+ *   (or ie_dev[0]).  c_out (optional): sqrt(I_E eta[0]).  eta and c_out are dtype's real type.
+ *   Deterministic: partials of PB_OVERLAP_CHUNK pixels summed in a fixed order.
  * pb_wfs_combine: out = alpha a + beta b (complex) or |alpha a + beta b|^2 (real_out: real).  coefs_host = re, im of
  *   alpha then of beta; each is multiplied by the device real scalar alpha_scale / beta_scale when given.  b may be
  *   NULL.
@@ -539,7 +537,7 @@ int pb_lp_modes(pb_handle_t h, int dtype, const void* r, const void* t, long lon
                 const double* plan_host, void* out, void* stream);
 int pb_overlap(pb_handle_t h, int dtype, const void* E, long long n, int nmodes, const void* modes,
                const void* const* mode_ptrs_host, int modes_complex, const double* ip_dev, const double* ie_dev,
-               void* partial, void* eta, void* c_out, void* stream);
+               void* eta, void* c_out, void* stream);
 int pb_wfs_combine(pb_handle_t h, int dtype, long long n, const void* a, const void* b, const double* coefs_host,
                    const void* alpha_scale, const void* beta_scale, int real_out, void* out, void* stream);
 int pb_grating(pb_handle_t h, int dtype, int kind, long long n, const void* x, double shift, const double* params_host,
@@ -570,12 +568,11 @@ int pb_psi(pb_handle_t h, int frame_type, int nframes, const void* const* frames
  *   out_type (PB_ELEM_F32 / F64).
  * pb_white_balance: a *= gain in place (a contiguous, real at dtype): gains_host[site] for a mosaic (kind 0, rows of
  *   nx) or gains_host[i % 3] for interleaved RGB (kind 1).  With sat_host, every gain is first divided by max(1,
- *   max_p(max(plane p) gains_p / sat_p)), computed on the device in work (fp64, 4 PB_WB_MAX_BLOCKS + 1 values).
+ *   max_p(max(plane p) gains_p / sat_p)), computed on the device.
  * pb_demosaic_malvar: (m, n, 3) RGB of out_type (PB_ELEM_F32 from f32 / u8 / u16, or PB_ELEM_F64) from an m x n
  *   mosaic of in_type with row pitch ld, rggb or bggr: Malvar-He-Cutler's 5x5 filters, scipy.ndimage's reflect
  *   boundary, accumulated in fp64.  One pass.
  * pb_bayer_assemble: (n, 3) = (Re rp, (Re g2p + g1) / 2, Re bp) for complex rp, g2p, bp and real g1 at dtype. */
-enum { PB_WB_MAX_BLOCKS = 1024 };
 int pb_expose(pb_handle_t h, int dtype, const void* aerial, long long n, long long nx, const void* prnu, long long prnu_sr,
               long long prnu_sc, const void* dcnu, long long dcnu_sr, long long dcnu_sc, const double* params_host,
               int frames, long long key, int code_bytes, const void* lut, long long lut_len, int out_bytes,
@@ -589,7 +586,7 @@ int pb_bayer_interleave(pb_handle_t h, int elem_bytes, const void* const* planes
 int pb_demosaic_deinterlace(pb_handle_t h, int in_type, const void* img, long long m, long long n, long long ld, int bggr,
                             int out_type, void* out, void* stream);
 int pb_white_balance(pb_handle_t h, int dtype, void* a, long long n, long long nx, int kind, const double* gains_host,
-                     const double* sat_host, void* work, void* stream);
+                     const double* sat_host, void* stream);
 int pb_demosaic_malvar(pb_handle_t h, int in_type, const void* img, long long m, long long n, long long ld, int bggr,
                        int out_type, void* out, void* stream);
 int pb_bayer_assemble(pb_handle_t h, int dtype, const void* rp, const void* g2p, const void* bp, const void* g1,
@@ -833,9 +830,8 @@ int pb_analytic_radial(pb_handle_t h, int in_type, int out_type, int kind, const
                        double b, void* out, void* stream);
 
 /* ---- Interferometric metrology (prysm/interferogram.py, prysm/util.py, prysm/polynomials/fitting.py lstsq) ----------
- * Real data of dtype's real type (PB_C64: fp32, PB_C128: fp64), dense (ny, nx) or n elements.  Every reduction
- * accumulates in fp64 and folds per-block partials in block order in the last block to finish (an integer arrival
- * counter in the handle's scratch, no float atomics), so repeated calls give the same bits.
+ * Real data of dtype's real type (PB_C64: fp32, PB_C128: fp64), dense (ny, nx) or n elements.  Every reduction is the
+ * library's fixed-order grid fold (DESIGN.md §4.4), so repeated calls give the same bits.
  * pb_nan_stats: res (DEVICE, 9 fp64) = finite count, sum, min, max and sum of squares of the finite values, NaN count,
  *   mean, then sum |x - mean| and sum (x - mean)^2 over the finite values (pass 2 reads the mean from res).  Two launches.
  * pb_masked_gram: modes (HOST array of k device pointers, NULL = the constant 1), each n elements; data n elements with

@@ -903,10 +903,9 @@ def segment_compose_adjoint(seg, nseg, masks, bases, nmodes, opdbar, max_window)
     """(nseg, nmodes) = per-segment windowed projections of opdbar * mask onto the basis (pb_segment_compose_adjoint)."""
     ny, nx = opdbar.shape
     nchunk = max(1, -(-int(max_window) // capi.SEGMENT_CHUNK))
-    partial = torch.empty(max(1, nseg * nchunk * nmodes), dtype=torch.float64, device=opdbar.device)
     out = torch.empty((nseg, nmodes), dtype=opdbar.dtype, device=opdbar.device)
     _call(lib.pb_segment_compose_adjoint, opdbar, _CODE[opdbar.dtype], ny, nx, int(nseg), _p(seg), _p(masks), _p(bases),
-          int(nmodes), _p(opdbar), nchunk, _p(partial), _p(out))
+          int(nmodes), _p(opdbar), nchunk, _p(out))
     return out
 
 
@@ -980,12 +979,9 @@ def overlap(E, modes, ip=None, ie=None, want_c=False):
     mc = first.is_complex()
     if (_REAL_OF[first.dtype] if mc else first.dtype) != rd:
         raise ValueError(f'modes of {first.dtype} with a field of {E.dtype}')
-    nchunk = -(-n // capi.OVERLAP_CHUNK)
-    work = torch.empty(nchunk * (3 * P + 1), dtype=torch.float64, device=E.device)
     eta = torch.empty(P, dtype=rd, device=E.device)
     c = torch.empty((), dtype=rd, device=E.device) if want_c else None
-    _call(lib.pb_overlap, E, _CODE[E.dtype], _p(E), n, P, _p(packed), ptrs, int(mc), _p(ip), _p(ie), _p(work), _p(eta),
-          _p(c))
+    _call(lib.pb_overlap, E, _CODE[E.dtype], _p(E), n, P, _p(packed), ptrs, int(mc), _p(ip), _p(ie), _p(eta), _p(c))
     del keep
     return eta, c
 
@@ -1148,9 +1144,7 @@ def white_balance(a, kind, gains, sat=None):
     with `sat` the gains are first descaled on the device so that no plane exceeds its saturation."""
     g, gp = _darr(gains)
     s, sp = (None, None) if sat is None else _darr(sat)
-    work = None if sat is None else torch.empty(4 * capi.WB_MAX_BLOCKS + 1, dtype=torch.float64, device=a.device)
-    _call(lib.pb_white_balance, a, _CODE[a.dtype], _p(a), a.numel(), a.shape[-1] if kind == 0 else 3, int(kind), gp, sp,
-          _p(work))
+    _call(lib.pb_white_balance, a, _CODE[a.dtype], _p(a), a.numel(), a.shape[-1] if kind == 0 else 3, int(kind), gp, sp)
     return a
 
 

@@ -69,10 +69,10 @@ __global__ void component_kernel(int which, const cplx<R>* __restrict__ in, long
     }
 }
 
-// sums[0..1] += sum w * a * conj(b)
+// sums[0..1] = sum w * a * conj(b)
 template <typename R>
 __global__ void dot_kernel(const cplx<R>* __restrict__ a, const cplx<R>* __restrict__ b, const R* __restrict__ w, long long n,
-                           double* __restrict__ sums) {
+                           double* __restrict__ part, unsigned* __restrict__ counter, double* __restrict__ sums) {
     double re = 0, im = 0;
     PB_GRID_STRIDE(i, n) {
         const cplx<R> x = a[i], y = b[i];
@@ -82,13 +82,17 @@ __global__ void dot_kernel(const cplx<R>* __restrict__ a, const cplx<R>* __restr
     }
     double v[2] = {re, im};
     block_reduce<256>(v, OpAdd{});
-    if (threadIdx.x == 0) { atomicAdd(&sums[0], v[0]); atomicAdd(&sums[1], v[1]); }
+    if (threadIdx.x == 0) { part[blockIdx.x * 2] = v[0]; part[blockIdx.x * 2 + 1] = v[1]; }
+    if (!arrive_last(counter)) return;
+    v[0] = fold_partials<256, 2>(part, 0, OpAdd{}, 0.0);
+    v[1] = fold_partials<256, 2>(part, 1, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) { sums[0] = v[0]; sums[1] = v[1]; }
 }
 
-// sums[2k..2k+1] += sum modes[k][i] * bar[i]      (bar real or complex)
+// sums[2k..2k+1] = sum modes[k][i] * bar[i]      (bar real or complex), mode k in grid row k
 template <typename R>
 __global__ void mode_projection_kernel(const R* __restrict__ modes, long long n, const void* __restrict__ bar, int bar_complex,
-                                       double* __restrict__ sums) {
+                                       double* __restrict__ part, unsigned* __restrict__ counters, double* __restrict__ sums) {
     const R* mode = modes + (long long)blockIdx.y * n;
     double re = 0, im = 0;
     PB_GRID_STRIDE(i, n) {
@@ -102,13 +106,20 @@ __global__ void mode_projection_kernel(const R* __restrict__ modes, long long n,
     }
     double v[2] = {re, im};
     block_reduce<256>(v, OpAdd{});
-    if (threadIdx.x == 0) { atomicAdd(&sums[2 * blockIdx.y], v[0]); atomicAdd(&sums[2 * blockIdx.y + 1], v[1]); }
+    if (threadIdx.x == 0) {
+        double* p = part + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 2;
+        p[0] = v[0]; p[1] = v[1];
+    }
+    if (!arrive_last(counters)) return;
+    v[0] = fold_partials<256, 2>(part, 0, OpAdd{}, 0.0);
+    v[1] = fold_partials<256, 2>(part, 1, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) { sums[2 * blockIdx.y] = v[0]; sums[2 * blockIdx.y + 1] = v[1]; }
 }
 
 // which 1 (mtf): S = sum bar*|D|;  2 (ptf): S = sum bar;  4 (otf): S = sum conj(D)*bar
 template <typename R>
 __global__ void otf_adjoint_reduce_kernel(int which, const void* __restrict__ bar, const cplx<R>* __restrict__ D, long long n,
-                                          double* __restrict__ sums) {
+                                          double* __restrict__ part, unsigned* __restrict__ counter, double* __restrict__ sums) {
     double re = 0, im = 0;
     PB_GRID_STRIDE(i, n) {
         if (which == 4) {
@@ -123,7 +134,11 @@ __global__ void otf_adjoint_reduce_kernel(int which, const void* __restrict__ ba
     }
     double v[2] = {re, im};
     block_reduce<256>(v, OpAdd{});
-    if (threadIdx.x == 0) { atomicAdd(&sums[0], v[0]); atomicAdd(&sums[1], v[1]); }
+    if (threadIdx.x == 0) { part[blockIdx.x * 2] = v[0]; part[blockIdx.x * 2 + 1] = v[1]; }
+    if (!arrive_last(counter)) return;
+    v[0] = fold_partials<256, 2>(part, 0, OpAdd{}, 0.0);
+    v[1] = fold_partials<256, 2>(part, 1, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) { sums[0] = v[0]; sums[1] = v[1]; }
 }
 
 template <typename R>
@@ -281,27 +296,19 @@ extern "C" int pb_component(pb_handle_t hh, int dtype, int which, const void* in
     return PB_OK;
 }
 
-// device scratch for nd doubles, zeroed on the stream
-static int zeroed_sums(Handle* h, int nd, cudaStream_t st, double** out) {
-    void* d = nullptr;
-    PB_TRY(ensure_scratch(h, 2, (size_t)nd * sizeof(double), &d));
-    PB_CUDA(h, cudaMemsetAsync(d, 0, (size_t)nd * sizeof(double), st));
-    *out = reinterpret_cast<double*>(d);
-    return PB_OK;
-}
-
 extern "C" int pb_dot(pb_handle_t hh, int dtype, const void* a, const void* b, const void* w, long long count,
                       double* out_host, void* stream) {
     PB_ENTER_REAL(hh);
     if (!a || !b || !out_host || count < 0) return fail(h, PB_ERR_INVALID, "bad dot arguments");
     out_host[0] = out_host[1] = 0.0;
     if (count == 0) return PB_OK;
-    double* sums = nullptr;
-    PB_TRY(zeroed_sums(h, 2, st, &sums));
-    const int g = (int)std::min<long long>((count + 255) / 256, (long long)h->sm_count * 4);
+    const int g = fold_blocks(count, h->sm_count);
+    double *part, *sums; unsigned* counter;
+    PB_TRY(fold_scratch(h, 1, g, 2, st, &part, &counter));
+    PB_TRY(ensure_scratch(h, 2, 2 * sizeof(double), (void**)&sums));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        dot_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)a, (const cplx<R>*)b, (const R*)w, count, sums);
+        dot_kernel<R><<<g, 256, 0, st>>>((const cplx<R>*)a, (const cplx<R>*)b, (const R*)w, count, part, counter, sums);
     });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -313,13 +320,13 @@ extern "C" int pb_mode_projection(pb_handle_t hh, int dtype, const void* modes, 
                                   int bar_complex, double* out_host, void* stream) {
     PB_ENTER_REAL(hh);
     if (k < 1 || count <= 0 || !modes || !bar || !out_host) return fail(h, PB_ERR_INVALID, "bad mode-projection arguments");
-    double* sums = nullptr;
-    PB_TRY(zeroed_sums(h, 2 * k, st, &sums));
     const int gx = (int)std::min<long long>((count + 255) / 256, std::max(1LL, (long long)h->sm_count * 4 / k));
-    dim3 g(gx, k);
+    double *part, *sums; unsigned* counters;
+    PB_TRY(fold_scratch(h, k, gx, 2, st, &part, &counters));
+    PB_TRY(ensure_scratch(h, 2, (size_t)2 * k * sizeof(double), (void**)&sums));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        mode_projection_kernel<R><<<g, 256, 0, st>>>((const R*)modes, count, bar, bar_complex, sums);
+        mode_projection_kernel<R><<<dim3(gx, k), 256, 0, st>>>((const R*)modes, count, bar, bar_complex, part, counters, sums);
     });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, sums, (size_t)2 * k * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -333,13 +340,13 @@ extern "C" int pb_otf_adjoint_seed(pb_handle_t hh, int dtype, int which, const v
     if ((which != 1 && which != 2 && which != 4) || !bar || !D || !data_bar || ny < 1 || nx < 1)
         return fail(h, PB_ERR_INVALID, "bad otf-adjoint arguments");
     const long long n = (long long)ny * nx, centre = (long long)(ny / 2) * nx + nx / 2;
-    double* sums = nullptr;
-    PB_TRY(zeroed_sums(h, 2, st, &sums));
-    const int gr = (int)std::min<long long>((n + 255) / 256, (long long)h->sm_count * 4);
-    const int g = grid_for(n, 256, h->sm_count);
+    const int gr = fold_blocks(n, h->sm_count), g = grid_for(n, 256, h->sm_count);
+    double *part, *sums; unsigned* counter;
+    PB_TRY(fold_scratch(h, 1, gr, 2, st, &part, &counter));
+    PB_TRY(ensure_scratch(h, 2, 2 * sizeof(double), (void**)&sums));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        otf_adjoint_reduce_kernel<R><<<gr, 256, 0, st>>>(which, bar, (const cplx<R>*)D, n, sums);
+        otf_adjoint_reduce_kernel<R><<<gr, 256, 0, st>>>(which, bar, (const cplx<R>*)D, n, part, counter, sums);
         otf_adjoint_apply_kernel<R><<<g, 256, 0, st>>>(which, bar, (const cplx<R>*)D, n, centre, sums, (cplx<R>*)data_bar);
     });
     PB_LAUNCH_CHECK(h);

@@ -23,6 +23,16 @@ int ensure_scratch(Handle* h, int slot, size_t bytes, void** out) {
     return PB_OK;
 }
 
+int fold_scratch(Handle* h, int rows, int blocks, int per, cudaStream_t st, double** part, unsigned** counters) {
+    void* w = nullptr;
+    const size_t bytes = (size_t)rows * blocks * per * sizeof(double);
+    PB_TRY(ensure_scratch(h, FOLD_SLOT, bytes + (size_t)rows * sizeof(unsigned), &w));
+    *part = (double*)w;
+    *counters = (unsigned*)((char*)w + bytes);
+    PB_CUDA(h, cudaMemsetAsync(*counters, 0, (size_t)rows * sizeof(unsigned), st));
+    return PB_OK;
+}
+
 int encode_tensor_map(Handle* h, CUtensorMap* map, CUtensorMapDataType type, int rank, const void* base,
                       const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
                       CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2) {
@@ -71,7 +81,7 @@ extern "C" int pb_destroy(pb_handle_t hh) {
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
     for (auto& kv : h->tables) cudaFree(kv.second);
-    for (int i = 0; i < 3; ++i) if (h->scratch[i]) cudaFree(h->scratch[i]);
+    for (void* p : h->scratch) if (p) cudaFree(p);
     for (auto& e : h->side_ev) if (e) cudaEventDestroy(e);
     if (h->side) cudaStreamDestroy(h->side);
     delete h;

@@ -115,6 +115,31 @@ __device__ inline void warp_partials(double (&v)[N], Op op, double (&sh)[THREADS
     __syncthreads();
 }
 
+// ---- the grid fold of a reduction (DESIGN.md §4.4) ----------------------------------------------------------------
+// Each block reduces its grid-stride share with block_reduce and thread 0 writes the block's N partials to
+// part[(blockIdx.y * gridDim.x + blockIdx.x) * N + k]; the last block of its row to arrive then folds the row's partials
+// in block order and runs the epilogue.  No float atomics: the same n on the same card gives the same bits.
+
+// true in the last block of row blockIdx.y of the grid to arrive; the block's partials must be written before the call
+__device__ inline bool arrive_last(unsigned* counter) {
+    __shared__ bool last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(counter + blockIdx.y, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (last) __threadfence();
+    return last;
+}
+
+// the fold over the blocks of row blockIdx.y, in block order per thread then block_reduce, of column k of part
+template <int THREADS, int N, typename Op>
+__device__ inline double fold_partials(const double* part, int k, Op op, double init) {
+    part += (size_t)blockIdx.y * gridDim.x * N;
+    double v = init;
+    for (int b = threadIdx.x; b < (int)gridDim.x; b += THREADS) v = op(v, __ldcg(part + (size_t)b * N + k));
+    return block_reduce<THREADS>(v, op);
+}
+
 // the sum of v over the block (blockDim.x == THREADS, a power of two) by a halving tree in sh, given to every thread
 template <int THREADS>
 __device__ inline double tree_sum(double v, double* sh) {
@@ -178,9 +203,10 @@ struct Handle {
     // kernel launches per route of the transform kernels (pb_route_launch_count; the codes are in prysm_b200.h)
     std::map<int, long long> route_launches;
     std::map<TwKey, void*> tables;
-    // scratch arenas, grown on demand (never on a warmed-up hot call)
-    void* scratch[3] = {nullptr, nullptr, nullptr};
-    size_t scratch_bytes[3] = {0, 0, 0};
+    // scratch arenas, grown on demand (never on a warmed-up hot call); slot FOLD_SLOT holds the partials and arrival
+    // counters of the grid folds
+    void* scratch[4] = {nullptr, nullptr, nullptr, nullptr};
+    size_t scratch_bytes[4] = {0, 0, 0, 0};
     int sm_count = 132;
     int max_smem_optin = 0;
     // kernels whose opt-in attributes (dynamic shared memory, carve-out) were set on THIS handle's device.
@@ -231,6 +257,11 @@ struct NvtxRange {
 inline int grid_for(long long n, int threads, int sm_count) {
     const long long g = (n + threads - 1) / threads;
     return (int)std::max<long long>(1, std::min<long long>(g, (long long)sm_count * 16));
+}
+
+// blocks of one row of a folded reduction over n items: enough to cover them in blocks of 256, at most 4 per SM
+inline int fold_blocks(long long n, int sm_count) {
+    return (int)std::max<long long>(1, std::min<long long>((n + 255) / 256, (long long)sm_count * 4));
 }
 
 #define PB_GRID_STRIDE(i, n) \
@@ -309,6 +340,9 @@ constexpr int route_code(int kind, int L, int flags) {
     } while (0)
 
 int ensure_scratch(Handle* h, int slot, size_t bytes, void** out);
+constexpr int FOLD_SLOT = 3;
+// the partials (rows * blocks * per doubles) and the rows arrival counters, zeroed on st, of a grid fold
+int fold_scratch(Handle* h, int rows, int blocks, int per, cudaStream_t st, double** part, unsigned** counters);
 // (A, B, C) of P_{n+1}^(alpha,beta) = (A x + B) P_n - C P_{n-1}, DLMF 18.9 as the reference writes them (synthesis.cu)
 void jacobi_abc(int n, double alpha, double beta, double* abc);
 // amp * exp(2 pi i kturns opd) into the dense complex array out (count elements in rows of nx); opd and amp (pb_amp_kind)

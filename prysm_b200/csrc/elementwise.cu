@@ -119,7 +119,8 @@ __global__ void otf_normalize_kernel(const cplx<R>* __restrict__ D, long long n,
 }
 
 template <typename R>
-__global__ void moments_kernel(const R* __restrict__ d, int ny, int nx, double* __restrict__ sums) {
+__global__ void moments_kernel(const R* __restrict__ d, int ny, int nx, double* __restrict__ part, unsigned* __restrict__ counter,
+                               double* __restrict__ sums) {
     double s[3] = {0, 0, 0};     // sum v, sum v y, sum v x
     const long long n = (long long)ny * nx;
     PB_GRID_STRIDE(i, n) {
@@ -128,14 +129,19 @@ __global__ void moments_kernel(const R* __restrict__ d, int ny, int nx, double* 
         s[0] += v; s[1] += v * y; s[2] += v * x;
     }
     block_reduce<256>(s, OpAdd{});
-    if (threadIdx.x == 0) { atomicAdd(&sums[0], s[0]); atomicAdd(&sums[1], s[1]); atomicAdd(&sums[2], s[2]); }
+    if (threadIdx.x == 0) { double* p = part + blockIdx.x * 3; p[0] = s[0]; p[1] = s[1]; p[2] = s[2]; }
+    if (!arrive_last(counter)) return;
+    s[0] = fold_partials<256, 3>(part, 0, OpAdd{}, 0.0);
+    s[1] = fold_partials<256, 3>(part, 1, OpAdd{}, 0.0);
+    s[2] = fold_partials<256, 3>(part, 2, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) { sums[0] = s[0]; sums[1] = s[1]; sums[2] = s[2]; }
 }
 
 // Baliga & Cohn encircled energy: r * sum( MTF * J1(2 pi r nu) / nu ) * dnu^2 on the fftrange*df grid, nu(0) -> 1e-16
-// (prysm/otf.py:319-414).  One block-reduction per radius (blockIdx.y), fp64 Bessel and accumulation.
+// (prysm/otf.py:319-414).  One folded reduction per radius (grid row blockIdx.y), fp64 Bessel and accumulation.
 template <typename R>
 __global__ void encircled_energy_kernel(const R* __restrict__ mtf, int ny, int nx, double df, const double* __restrict__ radii,
-                                        double* __restrict__ out) {
+                                        double* __restrict__ part, unsigned* __restrict__ counters, double* __restrict__ out) {
     const double r = radii[blockIdx.y];
     const long long n = (long long)ny * nx;
     double acc = 0.0;
@@ -147,7 +153,10 @@ __global__ void encircled_energy_kernel(const R* __restrict__ mtf, int ny, int n
         acc += (double)mtf[i] * j1(6.283185307179586476925 * r * nu) / nu;
     }
     acc = block_reduce<256>(acc, OpAdd{});
-    if (threadIdx.x == 0) atomicAdd(&out[blockIdx.y], acc * r * df * df);
+    if (threadIdx.x == 0) part[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = acc;
+    if (!arrive_last(counters)) return;
+    acc = fold_partials<256, 1>(part, 0, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) out[blockIdx.y] = acc * r * df * df;
 }
 
 // Bluestein pieces of one CZT axis built on the device from scalars (prysm/fttools.py:372-389, 277-281):
@@ -300,16 +309,16 @@ extern "C" int pb_moments(pb_handle_t hh, int dtype, const void* data, int ny, i
                           void* stream) {
     PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || !sums_host) return fail(h, PB_ERR_INVALID, "bad shape");
-    void* d = nullptr;
-    PB_TRY(ensure_scratch(h, 2, 3 * sizeof(double), &d));
-    PB_CUDA(h, cudaMemsetAsync(d, 0, 3 * sizeof(double), st));
     const int g = grid_for((long long)ny * nx, 256, h->sm_count);
+    double *part, *sums; unsigned* counter;
+    PB_TRY(fold_scratch(h, 1, g, 3, st, &part, &counter));
+    PB_TRY(ensure_scratch(h, 2, 3 * sizeof(double), (void**)&sums));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        moments_kernel<R><<<g, 256, 0, st>>>((const R*)data, ny, nx, (double*)d);
+        moments_kernel<R><<<g, 256, 0, st>>>((const R*)data, ny, nx, part, counter, sums);
     });
     PB_LAUNCH_CHECK(h);
-    PB_CUDA(h, cudaMemcpyAsync(sums_host, d, 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    PB_CUDA(h, cudaMemcpyAsync(sums_host, sums, 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
     PB_CUDA(h, cudaStreamSynchronize(st));
     return PB_OK;
 }
@@ -323,12 +332,12 @@ extern "C" int pb_encircled_energy(pb_handle_t hh, int dtype, const void* mtf, i
     double* dr = (double*)d;
     double* dout = dr + nr;
     PB_CUDA(h, cudaMemcpyAsync(dr, radii_mm_host, nr * sizeof(double), cudaMemcpyHostToDevice, st));
-    PB_CUDA(h, cudaMemsetAsync(dout, 0, nr * sizeof(double), st));
-    const int gx = (int)std::min<long long>(((long long)ny * nx + 255) / 256, (long long)h->sm_count * 4);
-    dim3 g(gx, nr);
+    const int gx = fold_blocks((long long)ny * nx, h->sm_count);
+    double* part; unsigned* counters;
+    PB_TRY(fold_scratch(h, nr, gx, 1, st, &part, &counters));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        encircled_energy_kernel<R><<<g, 256, 0, st>>>((const R*)mtf, ny, nx, df, dr, dout);
+        encircled_energy_kernel<R><<<dim3(gx, nr), 256, 0, st>>>((const R*)mtf, ny, nx, df, dr, part, counters, dout);
     });
     PB_LAUNCH_CHECK(h);
     PB_CUDA(h, cudaMemcpyAsync(out_host, dout, nr * sizeof(double), cudaMemcpyDeviceToHost, st));

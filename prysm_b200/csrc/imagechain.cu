@@ -18,21 +18,21 @@ __global__ void pack_complex_kernel(const R* __restrict__ re, const R* __restric
         out[i] = mk<R>(re[i], im ? s * im[i] : R(0));
 }
 
-// sums[0] += sum a^2, sums[1] += sum b^2
+// *scale = sqrt(sum a^2 / sum b^2), 1 when either sum is 0 or not finite
 template <typename R>
-__global__ void norms2_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, double* __restrict__ sums) {
+__global__ void balance_kernel(const R* __restrict__ a, const R* __restrict__ b, long long n, double* __restrict__ part,
+                               unsigned* __restrict__ counter, double* __restrict__ scale) {
     double s[2] = {0, 0};
     PB_GRID_STRIDE(i, n) {
         const double x = a[i], y = b[i];
         s[0] += x * x; s[1] += y * y;
     }
     block_reduce<256>(s, OpAdd{});
-    if (threadIdx.x == 0) { atomicAdd(&sums[0], s[0]); atomicAdd(&sums[1], s[1]); }
-}
-
-__global__ void balance_finalize_kernel(const double* __restrict__ sums, double* __restrict__ s) {
-    const double a = sums[0], b = sums[1];
-    *s = (a > 0.0 && b > 0.0 && isfinite(a) && isfinite(b)) ? sqrt(a / b) : 1.0;
+    if (threadIdx.x == 0) { part[blockIdx.x * 2] = s[0]; part[blockIdx.x * 2 + 1] = s[1]; }
+    if (!arrive_last(counter)) return;
+    const double sa = fold_partials<256, 2>(part, 0, OpAdd{}, 0.0);
+    const double sb = fold_partials<256, 2>(part, 1, OpAdd{}, 0.0);
+    if (threadIdx.x == 0) *scale = (sa > 0.0 && sb > 0.0 && isfinite(sa) && isfinite(sb)) ? sqrt(sa / sb) : 1.0;
 }
 
 template <typename R>
@@ -114,17 +114,14 @@ extern "C" int pb_balance_scale(pb_handle_t hh, int dtype, const void* a, const 
                                 void* stream) {
     PB_ENTER_REAL(hh);
     if (!a || !b || !s_dev || count <= 0) return fail(h, PB_ERR_INVALID, "bad balance arguments");
-    void* d = nullptr;
-    PB_TRY(ensure_scratch(h, 2, 2 * sizeof(double), &d));
-    PB_CUDA(h, cudaMemsetAsync(d, 0, 2 * sizeof(double), st));
-    const int g = (int)std::min<long long>((count + 255) / 256, (long long)h->sm_count * 4);
+    const int g = fold_blocks(count, h->sm_count);
+    double* part; unsigned* counter;
+    PB_TRY(fold_scratch(h, 1, g, 2, st, &part, &counter));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
-        norms2_kernel<R><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, (double*)d);
+        balance_kernel<R><<<g, 256, 0, st>>>((const R*)a, (const R*)b, count, part, counter, s_dev);
     });
-    balance_finalize_kernel<<<1, 1, 0, st>>>((const double*)d, s_dev);
     PB_LAUNCH_CHECK(h);
-    h->launches++;
     return PB_OK;
 }
 

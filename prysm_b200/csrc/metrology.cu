@@ -3,10 +3,8 @@
 // prologue and epilogue around pb_fft2, the band-limited trapezoid, the radial filter, the gradient, the finite
 // bounding box and the masked writes of the Interferogram methods.
 //
-// Every reduction accumulates in fp64 and runs in a fixed order: each block folds its grid-stride share with
-// block_reduce and writes its partials to scratch, and the last block to finish (an integer arrival counter, no float
-// atomics) folds the partials in block order.  The grid depends only on the size and the SM count, so repeated calls
-// give the same bits.
+// Every reduction accumulates in fp64 and combines its blocks with the grid fold of common.cuh (DESIGN.md §4.4), so
+// repeated calls give the same bits.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -17,28 +15,6 @@ constexpr int MET_THREADS = 256;
 constexpr int MET_TILE = 32;                 // pixels per shared-memory tile of the Gram kernel
 constexpr int MET_TILE_LD = MET_TILE + 1;    // its row stride: threads with consecutive (i, j) read different banks
 constexpr int MET_GRAM_PER_THREAD = (PB_GRAM_MAX_K + 1) * (PB_GRAM_MAX_K + 2) / 2 / MET_THREADS + 1;
-
-// the blocks of a reduction over n items: a fixed function of n and the SM count
-inline int met_blocks(long long n, int sm_count) { return std::min(grid_for(n, MET_THREADS, sm_count), 4 * sm_count); }
-
-// true in the last block of the grid to arrive; the block's partials must be written before the call
-__device__ inline bool arrive_last(unsigned* counter) {
-    __shared__ bool last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicAdd(counter, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (last) __threadfence();
-    return last;
-}
-
-// the fold over blocks, in block order per thread then block_reduce, of column k of part (gridDim.x rows of N)
-template <int N, typename Op>
-__device__ inline double fold_partials(const double* part, int k, Op op, double init) {
-    double v = init;
-    for (int b = threadIdx.x; b < (int)gridDim.x; b += MET_THREADS) v = op(v, __ldcg(part + (size_t)b * N + k));
-    return block_reduce<MET_THREADS>(v, op);
-}
 
 // ---- statistics -------------------------------------------------------------------------------------------------
 // pass 1: count, sum, min, max, sum of squares of the finite values, NaN count -> res[0..5]; res[6] = mean
@@ -65,12 +41,12 @@ __global__ void __launch_bounds__(MET_THREADS) stats_pass1_kernel(const T* __res
     }
     if (!arrive_last(counter)) return;
     double r[6];
-    r[0] = fold_partials<6>(part, 0, OpAdd{}, 0.0);
-    r[1] = fold_partials<6>(part, 1, OpAdd{}, 0.0);
-    r[2] = fold_partials<6>(part, 2, OpMin{}, CUDART_INF);
-    r[3] = fold_partials<6>(part, 3, OpMax{}, -CUDART_INF);
-    r[4] = fold_partials<6>(part, 4, OpAdd{}, 0.0);
-    r[5] = fold_partials<6>(part, 5, OpAdd{}, 0.0);
+    r[0] = fold_partials<MET_THREADS, 6>(part, 0, OpAdd{}, 0.0);
+    r[1] = fold_partials<MET_THREADS, 6>(part, 1, OpAdd{}, 0.0);
+    r[2] = fold_partials<MET_THREADS, 6>(part, 2, OpMin{}, CUDART_INF);
+    r[3] = fold_partials<MET_THREADS, 6>(part, 3, OpMax{}, -CUDART_INF);
+    r[4] = fold_partials<MET_THREADS, 6>(part, 4, OpAdd{}, 0.0);
+    r[5] = fold_partials<MET_THREADS, 6>(part, 5, OpAdd{}, 0.0);
     if (threadIdx.x == 0) {
         for (int k = 0; k < 6; ++k) res[k] = r[k];
         res[6] = r[1] / r[0];
@@ -94,8 +70,8 @@ __global__ void __launch_bounds__(MET_THREADS) stats_pass2_kernel(const T* __res
     block_reduce<MET_THREADS>(v, OpAdd{});
     if (threadIdx.x == 0) { part[(size_t)blockIdx.x * 2] = v[0]; part[(size_t)blockIdx.x * 2 + 1] = v[1]; }
     if (!arrive_last(counter)) return;
-    const double s0 = fold_partials<2>(part, 0, OpAdd{}, 0.0);
-    const double s1 = fold_partials<2>(part, 1, OpAdd{}, 0.0);
+    const double s0 = fold_partials<MET_THREADS, 2>(part, 0, OpAdd{}, 0.0);
+    const double s1 = fold_partials<MET_THREADS, 2>(part, 1, OpAdd{}, 0.0);
     if (threadIdx.x == 0) { res[7] = s0; res[8] = s1; *counter = 0; }
 }
 
@@ -222,7 +198,7 @@ __global__ void __launch_bounds__(MET_THREADS) psd_prologue_kernel(const T* __re
     s2 = block_reduce<MET_THREADS>(s2, OpAdd{});
     if (threadIdx.x == 0) part[blockIdx.x] = s2;
     if (!arrive_last(counter)) return;
-    const double s = fold_partials<1>(part, 0, OpAdd{}, 0.0);
+    const double s = fold_partials<MET_THREADS, 1>(part, 0, OpAdd{}, 0.0);
     if (threadIdx.x == 0) { res[0] = s; *counter = 0; }
 }
 
@@ -274,7 +250,7 @@ __global__ void __launch_bounds__(MET_THREADS) band_trapz_kernel(const T* __rest
     s = block_reduce<MET_THREADS>(s, OpAdd{});
     if (threadIdx.x == 0) part[blockIdx.x] = s;
     if (!arrive_last(counter)) return;
-    const double t = fold_partials<1>(part, 0, OpAdd{}, 0.0);
+    const double t = fold_partials<MET_THREADS, 1>(part, 0, OpAdd{}, 0.0);
     if (threadIdx.x == 0) { res[0] = t; *counter = 0; }
 }
 
@@ -410,23 +386,12 @@ __global__ void __launch_bounds__(MET_THREADS) pointwise_kernel(int op, const T*
 
 using namespace pb;
 
-// partials of a reduction of `blocks` blocks with `per` doubles each, and the arrival counter after them
-static int met_scratch(Handle* h, int blocks, int per, double** part, unsigned** counter, cudaStream_t st) {
-    void* w = nullptr;
-    const size_t bytes = (size_t)blocks * per * sizeof(double);
-    PB_TRY(ensure_scratch(h, 2, bytes + 64, &w));
-    *part = (double*)w;
-    *counter = (unsigned*)((char*)w + bytes);
-    PB_CUDA(h, cudaMemsetAsync(*counter, 0, sizeof(unsigned), st));
-    return PB_OK;
-}
-
 extern "C" int pb_nan_stats(pb_handle_t hh, int dtype, const void* x, long long n, double* res, void* stream) {
     PB_ENTER_REAL(hh);
     if (!x || !res || n < 0) return fail(h, PB_ERR_INVALID, "pb_nan_stats: null array or negative count");
-    const int blocks = met_blocks(n, h->sm_count);
+    const int blocks = fold_blocks(n, h->sm_count);
     double* part; unsigned* counter;
-    PB_TRY(met_scratch(h, blocks, 6, &part, &counter, st));
+    PB_TRY(fold_scratch(h, 1, blocks, 6, st, &part, &counter));
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
         stats_pass1_kernel<R><<<blocks, MET_THREADS, 0, st>>>((const R*)x, n, part, counter, res);
@@ -448,7 +413,7 @@ extern "C" int pb_masked_gram(pb_handle_t hh, int dtype, const void* const* mode
     const int P = (k + 1) * (k + 2) / 2;
     const int blocks = std::max(1, std::min<int>((int)((n + MET_TILE - 1) / MET_TILE), 2 * h->sm_count));
     double* part; unsigned* counter;
-    PB_TRY(met_scratch(h, blocks, P, &part, &counter, st));
+    PB_TRY(fold_scratch(h, 1, blocks, P, st, &part, &counter));
     const size_t smem = (size_t)(k + 1) * MET_TILE_LD * sizeof(double);
     with_real(dtype, [&](auto r) {
         using R = decltype(r);
@@ -466,9 +431,9 @@ extern "C" int pb_psd_prologue(pb_handle_t hh, int dtype, const void* height, in
         (shifted && !height) || !s2 || !flags || (kind == PB_WIN_AUTO && !corners))
         return fail(h, PB_ERR_INVALID, "pb_psd_prologue: bad shape, window kind or missing array");
     const long long n = (long long)ny * nx;
-    const int blocks = met_blocks(n, h->sm_count);
+    const int blocks = fold_blocks(n, h->sm_count);
     double* part; unsigned* counter;
-    PB_TRY(met_scratch(h, blocks, 1, &part, &counter, st));
+    PB_TRY(fold_scratch(h, 1, blocks, 1, st, &part, &counter));
     PbRect4 rect{};
     if (corners)
         for (int q = 0; q < 16; ++q) rect.v[q] = corners[q];
@@ -505,9 +470,9 @@ extern "C" int pb_band_trapz(pb_handle_t hh, int dtype, const void* psd, const v
     if (!psd || !res || ny < 1 || nx < 1 || (!r && (!fx || !fy)))
         return fail(h, PB_ERR_INVALID, "pb_band_trapz: null array or bad shape");
     const long long n = (long long)ny * nx;
-    const int blocks = met_blocks(n, h->sm_count);
+    const int blocks = fold_blocks(n, h->sm_count);
     double* part; unsigned* counter;
-    PB_TRY(met_scratch(h, blocks, 1, &part, &counter, st));
+    PB_TRY(fold_scratch(h, 1, blocks, 1, st, &part, &counter));
     with_real(dtype, [&](auto rr) {
         using R = decltype(rr);
         band_trapz_kernel<R><<<blocks, MET_THREADS, 0, st>>>((const R*)psd, (const R*)r, fx, fy, ny, nx, twod, flow, fhigh,

@@ -223,12 +223,14 @@ extern "C" int pb_segment_compose(pb_handle_t hh, int dtype, int ny, int nx, int
 
 extern "C" int pb_segment_compose_adjoint(pb_handle_t hh, int dtype, int ny, int nx, int nseg, const long long* seg,
                                           const void* masks, const void* bases, int nmodes, const void* opdbar, int nchunk,
-                                          double* partial, void* out, void* stream) {
+                                          void* out, void* stream) {
     PB_ENTER_REAL(hh);
     if (ny < 1 || nx < 1 || nseg < 0 || nmodes < 0 || nchunk < 1 || nseg > 65535)
         return fail(h, PB_ERR_INVALID, "bad compose adjoint arguments");
     if ((long long)nseg * nmodes == 0) return PB_OK;
-    if (!seg || !masks || !bases || !opdbar || !partial || !out) return fail(h, PB_ERR_INVALID, "null pointer");
+    if (!seg || !masks || !bases || !opdbar || !out) return fail(h, PB_ERR_INVALID, "null pointer");
+    double* partial = nullptr;
+    PB_TRY(ensure_scratch(h, FOLD_SLOT, (size_t)nseg * nchunk * nmodes * sizeof(double), (void**)&partial));
     const dim3 grid(nchunk, nseg);
     with_real(dtype, [&](auto r) {
         using R = decltype(r);

@@ -235,6 +235,7 @@ __global__ void deinterlace_kernel(const In* __restrict__ img, long long m2, lon
 
 // white balance: the gain of element i is gains[site] (mosaic, kind 0) or gains[i % 3] (rgb, kind 1)
 struct Gains4 { double g[4]; double sat[4]; };
+constexpr int kWbMaxBlocks = 1024;     // blocks of the white-balance launches; the ratio kernel folds their plane maxima
 
 __device__ __forceinline__ int wb_plane(int kind, long long i, long long nx) {
     if (kind == 1) return (int)(i % 3);
@@ -553,9 +554,9 @@ extern "C" int pb_demosaic_deinterlace(pb_handle_t hh, int in_type, const void* 
 }
 
 extern "C" int pb_white_balance(pb_handle_t hh, int dtype, void* a, long long n, long long nx, int kind,
-                                const double* gains_host, const double* sat_host, void* work, void* stream) {
+                                const double* gains_host, const double* sat_host, void* stream) {
     PB_ENTER(hh);
-    if (!a || !gains_host || n < 0 || nx < 1 || kind < 0 || kind > 1 || (sat_host && !work))
+    if (!a || !gains_host || n < 0 || nx < 1 || kind < 0 || kind > 1)
         return fail(h, PB_ERR_INVALID, "bad white-balance arguments");
     if (n == 0) return PB_OK;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -565,13 +566,15 @@ extern "C" int pb_white_balance(pb_handle_t hh, int dtype, void* a, long long n,
         g4.g[pl] = pl < nplanes ? gains_host[pl] : 1.0;
         g4.sat[pl] = sat_host && pl < nplanes ? sat_host[pl] : 1.0;
     }
-    const int g = std::min(grid_for(n, kSensorThreads, h->sm_count), (int)PB_WB_MAX_BLOCKS);
-    double* ratio = nullptr;
+    const int g = std::min(grid_for(n, kSensorThreads, h->sm_count), kWbMaxBlocks);
+    double *partial = nullptr, *ratio = nullptr;
+    if (sat_host) {
+        PB_TRY(ensure_scratch(h, FOLD_SLOT, (size_t)(4 * g + 1) * sizeof(double), (void**)&partial));
+        ratio = partial + 4 * g;
+    }
     if (!with_real(dtype, [&](auto r) {
             using T = decltype(r);
             if (sat_host) {
-                double* partial = (double*)work;
-                ratio = partial + 4 * PB_WB_MAX_BLOCKS;
                 wb_plane_max_kernel<T><<<g, kSensorThreads, 0, st>>>((const T*)a, n, nx, kind, partial);
                 wb_ratio_kernel<<<1, kSensorThreads, 0, st>>>(partial, g, nplanes, g4, ratio);
             }

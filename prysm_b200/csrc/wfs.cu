@@ -366,14 +366,15 @@ extern "C" int pb_lp_modes(pb_handle_t hh, int dtype, const void* r, const void*
 
 extern "C" int pb_overlap(pb_handle_t hh, int dtype, const void* E, long long n, int nmodes, const void* modes,
                           const void* const* mode_ptrs_host, int modes_complex, const double* ip_dev,
-                          const double* ie_dev, void* partial, void* eta, void* c_out, void* stream) {
+                          const double* ie_dev, void* eta, void* c_out, void* stream) {
     PB_ENTER_REAL(hh);
     if (n <= 0 || nmodes <= 0) return fail(h, PB_ERR_INVALID, "bad overlap sizes");
-    if (!E || !partial || !eta || (!modes && !mode_ptrs_host)) return fail(h, PB_ERR_INVALID, "null pointer");
+    if (!E || !eta || (!modes && !mode_ptrs_host)) return fail(h, PB_ERR_INVALID, "null pointer");
     const long long nchunk_ll = (n + PB_OVERLAP_CHUNK - 1) / PB_OVERLAP_CHUNK;
     if (nchunk_ll > (1LL << 30)) return fail(h, PB_ERR_UNSUPPORTED, "field too large for the chunked reduction");
     const int nchunk = (int)nchunk_ll;
-    double* part = reinterpret_cast<double*>(partial);
+    double* part = nullptr;
+    PB_TRY(ensure_scratch(h, FOLD_SLOT, (size_t)nchunk * (3 * nmodes + 1) * sizeof(double), (void**)&part));
     double* part_e = part + (long long)nmodes * nchunk * 3;
     const size_t esz = rsize(dtype) * (modes_complex ? 2 : 1);
     for (int p0 = 0; p0 < nmodes; p0 += kOvMax) {

@@ -38,8 +38,8 @@ PB_MAX_MODES = 64                     # csrc/elementwise.cu: #define PB_MAX_MODE
 
 
 def reduction_grid(n, sm_count, threads=THREADS):
-    """the reduction cap of pb_dot, pb_otf_adjoint_seed, pb_balance_scale and pb_encircled_energy (csrc/adjoint_ops.cu,
-    csrc/imagechain.cu, csrc/elementwise.cu: min(ceil(n/256), sm_count*4))"""
+    """the grid of pb_dot, pb_otf_adjoint_seed, pb_balance_scale and pb_encircled_energy (csrc/common.cuh fold_blocks:
+    min(ceil(n/256), sm_count*4))"""
     return min((n + threads - 1) // threads, sm_count * 4)
 
 
