@@ -1396,12 +1396,13 @@ def tf_nlayers(ops):
 
 
 def _tf_args(ops):
+    """(broadcast shape, ndim, shape, strides, operands) of the thin-film operands and any coating-design operands after
+    them, as the C ABI takes them: host arrays of CM_NOPS operand slots, the slots past len(ops) NULL."""
     bshape, dims, strides = tf_layout(ops)
-    shp = np.asarray(dims if dims else [1], dtype=np.int64)
-    ins = (C.c_void_p * len(ops))(*[t.data_ptr() for t in ops])
-    keep = (shp, strides, ins)
-    return bshape, len(dims), shp.ctypes.data_as(C.POINTER(C.c_longlong)), \
-        strides.ctypes.data_as(C.POINTER(C.c_longlong)), C.cast(ins, C.POINTER(C.c_void_p)), keep
+    shp = (C.c_longlong * max(len(dims), 1))(*(dims or [1]))
+    st = (C.c_longlong * (capi.CM_NOPS * (capi.TF_DIMS + 1)))(*strides.ravel().tolist())
+    ins = (C.c_void_p * capi.CM_NOPS)(*[t.data_ptr() for t in ops])
+    return bshape, len(dims), shp, st, ins
 
 
 def stack_eval(mode, pol, ops, outputs, rdtype, theta_scale=1.0):
@@ -1409,7 +1410,7 @@ def stack_eval(mode, pol, ops, outputs, rdtype, theta_scale=1.0):
     complex of the broadcast shape, E, H, Esq (N + 1, *shape), REFL, TRANS (shape), ABS (N, *shape), in rdtype's
     precision."""
     nlayers = tf_nlayers(ops)
-    bshape, nd, shp, stp, inp, keep = _tf_args(ops)
+    bshape, nd, shp, stp, inp = _tf_args(ops)
     cdtype = _CPLX_OF[rdtype]
     lead = {capi.TF_OUT_E: nlayers + 1, capi.TF_OUT_H: nlayers + 1, capi.TF_OUT_ESQ: nlayers + 1,
             capi.TF_OUT_ABS: nlayers}
@@ -1434,7 +1435,7 @@ def stack_grad(pol, kinds, ops, E, H, seeds, rdtype):
     boundary fields of stack_eval; seeds: dR, dT, dA, dEsq as contiguous fp64 device arrays of the full shapes, or
     None."""
     nlayers = tf_nlayers(ops)
-    bshape, nd, shp, stp, inp, keep = _tf_args(ops)
+    bshape, nd, shp, stp, inp = _tf_args(ops)
     both = kinds == capi.TF_GRAD_THICKNESS | capi.TF_GRAD_INDEX
     grad = torch.empty(((2,) if both else ()) + (nlayers,), dtype=rdtype, device=E.device)
     if nlayers == 0:
@@ -1445,38 +1446,25 @@ def stack_grad(pol, kinds, ops, E, H, seeds, rdtype):
     return grad
 
 
-def cm_layout(ops):
-    """(broadcast shape, ndim, shape, strides, operands, keep-alive) of the coating-design operands: the six thin-film
-    operands, target and weight, and optionally the needle index; the arrays are padded to CM_NOPS slots."""
-    bshape, dims, strides = tf_layout(ops)
-    full = np.zeros((capi.CM_NOPS, capi.TF_DIMS + 1), dtype=np.int64)
-    full[:len(ops)] = strides
-    shp = np.asarray(dims if dims else [1], dtype=np.int64)
-    ins = (C.c_void_p * capi.CM_NOPS)(*([t.data_ptr() for t in ops] + [None] * (capi.CM_NOPS - len(ops))))
-    return bshape, len(dims), shp, full, ins
-
-
 def coating_merit(quantity, pol, flags, ops, b0=0, b1=0, blist=None, value=None, residuals=None, grad=None,
                   rdtype=torch.float64):
     """One merit term (pb_coating_merit) over ops = the six thin-film operands, target and weight: the fp64 value
     into `value` (a one-element device array), sqrt(w) (q - target) into `residuals` (count, rdtype) and the
     gradient into `grad` (rdtype), each as `flags` (CM_OUT_*, CM_ACCUMULATE) asks."""
     nlayers = tf_nlayers(ops)
-    bshape, nd, shp, strides, ins = cm_layout(ops)
+    bshape, nd, shp, stp, inp = _tf_args(ops)
     nb = 0 if blist is None else blist.numel() // 2
-    _call(lib.pb_coating_merit, ops[0], _CODE[rdtype], int(quantity), int(pol), int(flags), nlayers, nd,
-          shp.ctypes.data_as(C.POINTER(C.c_longlong)), strides.ctypes.data_as(C.POINTER(C.c_longlong)),
-          C.cast(ins, C.POINTER(C.c_void_p)), int(b0), int(b1), _p(blist), nb, _p(value), _p(residuals), _p(grad))
+    _call(lib.pb_coating_merit, ops[0], _CODE[rdtype], int(quantity), int(pol), int(flags), nlayers, nd, shp, stp, inp,
+          int(b0), int(b1), _p(blist), nb, _p(value), _p(residuals), _p(grad))
 
 
 def needle(quantity, pol, ops, zpart, zlist, P, accumulate):
     """P(z) of an R or T term (pb_needle): ops = the six thin-film operands, target, weight and the needle index;
     zpart (2, nz) fp64 partial thicknesses, zlist the per-layer depth runs (int32), P (nz) written or added to."""
     nlayers = tf_nlayers(ops)
-    bshape, nd, shp, strides, ins = cm_layout(ops)
-    _call(lib.pb_needle, ops[0], _CODE[P.dtype], int(quantity), int(pol), nlayers, nd,
-          shp.ctypes.data_as(C.POINTER(C.c_longlong)), strides.ctypes.data_as(C.POINTER(C.c_longlong)),
-          C.cast(ins, C.POINTER(C.c_void_p)), _p(zpart), int(zpart.shape[1]), _p(zlist), _p(P), int(bool(accumulate)))
+    bshape, nd, shp, stp, inp = _tf_args(ops)
+    _call(lib.pb_needle, ops[0], _CODE[P.dtype], int(quantity), int(pol), nlayers, nd, shp, stp, inp, _p(zpart),
+          int(zpart.shape[1]), _p(zlist), _p(P), int(bool(accumulate)))
 
 
 def field_at_depth(pol, z, zb, n, n0, wvl, theta0, Eb, Hb, cdtype):

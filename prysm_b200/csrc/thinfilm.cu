@@ -100,6 +100,11 @@ __device__ inline TfSample tf_sample(const TfOps& op, long long i) {
     return s;
 }
 
+// the substrate's tilted admittance
+__device__ __forceinline__ double2 tf_eta_sub(const TfSample& s, int pol) {
+    return tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
+}
+
 // layer k of a sample: index, cos theta_k, phase thickness beta, admittance eta and thickness
 struct TfLayer { double2 n, cost, beta, eta; double d; };
 
@@ -121,6 +126,30 @@ __device__ inline void tf_apply(double2 sb, double2 cb, double2 eta, double2& v0
     const double2 a = cadd(cmul(cb, v0), cmul(tf_div(mis, eta), v1));
     const double2 b = cadd(cmul(cmul(mis, eta), v0), cmul(cb, v1));
     v0 = a; v1 = b;
+}
+
+// vbar <- M^H vbar, the same M
+__device__ __forceinline__ void tf_apply_adjoint(double2 sb, double2 cb, double2 eta, double2& vb0, double2& vb1) {
+    const double2 mis = make_double2(sb.y, -sb.x);
+    const double2 M01 = tf_div(mis, eta), M10 = cmul(mis, eta);
+    const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
+    const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
+    vb0 = nb0; vb1 = nb1;
+}
+
+// the forward sweep from v = v_N on the substrate side, v_k = M_k v_{k+1}, to v = v_0 = (B, C); visit(k, v0, v1) sees
+// every boundary k = N, ..., 0
+template <typename Visit>
+__device__ __forceinline__ void tf_sweep(const TfOps& op, const TfSample& s, int pol, double2& v0, double2& v1,
+                                         Visit&& visit) {
+    visit(op.nlayers, v0, v1);
+    for (int k = op.nlayers - 1; k >= 0; --k) {
+        const TfLayer L = tf_layer(op, s, k, pol);
+        double2 sb, cb;
+        tf_sincos(L.beta, &sb, &cb);
+        tf_apply(sb, cb, L.eta, v0, v1);
+        visit(k, v0, v1);
+    }
 }
 
 __device__ inline double tf_abs2(double2 a) { return a.x * a.x + a.y * a.y; }
@@ -145,28 +174,16 @@ __global__ void stack_eval_kernel(const TfOps op, long long count, TfOut o, TfSt
         // v_k, |v_k,E|^2 and the flux differences are staged in fp64 and scaled by t or |t|^2 once v_0 (hence t)
         // is known
         double g_below = 0.0;
-        if (fields) {
-            const long long ob = (long long)N * count + i;
-            if (sg.E) sg.E[ob] = v0;
-            if (sg.H) sg.H[ob] = v1;
-            if (sg.Esq) sg.Esq[ob] = tf_abs2(v0);
-            g_below = cmulc(v0, v1).x;
-        }
-        for (int k = N - 1; k >= 0; --k) {
-            const TfLayer L = tf_layer(op, s, k);
-            double2 sb, cb;
-            tf_sincos(L.beta, &sb, &cb);
-            tf_apply(sb, cb, L.eta, v0, v1);
-            if (fields) {
-                const long long ok = (long long)k * count + i;
-                if (sg.E) sg.E[ok] = v0;
-                if (sg.H) sg.H[ok] = v1;
-                if (sg.Esq) sg.Esq[ok] = tf_abs2(v0);
-                const double g = cmulc(v0, v1).x;
-                if (sg.A) sg.A[ok] = g - g_below;
-                g_below = g;
-            }
-        }
+        tf_sweep(op, s, op.pol, v0, v1, [&](int k, double2 e, double2 h) {
+            if (!fields) return;
+            const long long ok = (long long)k * count + i;
+            if (sg.E) sg.E[ok] = e;
+            if (sg.H) sg.H[ok] = h;
+            if (sg.Esq) sg.Esq[ok] = tf_abs2(e);
+            const double g = cmulc(e, h).x;
+            if (sg.A && k < N) sg.A[ok] = g - g_below;
+            g_below = g;
+        });
         double2 r, t;
         if (MODE == PB_TF_THINFILM) {
             // multilayer_stack_rt (thinfilm.py:295-311): term1 = 1 / (2 n0 cos0)
@@ -207,8 +224,15 @@ __global__ void stack_eval_kernel(const TfOps op, long long count, TfOut o, TfSt
     }
 }
 
-// cotangent of boundary field k from the field seeds (diff.py:204-224): flux_k = Re(E_k conj H_k) / Re(eta0) enters
-// A_k with +1 and A_{k-1} with -1
+// cotangent (Ebar, Hbar) = (H cf + 2 ce E, E cf) of a boundary field (E, H) (diff.py:204-224), from the coefficients
+// of its flux Re(E conj H) (cf) and of |E|^2 (ce)
+__device__ __forceinline__ void tf_field_cot(double cf, double ce, double2 E, double2 H, double2& Eb, double2& Hb) {
+    Eb = cadd(cscale(H, cf), cscale(E, 2.0 * ce));
+    Hb = cscale(E, cf);
+}
+
+// cotangent of boundary field k from the field seeds: flux_k = Re(E_k conj H_k) / Re(eta0) enters A_k with +1 and
+// A_{k-1} with -1
 __device__ inline void tf_field_bar(const double* dA, const double* dEsq, int N, long long count, long long i, int k,
                                     double inv_re0, double2 E, double2 H, double2& Eb, double2& Hb) {
     double fb = 0.0;
@@ -217,13 +241,69 @@ __device__ inline void tf_field_bar(const double* dA, const double* dEsq, int N,
         if (k > 0) fb -= dA[(long long)(k - 1) * count + i];
     }
     fb *= inv_re0;
-    Eb = cscale(H, fb);
-    Hb = cscale(E, fb);
-    if (dEsq) Eb = cadd(Eb, cscale(E, 2.0 * dEsq[(long long)k * count + i]));
+    tf_field_cot(fb, dEsq ? dEsq[(long long)k * count + i] : 0.0, E, H, Eb, Hb);
 }
 
-// One warp-uniform pass per 32 samples.  Each layer's contribution is summed over the warp and added by lane 0 to the
-// warp's own slot partial[(2 k + kind) * W + warp], written on the warp's first pass: no atomics, a fixed order.
+// vbar_0 = (Bbar, Cbar) from the amplitude cotangents rb, tb through the holomorphic partials of r and t in
+// (B, C) = v_0 (diff.py:162-188); den = eta0 B + C
+__device__ __forceinline__ void tf_seed(double2 r, double2 t, double2 eta0, double2 den, double2 rb, double2 tb,
+                                        double2& vb0, double2& vb1) {
+    const double2 inv_den = tf_div(make_double2(1.0, 0.0), den);
+    const double2 dr_dB = cmul(cmul(eta0, make_double2(1.0 - r.x, -r.y)), inv_den);
+    const double2 dr_dC = cmul(make_double2(-1.0 - r.x, -r.y), inv_den);
+    const double2 dt_dB = cmul(make_double2(-(t.x * eta0.x - t.y * eta0.y), -(t.x * eta0.y + t.y * eta0.x)), inv_den);
+    const double2 dt_dC = cmul(make_double2(-t.x, -t.y), inv_den);
+    vb0 = cadd(cmulc(rb, dr_dB), cmulc(tb, dt_dB));
+    vb1 = cadd(cmulc(rb, dr_dC), cmulc(tb, dt_dC));
+}
+
+// the thickness and index terms of one layer
+struct TfGrad { double th, ix; };
+
+// one layer of the reverse sweep: Mbar_k = vbar_k v_{k+1}^H through char_matrix_vjp (diff.py:22-60), the terms
+// `kinds` asks for (0 otherwise), then vbar <- M_k^H vbar.  n0sq_sin2 = n0^2 sin^2 theta0.
+__device__ __forceinline__ TfGrad tf_reverse_step(const TfLayer& L, double2 sb, double2 cb, double2 w0, double2 w1,
+                                                  int kinds, double2 n0sq_sin2, double wvl, int pol, double2& vb0,
+                                                  double2& vb1) {
+    const double2 m00 = cmulc(vb0, w0), m01 = cmulc(vb0, w1), m10 = cmulc(vb1, w0), m11 = cmulc(vb1, w1);
+    // c = sum conj(dM) * Mbar
+    const double2 ieta = tf_div(make_double2(1.0, 0.0), L.eta);
+    const double2 icb = make_double2(cb.y, -cb.x);                 // -i cos b
+    const double2 dB01 = cmul(icb, ieta), dB10 = cmul(icb, L.eta);
+    const double2 cbeta = csub(cadd(cmulc(m01, dB01), cmulc(m10, dB10)), cadd(cmulc(m00, sb), cmulc(m11, sb)));
+    const double2 isb = make_double2(-sb.y, sb.x);                 // i sin b
+    const double2 dE01 = cmul(isb, cmul(ieta, ieta)), dE10 = make_double2(-isb.x, -isb.y);
+    const double2 ceta = cadd(cmulc(m01, dE01), cmulc(m10, dE10));
+    TfGrad g{0.0, 0.0};
+    if (kinds & PB_TF_GRAD_THICKNESS) {
+        // dbeta/dd = 2 pi n cos / wvl (diff.py:110, 307)
+        const double2 dbdd = cscale(cmul(L.n, L.cost), 2.0 * M_PI / wvl);
+        g.th = cmulc(dbdd, cbeta).x;
+    }
+    if (kinds & PB_TF_GRAD_INDEX) {
+        // diff.py:328-339: dcos/dn = n0^2 sin0^2 / (n^3 cos)
+        const double2 n2 = cmul(L.n, L.n);
+        const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
+        const double2 ndc = cmul(L.n, dcdn);
+        const double2 dbdn = cscale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / wvl);
+        const double2 dedn = pol == PB_TF_POL_P
+            ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
+            : cadd(L.cost, ndc);
+        g.ix = cmulc(dbdn, cbeta).x + cmulc(dedn, ceta).x;
+    }
+    tf_apply_adjoint(sb, cb, L.eta, vb0, vb1);
+    return g;
+}
+
+// lane 0 adds the warp's sum of v to its own slot p, written on the warp's first visit: no atomics, a fixed order
+__device__ __forceinline__ void tf_warp_add(double v, bool act, int lane, bool first, double* p) {
+    v = warp_reduce(act ? v : 0.0, OpAdd{});
+    if (lane == 0) *p = first ? v : *p + v;
+}
+
+// One warp-uniform pass per 32 samples.  The sweeping kernels sum each contribution over the warp into the warp's
+// slot of a partial row (row * W + warp), and tf_reduce_kernel sums the rows.  The rows are only those asked for:
+// the thickness rows, then the index rows, N each.
 __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOps op, long long count, int kinds,
                                                                     const double2* __restrict__ E, const double2* __restrict__ H,
                                                                     const double* __restrict__ dR, const double* __restrict__ dT,
@@ -234,13 +314,13 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     const bool fseed = dA || dEsq;
+    const int ix0 = kinds & PB_TF_GRAD_THICKNESS ? N : 0;           // the first index row
     for (long long base = warp * 32; base < count; base += W * 32) {
         const bool first = base == warp * 32;
         const bool act = base + lane < count;
         const long long i = act ? base + lane : count - 1;
         const TfSample s = tf_sample(op, i);
-        const double2 nsub = s.nsub;
-        const double2 eta_sub = tf_admittance(nsub, tf_cos_snell(s.n0, nsub, s.sin0), op.pol);
+        const double2 eta_sub = tf_eta_sub(s, op.pol);
         const double2 eta0 = tf_admittance(s.n0, make_double2(s.cos0, 0.0), op.pol);
         const double inv_re0 = 1.0 / eta0.x;
         const double2 t = E[(long long)N * count + i];                  // f_N = t [1, eta_sub]
@@ -263,14 +343,8 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
                 tb = cadd(tb, cadd(cmulc(eb2, cmul(e, inv_t)), cmulc(hb2, cmul(hh, inv_t))));
             }
         }
-        // (B, C) = v_0 (diff.py:162-188): holomorphic partials of r and t
-        const double2 inv_den = tf_div(make_double2(1.0, 0.0), den);
-        const double2 dr_dB = cmul(cmul(eta0, make_double2(1.0 - r.x, -r.y)), inv_den);
-        const double2 dr_dC = cmul(make_double2(-1.0 - r.x, -r.y), inv_den);
-        const double2 dt_dB = cmul(make_double2(-(t.x * eta0.x - t.y * eta0.y), -(t.x * eta0.y + t.y * eta0.x)), inv_den);
-        const double2 dt_dC = cmul(make_double2(-t.x, -t.y), inv_den);
-        double2 vb0 = cadd(cmulc(rb, dr_dB), cmulc(tb, dt_dB));
-        double2 vb1 = cadd(cmulc(rb, dr_dC), cmulc(tb, dt_dC));
+        double2 vb0, vb1;
+        tf_seed(r, t, eta0, den, rb, tb, vb0, vb1);
         const double2 ct = cconj(t);
         if (fseed) {
             double2 eb2, hb2;
@@ -285,71 +359,36 @@ __global__ void __launch_bounds__(PB_TF_THREADS, 2) stack_grad_kernel(const TfOp
             tf_sincos(L.beta, &sb, &cb);
             const long long o1 = (long long)(k + 1) * count + i;
             const double2 e1 = E[o1], h1 = H[o1];
-            const double2 w0 = cmul(e1, inv_t), w1 = cmul(h1, inv_t);       // v_{k+1}
-            // Mbar = vbar v_{k+1}^H
-            const double2 m00 = cmulc(vb0, w0), m01 = cmulc(vb0, w1), m10 = cmulc(vb1, w0), m11 = cmulc(vb1, w1);
-            // char_matrix_vjp (diff.py:22-60): c = sum conj(dM) * Mbar
-            const double2 ieta = tf_div(make_double2(1.0, 0.0), L.eta);
-            const double2 icb = make_double2(cb.y, -cb.x);                 // -i cos b
-            const double2 dB01 = cmul(icb, ieta), dB10 = cmul(icb, L.eta);
-            const double2 cbeta = csub(cadd(cmulc(m01, dB01), cmulc(m10, dB10)), cadd(cmulc(m00, sb), cmulc(m11, sb)));
-            const double2 isb = make_double2(-sb.y, sb.x);                 // i sin b
-            const double2 dE01 = cmul(isb, cmul(ieta, ieta)), dE10 = make_double2(-isb.x, -isb.y);
-            const double2 ceta = cadd(cmulc(m01, dE01), cmulc(m10, dE10));
-            double gth = 0.0, gix = 0.0;
-            if (kinds & PB_TF_GRAD_THICKNESS) {
-                // dbeta/dd = 2 pi n cos / wvl (diff.py:110, 307)
-                const double2 dbdd = cscale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
-                gth = cmulc(dbdd, cbeta).x;
-            }
-            if (kinds & PB_TF_GRAD_INDEX) {
-                // diff.py:328-339: dcos/dn = n0^2 sin0^2 / (n^3 cos)
-                const double2 n2 = cmul(L.n, L.n);
-                const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
-                const double2 ndc = cmul(L.n, dcdn);
-                const double2 dbdn = cscale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
-                const double2 dedn = op.pol == PB_TF_POL_P
-                    ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
-                    : cadd(L.cost, ndc);
-                gix = cmulc(dbdn, cbeta).x + cmulc(dedn, ceta).x;
-            }
-            // vbar_{k+1} = M_k^H vbar_k (+ conj(t) fbar_{k+1})
-            const double2 mis = make_double2(sb.y, -sb.x);
-            const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
-            const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
-            const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
-            vb0 = nb0; vb1 = nb1;
+            const TfGrad g = tf_reverse_step(L, sb, cb, cmul(e1, inv_t), cmul(h1, inv_t), kinds, n0sq_sin2, s.wvl,
+                                             op.pol, vb0, vb1);
+            // vbar_{k+1} += conj(t) fbar_{k+1}
             if (fseed) {
                 double2 eb2, hb2;
                 tf_field_bar(dA, dEsq, N, count, i, k + 1, inv_re0, e1, h1, eb2, hb2);
                 vb0 = cadd(vb0, cmul(ct, eb2));
                 vb1 = cadd(vb1, cmul(ct, hb2));
             }
-            for (int kind = 0; kind < 2; ++kind) {
-                if (!(kinds & (1 << kind))) continue;
-                const double v = warp_reduce(act ? (kind == 0 ? gth : gix) : 0.0, OpAdd{});
-                if (lane == 0) {
-                    double* p = partial + (long long)(2 * k + kind) * W + warp;
-                    *p = first ? v : *p + v;
-                }
-            }
+            if (kinds & PB_TF_GRAD_THICKNESS) tf_warp_add(g.th, act, lane, first, partial + (long long)k * W + warp);
+            if (kinds & PB_TF_GRAD_INDEX) tf_warp_add(g.ix, act, lane, first, partial + (long long)(ix0 + k) * W + warp);
         }
     }
 }
 
-// grad[row, k] = sum over the first nw warps of partial[(2 k + kind) * W + w], in a fixed order
+// dst[row] = sum over the first nw warps of partial row `row`, in a fixed order, one block per row; with value, the last
+// row goes to *value in fp64 instead.  With accumulate the sums are added to what dst and value hold.
 template <typename R>
-__global__ void __launch_bounds__(PB_TF_THREADS) stack_grad_reduce_kernel(const double* __restrict__ partial, long long W,
-                                                                           long long nw, int N, int kinds, R* __restrict__ grad) {
+__global__ void __launch_bounds__(PB_TF_THREADS) tf_reduce_kernel(const double* __restrict__ partial, long long W,
+                                                                   long long nw, int accumulate, R* __restrict__ dst,
+                                                                   double* __restrict__ value) {
     __shared__ double sh[PB_TF_THREADS];
-    const int k = blockIdx.x % N, kind = blockIdx.x / N;
-    if (!(kinds & (1 << kind))) return;
-    const int row = kinds == (PB_TF_GRAD_THICKNESS | PB_TF_GRAD_INDEX) ? kind : 0;
-    const double* p = partial + (long long)(2 * k + kind) * W;
-    double acc = 0.0;
-    for (long long w = threadIdx.x; w < nw; w += blockDim.x) acc += p[w];
-    acc = tree_sum<PB_TF_THREADS>(acc, sh);
-    if (threadIdx.x == 0) grad[(long long)row * N + k] = (R)acc;
+    const int row = blockIdx.x;
+    const double* p = partial + (long long)row * W;
+    double a = 0.0;
+    for (long long w = threadIdx.x; w < nw; w += blockDim.x) a += p[w];
+    a = tree_sum<PB_TF_THREADS>(a, sh);
+    if (threadIdx.x) return;
+    if (value && row == gridDim.x - 1) *value = accumulate ? *value + a : a;
+    else dst[row] = accumulate ? dst[row] + (R)a : (R)a;
 }
 
 // stack.py:252-301: searchsorted(Z, z, 'right') - 1 clipped to [0, N - 1], then the partial layer below z applied to
@@ -404,6 +443,11 @@ struct CmTerm {
     long long cpad;                // stage pitch: count rounded up to whole warps
 };
 
+struct NeedleStrides { long long st[PB_TF_DIMS]; };
+
+// offset of sample i in a per-sample operand of strides st.  Target, weight and the needle index take this
+// decomposition of their own rather than travelling in TfOps through tf_sample's: that way the needle kernel keeps 118
+// registers, against 122 when their offsets come from tf_sample (and 120 with the needle index in CmTerm).
 __device__ inline long long cm_offset(const TfOps& op, const long long* st, long long i) {
     long long off = 0;
     for (int j = PB_TF_DIMS - 1; j >= 0; --j) {
@@ -430,19 +474,11 @@ __device__ inline CmFwd cm_rt(const TfSample& s, int pol, double2 v0, double2 v1
 
 __device__ inline CmFwd cm_forward(const TfOps& op, const TfSample& s, int pol, double2* V0, double2* V1,
                                    long long pitch, long long is) {
-    const int N = op.nlayers;
-    const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
-    double2 v0 = make_double2(1.0, 0.0), v1 = eta_sub;
-    V0[(long long)N * pitch + is] = v0;
-    V1[(long long)N * pitch + is] = v1;
-    for (int k = N - 1; k >= 0; --k) {
-        const TfLayer L = tf_layer(op, s, k, pol);
-        double2 sb, cb;
-        tf_sincos(L.beta, &sb, &cb);
-        tf_apply(sb, cb, L.eta, v0, v1);
-        V0[(long long)k * pitch + is] = v0;
-        V1[(long long)k * pitch + is] = v1;
-    }
+    double2 v0 = make_double2(1.0, 0.0), v1 = tf_eta_sub(s, pol);
+    tf_sweep(op, s, pol, v0, v1, [&](int k, double2 e, double2 h) {
+        V0[(long long)k * pitch + is] = e;
+        V1[(long long)k * pitch + is] = h;
+    });
     return cm_rt(s, pol, v0, v1);
 }
 
@@ -451,10 +487,7 @@ __device__ inline double cm_quantity(const CmTerm& tm, const TfSample& s, int po
                                      const double2* V1, long long pitch, long long is, int* arg) {
     switch (tm.quantity) {
     case PB_CM_Q_R: return tf_abs2(f.r);
-    case PB_CM_Q_T: {
-        const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
-        return eta_sub.x / f.eta0.x * f.t2;
-    }
+    case PB_CM_Q_T: return tf_eta_sub(s, pol).x / f.eta0.x * f.t2;
     case PB_CM_Q_ABS: {
         const long long o = (long long)tm.b0 * pitch + is;
         const double g0 = cmulc(V0[o], V1[o]).x, g1 = cmulc(V0[o + pitch], V1[o + pitch]).x;
@@ -481,8 +514,7 @@ __device__ inline void cm_field_bar(const CmSeed& sd, int k, double2 E, double2 
     double cf = 0.0, ce = 0.0;
     if (k == sd.ka) { cf += sd.cfa; ce += sd.cea; }
     if (k == sd.kb) { cf += sd.cfb; ce += sd.ceb; }
-    Eb = cadd(cscale(H, cf), cscale(E, 2.0 * ce));
-    Hb = cscale(E, cf);
+    tf_field_cot(cf, ce, E, H, Eb, Hb);
 }
 
 // the reverse-sweep start of one polarisation: vbar_0 from the amplitude and field seeds of dq, and the field seeds
@@ -494,10 +526,8 @@ __device__ inline void cm_seed(const CmTerm& tm, const TfSample& s, int pol, con
     sd.cfa = sd.cea = sd.cfb = sd.ceb = 0.0;
     double2 rb = make_double2(0.0, 0.0), tb = make_double2(0.0, 0.0);
     if (tm.quantity == PB_CM_Q_R) rb = cscale(f.r, 2.0 * dq);
-    else if (tm.quantity == PB_CM_Q_T) {
-        const double2 eta_sub = tf_admittance(s.nsub, tf_cos_snell(s.n0, s.nsub, s.sin0), pol);
-        tb = cscale(f.t, 2.0 * (eta_sub.x * inv_re0) * dq);
-    } else if (tm.quantity == PB_CM_Q_ABS) {
+    else if (tm.quantity == PB_CM_Q_T) tb = cscale(f.t, 2.0 * (tf_eta_sub(s, pol).x * inv_re0) * dq);
+    else if (tm.quantity == PB_CM_Q_ABS) {
         sd.ka = tm.b0; sd.cfa = dq * inv_re0;
         sd.kb = tm.b0 + 1; sd.cfb = -dq * inv_re0;
     } else if (tm.quantity == PB_CM_Q_ESQ) {
@@ -517,15 +547,7 @@ __device__ inline void cm_seed(const CmTerm& tm, const TfSample& s, int pol, con
         cm_field_bar(sd, k, cmul(f.t, v0), cmul(f.t, v1), eb2, hb2);
         tb = cadd(tb, cadd(cmulc(eb2, v0), cmulc(hb2, v1)));
     }
-    const double2 eb = cmul(f.eta0, V0[is]);
-    const double2 inv_den = tf_div(make_double2(1.0, 0.0), cadd(eb, V1[is]));
-    const double2 dr_dB = cmul(cmul(f.eta0, make_double2(1.0 - f.r.x, -f.r.y)), inv_den);
-    const double2 dr_dC = cmul(make_double2(-1.0 - f.r.x, -f.r.y), inv_den);
-    const double2 dt_dB = cmul(make_double2(-(f.t.x * f.eta0.x - f.t.y * f.eta0.y), -(f.t.x * f.eta0.y + f.t.y * f.eta0.x)),
-                               inv_den);
-    const double2 dt_dC = cmul(make_double2(-f.t.x, -f.t.y), inv_den);
-    vb0 = cadd(cmulc(rb, dr_dB), cmulc(tb, dt_dB));
-    vb1 = cadd(cmulc(rb, dr_dC), cmulc(tb, dt_dC));
+    tf_seed(f.r, f.t, f.eta0, cadd(cmul(f.eta0, V0[is]), V1[is]), rb, tb, vb0, vb1);
     if (sd.ka == 0 || sd.kb == 0) {
         double2 eb2, hb2;
         cm_field_bar(sd, 0, cmul(f.t, V0[is]), cmul(f.t, V1[is]), eb2, hb2);
@@ -538,13 +560,7 @@ __device__ inline void cm_seed(const CmTerm& tm, const TfSample& s, int pol, con
 // a / x for a real x, as numpy divides a complex array by a real one
 __device__ inline double2 cm_over(double2 a, double x) { return make_double2(a.x / x, a.y / x); }
 
-// lane 0 adds the warp's sum of v to its own slot p (written on the warp's first visit)
-__device__ inline void cm_warp_add(double v, bool act, int lane, bool first, double* p) {
-    v = warp_reduce(act ? v : 0.0, OpAdd{});
-    if (lane == 0) *p = first ? v : *p + v;
-}
-
-// partial rows: kind * N + k for the gradients, 2 N for the value
+// partial rows: the gradient rows, then the value row
 template <int NPOL>
 __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) coating_merit_kernel(const TfOps op, const CmTerm tm, long long count,
                                                                        int flags, double2* __restrict__ V0,
@@ -555,6 +571,8 @@ __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) coating_m
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     const int kinds = (flags >> 2) & 3;
+    const int ix0 = kinds & PB_TF_GRAD_THICKNESS ? N : 0;           // the first index row
+    const long long vrow = ix0 + (kinds & PB_TF_GRAD_INDEX ? N : 0);
     const long long pitch = tm.cpad;
     for (long long base = warp * 32; base < count; base += W * 32) {
         const bool first = base == warp * 32;
@@ -583,7 +601,7 @@ __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) coating_m
             if (resid_f32) ((float*)resid)[i] = (float)res;
             else ((double*)resid)[i] = res;
         }
-        if (flags & PB_CM_OUT_VALUE) cm_warp_add(w * (d * d), act, lane, first, partial + (long long)(2 * N) * W + warp);
+        if (flags & PB_CM_OUT_VALUE) tf_warp_add(w * (d * d), act, lane, first, partial + vrow * W + warp);
         if (!kinds) continue;
         const double dq = 2.0 * w * d / NPOL;
 #pragma unroll 1
@@ -603,84 +621,22 @@ __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) coating_m
                 tf_sincos(L.beta, &sb, &cb);
                 const long long o1 = (long long)(k + 1) * pitch + is;
                 const double2 w0 = v0[o1], w1 = v1[o1];                         // v_{k+1}
-                const double2 m00 = cmulc(vb0, w0), m01 = cmulc(vb0, w1), m10 = cmulc(vb1, w0), m11 = cmulc(vb1, w1);
-                const double2 ieta = tf_div(make_double2(1.0, 0.0), L.eta);
-                const double2 icb = make_double2(cb.y, -cb.x);                 // -i cos b
-                const double2 dB01 = cmul(icb, ieta), dB10 = cmul(icb, L.eta);
-                const double2 cbeta = csub(cadd(cmulc(m01, dB01), cmulc(m10, dB10)), cadd(cmulc(m00, sb), cmulc(m11, sb)));
-                if (kinds & PB_TF_GRAD_THICKNESS) {
-                    const double2 dbdd = cscale(cmul(L.n, L.cost), 2.0 * M_PI / s.wvl);
-                    cm_warp_add(cmulc(dbdd, cbeta).x, act, lane, first && p == 0, partial + (long long)k * W + warp);
-                }
-                if (kinds & PB_TF_GRAD_INDEX) {
-                    const double2 isb = make_double2(-sb.y, sb.x);             // i sin b
-                    const double2 dE01 = cmul(isb, cmul(ieta, ieta)), dE10 = make_double2(-isb.x, -isb.y);
-                    const double2 ceta = cadd(cmulc(m01, dE01), cmulc(m10, dE10));
-                    const double2 n2 = cmul(L.n, L.n);
-                    const double2 dcdn = tf_div(n0sq_sin2, cmul(cmul(n2, L.n), L.cost));
-                    const double2 ndc = cmul(L.n, dcdn);
-                    const double2 dbdn = cscale(cadd(L.cost, ndc), 2.0 * M_PI * L.d / s.wvl);
-                    const double2 dedn = pol == PB_TF_POL_P
-                        ? csub(tf_div(make_double2(1.0, 0.0), L.cost), tf_div(ndc, cmul(L.cost, L.cost)))
-                        : cadd(L.cost, ndc);
-                    cm_warp_add(cmulc(dbdn, cbeta).x + cmulc(dedn, ceta).x, act, lane, first && p == 0,
-                                partial + (long long)(N + k) * W + warp);
-                }
-                // vbar_{k+1} = M_k^H vbar_k (+ conj(t) fbar_{k+1})
-                const double2 mis = make_double2(sb.y, -sb.x);
-                const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
-                const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
-                const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
-                vb0 = nb0; vb1 = nb1;
+                const TfGrad g = tf_reverse_step(L, sb, cb, w0, w1, kinds, n0sq_sin2, s.wvl, pol, vb0, vb1);
+                // vbar_{k+1} += conj(t) fbar_{k+1}
                 if (k + 1 == sd.ka || k + 1 == sd.kb) {
                     double2 eb2, hb2;
                     cm_field_bar(sd, k + 1, cmul(f.t, w0), cmul(f.t, w1), eb2, hb2);
                     vb0 = cadd(vb0, cmul(ct, eb2));
                     vb1 = cadd(vb1, cmul(ct, hb2));
                 }
+                if (kinds & PB_TF_GRAD_THICKNESS)
+                    tf_warp_add(g.th, act, lane, first && p == 0, partial + (long long)k * W + warp);
+                if (kinds & PB_TF_GRAD_INDEX)
+                    tf_warp_add(g.ix, act, lane, first && p == 0, partial + (long long)(ix0 + k) * W + warp);
             }
         }
     }
 }
-
-// one block per partial row, the first nw warps summed in a fixed order: gradient rows into grad, the value row into
-// value (fp64); residuals rounded once to R
-// P[z] from the nz rows of needle partials, in the same fixed order
-template <typename R>
-__global__ void __launch_bounds__(PB_TF_THREADS) needle_reduce_kernel(const double* __restrict__ partial, long long W,
-                                                                       long long nw, int accumulate, R* __restrict__ P) {
-    __shared__ double sh[PB_TF_THREADS];
-    const double* p = partial + (long long)blockIdx.x * W;
-    double a = 0.0;
-    for (long long w = threadIdx.x; w < nw; w += blockDim.x) a += p[w];
-    a = tree_sum<PB_TF_THREADS>(a, sh);
-    if (threadIdx.x == 0) P[blockIdx.x] = accumulate ? P[blockIdx.x] + (R)a : (R)a;
-}
-
-template <typename R>
-__global__ void __launch_bounds__(PB_TF_THREADS) coating_merit_reduce_kernel(const double* __restrict__ partial,
-                                                                              long long W, long long nw, int N, int flags,
-                                                                              double* __restrict__ value,
-                                                                              R* __restrict__ grad) {
-    __shared__ double sh[PB_TF_THREADS];
-    const int row = blockIdx.x;
-    const bool acc = flags & PB_CM_ACCUMULATE;
-    const int kinds = (flags >> 2) & 3;
-    if (row < 2 * N) {
-        if (!(kinds & (1 << (row / N)))) return;
-    } else if (!(flags & PB_CM_OUT_VALUE)) return;
-    const double* p = partial + (long long)row * W;
-    double a = 0.0;
-    for (long long w = threadIdx.x; w < nw; w += blockDim.x) a += p[w];
-    a = tree_sum<PB_TF_THREADS>(a, sh);
-    if (threadIdx.x) return;
-    if (row == 2 * N) { *value = acc ? *value + a : a; return; }
-    const int kind = row / N, k = row % N;
-    R* g = grad + (kinds == (PB_TF_GRAD_THICKNESS | PB_TF_GRAD_INDEX) ? kind * N : 0) + k;
-    *g = acc ? *g + (R)a : (R)a;
-}
-
-struct NeedleStrides { long long st[PB_TF_DIMS]; };
 
 // P(z) of an R or T term (needle.py:18-91).  The assembled-matrix cotangent of diff.py's _rt_assembly_cotangent is
 // c_M = u w^H with u = (Bbar, Cbar) and w = (1, eta_sub), so Re tr(c_M^H L_j X R_{j+1}) = Re(vbar_j^H X v_{j+1}) with
@@ -746,19 +702,21 @@ __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) needle_ke
                     x0 = y0; x1 = y1;
                     tf_sincos(cscale(dbdd, zpart[zi]), &sb, &cb);
                     tf_apply(sb, cb, L.eta, x0, x1);
-                    cm_warp_add(cmulc(x0, vb0).x + cmulc(x1, vb1).x, act, lane, first && p == 0,
+                    tf_warp_add(cmulc(x0, vb0).x + cmulc(x1, vb1).x, act, lane, first && p == 0,
                                 partial + (long long)zi * W + warp);
                 }
                 double2 sb, cb;
                 tf_sincos(L.beta, &sb, &cb);
-                const double2 mis = make_double2(sb.y, -sb.x);
-                const double2 M01 = tf_div(mis, L.eta), M10 = cmul(mis, L.eta);
-                const double2 nb0 = cadd(cmulc(vb0, cb), cmulc(vb1, M10));
-                const double2 nb1 = cadd(cmulc(vb0, M01), cmulc(vb1, cb));
-                vb0 = nb0; vb1 = nb1;
+                tf_apply_adjoint(sb, cb, L.eta, vb0, vb1);
             }
         }
     }
+}
+
+// the n values of an outermost-first array of the C ABI right-aligned to PB_TF_DIMS dims, `fill` in front: the
+// calculation shape (fill 1) or an operand's strides (fill 0)
+static void tf_align(const long long* src, int n, long long fill, long long* dst) {
+    for (int j = 0; j < PB_TF_DIMS; ++j) dst[j] = j >= PB_TF_DIMS - n ? src[j - (PB_TF_DIMS - n)] : fill;
 }
 
 static int tf_ops(Handle* h, int pol, int nlayers, int ndim, const long long* shape, const long long* strides,
@@ -767,26 +725,34 @@ static int tf_ops(Handle* h, int pol, int nlayers, int ndim, const long long* sh
     if (nlayers < 0) return fail(h, PB_ERR_INVALID, "thinfilm: nlayers must be >= 0");
     if (ndim < 0 || ndim > PB_TF_DIMS) return fail(h, PB_ERR_INVALID, "thinfilm: the calculation shape has at most 4 dims");
     if ((ndim && !shape) || !strides || !in) return fail(h, PB_ERR_INVALID, "thinfilm: missing shape, strides or operands");
+    tf_align(shape, ndim, 1, op.shape);
     count = 1;
     for (int j = 0; j < PB_TF_DIMS; ++j) {
-        const int src = j - (PB_TF_DIMS - ndim);
-        op.shape[j] = src >= 0 ? shape[src] : 1;
         if (op.shape[j] < 0) return fail(h, PB_ERR_INVALID, "thinfilm: negative extent");
         count *= op.shape[j];
     }
     for (int q = 0; q < PB_TF_NOPS; ++q) {
-        op.p[q] = in[q];
         const bool layered = q == PB_TF_IN_N || q == PB_TF_IN_D;
         if (!in[q] && (!layered || nlayers > 0)) return fail(h, PB_ERR_INVALID, "thinfilm: missing operand");
-        for (int j = 0; j < PB_TF_DIMS; ++j) {
-            const int src = j - (PB_TF_DIMS - ndim);
-            op.st[q][j] = src >= 0 ? strides[5 * q + src] : 0;
-        }
+        op.p[q] = in[q];
+        tf_align(strides + 5 * q, ndim, 0, op.st[q]);
         op.st[q][PB_TF_DIMS] = layered ? strides[5 * q + PB_TF_DIMS] : 0;
     }
     op.nlayers = nlayers;
     op.pol = pol;
     op.theta_scale = 1.0;
+    return PB_OK;
+}
+
+// the second launch of a sweeping kernel with W warp slots per row: tf_reduce_kernel over its `rows` partial rows
+static int tf_reduce(Handle* h, cudaStream_t st, int dtype, const double* partial, long long W, long long count,
+                     long long rows, int accumulate, void* dst, double* value) {
+    const long long nw = std::min<long long>(W, (count + 31) / 32);     // warps that had at least one sample
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        tf_reduce_kernel<R><<<(unsigned)rows, PB_TF_THREADS, 0, st>>>(partial, W, nw, accumulate, (R*)dst, value);
+    });
+    PB_LAUNCH_CHECK(h);
     return PB_OK;
 }
 
@@ -854,20 +820,13 @@ extern "C" int pb_stack_grad(pb_handle_t hh, int dtype, int pol, int kinds, int 
     }
     const int g = grid_for(count, PB_TF_THREADS, h->sm_count);
     const long long W = (long long)g * (PB_TF_THREADS / 32);
-    const long long nw = std::min<long long>(W, (count + 31) / 32);     // warps that had at least one sample
     void* partial = nullptr;
-    PB_TRY(ensure_scratch(h, 2, (size_t)2 * nlayers * W * sizeof(double), &partial));
+    PB_TRY(ensure_scratch(h, 2, (size_t)ng * nlayers * W * sizeof(double), &partial));
     stack_grad_kernel<<<g, PB_TF_THREADS, 0, st>>>(op, count, kinds, (const double2*)E, (const double2*)H,
                                                    (const double*)seeds[0], (const double*)seeds[1],
                                                    (const double*)seeds[2], (const double*)seeds[3], (double*)partial);
     PB_LAUNCH_CHECK(h);
-    with_real(dtype, [&](auto r) {
-        using R = decltype(r);
-        stack_grad_reduce_kernel<R><<<2 * nlayers, PB_TF_THREADS, 0, st>>>((const double*)partial, W, nw, nlayers, kinds,
-                                                                           (R*)grad);
-    });
-    PB_LAUNCH_CHECK(h);
-    return PB_OK;
+    return tf_reduce(h, st, dtype, (const double*)partial, W, count, (long long)ng * nlayers, 0, grad, nullptr);
 }
 
 extern "C" int pb_field_at_depth(pb_handle_t hh, int dtype, int pol, int nlayers, const void* z, long long nz,
@@ -903,11 +862,8 @@ static int cm_setup(Handle* h, int quantity, int pol, int nlayers, int ndim, con
     tm.npol = pol == PB_CM_POL_AVG ? 2 : 1;
     tm.tgt = (const double*)in[PB_CM_IN_TARGET];
     tm.wgt = (const double*)in[PB_CM_IN_WEIGHT];
-    for (int j = 0; j < PB_TF_DIMS; ++j) {
-        const int src = j - (PB_TF_DIMS - ndim);
-        tm.st_tgt[j] = src >= 0 ? strides[5 * PB_CM_IN_TARGET + src] : 0;
-        tm.st_wgt[j] = src >= 0 ? strides[5 * PB_CM_IN_WEIGHT + src] : 0;
-    }
+    tf_align(strides + 5 * PB_CM_IN_TARGET, ndim, 0, tm.st_tgt);
+    tf_align(strides + 5 * PB_CM_IN_WEIGHT, ndim, 0, tm.st_wgt);
     tm.cpad = (count + 31) / 32 * 32;
     tm.b0 = tm.b1 = tm.nb = 0;
     tm.blist = nullptr;
@@ -958,25 +914,19 @@ extern "C" int pb_coating_merit(pb_handle_t hh, int dtype, int quantity, int pol
         if (!acc && kinds && nlayers) PB_CUDA(h, cudaMemsetAsync(grad, 0, (size_t)ng * nlayers * rsize(dtype), st));
         return PB_OK;
     }
+    const long long rows = (long long)ng * nlayers + (flags & PB_CM_OUT_VALUE ? 1 : 0);
     const int nt = cm_threads(tm.npol);
     const int g = grid_for(count, nt, h->sm_count);
     const long long W = (long long)g * (nt / 32);
-    const long long nw = std::min<long long>(W, (count + 31) / 32);
     double* partial;
     double2 *V0, *V1;
-    PB_TRY(cm_scratch(h, tm, nlayers, 2LL * nlayers + 1, W, &partial, &V0, &V1));
+    PB_TRY(cm_scratch(h, tm, nlayers, rows, W, &partial, &V0, &V1));
     if (tm.npol == 2) coating_merit_kernel<2><<<g, nt, 0, st>>>(op, tm, count, flags, V0, V1, partial, residuals,
                                                                 dtype == PB_C64);
     else coating_merit_kernel<1><<<g, nt, 0, st>>>(op, tm, count, flags, V0, V1, partial, residuals, dtype == PB_C64);
     PB_LAUNCH_CHECK(h);
-    if (!(flags & PB_CM_OUT_VALUE) && !(kinds && nlayers)) return PB_OK;
-    with_real(dtype, [&](auto r) {
-        using R = decltype(r);
-        coating_merit_reduce_kernel<R><<<2 * nlayers + 1, PB_TF_THREADS, 0, st>>>(partial, W, nw, nlayers, flags,
-                                                                                   (double*)value, (R*)grad);
-    });
-    PB_LAUNCH_CHECK(h);
-    return PB_OK;
+    if (!rows) return PB_OK;
+    return tf_reduce(h, st, dtype, partial, W, count, rows, acc, grad, flags & PB_CM_OUT_VALUE ? (double*)value : nullptr);
 }
 
 extern "C" int pb_needle(pb_handle_t hh, int dtype, int quantity, int pol, int nlayers, int ndim, const long long* shape,
@@ -997,31 +947,20 @@ extern "C" int pb_needle(pb_handle_t hh, int dtype, int quantity, int pol, int n
         if (!accumulate) PB_CUDA(h, cudaMemsetAsync(P, 0, (size_t)nz * rsize(dtype), st));
         return PB_OK;
     }
-    long long st_nn[PB_TF_DIMS];
-    for (int j = 0; j < PB_TF_DIMS; ++j) {
-        const int src = j - (PB_TF_DIMS - ndim);
-        st_nn[j] = src >= 0 ? strides[5 * PB_CM_IN_NEEDLE + src] : 0;
-    }
     const int nt = cm_threads(tm.npol);
     const int g = grid_for(count, nt, h->sm_count);
     const long long W = (long long)g * (nt / 32);
-    const long long nw = std::min<long long>(W, (count + 31) / 32);
     double* partial;
     double2 *V0, *V1;
     PB_TRY(cm_scratch(h, tm, nlayers, nz, W, &partial, &V0, &V1));
     NeedleStrides ns;
-    for (int j = 0; j < PB_TF_DIMS; ++j) ns.st[j] = st_nn[j];
+    tf_align(strides + 5 * PB_CM_IN_NEEDLE, ndim, 0, ns.st);
     auto launch = [&](auto kern) {
         kern<<<g, nt, 0, st>>>(op, tm, (const double2*)in[PB_CM_IN_NEEDLE], ns, count, (const double*)zpart, nz,
-                                          (const int*)zlist, V0, V1, partial);
+                               (const int*)zlist, V0, V1, partial);
     };
     if (tm.npol == 2) launch(needle_kernel<2>);
     else launch(needle_kernel<1>);
     PB_LAUNCH_CHECK(h);
-    with_real(dtype, [&](auto r) {
-        using R = decltype(r);
-        needle_reduce_kernel<R><<<(unsigned)nz, PB_TF_THREADS, 0, st>>>(partial, W, nw, accumulate, (R*)P);
-    });
-    PB_LAUNCH_CHECK(h);
-    return PB_OK;
+    return tf_reduce(h, st, dtype, partial, W, count, nz, accumulate, P, nullptr);
 }
