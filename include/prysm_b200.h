@@ -784,6 +784,40 @@ int pb_needle(pb_handle_t h, int dtype, int quantity, int pol, int nlayers, int 
               const long long* strides, const void* const* in, const void* zpart, long long nz, const void* zlist, void* P,
               int accumulate, void* stream);
 
+/* ---- Optical monitoring (prysm/x/coatings monitoring.py) on the thin-film chain above -------------------------------
+ * The monitor signal of a (B, C) = v is R = |r|^2 (PB_MON_R) or T = Re eta_sub / Re eta0 |t|^2 (PB_MON_T), r and t as
+ *   in coatings mode.  All arithmetic is fp64; outputs are rounded once to dtype's real type.
+ * pb_monitor_runs: simulate_run for `runs` as-built runs in one launch, one CTA per run; run r monitors at candidate
+ *   c = r / per_cand (runs <= ncand * per_cand).  in (HOST array of PB_TF_NOPS device pointers, dense): wavelength,
+ *   angle (radians), ambient and substrate index (ncand each), the layer indices (complex128, (nlayers, ncand)) at each
+ *   candidate's wavelength, and the nominal thicknesses (fp64, nlayers).  From v = [1, eta_sub], for k = nlayers - 1,
+ *   ..., 0 the signal of M_k(d_j) v is taken on the grid d_j = numpy.linspace(start, max_factor d_k, n_points), and
+ *   the layer stops at
+ *     PB_MON_LEVEL: the crossing of the level levels[c, k] (+ err[r, k]) nearest d_k, the first on a tie, at
+ *       d_i + frac (d_i+1 - d_i), frac = -s_i / (s_i+1 - s_i) (0 when equal), s = signal - level, a crossing wherever
+ *       sign(s_i) != sign(s_i+1); with none, the d of the first minimum of |s|.  levels (fp64, (ncand, nlayers));
+ *       n_points >= 1.
+ *     PB_MON_TURNING: the turning_index-th (>= 1) turning point, i + 1 wherever sign(sig_i+1 - sig_i) changes, or d_k
+ *       when there are fewer; then + err[r, k].
+ *   asbuilt[r, k] = max(d_real, 0), and v <- M_k(asbuilt[r, k]) v in fp64.  err (fp64, (runs, nlayers)) may be NULL.
+ *   Fixed-order block reductions, no atomics: repeated calls are bit-identical.
+ * pb_monitor_cut: level_cut (PB_MON_LEVEL: out[0] = the cut at `level` nearest `target`, NaN for the first crossing;
+ *   n >= 1) or turning_points (PB_MON_TURNING: out[0, *count) = the d of every turning point, count one device int64) of
+ *   the trace d, sig (n each, dtype's real type), with the arithmetic in that type.  One launch.
+ * pb_monitor_jacobian: J[c, w, k] = (Rr[c (nlayers + 1) + 1 + k, w] - Rr[c (nlayers + 1), w]) / eps for the realized
+ *   reflectance Rr (fp64, (ncand (nlayers + 1), nw)) of each candidate's base run followed by its nlayers perturbed
+ *   runs, and score[c] = sqrt(sum over w, k of J^2) by the fixed-order grid fold (DESIGN.md §4.4).  J ((ncand, nw,
+ *   nlayers)) or score (ncand) may be NULL.  One launch, ncand <= 65535. */
+typedef enum { PB_MON_LEVEL = 0, PB_MON_TURNING = 1 } pb_mon_strategy;
+typedef enum { PB_MON_R = 0, PB_MON_T = 1 } pb_mon_mode;
+int pb_monitor_runs(pb_handle_t h, int dtype, int strategy, int mode, int pol, int nlayers, long long ncand,
+                    const void* const* in, long long runs, long long per_cand, const void* err, const void* levels,
+                    long long n_points, double start, double max_factor, int turning_index, void* asbuilt, void* stream);
+int pb_monitor_cut(pb_handle_t h, int dtype, int strategy, const void* d, const void* sig, long long n, double level,
+                   double target, void* out, void* count, void* stream);
+int pb_monitor_jacobian(pb_handle_t h, int dtype, int ncand, int nlayers, long long nw, const void* Rr, double eps,
+                        void* J, void* score, void* stream);
+
 /* ---- PSF / MTF analysis (prysm/_richdata.py, prysm/coordinates.py uniform_cart_to_polar, prysm/psf.py, prysm/otf.py) --
  * Data is (ny, nx) on the fp64 ascending axes xax (nx) and yax (ny), device arrays.  Every sampling entry point uses one
  * linear interpolator, scipy's RegularGridInterpolator(method='linear'): interval = the largest i with axis[i] <= p

@@ -1467,6 +1467,43 @@ def needle(quantity, pol, ops, zpart, zlist, P, accumulate):
           int(zpart.shape[1]), _p(zlist), _p(P), int(bool(accumulate)))
 
 
+def monitor_runs(strategy, mode, pol, ops, runs, per_cand, err, levels, n_points, start, max_factor, turning_index,
+                 rdtype):
+    """(runs, N) as-built thicknesses in rdtype from one pb_monitor_runs launch: ops = wavelength, angle, ambient and
+    substrate index (ncand each), layer indices (N, ncand) and nominal thicknesses (N), dense fp64 / complex128 device
+    arrays; err (runs, N) and levels (ncand, N) fp64 or None."""
+    nlayers = int(ops[capi.TF_IN_D].shape[0])
+    out = torch.empty((runs, nlayers), dtype=rdtype, device=ops[0].device)
+    ins = (C.c_void_p * capi.TF_NOPS)(*[t.data_ptr() for t in ops])
+    _call(lib.pb_monitor_runs, ops[0], _CODE[rdtype], int(strategy), int(mode), int(pol), nlayers,
+          int(ops[capi.TF_IN_WVL].numel()), ins, int(runs), int(per_cand), _p(err), _p(levels), int(n_points),
+          float(start), float(max_factor), int(turning_index), _p(out))
+    return out
+
+
+def monitor_cut(strategy, d, sig, level=0.0, target=float('nan')):
+    """level_cut (a one-element device array) or turning_points (a device array and a device int64 count) of a trace
+    (pb_monitor_cut): d and sig of one real dtype."""
+    d, sig = d.contiguous(), sig.contiguous()
+    n = d.numel()
+    out = torch.empty(max(n, 1), dtype=d.dtype, device=d.device)
+    count = torch.zeros(1, dtype=torch.int64, device=d.device)
+    _call(lib.pb_monitor_cut, d, _CODE[d.dtype], int(strategy), _p(d), _p(sig), n, float(level), float(target),
+          _p(out), _p(count))
+    return out, count
+
+
+def monitor_jacobian(Rr, ncand, nlayers, eps, rdtype, want_J=True):
+    """J (ncand, W, N) and score (ncand) in rdtype from the realized reflectance Rr (ncand (N + 1), W) fp64
+    (pb_monitor_jacobian)."""
+    nw = int(Rr.shape[1])
+    J = torch.empty((ncand, nw, nlayers), dtype=rdtype, device=Rr.device) if want_J else None
+    score = torch.empty(ncand, dtype=rdtype, device=Rr.device)
+    _call(lib.pb_monitor_jacobian, Rr, _CODE[rdtype], int(ncand), int(nlayers), nw, _p(Rr), float(eps), _p(J),
+          _p(score))
+    return J, score
+
+
 def field_at_depth(pol, z, zb, n, n0, wvl, theta0, Eb, Hb, cdtype):
     """E, H (complex, like z) at depths z inside a stack (pb_field_at_depth): z, zb fp64, n, Eb, Hb complex128."""
     z = z.contiguous()

@@ -10,6 +10,7 @@ resolved on the host as the reference's `_resolve` does (a constant, a callable 
 `.nk`) and uploaded as one (layers, *wavelength shape) table.  Angles are radians, thicknesses and wavelengths
 microns.
 """
+import operator
 import types
 
 import numpy as np
@@ -591,3 +592,241 @@ def _host_as_merit(obj):
 def _host_needle_function(stack, targets, needle_material, z):
     """needle_function for the reference's synthesize loop, which takes np.argmin of P: P as a numpy array."""
     return _ops.asnumpy(needle_function(stack, targets, needle_material, z))
+
+
+# ---- optical monitoring (prysm/x/coatings monitoring.py) ----------------------------------------------------------
+# Any number of as-built runs is one pb_monitor_runs launch, one CTA per run: the layers are deposited from the
+# substrate up as a 2-vector sweep, so a layer step costs O(1) where the reference rebuilds the product of every layer
+# below it.  Traces, cutoff levels and the realized reflectance of the as-built stacks are pb_stack_eval launches, and J
+# with its scores one pb_monitor_jacobian launch: simulate_run is 2 launches (levels, runs) and one copy of the N
+# thicknesses, monitoring_error_sensitivity and choose_monitor_wavelength 4 launches whatever the number of candidates,
+# layers or grid points (choose_monitor_wavelength copies its scores once).  The monitor polarization follows the
+# reference's _admittance ('p' in any case is p, anything else s), and a mode other than 'R' monitors T.
+
+_STRATEGIES = {'level': capi.MON_LEVEL, 'turning': capi.MON_TURNING}
+_RUN_KWARGS = ('turning_index', 'signal_errors', 'thickness_errors', 'n_points', 'max_factor', 'levels')
+
+
+def _mon_pol(pol):
+    return capi.TF_POL_P if pol.lower() == 'p' else capi.TF_POL_S
+
+
+def _mon_signal(mode):
+    """(pb_monitor_runs mode, pb_stack_eval output) of the monitored quantity."""
+    return (capi.MON_R, capi.TF_OUT_REFL) if mode == 'R' else (capi.MON_T, capi.TF_OUT_TRANS)
+
+
+def _monitor_operands(stack, wvls, theta):
+    """The six pb_monitor_runs operands of the candidate monitor wavelengths wvls (a sequence): every index resolved on
+    the host at each wavelength as given, as the reference resolves it for one run."""
+    C, N = len(wvls), len(stack)
+    n0 = np.empty(C, dtype=np.complex128)
+    nsub = np.empty(C, dtype=np.complex128)
+    table = np.empty((N, C), dtype=np.complex128)
+    for c, w in enumerate(wvls):
+        n0[c] = _resolve(stack.ambient_index, w)
+        nsub[c] = _resolve(stack.substrate_index, w)
+        for j, n in enumerate(stack.indices):
+            table[j, c] = _resolve(n, w)
+    d = np.asarray(stack.thicknesses, dtype=config.precision)
+    return [_real(np.asarray(wvls, dtype=np.float64)), _real(np.full(C, theta, dtype=np.float64)), _cplx(n0),
+            _cplx(nsub), _cplx(table), _real(d)]
+
+
+def _cutoff(stack, ops, pol, mode):
+    """(C, N) fp64 nominal cutoff levels of the monitor operands `ops` in one pb_stack_eval over the (C, N) samples:
+    sample (c, k) is the stack with the layers above k at zero thickness, an exact identity in the sweep."""
+    N = len(stack)
+    d = np.asarray(stack.thicknesses, dtype=np.float64)
+    D = np.where(np.arange(N)[:, None] >= np.arange(N)[None, :], d[:, None], 0.0)
+    sops = [ops[0][:, None], ops[1][:, None], ops[2][:, None], ops[3][:, None], ops[4][:, :, None],
+            _real(D)[:, None, :]]
+    out = _mon_signal(mode)[1]
+    return _ops.stack_eval(capi.TF_COATINGS, _mon_pol(pol), sops, (out,), torch.float64)[out]
+
+
+def _err_rows(err, N):
+    """per-layer errors as a (rows, N) fp64 device array, or None"""
+    if err is None:
+        return None
+    e = _real(err)
+    if e.shape[-1] < N:
+        # the reference reads errors[k] for every layer k
+        raise IndexError(f'index {e.shape[-1]} is out of bounds for axis 0 with size {e.shape[-1]}')
+    # like the reference, entries past the N-th are not read
+    return (e[:N].reshape(1, N) if e.ndim == 1 else e[:, :N]).contiguous()
+
+
+def _as_built(stack, wvls, runs, per_cand, err, strategy='level', turning_index=1, theta=0.0, pol='s', mode='R',
+              n_points=600, max_factor=1.8, levels=None, rdtype=None):
+    """(runs, N) as-built thicknesses of the runs at the monitor wavelengths wvls, run r at wvls[r // per_cand]; err the
+    (runs, N) fp64 errors of the strategy or None.  Arguments are checked before any launch."""
+    rdtype = _rdtype() if rdtype is None else rdtype
+    N = len(stack)
+    if N == 0 or runs == 0:
+        return torch.empty((runs, N), dtype=rdtype, device=_ops.device())
+    code = _STRATEGIES.get(strategy)
+    if code is None:
+        raise ValueError("strategy must be 'level' or 'turning'")
+    n_points = operator.index(n_points)
+    if n_points < 0:
+        raise ValueError(f'Number of samples, {n_points}, must be non-negative.')
+    if code == capi.MON_LEVEL and n_points == 0:
+        raise ValueError('attempt to get argmin of an empty sequence')
+    if code == capi.MON_TURNING and turning_index < 1:
+        # the reference indexes its list of turning points with turning_index - 1; below 1 that is refused here
+        raise IndexError(f'turning_index must be 1 or more, got {turning_index}')
+    mcode = _mon_signal(mode)[0]
+    ops = _monitor_operands(stack, wvls, theta)
+    lv = None
+    if code == capi.MON_LEVEL:
+        if levels is None:
+            lv = _cutoff(stack, ops, pol, mode)
+        else:
+            lv = _real(levels).reshape(-1, N).expand(len(wvls), N).contiguous()
+    return _ops.monitor_runs(code, mcode, _mon_pol(pol), ops, runs, per_cand, err, lv, n_points, 1e-12,
+                             float(max_factor), int(turning_index), rdtype)
+
+
+def _strategy_errors(strategy, signal_errors, thickness_errors):
+    """the error vector the strategy reads: the level strategy ignores thickness errors, the turning one signal errors"""
+    return signal_errors if strategy == 'level' else thickness_errors if strategy == 'turning' else None
+
+
+def monitoring_trace(stack, layer, monitor_wvl, *, theta=0.0, pol='s', mode='R', n_points=400, max_factor=1.0):
+    """Monitor signal versus deposited thickness while growing layer `layer` (ambient side first; the layers after it,
+    Python's slice `layer + 1:`, lie below): (d grid, signal) as device arrays, one pb_stack_eval launch."""
+    th = np.asarray(stack.thicknesses, dtype=config.precision)
+    d_target = float(th[layer])
+    d_grid = np.linspace(0.0, max_factor * d_target, n_points)
+    below = list(stack.indices[layer + 1:])
+    # the growing layer's thickness varies per sample; the layers below are broadcast
+    D = np.empty((1 + len(below), d_grid.size), dtype=np.float64)
+    D[0] = d_grid
+    D[1:] = th[layer + 1:, None]
+    grow = types.SimpleNamespace(indices=[stack.indices[layer]] + below, thicknesses=D,
+                                 substrate_index=stack.substrate_index, ambient_index=stack.ambient_index)
+    ops, _ = _operands(grow, monitor_wvl, theta)
+    out = _mon_signal(mode)[1]
+    sig = _ops.stack_eval(capi.TF_COATINGS, _mon_pol(pol), ops, (out,), _rdtype())[out]
+    return torch.as_tensor(d_grid.astype(config.precision)).to(_ops.device()), sig
+
+
+def _trace(d, signal):
+    """d and signal as device arrays of one real dtype"""
+    d = d if isinstance(d, torch.Tensor) else torch.as_tensor(np.asarray(d))
+    s = signal if isinstance(signal, torch.Tensor) else torch.as_tensor(np.asarray(signal))
+    dt = torch.promote_types(d.dtype, s.dtype)
+    dt = dt if dt in (torch.float32, torch.float64) else torch.float64
+    return d.to(_ops.device(), dt).reshape(-1), s.to(_ops.device(), dt).reshape(-1)
+
+
+def turning_points(d, signal):
+    """Deposited thicknesses at the turning points (extrema) of a monitor trace: a device array, one launch and one
+    copy (of the count)."""
+    d, s = _trace(d, signal)
+    out, count = _ops.monitor_cut(capi.MON_TURNING, d, s)
+    return out[:int(count.item())]
+
+
+def level_cut(d, signal, level, target=None):
+    """Deposited thickness where the monitor signal crosses `level`: the crossing nearest `target`, or the first one;
+    with none, the thickness of the sample nearest the level.  A Python float, one launch and one copy."""
+    d, s = _trace(d, signal)
+    if d.numel() == 0:
+        raise ValueError('attempt to get argmin of an empty sequence')
+    out, _ = _ops.monitor_cut(capi.MON_LEVEL, d, s, float(level), float('nan') if target is None else float(target))
+    return float(out[0].item())
+
+
+def cutoff_levels(stack, monitor_wvl, *, theta=0.0, pol='s', mode='R', n_points=400):
+    """Nominal monitor level at the end of each layer's deposition (a device array, one launch)."""
+    N = len(stack)
+    if N == 0:
+        return torch.empty(0, dtype=_rdtype(), device=_ops.device())
+    return _cutoff(stack, _monitor_operands(stack, [monitor_wvl], theta), pol, mode)[0].to(_rdtype())
+
+
+def simulate_runs(stack, monitor_wvl, *, signal_errors=None, thickness_errors=None, strategy='level',
+                  turning_index=1, theta=0.0, pol='s', mode='R', n_points=600, max_factor=1.8, levels=None):
+    """Any number of monitored deposition runs in one launch (plus one for the cutoff levels): the (R, N) as-built
+    thicknesses as a device array.  The errors the strategy reads are (N,) or (R, N) (the level strategy reads
+    signal_errors, the turning strategy thickness_errors); monitor_wvl is one wavelength or one per run.  Run r equals
+    simulate_run with row r of the errors at monitor wavelength r, bit for bit."""
+    N = len(stack)
+    wvls = list(np.ravel(monitor_wvl)) if np.ndim(monitor_wvl) else [monitor_wvl]
+    err = _err_rows(_strategy_errors(strategy, signal_errors, thickness_errors), N) if N else None
+    rows = 1 if err is None else err.shape[0]
+    runs = max(rows, len(wvls))
+    if rows not in (1, runs) or len(wvls) not in (1, runs):
+        raise ValueError(f'{len(wvls)} monitor wavelengths and {rows} error rows do not make one set of runs')
+    if err is not None and rows != runs:
+        err = err.expand(runs, N).contiguous()
+    return _as_built(stack, wvls, runs, runs if len(wvls) == 1 else 1, err, strategy=strategy,
+                     turning_index=turning_index, theta=theta, pol=pol, mode=mode, n_points=n_points,
+                     max_factor=max_factor, levels=levels)
+
+
+def simulate_run(stack, monitor_wvl, *, strategy='level', turning_index=1, signal_errors=None, thickness_errors=None,
+                 theta=0.0, pol='s', mode='R', n_points=600, max_factor=1.8, levels=None):
+    """Simulate a monitored deposition run: the as-built stack, of the input stack's class, with host thicknesses."""
+    N = len(stack)
+    err = _err_rows(_strategy_errors(strategy, signal_errors, thickness_errors), N) if N else None
+    th = _as_built(stack, [monitor_wvl], 1, 1, err, strategy=strategy, turning_index=turning_index, theta=theta,
+                   pol=pol, mode=mode, n_points=n_points, max_factor=max_factor, levels=levels)
+    return type(stack)(stack.indices, _ops.asnumpy(th[0]), stack.substrate_index, stack.ambient_index)
+
+
+def _sensitivity(stack, wvls, design_wvls, strategy, theta, pol, design_pol, mode, eps, kwargs, want_J):
+    """(J (C, W, N) or None, scores (C,)) of the candidate monitor wavelengths wvls: each candidate's base run and its N
+    perturbed runs in one pb_monitor_runs launch, their realized reflectance in one pb_stack_eval, J and the scores in
+    one pb_monitor_jacobian."""
+    N, C = len(stack), len(wvls)
+    # the realized reflectance is read as the reference's RTA reads it, which refuses any polarization but s and p
+    ipol = _pol(design_pol)
+    dw = np.atleast_1d(np.asarray(design_wvls, dtype=config.precision))
+    if dw.ndim != 1:
+        raise ValueError(f'design_wvls must be one-dimensional, got shape {dw.shape}')
+    for k in kwargs:
+        if k not in _RUN_KWARGS:
+            raise TypeError(f"simulate_run() got an unexpected keyword argument '{k}'")
+    # the reference hands each perturbed run its own error vector, so one in kwargs is a second value for it
+    own = 'thickness_errors' if strategy == 'turning' else 'signal_errors'
+    if own in kwargs and N:
+        raise TypeError(f"simulate_run() got multiple values for keyword argument '{own}'")
+    kw = {k: v for k, v in kwargs.items() if k not in ('signal_errors', 'thickness_errors')}
+    if N == 0:
+        J = torch.zeros((C, dw.size, 0), dtype=_rdtype(), device=_ops.device()) if want_J else None
+        return J, torch.zeros(C, dtype=_rdtype(), device=_ops.device())
+    E = np.zeros((N + 1, N), dtype=np.float64)
+    E[1:] = np.eye(N) * np.asarray(eps, dtype=config.precision)
+    err = _real(np.tile(E, (C, 1)))
+    th = _as_built(stack, wvls, C * (N + 1), N + 1, err, strategy=strategy, theta=theta, pol=pol, mode=mode,
+                   rdtype=torch.float64, **kw)
+    # the realized reflectance of every as-built stack at the design wavelengths: (runs, W)
+    ops, _ = _operands(stack, dw, theta)
+    ops = [o[None] if o.ndim == 1 else o for o in ops[:4]] + [
+        ops[capi.TF_IN_N][:, None] if ops[capi.TF_IN_N].ndim == 2 else ops[capi.TF_IN_N], th.t()[:, :, None]]
+    Rr = _ops.stack_eval(capi.TF_COATINGS, ipol, ops, (capi.TF_OUT_REFL,),
+                         torch.float64)[capi.TF_OUT_REFL]
+    return _ops.monitor_jacobian(Rr, C, N, float(eps), _rdtype(), want_J)
+
+
+def monitoring_error_sensitivity(stack, monitor_wvl, design_wvls, *, strategy='level', theta=0.0, pol='s',
+                                 design_pol='s', mode='R', eps=1e-4, **kwargs):
+    """Jacobian (len(design_wvls), N) of the realized reflectance with respect to each layer's termination error (a
+    device array); four launches and no copy."""
+    J, _ = _sensitivity(stack, [monitor_wvl], design_wvls, strategy, theta, pol, design_pol, mode, eps, kwargs, True)
+    return J[0]
+
+
+def choose_monitor_wavelength(stack, candidates, design_wvls, *, strategy='level', theta=0.0, pol='s',
+                              design_pol='s', mode='R', eps=1e-4, **kwargs):
+    """The candidate monitor wavelength of lowest error sensitivity sqrt(sum J^2) (a Python float) and every
+    candidate's score (a device array): four launches for all candidates together and one copy (of the scores)."""
+    wvls = list(candidates)
+    if not wvls:
+        raise ValueError('attempt to get argmin of an empty sequence')
+    _, scores = _sensitivity(stack, wvls, design_wvls, strategy, theta, pol, design_pol, mode, eps, kwargs, False)
+    best = float(np.asarray(candidates)[int(np.argmin(_ops.asnumpy(scores)))])
+    return best, scores

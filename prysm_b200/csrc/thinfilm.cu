@@ -8,6 +8,7 @@
 // vbar_{k+1} += M_k^H vbar_k, Mbar_k = vbar_k v_{k+1}^H: v_{k+1} is never recovered from v_k by inverting M_k, which
 // through an absorbing or evanescent layer would amplify the rounding error by about exp(2 |Im beta|).
 // Every operand is fp64 and all arithmetic is fp64 in registers; the outputs are rounded once to the storage type.
+#include <climits>
 #include <cmath>
 
 #include "common.cuh"
@@ -108,12 +109,17 @@ __device__ __forceinline__ double2 tf_eta_sub(const TfSample& s, int pol) {
 // layer k of a sample: index, cos theta_k, phase thickness beta, admittance eta and thickness
 struct TfLayer { double2 n, cost, beta, eta; double d; };
 
+// the phase thickness 2 pi n d cos / wvl of a layer of index n and thickness d
+__device__ __forceinline__ double2 tf_beta(double2 n, double2 cost, double d, double wvl) {
+    return cscale(cmul(cscale(n, 2.0 * M_PI * d), cost), 1.0 / wvl);
+}
+
 __device__ inline TfLayer tf_layer(const TfOps& op, const TfSample& s, int k, int pol) {
     TfLayer L;
     L.n = ((const double2*)op.p[PB_TF_IN_N])[s.off_n + (long long)k * op.st[PB_TF_IN_N][PB_TF_DIMS]];
     L.d = ((const double*)op.p[PB_TF_IN_D])[s.off_d + (long long)k * op.st[PB_TF_IN_D][PB_TF_DIMS]];
     L.cost = tf_cos_snell(s.n0, L.n, s.sin0);
-    L.beta = cscale(cmul(cscale(L.n, 2.0 * M_PI * L.d), L.cost), 1.0 / s.wvl);
+    L.beta = tf_beta(L.n, L.cost, L.d, s.wvl);
     L.eta = tf_admittance(L.n, L.cost, pol);
     return L;
 }
@@ -713,6 +719,215 @@ __global__ void __launch_bounds__(cm_threads(NPOL), NPOL == 2 ? 3 : 2) needle_ke
     }
 }
 
+// ---- optical monitoring (prysm/x/coatings monitoring.py) --------------------------------------------------------
+// One CTA per as-built run deposits the layers from the substrate up: v = [1, eta_sub], and for k = N - 1, ..., 0 the
+// threads stride over the thickness grid d_j, each forming the monitor signal of M_k(d_j) v; the CTA picks the
+// termination thickness by the reference's rule with fixed-order block reductions and every thread advances
+// v <- M_k(d_real) v with the same operations, so v stays uniform over the CTA.  The decisions read the grid in tiles of
+// PB_MON_THREADS samples that overlap by two, so a thread sees samples i, i + 1 and i + 2 without a second evaluation.
+#define PB_MON_THREADS 128
+constexpr int MON_STEP = PB_MON_THREADS - 2;
+
+template <typename T> __device__ inline T mon_sign(T x) { return x > T(0) ? T(1) : x < T(0) ? T(-1) : x == T(0) ? T(0) : x; }
+
+// a distance as an argmin key: NaN counts as the smallest, as numpy's argmin takes the first NaN
+__device__ inline double mon_key(double x) { return isnan(x) ? -1.0 : x; }
+
+// numpy.linspace(start, stop, n)[i]: i step + start, step = (stop - start) / (n - 1), (i / (n - 1)) (stop - start) when
+// the step is 0, i (stop - start) + start for n = 1; the last of n > 1 points is stop
+__device__ inline double mon_grid(long long i, long long n, double start, double stop) {
+    if (n > 1 && i == n - 1) return stop;
+    const double delta = __dsub_rn(stop, start);
+    if (n > 1) {
+        const double div = (double)(n - 1), step = __ddiv_rn(delta, div);
+        return __dadd_rn(step != 0.0 ? __dmul_rn((double)i, step) : __dmul_rn(__ddiv_rn((double)i, div), delta), start);
+    }
+    return __dadd_rn(__dmul_rn((double)i, delta), start);
+}
+
+// one tile of the grid: sample base + t of thread t in sd / ss; thread t owns sample base + t for t < MON_STEP
+template <typename T, typename Pt>
+__device__ inline void mon_tile(long long base, long long n, T* sd, T* ss, Pt& pt) {
+    const long long i = base + threadIdx.x;
+    __syncthreads();                 // the previous tile may still be read
+    if (i < n) pt(i, sd[threadIdx.x], ss[threadIdx.x]);
+    __syncthreads();
+}
+
+// level_cut (monitoring.py:111-146) of the n samples pt(i, d_i, sig_i) for one CTA: s = sig - level, a crossing between
+// i and i + 1 wherever sign(s_i) != sign(s_i+1), at d_i + frac (d_i+1 - d_i) with frac = -s_i / (s_i+1 - s_i) (0 when
+// they are equal); the crossing nearest target, the first on a tie; with none, the d of the first minimum of |s|.
+// Arithmetic in T, one rounding per operation as numpy; n >= 1.  Every thread gets the result.
+template <typename T, typename Pt>
+__device__ T mon_level_cut(long long n, T level, T target, Pt&& pt) {
+    __shared__ T sd[PB_MON_THREADS], ss[PB_MON_THREADS];
+    __shared__ T res;
+    const int t = threadIdx.x;
+    double kc = INFINITY, kz = INFINITY;               // the thread's best keys: crossing, |s|
+    long long ic = LLONG_MAX, iz = LLONG_MAX;
+    T vc = T(0), vz = T(0);
+    for (long long base = 0; base < n; base += MON_STEP) {
+        mon_tile<T>(base, n, sd, ss, pt);
+        const long long i = base + t;
+        if (t >= MON_STEP || i >= n) continue;
+        const T s0 = ss[t] - level, d0 = sd[t];
+        const double z = mon_key((double)(s0 < T(0) ? -s0 : s0));
+        if (iz == LLONG_MAX || z < kz) { kz = z; iz = i; vz = d0; }
+        if (i + 1 >= n) continue;
+        const T s1 = ss[t + 1] - level, d1 = sd[t + 1];
+        if (mon_sign(s0) == mon_sign(s1)) continue;
+        const T frac = s1 == s0 ? T(0) : -s0 / (s1 - s0);
+        T c;
+        if constexpr (sizeof(T) == 8) c = __dadd_rn(d0, __dmul_rn(frac, __dsub_rn(d1, d0)));
+        else c = __fadd_rn(d0, __fmul_rn(frac, __fsub_rn(d1, d0)));
+        const T dist = c - target;
+        const double k = mon_key((double)(dist < T(0) ? -dist : dist));
+        if (ic == LLONG_MAX || k < kc) { kc = k; ic = i; vc = c; }
+    }
+    // the smallest key, then the first index holding it (a thread without a candidate holds no index)
+    double key[2] = {kc, kz};
+    block_reduce<PB_MON_THREADS>(key, OpMin{});
+    double idx[2] = {ic != LLONG_MAX && kc == key[0] ? (double)ic : INFINITY,
+                     iz != LLONG_MAX && kz == key[1] ? (double)iz : INFINITY};
+    block_reduce<PB_MON_THREADS>(idx, OpMin{});
+    const bool crossed = idx[0] != INFINITY;
+    if (crossed ? (double)ic == idx[0] : (double)iz == idx[1]) res = crossed ? vc : vz;
+    __syncthreads();
+    return res;
+}
+
+// turning_points (monitoring.py:88-108) of the n samples pt(i, d_i, sig_i) for one CTA: slope_i = sign(sig_i+1 - sig_i),
+// a turning point at i + 1 wherever slope_i != slope_i+1, in T.  With out, every one is written to out in order and
+// the count returned; otherwise the scan stops at the m-th (0-based), whose d goes to *found (every thread), and the
+// count returned is m + 1, or the whole count (< m + 1) when there are fewer.
+template <typename T, typename Pt>
+__device__ long long mon_turning(long long n, long long m, T* out, T* found, Pt&& pt) {
+    __shared__ T sd[PB_MON_THREADS], ss[PB_MON_THREADS];
+    __shared__ int wc[PB_MON_THREADS / 32];
+    __shared__ T res;
+    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+    long long count = 0;
+    for (long long base = 0; base < n; base += MON_STEP) {
+        mon_tile<T>(base, n, sd, ss, pt);
+        const long long i = base + t;
+        bool flag = false;
+        if (t < MON_STEP && i + 2 < n)
+            flag = mon_sign(ss[t + 1] - ss[t]) != mon_sign(ss[t + 2] - ss[t + 1]);
+        const unsigned b = __ballot_sync(0xffffffffu, flag);
+        if (lane == 0) wc[w] = __popc(b);
+        __syncthreads();
+        long long pos = count + __popc(b & ((1u << lane) - 1u));
+        for (int j = 0; j < PB_MON_THREADS / 32; ++j) {
+            if (j < w) pos += wc[j];
+            count += wc[j];
+        }
+        if (flag) {
+            if (out) out[pos] = sd[t + 1];
+            else if (pos == m) res = sd[t + 1];
+        }
+        if (!out && count > m) {
+            __syncthreads();
+            *found = res;
+            return m + 1;
+        }
+    }
+    return count;
+}
+
+// the monitor signal of (B, C) = v (_signal_curve, monitoring.py:15-45): R = |r|^2, or T = Re eta_sub / Re eta0 |t|^2
+__device__ inline double mon_signal(const TfSample& s, int pol, int mode, double2 eta_sub, double2 v0, double2 v1) {
+    const CmFwd f = cm_rt(s, pol, v0, v1);
+    return mode == PB_MON_R ? tf_abs2(f.r) : eta_sub.x / f.eta0.x * f.t2;
+}
+
+struct MonArgs {
+    const double* err;             // (runs, N) signal (level) or thickness (turning) errors, or NULL
+    const double* levels;          // (ncand, N) cutoff levels (level)
+    long long per_cand, npts;
+    double start, max_factor;
+    int strategy, mode, turning_index;
+};
+
+// simulate_run (monitoring.py:168-233) of run blockIdx.x, at candidate blockIdx.x / per_cand: asbuilt (runs, N)
+template <typename R>
+__global__ void __launch_bounds__(PB_MON_THREADS) monitor_runs_kernel(const TfOps op, const MonArgs a,
+                                                                      R* __restrict__ asbuilt) {
+    const long long run = blockIdx.x;
+    const long long c = run / a.per_cand;
+    const int N = op.nlayers, pol = op.pol;
+    const TfSample s = tf_sample(op, c);
+    const double2 eta_sub = tf_eta_sub(s, pol);
+    double2 v0 = make_double2(1.0, 0.0), v1 = eta_sub;
+    for (int k = N - 1; k >= 0; --k) {
+        const TfLayer L = tf_layer(op, s, k, pol);
+        const double stop = __dmul_rn(a.max_factor, L.d);
+        auto pt = [&](long long j, double& d, double& sig) {
+            d = mon_grid(j, a.npts, a.start, stop);
+            double2 sb, cb, w0 = v0, w1 = v1;
+            tf_sincos(tf_beta(L.n, L.cost, d, s.wvl), &sb, &cb);
+            tf_apply(sb, cb, L.eta, w0, w1);
+            sig = mon_signal(s, pol, a.mode, eta_sub, w0, w1);
+        };
+        const double* e = a.err ? a.err + run * N + k : nullptr;
+        double dr;
+        if (a.strategy == PB_MON_TURNING) {
+            double tp = 0.0;
+            const long long m = a.turning_index - 1;
+            dr = mon_turning<double>(a.npts, m, nullptr, &tp, pt) > m ? tp : L.d;
+            if (e) dr = __dadd_rn(dr, *e);
+        } else {
+            double lv = a.levels[c * N + k];
+            if (e) lv = __dadd_rn(lv, *e);
+            dr = mon_level_cut<double>(a.npts, lv, L.d, pt);
+        }
+        dr = 0.0 > dr ? 0.0 : dr;                    // Python's max(d_real, 0.0)
+        if (threadIdx.x == 0) asbuilt[run * N + k] = (R)dr;
+        double2 sb, cb;
+        tf_sincos(tf_beta(L.n, L.cost, dr, s.wvl), &sb, &cb);
+        tf_apply(sb, cb, L.eta, v0, v1);
+    }
+}
+
+// level_cut or turning_points of a given trace (d, sig of n samples) in one CTA: out[0] the cut, or out[0, count) the
+// turning points and *count their number
+template <typename T>
+__global__ void __launch_bounds__(PB_MON_THREADS) monitor_cut_kernel(int strategy, const T* __restrict__ d,
+                                                                     const T* __restrict__ sig, long long n, T level,
+                                                                     T target, T* __restrict__ out,
+                                                                     long long* __restrict__ count) {
+    auto pt = [&](long long i, T& di, T& si) { di = d[i]; si = sig[i]; };
+    if (strategy == PB_MON_TURNING) {
+        const long long c = mon_turning<T>(n, 0, out, nullptr, pt);
+        if (threadIdx.x == 0) *count = c;
+    } else {
+        const T v = mon_level_cut<T>(n, level, target, pt);
+        if (threadIdx.x == 0) out[0] = v;
+    }
+}
+
+// monitoring_error_sensitivity's J[c, w, k] = (Rr[c (N + 1) + 1 + k, w] - Rr[c (N + 1), w]) / eps of the realized
+// reflectance Rr (runs, W), and choose_monitor_wavelength's score[c] = sqrt(sum J[c]^2) by the grid fold (DESIGN.md
+// §4.4); grid row c
+template <typename R>
+__global__ void __launch_bounds__(256) monitor_jacobian_kernel(const double* __restrict__ Rr, int N, long long W,
+                                                               double eps, R* __restrict__ J, R* __restrict__ score,
+                                                               double* __restrict__ part, unsigned* __restrict__ counters) {
+    const long long c = blockIdx.y, cnt = W * N;
+    const double* R0 = Rr + c * (N + 1) * W;
+    double acc = 0.0;
+    PB_GRID_STRIDE(i, cnt) {
+        const long long w = i / N, k = i % N;
+        const double j = (R0[(k + 1) * W + w] - R0[w]) / eps;
+        if (J) J[c * cnt + i] = (R)j;
+        acc += j * j;
+    }
+    acc = block_reduce<256>(acc, OpAdd{});
+    if (threadIdx.x == 0) part[blockIdx.y * gridDim.x + blockIdx.x] = acc;
+    if (!arrive_last(counters)) return;
+    const double ss = fold_partials<256, 1>(part, 0, OpAdd{}, 0.0);
+    if (threadIdx.x == 0 && score) score[c] = (R)sqrt(ss);
+}
+
 // the n values of an outermost-first array of the C ABI right-aligned to PB_TF_DIMS dims, `fill` in front: the
 // calculation shape (fill 1) or an operand's strides (fill 0)
 static void tf_align(const long long* src, int n, long long fill, long long* dst) {
@@ -963,4 +1178,83 @@ extern "C" int pb_needle(pb_handle_t hh, int dtype, int quantity, int pol, int n
     else launch(needle_kernel<1>);
     PB_LAUNCH_CHECK(h);
     return tf_reduce(h, st, dtype, partial, W, count, nz, accumulate, P, nullptr);
+}
+
+extern "C" int pb_monitor_runs(pb_handle_t hh, int dtype, int strategy, int mode, int pol, int nlayers, long long ncand,
+                               const void* const* in, long long runs, long long per_cand, const void* err,
+                               const void* levels, long long n_points, double start, double max_factor,
+                               int turning_index, void* asbuilt, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (strategy != PB_MON_LEVEL && strategy != PB_MON_TURNING) return fail(h, PB_ERR_INVALID, "monitor: bad strategy");
+    if (mode != PB_MON_R && mode != PB_MON_T) return fail(h, PB_ERR_INVALID, "monitor: mode must be PB_MON_R or T");
+    if (pol != PB_TF_POL_S && pol != PB_TF_POL_P) return fail(h, PB_ERR_INVALID, "monitor: pol must be PB_TF_POL_S or P");
+    if (nlayers < 0 || ncand < 1 || runs < 0 || per_cand < 1 || runs > ncand * per_cand || runs > INT_MAX || n_points < 0)
+        return fail(h, PB_ERR_INVALID, "monitor: bad layer, candidate, run or grid counts");
+    if (runs && nlayers && (!in || !asbuilt || (strategy == PB_MON_LEVEL && (!levels || n_points < 1)) ||
+                            (strategy == PB_MON_TURNING && turning_index < 1)))
+        return fail(h, PB_ERR_INVALID, "monitor: missing operands, levels or output, an empty level grid, or a "
+                                       "turning index below 1");
+    if (!runs || !nlayers) return PB_OK;
+    for (int q = 0; q < PB_TF_NOPS; ++q)
+        if (!in[q]) return fail(h, PB_ERR_INVALID, "monitor: missing operand");
+    // candidate c is sample c of a one-axis calculation shape; the nominal thicknesses are shared
+    TfOps op{};
+    for (int j = 0; j < PB_TF_DIMS; ++j) op.shape[j] = j == PB_TF_DIMS - 1 ? ncand : 1;
+    for (int q = 0; q < PB_TF_NOPS; ++q) {
+        op.p[q] = in[q];
+        op.st[q][PB_TF_DIMS - 1] = q == PB_TF_IN_D ? 0 : 1;
+    }
+    op.st[PB_TF_IN_N][PB_TF_DIMS] = ncand;
+    op.st[PB_TF_IN_D][PB_TF_DIMS] = 1;
+    op.nlayers = nlayers;
+    op.pol = pol;
+    op.theta_scale = 1.0;
+    const MonArgs a{(const double*)err, (const double*)levels, per_cand, n_points, start, max_factor, strategy, mode,
+                    turning_index};
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        monitor_runs_kernel<R><<<(unsigned)runs, PB_MON_THREADS, 0, st>>>(op, a, (R*)asbuilt);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+extern "C" int pb_monitor_cut(pb_handle_t hh, int dtype, int strategy, const void* d, const void* sig, long long n,
+                              double level, double target, void* out, void* count, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (strategy != PB_MON_LEVEL && strategy != PB_MON_TURNING) return fail(h, PB_ERR_INVALID, "monitor: bad strategy");
+    if (n < 0 || (n && (!d || !sig || !out)) || (strategy == PB_MON_TURNING && !count))
+        return fail(h, PB_ERR_INVALID, "monitor: bad trace arguments");
+    if (strategy == PB_MON_LEVEL && n < 1) return fail(h, PB_ERR_INVALID, "monitor: level_cut of an empty trace");
+    with_real(dtype, [&](auto r) {
+        using T = decltype(r);
+        monitor_cut_kernel<T><<<1, PB_MON_THREADS, 0, st>>>(strategy, (const T*)d, (const T*)sig, n, (T)level, (T)target,
+                                                            (T*)out, (long long*)count);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
+}
+
+extern "C" int pb_monitor_jacobian(pb_handle_t hh, int dtype, int ncand, int nlayers, long long nw, const void* Rr,
+                                   double eps, void* J, void* score, void* stream) {
+    PB_ENTER_REAL(hh);
+    if (ncand < 0 || ncand > 65535 || nlayers < 0 || nw < 0 || (ncand && !Rr) || (!J && !score))
+        return fail(h, PB_ERR_INVALID, "monitor: bad jacobian arguments");
+    if (!ncand) return PB_OK;
+    const long long cnt = nw * nlayers;
+    if (!cnt) {
+        if (score) PB_CUDA(h, cudaMemsetAsync(score, 0, (size_t)ncand * rsize(dtype), st));
+        return PB_OK;
+    }
+    const int g = fold_blocks(cnt, h->sm_count);
+    double* part;
+    unsigned* counters;
+    PB_TRY(fold_scratch(h, ncand, g, 1, st, &part, &counters));
+    with_real(dtype, [&](auto r) {
+        using R = decltype(r);
+        monitor_jacobian_kernel<R><<<dim3(g, ncand), 256, 0, st>>>((const double*)Rr, nlayers, nw, eps, (R*)J, (R*)score,
+                                                                   part, counters);
+    });
+    PB_LAUNCH_CHECK(h);
+    return PB_OK;
 }

@@ -61,6 +61,8 @@ _COATINGS_STACK_FUNCS = ('stack_rt', 'RTA', 'internal_fields', 'field_at_depth')
 _COATINGS_DIFF_FUNCS = ('forward_eval', 'ForwardEval', 'thickness_gradient', 'index_gradient')
 _COATINGS_MERIT_NAMES = ('Reflectance', 'Transmittance', 'LayerAbsorptance', 'FieldIntensityAtBoundary',
                          'PeakFieldAtInterfaces', 'FieldInLayer', 'MeritFunction', 'as_merit')
+_COATINGS_MONITOR_FUNCS = ('monitoring_trace', 'cutoff_levels', 'simulate_run', 'monitoring_error_sensitivity',
+                           'choose_monitor_wavelength')
 _TARGETS = {
     'prysm.propagation.fft': {n: getattr(_prop, n) for n in ('focus', 'unfocus', 'focus_adjoint', 'unfocus_adjoint')},
     'prysm.propagation.angular_spectrum': {n: getattr(_prop, n) for n in (
@@ -112,11 +114,14 @@ _TARGETS = {
     # thin films.  The merit terms and the needle function run on the device.  The reference's refine, CoatingProblem
     # and synthesize bind as_merit, the gradients and needle_function at import time and feed the results to host
     # optimizer loops, so in those modules the names are re-bound to variants that hand back numpy (the evaluation is
-    # still on the device); insert_needle, cleanup and the optimizers stay the reference's.  monitoring keeps the
-    # reference's host engine.
+    # still on the device); insert_needle, cleanup and the optimizers stay the reference's.  Optical monitoring runs on
+    # the device: its five run-level functions are re-bound outright, and turning_points / level_cut are dispatched on
+    # their signal (below).
     'prysm.thinfilm': {'multilayer_stack_rt': _tf.multilayer_stack_rt},
     'prysm.x.coatings': {n: getattr(_coat, n) for n in
-                         _COATINGS_STACK_FUNCS + _COATINGS_DIFF_FUNCS + _COATINGS_MERIT_NAMES + ('needle_function',)},
+                         _COATINGS_STACK_FUNCS + _COATINGS_DIFF_FUNCS + _COATINGS_MERIT_NAMES + ('needle_function',)
+                         + _COATINGS_MONITOR_FUNCS},
+    'prysm.x.coatings.monitoring': {n: getattr(_coat, n) for n in _COATINGS_MONITOR_FUNCS},
     'prysm.x.coatings.stack': {n: getattr(_coat, n) for n in _COATINGS_STACK_FUNCS},
     'prysm.x.coatings.diff': {n: getattr(_coat, n) for n in _COATINGS_DIFF_FUNCS},
     'prysm.x.coatings.merit': {n: getattr(_coat, n) for n in _COATINGS_MERIT_NAMES},
@@ -130,6 +135,7 @@ _TARGETS = {
 # (engine function, argument name, position)}
 _STATS = {n: (getattr(_ifg, n), 'array', 0) for n in ('mean', 'pv', 'rms', 'Sa', 'std')}
 _LSTSQ = {'lstsq': (_poly.lstsq, 'data', 1)}
+_MONITOR_CUTS = {n: (getattr(_coat, n), 'signal', 1) for n in ('turning_points', 'level_cut')}
 _DISPATCHED = {
     'prysm.interferogram': {**_STATS, **_LSTSQ, 'fit_plane': (_ifg.fit_plane, 'z', 2),
                             'fit_sphere': (_ifg.fit_sphere, 'z', 0), 'make_window': (_ifg.make_window, 'signal', 0),
@@ -140,6 +146,8 @@ _DISPATCHED = {
     'prysm.util': _STATS,
     'prysm.polynomials': _LSTSQ,
     'prysm.polynomials.fitting': _LSTSQ,
+    'prysm.x.coatings': _MONITOR_CUTS,
+    'prysm.x.coatings.monitoring': _MONITOR_CUTS,
 }
 _IFG_PROPERTIES = ('dropout_percentage', 'pv', 'rms', 'Sa', 'std', 'strehl')
 _IFG_METHODS = ('pvr', 'fill', 'crop', 'recenter', 'remove_piston', 'remove_tiptilt', 'remove_power', 'mask',
